@@ -1,6 +1,6 @@
 """Benchmark of the Wan DiT denoise-step hot path (BASELINE.json metric: denoise-step latency & frames/s).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--shape A|B] [--impl b200|reference] [--no-extras]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--shape A|B] [--impl b200|reference] [--no-extras] [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 One "step" = one pass of the hot path over one batch of synthetic input = one denoise step of the DiT block stack
@@ -11,10 +11,14 @@ value = 81 frames / (4 denoise steps x step latency)  [frames/s], higher is bett
 Multi-GPU (N > 1): the video-token axis is sharded over ranks (128-row aligned); every block does one exchange step for the
 attention (turbodiffusion_b200/dist.py), "strong" scaling.
 
-The JSON line carries two roofline objects (W8A8 GEMM vs the MEASURED INT8 tensor peak of profiles/r02_hw_probes.json, and the
-fused attention kernel), `cpu_baseline` (the reference's CPU-runnable dense SDPA at the full shape, BASELINE.md 3) and
-`extra_configs`: short timed runs of the other BASELINE.json configs (shape B = Wan-14B 720p block stack at this N, the
-literal [1,24,32760,64] SageSLA shape, LTX-2 shape C kernels), so the driver's BENCH/SCALE records carry them too.
+The JSON line carries two roofline objects (W8A8 GEMM vs the H100 SXM data-sheet dense INT8 rate, and the fused attention
+kernel), `cpu_baseline` (the reference's CPU-runnable dense SDPA at the full shape, BASELINE.md 3) and `extra_configs`: short
+timed runs of the other BASELINE.json configs (shape B = Wan-14B 720p block stack at this N, the literal [1,24,32760,64]
+SageSLA shape, LTX-2 shape C kernels).
+
+--dump-outputs DIR writes what the timed step computed in its last step (a fixed, seeded sample of the block stack's output
+rows, float32) as DIR/<name>.npy, so that two builds can be compared output for output on identical inputs.  Under torchrun
+rank 0 writes the rows of its own shard; --profile runs write nothing.
 
 --impl reference times the reference's own CPU path for this metric: torch SDPA dense attention
 (rcm/utils/attention.py:152-166 body) on the bench's q/k/v shape, on all host cores; each step is ONE layer's attention call
@@ -46,24 +50,9 @@ FRAMES, DENOISE_STEPS = 81, 4
 
 
 def peaks():
-    """Roofline denominators: MEASURED_PEAKS.json (driver-written: HBM, bf16) + profiles/r02_hw_probes.json (this repo's
-    measurement of the INT8 tensor peak with the same protocol: torch._int_mm 8192^3 burst / 4 s sustained)."""
-    p = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "_source": "fallback"}
-    try:
-        p.update(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))))
-        p["_source"] = "measured"
-    except Exception:
-        pass
-    try:
-        hp = json.load(open(os.path.join(ROOT, "profiles", "r02_hw_probes.json")))
-        p["int8_tops_burst"] = max(hp.get("int8_tops_burst_cublaslt", 0.0), hp.get("int8_tops_burst_tdb200_rowwise", 0.0))
-        p["int8_tops_sustained"] = max(hp.get("int8_tops_sustained_cublaslt", 0.0), hp.get("int8_tops_sustained_tdb200_rowwise", 0.0))
-        p["_int8_source"] = "profiles/r02_hw_probes.json (torch._int_mm / tdb200 rowwise 8192^3; best of the two)"
-    except Exception:
-        p["int8_tops_burst"] = 2.0 * p["bf16_tflops"]
-        p["int8_tops_sustained"] = 2.0 * p["bf16_tflops_sustained"]
-        p["_int8_source"] = "2 x bf16 (no INT8 measurement file found)"
-    return p
+    """Roofline denominators: NVIDIA's H100 SXM data sheet, dense rates (a card allowed up to 700 W; a card set to a lower
+    power limit runs below them).  Data-sheet figures, not measurements."""
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "int8_tops": 1979.0, "_source": "NVIDIA H100 SXM data sheet (dense)"}
 
 
 class ClockSampler:
@@ -199,29 +188,7 @@ def run_reference(args, shape, rank, world):
     print(json.dumps(line), flush=True)
 
 
-# ------------------------------------------------------------------------------------------------ B200 arm
-def ncu_traffic(shape_key, world):
-    """dram bytes of ONE ffn-down GEMM launch from the committed `ncu --set full` summary of this round (single GPU only:
-    the sharded GEMM at N > 1 has a different M and was not captured)."""
-    if world != 1 or shape_key != "A":
-        return {"traffic": None}
-    for fn in ("r02_ncu_gemm.txt", "r01_ncu_gemm_final.txt"):
-        path = os.path.join(ROOT, "profiles", fn)
-        try:
-            tot = 0.0
-            for ln in open(path):
-                for key in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                    if ln.strip().startswith(key + " ="):
-                        val, unit = ln.split("=")[1].split()[:2]
-                        tot += float(val) * {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}[unit]
-            if tot:
-                return {"traffic": tot, "traffic_algorithmic": 407.9e6,
-                        "traffic_source": f"profiles/{fn} (ffn-down GEMM 32760x1536x8960, one launch)"}
-        except OSError:
-            continue
-    return {"traffic": None}
-
-
+# ------------------------------------------------------------------------------------------------ GPU arm
 def run_b200(shape_key, shape, args, dev, rank, world, local_rank, steps, warmup, want_e2e, sp_mode_req):
     """Build the block stack of `shape`, time `steps` denoise steps (eager pass with per-kernel events, then CUDA-graph
     replay), optionally the end-to-end variant with host buffers.  Returns a dict of measurements."""
@@ -319,8 +286,11 @@ def run_b200(shape_key, shape, args, dev, rank, world, local_rank, steps, warmup
             barrier()
             clk.mark_end()
         ms_step = max_over_ranks(s.elapsed_time(e) / steps)
+        y = ys
     else:
         ms_step = ms_eager
+    if args.dump_outputs and want_e2e and rank == 0:
+        dump_outputs(args.dump_outputs, y)
 
     res = {"ms_step": ms_step, "ms_eager": ms_eager, "launches": launches, "graph_note": graph_note, "clocks": clk.summary(),
            "sp_mode": sp_mode, "n_gemm": n_gemm, "gemm_ms": gemm_ms, "gemm_flops": gemm_flops, "gemm_share": gemm_ms / eager_total,
@@ -360,23 +330,34 @@ def run_b200(shape_key, shape, args, dev, rank, world, local_rank, steps, warmup
     return res
 
 
+def dump_outputs(out_dir, y):
+    """The block stack's output of the last timed step: 2048 rows drawn with a fixed seed (all rows when there are fewer),
+    float32 [rows, dim] (16-bit values are exact in float32)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    rows = y.shape[0]
+    idx = torch.randperm(rows, generator=torch.Generator().manual_seed(0))[:2048].sort().values
+    np.save(os.path.join(out_dir, "block_stack_out_rows.npy"), idx.double().numpy())
+    np.save(os.path.join(out_dir, "block_stack_out.npy"), y[idx.to(y.device)].float().cpu().numpy())
+
+
 def rooflines(res, pk, shape_key, world):
     gemm_ach = res["gemm_flops"] / res["gemm_ms"] / 1e9 if res["gemm_ms"] > 0 else 0.0
     attn_ach = res["attn_flops"] / res["attn_ms"] / 1e9 if res["attn_ms"] > 0 else 0.0
-    i8 = pk["int8_tops_sustained"]
+    i8 = pk["int8_tops"]
     # the fused attention kernel does half of its MACs in INT8 (Q.K^T) and half in bf16 (P.V): at equal MAC counts the
     # time-weighted peak is the harmonic mean of the two rates
-    mixed = 2.0 / (1.0 / i8 + 1.0 / pk["bf16_tflops_sustained"])
-    gemm = {"bound": "tensor", "kernel": "gemm_w8a8_kernel (tcgen05 kind::i8, per-128-K dequant)", "achieved": gemm_ach, "peak": i8,
+    mixed = 2.0 / (1.0 / i8 + 1.0 / pk["bf16_tflops"])
+    gemm = {"bound": "tensor", "kernel": "gemm_w8a8_kernel (wgmma int8, per-128-K dequant)", "achieved": gemm_ach, "peak": i8,
             "unit": "TFLOP/s", "frac": gemm_ach / i8 if i8 else None,
-            "frac_of_bf16_sustained_peak": gemm_ach / pk["bf16_tflops_sustained"],
-            "peak_source": f"INT8 sustained, {pk['_int8_source']}; bf16 from MEASURED_PEAKS.json ({pk['_source']})",
-            "launches": res["n_gemm"], "share_of_step": res["gemm_share"], **ncu_traffic(shape_key, world),
+            "frac_of_bf16_peak": gemm_ach / pk["bf16_tflops"],
+            "peak_source": pk["_source"],
+            "launches": res["n_gemm"], "share_of_step": res["gemm_share"], "traffic": None,
             "timed_in": "eager pass of the same K steps (CUDA events around each GEMM launch on the launch stream)"}
-    attn = {"bound": "tensor", "kernel": "sla_attn kernel (tcgen05 kind::i8 Q.K^T + kind::f16 P.V, fused softmax/linear branch)",
+    attn = {"bound": "tensor", "kernel": "sla_attn kernel (wgmma int8 Q.K^T + 16-bit P.V, fused softmax/linear branch)",
             "achieved": attn_ach, "peak": mixed, "unit": "TFLOP/s", "frac": attn_ach / mixed if mixed else None,
             "flops_split": {"int8_qk": 0.5, "bf16_pv": 0.5},
-            "peak_source": "harmonic mean of the measured INT8 and bf16 sustained peaks (equal MAC counts in each)",
+            "peak_source": f"harmonic mean of the INT8 and bf16 rates of the {pk['_source']} (equal MAC counts in each)",
             "launches": res["n_attn"], "share_of_step": res["attn_share"], "traffic": None,
             "timed_in": "eager pass (CUDA events around each fused-attention launch); FLOPs = H*Mblk*topk*4*128*64*D"}
     return gemm, attn
@@ -430,7 +411,7 @@ def extra_kernels(dev, args):
         ms = timeit(lambda: ltx.gemm_int8_post_scale_bias(a, a_s, b, b_s, bias))
         tf = 2.0 * m * n * kk / ms / 1e9
         out[name] = {"workload": f"per-row post-scale W8A8 GEMM {m}x{n}x{kk} (tilelang_w8a8.py:78-117 semantics)", "ms": ms,
-                     "tflops": tf, "frac_int8_peak": tf / pk["int8_tops_sustained"], "l2": "flushed"}
+                     "tflops": tf, "frac_int8_peak": tf / pk["int8_tops"], "l2": "flushed"}
         del a, b
     return out
 
@@ -465,11 +446,14 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--sp-mode", default="auto", choices=["auto", "allgather", "ulysses"],
                     help="N>1 attention exchange: K/V all-gather + moment all-reduce, or head<->sequence all-to-all "
-                         "(needs heads %% N == 0); auto = the mode that measured faster (dist.py pick_mode)")
+                         "(needs heads %% N == 0); auto = all-gather at N = 2, all-to-all from N = 4 up (dist.py pick_mode)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the extra_configs runs (shape B, 24x64, LTX shape C)")
     ap.add_argument("--profile", action="store_true", help="device-resident region only (for runs under ncu)")
     ap.add_argument("--no-graph", action="store_true", help="time the eager (Python-launched) step instead of the CUDA graph")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's output (a fixed, seeded row sample, float32) as DIR/<name>.npy; "
+                         "under torchrun rank 0 writes its own shard's rows; nothing is written with --profile")
     args = ap.parse_args()
     if args.profile:
         args.no_graph = True

@@ -1,5 +1,5 @@
 /*
- * tdb200.h — C ABI of libtdb200.so: the B200 (sm_100a) implementation of TurboDiffusion's denoise hot path.
+ * tdb200.h — C ABI of libtdb200.so: the H100 (sm_90a) implementation of TurboDiffusion's denoise hot path.
  *
  * This is the drop-in boundary.  Every entry point replaces one interface of the reference
  * (thu-ml/TurboDiffusion; citations are file:line inside that repository):
@@ -39,7 +39,7 @@ extern "C" {
 #define TDB200_ERR_INVALID_ARG (-1)  /* null pointer, bad size, misaligned buffer            */
 #define TDB200_ERR_UNSUPPORTED (-2)  /* shape/dtype outside what the kernels implement        */
 #define TDB200_ERR_CUDA (-3)         /* a CUDA runtime/driver call failed (see last_error)    */
-#define TDB200_ERR_ARCH (-4)         /* current device is not compute capability 10.x         */
+#define TDB200_ERR_ARCH (-4)         /* current device is not compute capability 9.x          */
 #define TDB200_ERR_WORKSPACE (-5)    /* caller-provided workspace too small                   */
 
 #define TDB200_DTYPE_BF16 0
@@ -69,7 +69,7 @@ int tdb200_gelu_quant_int8_block128(const void* x, int x_dtype, int64_t m, int64
  *   a_q [m,k] int8, a_s [ceil(m/128), k/128]; b_q [n,k] int8 ("TN": both K-major), b_s [ceil(n/128), k/128];
  *   bias [n] of dtype c_dtype or NULL; c [m,n] row-major of dtype c_dtype.
  *   Requires k % 128 == 0 and n % 8 == 0 (the reference silently skips such shapes, gemm/launch.hpp:34-35;
- *   here they return TDB200_ERR_UNSUPPORTED).  tcgen05 kind::i8, TMA-staged tiles, accumulators in TMEM.
+ *   here they return TDB200_ERR_UNSUPPORTED).  wgmma int8, TMA-staged tiles, accumulators in registers.
  * ------------------------------------------------------------------------------------------- */
 int tdb200_gemm_w8a8(const int8_t* a_q, const float* a_s, const int8_t* b_q, const float* b_s, const void* bias,
                      void* c, int c_dtype, int64_t m, int64_t n, int64_t k, void* stream);
@@ -168,7 +168,7 @@ int tdb200_rms_norm_rope_table(const void* x, int dtype, const float* w, const f
  *     (they are accumulated, so sequence shards can be summed with one all-reduce).
  * tdb200_sla_attn_fwd   o = T( sparse_softmax_attention(q_i8,k_i8,v; lut) + proj( phi(q) kv / (1e-5 + phi(q).ksum) ) )
  *     kvw [b,h,d(out),d(k)] T = (proj_w . kv) so that proj is folded into the moment matrix; proj_b [d] fp32.
- *     The int8 QK^T, online softmax (exp2), PV, linear branch and merge run in one tcgen05 kernel.
+ *     The int8 QK^T, online softmax (exp2), PV, linear branch and merge run in one wgmma kernel.
  * ------------------------------------------------------------------------------------------- */
 int tdb200_sla_quant_qk(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d,
                         float* kmean, int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale, void* q_pool,
@@ -247,27 +247,11 @@ int tdb200_ltx_split_rope(const void* x, const void* cos_freqs, const void* sin_
  *                       (IEEE division here; the reference's Triton `/` is div.full.f32, so exact .5 ties may differ)
  *   gemm_w8a8_rowwise:  c[i,j] = T( fma( float(sum_k a_q[i,k]*b_q[j,k]) * a_s[i], b_s[j], bias[j] ) ) -- the arithmetic the
  *                       reference's TileLang epilogue executes (I2FP, FMUL, FFMA under nvcc's default -fmad; see
- *                       tools/tilelang_epilogue_probe.py); int32 accumulation over all of K in TMEM, one epilogue per
+ *                       tools/tilelang_epilogue_probe.py); int32 accumulation over all of K in registers, one epilogue per
  *                       tile (no per-K-block dequant).  bias may be NULL (= 0).  k % 128 == 0, n % 8 == 0. */
 int tdb200_quant_int8_rowwise(const void* x, int dtype, int64_t m, int64_t k, int8_t* q, float* s, void* stream);
 int tdb200_gemm_w8a8_rowwise(const int8_t* a_q, const float* a_s, const int8_t* b_q, const float* b_s, const void* bias,
                              void* c, int c_dtype, int64_t m, int64_t n, int64_t k, void* stream);
-
-/* Diagnostics: runs a 128x128x64 bf16 tcgen05 MMA with a K-major A and an MN-major B tile staged by TMA and
- * writes the fp32 product to d_out [128,128].  a [128,64] bf16 row-major, b [64,128] bf16 row-major (d = a.b). */
-int tdb200_selftest_umma_bf16(const void* a, const void* b, float* d_out, void* stream);
-/* Diagnostics: phase trace of the fused attention kernel.  trace (device, 2*64*8 int64) or NULL to disable; see
- * sla_attn.cu (g_attn_trace) for the layout.  Synchronises the device (cudaMemcpyToSymbol). */
-int tdb200_debug_set_attn_trace(long long* trace_or_null);
-/* Diagnostics: TMEM->register read throughput.  One CTA per SM, `warps` (4/8/12/16) warps each issuing `iters`
- * tcgen05.ld.32x32b.x64 (8 KB per warp instruction), optionally followed by the GEMM's int->float + FMA dequant.
- * cycles_per_cta [#SMs] receives clock64() deltas. */
-int tdb200_selftest_tmem_read(int warps, int iters, int convert, long long* cycles_per_cta, float* sink, void* stream);
-/* XU (MUFU) throughput probe: mode 0/1/2 = ex2 f32 / bf16x2 / f16x2, 3/4/5 = tanh f32 / bf16x2 / f16x2; one CTA per SM with
- * `warps` warps, 8 independent chains x `iters` per thread; cycles_per_cta[sm_count]. Diagnostics only. */
-int tdb200_selftest_mufu(int mode, int warps, int iters, long long* cycles_per_cta, float* sink, void* stream);
-/* diagnostics: the exponential pass of the fused attention's softmax warps on register data (variants drop the packing / the row sums) */
-int tdb200_selftest_softmax_exps(int variant, int warps, int iters, long long* cycles_per_cta, float* sink, void* stream);
 
 #ifdef __cplusplus
 }

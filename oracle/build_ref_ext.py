@@ -1,10 +1,10 @@
 """Build the REFERENCE's own CUDA extension `turbo_diffusion_ops` (quant_cuda / gemm_cuda / *_norm_cuda) from the
 sources where they lie under /root/reference, into oracle/_ref/ (git-ignored, travels to the GPU box with gpurun).
 
-TEST INFRASTRUCTURE ONLY: used by tests/test_gpu_vs_reference_ext.py to cross-check the B200 kernels against the
-reference kernels on the same GPU and to time the reference GEMM on B200.  Never imported by turbodiffusion_b200.
+TEST INFRASTRUCTURE ONLY: used by tests/test_gpu_vs_reference_ext.py to cross-check the H100 kernels against the
+reference kernels on the same GPU and to time the reference GEMM on H100.  Never imported by turbodiffusion_b200.
 No reference source is copied into this repository; the compile reads them in place with the reference's own flags
-(setup.py:22-41), arch restricted to sm_100.
+(setup.py:22-41), arch restricted to sm_90.
 """
 import os
 import sys
@@ -31,7 +31,7 @@ def build(verbose=False):
                   "-U__CUDA_NO_BFLOAT16_OPERATORS__", "-U__CUDA_NO_BFLOAT16_CONVERSIONS__",
                   "-U__CUDA_NO_BFLOAT162_OPERATORS__", "-U__CUDA_NO_BFLOAT162_CONVERSIONS__", "--expt-relaxed-constexpr",
                   "--expt-extended-lambda", "--use_fast_math", "-lineinfo", "-DCUTLASS_DEBUG_TRACE_LEVEL=0", "-DNDEBUG",
-                  "-DEXECMODE=0", "-gencode", "arch=compute_100,code=sm_100"]
+                  "-DEXECMODE=0", "-gencode", "arch=compute_90,code=sm_90"]
     load(name="turbo_diffusion_ops",
          sources=[os.path.join(ops, f) for f in ("bindings.cpp", "quant/quant.cu", "norm/rmsnorm.cu", "norm/layernorm.cu", "gemm/gemm.cu")],
          extra_include_paths=[os.path.join(cutlass, "include"), os.path.join(cutlass, "tools", "util", "include"), ops],

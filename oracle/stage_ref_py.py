@@ -1,10 +1,9 @@
 """Stage the reference's own PYTHON sources (network, sampler-side utilities, model surgery, SLA Triton kernels, ops/core.py)
-into oracle/_ref/py/ so they travel to the GPU box with gpurun (oracle/_ref/ is git-ignored: nothing here enters history).
+into oracle/_ref/py/ (git-ignored: nothing here enters history), where tests/test_gpu_reference_model.py finds them.
 
-TEST INFRASTRUCTURE ONLY, like oracle/build_ref_ext.py: used by tests/test_gpu_reference_model.py (the UNMODIFIED reference
-WanModel run on this repo's operators through install()) and tools/ref_vs_ours.py (timing of the reference's Triton
-SparseLinearAttention / FastNorm kernels on the same B200).  Never imported by turbodiffusion_b200; /root/reference does
-not exist on the GPU box.
+TEST INFRASTRUCTURE ONLY, like oracle/build_ref_ext.py: the test runs the UNMODIFIED reference WanModel on this repo's
+operators through install().  Never imported by turbodiffusion_b200.  Needs the reference sources at /root/reference; without
+them nothing is staged and the test skips.
 
     python oracle/stage_ref_py.py        (also called by __graft_entry__.build() when /root/reference is present)
 """

@@ -217,10 +217,10 @@ def test_pick_mode():
     sp = SequenceParallel(32760, world=8, rank=0)
     assert sp.pick_mode(12) == "ulysses" and sp.pick_mode(40) == "ulysses" and sp.pick_mode(40, "allgather") == "allgather"
     assert sp.pick_mode(4) == "allgather"                    # fewer heads than ranks: only the all-gather mode applies
-    assert sp.pick_mode(12, "ulysses") == "ulysses"          # uneven head split (measured faster at N=8)
+    assert sp.pick_mode(12, "ulysses") == "ulysses"          # uneven head split
     with pytest.raises(ValueError):
         sp.pick_mode(4, "ulysses")                             # fewer heads than ranks
     assert SequenceParallel(32760, world=1, rank=0).pick_mode(12) == "allgather"
-    assert SequenceParallel(32760, world=2, rank=0).pick_mode(12) == "allgather"   # measured faster at N=2
-    assert SequenceParallel(32760, world=4, rank=0).pick_mode(12) == "ulysses"     # measured faster from N=4 up
+    assert SequenceParallel(32760, world=2, rank=0).pick_mode(12) == "allgather"   # N = 2: all-gather
+    assert SequenceParallel(32760, world=4, rank=0).pick_mode(12) == "ulysses"     # from N = 4 up: all-to-all
     assert SequenceParallel(32760, world=2, rank=0).pick_mode(12, "ulysses") == "ulysses"

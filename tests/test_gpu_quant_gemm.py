@@ -1,4 +1,4 @@
-"""GPU parity: a1 int8 block quant and a2 W8A8 tcgen05 GEMM against the CPU oracle (bit-exact)."""
+"""GPU parity: a1 int8 block quant and a2 W8A8 wgmma GEMM against the CPU oracle (bit-exact)."""
 import pytest
 import torch
 
@@ -54,7 +54,7 @@ GEMM_SHAPES = [
     (300, 384, 640),     # ragged M, N not a multiple of the 256 tile
     (129, 136, 128),     # N % 128 != 0 (n % 8 == 0)
     (1, 128, 128),
-    (2048, 1536, 1536),  # more tiles than SMs would need at 148 CTAs: exercises the persistent loop
+    (2048, 1536, 1536),  # more tiles (192) than the H100's 132 SMs: more than one wave of CTAs
 ]
 
 

@@ -24,7 +24,8 @@ REF_PY = os.path.join(ROOT, "oracle", "_ref", "py")
 
 def _import_reference():
     if not os.path.isdir(os.path.join(REF_PY, "rcm")):
-        pytest.skip("oracle/_ref/py not staged (run oracle/stage_ref_py.py where /root/reference exists)")
+        pytest.skip("oracle/_ref/py not staged: the test runs the upstream TurboDiffusion WanModel sources, which are not part of "
+                    "this repository (oracle/stage_ref_py.py stages them where /root/reference exists)")
     import turbodiffusion_b200
     turbodiffusion_b200.install()
     for p in (REF_PY, os.path.join(REF_PY, "inference")):

@@ -132,7 +132,7 @@ def test_attention_poly_exp2_experiment_coefficients():
     import numpy as np
     src = open(os.path.join(ROOT, "turbodiffusion_b200", "csrc", "sla_attn.cu")).read()
     if "poly_exp2_x2(float2 x)" not in src:
-        pytest.skip("the polynomial exp2 is not part of the current attention kernel (measured slower in round 2)")
+        pytest.skip("the polynomial exp2 is not part of the current attention kernel")
     body = src[src.index("poly_exp2_x2(float2 x)"):src.index("#endif", src.index("poly_exp2_x2(float2 x)"))]
     hexes = re.findall(r"(0x1\.[0-9a-f]+p-?\d+)f", body)
     c3, c2, c1, c0 = [np.float32(float.fromhex(h)) for h in (hexes[0], hexes[2], hexes[4], hexes[6])]

@@ -145,8 +145,8 @@ def test_ltx_row_quant_matches_the_reference_triton_kernel(k):
 
 
 def test_ltx_post_scale_epilogue_is_a_fused_multiply_add():
-    """The reference's TileLang epilogue executes fma(float(acc)*sA, sB, bias) (tools/tilelang_epilogue_probe.py,
-    profiles/r01_tilelang_epilogue_sass.txt).  Known answer where the fused and the unfused evaluation differ:
+    """The reference's TileLang epilogue executes fma(float(acc)*sA, sB, bias): its SASS has one I2FP, FMUL and FFMA per
+    element and no FADD (tools/tilelang_epilogue_probe.py prints that count).  Known answer where the fused and the unfused evaluation differ:
     (1+2^-12)(1+3*2^-12) = 1 + 2^-10 + 3*2^-24 is a rounding tie for a separate multiply (-> 1 + 2^-10 + 2^-22); with
     bias = -(1+2^-10) the unfused result is 4*2^-24, the fused one keeps 3*2^-24."""
     a_q = torch.tensor([[1] + [0] * 127], dtype=torch.int8)

@@ -56,7 +56,8 @@ def _run(mode):
     return json.loads(line[len("RESULT"):])
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="/root/reference is only present in the build container")
+@pytest.mark.skipif(not os.path.isdir(REF), reason="needs the upstream TurboDiffusion sources at /root/reference (not part of this repository): the test builds "
+                           "the upstream module tree itself")
 def test_unmodified_reference_surgery_builds_the_same_interface():
     ours, ref = _run("ours"), _run("ref")
     assert ours["types"]["attn_module"] == "turbodiffusion_b200" and ref["types"]["attn_module"] == "SLA"
@@ -93,7 +94,7 @@ print("RESULT" + json.dumps({
 '''
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/TurboT2AV/LTX-2/packages"), reason="build container only")
+@pytest.mark.skipif(not os.path.isdir("/root/reference/TurboT2AV/LTX-2/packages"), reason="needs the upstream TurboT2AV LTX-2 packages at /root/reference (not part of this repository)")
 def test_ltx_acceleration_backend_resolves_to_this_package():
     """The LTX-2 client (TurboT2AV ltx_distillation/acceleration.py) looks the W8A8 / FastNorm / SLA operators up by name
     at run time; with install() every lookup must land in turbodiffusion_b200 (incl. the gemm_cuda_swizzle* exports the

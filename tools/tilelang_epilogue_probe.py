@@ -2,8 +2,8 @@
 
 Imports the reference's TileLang kernel factory from /root/reference (read-only, build container only), lowers it to CUDA C
 with TileLang's own code generator, compiles that with nvcc the way TileLang's JIT does (default flags: -fmad=true, no
-fast-math; tilelang/jit/adapter/libgen.py) and counts the floating-point SASS instructions of the epilogue.  Result
-(profiles/r01_tilelang_epilogue_sass.txt): per thread 64 I2FP.F32.S32 + 64 FMUL + 64 FFMA and no FADD, i.e.
+fast-math; tilelang/jit/adapter/libgen.py) and counts the floating-point SASS instructions of the epilogue.  Result:
+per thread 64 I2FP.F32.S32 + 64 FMUL + 64 FFMA and no FADD, i.e.
     c = bf16( fma( float(acc) * sA[i], sB[j], bias[j] ) )
 which is what oracle.td_oracle.ltx_gemm_post_scale and tdb200_gemm_w8a8_rowwise compute.
 

@@ -1,4 +1,4 @@
-"""Mirror of turbodiffusion/SLA/core.py: SparseLinearAttention / SageSparseLinearAttention on B200.
+"""Mirror of turbodiffusion/SLA/core.py: SparseLinearAttention / SageSparseLinearAttention on H100.
 
 Same constructor arguments, parameters (`proj_l`, fp32, zero-init) and call convention (q,k,v in [B, L, H, D], result in
 the same layout and dtype; SLA/core.py:181-183,253).  The forward is five kernel launches:
@@ -9,7 +9,6 @@ Inputs are consumed in place in their [B, L, H, D] layout; no transposed copies 
 """
 from __future__ import annotations
 
-import os
 
 import torch
 import torch.nn as nn
@@ -47,20 +46,17 @@ def project_moments(proj_w: torch.Tensor, kv: torch.Tensor, dtype) -> torch.Tens
     return out
 
 
-ATTN_IMPL = os.environ.get("TDB200_ATTN_IMPL", "v1")  # "v1": one CTA per query block; "v2": persistent kernel (measured slower, see DESIGN)
-
-
 ATTN_TIMER = None  # bench.py installs a callable(h, mblk, topk, d) -> context manager to time the fused-attention launches
 
 
-def attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, impl=None, feature=0):
+def attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, feature=0):
     if ATTN_TIMER is not None:
         with ATTN_TIMER(q.shape[2] * q.shape[0], (q.shape[1] + 127) // 128, topk, q.shape[3]):
-            return _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk, impl, feature)
-    return _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk, impl, feature)
+            return _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk, feature)
+    return _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk, feature)
 
 
-def _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, impl=None, feature=0):
+def _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, feature=0):
     b, l, h, d = q.shape
     lk = v.shape[1] if lk is None else lk
     out = torch.empty_like(q)
@@ -70,11 +66,7 @@ def _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, impl=
         check(lib().tdb200_sla_attn_fwd_kseq(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v),
                                              ptr(q), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b),
                                              ptr(out), b, l, lk, h, d, float(sm_scale), stream_ptr(q.device)), "sla_attn_fwd")
-    elif (impl or ATTN_IMPL) == "v1" and d == 128 and feature == 0:
-        check(lib().tdb200_sla_attn_fwd(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v),
-                                        ptr(q), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b),
-                                        ptr(out), b, l, lk, h, d, float(sm_scale), stream_ptr(q.device)), "sla_attn_fwd")
-    else:
+    else:   # head-major INT8 K: head dims 64 and 128, every feature map
         check(lib().tdb200_sla_attn_fwd_v2(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v),
                                            ptr(q), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b),
                                            ptr(out), b, l, lk, h, d, float(sm_scale), feature, stream_ptr(q.device)),
@@ -137,13 +129,10 @@ class _SLABase(nn.Module):
         kv, ksum = linear_moments(k, v, self.feature)
         # proj_l folded into the moments: (phi(q) KV / den) W^T + b == phi(q) (W KV^T)^T / den + b ; kv is [dv, dk]
         kvw = project_moments(self.proj_l.weight, kv, self.dtype)  # [B,H,d_out,d_k]
-        # 128-wide heads with the softmax map run the one-CTA-per-query-block kernel (faster); 64-wide heads and the
-        # elu / relu maps run the persistent kernel, which has native 64-wide tiles and the feature-map switch
-        impl = ATTN_IMPL if (d == 128 and self.feature == 0) else "v2"
         if not self.quantised_qk and d == 128 and self.feature == 0:
             o = attn_fwd_qk16(q, k, v, lut, real_topk, kvw, ksum, self.proj_l.bias.float().contiguous(), d ** -0.5)
         else:
-            o = attn_fwd(prep, v, q, lut, real_topk, kvw, ksum, self.proj_l.bias.float().contiguous(), d ** -0.5, impl=impl,
+            o = attn_fwd(prep, v, q, lut, real_topk, kvw, ksum, self.proj_l.bias.float().contiguous(), d ** -0.5,
                          feature=self.feature)
         o = o if o.dtype == dtype else o.to(dtype)
         return (o, real_topk / nblk) if return_sparsity else o
@@ -172,7 +161,7 @@ class SparseLinearAttention(_SLABase):
         self.BLKQ, self.BLKK = BLKQ, BLKK
         if (BLKQ, BLKK) != (128, 64):
             import warnings
-            warnings.warn(f"SparseLinearAttention(BLKQ={BLKQ}, BLKK={BLKK}): the B200 kernels use 128-row query blocks and "
+            warnings.warn(f"SparseLinearAttention(BLKQ={BLKQ}, BLKK={BLKK}): these kernels use 128-row query blocks and "
                           "64-row key blocks (the configuration TurboDiffusion's modify_model.py:50 requests); block "
                           "selection differs from the reference for other sizes", stacklevel=2)
 
@@ -195,7 +184,7 @@ def get_vanilla_qk_quant(q, k, km=None, BLKQ=128, BLKK=64):
     """q,k [B,H,L,D] -> (q_int8 [B,H,L,D], q_scale [B,H,Mblk], k_int8 of (k - mean_L k), k_scale [B,H,Nblk]); call site
     SLA/core.py:200-203.  `km` is accepted for signature compatibility (the key mean is recomputed by the fused prepass)."""
     if (BLKQ, BLKK) != (128, 64):
-        raise NotImplementedError("the B200 path implements the non-sm90 block sizes (BLKQ=128, BLKK=64)")
+        raise NotImplementedError("this implementation uses the block sizes BLKQ=128, BLKK=64 on every architecture")
     prep = quant_qk(q.transpose(1, 2).contiguous(), k.transpose(1, 2).contiguous())
     return prep.q_i8, prep.q_scale, prep.k_i8, prep.k_scale
 
@@ -246,18 +235,18 @@ def qk_int8_sv_f8_accum_f16_block_sparse_attn_inst_buf_fuse_v_scale_with_pv_thre
     kvw = torch.zeros(b, h, d, d, dtype=v.dtype, device=v.device)
     ksum = torch.ones(b, h, d, dtype=torch.float32, device=v.device)
     pb = torch.zeros(d, dtype=torch.float32, device=v.device)
-    out = attn_fwd(prep, vt, qz, lut, lut.shape[-1], kvw, ksum, pb, sm_scale if sm_scale is not None else d ** -0.5, lk=lk,
-                   impl=None if d == 128 else "v2")
+    out = attn_fwd(prep, vt, qz, lut, lut.shape[-1], kvw, ksum, pb, sm_scale if sm_scale is not None else d ** -0.5, lk=lk)
     o.copy_(out.transpose(1, 2))
     return o
 
 
 class _QattnShim:
-    """SpargeAttn's `qattn` extension module holds the sm80 / sm90 kernels; on B200 the client takes the Sage2++ entry above."""
+    """SpargeAttn's `qattn` extension module holds its sm80 / sm90 kernels; here every architecture is served by the Sage2++
+    entry above (the fused kernel with the block sizes BLKQ=128, BLKK=64)."""
 
     def __getattr__(self, name):
-        raise NotImplementedError(f"SLA.core.qattn.{name}: sm80/sm90 SpargeAttn kernels have no B200 counterpart; "
-                                  "get_cuda_arch() reports sm100, which routes callers to the fused kernel")
+        raise NotImplementedError(f"SLA.core.qattn.{name}: the sm80/sm90 SpargeAttn kernels have no counterpart here; "
+                                  "call the Sage2++ entry, which runs the fused kernel")
 
 
 qattn = _QattnShim()

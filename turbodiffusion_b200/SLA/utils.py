@@ -1,4 +1,4 @@
-"""Mirror of turbodiffusion/SLA/utils.py: mean_pool, get_block_map, get_cuda_arch (B200 implementation)."""
+"""Mirror of turbodiffusion/SLA/utils.py: mean_pool, get_block_map, get_cuda_arch (H100 implementation)."""
 from __future__ import annotations
 
 import torch
@@ -10,10 +10,18 @@ def cdiv(a, b):
     return (a + b - 1) // b
 
 
+# The SpargeAttn kernel family this package serves on every GPU it runs on (see get_cuda_arch).
+SERVED_ARCH = "sm100"
+
+
 def get_cuda_arch(device_index):
-    """SLA/utils.py:70-71."""
-    major, minor = torch.cuda.get_device_capability(device_index)
-    return f"sm{major}{minor}"
+    """SLA/utils.py:70-71.  The reference (SLA/core.py:191-193, 211-235) and the LTX client (acceleration.py:286-378) use this
+    value only to choose a SpargeAttn kernel family and its block sizes: sm80/86/87 -> fp16-V kernels, sm90 -> the
+    BLKQ=64 / BLKK=128 Hopper kernels, anything else -> the Sage2++ entry with BLKQ=128 / BLKK=64.  This package implements
+    the last family (as the fused kernel) on every GPU, H100 included, so it reports that family's tag and callers take the
+    branch whose entry points exist here.  The device's compute capability is torch.cuda.get_device_capability()."""
+    torch.cuda.get_device_capability(device_index)   # an invalid device index raises like the reference's call
+    return SERVED_ARCH
 
 
 class QKPrep:
@@ -140,7 +148,7 @@ def get_block_map(q: torch.Tensor, k: torch.Tensor, topk_ratio: float, BLKQ: int
     """SLA/utils.py:55-67.  q,k [B, H, L, D].  Returns (sparse_map int8, lut int32 [B,H,Mblk,topk] ascending, topk).
     NOTE the reference returns the unsorted torch.topk indices (int64) as `lut`; only the SET is defined
     (sorted=False), and SageSLA rebuilds an ascending LUT from the map anyway (SLA/core.py:204)."""
-    assert (BLKQ, BLKK) == (128, 64), "the B200 path implements the non-sm90 block sizes (SLA/core.py:191-193)"
+    assert (BLKQ, BLKK) == (128, 64), "this implementation uses the block sizes BLKQ=128, BLKK=64 on every architecture (SLA/core.py:191-193)"
     prep = quant_qk(q.transpose(1, 2).contiguous(), k.transpose(1, 2).contiguous())
     nblk = prep.nblk
     topk = min(nblk, int(topk_ratio * nblk))

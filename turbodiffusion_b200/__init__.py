@@ -1,4 +1,4 @@
-"""turbodiffusion_b200 — B200 (sm_100a) implementation of TurboDiffusion's denoise hot path.
+"""turbodiffusion_b200 — H100 (sm_90a) implementation of TurboDiffusion's denoise hot path.
 
 Host code is Python/PyTorch (device memory, streams, torch.distributed); all arithmetic runs in hand-written CUDA
 kernels inside libtdb200.so, reached through the C ABI in include/tdb200.h.  The sub-packages mirror the reference's
@@ -15,7 +15,7 @@ __version__ = "0.1.0"
 def install() -> None:
     """Register this package under the reference's module names so unmodified reference code
     (`from ops import FastLayerNorm, FastRMSNorm, Int8Linear`, `from SLA import ...`, `import turbo_diffusion_ops`;
-    turbodiffusion/inference/modify_model.py:33-37) resolves to the B200 implementation."""
+    turbodiffusion/inference/modify_model.py:33-37) resolves to this implementation."""
     from . import ops, SLA, turbo_diffusion_ops
     for name, mod in (("turbo_diffusion_ops", turbo_diffusion_ops), ("ops", ops), ("SLA", SLA),
                       ("turbodiffusion.ops", ops), ("turbodiffusion.SLA", SLA)):

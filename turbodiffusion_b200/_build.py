@@ -1,9 +1,9 @@
-"""In-tree build of libtdb200.so (sm_100a only).  nvcc cross-compiles without a GPU.
+"""In-tree build of libtdb200.so (sm_90a only).  nvcc cross-compiles without a GPU.
 
     python -m turbodiffusion_b200._build [--force]
 
-Objects go to turbodiffusion_b200/csrc/build/, the library to turbodiffusion_b200/libtdb200.so (git-ignored,
-but shipped to the GPU box by gpurun).  cudart is linked statically so the library has no load-time dependency on
+Objects go to turbodiffusion_b200/csrc/build/, the library to turbodiffusion_b200/libtdb200.so (both git-ignored
+build products).  cudart is linked statically so the library has no load-time dependency on
 a particular libcudart.so; the driver entry point for cuTensorMapEncodeTiled is resolved at run time.
 """
 from __future__ import annotations
@@ -21,13 +21,13 @@ LIB_PATH = os.path.join(PKG_DIR, "libtdb200.so")
 INCLUDE = os.path.join(os.path.dirname(PKG_DIR), "include")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
 
 def _extra_defines():
-    """Experiment switches for kernel variants (e.g. TDB200_NVCC_DEFINES="-DTDB_GEMM_CVT_MIX=1"); unset = the shipped kernels.
+    """Extra nvcc defines for experimental kernel variants (TDB200_NVCC_DEFINES="-DNAME=VALUE ..."); unset = the shipped kernels.
     Changing it needs --force (object staleness only tracks source mtimes)."""
     return os.environ.get("TDB200_NVCC_DEFINES", "").split()
 
@@ -73,7 +73,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
                     raise RuntimeError(f"nvcc failed on {futs[fut]}:\n{r.stdout}\n{r.stderr}")
     objs = [os.path.join(BUILD, s[:-3] + ".o") for s in sources()]
     if force or jobs or _stale(LIB_PATH, objs):
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH] + objs
+        cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_PATH] + objs
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

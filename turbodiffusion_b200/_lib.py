@@ -12,7 +12,7 @@ import torch
 
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(PKG_DIR, "libtdb200.so")
-if os.environ.get("TDB200_LIB"):   # kernel-variant experiments: a differently compiled build of the same ABI (see profiles/r02_gemm_experiments.md, call 21)
+if os.environ.get("TDB200_LIB"):   # kernel-variant experiments: a differently compiled build of the same ABI
     LIB_PATH = os.environ["TDB200_LIB"]
 
 DTYPE_TAG = {torch.bfloat16: 0, torch.float16: 1}
@@ -62,11 +62,6 @@ _PROTOS = {
     "tdb200_ltx_split_rope": [_P, _P, _P, _I, _P, _I64, _I64, _I64, _I64, _P],
     "tdb200_quant_int8_rowwise": [_P, _I, _I64, _I64, _P, _P, _P],
     "tdb200_gemm_w8a8_rowwise": [_P, _P, _P, _P, _P, _P, _I, _I64, _I64, _I64, _P],
-    "tdb200_debug_set_attn_trace": [_P],
-    "tdb200_selftest_umma_bf16": [_P, _P, _P, _P],
-    "tdb200_selftest_tmem_read": [_I, _I, _I, _P, _P, _P],
-    "tdb200_selftest_mufu": [_I, _I, _I, _P, _P, _P],
-    "tdb200_selftest_softmax_exps": [_I, _I, _I, _P, _P, _P],
 }
 _RESTYPES = {"tdb200_last_error": c_char_p}
 

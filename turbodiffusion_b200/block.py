@@ -1,4 +1,4 @@
-"""The Wan DiT block hot path composed from the B200 operators: a fused restatement of
+"""The Wan DiT block hot path composed from the H100 operators: a fused restatement of
 `WanAttentionBlock.forward` (turbodiffusion/rcm/networks/wan2pt1.py:390-417) as TurboDiffusion runs it after model
 surgery (inference/modify_model.py:40-81): Int8Linear everywhere in the block, FastLayerNorm / FastRMSNorm,
 SageSLA self-attention, dense SDPA cross-attention over the text tokens.
@@ -25,19 +25,18 @@ from .turbo_diffusion_ops import (gelu_quant_cuda, gemm_cuda_bias_gelu, gemm_cud
 
 # FFN activation between the two W8A8 GEMMs:
 #   "fused": bias + GELU (one-MUFU tanh) + quantisation in the up-projection's epilogue: no 16-bit intermediate in HBM; the
-#            epilogue runs on the warps that dequantise (shape A: 0.886 ms vs 0.552 ms for the plain GEMM);
+#            epilogue runs on the warps that dequantise;
 #   "split": up-projection writes T(acc + bias); one HBM pass applies GELU(tanh) and the 128x128-block quantisation
-#            (tdb200_gelu_quant_int8_block128, 0.200 ms at shape A), no activation on the GEMM's dequant warps.
-# Measured in the step (profiles/r02_bench_ffn_modes.txt), both with packed arithmetic: fused 99.7 ms (up-projection 0.660 ms at shape A),
-# split 102.0 ms (0.492 ms + 0.200 ms) per denoise step -> fused is the default.
+#            (tdb200_gelu_quant_int8_block128), no activation on the GEMM's dequant warps.
+# fused is the default: it saves the 16-bit intermediate's round trip through HBM.
 FFN_ACT_MODE = os.environ.get("TDB200_FFN_ACT", "fused")
 
 # Self-attention q/k/v as ONE GEMM against the row-concatenated weights (the packing of the LTX client's fused to_qkv,
 # acceleration.py:836-860), outputs written as three contiguous matrices: bit-identical to the three GEMMs (scales are per
-# 128 weight rows), 31.1 -> 32 tile waves instead of 3 x (10.4 -> 11) at shape A and two launches fewer.
+# 128 weight rows), fewer partial tile waves and two launches fewer.
 #   "1": always, "0": never, "auto": single GPU yes; under a sequence-parallel hook no (the separate K projection lets the
 #   K exchange start under the V and Q projections).  Unless "0" the cross-attention k/v of the text tokens are one GEMM too
-#   (M = 512 rows: 24 tiles per projection on 148 SMs, so the fused launch costs what one of the two did).
+#   (M = 512 rows: 12 tiles per projection on 132 SMs, so the fused launch costs what one of the two did).
 FUSE_QKV = os.environ.get("TDB200_FUSE_QKV", "auto")
 
 LINEARS = ("self_attn.q", "self_attn.k", "self_attn.v", "self_attn.o", "cross_attn.q", "cross_attn.k", "cross_attn.v",
@@ -70,7 +69,7 @@ def random_block_state(dim: int, ffn_dim: int, heads: int, seed: int, device, dt
 
 
 class WanBlockB200:
-    """One DiT block on the B200 operators.  `sd` uses the reference state-dict keys relative to `blocks.<i>.`."""
+    """One DiT block on the H100 operators.  `sd` uses the reference state-dict keys relative to `blocks.<i>.`."""
 
     def __init__(self, sd: Dict[str, torch.Tensor], dim: int, heads: int, eps: float = 1e-6, topk: float = 0.1,
                  attention: str = "sagesla"):

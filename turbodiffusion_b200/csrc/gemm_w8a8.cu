@@ -1,58 +1,33 @@
-// a2. W8A8 GEMM with per-128-K-block rescale on tcgen05 (reference semantics: turbodiffusion/ops/gemm/kernel.hpp:391-427,
+// a2. W8A8 GEMM with per-128-K-block rescale on wgmma (reference semantics: turbodiffusion/ops/gemm/kernel.hpp:391-427,
 // utils.hpp:116-121, output cast kernel.hpp:471-477; bias add ops/core.py:410-411).
 //
 //   c[i,j] = T( fma-chain over kb of  float(int32 dot of K-block kb) * (a_s[i/128,kb]*b_s[j/128,kb]) )  [+ bias]
 //
-// Design (one persistent CTA per SM, 128x256 output tile, 128-deep K-blocks):
-//   warp 8   TMA producer: A tile [128 rows x 128 B] and B tile [256 rows x 128 B] per K-block, 128B-swizzled,
-//            3-stage ring, mbarrier complete_tx.
-//   warp 9   MMA issuer (one elected lane): 4 x tcgen05.mma.kind::i8 (M128 N256 K32) per K-block into one of two
-//            TMEM accumulator buffers (2 x 256 columns of int32), accumulate flag reset at every K-block because the
-//            reference rescales per K-block; tcgen05.commit releases the smem stage and publishes the TMEM buffer.
-//   warps 0-7 dequant/epilogue: thread = one output row (TMEM lane) x 128 columns.  Per K-block: four tcgen05.ld.x32
-//            chunks, software-pipelined (chunk c+1 is in flight while chunk c is converted, and chunk 0 of K-block
-//            kb+1 is requested before the last chunk of kb is converted), I2FP (exact, |sum| <= 2^21) + packed FFMA2
-//            with the block scale into 128 fp32 registers; the TMEM buffer is handed back as soon as its last chunk
-//            has landed in registers.  After the last K-block: round to T, (+bias), (GELU), write the warp's 32 x 128
-//            slice into its own swizzled staging buffer and hand it to the TMA store engine
-//            (cp.async.bulk.tensor store, clipped at the M/N edges by the tensor map); the warp moves on to the next
-//            tile while the store drains.
-// Measured (profiles/r01_gemm_experiments.md, profiles/r02_gemm_experiments.md): the chunk pipelining is +20..27 % over
-// load-wait-convert; 16 dequant warps x 64 columns is ~8 % slower; TMA multicast of the B tile inside 2-CTA clusters
-// (kept: -33 % L2->SM traffic) is throughput-neutral; converting a share of the partial sums on the XU pipe (I2F.RM)
-// is slower.  I2FP issues on the half-rate ALU pipe: 512 clk per 128x256 K-block, the same as its int8 MMA.
+// Design (one CTA per 128x128 output tile, 128-deep K-blocks; a tile is exactly one block of both scale grids):
+//   warp 8   TMA producer: A tile [128 rows x 128 B] and B tile [128 rows x 128 B] per K-block, 128B-swizzled,
+//            4-stage ring, mbarrier complete_tx.
+//   warpgroups 0-1  MMA + dequant + epilogue; warpgroup g owns output rows [64g, 64g+64) of the tile.  Per K-block four
+//            wgmma.m64n128k32.s32.s8.s8 into a 64-register int32 accumulator, then the int -> float conversion and the
+//            FFMA with the block scale into 64 fp32 registers; the two warpgroups' dequant and MMA phases interleave on
+//            the SM.  The accumulate flag is reset at every K-block because the reference rescales per K-block.  After the
+//            last K-block: round to T, (+bias), (GELU), store.
 // Integer accumulation is exact and the fp32 FMA chain runs in ascending kb order, so the result is bit-identical
 // to the reference restatement (oracle.int8_linear) on the same int8 inputs.
 #include "common.cuh"
 #include "host_common.h"
 
-// Measurement switches of round 2 (tools/gpu_gemm_variants.sh); the defaults are the measured winners.
-#ifndef TDB_GEMM_STAGES
-#define TDB_GEMM_STAGES 3    // TMA ring depth: 3 (8 KB staging per warp, one store round) or 4 (4 KB staging, two rounds)
-#endif
-#ifndef TDB_GEMM_XPF
-#define TDB_GEMM_XPF 0       // request chunk 0 of K-block kb+1 before converting the last chunk of kb: 0 never (fastest), 1 always (may block), 2 when its MMAs are done
-#endif
-
 namespace {
 
 using namespace tdb;
 
-constexpr int BM = 128, BN = 256, BK = 128;
-constexpr int kStages = TDB_GEMM_STAGES;
-constexpr int kStoreRounds = TDB_GEMM_STAGES >= 4 ? 2 : 1;
-constexpr int kEpiWarps = 8;
-constexpr int kTmaWarp = 8, kMmaWarp = 9;
-constexpr int kThreads = 384;  // warps 0-7 dequant/epilogue, 8 TMA, 9 MMA, 10-11 idle (complete the warpgroup)
-constexpr uint32_t kATile = BM * BK;            // 16 KB
-constexpr uint32_t kBTile = BN * BK;            // 32 KB
+constexpr int BM = 128, BN = 128, BK = 128;
+constexpr int kStages = 4;
+constexpr int kConsumerWarps = 8;                    // warpgroups 0-1
+constexpr int kThreads = kConsumerWarps * 32 + 32;   // + the TMA warp
+constexpr uint32_t kATile = BM * BK;                 // 16 KB
+constexpr uint32_t kBTile = BN * BK;                 // 16 KB
 constexpr uint32_t kStageBytes = kATile + kBTile;
-constexpr uint32_t kTmemCols = 512;             // 2 accumulator buffers x 256 int32 columns
-constexpr uint32_t kCStageBytes = (2 / kStoreRounds) * 32 * 128;  // per-warp output staging: 32 rows x 128 (or 64) columns of T in swizzled 4 KB boxes
-constexpr uint32_t kBiasSlot = 256;              // per-warp copy of the tile's 128 bias values (T)
-constexpr uint32_t kAlignSlack = kStages >= 4 ? 768 : 1024;  // 4 stages leave 768 B: the dynamic window starts 1024-aligned in practice (checked)
-constexpr size_t kSmemBytes = kAlignSlack + size_t(kStages) * kStageBytes + kEpiWarps * (kCStageBytes + kBiasSlot) +
-                              256 /*barriers*/;
+constexpr size_t kSmemBytes = 1024 + size_t(kStages) * kStageBytes + 256 /*barriers + amax exchange*/;
 
 struct GemmParams {
   const float* a_s;
@@ -60,473 +35,229 @@ struct GemmParams {
   const void* bias;
   void* c;
   int64_t m, n, k;
-  int k_blocks, n_tiles, m_tiles, total_tiles;  // total_tiles: tiles, or tile PAIRS in the cluster variant
-  int act;  // 0 none, 1 GELU(tanh) applied to the T-rounded (acc [+ bias]) value, result rounded to T again
+  int k_blocks;
+  int act;        // 0 none, 1 GELU(tanh) applied to the T-rounded (acc [+ bias]) value, result rounded to T again
   int8_t* out_q;  // when non-NULL: emit quant_int8_block128(T output) instead of the T output itself
   float* out_s;   // [ceil(m/128), n/128]
   int n_part;     // 16-bit output: columns per output matrix; c is [n / n_part, m, n_part] (n_part == n: the plain [m, n])
 };
 
-// 16-bit output box -> c [n / n_part, m, n_part]: the map is (column in part, row, part), so rows past m are clipped per part
-__device__ __forceinline__ void store_c(const void* tmap, const void* stage, int32_t col, int32_t row, int32_t n_part) {
-  const int32_t part = col / n_part;
-  tma_store_4d(tmap, stage, col - part * n_part, row, part, 0);
+// Two evaluations of gelu_tanh(x) = 0.5 x (1 + tanh(u)),  u = sqrt(2/pi) (x + 0.044715 x^3):
+//  * quantised output (the FFN hot path): tanh.approx (one MUFU, ABSOLUTE error <= 2^-11 on tanh, i.e. <= 2.5e-4 |x| on
+//    the result): far below the int8 step amax/128 the value is rounded to next; compared with the oracle's exact
+//    GELU the codes differ by one on ~1 % of the elements (tests/test_gpu_quant_gemm.py);
+//  * 16-bit output: x * sigmoid(2u) with ex2 + rcp (two MUFU, relative error ~2^-21 everywhere, including the negative
+//    tail where 1 + tanh(u) cancels): within one ulp of torch's fp32 GELU after rounding to T.
+__device__ __forceinline__ float gelu_tanh_approx(float x) {
+  const float u = __fmul_rn(__fmaf_rn(__fmul_rn(x, x), 0.7978845608028654f * 0.044715f, 0.7978845608028654f), x);
+  float t;
+  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(u));
+  const float hx = __fmul_rn(x, 0.5f);
+  return __fmaf_rn(hx, t, hx);
+}
+__device__ __forceinline__ float gelu_precise(float x) {
+  // -2u*log2(e) = x * (c1 + c3 x^2);  x * 1/(1 + 2^z);  z -> +inf gives x*0 = 0 (sign kept), z -> -inf gives x
+  const float z = x * fmaf(-0.10294324f, x * x, -2.3022082f);
+  float r;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + fast_exp2(z)));
+  return x * r;
 }
 
-// kCluster: CTAs are launched as clusters of 2 that work on vertically adjacent tiles (m, n) and (m+1, n).  Each CTA
-// loads its own A tile and HALF of the shared B tile, multicasting that half to both CTAs: 32 KB instead of 48 KB cross
-// the L2->SM fabric per CTA and K-block.  A stage may only be refilled when BOTH CTAs' MMAs have released it, so the
-// stage-empty barriers count 2 arrivals and the MMA warps commit to both CTAs.
 // kRowScale: the LTX-2 client's variant (TurboT2AV ltx_distillation/tilelang_w8a8.py:78-117): a_s [m] per activation row,
-// b_s [n] per output channel, int32 accumulation over ALL of K inside TMEM and ONE epilogue per tile
-// c = T(float(acc) * a_s[i] * b_s[j] + bias[j]).  No per-K-block dequant, so the tensor pipe is the limiter.
-template <typename T, bool kCluster, bool kRowScale>
+// b_s [n] per output channel, int32 accumulation over ALL of K in the wgmma accumulator and ONE epilogue per tile
+// c = T(float(acc) * a_s[i] * b_s[j] + bias[j]).
+template <typename T, bool kRowScale>
 __global__ void __launch_bounds__(kThreads, 1)
-gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 const __grid_constant__ CUtensorMap tmap_c, GemmParams p) {
+gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // 1024-aligned, stays a shared-space pointer
-  if (kAlignSlack < 1024 && ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u) > kAlignSlack) __trap();
-  uint8_t* c_stage = smem + size_t(kStages) * kStageBytes;  // [kEpiWarps][2 boxes][32 rows][128 B]
-  uint8_t* bias_slots = c_stage + kEpiWarps * kCStageBytes;  // [kEpiWarps][128 x T]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(bias_slots + kEpiWarps * kBiasSlot);
-  uint64_t* full_bar = bars;                      // [kStages]  TMA -> MMA
-  uint64_t* empty_bar = bars + kStages;           // [kStages]  MMA -> TMA
-  uint64_t* tmem_full = bars + 2 * kStages;       // [2]        MMA -> epilogue
-  uint64_t* tmem_empty = bars + 2 * kStages + 2;  // [2]        epilogue -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 4);
-  float* amax_x = reinterpret_cast<float*>(bars + 2 * kStages + 5);  // [kEpiWarps] block-amax exchange (quantised output)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + size_t(kStages) * kStageBytes);
+  uint64_t* full_bar = bars;                // [kStages]  TMA -> MMA
+  uint64_t* empty_bar = bars + kStages;     // [kStages]  MMA -> TMA (one arrival per consumer warp)
+  float* amax_x = reinterpret_cast<float*>(bars + 2 * kStages);  // [kConsumerWarps] block-amax exchange (quantised output)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t crank = kCluster ? cluster_ctarank() : 0u;
-  // work items: single tiles, or vertical tile pairs (one per cluster) in the cluster variant
-  const int work_first = kCluster ? int(blockIdx.x >> 1) : int(blockIdx.x);
-  const int work_stride = kCluster ? int(gridDim.x >> 1) : int(gridDim.x);
-  auto tile_of = [&](int work, int& m_tile, int& n_tile) {
-    n_tile = work % p.n_tiles;
-    m_tile = kCluster ? 2 * (work / p.n_tiles) + int(crank) : work / p.n_tiles;
-  };
+  const int n_tile = blockIdx.x, m_tile = blockIdx.y;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], kCluster ? 2 : 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], kEpiWarps);
+      mbar_init(&empty_bar[i], kConsumerWarps);
     }
     mbar_fence_init();
   }
-  if (warp == kMmaWarp) tmem_alloc<kTmemCols>(tmem_slot);
-  if (warp == kTmaWarp && lane == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    tma_prefetch_desc(&tmap_c);
-  }
-  tc_fence_before_sync();
-  if (kCluster) cluster_sync_all(); else __syncthreads();  // barrier inits visible cluster-wide before any remote arrive
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
 
-  if (warp >= kEpiWarps) {
-   reg_dealloc<56>();  // pool = 384 x 168 = 64512 regs = 256 x 224 + 128 x 56
-   if (warp == kTmaWarp) {
+  if (warp == kConsumerWarps) {
     // ------------------------------------------------------------------ TMA producer
     if (lane == 0) {
-      uint32_t it = 0;
-      for (int work = work_first; work < p.total_tiles; work += work_stride) {
-        int m_tile, n_tile;
-        tile_of(work, m_tile, n_tile);
-        for (int kb = 0; kb < p.k_blocks; ++kb, ++it) {
-          const uint32_t stage = it % kStages, phase = (it / kStages) & 1u;
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          uint8_t* sa = smem + size_t(stage) * kStageBytes;
-          mbar_expect_tx(&full_bar[stage], kStageBytes);
-          tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * BK, m_tile * BM);
-          if (kCluster)  // my half (128 rows) of the shared B tile, delivered to both CTAs
-            tma_load_2d_mcast(sa + kATile + crank * (kBTile / 2), &tmap_b, &full_bar[stage], kb * BK,
-                              n_tile * BN + int(crank) * (BN / 2), uint16_t(3));
-          else
-            tma_load_2d(sa + kATile, &tmap_b, &full_bar[stage], kb * BK, n_tile * BN);
-        }
+      tma_prefetch_desc(&tmap_a);
+      tma_prefetch_desc(&tmap_b);
+      for (int kb = 0; kb < p.k_blocks; ++kb) {
+        const uint32_t stage = kb % kStages, phase = (kb / kStages) & 1u;
+        mbar_wait(&empty_bar[stage], phase ^ 1u);
+        uint8_t* sa = smem + size_t(stage) * kStageBytes;
+        mbar_expect_tx(&full_bar[stage], kStageBytes);
+        tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * BK, m_tile * BM);
+        tma_load_2d(sa + kATile, &tmap_b, &full_bar[stage], kb * BK, n_tile * BN);
       }
     }
-  } else if (warp == kMmaWarp) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(kDFmtS32, kFmtS8, kFmtS8, 0, 0, BM, BN);
-      uint32_t it = 0, tile_it = 0;
-      for (int work = work_first; work < p.total_tiles; work += work_stride, ++tile_it) {
-        for (int kb = 0; kb < p.k_blocks; ++kb, ++it) {
-          const uint32_t stage = it % kStages, phase = (it / kStages) & 1u;
-          // per-block mode: one TMEM buffer per K-block; row-scale mode: one buffer per tile
-          const uint32_t bi = kRowScale ? tile_it : it;
-          const uint32_t buf = bi & 1u, bphase = (bi >> 1) & 1u;
-          if (!kRowScale || kb == 0) mbar_wait(&tmem_empty[buf], bphase ^ 1u);
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after_sync();
-          const uint32_t sa = smem_u32(smem + size_t(stage) * kStageBytes);
-          const uint64_t adesc = make_desc_kmajor_sw128(sa);
-          const uint64_t bdesc = make_desc_kmajor_sw128(sa + kATile);
-          const uint32_t d = tmem_base + buf * BN;
-#pragma unroll
-          for (int ks = 0; ks < BK / 32; ++ks) {
-            // advance 32 bytes (one K=32 int8 slice) inside the 128B swizzle row: +2 in 16-byte units
-            umma_i8_ss(d, adesc + uint64_t(ks * 2), bdesc + uint64_t(ks * 2), idesc,
-                       (ks > 0 || (kRowScale && kb > 0)) ? 1u : 0u);
-          }
-          if (kCluster) umma_commit_mcast(&empty_bar[stage], uint16_t(3)); else umma_commit(&empty_bar[stage]);
-          if (!kRowScale || kb == p.k_blocks - 1) umma_commit(&tmem_full[buf]);
-        }
-      }
-    }
-   }
-  } else {
-    // ------------------------------------------------------------------ dequant + epilogue warps
-    reg_alloc<224>();
-    const int q4 = warp & 3;           // TMEM lane quarter this warp may access
-    const int half = warp >> 2;        // which 128-column half of the 256-wide tile
-    const uint32_t lane_addr = uint32_t(q4 * 32) << 16;
-    uint32_t it = 0, tile_it = 0;
-    // K-block 0 scales of the tile about to start: fetched while the previous tile's epilogue runs (they sat exposed in front of
-    // the first dequant before: ~600 clk of L2 latency per tile, 7 % of a K = 1536 tile)
-    float as_first = 0.f, bs_first = 0.f;
-    auto first_scales = [&](int work, float& a0, float& b0) {
-      int mt, nt;
-      tile_of(work, mt, nt);
-      const int64_t c0 = int64_t(nt) * BN + half * 128;
-      a0 = __ldg(p.a_s + int64_t(mt < p.m_tiles ? mt : p.m_tiles - 1) * p.k_blocks);
-      b0 = __ldg(p.b_s + (c0 < p.n ? (c0 >> 7) : 0) * p.k_blocks);
-    };
-    if (!kRowScale && work_first < p.total_tiles) first_scales(work_first, as_first, bs_first);
-    for (int work = work_first; work < p.total_tiles; work += work_stride) {
-      int m_tile, n_tile;
-      tile_of(work, m_tile, n_tile);
-      const int64_t col0 = int64_t(n_tile) * BN + half * 128;
-      const bool half_active = col0 < p.n;
-      if (kRowScale) {
-        // ---- one epilogue per tile: c = T(fma(float(acc) * a_s[row], b_s[col], bias[col])): the reference's TileLang
-        //      epilogue compiles (nvcc default -fmad) to I2FP, FMUL, FFMA per element (tools/tilelang_epilogue_probe.py)
-        const uint32_t buf = tile_it & 1u, bphase = (tile_it >> 1) & 1u;
-        ++tile_it;
-        const int64_t row0r = int64_t(m_tile) * BM + q4 * 32;
-        const int64_t rowr = row0r + lane;
-        const float sa = (rowr < p.m) ? __ldg(p.a_s + rowr) : 0.f;
-        const T* biasr = static_cast<const T*>(p.bias);
-        uint8_t* stager = c_stage + warp * kCStageBytes;
-        mbar_wait(&tmem_full[buf], bphase);
-        tc_fence_after_sync();
-        const uint32_t t0r = tmem_base + lane_addr + buf * BN + half * 128;
-#pragma unroll
-        for (int pass = 0; pass < 2; ++pass) {
-          const int64_t colp = col0 + pass * 64;
-          uint32_t r[64];
-          tmem_ld_x64(t0r + pass * 64, r);
-          tmem_ld_wait();
-          if (pass == 1) {  // all TMEM reads of this tile are done: hand the buffer back before the stores
-            tc_fence_before_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[buf]);
-          }
-#pragma unroll
-          for (int ch = 0; ch < 8; ++ch) {
-            uint32_t w[4];
-            float sb[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-            uint32_t bw[4] = {0u, 0u, 0u, 0u};
-            if (half_active && colp + ch * 8 < p.n) {
-              const float4 s0 = __ldg(reinterpret_cast<const float4*>(p.b_s + colp + ch * 8));
-              const float4 s1 = __ldg(reinterpret_cast<const float4*>(p.b_s + colp + ch * 8) + 1);
-              sb[0] = s0.x; sb[1] = s0.y; sb[2] = s0.z; sb[3] = s0.w; sb[4] = s1.x; sb[5] = s1.y; sb[6] = s1.z; sb[7] = s1.w;
-              if (biasr != nullptr) {
-                const uint4 b4 = *reinterpret_cast<const uint4*>(biasr + colp + ch * 8);
-                bw[0] = b4.x; bw[1] = b4.y; bw[2] = b4.z; bw[3] = b4.w;
-              }
-            }
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float f0 = __int2float_rn(static_cast<int>(r[ch * 8 + 2 * j]));
-              const float f1 = __int2float_rn(static_cast<int>(r[ch * 8 + 2 * j + 1]));
-              const float y0 = __fmaf_rn(__fmul_rn(f0, sa), sb[2 * j], F16Traits<T>::lo(bw[j]));
-              const float y1 = __fmaf_rn(__fmul_rn(f1, sa), sb[2 * j + 1], F16Traits<T>::hi(bw[j]));
-              w[j] = F16Traits<T>::pack(y0, y1);
-            }
-            *reinterpret_cast<uint4*>(stager + lane * 128 + ((ch ^ (lane & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
-          }
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = 4 * i + (lane >> 3), cc = lane & 7;
-            const uint4 v = *reinterpret_cast<const uint4*>(stager + rr * 128 + ((cc ^ (rr & 7)) << 4));
-            const int64_t grow = row0r + rr;
-            if (half_active && grow < p.m && colp + cc * 8 < p.n)
-              stg_v4(static_cast<T*>(p.c) + grow * p.n + colp + cc * 8, v);
-          }
-          __syncwarp();
-        }
-        continue;
-      }
-      const float* as_row = p.a_s + int64_t(m_tile < p.m_tiles ? m_tile : p.m_tiles - 1) * p.k_blocks;  // odd tail pair
-      const float* bs_row = p.b_s + (half_active ? (col0 >> 7) : 0) * p.k_blocks;
-      const T* bias = static_cast<const T*>(p.bias);
-      // this warp's 128 bias values: lanes 0-15 fetch 16 bytes each now, the values go to shared memory at the epilogue
-      uint4 bias_reg = make_uint4(0u, 0u, 0u, 0u);
-      if (bias != nullptr && half_active && lane < 16 && col0 + lane * 8 < p.n)
-        bias_reg = __ldg(reinterpret_cast<const uint4*>(bias + col0) + lane);
-
-      float acc[128];
-#pragma unroll
-      for (int j = 0; j < 128; ++j) acc[j] = 0.0f;
-
-      // block scales are fetched one K-block ahead and only multiplied when used, so the global-load latency hides
-      // behind the previous K-block's dequant instead of stalling in front of the barrier wait
-      float as_next = as_first, bs_next = bs_first;
-      uint32_t ra[32], rb[32];
-      auto dq32 = [&](uint32_t (&r)[32], int base, float scale) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          const float f0 = __int2float_rn(static_cast<int>(r[j]));
-          const float f1 = __int2float_rn(static_cast<int>(r[j + 1]));
-          const float2 a = __ffma2_rn(make_float2(f0, f1), make_float2(scale, scale), make_float2(acc[base + j], acc[base + j + 1]));
-          acc[base + j] = a.x;
-          acc[base + j + 1] = a.y;
-        }
-      };
-      bool have_first = false;   // chunk 0 of the upcoming K-block has already been requested into `ra`
-      for (int kb = 0; kb < p.k_blocks; ++kb, ++it) {
-        const uint32_t buf = it & 1u;
-        const float scale = as_next * bs_next;
-        if (kb + 1 < p.k_blocks) {
-          as_next = __ldg(as_row + kb + 1);
-          bs_next = __ldg(bs_row + kb + 1);
-        }
-        const uint32_t t0 = tmem_base + lane_addr + buf * BN + half * 128;
-        if (!have_first) {
-          mbar_wait(&tmem_full[buf], (it >> 1) & 1u);
-          tc_fence_after_sync();
-          tmem_ld_x32(t0, ra);
-        }
-        have_first = false;
-        // chunk c+1 is in flight while chunk c is converted (ra/rb alternate); tcgen05.wait::ld covers the one load
-        // that is outstanding at that point
-        tmem_ld_wait();
-        tmem_ld_x32(t0 + 32, rb);
-        reg_fence_x32(ra);
-        dq32(ra, 0, scale);
-        tmem_ld_wait();
-        tmem_ld_x32(t0 + 64, ra);
-        reg_fence_x32(rb);
-        dq32(rb, 32, scale);
-        tmem_ld_wait();
-        tmem_ld_x32(t0 + 96, rb);
-        reg_fence_x32(ra);
-        dq32(ra, 64, scale);
-        tmem_ld_wait();
-        // every column of this buffer is in registers: hand it back to the MMA warp before converting the last chunk
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[buf]);
-#if TDB_GEMM_XPF
-        if (kb + 1 < p.k_blocks) {  // request chunk 0 of the next K-block so its TMEM latency hides behind the last convert
-          const uint32_t nbuf = (it + 1) & 1u, nphase = ((it + 1) >> 1) & 1u;
-#if TDB_GEMM_XPF == 1
-          mbar_wait(&tmem_full[nbuf], nphase);
-          have_first = true;
-#else
-          have_first = __all_sync(0xffffffffu, mbar_try_wait(&tmem_full[nbuf], nphase));  // only if its MMAs have finished
-#endif
-          if (have_first) {
-            tc_fence_after_sync();
-            tmem_ld_x32(tmem_base + lane_addr + nbuf * BN + half * 128, ra);
-          }
-        }
-#endif
-        reg_fence_x32(rb);
-        dq32(rb, 96, scale);
-      }
-
-      // ---- optional activation: nn.GELU(approximate="tanh") evaluated in fp32 on the T-rounded pre-activation
-      //      (rcm/networks/wan2pt1.py:375 FFN), tanh via MUFU (tanh.approx, |rel err| <= 2^-11)
-      const bool act_gelu = p.act == 1;
-      // Two evaluations of gelu_tanh(x) = 0.5 x (1 + tanh(u)),  u = sqrt(2/pi) (x + 0.044715 x^3):
-      //  * quantised output (the FFN hot path): tanh.approx (one MUFU, ABSOLUTE error <= 2^-11 on tanh, i.e. <= 2.5e-4 |x| on
-      //    the result): far below the int8 step amax/128 the value is rounded to next; measured against the oracle's exact
-      //    GELU the codes differ by one on ~1 % of the elements (tests/test_gpu_quant_gemm.py);
-      //  * 16-bit output: x * sigmoid(2u) with ex2 + rcp (two MUFU, relative error ~2^-21 everywhere, including the negative
-      //    tail where 1 + tanh(u) cancels): within one ulp of torch's fp32 GELU after rounding to T.
-      auto gelu = [](float x) {
-        const float inner = 0.7978845608028654f * fmaf(0.044715f * x * x, x, x);
-        float t;
-        asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(inner));
-        return 0.5f * x * (1.0f + t);
-      };
-      auto gelu_precise = [](float x) {
-        // -2u*log2(e) = x * (c1 + c3 x^2);  x * 1/(1 + 2^z);  z -> +inf gives x*0 = 0 (sign kept), z -> -inf gives x
-        const float z = x * fmaf(-0.10294324f, x * x, -2.3022082f);
-        float r;
-        asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + fast_exp2(z)));
-        return x * r;
-      };
-      // ---- tile epilogue.  The warp owns rows [row0, row0+32) x columns [col0, col0+128) of the tile; a thread owns one
-      //      ROW, so the values go through the warp's private swizzled staging buffer and leave as TMA box stores (the
-      //      tensor map clips rows >= m and columns >= n).  The buffer is reused one tile later: by then the store
-      //      engine has read it (wait_group.read), and the warp never waits for the global write itself.
-      if (work + work_stride < p.total_tiles) first_scales(work + work_stride, as_first, bs_first);  // used after this epilogue
-      const int64_t row0 = int64_t(m_tile) * BM + q4 * 32;
-      uint8_t* stage = c_stage + warp * kCStageBytes;
-      uint8_t* bslot = bias_slots + warp * kBiasSlot;
-      if (lane == 0) tma_store_wait_read<0>();   // previous tile's boxes have left the staging buffer
-      if (lane < 16) *reinterpret_cast<uint4*>(bslot + lane * 16) = bias_reg;
-      __syncwarp();
-      if (p.out_q != nullptr) {
-        // ---- fused a1: this thread's 128 values are one row of the 128x128 quant block (m_tile, col0/128).
-        //      y = the T-rounded value the plain epilogue would store; amax over the block; q = sat_s8(rint(y*128/amax)).
-        //      Packed arithmetic throughout (16-bit x2 add / max, f32x2 multiply-add): this epilogue runs on the warps that
-        //      dequantise, so its issue slots are on the tile's critical path.  The T-rounded values live in the first 64
-        //      accumulator registers as packed pairs between the two passes.
-        const bool row_in = row0 + lane < p.m;
-        uint32_t amax2 = 0u;
-        const float2 gc1 = make_float2(0.7978845608028654f, 0.7978845608028654f);
-        const float2 gc3 = make_float2(0.7978845608028654f * 0.044715f, 0.7978845608028654f * 0.044715f);
-        const float2 ghalf = make_float2(0.5f, 0.5f);
-        uint32_t yw[64];
-#pragma unroll
-        for (int ch = 0; ch < 16; ++ch) {
-          const uint4 b4 = *reinterpret_cast<const uint4*>(bslot + ch * 16);
-          const uint32_t bw[4] = {b4.x, b4.y, b4.z, b4.w};
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            uint32_t y = F16Traits<T>::pack(acc[ch * 8 + 2 * j], acc[ch * 8 + 2 * j + 1]);   // T(acc)
-            if (bias != nullptr) y = F16Traits<T>::add2(y, bw[j]);                            // T(T(acc) + bias)
-            if (act_gelu) {   // T(gelu_tanh(.)): u = x (c1 + c3 x^2), 0.5 x (1 + tanh u) = fma(0.5 x, tanh u, 0.5 x)
-              const float2 xv = make_float2(F16Traits<T>::lo(y), F16Traits<T>::hi(y));
-              const float2 u = __fmul2_rn(__ffma2_rn(__fmul2_rn(xv, xv), gc3, gc1), xv);
-              float2 t;
-              asm("tanh.approx.f32 %0, %1;" : "=f"(t.x) : "f"(u.x));
-              asm("tanh.approx.f32 %0, %1;" : "=f"(t.y) : "f"(u.y));
-              const float2 hx = __fmul2_rn(xv, ghalf);
-              const float2 g = __ffma2_rn(hx, t, hx);
-              y = F16Traits<T>::pack(g.x, g.y);
-            }
-            if (!(row_in && half_active)) y = 0u;
-            yw[ch * 4 + j] = y;
-            amax2 = F16Traits<T>::absmax2(amax2, y);
-          }
-        }
-        float amax = fmaxf(1e-8f, fmaxf(F16Traits<T>::lo(amax2), F16Traits<T>::hi(amax2)));
-        amax = warp_max(amax);
-        if (lane == 0) amax_x[warp] = amax;
-        named_bar_sync(1 + half, 128);  // the 4 warps (lane quarters) of this 128-column half
-#pragma unroll
-        for (int w = 0; w < 4; ++w) amax = fmaxf(amax, amax_x[half * 4 + w]);
-        const float r = __fdiv_rn(128.0f, amax);
-        const float2 r2 = make_float2(r, r);
-        if (q4 == 0 && lane == 0 && half_active && int64_t(m_tile) * BM < p.m)
-          p.out_s[int64_t(m_tile) * (p.n >> 7) + (col0 >> 7)] = amax * 0.0078125f;
-#pragma unroll
-        for (int ch = 0; ch < 8; ++ch) {  // 16 int8 per 16-byte chunk
-          uint32_t w[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint32_t y0 = yw[ch * 8 + j * 2], y1 = yw[ch * 8 + j * 2 + 1];
-            const float2 v0 = __fmul2_rn(make_float2(F16Traits<T>::lo(y0), F16Traits<T>::hi(y0)), r2);
-            const float2 v1 = __fmul2_rn(make_float2(F16Traits<T>::lo(y1), F16Traits<T>::hi(y1)), r2);
-            w[j] = pack4_s8_rne(v0.x, v0.y, v1.x, v1.y);
-          }
-          *reinterpret_cast<uint4*>(stage + lane * 128 + ((ch ^ (lane & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0 && half_active) {
-          tma_store_2d(&tmap_c, stage, int32_t(col0), int32_t(row0));  // int8 box: 128 columns x 32 rows
-          tma_store_commit();
-        }
-        named_bar_sync(1 + half, 128);  // amax_x is reused by the next tile
-        continue;
-      }
-#pragma unroll
-      for (int ch = 0; ch < 16; ++ch) {  // 8 columns per 16-byte chunk; box 0 = columns 0-63, box 1 = columns 64-127
-        if (kStoreRounds == 2 && ch == 8) {  // small staging buffer: the first box must have left it before the second is written
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            if (half_active) {
-              store_c(&tmap_c, stage, int32_t(col0), int32_t(row0), p.n_part);
-              tma_store_commit();
-            }
-            tma_store_wait_read<0>();
-          }
-          __syncwarp();
-        }
-        uint32_t w[4];
-        uint32_t bw[4] = {0u, 0u, 0u, 0u};
-        if (bias != nullptr) {
-          const uint4 b4 = *reinterpret_cast<const uint4*>(bslot + ch * 16);
-          bw[0] = b4.x; bw[1] = b4.y; bw[2] = b4.z; bw[3] = b4.w;
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          // T(acc) then the packed 16-bit add: one rounding each, exactly the module's `out + bias` on 16-bit tensors
-          uint32_t y = F16Traits<T>::pack(acc[ch * 8 + 2 * j], acc[ch * 8 + 2 * j + 1]);
-          if (bias != nullptr) y = F16Traits<T>::add2(y, bw[j]);
-          if (act_gelu) y = F16Traits<T>::pack(gelu_precise(F16Traits<T>::lo(y)), gelu_precise(F16Traits<T>::hi(y)));
-          w[j] = y;
-        }
-        *reinterpret_cast<uint4*>(stage + (kStoreRounds == 2 ? 0 : (ch >> 3) * 4096) + lane * 128 + (((ch & 7) ^ (lane & 7)) << 4)) =
-            make_uint4(w[0], w[1], w[2], w[3]);
-      }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0 && half_active) {
-        if (kStoreRounds == 1) {
-          store_c(&tmap_c, stage, int32_t(col0), int32_t(row0), p.n_part);
-          if (col0 + 64 < p.n) store_c(&tmap_c, stage + 4096, int32_t(col0 + 64), int32_t(row0), p.n_part);
-        } else if (col0 + 64 < p.n) {
-          store_c(&tmap_c, stage, int32_t(col0 + 64), int32_t(row0), p.n_part);
-        }
-        tma_store_commit();
-      }
-    }
-    if (lane == 0) tma_store_wait_read<0>();  // shared memory must outlive the last store's reads
+    return;
   }
 
-  tc_fence_before_sync();
-  if (kCluster) cluster_sync_all(); else __syncthreads();  // the peer may still multicast into / arrive on this CTA
-  if (warp == kMmaWarp) {
-    tc_fence_after_sync();
-    tmem_dealloc<kTmemCols>(tmem_base);
+  // ------------------------------------------------------------------ MMA + dequant + epilogue warpgroups
+  const int wg = warp >> 2, w4 = warp & 3;
+  const uint32_t sbase = smem_u32(smem);
+  // the four K=32 steps of K-block kb into `d` (onto its contents when `acc_in`)
+  auto issue = [&](uint32_t (&d)[64], int kb, bool acc_in) {
+    const uint32_t stage = kb % kStages;
+    mbar_wait(&full_bar[stage], (kb / kStages) & 1u);
+    const uint32_t sa = sbase + stage * kStageBytes;
+    const uint64_t adesc = make_desc_kmajor_sw128(sa + wg * (64 * 128));
+    const uint64_t bdesc = make_desc_kmajor_sw128(sa + kATile);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < BK / 32; ++ks)  // +32 bytes (one K=32 int8 slice) inside the 128B swizzle row: +2 in 16-byte units
+      wgmma_i8_ss<BN>(d, adesc + uint64_t(ks * 2), bdesc + uint64_t(ks * 2), (ks > 0 || acc_in) ? 1u : 0u);
+    wgmma_commit();
+  };
+  auto release = [&](int kb) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[kb % kStages]);
+  };
+
+  // fragment coordinates (common.cuh): register i holds row r_lo + 8 ((i >> 1) & 1), column 8 (i >> 2) + cq + (i & 1)
+  const int r_lo = wg * 64 + w4 * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const int64_t row0 = int64_t(m_tile) * BM + r_lo, row1 = row0 + 8;
+  const int64_t col_base = int64_t(n_tile) * BN + cq;
+  const T* bias = static_cast<const T*>(p.bias);
+
+  if constexpr (kRowScale) {
+    uint32_t ia[64];
+    for (int kb = 0; kb < p.k_blocks; ++kb) {
+      issue(ia, kb, kb > 0);
+      wgmma_wait<0>();
+      reg_fence(ia);
+      release(kb);
+    }
+    // c = T(fma(float(acc) * a_s[row], b_s[col], bias[col])): the reference's TileLang epilogue compiles (nvcc default
+    // -fmad) to I2FP, FMUL, FFMA per element (tools/tilelang_epilogue_probe.py)
+    const float sa0 = row0 < p.m ? __ldg(p.a_s + row0) : 0.f, sa1 = row1 < p.m ? __ldg(p.a_s + row1) : 0.f;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int64_t col = col_base + 8 * j;
+      if (col >= p.n) continue;
+      const float sb0 = __ldg(p.b_s + col), sb1 = __ldg(p.b_s + col + 1);
+      const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float sa = h ? sa1 : sa0;
+        const float y0 = __fmaf_rn(__fmul_rn(__int2float_rn(static_cast<int>(ia[4 * j + 2 * h])), sa), sb0, F16Traits<T>::lo(bw));
+        const float y1 = __fmaf_rn(__fmul_rn(__int2float_rn(static_cast<int>(ia[4 * j + 2 * h + 1])), sa), sb1, F16Traits<T>::hi(bw));
+        const int64_t row = h ? row1 : row0;
+        if (row < p.m) *reinterpret_cast<uint32_t*>(static_cast<T*>(p.c) + row * p.n + col) = F16Traits<T>::pack(y0, y1);
+      }
+    }
+    return;
+  }
+
+  // block scales: a_s [m/128, k_blocks] row m_tile, b_s [n/128, k_blocks] row n_tile (the tile is one 128-column block)
+  const float* as_row = p.a_s + int64_t(m_tile) * p.k_blocks;
+  const float* bs_row = p.b_s + int64_t(n_tile) * p.k_blocks;
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+  // float(s) without the conversion unit: as_float(0x4B400000 + s) == 1.5*2^23 + s exactly for |s| < 2^22 (a K-block sum
+  // is at most 128^3 = 2^21 in magnitude), and subtracting 1.5*2^23 is exact, so this is the same value __int2float_rn gives
+  // on the full-rate integer-add and FP32 pipes
+  constexpr float kMagicF = 12582912.0f;
+  constexpr int kMagicI = 0x4B400000;
+  uint32_t ia[64];
+  for (int kb = 0; kb < p.k_blocks; ++kb) {
+    issue(ia, kb, false);
+    const float scale = __ldg(as_row + kb) * __ldg(bs_row + kb);
+    wgmma_wait<0>();
+    reg_fence(ia);
+    release(kb);
+#pragma unroll
+    for (int i = 0; i < 64; ++i)
+      acc[i] = __fmaf_rn(__fsub_rn(__int_as_float(static_cast<int>(ia[i]) + kMagicI), kMagicF), scale, acc[i]);
+  }
+
+  const bool act_gelu = p.act == 1;
+  if (p.out_q != nullptr) {
+    // ---- fused a1: the tile is one 128x128 quant block (m_tile, n_tile).  y = the T-rounded value the plain epilogue
+    //      would store (rows >= m count as 0); amax over the block; q = sat_s8(rint(y*128/amax)).
+    uint32_t yw[32];
+    uint32_t amax2 = 0u;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int64_t col = col_base + 8 * j;
+      const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        uint32_t y = F16Traits<T>::pack(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);   // T(acc)
+        if (bias != nullptr) y = F16Traits<T>::add2(y, bw);                            // T(T(acc) + bias)
+        if (act_gelu) y = F16Traits<T>::pack(gelu_tanh_approx(F16Traits<T>::lo(y)), gelu_tanh_approx(F16Traits<T>::hi(y)));
+        if ((h ? row1 : row0) >= p.m) y = 0u;
+        yw[2 * j + h] = y;
+        amax2 = F16Traits<T>::absmax2(amax2, y);
+      }
+    }
+    float amax = fmaxf(1e-8f, fmaxf(F16Traits<T>::lo(amax2), F16Traits<T>::hi(amax2)));
+    amax = warp_max(amax);
+    if (lane == 0) amax_x[warp] = amax;
+    named_bar_sync(1, kConsumerWarps * 32);
+#pragma unroll
+    for (int w = 0; w < kConsumerWarps; ++w) amax = fmaxf(amax, amax_x[w]);
+    const float r = __fdiv_rn(128.0f, amax);
+    if (threadIdx.x == 0) p.out_s[int64_t(m_tile) * (p.n >> 7) + n_tile] = amax * 0.0078125f;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int64_t col = col_base + 8 * j;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t y = yw[2 * j + h];
+        const int q0 = __float2int_rn(fminf(__fmul_rn(F16Traits<T>::lo(y), r), 127.0f));
+        const int q1 = __float2int_rn(fminf(__fmul_rn(F16Traits<T>::hi(y), r), 127.0f));
+        const int64_t row = h ? row1 : row0;
+        if (row < p.m)
+          *reinterpret_cast<uint16_t*>(p.out_q + row * p.n + col) = static_cast<uint16_t>((q0 & 0xFF) | ((q1 & 0xFF) << 8));
+      }
+    }
+    return;
+  }
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int64_t col = col_base + 8 * j;
+    if (col >= p.n) continue;
+    const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
+    const int64_t part = col / p.n_part;
+    T* cp = static_cast<T*>(p.c) + part * p.m * p.n_part + (col - part * p.n_part);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      // T(acc) then the packed 16-bit add: one rounding each, exactly the module's `out + bias` on 16-bit tensors
+      uint32_t y = F16Traits<T>::pack(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      if (bias != nullptr) y = F16Traits<T>::add2(y, bw);
+      if (act_gelu) y = F16Traits<T>::pack(gelu_precise(F16Traits<T>::lo(y)), gelu_precise(F16Traits<T>::hi(y)));
+      const int64_t row = h ? row1 : row0;
+      if (row < p.m) *reinterpret_cast<uint32_t*>(cp + row * p.n_part) = y;
+    }
   }
 }
 
-template <typename T, bool kCluster, bool kRowScale>
-int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const GemmParams& p, cudaStream_t st) {
-  auto kern = gemm_w8a8_kernel<T, kCluster, kRowScale>;
-  static bool attr_set[64] = {false};  // per device: the attribute is sticky, no need to set it on every launch
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-    if (int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kSmemBytes)),
-                            "cudaFuncSetAttribute(gemm_w8a8)"))
-      return rc;
-    if (dev >= 0 && dev < 64) attr_set[dev] = true;
-  }
-  int grid = kCluster ? 2 * p.total_tiles : p.total_tiles;
-  const int cap = kCluster ? (sm_count() & ~1) : sm_count();
-  if (grid > cap) grid = cap;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = kSmemBytes;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = kCluster ? 2 : 1;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return check_cuda(cudaLaunchKernelEx(&cfg, kern, ta, tb, tc, p), "gemm_w8a8_kernel launch");
+template <typename T, bool kRowScale>
+int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int64_t m_tiles, int64_t n_tiles,
+           cudaStream_t st) {
+  auto kern = gemm_w8a8_kernel<T, kRowScale>;
+  static bool attr_done[64] = {false};
+  if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), kSmemBytes, attr_done,
+                                         "cudaFuncSetAttribute(gemm_w8a8)"))
+    return rc;
+  kern<<<dim3(static_cast<unsigned>(n_tiles), static_cast<unsigned>(m_tiles)), kThreads, kSmemBytes, st>>>(ta, tb, p);
+  return check_launch("gemm_w8a8_kernel");
 }
 
 }  // namespace
@@ -577,9 +308,9 @@ static int gemm_impl(const int8_t* a_q, const float* a_s, const int8_t* b_q, con
                      int8_t* out_q, float* out_s, int c_dtype, int64_t m, int64_t n, int64_t k, int epilogue, void* stream,
                      bool row_scale, int64_t parts) {
   using namespace tdb;
-  if (parts < 1 || n % parts != 0 || (parts > 1 && (n / parts) % BN != 0))
-    return fail(TDB200_ERR_UNSUPPORTED, "gemm_w8a8_split: n=%lld must split into %lld parts of a multiple of %d columns",
-                (long long)n, (long long)parts, BN);
+  if (parts < 1 || n % parts != 0 || (parts > 1 && (n / parts) % 256 != 0))
+    return fail(TDB200_ERR_UNSUPPORTED, "gemm_w8a8_split: n=%lld must split into %lld parts of a multiple of 256 columns",
+                (long long)n, (long long)parts);
   if (epilogue != TDB200_EPILOGUE_NONE && epilogue != TDB200_EPILOGUE_GELU_TANH)
     return fail(TDB200_ERR_INVALID_ARG, "gemm_w8a8_ex: unknown epilogue %d", epilogue);
   if (!a_q || !a_s || !b_q || !b_s || !c) return fail(TDB200_ERR_INVALID_ARG, "gemm_w8a8: null pointer");
@@ -593,30 +324,17 @@ static int gemm_impl(const int8_t* a_q, const float* a_s, const int8_t* b_q, con
     return fail(TDB200_ERR_INVALID_ARG, "gemm_w8a8: a_q, b_q, c and bias must be 16-byte aligned");
   if (m > (int64_t(1) << 31) - 256 || n > (int64_t(1) << 31) - 256 || k > (int64_t(1) << 31) - 256)
     return fail(TDB200_ERR_UNSUPPORTED, "gemm_w8a8: dimension exceeds int32 TMA coordinates");
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
 
-  const int64_t m_tiles = cdiv64(m, BM);
-  const bool use_cluster = m_tiles >= 2;  // pairs of vertically adjacent tiles share the B tile by TMA multicast
+  const int64_t m_tiles = cdiv64(m, BM), n_tiles = cdiv64(n, BN);
+  if (m_tiles > 65535) return fail(TDB200_ERR_UNSUPPORTED, "gemm_w8a8: m=%lld exceeds %d rows", (long long)m, 65535 * BM);
   if (c_dtype != TDB200_DTYPE_BF16 && c_dtype != TDB200_DTYPE_FP16)
     return fail(TDB200_ERR_UNSUPPORTED, "gemm_w8a8: output dtype tag %d (bf16/fp16 only, gemm.cu:41-65)", c_dtype);
-  CUtensorMap ta, tb, tc;
+  CUtensorMap ta, tb;
   if (int rc = make_tmap_2d(&ta, a_q, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, uint64_t(k), uint64_t(m), uint64_t(k), BK, BM))
     return rc;
-  if (int rc = make_tmap_2d(&tb, b_q, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, uint64_t(k), uint64_t(n), uint64_t(k), BK,
-                            use_cluster ? BN / 2 : BN))
+  if (int rc = make_tmap_2d(&tb, b_q, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, uint64_t(k), uint64_t(n), uint64_t(k), BK, BN))
     return rc;
-  // output boxes of the TMA-store epilogue: one warp's 32 rows x 64 columns of T, or x 128 int8 codes (quantised output)
-  if (out_q != nullptr) {
-    if (int rc = make_tmap_2d(&tc, out_q, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, uint64_t(n), uint64_t(m), uint64_t(n), 128, 32))
-      return rc;
-  } else {
-    const CUtensorMapDataType t16 = c_dtype == TDB200_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-    const uint64_t n_part = uint64_t(n / parts);
-    const uint64_t dims[4] = {n_part, uint64_t(m), uint64_t(parts), 1};
-    const uint64_t str[3] = {n_part * 2, uint64_t(m) * n_part * 2, uint64_t(m) * uint64_t(n) * 2};
-    const uint32_t box[4] = {64, 32, 1, 1};
-    if (int rc = make_tmap_4d(&tc, c, t16, 2, dims, str, box)) return rc;
-  }
 
   GemmParams p;
   p.a_s = a_s;
@@ -631,22 +349,12 @@ static int gemm_impl(const int8_t* a_q, const float* a_s, const int8_t* b_q, con
   p.out_s = out_s;
   p.n_part = static_cast<int>(n / parts);
   p.k_blocks = static_cast<int>(k / BK);
-  p.n_tiles = static_cast<int>(cdiv64(n, BN));
-  p.m_tiles = static_cast<int>(m_tiles);
-  const int64_t total = (use_cluster ? cdiv64(m_tiles, 2) : m_tiles) * p.n_tiles;
-  if (total > (int64_t(1) << 29)) return fail(TDB200_ERR_UNSUPPORTED, "gemm_w8a8: too many tiles");
-  p.total_tiles = static_cast<int>(total);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (row_scale) {
     if (k > 16384 * 8) return fail(TDB200_ERR_UNSUPPORTED, "gemm_w8a8_rowwise: k too large for int32 accumulation");
-    if (c_dtype == TDB200_DTYPE_BF16)
-      return use_cluster ? launch<__nv_bfloat16, true, true>(ta, tb, tc, p, st) : launch<__nv_bfloat16, false, true>(ta, tb, tc, p, st);
-    if (c_dtype == TDB200_DTYPE_FP16)
-      return use_cluster ? launch<__half, true, true>(ta, tb, tc, p, st) : launch<__half, false, true>(ta, tb, tc, p, st);
+    if (c_dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16, true>(ta, tb, p, m_tiles, n_tiles, st);
+    return launch<__half, true>(ta, tb, p, m_tiles, n_tiles, st);
   }
-  if (c_dtype == TDB200_DTYPE_BF16)
-    return use_cluster ? launch<__nv_bfloat16, true, false>(ta, tb, tc, p, st) : launch<__nv_bfloat16, false, false>(ta, tb, tc, p, st);
-  if (c_dtype == TDB200_DTYPE_FP16)
-    return use_cluster ? launch<__half, true, false>(ta, tb, tc, p, st) : launch<__half, false, false>(ta, tb, tc, p, st);
-  return fail(TDB200_ERR_UNSUPPORTED, "gemm_w8a8: output dtype tag %d (bf16/fp16 only, gemm.cu:41-65)", c_dtype);
+  if (c_dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16, false>(ta, tb, p, m_tiles, n_tiles, st);
+  return launch<__half, false>(ta, tb, p, m_tiles, n_tiles, st);
 }

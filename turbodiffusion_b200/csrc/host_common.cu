@@ -31,16 +31,16 @@ int check_launch(const char* kernel_name) { return check_cuda(cudaGetLastError()
 int sm_count() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
   }
   return cached[dev];
 }
 
-int require_sm100() {
+int require_sm90() {
   static int ok[64] = {0};  // 0 unknown, 1 ok, -1 bad
   int dev = 0;
   int rc = check_cuda(cudaGetDevice(&dev), "cudaGetDevice");
@@ -50,10 +50,10 @@ int require_sm100() {
     int major = 0;
     rc = check_cuda(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev), "cudaDeviceGetAttribute");
     if (rc) return rc;
-    ok[dev] = (major == 10) ? 1 : -1;
+    ok[dev] = (major == 9) ? 1 : -1;
   }
   if (ok[dev] < 0)
-    return fail(TDB200_ERR_ARCH, "libtdb200 kernels are built for sm_100a only; device %d is not compute capability 10.x", dev);
+    return fail(TDB200_ERR_ARCH, "libtdb200 kernels are built for sm_90a only; device %d is not compute capability 9.x", dev);
   return 0;
 }
 

@@ -21,8 +21,8 @@ int check_launch(const char* kernel_name);
 // Number of SMs of the current device (cached per device).
 int sm_count();
 
-// Verifies the current device is compute capability 10.x; the kernels are sm_100a-only.
-int require_sm100();
+// Verifies the current device is compute capability 9.x; the kernels are sm_90a-only.
+int require_sm90();
 
 // Rank-2 tiled tensor map over a row-major [outer, inner] matrix of `elem_bytes`-sized elements.
 // `row_stride_bytes` is the distance between consecutive outer indices (multiple of 16).

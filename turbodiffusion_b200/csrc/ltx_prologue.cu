@@ -167,7 +167,7 @@ int run(const char* name, const void* x, const void* res, int dtype, const float
   if (!aligned16(x) || !aligned16(y) || !aligned16(table) || !aligned16(ts) || (res && !aligned16(res)))
     return fail(TDB200_ERR_INVALID_ARG, "%s: buffers must be 16-byte aligned", name);
   if (b * tokens > 0x7FFFFFFFll) return fail(TDB200_ERR_UNSUPPORTED, "%s: too many rows", name);
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
   LtxParams p{x, res, table, ts, y, b * tokens, int(tokens), int(ts_tokens), int(n), num_ada, idx0, idx1, eps};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16, kOp>(p, st);
@@ -199,7 +199,7 @@ extern "C" int tdb200_ltx_split_rope(const void* x, const void* cos_freqs, const
   using namespace tdb;
   if (!x || !cos_freqs || !sin_freqs || !y) return fail(TDB200_ERR_INVALID_ARG, "ltx_split_rope: null pointer");
   if (b <= 0 || t <= 0 || h <= 0 || d <= 0 || d % 16 != 0) return fail(TDB200_ERR_INVALID_ARG, "ltx_split_rope: bad shape (d %% 16 == 0)");
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
   const int64_t chunks = b * t * h * (d / 16);
   int64_t grid = (chunks + 255) / 256;
   const int64_t cap = int64_t(sm_count()) * 16;
@@ -275,7 +275,7 @@ extern "C" int tdb200_quant_int8_rowwise(const void* x, int dtype, int64_t m, in
   if (m == 0) return TDB200_OK;
   if (!aligned16(x) || (reinterpret_cast<uintptr_t>(q) & 7u)) return fail(TDB200_ERR_INVALID_ARG, "quant_int8_rowwise: misaligned buffer");
   if (m > 0x7FFFFFFFll) return fail(TDB200_ERR_UNSUPPORTED, "quant_int8_rowwise: too many rows");
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int nchunks = static_cast<int>(k / 8);
   const unsigned grid = static_cast<unsigned>(m);

@@ -82,7 +82,7 @@ __device__ __forceinline__ void load_params(const float* __restrict__ p, float* 
 // difference (< 1e-6 abs) moves a bf16 result by one ulp in ~1e-4 of the elements, inside the stated RoPE tolerance,
 // and keeps this kernel HBM-bound instead of bound by the ~40-instruction accurate sincosf.
 __device__ __forceinline__ void rope_sincos(float x, float* sn, float* cs) {
-  const float n = rintf(x * 0.15915494309189535f);   // (a magic-add rounding on the FMA pipe measured slower here: 72 vs 62 us)
+  const float n = rintf(x * 0.15915494309189535f);
   float r = fmaf(n, -6.2831854820251465f, x);
   r = fmaf(n, 1.7484555e-7f, r);
   *sn = __sinf(r);
@@ -113,7 +113,7 @@ struct RowParams {
 // kWarpRow = false: one CTA per row (reductions through shared memory, two __syncthreads each).
 // kWarpRow = true : one WARP per row, kThreads/32 rows per CTA: the reductions are shuffles only, no CTA barrier, and a
 //   lane keeps kChunks independent 16-byte loads in flight (6 for dim 1536, 20 for dim 5120), which is what an HBM-bound
-//   row kernel needs; round 1's CTA-per-row form reached 0.27-0.6 of the HBM peak.
+//   row kernel needs.  The CTA-per-row form serves longer rows.
 template <typename T, int kNorm, int kPost, int kThreads, int kChunks, bool kResidIn = false, bool kWarpRow = false>
 __global__ void __launch_bounds__(kThreads) row_norm_kernel(RowParams p) {
   __shared__ float red[kThreads / 32];
@@ -252,7 +252,7 @@ __global__ void __launch_bounds__(kThreads) row_norm_kernel(RowParams p) {
       if (kPost == kPostRopeTable) {
         // the same rotation with (cos, sin) read from a table built once per angle tensor: every head of a row and every
         // layer / projection of a step reuse the same 64 pairs, so the table lines stay in L1/L2 and the kernel keeps no
-        // range reduction or MUFU work (the sincos form is issue-bound: profiles/r02_ncu_prologue.txt)
+        // range reduction or MUFU work (the in-kernel sincos form spends issue slots on both)
         float cs[E];
         load_params<E>(p.angles + (row * (p.d >> 1) + ((col % p.d) >> 1)) * 2, cs);
 #pragma unroll
@@ -278,9 +278,9 @@ int launch_rows(const RowParams& p, cudaStream_t st) {
 #define TDB_LAUNCH_W(CH)                                                                   \
   row_norm_kernel<T, kNorm, kPost, 256, CH, kResidIn, true><<<wgrid, 256, 0, st>>>(p);    \
   return check_launch("row_norm_kernel(warp)")
-    // measured (profiles/r02_microbench_prologue.jsonl): the warp-per-row form wins for dim 1536 (LayerNorm 0.61 -> 0.79 of the HBM
-    // peak, RMSNorm+RoPE 0.37 -> 0.49) and loses for dim 5120 (20 chunks per lane: registers cut the occupancy), so it is
-    // used up to 8 chunks per lane (n <= 2048 16-bit elements)
+    // used up to 8 chunks per lane (n <= 2048 16-bit elements, e.g. dim 1536): more chunks per lane hold more registers and cut
+    // the occupancy the shuffle-only form relies on, so longer rows (dim 5120) take the CTA-per-row form.  The threshold has not
+    // been re-measured on H100.
     if (nchunks <= 32 * 2) { TDB_LAUNCH_W(2); }
     if (nchunks <= 32 * 4) { TDB_LAUNCH_W(4); }
     if (nchunks <= 32 * 6) { TDB_LAUNCH_W(6); }
@@ -306,7 +306,7 @@ int check_rows(const char* name, const void* x, const void* y, int64_t m, int64_
   if (n % elems_per_chunk != 0)
     return fail(TDB200_ERR_UNSUPPORTED, "%s: n=%lld must be a multiple of %d", name, (long long)n, elems_per_chunk);
   if (!aligned16(x) || !aligned16(y)) return fail(TDB200_ERR_INVALID_ARG, "%s: buffers must be 16-byte aligned", name);
-  return require_sm100();
+  return require_sm90();
 }
 
 template <int kNorm, int kPost>

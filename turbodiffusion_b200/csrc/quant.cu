@@ -76,9 +76,9 @@ __global__ void __launch_bounds__(kThreads) quant_int8_block128_kernel(const T* 
 // gelu_tanh(x) = 0.5 x (1 + tanh(u)), u = sqrt(2/pi) (x + 0.044715 x^3) (nn.GELU(approximate="tanh"), rcm/networks/wan2pt1.py:375),
 // tanh by MUFU (tanh.approx.f32, absolute error <= 2^-11): the same evaluation as the GEMM's fused quantised-output epilogue, whose
 // int8 codes it reproduces; against torch's fp32 GELU the codes differ by one on ~1 % of the elements (the error is ~2 % of an
-// int8 step).  Arithmetic is packed (f32x2 FMUL2/FFMA2, bf16x2 max) because the kernel is bound by issue slots, not by HBM:
-// measured forms at shape A 32760 x 8960 (profiles/r02_microbench_prologue.jsonl): ex2+rcp sigmoid 0.285 ms, Newton reciprocal on
-// the FMA pipe 0.371 ms.
+// int8 step).  The per-element work is kept to one MUFU tanh and a few FP32 multiply-adds (lane-wise f32x2 helpers of
+// common.cuh, one FMUL/FFMA per lane on sm_90) plus packed bf16x2 max for the block amax, so that the kernel stays close to
+// its 3 bytes of HBM traffic per element.
 template <typename T>
 __global__ void __launch_bounds__(kThreads) gelu_quant_int8_block128_kernel(const T* __restrict__ x, int8_t* __restrict__ q,
                                                                             float* __restrict__ s, int64_t m, int64_t k,
@@ -108,12 +108,12 @@ __global__ void __launch_bounds__(kThreads) gelu_quant_int8_block128_kernel(cons
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float2 xv = make_float2(F16Traits<T>::lo(w[j]), F16Traits<T>::hi(w[j]));
-      const float2 u = __fmul2_rn(__ffma2_rn(__fmul2_rn(xv, xv), c3, c1), xv);
+      const float2 u = fmul2_rn(ffma2_rn(fmul2_rn(xv, xv), c3, c1), xv);
       float2 t;
       asm("tanh.approx.f32 %0, %1;" : "=f"(t.x) : "f"(u.x));
       asm("tanh.approx.f32 %0, %1;" : "=f"(t.y) : "f"(u.y));
-      const float2 hx = __fmul2_rn(xv, half2v);
-      const float2 y = __ffma2_rn(hx, t, hx);
+      const float2 hx = fmul2_rn(xv, half2v);
+      const float2 y = ffma2_rn(hx, t, hx);
       g[p][j] = F16Traits<T>::pack(y.x, y.y);
       amax2 = F16Traits<T>::absmax2(amax2, g[p][j]);
     }
@@ -133,8 +133,8 @@ __global__ void __launch_bounds__(kThreads) gelu_quant_int8_block128_kernel(cons
     uint32_t word[2];
 #pragma unroll
     for (int j = 0; j < 4; j += 2) {
-      const float2 v0 = __fmul2_rn(make_float2(F16Traits<T>::lo(g[p][j]), F16Traits<T>::hi(g[p][j])), r2);
-      const float2 v1 = __fmul2_rn(make_float2(F16Traits<T>::lo(g[p][j + 1]), F16Traits<T>::hi(g[p][j + 1])), r2);
+      const float2 v0 = fmul2_rn(make_float2(F16Traits<T>::lo(g[p][j]), F16Traits<T>::hi(g[p][j])), r2);
+      const float2 v1 = fmul2_rn(make_float2(F16Traits<T>::lo(g[p][j + 1]), F16Traits<T>::hi(g[p][j + 1])), r2);
       word[j >> 1] = pack4_s8_rne(v0.x, v0.y, v1.x, v1.y);
     }
     if (col_ok && row < m) *reinterpret_cast<uint2*>(q + row * k + col) = make_uint2(word[0], word[1]);
@@ -151,7 +151,7 @@ static int quant_impl(const void* x, int x_dtype, int64_t m, int64_t k, int8_t* 
   if (k % 8 != 0) return fail(TDB200_ERR_UNSUPPORTED, "quant_int8_block128: k=%lld must be a multiple of 8", (long long)k);
   if (!aligned16(x) || (reinterpret_cast<uintptr_t>(q) & 7u))
     return fail(TDB200_ERR_INVALID_ARG, "quant_int8_block128: x must be 16-byte and q 8-byte aligned");
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
   const int64_t kb = cdiv64(k, kBlk), mb = cdiv64(m, kBlk);
   if (mb > 65535) return fail(TDB200_ERR_UNSUPPORTED, "quant_int8_block128: m too large (%lld)", (long long)m);
   dim3 grid(static_cast<unsigned>(kb), static_cast<unsigned>(mb));

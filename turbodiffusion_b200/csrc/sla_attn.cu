@@ -1,23 +1,23 @@
 // a9 + a10. Fused SageSLA attention forward for one (128-row query block, head, batch) per CTA:
-//   block-sparse INT8 Q.K^T -> online softmax (exp2) -> bf16 P.V, then the linear branch phi(Q).KVW / (eps + phi(Q).ksum)
-//   and the merge, all in one tcgen05 kernel.
+//   block-sparse INT8 Q.K^T -> online softmax (exp2) -> 16-bit P.V, then the linear branch phi(Q).KVW / (eps + phi(Q).ksum)
+//   folded into the same accumulator, all in one wgmma kernel.
 //   reference: Sage call site turbodiffusion/SLA/core.py:231-235 (arithmetic in third-party SpargeAttn, unpinned);
 //   the in-tree statement of the same attention is the Triton kernel SLA/kernel.py:33-82 (tail masking :57-62, exp2 with
 //   qk_scale*log2e :60, row sum from unrounded P :71, P cast before P.V :73); linear branch + merge SLA/core.py:243-253.
 //
-// CTA = 6 warps.  warps 0-3: softmax, thread == query row == TMEM lane.  warp 4: TMA producer.  warp 5: MMA issuer.
-//   S[2]  TMEM cols [0,128)   int32 128x64 per buffer (double-buffered so Q.K^T of block j+1 overlaps softmax of j)
-//   O     TMEM cols [128,256) fp32 128x128, accumulated by the tensor core across all selected key blocks
-//   After the loop the S columns are reused for the linear-branch product.
-// shared memory (104 KB + LUT, two CTAs per SM): Q int8 16 KB | K int8 3x8 KB | V bf16 3x16 KB | P bf16 16 KB.
-//   K and V travel in separate 3-deep TMA rings (K freed right after Q.K^T, V after P.V): the gathered key blocks
-//   are latency-bound L2/HBM reads, so the prefetch distance matters more than anything else.
-//   Q/K/P (and phi(Q), KVW) are K-major 128B-swizzled; V is consumed MN-major straight from its [L, D] rows, so no
-//   transposed/quantised copy of V is ever materialised.
+// CTA = 2 consumer warpgroups + 1 TMA warp.  Warpgroup g owns query rows [64g, 64g+64) of the block; every thread holds two
+//   rows of the fragments (common.cuh): S[64 x 64] in 32 registers (wgmma m64n64, A = Q and B = K from shared memory),
+//   P converted in registers straight into the A fragments of P.V (wgmma m64nHD, A from registers, B = V MN-major from
+//   shared memory, so no transposed copy of V is ever materialised), and the O accumulator [64 x HD] in HD/2 registers.
+//   Row maxima / sums are reduced across the four lanes that share a row.
+//   After the last key block the linear branch adds A.KVW^T to O with A = phi(q) * l / den in registers, so that
+//   O / l = softmax part + phi(q).KVW^T / den, and out = O / l + proj_b.
+// Shared memory: Q | K ring | V ring (3 stages each; K and V released per warp as soon as their MMA retired) | KVW.
+//   Q/K/KVW are K-major swizzled (128B rows, or 64B rows for 64-wide int8 heads).
 // The O accumulator is only rescaled when a row maximum grows by more than 2^8 (lazy rescale): P stays <= 256, which
 // bf16/fp32 hold exactly as well as P <= 1, and the final O / l normalisation is unchanged.
-#include <stdlib.h>
-
+// Entry points: tdb200_sla_attn_fwd (INT8 Q/K, head-major K), _kseq (INT8 K in [b, lk, h, d]), _qk16 (16-bit Q/K read from
+// the module layout [b, l, h, d], fp32 scores) and _v2 (INT8, head dims 64 and 128, feature maps of the linear branch).
 #include <type_traits>
 
 #include "common.cuh"
@@ -26,42 +26,26 @@
 namespace {
 using namespace tdb;
 
-constexpr int D = 128;
 constexpr int BLKQ = 128, BLKK = 64;
-constexpr int kThreads = 192;
-constexpr int kSoftmaxWarps = 4, kTmaWarp = 4, kMmaWarp = 5;
-constexpr uint32_t kVBytes = BLKK * D * 2;        // 16 KB (two 64-column blocks of 8 KB)
-constexpr uint32_t kPBytes = BLKQ * BLKK * 2;     // 16 KB
-constexpr uint32_t kBarBytes = 256;
-// kQK16 = false: Sage path, INT8 Q/K tiles (a9).  kQK16 = true: the non-quantised SLA path (a9', SLA/kernel.py:33-82): Q and K
-// are consumed as 16-bit tiles straight from the module layout [B,L,H,D] (two 64-column K-major chunks each), Q.K^T is a
-// kind::f16 MMA into fp32 scores.  The 16-bit tiles are twice as large, so that variant runs two-stage rings.
-template <bool kQK16>
+constexpr int kConsumerWarps = 8;
+constexpr int kThreads = kConsumerWarps * 32 + 32;
+constexpr int kStages = 3;
+constexpr float kLog2e = 1.4426950408889634f;
+constexpr float kRescaleThreshold = 8.0f;  // log2 domain
+
+template <int HD, bool kQK16>
 struct Lay {
-  static constexpr int kStages = kQK16 ? 2 : 3;     // K and V rings (separate: K is released after Q.K^T, V after P.V)
-  static constexpr uint32_t kQBytes = kQK16 ? BLKQ * D * 2 : BLKQ * D;   // 32 KB | 16 KB
-  static constexpr uint32_t kKBytes = kQK16 ? BLKK * D * 2 : BLKK * D;   // 16 KB |  8 KB
+  static constexpr uint32_t kQBytes = kQK16 ? BLKQ * HD * 2 : BLKQ * HD;   // 16-bit: HD/64 chunks of [128 rows x 128 B]
+  static constexpr uint32_t kKBytes = kQK16 ? BLKK * HD * 2 : BLKK * HD;
+  static constexpr uint32_t kVBytes = BLKK * HD * 2;                       // HD/64 boxes of [64 keys x 128 B]
+  static constexpr uint32_t kWBytes = HD * HD * 2;                         // HD/64 d_k chunks of [HD rows x 128 B]
   static constexpr uint32_t kOffQ = 0;
   static constexpr uint32_t kOffK = kOffQ + kQBytes;
   static constexpr uint32_t kOffV = kOffK + kStages * kKBytes;
-  static constexpr uint32_t kOffP = kOffV + kStages * kVBytes;
-  static constexpr uint32_t kOffBars = kOffP + kPBytes;      // 104 KB | 112 KB
-  static constexpr uint32_t kOffLut = kOffBars + kBarBytes;
+  static constexpr uint32_t kOffW = kOffV + kStages * kVBytes;
+  static constexpr uint32_t kOffBars = kOffW + kWBytes;
+  static constexpr uint32_t kOffLut = kOffBars + 256;
 };
-constexpr uint32_t kTmemCols = 256;
-constexpr uint32_t kColS = 0, kColO = 128;
-constexpr float kLog2e = 1.4426950408889634f;
-constexpr float kRescaleThreshold = 8.0f;         // log2 domain
-
-// Optional phase trace (diagnostics): when set through tdb200_debug_set_attn_trace(), lane 0 of softmax warp 0 of CTAs
-// (x == 1, y == 0, z == 0) and (x == 3, ...) records clock64() at the phase boundaries of its first 64 iterations:
-// trace[slot][j][0..6] = loop top, S ready, S in registers, max/vote done, exps done, P buffer free, P published;
-// [7] = S(j+1) ready and its tcgen05.ld issued (between 4 and 5).
-__device__ long long* g_attn_trace = nullptr;
-#define TDB_TRACE(slot_ok, j, k)                                                       \
-  do {                                                                                 \
-    if ((slot_ok) && (j) < 64) trace_base[(j) * 8 + (k)] = clock64();                  \
-  } while (0)
 
 struct AttnParams {
   const float* q_scale;   // [b,h,mblk]
@@ -71,31 +55,38 @@ struct AttnParams {
   const float* ksum;      // [b,h,d]
   const float* proj_b;    // [d]
   void* out;              // [b,l,h,d] T
-  int l, lk, h, mblk, nblk, topk;
+  int l, lk, h, mblk, nblk, topk, feature;  // feature: 0 softmax, 1 elu+1, 2 relu (SLA/core.py:57-73)
   float sm_scale;
 };
 
-enum Bar {
-  kBarQFull = 0, kBarKFull = 1 /*3*/, kBarKEmpty = 4 /*3*/, kBarVFull = 7 /*3*/, kBarVEmpty = 10 /*3*/,
-  kBarSFull = 13 /*2*/, kBarSEmpty = 15 /*2*/, kBarPFull = 17, kBarPEmpty = 18, kBarPvDone = 19, kBarKvwFull = 20,
-  kBarPhiFull = 21, kBarOlFull = 22, kNumBars = 23
-};
+enum Bar { kQFull = 0, kKFull = 1 /*3*/, kKEmpty = 4 /*3*/, kVFull = 7 /*3*/, kVEmpty = 10 /*3*/, kNumBars = 13 };
 
-template <typename T, bool kQK16>
-__global__ void __launch_bounds__(kThreads, 2)
-sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q8, const __grid_constant__ CUtensorMap tmap_k8,
-                    const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw,
-                    const __grid_constant__ CUtensorMap tmap_out, AttnParams p) {
-  using L = Lay<kQK16>;
-  constexpr int kStages = L::kStages;
-  constexpr uint32_t kOffQ8 = L::kOffQ, kOffK8 = L::kOffK, kOffV = L::kOffV, kOffP = L::kOffP, kOffBars = L::kOffBars, kOffLut = L::kOffLut;
-  constexpr uint32_t kQ8Bytes = L::kQBytes, kK8Bytes = L::kKBytes;
+__device__ __forceinline__ float feat(float x, float off_log2, int feature) {
+  // softmax numerator exp(x - max) | elu(x)+1 | relu(x)
+  if (feature == 0) return fast_exp2(fmaf(x, kLog2e, -off_log2));
+  if (feature == 1) return x > 0.f ? x + 1.0f : fast_exp2(x * kLog2e);
+  return fmaxf(x, 0.f);
+}
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+template <typename T, int HD, bool kQK16>
+__global__ void __launch_bounds__(kThreads, 1)
+sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                    const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw, AttnParams p) {
+  using L = Lay<HD, kQK16>;
+  constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // 1024-aligned, stays a shared-space pointer
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + kNumBars);
-  uint16_t* s_lut = reinterpret_cast<uint16_t*>(smem + kOffLut);                 // [topk] key-block ids
-  float* s_ksc = reinterpret_cast<float*>(smem + kOffLut + ((p.topk * 2 + 15) & ~15));  // [topk] k_scale of those blocks
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kOffBars);
+  uint16_t* s_lut = reinterpret_cast<uint16_t*>(smem + L::kOffLut);                 // [topk] key-block ids
+  float* s_ksc = reinterpret_cast<float*>(smem + L::kOffLut + ((p.topk * 2 + 15) & ~15));  // [topk] k_scale of those blocks
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
@@ -103,26 +94,15 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q8, const __grid_co
   const int T_blocks = p.topk;
 
   if (threadIdx.x == 0) {
-    mbar_init(&bars[kBarQFull], 1);
+    mbar_init(&bars[kQFull], 1);
     for (int i = 0; i < kStages; ++i) {
-      mbar_init(&bars[kBarKFull + i], 1);
-      mbar_init(&bars[kBarKEmpty + i], 1);
-      mbar_init(&bars[kBarVFull + i], 1);
-      mbar_init(&bars[kBarVEmpty + i], 1);
+      mbar_init(&bars[kKFull + i], 1);
+      mbar_init(&bars[kKEmpty + i], kConsumerWarps);
+      mbar_init(&bars[kVFull + i], 1);
+      mbar_init(&bars[kVEmpty + i], kConsumerWarps);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bars[kBarSFull + i], 1);
-      mbar_init(&bars[kBarSEmpty + i], kSoftmaxWarps);
-    }
-    mbar_init(&bars[kBarPFull], kSoftmaxWarps);
-    mbar_init(&bars[kBarPEmpty], 1);
-    mbar_init(&bars[kBarPvDone], 1);
-    mbar_init(&bars[kBarKvwFull], 1);
-    mbar_init(&bars[kBarPhiFull], kSoftmaxWarps);
-    mbar_init(&bars[kBarOlFull], 1);
     mbar_fence_init();
   }
-  if (warp == kMmaWarp) tmem_alloc<kTmemCols>(tmem_slot);
   {
     const int32_t* lut_row = p.lut + (int64_t(bh) * p.mblk + m_blk) * p.topk;
     const float* ksc_row = p.k_scale + int64_t(bh) * p.nblk;
@@ -132,427 +112,261 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q8, const __grid_co
       s_ksc[i] = kQK16 ? 1.0f : __ldg(ksc_row + blk);
     }
   }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == kTmaWarp) {
+  if (warp == kConsumerWarps) {
     // =============================================================== TMA producer
     if (lane == 0) {
-      tma_prefetch_desc(&tmap_q8);
-      tma_prefetch_desc(&tmap_k8);
+      tma_prefetch_desc(&tmap_q);
+      tma_prefetch_desc(&tmap_k);
       tma_prefetch_desc(&tmap_v);
       tma_prefetch_desc(&tmap_kvw);
-      tma_prefetch_desc(&tmap_out);
-      mbar_expect_tx(&bars[kBarQFull], kQ8Bytes);
-      if constexpr (kQK16) {  // 16-bit Q rows from [B,L,H,D]: two 64-column chunks of 128 rows x 128 B
-        tma_load_4d(smem + kOffQ8, &tmap_q8, &bars[kBarQFull], 0, hh, m_blk * BLKQ, b);
-        tma_load_4d(smem + kOffQ8 + kQ8Bytes / 2, &tmap_q8, &bars[kBarQFull], 64, hh, m_blk * BLKQ, b);
+      mbar_expect_tx(&bars[kQFull], L::kQBytes + L::kWBytes);
+      if constexpr (kQK16) {  // 16-bit Q rows from [B,L,H,D]: HD/64 chunks of 128 rows x 128 B
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c)
+          tma_load_4d(smem + L::kOffQ + c * (BLKQ * 128), &tmap_q, &bars[kQFull], c * 64, hh, m_blk * BLKQ, b);
       } else {
-        tma_load_4d(smem + kOffQ8, &tmap_q8, &bars[kBarQFull], 0, m_blk * BLKQ, bh, 0);
+        tma_load_4d(smem + L::kOffQ, &tmap_q, &bars[kQFull], 0, m_blk * BLKQ, bh, 0);
       }
+#pragma unroll
+      for (int c = 0; c < HD / 64; ++c)  // KVW: d_k chunk c of the [d_out, d_k] matrix of this head
+        tma_load_4d(smem + L::kOffW + c * (HD * 128), &tmap_kvw, &bars[kQFull], c * 64, 0, bh, 0);
       for (int j = 0; j < T_blocks; ++j) {
         const int st = j % kStages;
         const uint32_t ph = ((j / kStages) & 1) ^ 1;
         const int blk = s_lut[j];
-        mbar_wait(&bars[kBarKEmpty + st], ph);
-        mbar_expect_tx(&bars[kBarKFull + st], kK8Bytes);
-        if constexpr (kQK16) {
-          tma_load_4d(smem + kOffK8 + st * kK8Bytes, &tmap_k8, &bars[kBarKFull + st], 0, hh, blk * BLKK, b);
-          tma_load_4d(smem + kOffK8 + st * kK8Bytes + kK8Bytes / 2, &tmap_k8, &bars[kBarKFull + st], 64, hh, blk * BLKK, b);
-        } else {
-          tma_load_4d(smem + kOffK8 + st * kK8Bytes, &tmap_k8, &bars[kBarKFull + st], 0, blk * BLKK, hh, b);
-        }
-        mbar_wait(&bars[kBarVEmpty + st], ph);
-        mbar_expect_tx(&bars[kBarVFull + st], kVBytes);
-        uint8_t* sv = smem + kOffV + st * kVBytes;
-        tma_load_4d(sv, &tmap_v, &bars[kBarVFull + st], 0, hh, blk * BLKK, b);
-        tma_load_4d(sv + kVBytes / 2, &tmap_v, &bars[kBarVFull + st], 64, hh, blk * BLKK, b);
-      }
-      // KVW (2 x 16 KB K-chunks of the folded moment matrix) goes into the two V stages the LAST key block does not use:
-      // they are released one and two iterations before the loop ends, so this load's latency hides behind the tail.
-      mbar_expect_tx(&bars[kBarKvwFull], 2 * kVBytes);
-      for (int c = 0; c < 2; ++c) {
-        const int st = (T_blocks + c) % kStages;
-        const int uses = (T_blocks - st + kStages - 1) / kStages;
-        if (uses > 0) mbar_wait(&bars[kBarVEmpty + st], (uses - 1) & 1);
-        tma_load_4d(smem + kOffV + st * kVBytes, &tmap_kvw, &bars[kBarKvwFull], c * 64, 0, bh, 0);  // d_k chunk c
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    // =============================================================== MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc_qk = make_idesc(kDFmtS32, kFmtS8, kFmtS8, 0, 0, BLKQ, BLKK);
-      constexpr uint32_t f16fmt = std::is_same<T, __nv_bfloat16>::value ? kFmtBF16 : kFmtF16;
-      constexpr uint32_t idesc_qk16 = make_idesc(kDFmtF32, f16fmt, f16fmt, 0, 0, BLKQ, BLKK);
-      constexpr uint32_t idesc_pv = make_idesc(kDFmtF32, kFmtBF16, kFmtBF16, 0, 1, BLKQ, D);
-      constexpr uint32_t idesc_lin = make_idesc(kDFmtF32, kFmtBF16, kFmtBF16, 0, 0, BLKQ, D);
-      constexpr uint32_t idesc_pv16 = make_idesc(kDFmtF32, kFmtF16, kFmtF16, 0, 1, BLKQ, D);
-      constexpr uint32_t idesc_lin16 = make_idesc(kDFmtF32, kFmtF16, kFmtF16, 0, 0, BLKQ, D);
-      constexpr bool is_bf16 = sizeof(T) == 2 && std::is_same<T, __nv_bfloat16>::value;
-      const uint32_t id_pv = is_bf16 ? idesc_pv : idesc_pv16;
-      const uint32_t id_lin = is_bf16 ? idesc_lin : idesc_lin16;
-      const uint32_t sbase = smem_u32(smem);
-      const uint64_t qdesc = make_desc_kmajor_sw128(sbase + kOffQ8);
-
-      auto issue_pv = [&](int i) {
-        const int st = i % kStages;
-        mbar_wait(&bars[kBarPFull], i & 1);
-        mbar_wait(&bars[kBarVFull + st], (i / kStages) & 1);
-        tc_fence_after_sync();
-        const uint64_t vdesc = make_desc_mnmajor_sw128(sbase + kOffV + st * kVBytes, kVBytes / 2);
-#pragma unroll
-        for (int ks = 0; ks < BLKK / 16; ++ks)  // K=16 keys per MMA: P +8 TMEM columns, V +16 rows (2048 B)
-          umma_f16_ts(tmem_base + kColO, tmem_base + kColS + uint32_t(i & 1) * BLKK + uint32_t(ks * 8),
-                      vdesc + uint64_t(ks * 128), id_pv, (i > 0 || ks > 0) ? 1u : 0u);
-        umma_commit(&bars[kBarVEmpty + st]);
-        umma_commit(&bars[kBarPEmpty]);
-        umma_commit(&bars[kBarPvDone]);
-      };
-
-      mbar_wait(&bars[kBarQFull], 0);
-      for (int j = 0; j < T_blocks; ++j) {
-        const int st = j % kStages, sb = j & 1;
-        mbar_wait(&bars[kBarKFull + st], (j / kStages) & 1);
-        mbar_wait(&bars[kBarSEmpty + sb], ((j >> 1) & 1) ^ 1);
-        tc_fence_after_sync();
-        const uint64_t kdesc = make_desc_kmajor_sw128(sbase + kOffK8 + st * kK8Bytes);
+        mbar_wait(&bars[kKEmpty + st], ph);
+        mbar_expect_tx(&bars[kKFull + st], L::kKBytes);
+        uint8_t* sk = smem + L::kOffK + st * L::kKBytes;
         if constexpr (kQK16) {
 #pragma unroll
-          for (int ks = 0; ks < D / 16; ++ks) {  // K = 16 elements per MMA: chunk ks/4, +32 bytes per step inside the chunk
-            const uint64_t qd = make_desc_kmajor_sw128(sbase + kOffQ8 + (ks >> 2) * (kQ8Bytes / 2)) + uint64_t((ks & 3) * 2);
-            const uint64_t kd = make_desc_kmajor_sw128(sbase + kOffK8 + st * kK8Bytes + (ks >> 2) * (kK8Bytes / 2)) + uint64_t((ks & 3) * 2);
-            umma_f16_ss(tmem_base + kColS + sb * BLKK, qd, kd, idesc_qk16, ks > 0 ? 1u : 0u);
-          }
+          for (int c = 0; c < HD / 64; ++c)
+            tma_load_4d(sk + c * (BLKK * 128), &tmap_k, &bars[kKFull + st], c * 64, hh, blk * BLKK, b);
         } else {
-#pragma unroll
-          for (int ks = 0; ks < D / 32; ++ks)
-            umma_i8_ss(tmem_base + kColS + sb * BLKK, qdesc + uint64_t(ks * 2), kdesc + uint64_t(ks * 2), idesc_qk,
-                       ks > 0 ? 1u : 0u);
+          tma_load_4d(sk, &tmap_k, &bars[kKFull + st], 0, blk * BLKK, hh, b);
         }
-        umma_commit(&bars[kBarSFull + sb]);
-        umma_commit(&bars[kBarKEmpty + st]);
-        if (j > 0) issue_pv(j - 1);
-      }
-      issue_pv(T_blocks - 1);
-
-      // ---- linear branch, folded into the P.V accumulator:  O += A[128 x 128] . KVW^T  with  A = phi(q) * l / den  (so that
-      //      O / l afterwards equals  softmax-part + phi(q).KVW^T / den)
-      mbar_wait(&bars[kBarPhiFull], 0);
-      mbar_wait(&bars[kBarKvwFull], 0);
-      tc_fence_after_sync();
+        mbar_wait(&bars[kVEmpty + st], ph);
+        mbar_expect_tx(&bars[kVFull + st], L::kVBytes);
+        uint8_t* sv = smem + L::kOffV + st * L::kVBytes;
 #pragma unroll
-      for (int ks = 0; ks < D / 16; ++ks) {
-        // 64-wide K chunk (A: chunk 0 in the P buffer, chunk 1 in the freed Q tile; KVW: the two V stages the last
-        // key block did not use), +32 B per K=16 step
-        const uint64_t adesc = make_desc_kmajor_sw128(sbase + ((ks >> 2) ? kOffQ8 : kOffP) + (ks & 3) * 32);
-        const uint64_t bdesc =
-            make_desc_kmajor_sw128(sbase + kOffV + ((T_blocks + (ks >> 2)) % kStages) * kVBytes + (ks & 3) * 32);
-        umma_f16_ss(tmem_base + kColO, adesc, bdesc, id_lin, 1u);
+        for (int c = 0; c < HD / 64; ++c)
+          tma_load_4d(sv + c * (BLKK * 128), &tmap_v, &bars[kVFull + st], c * 64, hh, blk * BLKK, b);
       }
-      umma_commit(&bars[kBarOlFull]);
     }
-  } else {
-    // =============================================================== softmax / correction / epilogue warps
-    const int r = warp * 32 + lane;                     // query row inside the block == TMEM lane
-    const uint32_t lane_addr = uint32_t(warp * 32) << 16;
-    const int64_t q_row = int64_t(m_blk) * BLKQ + r;
-    // INT8 path: S holds int32 dot products; as_float(s + kMagicI) == kMagicF + s exactly, folded into the exponent's bias.
-    // 16-bit path: S already holds fp32 scores: the same expressions with a zero magic constant.
-    const float qsc = (kQK16 ? 1.0f : __ldg(p.q_scale + int64_t(bh) * p.mblk + m_blk)) * p.sm_scale * kLog2e;
-    constexpr float kMagicF = kQK16 ? 0.0f : 12582912.0f;   // 1.5 * 2^23: as_float(0x4B400000 + i) == kMagicF + i for |i| < 2^22
-    constexpr int kMagicI = kQK16 ? 0 : 0x4B400000;
-    constexpr uint32_t kMasked = kQK16 ? 0xFF800000u : 0x80000000u;   // -inf | INT_MIN
-    uint8_t* const sP = smem + kOffP;
-    {  // the row of q this thread needs for the linear branch after the loop: start moving it towards L2 now
-      const T* qrow = static_cast<const T*>(p.q) + ((int64_t(b) * p.l + (q_row < p.l ? q_row : p.l - 1)) * p.h + hh) * D;
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(qrow));
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(qrow + 64));
+    return;
+  }
+
+  // =============================================================== consumer warpgroups
+  const int wg = warp >> 2, w4 = warp & 3;
+  const int r_lo = wg * 64 + w4 * 16 + (lane >> 2);   // rows r_lo and r_lo + 8 of the block (fragment layout, common.cuh)
+  const int cq = 2 * (lane & 3);                       // column pair offset inside every 8-column slice
+  const uint32_t sbase = smem_u32(smem);
+  // INT8 path: scores are int32 dot products scaled by q_scale * k_scale; 16-bit path: fp32 scores.  Both in the log2 domain.
+  const float qsc = (kQK16 ? 1.0f : __ldg(p.q_scale + int64_t(bh) * p.mblk + m_blk)) * p.sm_scale * kLog2e;
+
+  float o[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+  float m_used[2] = {-INFINITY, -INFINITY}, l_part[2] = {0.f, 0.f};  // l_part: this thread's columns of the row sum
+
+  mbar_wait(&bars[kQFull], 0);
+  for (int j = 0; j < T_blocks; ++j) {
+    const int st = j % kStages;
+    const uint32_t ph = (j / kStages) & 1;
+    const int blk = s_lut[j];
+    const float sc = qsc * s_ksc[j];
+    const int valid = p.lk - blk * BLKK;                // < 64 only in the ragged last key block
+
+    // ---- S = Q.K^T for this warpgroup's 64 rows
+    float s[32];
+    mbar_wait(&bars[kKFull + st], ph);
+    const uint32_t sk = sbase + L::kOffK + st * L::kKBytes;
+    if constexpr (kQK16) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) s[i] = 0.f;
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < HD / 16; ++ks) {  // K = 16 elements per MMA: chunk ks/4, +32 bytes per step inside the chunk
+        const uint64_t qd = make_desc_kmajor_sw128(sbase + L::kOffQ + (ks >> 2) * (BLKQ * 128) + wg * (64 * 128)) + uint64_t((ks & 3) * 2);
+        const uint64_t kd = make_desc_kmajor_sw128(sk + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
+        wgmma_f16_ss<64, kBF16>(s, qd, kd, ks > 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(s);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) s[i] *= sc;
+    } else {
+      uint32_t si[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) si[i] = 0u;
+      // int8 rows are HD bytes: 128-byte swizzle for 128-wide heads, 64-byte swizzle for 64-wide heads
+      const uint32_t qa = sbase + L::kOffQ + wg * (64 * HD);
+      const uint64_t qdesc = HD == 128 ? make_desc_kmajor_sw128(qa) : make_desc_kmajor_sw64(qa);
+      const uint64_t kdesc = HD == 128 ? make_desc_kmajor_sw128(sk) : make_desc_kmajor_sw64(sk);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < HD / 32; ++ks)
+        wgmma_i8_ss<64>(si, qdesc + uint64_t(ks * 2), kdesc + uint64_t(ks * 2), ks > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(si);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) s[i] = static_cast<float>(static_cast<int>(si[i])) * sc;
     }
-
-    long long* trace_base = nullptr;
-    const bool tracing = g_attn_trace != nullptr && warp == 0 && lane == 0 && hh == 0 && b == 0 && (m_blk == 1 || m_blk == 3);
-    if (tracing) trace_base = g_attn_trace + (m_blk == 1 ? 0 : 64 * 8);
-    if (tracing) trace_base[62 * 8 + 0] = clock64();   // row 62: tile-level marks (0 entry, 1 first S, 2 loop exit, 3 phi, 4 OL, 5 stores)
-    float m_used = -INFINITY, l_sum = 0.f;
-    // The S tile of block j+1 is pulled out of TMEM while P(j) is being published (Q.K^T runs one block ahead), so the
-    // tcgen05.ld latency no longer sits in front of the row max.
-    uint32_t s0[32], s1[32];
-    mbar_wait(&bars[kBarSFull + 0], 0);
-    tc_fence_after_sync();
-    tmem_ld_x32(tmem_base + lane_addr + kColS, s0);
-    tmem_ld_x32(tmem_base + lane_addr + kColS + 32, s1);
-    if (tracing) trace_base[62 * 8 + 1] = clock64();
-    for (int j = 0; j < T_blocks; ++j) {
-      TDB_TRACE(tracing, j, 0);
-      const int st = j & 1;
-      const int blk = s_lut[j];
-      const float sc = qsc * s_ksc[j];
-      const int valid = p.lk - blk * BLKK;              // < 64 only in the ragged last key block
-      TDB_TRACE(tracing, j, 1);
-      tmem_ld_wait();
-      TDB_TRACE(tracing, j, 2);
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars[kBarSEmpty + st]);
-
-      // ---- row max on the raw int32 scores (sc > 0); the ragged last key block (valid < 64) first overwrites its
-      //      masked columns with INT_MIN so the hot path carries no per-element predicates
-      if (valid < BLKK) {
-#pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          if (c >= valid) s0[c] = kMasked;
-          if (c + 32 >= valid) s1[c] = kMasked;
-        }
-      }
-      // four independent max chains (depth 8 instead of 32: only two softmax warps share a scheduler, so serial
-      // dependency chains, not issue slots, were the limiter)
-      float m_blk_f;
-      if constexpr (kQK16) {
-        float fa = -INFINITY, fb = fa, fc = fa, fd = fa;
-#pragma unroll
-        for (int c = 0; c < 32; c += 4) {
-          fa = fmaxf(fa, fmaxf(__uint_as_float(s0[c]), __uint_as_float(s0[c + 1])));
-          fb = fmaxf(fb, fmaxf(__uint_as_float(s0[c + 2]), __uint_as_float(s0[c + 3])));
-          fc = fmaxf(fc, fmaxf(__uint_as_float(s1[c]), __uint_as_float(s1[c + 1])));
-          fd = fmaxf(fd, fmaxf(__uint_as_float(s1[c + 2]), __uint_as_float(s1[c + 3])));
-        }
-        m_blk_f = fmaxf(fmaxf(fa, fb), fmaxf(fc, fd)) * sc;
-      } else {
-        int mxa = -2147483647 - 1, mxb = mxa, mxc = mxa, mxd = mxa;
-#pragma unroll
-        for (int c = 0; c < 32; c += 4) {
-          mxa = __vimax3_s32(mxa, static_cast<int>(s0[c]), static_cast<int>(s0[c + 1]));
-          mxb = __vimax3_s32(mxb, static_cast<int>(s0[c + 2]), static_cast<int>(s0[c + 3]));
-          mxc = __vimax3_s32(mxc, static_cast<int>(s1[c]), static_cast<int>(s1[c + 1]));
-          mxd = __vimax3_s32(mxd, static_cast<int>(s1[c + 2]), static_cast<int>(s1[c + 3]));
-        }
-        const int mx = max(max(mxa, mxb), max(mxc, mxd));
-        m_blk_f = static_cast<float>(mx) * sc;
-      }
-
-      // ---- lazy rescale of the O accumulator (warp-uniform decision: tcgen05.ld/st are warp-collective)
-      const bool grow = m_blk_f > m_used + kRescaleThreshold;
-      if (j == 0) {
-        m_used = m_blk_f;
-      } else if (__any_sync(0xffffffffu, grow)) {
-        const float m_new = grow ? m_blk_f : m_used;
-        const float alpha = fast_exp2(m_used - m_new);
-        mbar_wait(&bars[kBarPvDone], (j - 1) & 1);      // P.V of block j-1 has retired; block j's is not issued yet
-        tc_fence_after_sync();
-        const uint32_t to = tmem_base + lane_addr + kColO;
-#pragma unroll
-        for (int c = 0; c < D / 32; ++c) {
-          uint32_t o[32];
-          tmem_ld_x32(to + c * 32, o);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-          tmem_st_x32(to + c * 32, o);
-        }
-        tmem_st_wait();
-        tc_fence_before_sync();
-        l_sum *= alpha;
-        m_used = m_new;
-      }
-
-      TDB_TRACE(tracing, j, 3);
-      // ---- P = exp2(s*sc - m_used); int->float via the magic-number add keeps the XU pipe free for ex2; the scale+bias
-      //      FMA and the row-sum adds run as packed f32x2 instructions.  Masked columns hold INT_MIN (a very negative
-      //      score); their exact removal happens in the ragged-block fix-up below.
-      const float cbias = -fmaf(kMagicF, sc, m_used);
-      const float2 sc2 = make_float2(sc, sc), cb2 = make_float2(cbias, cbias);
-      float2 psa = make_float2(0.f, 0.f), psb = psa, psc = psa, psd = psa;  // independent row-sum chains
-      uint32_t pw[32];
-#pragma unroll
-      for (int c = 0; c < 32; c += 4) {
-        float2 t0 = __ffma2_rn(make_float2(__int_as_float(static_cast<int>(s0[c]) + kMagicI),
-                                           __int_as_float(static_cast<int>(s0[c + 1]) + kMagicI)), sc2, cb2);
-        float2 t1 = __ffma2_rn(make_float2(__int_as_float(static_cast<int>(s0[c + 2]) + kMagicI),
-                                           __int_as_float(static_cast<int>(s0[c + 3]) + kMagicI)), sc2, cb2);
-        float2 t2 = __ffma2_rn(make_float2(__int_as_float(static_cast<int>(s1[c]) + kMagicI),
-                                           __int_as_float(static_cast<int>(s1[c + 1]) + kMagicI)), sc2, cb2);
-        float2 t3 = __ffma2_rn(make_float2(__int_as_float(static_cast<int>(s1[c + 2]) + kMagicI),
-                                           __int_as_float(static_cast<int>(s1[c + 3]) + kMagicI)), sc2, cb2);
-        t0.x = fast_exp2(t0.x); t0.y = fast_exp2(t0.y);
-        t1.x = fast_exp2(t1.x); t1.y = fast_exp2(t1.y);
-        t2.x = fast_exp2(t2.x); t2.y = fast_exp2(t2.y);
-        t3.x = fast_exp2(t3.x); t3.y = fast_exp2(t3.y);
-        psa = __fadd2_rn(psa, t0);
-        psb = __fadd2_rn(psb, t1);
-        psc = __fadd2_rn(psc, t2);
-        psd = __fadd2_rn(psd, t3);
-        pw[c >> 1] = F16Traits<T>::pack(t0.x, t0.y);
-        pw[(c >> 1) + 1] = F16Traits<T>::pack(t1.x, t1.y);
-        pw[16 + (c >> 1)] = F16Traits<T>::pack(t2.x, t2.y);
-        pw[17 + (c >> 1)] = F16Traits<T>::pack(t3.x, t3.y);
-      }
-      const float2 ps2 = __fadd2_rn(__fadd2_rn(psa, psb), __fadd2_rn(psc, psd));
-      float psum = ps2.x + ps2.y;
-      if (valid < BLKK) {
-        // exact fix-up of the ragged block: every masked column produced the same p (same INT_MIN input); remove it
-        // from the row sum and clear its 16-bit slot so the tensor core multiplies V's zero-filled rows by zero
-        const float pm = fast_exp2(fmaf(__int_as_float(static_cast<int>(kMasked) + kMagicI), sc, cbias));
-        psum -= static_cast<float>(BLKK - valid) * pm;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          if (2 * i >= valid) pw[i] = 0u;
-          else if (2 * i + 1 >= valid) pw[i] &= 0x0000FFFFu;
-        }
-      }
-      l_sum += psum;
-      TDB_TRACE(tracing, j, 4);
-      if (j + 1 < T_blocks) {  // prefetch S(j+1): s0/s1 are dead (P lives in pw)
-        mbar_wait(&bars[kBarSFull + (st ^ 1)], ((j + 1) >> 1) & 1);
-        tc_fence_after_sync();
-        const uint32_t tn = tmem_base + lane_addr + kColS + (st ^ 1) * BLKK;
-        tmem_ld_x32(tn, s0);
-        tmem_ld_x32(tn + 32, s1);
-      }
-      TDB_TRACE(tracing, j, 7);
-
-      // ---- P row -> tensor memory: 32 packed columns over the S buffer this block was read from.  The softmax warps may run
-      //      at most one P.V ahead of the tensor pipe (two ahead would alias the phase bit in the lazy-rescale wait above).
-      //      S(j+1) full - waited for just above - already implies that: its tcgen05.commit was issued after P.V(j-1)'s MMAs,
-      //      and a commit completes only when every earlier MMA of the issuing thread has.  Only the last block, which has no
-      //      next S tile, polls the P.V barrier itself (a poll costs ~65 clk even when the phase is long complete).
-      if (j + 1 >= T_blocks) mbar_wait(&bars[kBarPEmpty], (j & 1) ^ 1);
-      TDB_TRACE(tracing, j, 5);
-      tmem_st_x32(tmem_base + lane_addr + kColS + uint32_t(st) * BLKK, pw);
-      tmem_st_wait();
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars[kBarPFull]);
-      TDB_TRACE(tracing, j, 6);
-    }
-    if (tracing) trace_base[63 * 8 + 7] = clock64();  // loop exit
-    if (tracing) trace_base[62 * 8 + 2] = clock64();
-
-    // ---- linear branch operand (SLA/core.py:243): e_j = exp(q_j - max_j q), ONE exponential per element kept in fp32 registers,
-    //      E = sum e_j, F = sum e_j * ksum_j;  phi_j = e_j / E,  den = 1e-5 + sum_j phi_j ksum_j = 1e-5 + F / E;
-    //      the tensor core receives A_j = T(phi_j * l / den), so that O + A.KVW^T = l * (O/l + phi.KVW^T/den).
-    uint32_t aw[D / 2];
-    {
-      const T* qrow = static_cast<const T*>(p.q) + ((int64_t(b) * p.l + (q_row < p.l ? q_row : p.l - 1)) * p.h + hh) * D;
-      float qm0 = -INFINITY, qm1 = -INFINITY, qm2 = -INFINITY, qm3 = -INFINITY;
-#pragma unroll
-      for (int c = 0; c < D / 8; ++c) {
-        const uint4 raw = __ldg(reinterpret_cast<const uint4*>(qrow) + c);
-        aw[4 * c] = raw.x; aw[4 * c + 1] = raw.y; aw[4 * c + 2] = raw.z; aw[4 * c + 3] = raw.w;
-        qm0 = fmaxf(qm0, fmaxf(F16Traits<T>::lo(raw.x), F16Traits<T>::hi(raw.x)));
-        qm1 = fmaxf(qm1, fmaxf(F16Traits<T>::lo(raw.y), F16Traits<T>::hi(raw.y)));
-        qm2 = fmaxf(qm2, fmaxf(F16Traits<T>::lo(raw.z), F16Traits<T>::hi(raw.z)));
-        qm3 = fmaxf(qm3, fmaxf(F16Traits<T>::lo(raw.w), F16Traits<T>::hi(raw.w)));
-      }
-      const float qoff = fmaxf(fmaxf(qm0, qm1), fmaxf(qm2, qm3)) * kLog2e;
-      const float* ks = p.ksum + int64_t(bh) * D;
-      float e[D];
-      float e0 = 0.f, e1 = 0.f, e2 = 0.f, e3 = 0.f, f0 = 0.f, f1 = 0.f, f2 = 0.f, f3 = 0.f;  // independent chains
-#pragma unroll
-      for (int i = 0; i < D / 2; i += 2) {
-        const float4 k4 = __ldg(reinterpret_cast<const float4*>(ks + 2 * i));
-        e[2 * i] = fast_exp2(fmaf(F16Traits<T>::lo(aw[i]), kLog2e, -qoff));
-        e[2 * i + 1] = fast_exp2(fmaf(F16Traits<T>::hi(aw[i]), kLog2e, -qoff));
-        e[2 * i + 2] = fast_exp2(fmaf(F16Traits<T>::lo(aw[i + 1]), kLog2e, -qoff));
-        e[2 * i + 3] = fast_exp2(fmaf(F16Traits<T>::hi(aw[i + 1]), kLog2e, -qoff));
-        e0 += e[2 * i]; e1 += e[2 * i + 1]; e2 += e[2 * i + 2]; e3 += e[2 * i + 3];
-        f0 = fmaf(e[2 * i], k4.x, f0); f1 = fmaf(e[2 * i + 1], k4.y, f1);
-        f2 = fmaf(e[2 * i + 2], k4.z, f2); f3 = fmaf(e[2 * i + 3], k4.w, f3);
-      }
-      const float inv_e = 1.0f / ((e0 + e1) + (e2 + e3));
-      const float den = fmaf((f0 + f1) + (f2 + f3), inv_e, 1e-5f);
-      const float cscale = inv_e * l_sum / den;
-#pragma unroll
-      for (int i = 0; i < D / 2; ++i) aw[i] = F16Traits<T>::pack(e[2 * i] * cscale, e[2 * i + 1] * cscale);
-    }
-    // all MMAs retired -> the P buffer and the Q tile may be overwritten with A (two 64-wide K chunks of 16 KB)
-    mbar_wait(&bars[kBarPvDone], (T_blocks - 1) & 1);
-    tc_fence_after_sync();
-#pragma unroll
-    for (int c = 0; c < 16; ++c) {
-      uint8_t* dst = ((c >> 3) ? smem + kOffQ8 : sP) + r * 128 + (((c & 7) ^ (r & 7)) << 4);
-      *reinterpret_cast<uint4*>(dst) = make_uint4(aw[4 * c], aw[4 * c + 1], aw[4 * c + 2], aw[4 * c + 3]);
-    }
-    fence_proxy_async_smem();
     __syncwarp();
-    if (lane == 0) mbar_arrive(&bars[kBarPhiFull]);
-    if (tracing) trace_base[62 * 8 + 3] = clock64();
+    if (lane == 0) mbar_arrive(&bars[kKEmpty + st]);
 
-    // ---- out = T( O / l + proj_b ): the two staging buffers (P buffer: columns 0-63, Q tile: columns 64-127; both free once the
-    //      linear MMA has retired) hold 128 rows x 128 bytes each in the 128B-swizzled TMA layout and leave as two box stores
-    //      (rows >= l are clipped by the tensor map)
-    mbar_wait(&bars[kBarOlFull], 0);
-    tc_fence_after_sync();
-    if (tracing) trace_base[62 * 8 + 4] = clock64();
-    const float inv_l = 1.0f / l_sum;
+    // ---- ragged last key block: columns past lk do not exist
+    if (valid < BLKK) {
 #pragma unroll
-    for (int c = 0; c < D / 32; ++c) {
-      uint32_t o[32];
-      tmem_ld_x32(tmem_base + lane_addr + kColO + c * 32, o);
-      tmem_ld_wait();
-      const float4* pb4 = reinterpret_cast<const float4*>(p.proj_b + c * 32);
-      uint8_t* stg = ((c >> 1) ? smem + kOffQ8 : sP) + r * 128;
+      for (int i = 0; i < 32; ++i)
+        if (8 * (i >> 2) + cq + (i & 1) >= valid) s[i] = -INFINITY;
+    }
+    // ---- row maxima and the lazy rescale of the O accumulator (per row: alpha == 1 exactly where the maximum is kept)
 #pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const float4 b0 = __ldg(pb4 + 2 * g), b1 = __ldg(pb4 + 2 * g + 1);
-        uint4 w;
-        w.x = F16Traits<T>::pack(fmaf(__uint_as_float(o[g * 8 + 0]), inv_l, b0.x), fmaf(__uint_as_float(o[g * 8 + 1]), inv_l, b0.y));
-        w.y = F16Traits<T>::pack(fmaf(__uint_as_float(o[g * 8 + 2]), inv_l, b0.z), fmaf(__uint_as_float(o[g * 8 + 3]), inv_l, b0.w));
-        w.z = F16Traits<T>::pack(fmaf(__uint_as_float(o[g * 8 + 4]), inv_l, b1.x), fmaf(__uint_as_float(o[g * 8 + 5]), inv_l, b1.y));
-        w.w = F16Traits<T>::pack(fmaf(__uint_as_float(o[g * 8 + 6]), inv_l, b1.z), fmaf(__uint_as_float(o[g * 8 + 7]), inv_l, b1.w));
-        const int ch = (c & 1) * 4 + g;                      // 16-byte chunk inside the 128-byte half row
-        *reinterpret_cast<uint4*>(stg + ((ch ^ (r & 7)) << 4)) = w;
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if (((i >> 1) & 1) == h) mx = fmaxf(mx, s[i]);
+      mx = quad_max(mx);
+      if (j == 0) {
+        m_used[h] = mx;
+      } else if (mx > m_used[h] + kRescaleThreshold) {
+        const float alpha = fast_exp2(m_used[h] - mx);
+#pragma unroll
+        for (int i = 0; i < HD / 2; ++i)
+          if (((i >> 1) & 1) == h) o[i] *= alpha;
+        l_part[h] *= alpha;
+        m_used[h] = mx;
       }
     }
-    fence_proxy_async_smem();
-    named_bar_sync(1, kSoftmaxWarps * 32);                   // all 128 rows are staged
-    if (threadIdx.x == 0) {
-      tma_store_4d(&tmap_out, sP, 0, hh, m_blk * BLKQ, b);
-      tma_store_4d(&tmap_out, smem + kOffQ8, 64, hh, m_blk * BLKQ, b);
-      tma_store_commit();
-      tma_store_wait_read<0>();                              // shared memory must outlive the reads of the store engine
+    // ---- P = exp2(s - m_used); the row sum is taken from the unrounded P, the tensor core gets P rounded to T
+    uint32_t pa[BLKK / 16][4];
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int h = (i >> 1) & 1;
+      const float p0 = fast_exp2(s[i] - m_used[h]), p1 = fast_exp2(s[i + 1] - m_used[h]);
+      l_part[h] += p0 + p1;
+      pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0, p1);
     }
-    if (tracing) trace_base[62 * 8 + 5] = clock64();
-    tc_fence_before_sync();
-  }
 
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    tc_fence_after_sync();
-    tmem_dealloc<kTmemCols>(tmem_base);
+    // ---- O += P.V  (V: [64 keys x HD] rows, MN-major operand; +16 keys = +2048 B per K step)
+    mbar_wait(&bars[kVFull + st], ph);
+    const uint64_t vdesc = make_desc_mnmajor_sw128(sbase + L::kOffV + st * L::kVBytes, BLKK * 128);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BLKK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(o, pa[kk], vdesc + uint64_t(kk * 128));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+#pragma unroll
+    for (int kk = 0; kk < BLKK / 16; ++kk) reg_fence(pa[kk]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars[kVEmpty + st]);
+  }
+  const float l_tot[2] = {quad_sum(l_part[0]), quad_sum(l_part[1])};
+
+  // ---- linear branch operand (SLA/core.py:243).  f_j = feature map numerator of the query row:
+  //      E = sum f_j, F = sum f_j * ksum_j;  phi_j = f_j / E (softmax) or f_j;  den = 1e-5 + sum_j phi_j ksum_j;
+  //      A_j = T(phi_j * l / den), so that O + A.KVW^T = l * (O/l + phi.KVW^T/den).
+  //      This thread holds, for each K=16 step kk, the column pairs 16 kk + cq and 16 kk + 8 + cq of its two rows.
+  uint32_t qa[HD / 16][4];
+  const int64_t qrow0 = int64_t(m_blk) * BLKQ + r_lo;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t qr = qrow0 + 8 * h;
+    const T* qrow = static_cast<const T*>(p.q) + ((int64_t(b) * p.l + (qr < p.l ? qr : p.l - 1)) * p.h + hh) * HD;
+#pragma unroll
+    for (int kk = 0; kk < HD / 16; ++kk) {
+      qa[kk][h] = __ldg(reinterpret_cast<const unsigned int*>(qrow + 16 * kk + cq));
+      qa[kk][2 + h] = __ldg(reinterpret_cast<const unsigned int*>(qrow + 16 * kk + 8 + cq));
+    }
+  }
+  const float* ks = p.ksum + int64_t(bh) * HD;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float off = 0.f;
+    if (p.feature == 0) {
+      float qm = -INFINITY;
+#pragma unroll
+      for (int kk = 0; kk < HD / 16; ++kk)
+#pragma unroll
+        for (int u = 0; u < 2; ++u)
+          qm = fmaxf(qm, fmaxf(F16Traits<T>::lo(qa[kk][h + 2 * u]), F16Traits<T>::hi(qa[kk][h + 2 * u])));
+      off = quad_max(qm) * kLog2e;
+    }
+    float e = 0.f, f = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < HD / 16; ++kk)
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const uint32_t w = qa[kk][h + 2 * u];
+        const float2 k2 = __ldg(reinterpret_cast<const float2*>(ks + 16 * kk + 8 * u + cq));
+        const float a0 = feat(F16Traits<T>::lo(w), off, p.feature), a1 = feat(F16Traits<T>::hi(w), off, p.feature);
+        e += a0 + a1;
+        f = fmaf(a0, k2.x, fmaf(a1, k2.y, f));
+      }
+    const float E = quad_sum(e), F = quad_sum(f);
+    const float inv_e = p.feature == 0 ? 1.0f / E : 1.0f;
+    const float den = 1e-5f + F * inv_e;
+    const float cscale = inv_e * l_tot[h] / den;
+#pragma unroll
+    for (int kk = 0; kk < HD / 16; ++kk)
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const uint32_t w = qa[kk][h + 2 * u];
+        qa[kk][h + 2 * u] = F16Traits<T>::pack(feat(F16Traits<T>::lo(w), off, p.feature) * cscale,
+                                               feat(F16Traits<T>::hi(w), off, p.feature) * cscale);
+      }
+  }
+  // ---- O += A . KVW^T  (KVW: [d_out rows x d_k] K-major, d_k chunk kk/4, +32 bytes per K=16 step inside the chunk)
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < HD / 16; ++kk)
+    wgmma_f16_rs<HD, kBF16, 0>(o, qa[kk], make_desc_kmajor_sw128(sbase + L::kOffW + (kk >> 2) * (HD * 128)) + uint64_t((kk & 3) * 2));
+  wgmma_commit();
+  wgmma_wait<0>();
+  reg_fence(o);
+#pragma unroll
+  for (int kk = 0; kk < HD / 16; ++kk) reg_fence(qa[kk]);
+
+  // ---- out = T( O / l + proj_b )
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t qr = qrow0 + 8 * h;
+    if (qr >= p.l) continue;
+    const float inv_l = 1.0f / l_tot[h];
+    T* orow = static_cast<T*>(p.out) + ((int64_t(b) * p.l + qr) * p.h + hh) * HD;
+#pragma unroll
+    for (int c = 0; c < HD / 8; ++c) {
+      const float2 pb = __ldg(reinterpret_cast<const float2*>(p.proj_b + 8 * c + cq));
+      *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) =
+          F16Traits<T>::pack(fmaf(o[4 * c + 2 * h], inv_l, pb.x), fmaf(o[4 * c + 2 * h + 1], inv_l, pb.y));
+    }
   }
 }
 
-}  // namespace
-
-extern "C" int tdb200_debug_set_attn_trace(long long* trace_or_null) {
-  return tdb::check_cuda(cudaMemcpyToSymbol(g_attn_trace, &trace_or_null, sizeof(trace_or_null)), "cudaMemcpyToSymbol(g_attn_trace)");
-}
-
-template <bool kQK16>
-static int launch_v1(const void* q_op, const float* q_scale, const void* k_op, const float* k_scale, const void* v, const void* q,
-                     int dtype, const int32_t* lut, int64_t topk, const void* kvw, const float* ksum, const float* proj_b,
-                     void* out, int64_t b, int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream,
-                     bool k_seq_major = false) {
-  using namespace tdb;
-  using L = Lay<kQK16>;
-  if (!q_op || !k_op || !v || !q || !lut || !kvw || !ksum || !proj_b || !out || (!kQK16 && (!q_scale || !k_scale)))
-    return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: null pointer");
-  if (b <= 0 || l <= 0 || lk <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: bad shape");
-  if (d != D) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (this kernel implements d=128)", (long long)d);
-  if (k_seq_major && b != 1)
-    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_kseq: batch %lld (the gathered [lk_pad, h, d] key slab is one sequence)", (long long)b);
+// kQK16: 16-bit Q and K in [b, l, h, d]; otherwise INT8 Q [b*h, l, d] and INT8 K [b, h, lk, d] (or [b, lk, h, d] when k_seq_major)
+template <int HD, bool kQK16>
+int launch(const void* q_op, const float* q_scale, const void* k_op, const float* k_scale, const void* v, const void* q, int dtype,
+           const int32_t* lut, int64_t topk, const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
+           int64_t l, int64_t lk, int64_t h, float sm_scale, int feature, bool k_seq_major, void* stream) {
+  using L = Lay<HD, kQK16>;
+  const int64_t d = HD;
   const int64_t mblk = cdiv64(l, BLKQ), nblk = cdiv64(lk, BLKK);
   if (topk <= 0 || topk > nblk) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: topk=%lld outside [1, %lld]", (long long)topk, (long long)nblk);
-  if (nblk > 65535 || h > 65535 || b > 65535) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: dimension too large");
+  if (nblk > 65535 || h > 65535 || b > 65535 || mblk > 0x7FFFFFFF) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: dimension too large");
   const size_t lut_bytes = ((size_t(topk) * 2 + 15) & ~size_t(15)) + size_t(topk) * 4;
-  static const bool one_cta_per_sm = getenv("TDB200_ATTN_ONE_CTA_PER_SM") != nullptr;  // diagnostics: timeline without a sibling CTA
-  const size_t smem = 1024 + L::kOffLut + lut_bytes + ((one_cta_per_sm && !kQK16) ? 64 * 1024 : 0);
+  const size_t smem = 1024 + L::kOffLut + lut_bytes;
   if (smem > 227 * 1024) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: topk=%lld too large for on-chip LUT", (long long)topk);
-  if (int rc = require_sm100()) return rc;
+  if (dtype != TDB200_DTYPE_BF16 && dtype != TDB200_DTYPE_FP16) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: dtype tag %d", dtype);
+  if (int rc = require_sm90()) return rc;
 
   const CUtensorMapDataType t16 = dtype == TDB200_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const int sw8 = HD == 128 ? 128 : 64;
   CUtensorMap tq, tk, tv, tw;
   if (kQK16) {  // 16-bit Q / K rows in the module layout [b, l, h, d]
     const uint64_t dq[4] = {uint64_t(d), uint64_t(h), uint64_t(l), uint64_t(b)};
@@ -567,15 +381,15 @@ static int launch_v1(const void* q_op, const float* q_scale, const void* k_op, c
     {
       const uint64_t dims[4] = {uint64_t(d), uint64_t(l), uint64_t(b * h), 1};
       const uint64_t str[3] = {uint64_t(d), uint64_t(l * d), uint64_t(b * h * l * d)};
-      const uint32_t box[4] = {D, BLKQ, 1, 1};
-      if (int rc = make_tmap_4d(&tq, q_op, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, dims, str, box)) return rc;
+      const uint32_t box[4] = {uint32_t(HD), BLKQ, 1, 1};
+      if (int rc = make_tmap_4d(&tq, q_op, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, dims, str, box, sw8)) return rc;
     }
     {
       // INT8 K: head-major [b, h, lk, d] (tdb200_sla_quant_qk) or, for sequence-parallel callers, the gathered [b, lk, h, d]
       const uint64_t dims[4] = {uint64_t(d), uint64_t(lk), uint64_t(h), uint64_t(b)};
       const uint64_t str[3] = {uint64_t(k_seq_major ? h * d : d), uint64_t(k_seq_major ? d : lk * d), uint64_t(h * lk * d)};
-      const uint32_t box[4] = {D, BLKK, 1, 1};
-      if (int rc = make_tmap_4d(&tk, k_op, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, dims, str, box)) return rc;
+      const uint32_t box[4] = {uint32_t(HD), BLKK, 1, 1};
+      if (int rc = make_tmap_4d(&tk, k_op, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, dims, str, box, sw8)) return rc;
     }
   }
   {
@@ -587,15 +401,8 @@ static int launch_v1(const void* q_op, const float* q_scale, const void* k_op, c
   {
     const uint64_t dims[4] = {uint64_t(d), uint64_t(d), uint64_t(b * h), 1};
     const uint64_t str[3] = {uint64_t(d * 2), uint64_t(d * d * 2), uint64_t(b * h * d * d * 2)};
-    const uint32_t box[4] = {64, D, 1, 1};
+    const uint32_t box[4] = {64, uint32_t(HD), 1, 1};
     if (int rc = make_tmap_4d(&tw, kvw, t16, 2, dims, str, box)) return rc;
-  }
-  CUtensorMap to;
-  {  // output tile store: [b, l, h, d] T, one box = 128 rows x 64 columns of one head
-    const uint64_t dims[4] = {uint64_t(d), uint64_t(h), uint64_t(l), uint64_t(b)};
-    const uint64_t str[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(l * h * d * 2)};
-    const uint32_t box[4] = {64, 1, BLKQ, 1};
-    if (int rc = make_tmap_4d(&to, out, t16, 2, dims, str, box)) return rc;
   }
   AttnParams p;
   p.q_scale = q_scale;
@@ -611,28 +418,43 @@ static int launch_v1(const void* q_op, const float* q_scale, const void* k_op, c
   p.mblk = int(mblk);
   p.nblk = int(nblk);
   p.topk = int(topk);
+  p.feature = feature;
   p.sm_scale = sm_scale;
   dim3 grid(static_cast<unsigned>(mblk), static_cast<unsigned>(h), static_cast<unsigned>(b));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define TDB_ATTN(T)                                                                                                   \
   do {                                                                                                                \
-    if (int rc = check_cuda(cudaFuncSetAttribute(sla_attn_fwd_kernel<T, kQK16>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                                 static_cast<int>(smem)), "cudaFuncSetAttribute(sla_attn)"))        \
+    if (int rc = check_cuda(cudaFuncSetAttribute(sla_attn_fwd_kernel<T, HD, kQK16>,                                   \
+                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), \
+                            "cudaFuncSetAttribute(sla_attn)"))                                                        \
       return rc;                                                                                                      \
-    sla_attn_fwd_kernel<T, kQK16><<<grid, kThreads, smem, st>>>(tq, tk, tv, tw, to, p);                               \
+    sla_attn_fwd_kernel<T, HD, kQK16><<<grid, kThreads, smem, st>>>(tq, tk, tv, tw, p);                               \
     return check_launch("sla_attn_fwd_kernel");                                                                       \
   } while (0)
   if (dtype == TDB200_DTYPE_BF16) TDB_ATTN(__nv_bfloat16);
-  if (dtype == TDB200_DTYPE_FP16) TDB_ATTN(__half);
+  TDB_ATTN(__half);
 #undef TDB_ATTN
-  return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: dtype tag %d", dtype);
 }
+
+int check_common(const void* q_op, const void* k_op, const void* v, const void* q, const int32_t* lut, const void* kvw,
+                 const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk, int64_t h) {
+  if (!q_op || !k_op || !v || !q || !lut || !kvw || !ksum || !proj_b || !out)
+    return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: null pointer");
+  if (b <= 0 || l <= 0 || lk <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: bad shape");
+  return 0;
+}
+
+}  // namespace
 
 extern "C" int tdb200_sla_attn_fwd(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
                                    const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk,
                                    const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
                                    int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  return launch_v1<false>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, d, sm_scale, stream);
+  if (int rc = check_common(q_i8, k_i8, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
+  if (!q_scale || !k_scale) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: null pointer");
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (this kernel implements d=128)", (long long)d);
+  return launch<128, false>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, sm_scale, 0,
+                            false, stream);
 }
 
 // the same kernel reading INT8 K in the [b, lk, h, d] layout (tdb200_sla_quant_k_seq; what sequence-parallel ranks all-gather)
@@ -640,12 +462,36 @@ extern "C" int tdb200_sla_attn_fwd_kseq(const int8_t* q_i8, const float* q_scale
                                         const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk,
                                         const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
                                         int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  return launch_v1<false>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, d, sm_scale, stream,
-                          true);
+  if (int rc = check_common(q_i8, k_i8, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
+  if (!q_scale || !k_scale) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: null pointer");
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (this kernel implements d=128)", (long long)d);
+  if (b != 1)
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_kseq: batch %lld (the gathered [lk_pad, h, d] key slab is one sequence)", (long long)b);
+  return launch<128, false>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, sm_scale, 0,
+                            true, stream);
 }
 
 extern "C" int tdb200_sla_attn_fwd_qk16(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
                                         const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
                                         int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  return launch_v1<true>(q, nullptr, k, nullptr, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, d, sm_scale, stream);
+  if (int rc = check_common(q, k, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (this kernel implements d=128)", (long long)d);
+  return launch<128, true>(q, nullptr, k, nullptr, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, sm_scale, 0, false,
+                           stream);
+}
+
+extern "C" int tdb200_sla_attn_fwd_v2(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
+                                      const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk,
+                                      const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
+                                      int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, int feature,
+                                      void* stream) {
+  if (int rc = check_common(q_i8, k_i8, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
+  if (!q_scale || !k_scale) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: null pointer");
+  if (d != 64 && d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (64 or 128, SLA/core.py:207)", (long long)d);
+  if (feature < 0 || feature > 2) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: feature map tag %d", feature);
+  if (d == 128)
+    return launch<128, false>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, sm_scale,
+                              feature, false, stream);
+  return launch<64, false>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, sm_scale,
+                           feature, false, stream);
 }

@@ -120,7 +120,7 @@ extern "C" int tdb200_sla_block_map(const void* q_pool, const void* k_pool, int 
   const size_t smem = size_t(kRows) * d * 4 + size_t(kRows) * nblk * 2;
   if (smem > 200 * 1024) return fail(TDB200_ERR_UNSUPPORTED, "sla_block_map: nblk=%lld too large for the on-chip score rows", (long long)nblk);
   if (!aligned16(k_pool)) return fail(TDB200_ERR_INVALID_ARG, "sla_block_map: k_pool must be 16-byte aligned");
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   dim3 grid(static_cast<unsigned>(cdiv64(mblk, kRows)), static_cast<unsigned>(b * h));
 #define TDB_BM(T, D)                                                                                             \

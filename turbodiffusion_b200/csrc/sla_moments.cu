@@ -5,14 +5,14 @@
 // Both outputs are ACCUMULATED in fp32 with red.global.add (caller zeroes them), so sequence shards and the split-L
 // CTAs of one GPU combine by plain addition (and one all-reduce across GPUs).
 //
-// CTA = 6 warps, 128 key rows per tile.  warps 0-3: thread == key row: load the row, softmax over D (MUFU ex2), write
-// phi(k) into shared memory in the MN-major 128B-swizzled operand layout, then column-sum the tile for ksum.
-// warp 4: TMA loads of the V tile (consumed MN-major as the A operand: M = value channel).  warp 5: tcgen05.mma
-// kind::f16, D[128(dv) x 128(dk)] += V^T . phi(K), fp32 accumulator in TMEM across all tiles of this CTA.
-// 64-wide heads (SLA/core.py:207) run through the same 128x128 tile as PAIRS of adjacent heads: in the [L, H, 64] layout two
-// heads are 128 contiguous columns, i.e. exactly one 128-wide row of V and of K.  The tensor core then produces
-// [V_a | V_b]^T . [phi(K_a) | phi(K_b)]; its two diagonal 64x64 blocks are the two heads' moment matrices (the off-diagonal
-// blocks are discarded), so a pair costs what one 128-wide head costs.  phi is evaluated per 64-wide half.
+// CTA = 2 warpgroups, 128 key rows per tile.  Two threads per key row (each owns 64 of its 128 channels): load the row,
+// feature map (softmax over D with MUFU ex2), write phi(k) into shared memory in the MN-major 128B-swizzled operand layout;
+// thread 0 streams the V tiles in by TMA (3-stage ring).  Warpgroup g then issues wgmma (16-bit inputs, fp32 accumulator in
+// registers across all tiles of this CTA): D[64 (dv rows 64g..) x 128 (dk)] += V^T . phi(K), both operands MN-major, and
+// column-sums the tile for ksum while the MMAs run.
+// 64-wide heads (SLA/core.py:207) run through the same 128-row tile as PAIRS of adjacent heads: in the [L, H, 64] layout two
+// heads are 128 contiguous columns, i.e. exactly one 128-wide row of V and of K.  Warpgroup g computes only the diagonal
+// 64x64 block of head 2*pair+g (N = 64), and phi is evaluated per 64-wide half.
 // Feature maps (SLA/core.py:57-73): 0 softmax over the head dim, 1 elu(x)+1, 2 relu(x).
 #include <type_traits>
 
@@ -24,16 +24,15 @@ using namespace tdb;
 
 constexpr int D = 128;
 constexpr int kRowsPerTile = 128;
-constexpr int kThreads = 192;
+constexpr int kThreads = 256;
+constexpr int kVStages = 3;
 constexpr uint32_t kOperandBytes = kRowsPerTile * D * 2;  // 32 KB: two 64-channel blocks of 128 rows x 128 B
 constexpr uint32_t kBlockBytes = kOperandBytes / 2;       // 16 KB
-constexpr uint32_t kOffV = 0;                             // 2 stages
-constexpr uint32_t kOffPhi = 2 * kOperandBytes;           // 2 stages
-constexpr uint32_t kOffBars = 4 * kOperandBytes;          // 128 KB
+constexpr uint32_t kOffV = 0;                             // kVStages stages
+constexpr uint32_t kOffPhi = kVStages * kOperandBytes;
+constexpr uint32_t kOffBars = kOffPhi + kOperandBytes;    // 128 KB
 constexpr size_t kSmemBytes = 1024 + kOffBars + 128;
 constexpr float kLog2e = 1.4426950408889634f;
-
-enum Bar { kVFull = 0 /*2*/, kPhiFull = 2 /*2*/, kStageEmpty = 4 /*2*/, kAccFull = 6, kNumBars = 7 };
 
 struct MomParams {
   const void* k;
@@ -44,223 +43,174 @@ struct MomParams {
   int feature;   // 0 softmax, 1 elu+1, 2 relu
 };
 
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
 template <typename T, bool kPair>
 __global__ void __launch_bounds__(kThreads, 1)
 sla_moments_kernel(const __grid_constant__ CUtensorMap tmap_v, MomParams p) {
+  constexpr int N = kPair ? 64 : 128;          // key channels of this warpgroup's accumulator
+  constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // 1024-aligned, stays a shared-space pointer
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + kNumBars);
+  uint64_t* vfull = reinterpret_cast<uint64_t*>(smem + kOffBars);                 // [kVStages]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int hh = blockIdx.x, split = blockIdx.y, b = blockIdx.z;  // heads (or head pairs) fastest: DRAM page locality of [L, H, D]
-  constexpr bool pair = kPair;
-  const int head0 = pair ? 2 * hh : hh;                            // first real head of this CTA
-  const bool second_ok = !pair || head0 + 1 < p.h;                 // odd head count: the last pair has one real head
+  const int head0 = kPair ? 2 * hh : hh;                           // first real head of this CTA
+  const bool second_ok = !kPair || head0 + 1 < p.h;                // odd head count: the last pair has one real head
   const int64_t row_elems = int64_t(p.h) * p.hd;                   // elements per token row of k / v
   const int my_tiles = (p.tiles - split + p.splits - 1) / p.splits;  // tiles split, split+splits, ...
+  if (my_tiles <= 0) return;   // more splits than tiles
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bars[kVFull + i], 1);
-      mbar_init(&bars[kPhiFull + i], 4);
-      mbar_init(&bars[kStageEmpty + i], 1);
-    }
-    mbar_init(&bars[kAccFull], 1);
+    for (int i = 0; i < kVStages; ++i) mbar_init(&vfull[i], 1);
     mbar_fence_init();
   }
-  if (warp == 5) tmem_alloc<128>(tmem_slot);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-  if (my_tiles <= 0) {  // nothing to do (more splits than tiles); still release TMEM
-    __syncthreads();
-    if (warp == 5) tmem_dealloc<128>(tmem_base);
-    return;
+  auto load_v = [&](int i) {   // thread 0: V tile i -> stage i % kVStages
+    const int st = i % kVStages, tile = split + i * p.splits;
+    uint8_t* sv = smem + kOffV + st * kOperandBytes;
+    mbar_expect_tx(&vfull[st], kOperandBytes);
+    // 128-wide head: columns [0,64) and [64,128) of head hh; 64-wide heads: heads 2hh and 2hh+1 (a missing second
+    // head is out of range in the head dimension, which TMA fills with zeros)
+    tma_load_4d(sv, &tmap_v, &vfull[st], 0, head0, tile * kRowsPerTile, b);
+    tma_load_4d(sv + kBlockBytes, &tmap_v, &vfull[st], kPair ? 0 : 64, kPair ? head0 + 1 : head0, tile * kRowsPerTile, b);
+  };
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_v);
+    for (int i = 0; i < kVStages - 1 && i < my_tiles; ++i) load_v(i);
   }
 
-  if (warp == 4) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmap_v);
-      for (int i = 0; i < my_tiles; ++i) {
-        const int st = i & 1, tile = split + i * p.splits;
-        mbar_wait(&bars[kStageEmpty + st], ((i >> 1) & 1) ^ 1);
-        mbar_expect_tx(&bars[kVFull + st], kOperandBytes);
-        uint8_t* sv = smem + kOffV + st * kOperandBytes;
-        // 128-wide head: columns [0,64) and [64,128) of head hh; 64-wide heads: heads 2hh and 2hh+1 (a missing second
-        // head is out of range in the head dimension, which TMA fills with zeros)
-        tma_load_4d(sv, &tmap_v, &bars[kVFull + st], 0, head0, tile * kRowsPerTile, b);
-        tma_load_4d(sv + kBlockBytes, &tmap_v, &bars[kVFull + st], pair ? 0 : 64, pair ? head0 + 1 : head0, tile * kRowsPerTile, b);
+  const int r = threadIdx.x >> 1, half = threadIdx.x & 1;   // key row inside the tile, which 64 of its 128 channels
+  const int wg = warp >> 2;
+  const uint32_t sbase = smem_u32(smem);
+  uint8_t* const sphi = smem + kOffPhi;
+  float acc[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  float ksum_acc = 0.f;
+  // The key rows of tile i+1 are requested before tile i is transformed (eight independent 16-byte loads per thread in
+  // flight under the exponentials), and phi needs ONE exponential per element: e_j is kept in fp32 registers until the
+  // row sum is known.
+  auto load_row = [&](int i, uint4 (&dst)[8]) {
+    const int64_t row = int64_t(split + i * p.splits) * kRowsPerTile + r;
+    const bool ok = i < my_tiles && row < p.l && (half == 0 || second_ok);   // missing second head: zeros
+    const uint4* src = reinterpret_cast<const uint4*>(static_cast<const T*>(p.k) + (int64_t(b) * p.l + (ok ? row : 0)) * row_elems +
+                                                      int64_t(head0) * p.hd + half * 64);
+#pragma unroll
+    for (int c = 0; c < 8; ++c) dst[c] = ok ? ldg_nc_v4(src + c) : make_uint4(0u, 0u, 0u, 0u);
+  };
+  uint4 cur[8];
+  load_row(0, cur);
+  for (int i = 0; i < my_tiles; ++i) {
+    const int tile = split + i * p.splits;
+    const int64_t row = int64_t(tile) * kRowsPerTile + r;
+    uint4 nxt[8];
+    load_row(i + 1, nxt);
+    uint32_t w[32];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) { w[4 * c] = cur[c].x; w[4 * c + 1] = cur[c].y; w[4 * c + 2] = cur[c].z; w[4 * c + 3] = cur[c].w; }
+    const bool live = row < p.l && (half == 0 || second_ok);
+    if (p.feature == 0) {
+      // softmax over the head: my 64 channels, combined with the partner thread's for a 128-wide head
+      float m = -INFINITY;
+#pragma unroll
+      for (int q = 0; q < 32; ++q) m = fmaxf(m, fmaxf(F16Traits<T>::lo(w[q]), F16Traits<T>::hi(w[q])));
+      if (!kPair) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+      const float off = m * kLog2e;
+      float e[64];
+      float sa = 0.f, sb = 0.f;
+#pragma unroll
+      for (int q = 0; q < 32; ++q) {
+        e[2 * q] = fast_exp2(fmaf(F16Traits<T>::lo(w[q]), kLog2e, -off));
+        e[2 * q + 1] = fast_exp2(fmaf(F16Traits<T>::hi(w[q]), kLog2e, -off));
+        sa += e[2 * q];
+        sb += e[2 * q + 1];
       }
-    }
-  } else if (warp == 5) {
-    if (lane == 0) {
-      constexpr bool is_bf16 = std::is_same<T, __nv_bfloat16>::value;
-      constexpr uint32_t idesc = make_idesc(kDFmtF32, is_bf16 ? kFmtBF16 : kFmtF16, is_bf16 ? kFmtBF16 : kFmtF16, 1, 1, D, D);
-      const uint32_t sbase = smem_u32(smem);
-      for (int i = 0; i < my_tiles; ++i) {
-        const int st = i & 1;
-        mbar_wait(&bars[kVFull + st], (i >> 1) & 1);
-        mbar_wait(&bars[kPhiFull + st], (i >> 1) & 1);
-        tc_fence_after_sync();
-        const uint64_t adesc = make_desc_mnmajor_sw128(sbase + kOffV + st * kOperandBytes, kBlockBytes);
-        const uint64_t bdesc = make_desc_mnmajor_sw128(sbase + kOffPhi + st * kOperandBytes, kBlockBytes);
+      float sum = sa + sb;
+      if (!kPair) sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+      const float inv = 1.0f / sum;
 #pragma unroll
-        for (int ks = 0; ks < kRowsPerTile / 16; ++ks)  // K = 16 key rows per MMA: +2048 B in both operands
-          umma_f16_ss(tmem_base, adesc + uint64_t(ks * 128), bdesc + uint64_t(ks * 128), idesc, (i > 0 || ks > 0) ? 1u : 0u);
-        umma_commit(&bars[kStageEmpty + st]);
-      }
-      umma_commit(&bars[kAccFull]);
-    }
-  } else {
-    const int r = warp * 32 + lane;  // key row inside the tile; later: value channel (TMEM lane) / key channel (ksum)
-    float ksum_acc = 0.f;
-    // The key rows of tile i+1 are requested before tile i is transformed (16 independent 16-byte loads per thread in flight
-    // under the exponentials), and phi needs ONE exponential per element: e_j is kept in fp32 registers until the row sum is
-    // known.  (Round 1 loaded, waited, and evaluated every exponential twice: 9.8k clk per 128-row tile.)
-    auto load_row = [&](int i, uint4 (&dst)[D / 8]) {
-      const int64_t row = int64_t(split + i * p.splits) * kRowsPerTile + r;
-      const int nload = (i < my_tiles && row < p.l) ? (second_ok ? D / 8 : D / 16) : 0;   // missing second head: zeros
-      const uint4* src = reinterpret_cast<const uint4*>(static_cast<const T*>(p.k) +
-                                                        (int64_t(b) * p.l + (row < p.l ? row : 0)) * row_elems + int64_t(head0) * p.hd);
-#pragma unroll
-      for (int c = 0; c < D / 8; ++c) {
-        dst[c] = make_uint4(0u, 0u, 0u, 0u);
-        if (c < nload) dst[c] = ldg_nc_v4(src + c);
-      }
-    };
-    uint4 cur[D / 8];
-    load_row(0, cur);
-    for (int i = 0; i < my_tiles; ++i) {
-      const int st = i & 1, tile = split + i * p.splits;
-      const int64_t row = int64_t(tile) * kRowsPerTile + r;
-      uint4 nxt[D / 8];
-      load_row(i + 1, nxt);
-      uint32_t w[D / 2];
-#pragma unroll
-      for (int c = 0; c < D / 8; ++c) { w[4 * c] = cur[c].x; w[4 * c + 1] = cur[c].y; w[4 * c + 2] = cur[c].z; w[4 * c + 3] = cur[c].w; }
-      if (row < p.l) {
-        // phi over each segment of the row (one 128-wide segment, or two 64-wide segments for a pair of 64-wide heads)
-        constexpr int kSeg = kPair ? 2 : 1, kWps = (D / 2) / kSeg;   // segments, 32-bit words per segment
-#pragma unroll
-        for (int sgm = 0; sgm < kSeg; ++sgm) {
-          const int w0 = sgm * kWps;
-          if (p.feature == 0) {
-            float m0 = -INFINITY, m1 = -INFINITY;
-#pragma unroll
-            for (int q = 0; q < kWps; q += 2) {
-              m0 = fmaxf(m0, fmaxf(F16Traits<T>::lo(w[w0 + q]), F16Traits<T>::hi(w[w0 + q])));
-              m1 = fmaxf(m1, fmaxf(F16Traits<T>::lo(w[w0 + q + 1]), F16Traits<T>::hi(w[w0 + q + 1])));
-            }
-            const float off = fmaxf(m0, m1) * kLog2e;
-            float e[2 * kWps];
-            float sa = 0.f, sb = 0.f, sc4 = 0.f, sd = 0.f;  // independent chains
-#pragma unroll
-            for (int q = 0; q < kWps; q += 2) {
-              e[2 * q] = fast_exp2(fmaf(F16Traits<T>::lo(w[w0 + q]), kLog2e, -off));
-              e[2 * q + 1] = fast_exp2(fmaf(F16Traits<T>::hi(w[w0 + q]), kLog2e, -off));
-              e[2 * q + 2] = fast_exp2(fmaf(F16Traits<T>::lo(w[w0 + q + 1]), kLog2e, -off));
-              e[2 * q + 3] = fast_exp2(fmaf(F16Traits<T>::hi(w[w0 + q + 1]), kLog2e, -off));
-              sa += e[2 * q]; sb += e[2 * q + 1]; sc4 += e[2 * q + 2]; sd += e[2 * q + 3];
-            }
-            const float inv = 1.0f / ((sa + sb) + (sc4 + sd));
-#pragma unroll
-            for (int q = 0; q < kWps; ++q) w[w0 + q] = F16Traits<T>::pack(e[2 * q] * inv, e[2 * q + 1] * inv);
-          } else {
-#pragma unroll
-            for (int q = 0; q < kWps; ++q) {
-              const float a = F16Traits<T>::lo(w[w0 + q]), c = F16Traits<T>::hi(w[w0 + q]);
-              const float fa = p.feature == 1 ? (a > 0.f ? a + 1.0f : fast_exp2(a * kLog2e)) : fmaxf(a, 0.f);
-              const float fc = p.feature == 1 ? (c > 0.f ? c + 1.0f : fast_exp2(c * kLog2e)) : fmaxf(c, 0.f);
-              w[w0 + q] = F16Traits<T>::pack(fa, fc);
-            }
-          }
-        }
-        if (!second_ok) {
-#pragma unroll
-          for (int q = D / 4; q < D / 2; ++q) w[q] = 0u;
-        }
-      } else {
-#pragma unroll
-        for (int q = 0; q < D / 2; ++q) w[q] = 0u;
-      }
-#pragma unroll
-      for (int c = 0; c < D / 8; ++c) cur[c] = nxt[c];
-      // stage free? (the MMA that read it two tiles ago has retired)
-      mbar_wait(&bars[kStageEmpty + st], ((i >> 1) & 1) ^ 1);
-      uint8_t* sphi = smem + kOffPhi + st * kOperandBytes;
-#pragma unroll
-      for (int c = 0; c < 16; ++c)
-        *reinterpret_cast<uint4*>(sphi + (c >> 3) * kBlockBytes + r * 128 + (((c & 7) ^ (r & 7)) << 4)) =
-            make_uint4(w[4 * c], w[4 * c + 1], w[4 * c + 2], w[4 * c + 3]);
-      fence_proxy_async_smem();
-      named_bar_sync(1, 128);  // all 128 rows of the tile are written (also orders the ksum reads below)
-      if (lane == 0) mbar_arrive(&bars[kPhiFull + st]);
-      // ---- ksum: thread r sums key channel r over the 128 rows of the tile
-      {
-        const uint8_t* colbase = sphi + (r >> 6) * kBlockBytes + (r & 7) * 2;
-        const int chunk = (r & 63) >> 3;
-        float s4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 8
-        for (int rr = 0; rr < kRowsPerTile; rr += 4) {
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const unsigned short raw =
-                *reinterpret_cast<const unsigned short*>(colbase + (rr + u) * 128 + ((chunk ^ ((rr + u) & 7)) << 4));
-            s4[u] += F16Traits<T>::lo(static_cast<uint32_t>(raw));
-          }
-        }
-        ksum_acc += (s4[0] + s4[1]) + (s4[2] + s4[3]);
-      }
-    }
-    // thread r holds key channel r of the 128-wide row: head0's channel r, or (pairs) channel r-64 of head0+1
-    if (!pair) {
-      atomicAdd(p.ksum + (int64_t(b) * p.h + head0) * D + r, ksum_acc);
-    } else if (r < 64 || second_ok) {
-      atomicAdd(p.ksum + (int64_t(b) * p.h + head0 + (r >> 6)) * 64 + (r & 63), ksum_acc);
-    }
-    // ---- kv: TMEM lane r = value channel r, 128 key channels
-    mbar_wait(&bars[kAccFull], 0);
-    tc_fence_after_sync();
-    if (!pair) {
-      float* dst = p.kv + ((int64_t(b) * p.h + head0) * D + r) * D;
-#pragma unroll
-      for (int c = 0; c < D / 32; ++c) {
-        uint32_t o[32];
-        tmem_ld_x32(tmem_base + (uint32_t(warp * 32) << 16) + c * 32, o);
-        tmem_ld_wait();
-#pragma unroll
-        for (int q = 0; q < 32; q += 4)
-          red_add_v4(dst + c * 32 + q, __uint_as_float(o[q]), __uint_as_float(o[q + 1]), __uint_as_float(o[q + 2]),
-                     __uint_as_float(o[q + 3]));
-      }
+      for (int q = 0; q < 32; ++q) w[q] = F16Traits<T>::pack(e[2 * q] * inv, e[2 * q + 1] * inv);
     } else {
-      // lane r = value channel (r & 63) of head0 + (r >> 6); its diagonal block is key columns [64*(r>>6), +64)
-      const int sub = r >> 6;                        // warp-uniform (warps 0,1 -> head0; warps 2,3 -> head0+1)
-      float* dst = p.kv + ((int64_t(b) * p.h + head0 + sub) * 64 + (r & 63)) * 64;
 #pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t o[32];
-        tmem_ld_x32(tmem_base + (uint32_t(warp * 32) << 16) + sub * 64 + c * 32, o);
-        tmem_ld_wait();
-        if (sub == 0 || second_ok) {
-#pragma unroll
-          for (int q = 0; q < 32; q += 4)
-            red_add_v4(dst + c * 32 + q, __uint_as_float(o[q]), __uint_as_float(o[q + 1]), __uint_as_float(o[q + 2]),
-                       __uint_as_float(o[q + 3]));
-        }
+      for (int q = 0; q < 32; ++q) {
+        const float a = F16Traits<T>::lo(w[q]), c = F16Traits<T>::hi(w[q]);
+        const float fa = p.feature == 1 ? (a > 0.f ? a + 1.0f : fast_exp2(a * kLog2e)) : fmaxf(a, 0.f);
+        const float fc = p.feature == 1 ? (c > 0.f ? c + 1.0f : fast_exp2(c * kLog2e)) : fmaxf(c, 0.f);
+        w[q] = F16Traits<T>::pack(fa, fc);
       }
     }
-    tc_fence_before_sync();
+    if (!live) {
+#pragma unroll
+      for (int q = 0; q < 32; ++q) w[q] = 0u;
+    }
+#pragma unroll
+    for (int c = 0; c < 8; ++c) cur[c] = nxt[c];
+    // every warpgroup's MMAs of tile i-1 have retired (they read the phi buffer and V stage (i-1) % kVStages)
+    wgmma_wait<0>();
+    __syncthreads();
+    if (threadIdx.x == 0 && i + kVStages - 1 < my_tiles) load_v(i + kVStages - 1);
+#pragma unroll
+    for (int c = 0; c < 8; ++c)
+      *reinterpret_cast<uint4*>(sphi + half * kBlockBytes + r * 128 + ((c ^ (r & 7)) << 4)) =
+          make_uint4(w[4 * c], w[4 * c + 1], w[4 * c + 2], w[4 * c + 3]);
+    fence_proxy_async_smem();
+    __syncthreads();   // all 128 rows of phi are written (also orders the ksum reads below)
+    {
+      const int st = i % kVStages;
+      mbar_wait(&vfull[st], (i / kVStages) & 1);
+      // A = V^T (dv rows of block wg), B = phi (key channels; a pair's warpgroup takes its own 64-channel block): both MN-major,
+      // K = 16 key rows per MMA: +2048 B in both operands
+      const uint64_t adesc = make_desc_mnmajor_sw128(sbase + kOffV + st * kOperandBytes + wg * kBlockBytes, kBlockBytes);
+      const uint64_t bdesc = make_desc_mnmajor_sw128(sbase + kOffPhi + (kPair ? wg * kBlockBytes : 0), kBlockBytes);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < kRowsPerTile / 16; ++ks)
+        wgmma_f16_ss_mn<N, kBF16>(acc, adesc + uint64_t(ks * 128), bdesc + uint64_t(ks * 128), 1u);
+      wgmma_commit();
+    }
+    // ---- ksum: thread t sums key channel t % 128 over half of the 128 rows of the tile
+    {
+      const int col = threadIdx.x & 127, r0 = (threadIdx.x >> 7) * 64;
+      const uint8_t* colbase = sphi + (col >> 6) * kBlockBytes + (col & 7) * 2;
+      const int chunk = (col & 63) >> 3;
+      float s4[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll 4
+      for (int rr = r0; rr < r0 + 64; rr += 4) {
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const unsigned short raw =
+              *reinterpret_cast<const unsigned short*>(colbase + (rr + u) * 128 + ((chunk ^ ((rr + u) & 7)) << 4));
+          s4[u] += F16Traits<T>::lo(static_cast<uint32_t>(raw));
+        }
+      }
+      ksum_acc += (s4[0] + s4[1]) + (s4[2] + s4[3]);
+    }
   }
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after_sync();
-    tmem_dealloc<128>(tmem_base);
+  wgmma_wait<0>();
+  reg_fence(acc);
+  {
+    // thread t holds key channel t % 128 of the 128-wide row: head0's channel, or (pairs) channel c-64 of head0+1
+    const int col = threadIdx.x & 127;
+    if (!kPair) {
+      atomicAdd(p.ksum + (int64_t(b) * p.h + head0) * D + col, ksum_acc);
+    } else if (col < 64 || second_ok) {
+      atomicAdd(p.ksum + (int64_t(b) * p.h + head0 + (col >> 6)) * 64 + (col & 63), ksum_acc);
+    }
+  }
+  // ---- kv: accumulator rows = value channels, columns = key channels (fragment layout, common.cuh)
+  const int w4 = warp & 3;
+  const int dv_lo = w4 * 16 + (lane >> 2), cq = 2 * (lane & 3);
+  if (!kPair || wg == 0 || second_ok) {
+    float* dst = kPair ? p.kv + (int64_t(b) * p.h + head0 + wg) * 64 * 64
+                       : p.kv + (int64_t(b) * p.h + head0) * D * D + int64_t(wg) * 64 * D;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+      for (int h2 = 0; h2 < 2; ++h2)
+        red_add_v2(dst + int64_t(dv_lo + 8 * h2) * N + 8 * j + cq, acc[4 * j + 2 * h2], acc[4 * j + 2 * h2 + 1]);
   }
 }
 
@@ -275,7 +225,7 @@ static int moments_impl(const void* k, const void* v, int dtype, int64_t b, int6
   if (feature < 0 || feature > 2) return fail(TDB200_ERR_INVALID_ARG, "sla_linear_moments: feature map tag %d", feature);
   if (h > 65535 || b > 65535) return fail(TDB200_ERR_UNSUPPORTED, "sla_linear_moments: h or b too large");
   if (!aligned16(k) || !aligned16(kv)) return fail(TDB200_ERR_INVALID_ARG, "sla_linear_moments: buffers must be 16-byte aligned");
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
   const CUtensorMapDataType t16 = dtype == TDB200_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUtensorMap tv;
   {
@@ -361,7 +311,7 @@ extern "C" int tdb200_sla_project_moments(const float* proj_w, const float* kv, 
   if (!proj_w || !kv || !kvw) return fail(TDB200_ERR_INVALID_ARG, "sla_project_moments: null pointer");
   if (bh <= 0 || bh > 0x7FFFFFFF) return fail(TDB200_ERR_INVALID_ARG, "sla_project_moments: bad shape");
   if (d != 64 && d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_project_moments: head dim %lld (64 or 128)", (long long)d);
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   dim3 grid(static_cast<unsigned>(bh), static_cast<unsigned>(d / 32));
 #define TDB_PM(T, D) project_moments_kernel<T, D><<<grid, D, 0, st>>>(proj_w, kv, static_cast<T*>(kvw)); return check_launch("project_moments_kernel")

@@ -230,7 +230,7 @@ extern "C" int tdb200_sla_quant_qk(const void* q, const void* k, int dtype, int6
     return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_qk: h, b or sequence length too large");
   if ((q && (!aligned16(q) || !aligned16(q_i8))) || (k && (!aligned16(k) || !aligned16(k_i8))))
     return fail(TDB200_ERR_INVALID_ARG, "sla_quant_qk: buffers must be 16-byte aligned");
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define TDB_RUN(T, D) return run<T, D>(q, k, b, lq, l, h, kmean, q_i8, q_scale, k_i8, k_scale, q_pool, k_pool, st)
   if (dtype == TDB200_DTYPE_BF16) {
@@ -255,7 +255,7 @@ extern "C" int tdb200_sla_kmean_partial(const void* k, int dtype, int64_t b, int
   if (d != 64 && d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_kmean_partial: head dim %lld (64 or 128)", (long long)d);
   if (h > 65535 || b > 65535 || cdiv64(l, kMeanRows) > 65535) return fail(TDB200_ERR_UNSUPPORTED, "sla_kmean_partial: dimension too large");
   if (!aligned16(k)) return fail(TDB200_ERR_INVALID_ARG, "sla_kmean_partial: k must be 16-byte aligned");
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (dtype == TDB200_DTYPE_BF16) return d == 128 ? run_kmean_partial<__nv_bfloat16, 128>(k, b, l, h, partial, st) : run_kmean_partial<__nv_bfloat16, 64>(k, b, l, h, partial, st);
   if (dtype == TDB200_DTYPE_FP16) return d == 128 ? run_kmean_partial<__half, 128>(k, b, l, h, partial, st) : run_kmean_partial<__half, 64>(k, b, l, h, partial, st);
@@ -268,7 +268,7 @@ extern "C" int tdb200_sla_kmean_final(const float* partial, int64_t b, int64_t h
   if (!partial || !kmean) return fail(TDB200_ERR_INVALID_ARG, "sla_kmean_final: null pointer");
   if (b <= 0 || h <= 0 || chunks <= 0 || l_total <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_kmean_final: bad shape");
   if (d != 64 && d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_kmean_final: head dim %lld (64 or 128)", (long long)d);
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
   kmean_final_kernel<<<static_cast<unsigned>(b * h), 1024, 0, static_cast<cudaStream_t>(stream)>>>(partial, kmean, l_total,
                                                                                                   static_cast<int>(chunks), static_cast<int>(d));
   return check_launch("kmean_final_kernel");
@@ -282,7 +282,7 @@ extern "C" int tdb200_sla_quant_k_seq(const void* k, const float* kmean, int dty
   if (d != 64 && d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_k_seq: head dim %lld (64 or 128)", (long long)d);
   if (h > 65535 || b > 65535 || cdiv64(l, 64) > 65535) return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_k_seq: dimension too large");
   if (!aligned16(k) || !aligned16(k_i8)) return fail(TDB200_ERR_INVALID_ARG, "sla_quant_k_seq: buffers must be 16-byte aligned");
-  if (int rc = require_sm100()) return rc;
+  if (int rc = require_sm90()) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define TDB_RUN(T, D) return run_k_quant<T, D>(k, b, l, h, kmean, k_i8, k_scale, k_pool, true, st)
   if (dtype == TDB200_DTYPE_BF16) {

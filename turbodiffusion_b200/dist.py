@@ -21,7 +21,7 @@ H % world == 0 (12 heads do not split 8 ways).  UlyssesAttention below implement
 turn the local [rows, H, D] slabs of q, k, v into [L, H/world, D] (all rows, this rank's heads), the unchanged single-GPU SLA
 forward runs on those heads, and a fourth all-to-all brings the output back to [rows, H, D].  Per rank and layer it moves
 4*(N-1)/N^2 * L*dim*2 bytes instead of 2*(N-1)/N * L*dim*2 for the K/V all-gather (4x less at N = 8) and no rank repeats
-the K-side preparation of the full sequence; `SequenceParallel.install(mode="auto")` picks it where it measured faster
+the K-side preparation of the full sequence; `SequenceParallel.install(mode="auto")` picks it from four GPUs up
 (see pick_mode).
 """
 from __future__ import annotations
@@ -320,7 +320,7 @@ class UnevenUlyssesAttention(UlyssesAttention):
     """The same exchange when heads % world != 0 (e.g. the 12 heads of Wan-1.3B on 8 GPUs -> 2,2,2,2,1,1,1,1): rank r takes
     the contiguous head range split_heads() assigns it; every all-to-all uses per-peer split sizes in units of one
     [D]-row (rows * heads_of_peer).  The slab <-> per-peer-chunk reordering is ONE gather kernel each way (a precomputed row
-    permutation), not one copy per peer.  Measured on 8 B200s at shape A: 26.4 ms/step vs 30.4 for the all-gather mode."""
+    permutation), not one copy per peer."""
 
     def __init__(self, sp: "SequenceParallel", prims, heads: int, compute_dtype=None):
         super().__init__(sp, prims, compute_dtype)
@@ -386,11 +386,10 @@ class SequenceParallel:
         if mode not in ("auto", "allgather", "ulysses"):
             raise ValueError(f"unknown sequence-parallel mode {mode!r}")
         if mode == "auto":
-            # measured on B200, shape A, ms/step all-gather vs all-to-all (profiles/r02_bench_n{2,4,8}*): N=2 57.6 vs 64.5 (the
-            # all-gather's exchanges hide under the V / Q projections; the all-to-all has the output exchange and the slab
-            # permutes on the critical path), N=4 37.8 vs 35.5, N=8 30.4 vs 26.4 (12 heads -> uneven split 2,2,2,2,1,1,1,1);
-            # shape B at N=8 (40 heads): 251.8 ms/step, 6.5x one GPU.  From N=4 up the all-to-all moves N/2 times fewer bytes
-            # and has no per-rank work that grows with the full sequence.
+            # at N=2 the all-gather's exchanges hide under the V / Q projections, while the all-to-all has the output exchange
+            # and the slab permutes on the critical path; from N=4 up the all-to-all moves N/2 times fewer bytes and has no
+            # per-rank work that grows with the full sequence (12 heads at N=8 -> uneven split 2,2,2,2,1,1,1,1).  Not measured
+            # on H100.
             return "ulysses" if self.world >= 4 and heads >= self.world else "allgather"
         if mode == "ulysses" and heads < self.world:
             raise ValueError(f"mode 'ulysses' needs at least one head per rank (heads={heads}, world={self.world})")

@@ -1,4 +1,4 @@
-"""LTX-2 (TurboT2AV) prologue operators on B200 — the second client of the operator API (SURVEY 8a row a12).
+"""LTX-2 (TurboT2AV) prologue operators on H100 — the second client of the operator API (SURVEY 8a row a12).
 
 Same signatures as the fused helpers in ltx_core/model/transformer/transformer.py:46-94 and the Triton fast path
 (ltx_distillation/fast_norm_kernels.py): x [B, T, N] bf16/fp16, scale_shift_table [num_ada, N], timestep [B, Tt, num_ada*N]

@@ -108,7 +108,7 @@ class Int8Linear(nn.Module):
             self.bias = None
 
     def forward(self, x):
-        # quant + tcgen05 GEMM with the bias add fused into the epilogue (same value as `out + self.bias`)
+        # quant + wgmma GEMM with the bias add fused into the epilogue (same value as `out + self.bias`)
         return int8_linear(x, self.int8_weight, self.scale, self.bias)
 
     @classmethod

@@ -4,7 +4,7 @@ Same function names, argument order and return values as the reference extension
 libtdb200.so through its C ABI on the current CUDA stream.  Extra exports `gemm_cuda_swizzle` and
 `gemm_cuda_swizzle_bias` are the ones TurboT2AV's acceleration.py looks up with getattr
 (ltx_distillation/acceleration.py:695-701); the swizzle arguments are accepted and ignored (tile order is
-an implementation detail of the persistent tcgen05 kernel).
+an implementation detail of the GEMM kernel).
 """
 from __future__ import annotations
 

@@ -151,7 +151,8 @@ int tdb200_rms_norm_rope_table(const void* x, int dtype, const float* w, const f
 /* ---------------------------------------------------------------------------------------------
  * a7-a10. SLA / SageSLA.  q, k, v, out are [b, l, h, d] contiguous 16-bit (the layout the module is
  * called with, SLA/core.py:181-183), d in {64, 128}.  Block sizes: BLKQ = 128 query rows, BLKK = 64 key rows
- * (the non-sm90 branch, SLA/core.py:191-193).  mblk = ceil(l/128), nblk = ceil(l/64).
+ * (the non-sm90 branch, SLA/core.py:191-193).  mblk = ceil(l/128), nblk = ceil(l/64).  The *_blocks entry points also
+ * serve the sm90 branch's BLKQ = 64, BLKK = 128 (mblk = ceil(l/64), nblk = ceil(l/128)).
  *
  * tdb200_sla_quant_qk   one pass over q [b,lq,h,d] and two over k [b,lk,h,d] (lq != lk when the query rows are one rank's
  *     sequence shard and k is the gathered key slab; mblk = ceil(lq/128), nblk = ceil(lk/64)):
@@ -218,6 +219,21 @@ int tdb200_sla_attn_fwd_v2(const int8_t* q_i8, const float* q_scale, const int8_
                            const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk, const void* kvw,
                            const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
                            int64_t h, int64_t d, float sm_scale, int feature, void* stream);
+/* The SageSLA pair with the block geometry as an argument: (blkq, blkk) = (128, 64), the sizes of the entry points above, or
+ * (64, 128), SpargeAttn's Hopper family (SLA/core.py:191-193, 226-229).  Any other pair returns TDB200_ERR_UNSUPPORTED.
+ *   tdb200_sla_quant_qk_blocks  tdb200_sla_quant_qk with q pooled / quantised per blkq rows and smoothed k per blkk rows:
+ *                               q_scale [b,h,ceil(lq/blkq)], q_pool [b,h,ceil(lq/blkq),d], k_scale [b,h,ceil(lk/blkk)],
+ *                               k_pool [b,h,ceil(lk/blkk),d]; kmean and the code layouts are unchanged.
+ *   tdb200_sla_attn_fwd_blocks  tdb200_sla_attn_fwd_v2 on those blocks (lut [b,h,ceil(l/blkq),topk] of blkk-row key blocks);
+ *                               (128, 64) is tdb200_sla_attn_fwd_v2 itself.  With (64, 128) one CTA per 64-row query block
+ *                               runs two consumer warpgroups on alternate key blocks and merges their softmax states. */
+int tdb200_sla_quant_qk_blocks(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d,
+                               float* kmean, int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale, void* q_pool,
+                               void* k_pool, int64_t blkq, int64_t blkk, void* stream);
+int tdb200_sla_attn_fwd_blocks(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
+                               const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk, const void* kvw,
+                               const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
+                               int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq, int64_t blkk, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * a12. LTX-2 (TurboT2AV) prologue variants   (ltx_core/model/transformer/transformer.py:21-94; Triton fast path

@@ -15,7 +15,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .._lib import DTYPE_TAG, check, lib, ptr, require_cuda, stream_ptr
-from .utils import QKPrep, block_map_from_pools, get_block_map, get_cuda_arch, quant_qk  # noqa: F401
+from .utils import SAGE_BLOCKS, QKPrep, block_map_from_pools, get_block_map, get_cuda_arch, quant_qk  # noqa: F401
 
 SAGESLA_ENABLED = True   # the INT8 path is built in (no SpargeAttn dependency)
 SAGE2PP_ENABLED = True
@@ -49,28 +49,30 @@ def project_moments(proj_w: torch.Tensor, kv: torch.Tensor, dtype) -> torch.Tens
 ATTN_TIMER = None  # bench.py installs a callable(h, mblk, topk, d) -> context manager to time the fused-attention launches
 
 
-def attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, feature=0):
+def attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, feature=0, blkq=128, blkk=64):
+    """(blkq, blkk): the block sizes `prep` and `lut` were built with, (128, 64) or (64, 128)."""
     if ATTN_TIMER is not None:
-        with ATTN_TIMER(q.shape[2] * q.shape[0], (q.shape[1] + 127) // 128, topk, q.shape[3]):
-            return _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk, feature)
-    return _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk, feature)
+        # bench.py counts H*Mblk*topk*4*128*64*D FLOPs: exact for both families, BLKQ*BLKK = 8192 in each
+        with ATTN_TIMER(q.shape[2] * q.shape[0], (q.shape[1] + blkq - 1) // blkq, topk, q.shape[3]):
+            return _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk, feature, blkq, blkk)
+    return _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk, feature, blkq, blkk)
 
 
-def _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, feature=0):
+def _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, feature=0, blkq=128, blkk=64):
     b, l, h, d = q.shape
     lk = v.shape[1] if lk is None else lk
     out = torch.empty_like(q)
     if getattr(prep, "k_seq_major", False):   # INT8 K in the gathered [B, Lk, H, D] layout (dist.py)
-        if d != 128 or feature != 0:
-            raise NotImplementedError("sequence-major INT8 K is served by the 128-wide softmax kernel only")
+        if d != 128 or feature != 0 or (blkq, blkk) != (128, 64):
+            raise NotImplementedError("sequence-major INT8 K is served by the 128-wide softmax kernel on 128x64 blocks only")
         check(lib().tdb200_sla_attn_fwd_kseq(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v),
                                              ptr(q), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b),
                                              ptr(out), b, l, lk, h, d, float(sm_scale), stream_ptr(q.device)), "sla_attn_fwd")
-    else:   # head-major INT8 K: head dims 64 and 128, every feature map
-        check(lib().tdb200_sla_attn_fwd_v2(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v),
-                                           ptr(q), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b),
-                                           ptr(out), b, l, lk, h, d, float(sm_scale), feature, stream_ptr(q.device)),
-              "sla_attn_fwd")
+    else:   # head-major INT8 K: head dims 64 and 128, every feature map, both block geometries
+        check(lib().tdb200_sla_attn_fwd_blocks(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v),
+                                               ptr(q), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b),
+                                               ptr(out), b, l, lk, h, d, float(sm_scale), feature, blkq, blkk,
+                                               stream_ptr(q.device)), "sla_attn_fwd")
     return out
 
 
@@ -87,6 +89,10 @@ def attn_fwd_qk16(q, k, v, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None):
 
 class _SLABase(nn.Module):
     quantised_qk = True   # SageSparseLinearAttention: INT8 Q.K^T; SparseLinearAttention: 16-bit Q.K^T (128-wide heads)
+
+    def block_sizes(self, device_index):
+        """(BLKQ, BLKK) of this call."""
+        return 128, 64
 
     def __init__(self, head_dim, topk, feature_map="softmax", use_bf16=True, tie_feature_map_qk=True):
         super().__init__()
@@ -117,7 +123,8 @@ class _SLABase(nn.Module):
         b, l, h, d = q.shape
         if d not in (64, 128):
             raise AssertionError("headdim should be in [64, 128].")  # SLA/core.py:207
-        prep = quant_qk(q, k)
+        blkq, blkk = self.block_sizes(q.device.index)
+        prep = quant_qk(q, k, blkq=blkq, blkk=blkk)
         nblk = prep.nblk
         real_topk = min(nblk, int(self.topk * nblk))
         if real_topk < 1:
@@ -133,7 +140,7 @@ class _SLABase(nn.Module):
             o = attn_fwd_qk16(q, k, v, lut, real_topk, kvw, ksum, self.proj_l.bias.float().contiguous(), d ** -0.5)
         else:
             o = attn_fwd(prep, v, q, lut, real_topk, kvw, ksum, self.proj_l.bias.float().contiguous(), d ** -0.5,
-                         feature=self.feature)
+                         feature=self.feature, blkq=blkq, blkk=blkk)
         o = o if o.dtype == dtype else o.to(dtype)
         return (o, real_topk / nblk) if return_sparsity else o
 
@@ -172,6 +179,10 @@ class SageSparseLinearAttention(_SLABase):
     def __init__(self, head_dim, topk, feature_map="softmax", use_bf16=True, tie_feature_map_qk=True):
         super().__init__(head_dim, topk, feature_map, use_bf16, tie_feature_map_qk)
 
+    def block_sizes(self, device_index):
+        """The reference's choice (SLA/core.py:191-193): BLKQ=64 / BLKK=128 where get_cuda_arch reports sm90, else 128 / 64."""
+        return SAGE_BLOCKS["sm90"] if get_cuda_arch(device_index) == "sm90" else SAGE_BLOCKS["sm100"]
+
 
 # ------------------------------------------------------------------------------------------------------------------------
 # Names the LTX-2 client reaches for inside `SLA.core` (TurboT2AV ltx_distillation/acceleration.py:260-383,
@@ -182,10 +193,11 @@ class SageSparseLinearAttention(_SLABase):
 # ------------------------------------------------------------------------------------------------------------------------
 def get_vanilla_qk_quant(q, k, km=None, BLKQ=128, BLKK=64):
     """q,k [B,H,L,D] -> (q_int8 [B,H,L,D], q_scale [B,H,Mblk], k_int8 of (k - mean_L k), k_scale [B,H,Nblk]); call site
-    SLA/core.py:200-203.  `km` is accepted for signature compatibility (the key mean is recomputed by the fused prepass)."""
-    if (BLKQ, BLKK) != (128, 64):
-        raise NotImplementedError("this implementation uses the block sizes BLKQ=128, BLKK=64 on every architecture")
-    prep = quant_qk(q.transpose(1, 2).contiguous(), k.transpose(1, 2).contiguous())
+    SLA/core.py:200-203.  `km` is accepted for signature compatibility (the key mean is recomputed by the fused prepass).
+    (BLKQ, BLKK) is (128, 64) or the Hopper family's (64, 128)."""
+    if (BLKQ, BLKK) not in SAGE_BLOCKS.values():
+        raise NotImplementedError(f"block sizes BLKQ={BLKQ}, BLKK={BLKK}: this implementation serves (128, 64) and (64, 128)")
+    prep = quant_qk(q.transpose(1, 2).contiguous(), k.transpose(1, 2).contiguous(), blkq=BLKQ, blkk=BLKK)
     return prep.q_i8, prep.q_scale, prep.k_i8, prep.k_scale
 
 
@@ -217,9 +229,7 @@ class _FusedShim:
 fused = _FusedShim()
 
 
-def qk_int8_sv_f8_accum_f16_block_sparse_attn_inst_buf_fuse_v_scale_with_pv_threshold(
-        q_int8, k_int8, v_fp8, o, lut, valid_block_num, pvthreshold, q_scale, k_scale, v_scale, tensor_layout=1,
-        is_causal=False, qk_quant_gran=1, sm_scale=None, return_lse=0):
+def _sparse_only_attn(q_int8, k_int8, v_fp8, o, lut, q_scale, k_scale, sm_scale, blkq, blkk):
     """Sparse (softmax) branch only: o [B,H,L,D] <- block-sparse INT8-QK attention over the LUT's key blocks, the linear
     branch switched off (zero moments, zero bias).  Same kernel as SageSparseLinearAttention.forward."""
     v = getattr(v_fp8, "_tdb200_src", None)
@@ -229,24 +239,41 @@ def qk_int8_sv_f8_accum_f16_block_sparse_attn_inst_buf_fuse_v_scale_with_pv_thre
     lk = k_int8.shape[2]
     prep = QKPrep()
     prep.q_i8, prep.q_scale, prep.k_i8, prep.k_scale = q_int8, q_scale, k_int8, k_scale
-    prep.mblk, prep.nblk = (lq + 127) // 128, (lk + 63) // 64
+    prep.mblk, prep.nblk = (lq + blkq - 1) // blkq, (lk + blkk - 1) // blkk
     vt = v.transpose(1, 2).contiguous()                       # [B,L,H,D]
     qz = torch.zeros(b, lq, h, d, dtype=v.dtype, device=v.device)
     kvw = torch.zeros(b, h, d, d, dtype=v.dtype, device=v.device)
     ksum = torch.ones(b, h, d, dtype=torch.float32, device=v.device)
     pb = torch.zeros(d, dtype=torch.float32, device=v.device)
-    out = attn_fwd(prep, vt, qz, lut, lut.shape[-1], kvw, ksum, pb, sm_scale if sm_scale is not None else d ** -0.5, lk=lk)
+    out = attn_fwd(prep, vt, qz, lut, lut.shape[-1], kvw, ksum, pb, sm_scale if sm_scale is not None else d ** -0.5, lk=lk,
+                   blkq=blkq, blkk=blkk)
     o.copy_(out.transpose(1, 2))
     return o
 
 
+def qk_int8_sv_f8_accum_f16_block_sparse_attn_inst_buf_fuse_v_scale_with_pv_threshold(
+        q_int8, k_int8, v_fp8, o, lut, valid_block_num, pvthreshold, q_scale, k_scale, v_scale, tensor_layout=1,
+        is_causal=False, qk_quant_gran=1, sm_scale=None, return_lse=0):
+    """The Sage2++ entry (BLKQ=128, BLKK=64): see _sparse_only_attn."""
+    return _sparse_only_attn(q_int8, k_int8, v_fp8, o, lut, q_scale, k_scale, sm_scale, *SAGE_BLOCKS["sm100"])
+
+
 class _QattnShim:
-    """SpargeAttn's `qattn` extension module holds its sm80 / sm90 kernels; here every architecture is served by the Sage2++
-    entry above (the fused kernel with the block sizes BLKQ=128, BLKK=64)."""
+    """SpargeAttn's `qattn` extension module holds its sm80 / sm90 kernels.  The sm90 entry (BLKQ=64, BLKK=128) runs the fused
+    kernel on those blocks; the sm80 kernels have no counterpart here."""
+
+    @staticmethod
+    def qk_int8_sv_f8_accum_f32_block_sparse_attn_inst_buf_fuse_v_scale_with_pv_threshold_sm90(
+            q_int8, k_int8, v_fp8, o, lut, valid_block_num, pvthreshold, q_scale, k_scale, v_scale, tensor_layout=1,
+            is_causal=False, qk_quant_gran=1, sm_scale=None, return_lse=0):
+        """The Hopper entry (SLA/core.py:226-229), BLKQ=64 / BLKK=128: see _sparse_only_attn.  The argument list is taken to
+        be the Sage2++ entry's, as recorded in SURVEY.md section 2.2; the SpargeAttn sources are not in this tree, so that
+        signature is unverified."""
+        return _sparse_only_attn(q_int8, k_int8, v_fp8, o, lut, q_scale, k_scale, sm_scale, *SAGE_BLOCKS["sm90"])
 
     def __getattr__(self, name):
-        raise NotImplementedError(f"SLA.core.qattn.{name}: the sm80/sm90 SpargeAttn kernels have no counterpart here; "
-                                  "call the Sage2++ entry, which runs the fused kernel")
+        raise NotImplementedError(f"SLA.core.qattn.{name}: the sm80 SpargeAttn kernels have no counterpart here; "
+                                  "call the Sage2++ entry or qattn's sm90 entry, which run the fused kernel")
 
 
 qattn = _QattnShim()

@@ -10,16 +10,30 @@ def cdiv(a, b):
     return (a + b - 1) // b
 
 
-# The SpargeAttn kernel family this package serves on every GPU it runs on (see get_cuda_arch).
+# The SpargeAttn kernel family this package serves (see get_cuda_arch); changed with set_served_arch().
 SERVED_ARCH = "sm100"
+SAGE_BLOCKS = {"sm100": (128, 64), "sm90": (64, 128)}   # (BLKQ, BLKK) of each family, SLA/core.py:191-193
+
+
+def set_served_arch(arch: str) -> str:
+    """Select the SpargeAttn kernel family get_cuda_arch reports, and with it SageSLA's block sizes: "sm100" (the default,
+    the Sage2++ family, BLKQ=128 / BLKK=64) or "sm90" (the Hopper family the reference picks on an H100, BLKQ=64 /
+    BLKK=128).  Returns the previous value.  Both families run on the H100; sequence parallelism (dist.py) serves "sm100"
+    only and raises NotImplementedError, at install and at every call, while "sm90" is set."""
+    global SERVED_ARCH
+    if arch not in SAGE_BLOCKS:
+        raise ValueError(f"served arch must be one of {sorted(SAGE_BLOCKS)}, got {arch!r}")
+    prev, SERVED_ARCH = SERVED_ARCH, arch
+    return prev
 
 
 def get_cuda_arch(device_index):
     """SLA/utils.py:70-71.  The reference (SLA/core.py:191-193, 211-235) and the LTX client (acceleration.py:286-378) use this
     value only to choose a SpargeAttn kernel family and its block sizes: sm80/86/87 -> fp16-V kernels, sm90 -> the
     BLKQ=64 / BLKK=128 Hopper kernels, anything else -> the Sage2++ entry with BLKQ=128 / BLKK=64.  This package implements
-    the last family (as the fused kernel) on every GPU, H100 included, so it reports that family's tag and callers take the
-    branch whose entry points exist here.  The device's compute capability is torch.cuda.get_device_capability()."""
+    the last two (as the fused kernel) on every GPU, H100 included, and reports the one chosen with set_served_arch()
+    ("sm100" unless changed), so callers take a branch whose entry points exist here.  The device's compute capability is
+    torch.cuda.get_device_capability()."""
     torch.cuda.get_device_capability(device_index)   # an invalid device index raises like the reference's call
     return SERVED_ARCH
 
@@ -29,17 +43,17 @@ class QKPrep:
     __slots__ = ("kmean", "q_i8", "q_scale", "k_i8", "k_scale", "q_pool", "k_pool", "mblk", "nblk", "k_seq_major")
 
 
-def quant_qk(q: torch.Tensor, k: torch.Tensor, lk: int = None) -> QKPrep:
+def quant_qk(q: torch.Tensor, k: torch.Tensor, lk: int = None, blkq: int = 128, blkk: int = 64) -> QKPrep:
     """One pass over q, two over k: key mean, pooled block means (SLA/utils.py:21-52), Sage INT8 Q / smoothed-K
     (SLA/core.py:197-203).  q [B, Lq, H, D], k [B, >=lk, H, D] contiguous bf16/fp16; only the first `lk` key rows are
-    used (sequence-parallel callers pass the gathered, tail-padded key slab)."""
+    used (sequence-parallel callers pass the gathered, tail-padded key slab).  (blkq, blkk): (128, 64) or (64, 128)."""
     require_cuda(q, k)
     b, lq, h, d = q.shape
     lk = k.shape[1] if lk is None else lk
     assert k.shape[0] == b and k.shape[2:] == q.shape[2:] and lk <= k.shape[1]
     assert q.is_contiguous() and k.is_contiguous() and (b == 1 or lk == k.shape[1])
     dev = q.device
-    mblk, nblk = cdiv(lq, 128), cdiv(lk, 64)
+    mblk, nblk = cdiv(lq, blkq), cdiv(lk, blkk)
     o = QKPrep()
     o.mblk, o.nblk = mblk, nblk
     o.kmean = torch.empty(b, h, d, dtype=torch.float32, device=dev)
@@ -49,39 +63,42 @@ def quant_qk(q: torch.Tensor, k: torch.Tensor, lk: int = None) -> QKPrep:
     o.k_scale = torch.empty(b, h, nblk, dtype=torch.float32, device=dev)
     o.q_pool = torch.empty(b, h, mblk, d, dtype=q.dtype, device=dev)
     o.k_pool = torch.empty(b, h, nblk, d, dtype=q.dtype, device=dev)
-    check(lib().tdb200_sla_quant_qk(ptr(q), ptr(k), DTYPE_TAG[q.dtype], b, lq, lk, h, d, ptr(o.kmean), ptr(o.q_i8),
-                                    ptr(o.q_scale), ptr(o.k_i8), ptr(o.k_scale), ptr(o.q_pool), ptr(o.k_pool),
-                                    stream_ptr(dev)), "sla_quant_qk")
+    check(lib().tdb200_sla_quant_qk_blocks(ptr(q), ptr(k), DTYPE_TAG[q.dtype], b, lq, lk, h, d, ptr(o.kmean), ptr(o.q_i8),
+                                           ptr(o.q_scale), ptr(o.k_i8), ptr(o.k_scale), ptr(o.q_pool), ptr(o.k_pool), blkq, blkk,
+                                           stream_ptr(dev)), "sla_quant_qk_blocks")
     return o
 
 
-def quant_q_only(q: torch.Tensor) -> QKPrep:
+def quant_q_only(q: torch.Tensor, blkq: int = 128) -> QKPrep:
     """The query half of quant_qk (pooled means + Sage INT8 of q); fill in the key half later with quant_k_into()."""
     require_cuda(q)
     b, lq, h, d = q.shape
     dev = q.device
     o = QKPrep()
-    o.mblk = cdiv(lq, 128)
+    o.mblk = cdiv(lq, blkq)
     o.q_i8 = torch.empty(b, h, lq, d, dtype=torch.int8, device=dev)
     o.q_scale = torch.empty(b, h, o.mblk, dtype=torch.float32, device=dev)
     o.q_pool = torch.empty(b, h, o.mblk, d, dtype=q.dtype, device=dev)
-    check(lib().tdb200_sla_quant_qk(ptr(q), None, DTYPE_TAG[q.dtype], b, lq, lq, h, d, None, ptr(o.q_i8), ptr(o.q_scale), None,
-                                    None, ptr(o.q_pool), None, stream_ptr(dev)), "sla_quant_qk", launches=1)
+    # the key block size only matters to the key half; any valid pair with this blkq serves
+    check(lib().tdb200_sla_quant_qk_blocks(ptr(q), None, DTYPE_TAG[q.dtype], b, lq, lq, h, d, None, ptr(o.q_i8), ptr(o.q_scale),
+                                           None, None, ptr(o.q_pool), None, blkq, 64 if blkq == 128 else 128, stream_ptr(dev)),
+          "sla_quant_qk_blocks", launches=1)
     return o
 
 
-def quant_k_into(o: QKPrep, k: torch.Tensor, lk: int) -> QKPrep:
+def quant_k_into(o: QKPrep, k: torch.Tensor, lk: int, blkk: int = 64) -> QKPrep:
     """The key half of quant_qk on the first `lk` rows of k [B, >=lk, H, D]."""
     require_cuda(k)
     b, _, h, d = k.shape
     dev = k.device
-    o.nblk = cdiv(lk, 64)
+    o.nblk = cdiv(lk, blkk)
     o.kmean = torch.empty(b, h, d, dtype=torch.float32, device=dev)
     o.k_i8 = torch.empty(b, h, lk, d, dtype=torch.int8, device=dev)
     o.k_scale = torch.empty(b, h, o.nblk, dtype=torch.float32, device=dev)
     o.k_pool = torch.empty(b, h, o.nblk, d, dtype=k.dtype, device=dev)
-    check(lib().tdb200_sla_quant_qk(None, ptr(k), DTYPE_TAG[k.dtype], b, lk, lk, h, d, ptr(o.kmean), None, None, ptr(o.k_i8),
-                                    ptr(o.k_scale), None, ptr(o.k_pool), stream_ptr(dev)), "sla_quant_qk", launches=3)
+    check(lib().tdb200_sla_quant_qk_blocks(None, ptr(k), DTYPE_TAG[k.dtype], b, lk, lk, h, d, ptr(o.kmean), None, None,
+                                           ptr(o.k_i8), ptr(o.k_scale), None, ptr(o.k_pool), 128 if blkk == 64 else 64, blkk,
+                                           stream_ptr(dev)), "sla_quant_qk_blocks", launches=3)
     return o
 
 
@@ -147,9 +164,10 @@ def mean_pool(x: torch.Tensor, BLK: int) -> torch.Tensor:
 def get_block_map(q: torch.Tensor, k: torch.Tensor, topk_ratio: float, BLKQ: int = 128, BLKK: int = 64):
     """SLA/utils.py:55-67.  q,k [B, H, L, D].  Returns (sparse_map int8, lut int32 [B,H,Mblk,topk] ascending, topk).
     NOTE the reference returns the unsorted torch.topk indices (int64) as `lut`; only the SET is defined
-    (sorted=False), and SageSLA rebuilds an ascending LUT from the map anyway (SLA/core.py:204)."""
-    assert (BLKQ, BLKK) == (128, 64), "this implementation uses the block sizes BLKQ=128, BLKK=64 on every architecture (SLA/core.py:191-193)"
-    prep = quant_qk(q.transpose(1, 2).contiguous(), k.transpose(1, 2).contiguous())
+    (sorted=False), and SageSLA rebuilds an ascending LUT from the map anyway (SLA/core.py:204).  (BLKQ, BLKK) is one of the
+    two SageSLA families, (128, 64) or (64, 128) (SLA/core.py:191-193)."""
+    assert (BLKQ, BLKK) in SAGE_BLOCKS.values(), f"block sizes BLKQ={BLKQ}, BLKK={BLKK}: this implementation serves (128, 64) and (64, 128)"
+    prep = quant_qk(q.transpose(1, 2).contiguous(), k.transpose(1, 2).contiguous(), blkq=BLKQ, blkk=BLKK)
     nblk = prep.nblk
     topk = min(nblk, int(topk_ratio * nblk))
     sparse_map, lut = block_map_from_pools(prep.q_pool, prep.k_pool, topk)

@@ -12,11 +12,14 @@ import sys
 __version__ = "0.1.0"
 
 
-def install() -> None:
+def install(sage_arch: str = "sm100") -> None:
     """Register this package under the reference's module names so unmodified reference code
     (`from ops import FastLayerNorm, FastRMSNorm, Int8Linear`, `from SLA import ...`, `import turbo_diffusion_ops`;
-    turbodiffusion/inference/modify_model.py:33-37) resolves to this implementation."""
+    turbodiffusion/inference/modify_model.py:33-37) resolves to this implementation.  `sage_arch` is handed to
+    SLA.utils.set_served_arch: "sm90" gives SageSLA the block sizes the reference uses on an H100 (BLKQ=64, BLKK=128)."""
     from . import ops, SLA, turbo_diffusion_ops
+    from .SLA.utils import set_served_arch
+    set_served_arch(sage_arch)
     for name, mod in (("turbo_diffusion_ops", turbo_diffusion_ops), ("ops", ops), ("SLA", SLA),
                       ("turbodiffusion.ops", ops), ("turbodiffusion.SLA", SLA)):
         sys.modules[name] = mod

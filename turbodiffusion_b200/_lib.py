@@ -56,6 +56,9 @@ _PROTOS = {
     "tdb200_sla_attn_fwd_qk16": [_P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_sla_attn_fwd_v2": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F, _I,
                                _P],
+    "tdb200_sla_quant_qk_blocks": [_P, _P, _I, _I64, _I64, _I64, _I64, _I64, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _P],
+    "tdb200_sla_attn_fwd_blocks": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F,
+                                   _I, _I64, _I64, _P],
     "tdb200_ltx_modulated_rms_norm_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_ltx_modulate_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
     "tdb200_ltx_gated_residual_ada": [_P, _P, _I, _P, _P, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
@@ -125,7 +128,7 @@ class _DeviceGuarded:
 
 
 LAUNCHES = 0  # kernels launched through the C ABI (each entry point documents how many it enqueues)
-_KERNELS_PER_CALL = {"sla_quant_qk": 4, "layernorm_modulate_quant": 2}  # upper bounds per entry point
+_KERNELS_PER_CALL = {"sla_quant_qk": 4, "sla_quant_qk_blocks": 4, "layernorm_modulate_quant": 2}  # upper bounds per entry point
 
 
 def check(rc: int, what: str, launches: int = None) -> None:

@@ -164,12 +164,13 @@ __global__ void __launch_bounds__(ROWS* D / 64) pool_quant_kernel(const T* __res
   }
 }
 
-template <typename T, int D>
+// BQ / BK: query / key block rows, (128, 64) or (64, 128)
+template <typename T, int D, int BQ>
 int run_q(const void* q, int64_t b, int64_t lq, int64_t h, int8_t* q_i8, float* q_scale, void* q_pool, cudaStream_t st) {
-  const int mblk = static_cast<int>(cdiv64(lq, 128));
+  const int mblk = static_cast<int>(cdiv64(lq, BQ));
   dim3 gq(static_cast<unsigned>(h), mblk, static_cast<unsigned>(b));
-  pool_quant_kernel<T, D, 128, false><<<gq, 128 * D / 64, 0, st>>>(static_cast<const T*>(q), nullptr, q_i8, q_scale,
-                                                                   static_cast<T*>(q_pool), lq, static_cast<int>(h), mblk, D, lq * D);
+  pool_quant_kernel<T, D, BQ, false><<<gq, BQ * D / 64, 0, st>>>(static_cast<const T*>(q), nullptr, q_i8, q_scale,
+                                                                 static_cast<T*>(q_pool), lq, static_cast<int>(h), mblk, D, lq * D);
   return check_launch("pool_quant_kernel<q>");
 }
 
@@ -182,18 +183,18 @@ int run_kmean_partial(const void* k, int64_t b, int64_t l, int64_t h, float* par
 }
 
 // seq_major: k_i8 keeps the input's [b, l, h, d] layout (what a sequence-parallel rank all-gathers) instead of [b, h, l, d]
-template <typename T, int D>
+template <typename T, int D, int BK = 64>
 int run_k_quant(const void* k, int64_t b, int64_t l, int64_t h, const float* kmean, int8_t* k_i8, float* k_scale, void* k_pool,
                 bool seq_major, cudaStream_t st) {
-  const int nblk = static_cast<int>(cdiv64(l, 64));
+  const int nblk = static_cast<int>(cdiv64(l, BK));
   dim3 gk(static_cast<unsigned>(h), nblk, static_cast<unsigned>(b));
-  pool_quant_kernel<T, D, 64, true><<<gk, 64 * D / 64, 0, st>>>(static_cast<const T*>(k), kmean, k_i8, k_scale,
+  pool_quant_kernel<T, D, BK, true><<<gk, BK * D / 64, 0, st>>>(static_cast<const T*>(k), kmean, k_i8, k_scale,
                                                                 static_cast<T*>(k_pool), l, static_cast<int>(h), nblk,
                                                                 seq_major ? h * D : D, seq_major ? D : l * D);
   return check_launch("pool_quant_kernel<k>");
 }
 
-template <typename T, int D>
+template <typename T, int D, int BK>
 int run_k(const void* k, int64_t b, int64_t l, int64_t h, float* kmean, int8_t* k_i8, float* k_scale, void* k_pool,
           cudaStream_t st) {
   const int chunks = static_cast<int>(cdiv64(l, kMeanRows));
@@ -203,36 +204,36 @@ int run_k(const void* k, int64_t b, int64_t l, int64_t h, float* kmean, int8_t* 
   if (int rc = run_kmean_partial<T, D>(k, b, l, h, partial, st)) return rc;
   kmean_final_kernel<<<static_cast<unsigned>(b * h), 1024, 0, st>>>(partial, kmean, l, chunks, D);
   if (int rc = check_launch("kmean_final_kernel")) return rc;
-  return run_k_quant<T, D>(k, b, l, h, kmean, k_i8, k_scale, k_pool, false, st);
+  return run_k_quant<T, D, BK>(k, b, l, h, kmean, k_i8, k_scale, k_pool, false, st);
 }
 
-template <typename T, int D>
+template <typename T, int D, int BQ, int BK>
 int run(const void* q, const void* k, int64_t b, int64_t lq, int64_t l, int64_t h, float* kmean, int8_t* q_i8,
         float* q_scale, int8_t* k_i8, float* k_scale, void* q_pool, void* k_pool, cudaStream_t st) {
   if (q != nullptr)
-    if (int rc = run_q<T, D>(q, b, lq, h, q_i8, q_scale, q_pool, st)) return rc;
+    if (int rc = run_q<T, D, BQ>(q, b, lq, h, q_i8, q_scale, q_pool, st)) return rc;
   if (k != nullptr)
-    if (int rc = run_k<T, D>(k, b, l, h, kmean, k_i8, k_scale, k_pool, st)) return rc;
+    if (int rc = run_k<T, D, BK>(k, b, l, h, kmean, k_i8, k_scale, k_pool, st)) return rc;
   return TDB200_OK;
 }
 
-}  // namespace
-
-extern "C" int tdb200_sla_quant_qk(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int64_t l, int64_t h,
-                                   int64_t d, float* kmean, int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale,
-                                   void* q_pool, void* k_pool, void* stream) {
-  using namespace tdb;
+// (blkq, blkk) is (128, 64) or (64, 128); the callers check it
+int quant_qk(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int64_t l, int64_t h, int64_t d, float* kmean,
+             int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale, void* q_pool, void* k_pool, int64_t blkq, int64_t blkk,
+             void* stream) {
   if ((!q && !k) || (q && (!q_i8 || !q_scale || !q_pool)) || (k && (!kmean || !k_i8 || !k_scale || !k_pool)))
     return fail(TDB200_ERR_INVALID_ARG, "sla_quant_qk: null pointer");
   if (b <= 0 || l <= 0 || lq <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_quant_qk: bad shape");
   if (d != 64 && d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_qk: head dim %lld (64 or 128, SLA/core.py:207)", (long long)d);
-  if (h > 65535 || b > 65535 || cdiv64(l, 64) > 65535 || cdiv64(lq, 128) > 65535)
+  if (h > 65535 || b > 65535 || cdiv64(l, blkk) > 65535 || cdiv64(lq, blkq) > 65535)
     return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_qk: h, b or sequence length too large");
   if ((q && (!aligned16(q) || !aligned16(q_i8))) || (k && (!aligned16(k) || !aligned16(k_i8))))
     return fail(TDB200_ERR_INVALID_ARG, "sla_quant_qk: buffers must be 16-byte aligned");
   if (int rc = require_sm90()) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define TDB_RUN(T, D) return run<T, D>(q, k, b, lq, l, h, kmean, q_i8, q_scale, k_i8, k_scale, q_pool, k_pool, st)
+#define TDB_RUN(T, D)                                                                                                    \
+  return blkq == 128 ? run<T, D, 128, 64>(q, k, b, lq, l, h, kmean, q_i8, q_scale, k_i8, k_scale, q_pool, k_pool, st)    \
+                     : run<T, D, 64, 128>(q, k, b, lq, l, h, kmean, q_i8, q_scale, k_i8, k_scale, q_pool, k_pool, st)
   if (dtype == TDB200_DTYPE_BF16) {
     if (d == 128) TDB_RUN(__nv_bfloat16, 128);
     TDB_RUN(__nv_bfloat16, 64);
@@ -242,6 +243,26 @@ extern "C" int tdb200_sla_quant_qk(const void* q, const void* k, int dtype, int6
   }
 #undef TDB_RUN
   return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_qk: dtype tag %d", dtype);
+}
+
+}  // namespace
+
+extern "C" int tdb200_sla_quant_qk(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int64_t l, int64_t h,
+                                   int64_t d, float* kmean, int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale,
+                                   void* q_pool, void* k_pool, void* stream) {
+  return quant_qk(q, k, dtype, b, lq, l, h, d, kmean, q_i8, q_scale, k_i8, k_scale, q_pool, k_pool, 128, 64, stream);
+}
+
+// tdb200_sla_quant_qk with the block geometry chosen by the caller: Q pooled / quantised per blkq rows, smoothed K per blkk rows,
+// (blkq, blkk) = (128, 64) or (64, 128).  The key mean is the same (its 128-row partials do not depend on the block size).
+extern "C" int tdb200_sla_quant_qk_blocks(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int64_t l, int64_t h,
+                                          int64_t d, float* kmean, int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale,
+                                          void* q_pool, void* k_pool, int64_t blkq, int64_t blkk, void* stream) {
+  using namespace tdb;
+  if (!((blkq == 128 && blkk == 64) || (blkq == 64 && blkk == 128)))
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_qk_blocks: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 128)",
+                (long long)blkq, (long long)blkk);
+  return quant_qk(q, k, dtype, b, lq, l, h, d, kmean, q_i8, q_scale, k_i8, k_scale, q_pool, k_pool, blkq, blkk, stream);
 }
 
 // ---- the key half split in three, for sequence-parallel ranks (dist.py): each rank reduces ITS rows to 128-row partial sums,
@@ -284,7 +305,7 @@ extern "C" int tdb200_sla_quant_k_seq(const void* k, const float* kmean, int dty
   if (!aligned16(k) || !aligned16(k_i8)) return fail(TDB200_ERR_INVALID_ARG, "sla_quant_k_seq: buffers must be 16-byte aligned");
   if (int rc = require_sm90()) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define TDB_RUN(T, D) return run_k_quant<T, D>(k, b, l, h, kmean, k_i8, k_scale, k_pool, true, st)
+#define TDB_RUN(T, D) return run_k_quant<T, D, 64>(k, b, l, h, kmean, k_i8, k_scale, k_pool, true, st)
   if (dtype == TDB200_DTYPE_BF16) {
     if (d == 128) TDB_RUN(__nv_bfloat16, 128);
     TDB_RUN(__nv_bfloat16, 64);

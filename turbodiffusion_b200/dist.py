@@ -32,9 +32,19 @@ from typing import Optional
 import torch
 import torch.distributed as dist
 
+from .SLA import utils as sla_utils
+
 
 def cdiv(a: int, b: int) -> int:
     return (a + b - 1) // b
+
+
+def require_default_sage_blocks() -> None:
+    """Every path here (quant_k_seq, attn_fwd_kseq, SPAttention's nblk, the Ulysses prims) works on the sm100 SageSLA family's
+    64-row key blocks; refuse, at install and at every call, rather than run it while a single GPU would run 64/128 blocks."""
+    if sla_utils.SERVED_ARCH != "sm100":
+        raise NotImplementedError(f"sequence parallelism serves the sm100 SageSLA family (BLKQ=128, BLKK=64) only; the "
+                                  f"served arch is {sla_utils.SERVED_ARCH!r} (SLA.utils.set_served_arch)")
 
 
 def shard_rows(total_rows: int, world: int, rank: int, align: int = 128):
@@ -189,6 +199,7 @@ class SPAttention:
         self._pending = (kx, v_full.unsqueeze(0), kv, ksum, works + [wv] + red)
 
     def __call__(self, q, k, v):
+        require_default_sage_blocks()
         sp = self.sp
         dtype = q.dtype
         q = q.to(self._cdt(q)).contiguous()
@@ -295,6 +306,7 @@ class UlyssesAttention:
         return get
 
     def __call__(self, q, k, v):
+        require_default_sage_blocks()
         sp, w = self.sp, self.sp.world
         dtype = q.dtype
         for name, t in (("q", q), ("k", k), ("v", v)):
@@ -356,6 +368,7 @@ class UnevenUlyssesAttention(UlyssesAttention):
         self._pending[name] = (recv.view(sp.total_rows, mine, d), work)
 
     def __call__(self, q, k, v):
+        require_default_sage_blocks()
         sp = self.sp
         dtype = q.dtype
         for name, t in (("q", q), ("k", k), ("v", v)):
@@ -400,6 +413,7 @@ class SequenceParallel:
         `WanSelfAttention.attn_op.local_attn`, inference/modify_model.py:48-52).  Returns the mode used:
         "allgather" (K/V all-gather + moment all-reduce, any head count) or "ulysses" (head<->sequence all-to-all; with
         heads % world != 0 the uneven-split variant)."""
+        require_default_sage_blocks()
         used = None
         for blk in model.blocks:
             used = self.pick_mode(blk.heads, mode)

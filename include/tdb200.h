@@ -234,6 +234,18 @@ int tdb200_sla_attn_fwd_blocks(const int8_t* q_i8, const float* q_scale, const i
                                const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk, const void* kvw,
                                const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
                                int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq, int64_t blkk, void* stream);
+/* The sequence-parallel key half on either block family (the gathered key mean and its 128-row partials serve both):
+ *   tdb200_sla_quant_k_seq_blocks   tdb200_sla_quant_k_seq pooling / quantising per blkk rows, blkk = 64 or 128: k_i8 in the
+ *                                   input layout [b,l,h,d], k_scale [b,h,ceil(l/blkk)], k_pool [b,h,ceil(l/blkk),d]; 64 is
+ *                                   tdb200_sla_quant_k_seq itself.
+ *   tdb200_sla_attn_fwd_kseq_blocks tdb200_sla_attn_fwd_kseq on (blkq, blkk) = (128, 64), which is that call itself, or (64, 128);
+ *                                   d = 128, softmax map, b = 1, k_i8 in [1,lk,h,d].  Other pairs return TDB200_ERR_UNSUPPORTED. */
+int tdb200_sla_quant_k_seq_blocks(const void* k, const float* kmean, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
+                                  int8_t* k_i8, float* k_scale, void* k_pool, int64_t blkk, void* stream);
+int tdb200_sla_attn_fwd_kseq_blocks(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
+                                    const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk, const void* kvw,
+                                    const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
+                                    int64_t h, int64_t d, float sm_scale, int64_t blkq, int64_t blkk, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * a12. LTX-2 (TurboT2AV) prologue variants   (ltx_core/model/transformer/transformer.py:21-94; Triton fast path

@@ -63,11 +63,12 @@ def _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, featu
     lk = v.shape[1] if lk is None else lk
     out = torch.empty_like(q)
     if getattr(prep, "k_seq_major", False):   # INT8 K in the gathered [B, Lk, H, D] layout (dist.py)
-        if d != 128 or feature != 0 or (blkq, blkk) != (128, 64):
-            raise NotImplementedError("sequence-major INT8 K is served by the 128-wide softmax kernel on 128x64 blocks only")
-        check(lib().tdb200_sla_attn_fwd_kseq(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v),
-                                             ptr(q), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b),
-                                             ptr(out), b, l, lk, h, d, float(sm_scale), stream_ptr(q.device)), "sla_attn_fwd")
+        if d != 128 or feature != 0:
+            raise NotImplementedError("sequence-major INT8 K is served by the 128-wide softmax kernels only")
+        check(lib().tdb200_sla_attn_fwd_kseq_blocks(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v),
+                                                    ptr(q), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b),
+                                                    ptr(out), b, l, lk, h, d, float(sm_scale), blkq, blkk, stream_ptr(q.device)),
+              "sla_attn_fwd")
     else:   # head-major INT8 K: head dims 64 and 128, every feature map, both block geometries
         check(lib().tdb200_sla_attn_fwd_blocks(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v),
                                                ptr(q), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b),

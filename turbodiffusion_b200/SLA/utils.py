@@ -18,8 +18,9 @@ SAGE_BLOCKS = {"sm100": (128, 64), "sm90": (64, 128)}   # (BLKQ, BLKK) of each f
 def set_served_arch(arch: str) -> str:
     """Select the SpargeAttn kernel family get_cuda_arch reports, and with it SageSLA's block sizes: "sm100" (the default,
     the Sage2++ family, BLKQ=128 / BLKK=64) or "sm90" (the Hopper family the reference picks on an H100, BLKQ=64 /
-    BLKK=128).  Returns the previous value.  Both families run on the H100; sequence parallelism (dist.py) serves "sm100"
-    only and raises NotImplementedError, at install and at every call, while "sm90" is set."""
+    BLKK=128).  Returns the previous value.  Both families run on the H100.  Sequence parallelism (dist.py) serves both:
+    its hooks are built for one family (`SequenceParallel.install(model, mode, sage_arch=...)`, "sm100" by default) and
+    raise NotImplementedError, at install and at every call, while the served arch names the other."""
     global SERVED_ARCH
     if arch not in SAGE_BLOCKS:
         raise ValueError(f"served arch must be one of {sorted(SAGE_BLOCKS)}, got {arch!r}")
@@ -124,17 +125,17 @@ def kmean_from_partials(partials: torch.Tensor, l_total: int) -> torch.Tensor:
     return out
 
 
-def quant_k_seq(k: torch.Tensor, kmean: torch.Tensor, k_i8=None):
-    """Smoothed Sage INT8 of the rows of k [B, rows, H, D] against a given key mean: (k_i8 [B, rows, H, D] int8 -- the input
-    layout --, k_scale [B, H, ceil(rows/64)] fp32, k_pool [B, H, ceil(rows/64), D])."""
+def quant_k_seq(k: torch.Tensor, kmean: torch.Tensor, k_i8=None, blkk: int = 64):
+    """Smoothed Sage INT8 of the rows of k [B, rows, H, D] against a given key mean, per `blkk` (64 or 128) rows: (k_i8
+    [B, rows, H, D] int8 -- the input layout --, k_scale [B, H, ceil(rows/blkk)] fp32, k_pool [B, H, ceil(rows/blkk), D])."""
     require_cuda(k, kmean)
     b, rows, h, d = k.shape
-    nb = cdiv(rows, 64)
+    nb = cdiv(rows, blkk)
     k_i8 = torch.empty(b, rows, h, d, dtype=torch.int8, device=k.device) if k_i8 is None else k_i8
     k_scale = torch.empty(b, h, nb, dtype=torch.float32, device=k.device)
     k_pool = torch.empty(b, h, nb, d, dtype=k.dtype, device=k.device)
-    check(lib().tdb200_sla_quant_k_seq(ptr(k), ptr(kmean), DTYPE_TAG[k.dtype], b, rows, h, d, ptr(k_i8), ptr(k_scale),
-                                       ptr(k_pool), stream_ptr(k.device)), "sla_quant_k_seq")
+    check(lib().tdb200_sla_quant_k_seq_blocks(ptr(k), ptr(kmean), DTYPE_TAG[k.dtype], b, rows, h, d, ptr(k_i8), ptr(k_scale),
+                                              ptr(k_pool), blkk, stream_ptr(k.device)), "sla_quant_k_seq")
     return k_i8, k_scale, k_pool
 
 

@@ -59,6 +59,9 @@ _PROTOS = {
     "tdb200_sla_quant_qk_blocks": [_P, _P, _I, _I64, _I64, _I64, _I64, _I64, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _P],
     "tdb200_sla_attn_fwd_blocks": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F,
                                    _I, _I64, _I64, _P],
+    "tdb200_sla_quant_k_seq_blocks": [_P, _P, _I, _I64, _I64, _I64, _I64, _P, _P, _P, _I64, _P],
+    "tdb200_sla_attn_fwd_kseq_blocks": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64,
+                                        _F, _I64, _I64, _P],
     "tdb200_ltx_modulated_rms_norm_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_ltx_modulate_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
     "tdb200_ltx_gated_residual_ada": [_P, _P, _I, _P, _P, _I, _I, _P, _I64, _I64, _I64, _I64, _P],

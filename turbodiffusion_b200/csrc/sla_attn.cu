@@ -711,6 +711,30 @@ extern "C" int tdb200_sla_attn_fwd_kseq(const int8_t* q_i8, const float* q_scale
                             true, stream);
 }
 
+// tdb200_sla_attn_fwd_kseq with the block geometry chosen by the caller: (128, 64) is tdb200_sla_attn_fwd_kseq itself, (64, 128)
+// runs sla_attn_fwd_q64_kernel.  Its producer loads K at (0, blk*BK, head, b) over the dims (d, lk, h, b), so the sequence-major
+// layout is only a different set of tensor-map strides.
+extern "C" int tdb200_sla_attn_fwd_kseq_blocks(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
+                                               const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk,
+                                               const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
+                                               int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, int64_t blkq,
+                                               int64_t blkk, void* stream) {
+  const bool hopper = blkq == kHopperBlkQ && blkk == kHopperBlkK;
+  if (!hopper && !(blkq == BLKQ && blkk == BLKK))
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_kseq_blocks: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 128)",
+                (long long)blkq, (long long)blkk);
+  if (!hopper)
+    return tdb200_sla_attn_fwd_kseq(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, d,
+                                    sm_scale, stream);
+  if (int rc = check_common(q_i8, k_i8, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
+  if (!q_scale || !k_scale) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: null pointer");
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (this kernel implements d=128)", (long long)d);
+  if (b != 1)
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_kseq: batch %lld (the gathered [lk_pad, h, d] key slab is one sequence)", (long long)b);
+  return launch<128, false, kHopperBlkQ, kHopperBlkK>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out,
+                                                      b, l, lk, h, sm_scale, 0, true, stream);
+}
+
 extern "C" int tdb200_sla_attn_fwd_qk16(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
                                         const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
                                         int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {

@@ -295,17 +295,21 @@ extern "C" int tdb200_sla_kmean_final(const float* partial, int64_t b, int64_t h
   return check_launch("kmean_final_kernel");
 }
 
-extern "C" int tdb200_sla_quant_k_seq(const void* k, const float* kmean, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
-                                      int8_t* k_i8, float* k_scale, void* k_pool, void* stream) {
+extern "C" int tdb200_sla_quant_k_seq_blocks(const void* k, const float* kmean, int dtype, int64_t b, int64_t l, int64_t h,
+                                             int64_t d, int8_t* k_i8, float* k_scale, void* k_pool, int64_t blkk, void* stream) {
   using namespace tdb;
+  if (blkk != 64 && blkk != 128)
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_k_seq_blocks: key block size %lld (BLKK = 64 or 128)", (long long)blkk);
   if (!k || !kmean || !k_i8 || !k_scale || !k_pool) return fail(TDB200_ERR_INVALID_ARG, "sla_quant_k_seq: null pointer");
   if (b <= 0 || l <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_quant_k_seq: bad shape");
   if (d != 64 && d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_k_seq: head dim %lld (64 or 128)", (long long)d);
-  if (h > 65535 || b > 65535 || cdiv64(l, 64) > 65535) return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_k_seq: dimension too large");
+  if (h > 65535 || b > 65535 || cdiv64(l, blkk) > 65535) return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_k_seq: dimension too large");
   if (!aligned16(k) || !aligned16(k_i8)) return fail(TDB200_ERR_INVALID_ARG, "sla_quant_k_seq: buffers must be 16-byte aligned");
   if (int rc = require_sm90()) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define TDB_RUN(T, D) return run_k_quant<T, D, 64>(k, b, l, h, kmean, k_i8, k_scale, k_pool, true, st)
+#define TDB_RUN(T, D)                                                                                 \
+  return blkk == 64 ? run_k_quant<T, D, 64>(k, b, l, h, kmean, k_i8, k_scale, k_pool, true, st)      \
+                    : run_k_quant<T, D, 128>(k, b, l, h, kmean, k_i8, k_scale, k_pool, true, st)
   if (dtype == TDB200_DTYPE_BF16) {
     if (d == 128) TDB_RUN(__nv_bfloat16, 128);
     TDB_RUN(__nv_bfloat16, 64);
@@ -315,4 +319,9 @@ extern "C" int tdb200_sla_quant_k_seq(const void* k, const float* kmean, int dty
   }
 #undef TDB_RUN
   return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_k_seq: dtype tag %d", dtype);
+}
+
+extern "C" int tdb200_sla_quant_k_seq(const void* k, const float* kmean, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
+                                      int8_t* k_i8, float* k_scale, void* k_pool, void* stream) {
+  return tdb200_sla_quant_k_seq_blocks(k, kmean, dtype, b, l, h, d, k_i8, k_scale, k_pool, 64, stream);
 }

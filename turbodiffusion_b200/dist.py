@@ -11,10 +11,17 @@ Every GEMM / norm / modulation / RoPE / FFN in the block is row-independent, so 
     3. the block map over all key blocks and the fused attention over the gathered K/V run locally for this rank's query rows
        (with the 16-bit K exchange also the key mean / INT8 / pooling of the WHOLE key sequence, repeated on every rank).
 
-Shard boundaries are multiples of 128 rows, so 128x128 quant blocks, 128-row query blocks and 64-row key blocks never
-straddle ranks and the result equals the single-GPU computation block for block.  Only the last rank may be short; the
+Shard boundaries are multiples of 128 rows, so 128x128 quant blocks and the SageSLA blocks of either family (128-row query
+and 64-row key blocks for "sm100", 64-row query and 128-row key blocks for "sm90"; 128 = max(BLKQ, BLKK) in both) never
+straddle ranks and the result equals the single-GPU computation block for block.  The key mean is built from 128-row
+partial sums in both families, so the gathered mean is the single-GPU one bit for bit.  Only the last rank may be short; the
 all-gather pads it with zero rows at the very END of the sequence, so the gathered slab is simply the full tensor followed
 by < 128*world padding rows that the kernels never read (lk = L).
+
+The hooks run the SageSLA block family they were built for (`sage_arch`, "sm100" by default): a sequence-parallel model
+under SLA.utils.set_served_arch("sm90") is installed with `SequenceParallel.install(model, mode, sage_arch="sm90")`.
+Installing, or calling a hook, while the served arch names the other family raises NotImplementedError, since the
+single-GPU module would then run one block geometry and the hooks the other.
 
 The reference's own scheme is Ulysses all-to-all (rcm/utils/a2a_cp.py:66-182; heads <-> sequence), which needs
 H % world == 0 (12 heads do not split 8 ways).  UlyssesAttention below implements it as the second mode: three all-to-alls
@@ -39,12 +46,23 @@ def cdiv(a: int, b: int) -> int:
     return (a + b - 1) // b
 
 
-def require_default_sage_blocks() -> None:
-    """Every path here (quant_k_seq, attn_fwd_kseq, SPAttention's nblk, the Ulysses prims) works on the sm100 SageSLA family's
-    64-row key blocks; refuse, at install and at every call, rather than run it while a single GPU would run 64/128 blocks."""
-    if sla_utils.SERVED_ARCH != "sm100":
-        raise NotImplementedError(f"sequence parallelism serves the sm100 SageSLA family (BLKQ=128, BLKK=64) only; the "
-                                  f"served arch is {sla_utils.SERVED_ARCH!r} (SLA.utils.set_served_arch)")
+def sage_blocks(sage_arch: str):
+    """(BLKQ, BLKK) of a SageSLA family, "sm100" or "sm90" (SLA.utils.SAGE_BLOCKS)."""
+    if sage_arch not in sla_utils.SAGE_BLOCKS:
+        raise ValueError(f"sage_arch must be one of {sorted(sla_utils.SAGE_BLOCKS)}, got {sage_arch!r}")
+    return sla_utils.SAGE_BLOCKS[sage_arch]
+
+
+def require_served_arch(sage_arch: str) -> None:
+    """Refuse, at install and at every hook call, to run `sage_arch`'s block sizes while a single GPU would run the other
+    family's (SLA.utils.set_served_arch)."""
+    served = sla_utils.SERVED_ARCH
+    if served != sage_arch:
+        bq, bk = sla_utils.SAGE_BLOCKS[sage_arch]
+        sq, sk = sla_utils.SAGE_BLOCKS[served]
+        raise NotImplementedError(f"sequence parallelism built for the {sage_arch} SageSLA family (BLKQ={bq}, BLKK={bk}) "
+                                  f"while the served arch is {served!r} (BLKQ={sq}, BLKK={sk}); install it with "
+                                  f"sage_arch={served!r} or select {sage_arch!r} with SLA.utils.set_served_arch")
 
 
 def shard_rows(total_rows: int, world: int, rank: int, align: int = 128):
@@ -62,27 +80,31 @@ class GpuPrimitives:
     `int8_k`: the rank quantises its OWN key rows and the exchange carries INT8 K (+ per-block scales and pooled means) instead
     of 16-bit K; the key mean stays global and bit-identical to the single-GPU one because the ranks all-gather the 128-row
     partial sums the single-GPU reduction is built from (tdb200_sla_kmean_partial / _final).  Served by the 128-wide softmax
-    kernel; other head dims / feature maps keep the 16-bit exchange."""
+    kernels of both block families; other head dims / feature maps keep the 16-bit exchange.  `sage_arch` selects the block
+    family (BLKQ, BLKK) every method works on."""
 
-    def __init__(self, sla_module):
+    def __init__(self, sla_module, sage_arch: str = "sm100"):
         self.sla = sla_module
+        self.sage_arch = sage_arch
+        self.blkq, self.blkk = sage_blocks(sage_arch)
         self.int8_k = (getattr(sla_module, "quantised_qk", True) and getattr(sla_module, "feature", 0) == 0
                        and os.environ.get("TDB200_SP_INT8_K", "1") != "0")       # "0": the 16-bit K exchange, for A/B timing
 
     def prepare_q(self, q):
         from .SLA.utils import quant_q_only
-        return quant_q_only(q)
+        return quant_q_only(q, self.blkq)
 
     def attention(self, q, k_full, v_full, lk, kv, ksum, qprep=None):
         from .SLA.core import attn_fwd, project_moments
         from .SLA.utils import block_map_from_pools, quant_k_into, quant_q_only
         sla = self.sla
         d = q.shape[-1]
-        prep = quant_k_into(qprep if qprep is not None else quant_q_only(q), k_full, lk)
+        prep = quant_k_into(qprep if qprep is not None else quant_q_only(q, self.blkq), k_full, lk, self.blkk)
         topk = min(prep.nblk, int(sla.topk * prep.nblk))
         _, lut = block_map_from_pools(prep.q_pool, prep.k_pool, topk)
         kvw = project_moments(sla.proj_l.weight, kv, q.dtype)
-        return attn_fwd(prep, v_full, q, lut, topk, kvw, ksum, sla.proj_l.bias.float().contiguous(), d ** -0.5, lk=lk)
+        return attn_fwd(prep, v_full, q, lut, topk, kvw, ksum, sla.proj_l.bias.float().contiguous(), d ** -0.5, lk=lk,
+                        blkq=self.blkq, blkk=self.blkk)
 
     def moments(self, k_local, v_local):
         from .SLA.core import linear_moments
@@ -99,20 +121,21 @@ class GpuPrimitives:
 
     def k_quant(self, k_local, kmean, k_i8_out=None):
         from .SLA.utils import quant_k_seq
-        return quant_k_seq(k_local, kmean, k_i8_out)
+        return quant_k_seq(k_local, kmean, k_i8_out, blkk=self.blkk)
 
     def attention_i8(self, q, qprep, k_i8_full, k_scale, k_pool, kmean, v_full, lk, kv, ksum):
         from .SLA.core import attn_fwd, project_moments
-        from .SLA.utils import block_map_from_pools, cdiv as _cdiv, quant_q_only
+        from .SLA.utils import block_map_from_pools, quant_q_only
         sla = self.sla
         d = q.shape[-1]
-        prep = qprep if qprep is not None else quant_q_only(q)
+        prep = qprep if qprep is not None else quant_q_only(q, self.blkq)
         prep.kmean, prep.k_i8, prep.k_scale, prep.k_pool = kmean, k_i8_full, k_scale, k_pool
-        prep.nblk, prep.k_seq_major = _cdiv(lk, 64), True
+        prep.nblk, prep.k_seq_major = cdiv(lk, self.blkk), True
         topk = min(prep.nblk, int(sla.topk * prep.nblk))
         _, lut = block_map_from_pools(prep.q_pool, prep.k_pool, topk)
         kvw = project_moments(sla.proj_l.weight, kv, q.dtype)
-        return attn_fwd(prep, v_full, q, lut, topk, kvw, ksum, sla.proj_l.bias.float().contiguous(), d ** -0.5, lk=lk)
+        return attn_fwd(prep, v_full, q, lut, topk, kvw, ksum, sla.proj_l.bias.float().contiguous(), d ** -0.5, lk=lk,
+                        blkq=self.blkq, blkk=self.blkk)
 
 
 class SPAttention:
@@ -122,10 +145,13 @@ class SPAttention:
     stream) and overlap with the V and Q projections, Q RMSNorm+RoPE and the Q-side quantisation that the block and __call__
     run before waiting on them.  With `prims.int8_k` the K exchange is: all-gather of the key-mean partials (tiny) -> global
     mean -> local smoothing / INT8 / pooling -> all-gather of INT8 K [rows, H, D], k_scale and k_pool; otherwise the 16-bit K
-    slab is gathered and every rank prepares the whole key sequence."""
+    slab is gathered and every rank prepares the whole key sequence.  `sage_arch` is the block family of `prims`; the scales
+    and pooled means travel per BLKK-row key block."""
 
-    def __init__(self, sp: "SequenceParallel", prims):
+    def __init__(self, sp: "SequenceParallel", prims, sage_arch: str = "sm100"):
         self.sp, self.prims = sp, prims
+        self.sage_arch = sage_arch
+        self.blocks = sage_blocks(sage_arch)
         self._bufs = {}
         self._pending = None
         self._pending_k = None
@@ -165,7 +191,7 @@ class SPAttention:
             self._pending_k = (k, ("bf16", k_full.unsqueeze(0)), [wk])
             return
         _, rows, h, d = k.shape
-        w, cp, nbp = sp.world, sp.rows_pad // 128, sp.rows_pad // 64
+        w, cp, nbp = sp.world, sp.rows_pad // 128, sp.rows_pad // self.blocks[1]
         part = self.prims.k_partials(k)                                        # [1, H, ceil(rows/128), D]
         recv, wp = self._gather_async("kpart", part[0].transpose(0, 1), cp)     # rows = chunks: [w*cp, H, D]
         wp.wait()
@@ -199,7 +225,7 @@ class SPAttention:
         self._pending = (kx, v_full.unsqueeze(0), kv, ksum, works + [wv] + red)
 
     def __call__(self, q, k, v):
-        require_default_sage_blocks()
+        require_served_arch(self.sage_arch)
         sp = self.sp
         dtype = q.dtype
         q = q.to(self._cdt(q)).contiguous()
@@ -214,7 +240,7 @@ class SPAttention:
             out = self.prims.attention(q, kx[1], v_full, sp.total_rows, kv, ksum, qprep)
         else:
             _, k8_full, ks_full, kp_full, kmean = kx
-            nblk = cdiv(sp.total_rows, 64)
+            nblk = cdiv(sp.total_rows, self.blocks[1])
             k_scale = ks_full[:nblk].transpose(0, 1).contiguous().unsqueeze(0)             # [1, H, nblk]
             k_pool = kp_full[:nblk].transpose(0, 1).contiguous().unsqueeze(0)              # [1, H, nblk, D]
             out = self.prims.attention_i8(q, qprep, k8_full, k_scale, k_pool, kmean, v_full, sp.total_rows, kv, ksum)
@@ -224,10 +250,12 @@ class SPAttention:
 class UlyssesGpuPrims:
     """Per-rank attention for the head<->sequence mode: the single-GPU SLA pipeline on this rank's heads, split so that each
     stage starts as soon as the tensor it needs has arrived (K: key mean + INT8 + pooled means; Q: INT8 + pooled means +
-    block map; V: linear moments + fused attention)."""
+    block map; V: linear moments + fused attention) on the blocks of `sage_arch`."""
 
-    def __init__(self, sla_module):
+    def __init__(self, sla_module, sage_arch: str = "sm100"):
         self.sla = sla_module
+        self.sage_arch = sage_arch
+        self.blkq, self.blkk = sage_blocks(sage_arch)
 
     def attend(self, get_q, get_k, get_v):
         from .SLA.core import attn_fwd, linear_moments, project_moments
@@ -237,9 +265,9 @@ class UlyssesGpuPrims:
         d = k.shape[-1]
         if d != 128:
             return sla(get_q(), k, get_v())
-        kp = quant_k_into(QKPrep(), k, k.shape[1])
+        kp = quant_k_into(QKPrep(), k, k.shape[1], self.blkk)
         q = get_q()
-        prep = quant_q_only(q)
+        prep = quant_q_only(q, self.blkq)
         for f in ("kmean", "k_i8", "k_scale", "k_pool", "nblk"):
             setattr(prep, f, getattr(kp, f))
         topk = min(prep.nblk, int(sla.topk * prep.nblk))
@@ -247,7 +275,8 @@ class UlyssesGpuPrims:
         v = get_v()
         kv, ksum = linear_moments(k, v)
         kvw = project_moments(sla.proj_l.weight, kv, q.dtype)
-        return attn_fwd(prep, v, q, lut, topk, kvw, ksum, sla.proj_l.bias.float().contiguous(), d ** -0.5)
+        return attn_fwd(prep, v, q, lut, topk, kvw, ksum, sla.proj_l.bias.float().contiguous(), d ** -0.5,
+                        blkq=self.blkq, blkk=self.blkk)
 
 
 class UlyssesAttention:
@@ -255,12 +284,15 @@ class UlyssesAttention:
     call start_q / start_k / start_kv as each tensor appears: the Q exchange then runs under the K and V projections, the K
     exchange under the V projection, and the V exchange under the K- and Q-side preparation inside `prims.attend`, which
     receives three callables that wait for and return the full-sequence [1, L, H/world, D] tensors.  The output goes back
-    to its rows with a fourth all-to-all.  Uneven shards use all_to_all_single's split sizes: no padding rows move."""
+    to its rows with a fourth all-to-all.  Uneven shards use all_to_all_single's split sizes: no padding rows move.
+    `sage_arch` is the block family of `prims`; the exchange itself does not depend on it."""
 
     q_first = True
 
-    def __init__(self, sp: "SequenceParallel", prims, compute_dtype=None):
+    def __init__(self, sp: "SequenceParallel", prims, compute_dtype=None, sage_arch: str = "sm100"):
         self.sp, self.prims, self.cdt = sp, prims, compute_dtype
+        self.sage_arch = sage_arch
+        self.blocks = sage_blocks(sage_arch)
         self.rows_of = [shard_rows(sp.total_rows, sp.world, r)[1] - shard_rows(sp.total_rows, sp.world, r)[0]
                         for r in range(sp.world)]
         self._bufs = {}
@@ -306,7 +338,7 @@ class UlyssesAttention:
         return get
 
     def __call__(self, q, k, v):
-        require_default_sage_blocks()
+        require_served_arch(self.sage_arch)
         sp, w = self.sp, self.sp.world
         dtype = q.dtype
         for name, t in (("q", q), ("k", k), ("v", v)):
@@ -334,8 +366,8 @@ class UnevenUlyssesAttention(UlyssesAttention):
     [D]-row (rows * heads_of_peer).  The slab <-> per-peer-chunk reordering is ONE gather kernel each way (a precomputed row
     permutation), not one copy per peer."""
 
-    def __init__(self, sp: "SequenceParallel", prims, heads: int, compute_dtype=None):
-        super().__init__(sp, prims, compute_dtype)
+    def __init__(self, sp: "SequenceParallel", prims, heads: int, compute_dtype=None, sage_arch: str = "sm100"):
+        super().__init__(sp, prims, compute_dtype, sage_arch)
         if heads < sp.world:
             raise ValueError(f"Ulysses exchange needs at least one head per rank (heads={heads}, world={sp.world})")
         self.heads = heads
@@ -368,7 +400,7 @@ class UnevenUlyssesAttention(UlyssesAttention):
         self._pending[name] = (recv.view(sp.total_rows, mine, d), work)
 
     def __call__(self, q, k, v):
-        require_default_sage_blocks()
+        require_served_arch(self.sage_arch)
         sp = self.sp
         dtype = q.dtype
         for name, t in (("q", q), ("k", k), ("v", v)):
@@ -408,21 +440,25 @@ class SequenceParallel:
             raise ValueError(f"mode 'ulysses' needs at least one head per rank (heads={heads}, world={self.world})")
         return mode
 
-    def install(self, model, mode: str = "auto") -> str:
+    def install(self, model, mode: str = "auto", sage_arch: str = "sm100") -> str:
         """Replace every block's attention callable by the sequence-parallel one (the reference seam is
         `WanSelfAttention.attn_op.local_attn`, inference/modify_model.py:48-52).  Returns the mode used:
         "allgather" (K/V all-gather + moment all-reduce, any head count) or "ulysses" (head<->sequence all-to-all; with
-        heads % world != 0 the uneven-split variant)."""
-        require_default_sage_blocks()
+        heads % world != 0 the uneven-split variant).  `sage_arch` is the SageSLA block family the hooks run, "sm100"
+        (BLKQ=128, BLKK=64) or "sm90" (BLKQ=64, BLKK=128); it must be the served arch (SLA.utils.set_served_arch), which
+        the single-GPU module follows."""
+        sage_blocks(sage_arch)
+        require_served_arch(sage_arch)
         used = None
         for blk in model.blocks:
             used = self.pick_mode(blk.heads, mode)
+            prims = UlyssesGpuPrims(blk.sla, sage_arch) if used == "ulysses" else GpuPrimitives(blk.sla, sage_arch)
             if used == "ulysses" and blk.heads % self.world:
-                blk.attn_hook = UnevenUlyssesAttention(self, UlyssesGpuPrims(blk.sla), blk.heads, compute_dtype=blk.sla.dtype)
+                blk.attn_hook = UnevenUlyssesAttention(self, prims, blk.heads, compute_dtype=blk.sla.dtype, sage_arch=sage_arch)
             elif used == "ulysses":
-                blk.attn_hook = UlyssesAttention(self, UlyssesGpuPrims(blk.sla), compute_dtype=blk.sla.dtype)
+                blk.attn_hook = UlyssesAttention(self, prims, compute_dtype=blk.sla.dtype, sage_arch=sage_arch)
             else:
-                blk.attn_hook = SPAttention(self, GpuPrimitives(blk.sla))
+                blk.attn_hook = SPAttention(self, prims, sage_arch)
         self.mode = used
         return used
 

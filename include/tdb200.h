@@ -248,6 +248,29 @@ int tdb200_sla_attn_fwd_kseq_blocks(const int8_t* q_i8, const float* q_scale, co
                                     int64_t h, int64_t d, float sm_scale, int64_t blkq, int64_t blkk, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * a9' backward. Gradients of the block-sparse 16-bit attention (the sparse branch of SparseLinearAttention; reference: the
+ * autograd function `_attention`, SLA/kernel.py:240-319).  d = 128, BLKQ = 128, BLKK = 64, q/k/v/o_s/d_o/dq/dk/dv
+ * [b, l, h, d] contiguous 16-bit (lk = l), lut [b,h,mblk,topk] int32 of distinct key-block ids per row.
+ *   tdb200_sla_attn_fwd_qk16_lse  o_s = T(softmax part of tdb200_sla_attn_fwd_qk16) (no linear branch, no proj_b) and
+ *                                 lse [b,h,l] fp32 = m + log2(l) of the scores in the log2 domain (S * sm_scale * log2e).
+ *   tdb200_sla_attn_bwd_qk16      dq, dk, dv of o_s w.r.t. q, k, v for the incoming gradient d_o, given the forward's o_s and
+ *                                 lse.  P and dS are rounded to T only as MMA operands, accumulation is fp32, no atomics
+ *                                 (bit-for-bit reproducible); key blocks no query block selected get zero dk / dv.  Four kernel
+ *                                 launches and no host synchronisation, so the call can be captured in a CUDA graph.
+ *   tdb200_sla_attn_bwd_workspace_bytes  host-only size of the workspace the backward needs (or a negative error code):
+ *                                 delta [b,h,l] fp32, then the key-major index of the LUT: offsets [b*h, nblk+1], cursors
+ *                                 [b*h, nblk] and entries [b*h, mblk*topk] int32, each 256-byte aligned.
+ * Errors: null pointer, bad shape or topk outside [1, nblk] -> TDB200_ERR_INVALID_ARG; d != 128 or a bad dtype tag ->
+ * TDB200_ERR_UNSUPPORTED; workspace_bytes below the size query -> TDB200_ERR_WORKSPACE.
+ * ------------------------------------------------------------------------------------------- */
+int tdb200_sla_attn_fwd_qk16_lse(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
+                                 void* o_s, float* lse, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale, void* stream);
+int tdb200_sla_attn_bwd_qk16(const void* q, const void* k, const void* v, const void* o_s, const void* d_o, const float* lse,
+                             int dtype, const int32_t* lut, int64_t topk, void* dq, void* dk, void* dv, void* workspace,
+                             int64_t workspace_bytes, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale, void* stream);
+int64_t tdb200_sla_attn_bwd_workspace_bytes(int64_t b, int64_t h, int64_t l, int64_t topk);
+
+/* ---------------------------------------------------------------------------------------------
  * a12. LTX-2 (TurboT2AV) prologue variants   (ltx_core/model/transformer/transformer.py:21-94; Triton fast path
  *      ltx_distillation/fast_norm_kernels.py:388-473).  x, y, residual [b, tokens, n] 16-bit; table [num_ada, n] fp32;
  *      timestep [b, ts_tokens, num_ada*n] 16-bit with ts_tokens in {1, tokens}; ada value i = table[i] + timestep[.., i, :].

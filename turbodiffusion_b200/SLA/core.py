@@ -88,6 +88,49 @@ def attn_fwd_qk16(q, k, v, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None):
     return out
 
 
+def attn_fwd_qk16_lse(q, k, v, lut, topk, sm_scale):
+    """Sparse branch of attn_fwd_qk16 alone, for the training path: (o_s [B,L,H,D] in q.dtype, lse [B,H,L] fp32), lse being
+    the row log-sum-exp of the scores in log2 units (scores scaled by sm_scale * log2(e)).  `lut` [B,H,Mblk,topk] int32."""
+    b, l, h, d = q.shape
+    o_s = torch.empty_like(q)
+    lse = torch.empty(b, h, l, dtype=torch.float32, device=q.device)
+    check(lib().tdb200_sla_attn_fwd_qk16_lse(ptr(q), ptr(k), ptr(v), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(o_s), ptr(lse), b, l, h,
+                                             d, float(sm_scale), stream_ptr(q.device)), "sla_attn_fwd_qk16_lse")
+    return o_s, lse
+
+
+def attn_bwd_qk16(q, k, v, o_s, d_o, lse, lut, topk, sm_scale):
+    """(dq, dk, dv) of attn_fwd_qk16_lse's o_s for the incoming gradient d_o; all [B,L,H,D] contiguous in q.dtype."""
+    b, l, h, d = q.shape
+    dq, dk, dv = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
+    nbytes = lib().tdb200_sla_attn_bwd_workspace_bytes(b, h, l, topk)
+    check(0 if nbytes >= 0 else nbytes, "sla_attn_bwd_workspace_bytes", launches=0)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
+    check(lib().tdb200_sla_attn_bwd_qk16(ptr(q), ptr(k), ptr(v), ptr(o_s), ptr(d_o), ptr(lse), DTYPE_TAG[q.dtype], ptr(lut), topk,
+                                         ptr(dq), ptr(dk), ptr(dv), ptr(ws), nbytes, b, l, h, d, float(sm_scale),
+                                         stream_ptr(q.device)), "sla_attn_bwd_qk16")
+    return dq, dk, dv
+
+
+class SparseAttention16(torch.autograd.Function):
+    """o_s = block-sparse softmax attention of q, k, v ([B,L,H,D], 16-bit, d = 128) over `lut`'s key blocks, differentiable in
+    q, k and v (the reference's `_attention`, SLA/kernel.py:240-319)."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, lut, topk, sm_scale):
+        o_s, lse = attn_fwd_qk16_lse(q, k, v, lut, topk, sm_scale)
+        ctx.save_for_backward(q, k, v, o_s, lse, lut)
+        ctx.topk, ctx.sm_scale = topk, sm_scale
+        return o_s
+
+    @staticmethod
+    def backward(ctx, d_o):
+        q, k, v, o_s, lse, lut = ctx.saved_tensors
+        d_o = d_o.to(q.dtype).contiguous()
+        dq, dk, dv = attn_bwd_qk16(q, k, v, o_s, d_o, lse, lut, ctx.topk, ctx.sm_scale)
+        return dq, dk, dv, None, None, None
+
+
 class _SLABase(nn.Module):
     quantised_qk = True   # SageSparseLinearAttention: INT8 Q.K^T; SparseLinearAttention: 16-bit Q.K^T (128-wide heads)
 
@@ -117,7 +160,11 @@ class _SLABase(nn.Module):
             nn.init.zeros_(self.proj_l.bias)
 
     def forward(self, q, k, v, return_sparsity=False):
-        """q,k,v [B, L, H, D] (any float dtype), D in {64, 128} (SLA/core.py:207) -> [B, L, H, D] in q.dtype."""
+        """q,k,v [B, L, H, D] (any float dtype), D in {64, 128} (SLA/core.py:207) -> [B, L, H, D] in q.dtype.
+        SparseLinearAttention with grad enabled and any of q, k, v requiring grad takes the differentiable training path
+        (_forward_train); every other call runs the fused forward-only kernels."""
+        if not self.quantised_qk and torch.is_grad_enabled() and any(t.requires_grad for t in (q, k, v)):
+            return self._forward_train(q, k, v, return_sparsity)
         require_cuda(q, k, v)
         dtype = q.dtype
         q, k, v = (t if (t.dtype == self.dtype and t.is_contiguous()) else t.to(self.dtype).contiguous() for t in (q, k, v))
@@ -143,6 +190,34 @@ class _SLABase(nn.Module):
             o = attn_fwd(prep, v, q, lut, real_topk, kvw, ksum, self.proj_l.bias.float().contiguous(), d ** -0.5,
                          feature=self.feature, blkq=blkq, blkk=blkk)
         o = o if o.dtype == dtype else o.to(dtype)
+        return (o, real_topk / nblk) if return_sparsity else o
+
+    def _forward_train(self, q, k, v, return_sparsity):
+        """The reference's SparseLinearAttention.forward (SLA/core.py:81-119) with autograd: the same block selection as the
+        fused path, the sparse branch through SparseAttention16, the linear branch and proj_l in torch at the reference's
+        rounding points (feature maps -> dtype, bmm in dtype, proj_l evaluated in dtype as under its autocast)."""
+        if q.shape[-1] != 128:
+            raise NotImplementedError(f"SparseLinearAttention backward: head dim {q.shape[-1]}; gradients are served for d = 128")
+        require_cuda(q, k, v)
+        dtype = q.dtype
+        q, k, v = (t if (t.dtype == self.dtype and t.is_contiguous()) else t.to(self.dtype).contiguous() for t in (q, k, v))
+        d = q.shape[-1]
+        with torch.no_grad():
+            prep = quant_qk(q.detach(), k.detach())
+            nblk = prep.nblk
+            real_topk = max(1, min(nblk, int(self.topk * nblk)))
+            sparse_map, lut = block_map_from_pools(prep.q_pool, prep.k_pool, real_topk)
+        if getattr(self, "_keep_selection", None) is not None:
+            self._keep_selection.update(lut=lut, sparse_map=sparse_map, topk=real_topk)
+        o_s = SparseAttention16.apply(q, k, v, lut, real_topk, d ** -0.5)
+        qh, kh, vh = (t.transpose(1, 2) for t in (q, k, v))                       # [B, H, L, D] views
+        c_q = self.feature_map_q(qh).contiguous().to(self.dtype)
+        c_k = self.feature_map_k(kh).contiguous().to(self.dtype)
+        kvsum = c_k.transpose(-1, -2) @ vh
+        ksum = torch.sum(c_k, dim=-2, keepdim=True)
+        o_l = (c_q @ kvsum) / (1e-5 + (c_q * ksum).sum(dim=-1, keepdim=True))
+        o_l = F.linear(o_l.to(self.dtype), self.proj_l.weight.to(self.dtype), self.proj_l.bias.to(self.dtype))
+        o = (o_s + o_l.transpose(1, 2)).to(dtype).contiguous()
         return (o, real_topk / nblk) if return_sparsity else o
 
     def forward_with_lut(self, q, k, v):

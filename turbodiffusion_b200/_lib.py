@@ -62,6 +62,9 @@ _PROTOS = {
     "tdb200_sla_quant_k_seq_blocks": [_P, _P, _I, _I64, _I64, _I64, _I64, _P, _P, _P, _I64, _P],
     "tdb200_sla_attn_fwd_kseq_blocks": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64,
                                         _F, _I64, _I64, _P],
+    "tdb200_sla_attn_fwd_qk16_lse": [_P, _P, _P, _I, _P, _I64, _P, _P, _I64, _I64, _I64, _I64, _F, _P],
+    "tdb200_sla_attn_bwd_qk16": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F, _P],
+    "tdb200_sla_attn_bwd_workspace_bytes": [_I64, _I64, _I64, _I64],
     "tdb200_ltx_modulated_rms_norm_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_ltx_modulate_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
     "tdb200_ltx_gated_residual_ada": [_P, _P, _I, _P, _P, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
@@ -69,7 +72,7 @@ _PROTOS = {
     "tdb200_quant_int8_rowwise": [_P, _I, _I64, _I64, _P, _P, _P],
     "tdb200_gemm_w8a8_rowwise": [_P, _P, _P, _P, _P, _P, _I, _I64, _I64, _I64, _P],
 }
-_RESTYPES = {"tdb200_last_error": c_char_p}
+_RESTYPES = {"tdb200_last_error": c_char_p, "tdb200_sla_attn_bwd_workspace_bytes": c_int64}
 
 _lib = None
 
@@ -131,7 +134,7 @@ class _DeviceGuarded:
 
 
 LAUNCHES = 0  # kernels launched through the C ABI (each entry point documents how many it enqueues)
-_KERNELS_PER_CALL = {"sla_quant_qk": 4, "sla_quant_qk_blocks": 4, "layernorm_modulate_quant": 2}  # upper bounds per entry point
+_KERNELS_PER_CALL = {"sla_quant_qk": 4, "sla_quant_qk_blocks": 4, "layernorm_modulate_quant": 2, "sla_attn_bwd_qk16": 4}  # upper bounds per entry point
 
 
 def check(rc: int, what: str, launches: int = None) -> None:

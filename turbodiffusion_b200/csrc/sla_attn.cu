@@ -58,6 +58,7 @@ struct AttnParams {
   void* out;              // [b,l,h,d] T
   int l, lk, h, mblk, nblk, topk, feature;  // feature: 0 softmax, 1 elu+1, 2 relu (SLA/core.py:57-73)
   float sm_scale;
+  float* lse;             // [b,h,l] fp32, log2 domain (kLse kernels only)
 };
 
 enum Bar { kQFull = 0, kKFull = 1 /*3*/, kKEmpty = 4 /*3*/, kVFull = 7 /*3*/, kVEmpty = 10 /*3*/, kNumBars = 13 };
@@ -164,7 +165,9 @@ __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const fl
   }
 }
 
-template <typename T, int HD, bool kQK16>
+// kLse: the sparse branch alone for the training path (sla_attn_bwd.cu): out = T(O / l) and lse[b,h,row] = m_used + log2(l),
+// the row log-sum-exp of the scores in the kernel's log2 domain (scaled by sm_scale * log2e).  No KVW load, no linear branch.
+template <typename T, int HD, bool kQK16, bool kLse = false>
 __global__ void __launch_bounds__(kThreads, 1)
 sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                     const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw, AttnParams p) {
@@ -208,8 +211,8 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
       tma_prefetch_desc(&tmap_q);
       tma_prefetch_desc(&tmap_k);
       tma_prefetch_desc(&tmap_v);
-      tma_prefetch_desc(&tmap_kvw);
-      mbar_expect_tx(&bars[kQFull], L::kQBytes + L::kWBytes);
+      if constexpr (!kLse) tma_prefetch_desc(&tmap_kvw);
+      mbar_expect_tx(&bars[kQFull], L::kQBytes + (kLse ? 0 : L::kWBytes));
       if constexpr (kQK16) {  // 16-bit Q rows from [B,L,H,D]: HD/64 chunks of 128 rows x 128 B
 #pragma unroll
         for (int c = 0; c < HD / 64; ++c)
@@ -217,9 +220,11 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
       } else {
         tma_load_4d(smem + L::kOffQ, &tmap_q, &bars[kQFull], 0, m_blk * BLKQ, bh, 0);
       }
+      if constexpr (!kLse) {
 #pragma unroll
-      for (int c = 0; c < HD / 64; ++c)  // KVW: d_k chunk c of the [d_out, d_k] matrix of this head
-        tma_load_4d(smem + L::kOffW + c * (HD * 128), &tmap_kvw, &bars[kQFull], c * 64, 0, bh, 0);
+        for (int c = 0; c < HD / 64; ++c)  // KVW: d_k chunk c of the [d_out, d_k] matrix of this head
+          tma_load_4d(smem + L::kOffW + c * (HD * 128), &tmap_kvw, &bars[kQFull], c * 64, 0, bh, 0);
+      }
       for (int j = 0; j < T_blocks; ++j) {
         const int st = j % kStages;
         const uint32_t ph = ((j / kStages) & 1) ^ 1;
@@ -355,7 +360,21 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     __syncwarp();
     if (lane == 0) mbar_arrive(&bars[kVEmpty + st]);
   }
-  linear_branch_store<T, HD>(o, l_part, p, sbase + L::kOffW, int64_t(m_blk) * BLKQ + r_lo, cq, b, hh, bh);
+  if constexpr (kLse) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t qr = int64_t(m_blk) * BLKQ + r_lo + 8 * h;
+      if (qr >= p.l) continue;
+      const float l_tot = quad_sum(l_part[h]), inv_l = 1.0f / l_tot;
+      if ((lane & 3) == 0) p.lse[int64_t(bh) * p.l + qr] = m_used[h] + __log2f(l_tot);
+      T* orow = static_cast<T*>(p.out) + ((int64_t(b) * p.l + qr) * p.h + hh) * HD;
+#pragma unroll
+      for (int c = 0; c < HD / 8; ++c)
+        *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) = F16Traits<T>::pack(o[4 * c + 2 * h] * inv_l, o[4 * c + 2 * h + 1] * inv_l);
+    }
+  } else {
+    linear_branch_store<T, HD>(o, l_part, p, sbase + L::kOffW, int64_t(m_blk) * BLKQ + r_lo, cq, b, hh, bh);
+  }
 }
 
 // SpargeAttn's Hopper block geometry (SLA/core.py:191-193, 226-229 on sm90): BLKQ = 64 query rows, BLKK = 128 key rows.
@@ -581,18 +600,19 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
   linear_branch_store<T, HD>(o, l_part, p, sbase + L::kOffW, int64_t(m_blk) * BQ + r_lo, cq, b, hh, bh);
 }
 
-template <typename T, int HD, bool kQK16, int kBQ>
+template <typename T, int HD, bool kQK16, int kBQ, bool kLse>
 constexpr auto attn_kernel() {
   if constexpr (kBQ == kHopperBlkQ) return sla_attn_fwd_q64_kernel<T, HD>;
-  else return sla_attn_fwd_kernel<T, HD, kQK16>;
+  else return sla_attn_fwd_kernel<T, HD, kQK16, kLse>;
 }
 
 // kQK16: 16-bit Q and K in [b, l, h, d]; otherwise INT8 Q [b*h, l, d] and INT8 K [b, h, lk, d] (or [b, lk, h, d] when k_seq_major).
 // kBQ x kBK: the block geometry, 128 x 64 (sla_attn_fwd_kernel) or 64 x 128 (sla_attn_fwd_q64_kernel, INT8 head-major K only).
-template <int HD, bool kQK16, int kBQ = BLKQ, int kBK = BLKK>
+// kLse (16-bit 128 x 64 only): sparse branch and row log-sum-exp into `lse`; kvw, ksum and proj_b are not read.
+template <int HD, bool kQK16, int kBQ = BLKQ, int kBK = BLKK, bool kLse = false>
 int launch(const void* q_op, const float* q_scale, const void* k_op, const float* k_scale, const void* v, const void* q, int dtype,
            const int32_t* lut, int64_t topk, const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
-           int64_t l, int64_t lk, int64_t h, float sm_scale, int feature, bool k_seq_major, void* stream) {
+           int64_t l, int64_t lk, int64_t h, float sm_scale, int feature, bool k_seq_major, void* stream, float* lse = nullptr) {
   using L = Lay<HD, kQK16, kBQ, kBK>;
   const int64_t d = HD;
   const int64_t mblk = cdiv64(l, kBQ), nblk = cdiv64(lk, kBK);
@@ -637,7 +657,9 @@ int launch(const void* q_op, const float* q_scale, const void* k_op, const float
     const uint32_t box[4] = {64, 1, kBK, 1};
     if (int rc = make_tmap_4d(&tv, v, t16, 2, dims, str, box)) return rc;
   }
-  {
+  if (kLse) {
+    tw = tv;  // not read
+  } else {
     const uint64_t dims[4] = {uint64_t(d), uint64_t(d), uint64_t(b * h), 1};
     const uint64_t str[3] = {uint64_t(d * 2), uint64_t(d * d * 2), uint64_t(b * h * d * d * 2)};
     const uint32_t box[4] = {64, uint32_t(HD), 1, 1};
@@ -659,12 +681,13 @@ int launch(const void* q_op, const float* q_scale, const void* k_op, const float
   p.topk = int(topk);
   p.feature = feature;
   p.sm_scale = sm_scale;
+  p.lse = lse;
   dim3 grid(static_cast<unsigned>(mblk), static_cast<unsigned>(h), static_cast<unsigned>(b));
   const int threads = kBQ == kHopperBlkQ ? kThreadsQ64 : kThreads;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define TDB_ATTN(T)                                                                                                   \
   do {                                                                                                                \
-    const auto kern = attn_kernel<T, HD, kQK16, kBQ>();                                                               \
+    const auto kern = attn_kernel<T, HD, kQK16, kBQ, kLse>();                                                               \
     if (int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), \
                             "cudaFuncSetAttribute(sla_attn)"))                                                        \
       return rc;                                                                                                      \
@@ -742,6 +765,17 @@ extern "C" int tdb200_sla_attn_fwd_qk16(const void* q, const void* k, const void
   if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (this kernel implements d=128)", (long long)d);
   return launch<128, true>(q, nullptr, k, nullptr, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, sm_scale, 0, false,
                            stream);
+}
+
+// The sparse branch of tdb200_sla_attn_fwd_qk16 with its row log-sum-exp, the forward half of the training path.
+extern "C" int tdb200_sla_attn_fwd_qk16_lse(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
+                                            void* o_s, float* lse, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale,
+                                            void* stream) {
+  if (!q || !k || !v || !lut || !o_s || !lse) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd_qk16_lse: null pointer");
+  if (b <= 0 || l <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd_qk16_lse: bad shape");
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_qk16_lse: head dim %lld (this kernel implements d=128)", (long long)d);
+  return launch<128, true, BLKQ, BLKK, true>(q, nullptr, k, nullptr, v, q, dtype, lut, topk, nullptr, nullptr, nullptr, o_s, b, l, l, h,
+                                             sm_scale, 0, false, stream, lse);
 }
 
 extern "C" int tdb200_sla_attn_fwd_v2(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,

@@ -1,0 +1,583 @@
+// Backward of the block-sparse 16-bit attention (the sparse branch of SparseLinearAttention; reference: the autograd function
+// `_attention`, SLA/kernel.py:240-319, whose backward runs _attn_bwd_preprocess / _attn_bwd_dq / _attn_bwd_dkdv, :85-237).
+// Block geometry of the forward: BLKQ = 128 query rows, BLKK = 64 key rows, 128-wide heads, q/k/v/o/dO/dq/dk/dv in the module
+// layout [b, l, h, d].  The forward (sla_attn.cu, kLse) leaves o_s = T(O / l) and lse = m + log2(l) in the log2 domain, so that
+// P = exp2(S * sm_scale * log2e - lse) is recomputed exactly as the forward normalised it.
+//
+//   sla_bwd_delta_kernel      delta[b,h,row] = sum_d T(dO) * T(o_s), fp32
+//   sla_bwd_kmajor_index_kernel  the LUT transposed: for every (b, h, key block) the ascending list of the query blocks that
+//                                selected it (CSR offsets + entries), built on the device without a host synchronisation
+//   sla_bwd_dq_kernel         one CTA per (query block, head, batch): Q_i and dO_i resident, K_j / V_j streamed over the LUT row;
+//                             S = Q.K^T, dP = dO.V^T, dS = P o (dP - delta), dQ += dS.K  (K tile as the MN-major operand)
+//   sla_bwd_dkdv_kernel       one CTA per (key block, head, batch): K_j and V_j resident, (Q_i, dO_i) streamed over the key
+//                             block's list; S^T = K.Q^T, dP^T = V.dO^T, dV += P^T.dO, dK += dS^T.Q  (Q / dO tiles MN-major)
+//
+// Rounding points (FlashAttention-2's): P and dS are formed in fp32 and rounded to T only as MMA operands; dQ, dK, dV accumulate
+// in fp32 registers and are rounded to T once.  No floating-point atomics: every output element is written by one thread in a
+// fixed order, so the gradients are bit-for-bit reproducible.  Key columns >= l are masked to -inf; query rows >= l get
+// lse = +inf (P = 0) and delta = 0 explicitly, because TMA zero-fill gives their scores, not their statistics.
+#include <type_traits>
+
+#include "common.cuh"
+#include "host_common.h"
+
+namespace {
+using namespace tdb;
+
+constexpr int HD = 128, BLKQ = 128, BLKK = 64;
+constexpr float kLog2e = 1.4426950408889634f;
+
+struct BwdParams {
+  const float* lse;        // [b,h,l]
+  const float* delta;      // [b,h,l]
+  const int32_t* lut;      // [b,h,mblk,topk]       (dQ)
+  const int32_t* kv_off;   // [b*h, nblk+1]          (dK/dV: CSR offsets into kv_idx)
+  const int32_t* kv_idx;   // [b*h, mblk*topk]
+  void* dq;                // [b,l,h,d] T
+  void* dk;
+  void* dv;
+  int l, h, mblk, nblk, topk;
+  float sm_scale;
+};
+
+// ------------------------------------------------------------------------------------------------ preprocessing
+// One warp per (b, row, head); lanes take 4 consecutive columns, then a butterfly sum (fixed order).
+template <typename T>
+__global__ void __launch_bounds__(256) sla_bwd_delta_kernel(const T* o, const T* d_o, float* delta, int64_t rows, int l, int h) {
+  const int64_t r = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (r >= rows) return;
+  const uint2 ov = *reinterpret_cast<const uint2*>(o + r * HD + lane * 4);
+  const uint2 gv = *reinterpret_cast<const uint2*>(d_o + r * HD + lane * 4);
+  float acc = F16Traits<T>::lo(ov.x) * F16Traits<T>::lo(gv.x);
+  acc = fmaf(F16Traits<T>::hi(ov.x), F16Traits<T>::hi(gv.x), acc);
+  acc = fmaf(F16Traits<T>::lo(ov.y), F16Traits<T>::lo(gv.y), acc);
+  acc = fmaf(F16Traits<T>::hi(ov.y), F16Traits<T>::hi(gv.y), acc);
+  acc = warp_sum(acc);
+  if (lane == 0) {
+    const int64_t bl = r / h;           // b * l + row
+    const int hh = int(r - bl * h);
+    const int64_t b = bl / l, row = bl - b * l;
+    delta[(b * h + hh) * l + row] = acc;
+  }
+}
+
+// One CTA per (b, h): count the selections of every key block, exclusive scan into offsets, then fill the lists taking query
+// blocks in ascending order (one LUT row per step).  The integer atomics only hand out slots; within a step every slot of one
+// key block receives the same query-block id, so the index does not depend on their order.
+constexpr int kIndexThreads = 256;
+__global__ void __launch_bounds__(kIndexThreads) sla_bwd_kmajor_index_kernel(const int32_t* lut, int mblk, int nblk, int topk,
+                                                                             int32_t* kv_off, int32_t* cursor, int32_t* kv_idx) {
+  __shared__ int32_t scan[kIndexThreads];
+  const int bh = blockIdx.x, t = threadIdx.x;
+  const int64_t n_sel = int64_t(mblk) * topk;
+  const int32_t* lt = lut + bh * n_sel;
+  int32_t* off = kv_off + int64_t(bh) * (nblk + 1);
+  int32_t* cur = cursor + int64_t(bh) * nblk;
+  int32_t* idx = kv_idx + bh * n_sel;
+  for (int k = t; k < nblk; k += kIndexThreads) cur[k] = 0;
+  __syncthreads();
+  for (int64_t e = t; e < n_sel; e += kIndexThreads) atomicAdd(&cur[__ldg(lt + e)], 1);
+  __syncthreads();
+  int32_t carry = 0;
+  for (int k0 = 0; k0 < nblk; k0 += kIndexThreads) {
+    const int32_t c = k0 + t < nblk ? cur[k0 + t] : 0;
+    scan[t] = c;
+    __syncthreads();
+    for (int s = 1; s < kIndexThreads; s <<= 1) {  // inclusive Hillis-Steele scan
+      const int32_t v = t >= s ? scan[t - s] : 0;
+      __syncthreads();
+      scan[t] += v;
+      __syncthreads();
+    }
+    if (k0 + t < nblk) {
+      off[k0 + t] = carry + scan[t] - c;
+      cur[k0 + t] = 0;
+    }
+    carry += scan[kIndexThreads - 1];
+    __syncthreads();
+  }
+  if (t == 0) off[nblk] = carry;
+  __syncthreads();
+  for (int i = 0; i < mblk; ++i) {
+    for (int e = t; e < topk; e += kIndexThreads) {
+      const int k = __ldg(lt + int64_t(i) * topk + e);
+      idx[off[k] + atomicAdd(&cur[k], 1)] = i;
+    }
+    __syncthreads();
+  }
+}
+
+// Rows r0 and r0 + 8 of an m64n128 fp32 accumulator (fragment layout, common.cuh) -> T(acc * scale) at rows [row0, row0 + 8].
+template <typename T>
+__device__ __forceinline__ void store_rows(const float (&acc)[HD / 2], float scale, void* out, int64_t row0, int l, int h, int hh,
+                                           int b, int cq) {
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    const int64_t r = row0 + 8 * hf;
+    if (r >= l) continue;
+    T* orow = static_cast<T*>(out) + ((int64_t(b) * l + r) * h + hh) * HD;
+#pragma unroll
+    for (int c = 0; c < HD / 8; ++c)
+      *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) = F16Traits<T>::pack(acc[4 * c + 2 * hf] * scale, acc[4 * c + 2 * hf + 1] * scale);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ dQ
+// CTA = 2 consumer warpgroups (64 query rows each, like sla_attn_fwd_kernel) + 1 TMA warp.  Per thread: dQ 64, S 32, dP 32 fp32
+// registers and the dS A fragments.  Shared memory: Q | dO (resident) | K ring | V ring (3 stages); V is released as soon as
+// dP has retired, K after dQ += dS.K.
+namespace dq {
+constexpr int kConsumerWarps = 8, kThreads = kConsumerWarps * 32 + 32, kStages = 3;
+constexpr uint32_t kTileQ = BLKQ * HD * 2, kTileK = BLKK * HD * 2;   // 32 KB, 16 KB
+constexpr uint32_t kOffQ = 0, kOffDO = kTileQ, kOffK = 2 * kTileQ, kOffV = kOffK + kStages * kTileK;
+constexpr uint32_t kOffBars = kOffV + kStages * kTileK, kOffLut = kOffBars + 256;
+enum Bar { kQFull = 0, kKFull = 1, kKEmpty = 4, kVFull = 7, kVEmpty = 10 };
+}  // namespace dq
+
+template <typename T>
+__global__ void __launch_bounds__(dq::kThreads, 1)
+sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
+                  const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v, BwdParams p) {
+  using namespace dq;
+  constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
+  uint16_t* s_lut = reinterpret_cast<uint16_t*>(smem + kOffLut);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
+  const int bh = b * p.h + hh;
+
+  if (threadIdx.x == 0) {
+    mbar_init(&bars[kQFull], 1);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&bars[kKFull + i], 1);
+      mbar_init(&bars[kKEmpty + i], kConsumerWarps);
+      mbar_init(&bars[kVFull + i], 1);
+      mbar_init(&bars[kVEmpty + i], kConsumerWarps);
+    }
+    mbar_fence_init();
+  }
+  {
+    const int32_t* lut_row = p.lut + (int64_t(bh) * p.mblk + m_blk) * p.topk;
+    for (int i = threadIdx.x; i < p.topk; i += kThreads) s_lut[i] = static_cast<uint16_t>(__ldg(lut_row + i));
+  }
+  __syncthreads();
+
+  if (warp == kConsumerWarps) {
+    // =============================================================== TMA producer
+    if (lane == 0) {
+      tma_prefetch_desc(&tmap_q);
+      tma_prefetch_desc(&tmap_do);
+      tma_prefetch_desc(&tmap_k);
+      tma_prefetch_desc(&tmap_v);
+      mbar_expect_tx(&bars[kQFull], 2 * kTileQ);
+#pragma unroll
+      for (int c = 0; c < HD / 64; ++c) {
+        tma_load_4d(smem + kOffQ + c * (BLKQ * 128), &tmap_q, &bars[kQFull], c * 64, hh, m_blk * BLKQ, b);
+        tma_load_4d(smem + kOffDO + c * (BLKQ * 128), &tmap_do, &bars[kQFull], c * 64, hh, m_blk * BLKQ, b);
+      }
+      for (int j = 0; j < p.topk; ++j) {
+        const int st = j % kStages;
+        const uint32_t ph = ((j / kStages) & 1) ^ 1;
+        const int blk = s_lut[j];
+        mbar_wait(&bars[kKEmpty + st], ph);
+        mbar_expect_tx(&bars[kKFull + st], kTileK);
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c)
+          tma_load_4d(smem + kOffK + st * kTileK + c * (BLKK * 128), &tmap_k, &bars[kKFull + st], c * 64, hh, blk * BLKK, b);
+        mbar_wait(&bars[kVEmpty + st], ph);
+        mbar_expect_tx(&bars[kVFull + st], kTileK);
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c)
+          tma_load_4d(smem + kOffV + st * kTileK + c * (BLKK * 128), &tmap_v, &bars[kVFull + st], c * 64, hh, blk * BLKK, b);
+      }
+    }
+    return;
+  }
+
+  // =============================================================== consumer warpgroups
+  const int wg = warp >> 2, w4 = warp & 3;
+  const int r_lo = wg * 64 + w4 * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const uint32_t sbase = smem_u32(smem);
+  const float sc = p.sm_scale * kLog2e;
+  float lse[2], dlt[2];
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    const int64_t r = int64_t(m_blk) * BLKQ + r_lo + 8 * hf;
+    lse[hf] = r < p.l ? __ldg(p.lse + int64_t(bh) * p.l + r) : INFINITY;
+    dlt[hf] = r < p.l ? __ldg(p.delta + int64_t(bh) * p.l + r) : 0.f;
+  }
+  float acc[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) acc[i] = 0.f;
+
+  mbar_wait(&bars[kQFull], 0);
+  for (int j = 0; j < p.topk; ++j) {
+    const int st = j % kStages;
+    const uint32_t ph = (j / kStages) & 1;
+    const int valid = p.l - s_lut[j] * BLKK;
+    const uint32_t sk = sbase + kOffK + st * kTileK, sv = sbase + kOffV + st * kTileK;
+
+    // ---- S = Q.K^T and dP = dO.V^T for this warpgroup's 64 rows (all operands K-major over d)
+    float s[32], dp[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s[i] = dp[i] = 0.f;
+    mbar_wait(&bars[kKFull + st], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks) {
+      const uint64_t qd = make_desc_kmajor_sw128(sbase + kOffQ + (ks >> 2) * (BLKQ * 128) + wg * (64 * 128)) + uint64_t((ks & 3) * 2);
+      const uint64_t kd = make_desc_kmajor_sw128(sk + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
+      wgmma_f16_ss<64, kBF16>(s, qd, kd, ks > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    mbar_wait(&bars[kVFull + st], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks) {
+      const uint64_t gd = make_desc_kmajor_sw128(sbase + kOffDO + (ks >> 2) * (BLKQ * 128) + wg * (64 * 128)) + uint64_t((ks & 3) * 2);
+      const uint64_t vd = make_desc_kmajor_sw128(sv + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
+      wgmma_f16_ss<64, kBF16>(dp, gd, vd, ks > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    reg_fence(dp);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars[kVEmpty + st]);
+
+    // ---- P = exp2(S sc - lse) (columns past l masked), dS = P o (dP - delta), rounded to T into the A fragments
+    uint32_t da[BLKK / 16][4];
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int hf = (i >> 1) & 1, col = 8 * (i >> 2) + cq;
+      const float p0 = col < valid ? fast_exp2(fmaf(s[i], sc, -lse[hf])) : 0.f;
+      const float p1 = col + 1 < valid ? fast_exp2(fmaf(s[i + 1], sc, -lse[hf])) : 0.f;
+      da[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0 * (dp[i] - dlt[hf]), p1 * (dp[i + 1] - dlt[hf]));
+    }
+    // ---- dQ += dS.K  (K: [64 keys x HD], the MN-major operand; +16 keys = +2048 B per K step)
+    const uint64_t kmn = make_desc_mnmajor_sw128(sk, BLKK * 128);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BLKK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(acc, da[kk], kmn + uint64_t(kk * 128));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(acc);
+#pragma unroll
+    for (int kk = 0; kk < BLKK / 16; ++kk) reg_fence(da[kk]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars[kKEmpty + st]);
+  }
+  store_rows<T>(acc, p.sm_scale, p.dq, int64_t(m_blk) * BLKQ + r_lo, p.l, p.h, hh, b, cq);
+}
+
+// ------------------------------------------------------------------------------------------------ dK / dV
+// CTA = a producer warpgroup (one warp issues TMA; setmaxnreg hands its registers to the consumers) + 2 consumer warpgroups.
+// Both consumers work on the same 64 key rows; warpgroup g takes query rows [64g, 64g + 64) of every streamed query block:
+// S^T and dP^T are 64 x 64 tiles (32 registers each), the partial dK and dV 64 x 128 (64 + 64).  The 128 lse / delta values
+// of a query block are staged in shared memory per warpgroup (double-buffered, one named barrier per step).  At the end
+// warpgroup 1 hands its partials to warpgroup 0 through the drained ring, which adds them (fixed order) and stores.
+namespace dkv {
+constexpr int kThreads = 3 * 128, kStages = 2;
+constexpr uint32_t kProducerRegs = 40, kConsumerRegs = 232;   // 128 * 40 + 256 * 232 <= 65536
+constexpr uint32_t kTileQ = BLKQ * HD * 2, kTileK = BLKK * HD * 2;
+constexpr uint32_t kOffK = 0, kOffV = kTileK, kOffQ = 2 * kTileK, kOffDO = kOffQ + kStages * kTileQ;
+constexpr uint32_t kOffStats = kOffDO + kStages * kTileQ;             // [warpgroup][buffer][lse 64 | delta 64] fp32
+constexpr uint32_t kOffBars = kOffStats + 2 * 2 * 128 * 4;
+constexpr uint32_t kSmem = kOffBars + 64;
+enum Bar { kKVFull = 0, kFull = 1 /*2*/, kEmpty = 3 /*2*/ };
+static_assert(HD * 128 * 4 <= 2 * kStages * kTileQ, "partial dK / dV do not fit in the ring");
+}  // namespace dkv
+
+template <typename T>
+__global__ void __launch_bounds__(dkv::kThreads, 1)
+sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
+                    const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v, BwdParams p) {
+  using namespace dkv;
+  constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
+  const int bh = b * p.h + hh;
+  const int32_t* kv_off = p.kv_off + int64_t(bh) * (p.nblk + 1);
+  const int32_t* list = p.kv_idx + int64_t(bh) * p.mblk * p.topk + __ldg(kv_off + n_blk);
+  const int n_list = __ldg(kv_off + n_blk + 1) - __ldg(kv_off + n_blk);
+
+  if (n_list == 0) {  // no query block selected this key block: its gradients are zero (the outputs are not pre-zeroed)
+    for (int e = threadIdx.x; e < BLKK * HD / 8; e += kThreads) {
+      const int64_t r = int64_t(n_blk) * BLKK + e / (HD / 8);
+      if (r >= p.l) break;
+      const int64_t o = ((int64_t(b) * p.l + r) * p.h + hh) * HD + (e % (HD / 8)) * 8;
+      stg_v4(static_cast<T*>(p.dk) + o, make_uint4(0, 0, 0, 0));
+      stg_v4(static_cast<T*>(p.dv) + o, make_uint4(0, 0, 0, 0));
+    }
+    return;
+  }
+  if (threadIdx.x == 0) {
+    mbar_init(&bars[kKVFull], 1);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&bars[kFull + i], 1);
+      mbar_init(&bars[kEmpty + i], 8);   // both consumer warpgroups read every stage
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // =============================================================== TMA producer
+    reg_dealloc<kProducerRegs>();
+    if (warp == 8 && lane == 0) {
+      tma_prefetch_desc(&tmap_q);
+      tma_prefetch_desc(&tmap_do);
+      tma_prefetch_desc(&tmap_k);
+      tma_prefetch_desc(&tmap_v);
+      mbar_expect_tx(&bars[kKVFull], 2 * kTileK);
+#pragma unroll
+      for (int c = 0; c < HD / 64; ++c) {
+        tma_load_4d(smem + kOffK + c * (BLKK * 128), &tmap_k, &bars[kKVFull], c * 64, hh, n_blk * BLKK, b);
+        tma_load_4d(smem + kOffV + c * (BLKK * 128), &tmap_v, &bars[kKVFull], c * 64, hh, n_blk * BLKK, b);
+      }
+      for (int j = 0; j < n_list; ++j) {
+        const int st = j % kStages;
+        const uint32_t ph = ((j / kStages) & 1) ^ 1;
+        const int qb = __ldg(list + j);
+        mbar_wait(&bars[kEmpty + st], ph);
+        mbar_expect_tx(&bars[kFull + st], 2 * kTileQ);
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c) {
+          tma_load_4d(smem + kOffQ + st * kTileQ + c * (BLKQ * 128), &tmap_q, &bars[kFull + st], c * 64, hh, qb * BLKQ, b);
+          tma_load_4d(smem + kOffDO + st * kTileQ + c * (BLKQ * 128), &tmap_do, &bars[kFull + st], c * 64, hh, qb * BLKQ, b);
+        }
+      }
+    }
+    return;
+  }
+
+  // =============================================================== consumer warpgroups
+  reg_alloc<kConsumerRegs>();
+  const int wg = warp >> 2, w4 = warp & 3, t = threadIdx.x & 127;
+  const int kr_lo = w4 * 16 + (lane >> 2);   // key rows kr_lo, kr_lo + 8 of the block
+  const int cq = 2 * (lane & 3);
+  const uint32_t sbase = smem_u32(smem);
+  const float sc = p.sm_scale * kLog2e;
+  float* stats = reinterpret_cast<float*>(smem + kOffStats) + wg * 256;
+  float dk[HD / 2], dv[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) dk[i] = dv[i] = 0.f;
+
+  mbar_wait(&bars[kKVFull], 0);
+  for (int j = 0; j < n_list; ++j) {
+    const int st = j % kStages;
+    const uint32_t ph = (j / kStages) & 1;
+    const int qb = __ldg(list + j);
+    // ---- lse / delta of this warpgroup's 64 query rows; query rows >= l: P = 0 and delta = 0
+    float* sb = stats + (j & 1) * 128;
+    {
+      const int64_t r = int64_t(qb) * BLKQ + wg * 64 + (t & 63);
+      const bool in = r < p.l;
+      sb[t] = t < 64 ? (in ? __ldg(p.lse + int64_t(bh) * p.l + r) : INFINITY) : (in ? __ldg(p.delta + int64_t(bh) * p.l + r) : 0.f);
+    }
+    named_bar_sync(1 + wg, 128);
+
+    // ---- S^T = K.Q^T and dP^T = V.dO^T over this warpgroup's 64 query rows (all operands K-major over d)
+    const uint32_t sq = sbase + kOffQ + st * kTileQ + wg * (64 * 128), sg = sbase + kOffDO + st * kTileQ + wg * (64 * 128);
+    float s[32], dp[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s[i] = dp[i] = 0.f;
+    mbar_wait(&bars[kFull + st], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks) {
+      const uint64_t kd = make_desc_kmajor_sw128(sbase + kOffK + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
+      const uint64_t qd = make_desc_kmajor_sw128(sq + (ks >> 2) * (BLKQ * 128)) + uint64_t((ks & 3) * 2);
+      wgmma_f16_ss<64, kBF16>(s, kd, qd, ks > 0 ? 1u : 0u);
+    }
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks) {
+      const uint64_t vd = make_desc_kmajor_sw128(sbase + kOffV + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
+      const uint64_t gd = make_desc_kmajor_sw128(sg + (ks >> 2) * (BLKQ * 128)) + uint64_t((ks & 3) * 2);
+      wgmma_f16_ss<64, kBF16>(dp, vd, gd, ks > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    reg_fence(dp);
+
+    // ---- P^T (columns = query rows) rounded to T; dV += P^T.dO with dO as the MN-major operand (+16 rows = +2048 B per K step).
+    //      Key rows >= l only reach dK / dV rows that are never stored, so they need no mask.
+    uint32_t pa[4][4], da[4][4];
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const float2 ls = *reinterpret_cast<const float2*>(sb + 8 * (i >> 2) + cq);
+      s[i] = fast_exp2(fmaf(s[i], sc, -ls.x));
+      s[i + 1] = fast_exp2(fmaf(s[i + 1], sc, -ls.y));
+      pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(s[i], s[i + 1]);
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_f16_rs<HD, kBF16, 1>(dv, pa[kk], make_desc_mnmajor_sw128(sg, BLKQ * 128) + uint64_t(kk * 128));
+    wgmma_commit();
+    // ---- dS^T = P^T o (dP^T - delta) rounded to T; dK += dS^T.Q
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const float2 dl = *reinterpret_cast<const float2*>(sb + 64 + 8 * (i >> 2) + cq);
+      da[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(s[i] * (dp[i] - dl.x), s[i + 1] * (dp[i + 1] - dl.y));
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_f16_rs<HD, kBF16, 1>(dk, da[kk], make_desc_mnmajor_sw128(sq, BLKQ * 128) + uint64_t(kk * 128));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(dv);
+    reg_fence(dk);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      reg_fence(pa[kk]);
+      reg_fence(da[kk]);
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars[kEmpty + st]);
+  }
+
+  // ---- warpgroup 1's partials -> warpgroup 0 through the ring (every stage has been consumed by both); [value][thread] layout
+  float* xchg = reinterpret_cast<float*>(smem + kOffQ) + t;
+  named_bar_sync(3, 256);
+  if (wg == 1) {
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) {
+      xchg[i * 128] = dk[i];
+      xchg[(HD / 2 + i) * 128] = dv[i];
+    }
+  }
+  named_bar_sync(3, 256);
+  if (wg == 1) return;
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) {
+    dk[i] += xchg[i * 128];
+    dv[i] += xchg[(HD / 2 + i) * 128];
+  }
+  const int64_t row0 = int64_t(n_blk) * BLKK + kr_lo;
+  store_rows<T>(dk, p.sm_scale, p.dk, row0, p.l, p.h, hh, b, cq);
+  store_rows<T>(dv, 1.0f, p.dv, row0, p.l, p.h, hh, b, cq);
+}
+
+// ------------------------------------------------------------------------------------------------ host
+struct WsLayout {
+  size_t delta, kv_off, cursor, kv_idx, total;
+};
+size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
+WsLayout ws_layout(int64_t b, int64_t h, int64_t l, int64_t topk) {
+  const int64_t mblk = cdiv64(l, BLKQ), nblk = cdiv64(l, BLKK), bh = b * h;
+  WsLayout w;
+  w.delta = 0;
+  w.kv_off = w.delta + align256(size_t(bh * l) * 4);
+  w.cursor = w.kv_off + align256(size_t(bh * (nblk + 1)) * 4);
+  w.kv_idx = w.cursor + align256(size_t(bh * nblk) * 4);
+  w.total = w.kv_idx + align256(size_t(bh * mblk * topk) * 4);
+  return w;
+}
+
+// [b, l, h, d] 16-bit tensor, boxes of 64 columns x `rows` sequence rows of one head
+int tmap_rows(CUtensorMap* m, const void* base, CUtensorMapDataType t16, int64_t b, int64_t l, int64_t h, uint32_t rows) {
+  const uint64_t dims[4] = {uint64_t(HD), uint64_t(h), uint64_t(l), uint64_t(b)};
+  const uint64_t str[3] = {uint64_t(HD * 2), uint64_t(h * HD * 2), uint64_t(l * h * HD * 2)};
+  const uint32_t box[4] = {64, 1, rows, 1};
+  return make_tmap_4d(m, base, t16, 2, dims, str, box);
+}
+
+template <typename T>
+int launch_bwd(const void* q, const void* k, const void* v, const void* o_s, const void* d_o, const float* lse, const int32_t* lut,
+               int64_t topk, void* dq, void* dk, void* dv, uint8_t* ws, int64_t b, int64_t l, int64_t h, float sm_scale,
+               cudaStream_t st) {
+  const int64_t mblk = cdiv64(l, BLKQ), nblk = cdiv64(l, BLKK);
+  const WsLayout w = ws_layout(b, h, l, topk);
+  float* delta = reinterpret_cast<float*>(ws + w.delta);
+  int32_t* kv_off = reinterpret_cast<int32_t*>(ws + w.kv_off);
+  int32_t* cursor = reinterpret_cast<int32_t*>(ws + w.cursor);
+  int32_t* kv_idx = reinterpret_cast<int32_t*>(ws + w.kv_idx);
+  const CUtensorMapDataType t16 = std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                                        : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUtensorMap tq, tdo, tk, tv;
+  if (int rc = tmap_rows(&tq, q, t16, b, l, h, BLKQ)) return rc;
+  if (int rc = tmap_rows(&tdo, d_o, t16, b, l, h, BLKQ)) return rc;
+  if (int rc = tmap_rows(&tk, k, t16, b, l, h, BLKK)) return rc;
+  if (int rc = tmap_rows(&tv, v, t16, b, l, h, BLKK)) return rc;
+
+  const int64_t rows = b * l * h;
+  sla_bwd_delta_kernel<T><<<unsigned(cdiv64(rows, 8)), 256, 0, st>>>(static_cast<const T*>(o_s), static_cast<const T*>(d_o), delta,
+                                                                       rows, int(l), int(h));
+  if (int rc = check_launch("sla_bwd_delta_kernel")) return rc;
+  sla_bwd_kmajor_index_kernel<<<unsigned(b * h), kIndexThreads, 0, st>>>(lut, int(mblk), int(nblk), int(topk), kv_off, cursor, kv_idx);
+  if (int rc = check_launch("sla_bwd_kmajor_index_kernel")) return rc;
+
+  BwdParams p;
+  p.lse = lse;
+  p.delta = delta;
+  p.lut = lut;
+  p.kv_off = kv_off;
+  p.kv_idx = kv_idx;
+  p.dq = dq;
+  p.dk = dk;
+  p.dv = dv;
+  p.l = int(l);
+  p.h = int(h);
+  p.mblk = int(mblk);
+  p.nblk = int(nblk);
+  p.topk = int(topk);
+  p.sm_scale = sm_scale;
+
+  const size_t smem_dq = 1024 + dq::kOffLut + ((size_t(topk) * 2 + 15) & ~size_t(15));
+  if (int rc = check_cuda(cudaFuncSetAttribute(sla_bwd_dq_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_dq)),
+                          "cudaFuncSetAttribute(sla_bwd_dq)"))
+    return rc;
+  sla_bwd_dq_kernel<T><<<dim3(unsigned(mblk), unsigned(h), unsigned(b)), dq::kThreads, smem_dq, st>>>(tq, tdo, tk, tv, p);
+  if (int rc = check_launch("sla_bwd_dq_kernel")) return rc;
+
+  const size_t smem_kv = 1024 + dkv::kSmem;
+  if (int rc = check_cuda(cudaFuncSetAttribute(sla_bwd_dkdv_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_kv)),
+                          "cudaFuncSetAttribute(sla_bwd_dkdv)"))
+    return rc;
+  sla_bwd_dkdv_kernel<T><<<dim3(unsigned(nblk), unsigned(h), unsigned(b)), dkv::kThreads, smem_kv, st>>>(tq, tdo, tk, tv, p);
+  return check_launch("sla_bwd_dkdv_kernel");
+}
+
+}  // namespace
+
+extern "C" int64_t tdb200_sla_attn_bwd_workspace_bytes(int64_t b, int64_t h, int64_t l, int64_t topk) {
+  if (b <= 0 || h <= 0 || l <= 0 || topk <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_bwd_workspace_bytes: bad shape");
+  return int64_t(ws_layout(b, h, l, topk).total);
+}
+
+extern "C" int tdb200_sla_attn_bwd_qk16(const void* q, const void* k, const void* v, const void* o_s, const void* d_o, const float* lse,
+                                        int dtype, const int32_t* lut, int64_t topk, void* dq, void* dk, void* dv, void* workspace,
+                                        int64_t workspace_bytes, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale,
+                                        void* stream) {
+  if (!q || !k || !v || !o_s || !d_o || !lse || !lut || !dq || !dk || !dv || !workspace)
+    return fail(TDB200_ERR_INVALID_ARG, "sla_attn_bwd_qk16: null pointer");
+  if (b <= 0 || l <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_bwd_qk16: bad shape");
+  const int64_t mblk = cdiv64(l, BLKQ), nblk = cdiv64(l, BLKK);
+  if (topk <= 0 || topk > nblk)
+    return fail(TDB200_ERR_INVALID_ARG, "sla_attn_bwd_qk16: topk=%lld outside [1, %lld]", (long long)topk, (long long)nblk);
+  if (d != HD) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_bwd_qk16: head dim %lld (this kernel implements d=128)", (long long)d);
+  if (dtype != TDB200_DTYPE_BF16 && dtype != TDB200_DTYPE_FP16)
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_bwd_qk16: dtype tag %d", dtype);
+  if (nblk > 65535 || h > 65535 || b > 65535 || b * h * mblk * topk > 0x7FFFFFFF)
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_bwd_qk16: dimension too large");
+  if (1024 + dq::kOffLut + ((size_t(topk) * 2 + 15) & ~size_t(15)) > 227 * 1024)
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_bwd_qk16: topk=%lld too large for on-chip LUT", (long long)topk);
+  const int64_t need = int64_t(ws_layout(b, h, l, topk).total);
+  if (workspace_bytes < need)
+    return fail(TDB200_ERR_WORKSPACE, "sla_attn_bwd_qk16: workspace of %lld bytes, %lld needed", (long long)workspace_bytes,
+                (long long)need);
+  if (int rc = require_sm90()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  if (dtype == TDB200_DTYPE_BF16)
+    return launch_bwd<__nv_bfloat16>(q, k, v, o_s, d_o, lse, lut, topk, dq, dk, dv, ws, b, l, h, sm_scale, st);
+  return launch_bwd<__half>(q, k, v, o_s, d_o, lse, lut, topk, dq, dk, dv, ws, b, l, h, sm_scale, st);
+}

@@ -3,14 +3,19 @@
 //
 //   c[i,j] = T( fma-chain over kb of  float(int32 dot of K-block kb) * (a_s[i/128,kb]*b_s[j/128,kb]) )  [+ bias]
 //
-// Design (one CTA per 128x128 output tile, 128-deep K-blocks; a tile is exactly one block of both scale grids):
-//   warp 8   TMA producer: A tile [128 rows x 128 B] and B tile [128 rows x 128 B] per K-block, 128B-swizzled,
-//            4-stage ring, mbarrier complete_tx.
-//   warpgroups 0-1  MMA + dequant + epilogue; warpgroup g owns output rows [64g, 64g+64) of the tile.  Per K-block four
-//            wgmma.m64n128k32.s32.s8.s8 into a 64-register int32 accumulator, then the int -> float conversion and the
-//            FFMA with the block scale into 64 fp32 registers; the two warpgroups' dequant and MMA phases interleave on
-//            the SM.  The accumulate flag is reset at every K-block because the reference rescales per K-block.  After the
-//            last K-block: round to T, (+bias), (GELU), store.
+// Design (one CTA per 128x256 output tile, 128-deep K-blocks; the tile is one 128-row block of the activation scale grid
+// and two 128-column blocks ("halves") of the weight scale grid):
+//   warpgroup 2  TMA producer (one thread of warp 8; setmaxnreg gives its registers to the consumers, whose two fp32
+//            accumulators and int32 staging accumulator do not fit in the 168 a 384-thread CTA starts with): A tile
+//            [128 rows x 128 B] and B tile [256 rows x 128 B] per K-block, 128B-swizzled, 4-stage ring, mbarrier
+//            complete_tx.  The wide tile does twice the MMA work of a 128x128 one for 1.5x the operand bytes pulled from
+//            L2, and pays the ring fill and the epilogue once per twice the work (DESIGN.md, a2).
+//   warpgroups 0-1  MMA + dequant + epilogue; warpgroup g owns output rows [64g, 64g+64) of the tile.  Per K-block and
+//            half: four wgmma.m64n128k32.s32.s8.s8 into one 64-register int32 staging accumulator, then the int -> float
+//            conversion and the FFMA with that half's block scale into the half's 64 fp32 registers; the two warpgroups'
+//            dequant and MMA phases interleave on the SM.  The accumulate flag is reset at every K-block because the
+//            reference rescales per K-block.  After the last K-block, per half: round to T, (+bias), (GELU), store.
+//            A half that lies entirely past n is not stored, and in the block-scale variant not multiplied either.
 // Integer accumulation is exact and the fp32 FMA chain runs in ascending kb order, so the result is bit-identical
 // to the reference restatement (oracle.int8_linear) on the same int8 inputs.
 #include "common.cuh"
@@ -20,12 +25,14 @@ namespace {
 
 using namespace tdb;
 
-constexpr int BM = 128, BN = 128, BK = 128;
+constexpr int BM = 128, BN = 256, BK = 128;
+constexpr int BH = 128;                              // one half of the tile: one weight-scale block, one MMA N
 constexpr int kStages = 4;
 constexpr int kConsumerWarps = 8;                    // warpgroups 0-1
-constexpr int kThreads = kConsumerWarps * 32 + 32;   // + the TMA warp
+constexpr int kThreads = kConsumerWarps * 32 + 128;  // + the TMA warpgroup
+constexpr uint32_t kProducerRegs = 40, kConsumerRegs = 232;   // 128 * 40 + 256 * 232 <= 65536
 constexpr uint32_t kATile = BM * BK;                 // 16 KB
-constexpr uint32_t kBTile = BN * BK;                 // 16 KB
+constexpr uint32_t kBTile = BN * BK;                 // 32 KB: half h at +16 KB h
 constexpr uint32_t kStageBytes = kATile + kBTile;
 constexpr size_t kSmemBytes = 1024 + size_t(kStages) * kStageBytes + 256 /*barriers + amax exchange*/;
 
@@ -74,7 +81,7 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + size_t(kStages) * kStageBytes);
   uint64_t* full_bar = bars;                // [kStages]  TMA -> MMA
   uint64_t* empty_bar = bars + kStages;     // [kStages]  MMA -> TMA (one arrival per consumer warp)
-  float* amax_x = reinterpret_cast<float*>(bars + 2 * kStages);  // [kConsumerWarps] block-amax exchange (quantised output)
+  float* amax_x = reinterpret_cast<float*>(bars + 2 * kStages);  // [2][kConsumerWarps] block-amax exchange per half
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -89,9 +96,10 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   }
   __syncthreads();
 
-  if (warp == kConsumerWarps) {
+  if (warp >= kConsumerWarps) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    reg_dealloc<kProducerRegs>();
+    if (warp == kConsumerWarps && lane == 0) {
       tma_prefetch_desc(&tmap_a);
       tma_prefetch_desc(&tmap_b);
       for (int kb = 0; kb < p.k_blocks; ++kb) {
@@ -107,21 +115,21 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   }
 
   // ------------------------------------------------------------------ MMA + dequant + epilogue warpgroups
+  reg_alloc<kConsumerRegs>();
   const int wg = warp >> 2, w4 = warp & 3;
   const uint32_t sbase = smem_u32(smem);
-  // the four K=32 steps of K-block kb into `d` (onto its contents when `acc_in`)
-  auto issue = [&](uint32_t (&d)[64], int kb, bool acc_in) {
-    const uint32_t stage = kb % kStages;
-    mbar_wait(&full_bar[stage], (kb / kStages) & 1u);
-    const uint32_t sa = sbase + stage * kStageBytes;
+  // the four K=32 steps of K-block kb against half `h` of the B tile into `d` (onto its contents when `acc_in`); the caller
+  // has waited on the stage's full barrier and commits the group
+  auto issue = [&](uint32_t (&d)[64], int kb, int h, bool acc_in) {
+    const uint32_t sa = sbase + (kb % kStages) * kStageBytes;
     const uint64_t adesc = make_desc_kmajor_sw128(sa + wg * (64 * 128));
-    const uint64_t bdesc = make_desc_kmajor_sw128(sa + kATile);
+    const uint64_t bdesc = make_desc_kmajor_sw128(sa + kATile + h * (BH * BK));
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < BK / 32; ++ks)  // +32 bytes (one K=32 int8 slice) inside the 128B swizzle row: +2 in 16-byte units
-      wgmma_i8_ss<BN>(d, adesc + uint64_t(ks * 2), bdesc + uint64_t(ks * 2), (ks > 0 || acc_in) ? 1u : 0u);
-    wgmma_commit();
+      wgmma_i8_ss<BH>(d, adesc + uint64_t(ks * 2), bdesc + uint64_t(ks * 2), (ks > 0 || acc_in) ? 1u : 0u);
   };
+  auto wait_full = [&](int kb) { mbar_wait(&full_bar[kb % kStages], (kb / kStages) & 1u); };
   auto release = [&](int kb) {
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[kb % kStages]);
@@ -131,121 +139,158 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int r_lo = wg * 64 + w4 * 16 + (lane >> 2);
   const int cq = 2 * (lane & 3);
   const int64_t row0 = int64_t(m_tile) * BM + r_lo, row1 = row0 + 8;
-  const int64_t col_base = int64_t(n_tile) * BN + cq;
   const T* bias = static_cast<const T*>(p.bias);
+  // the second half holds at least one column < n (CTA-uniform)
+  const bool has_hi = int64_t(n_tile) * BN + BH < p.n;
 
   if constexpr (kRowScale) {
-    uint32_t ia[64];
+    uint32_t ia0[64], ia1[64];
+    // K-block kb's MMAs chain onto kb-1's in flight (same accumulators, in order): wait only for kb-1 to free its slot,
+    // so the tensor pipe does not drain at every K-block of a long K
     for (int kb = 0; kb < p.k_blocks; ++kb) {
-      issue(ia, kb, kb > 0);
-      wgmma_wait<0>();
-      reg_fence(ia);
-      release(kb);
+      wait_full(kb);
+      issue(ia0, kb, 0, kb > 0);
+      issue(ia1, kb, 1, kb > 0);   // unconditional: a wgmma under a branch costs an injected warpgroup.arrive per K-block
+      wgmma_commit();
+      if (kb > 0) {
+        wgmma_wait<1>();
+        release(kb - 1);
+      }
     }
+    wgmma_wait<0>();
+    reg_fence(ia0);
+    reg_fence(ia1);
     // c = T(fma(float(acc) * a_s[row], b_s[col], bias[col])): the reference's TileLang epilogue compiles (nvcc default
     // -fmad) to I2FP, FMUL, FFMA per element (tools/tilelang_epilogue_probe.py)
     const float sa0 = row0 < p.m ? __ldg(p.a_s + row0) : 0.f, sa1 = row1 < p.m ? __ldg(p.a_s + row1) : 0.f;
+    auto store = [&](const uint32_t (&ia)[64], int hf) {
+      const int64_t col_base = int64_t(n_tile) * BN + hf * BH + cq;
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int64_t col = col_base + 8 * j;
-      if (col >= p.n) continue;
-      const float sb0 = __ldg(p.b_s + col), sb1 = __ldg(p.b_s + col + 1);
-      const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
+      for (int j = 0; j < BH / 8; ++j) {
+        const int64_t col = col_base + 8 * j;
+        if (col >= p.n) continue;
+        const float sb0 = __ldg(p.b_s + col), sb1 = __ldg(p.b_s + col + 1);
+        const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const float sa = h ? sa1 : sa0;
-        const float y0 = __fmaf_rn(__fmul_rn(__int2float_rn(static_cast<int>(ia[4 * j + 2 * h])), sa), sb0, F16Traits<T>::lo(bw));
-        const float y1 = __fmaf_rn(__fmul_rn(__int2float_rn(static_cast<int>(ia[4 * j + 2 * h + 1])), sa), sb1, F16Traits<T>::hi(bw));
-        const int64_t row = h ? row1 : row0;
-        if (row < p.m) *reinterpret_cast<uint32_t*>(static_cast<T*>(p.c) + row * p.n + col) = F16Traits<T>::pack(y0, y1);
+        for (int h = 0; h < 2; ++h) {
+          const float sa = h ? sa1 : sa0;
+          const float y0 = __fmaf_rn(__fmul_rn(__int2float_rn(static_cast<int>(ia[4 * j + 2 * h])), sa), sb0, F16Traits<T>::lo(bw));
+          const float y1 = __fmaf_rn(__fmul_rn(__int2float_rn(static_cast<int>(ia[4 * j + 2 * h + 1])), sa), sb1, F16Traits<T>::hi(bw));
+          const int64_t row = h ? row1 : row0;
+          if (row < p.m) *reinterpret_cast<uint32_t*>(static_cast<T*>(p.c) + row * p.n + col) = F16Traits<T>::pack(y0, y1);
+        }
       }
-    }
+    };
+    store(ia0, 0);
+    if (has_hi) store(ia1, 1);
     return;
   }
 
-  // block scales: a_s [m/128, k_blocks] row m_tile, b_s [n/128, k_blocks] row n_tile (the tile is one 128-column block)
+  // block scales: a_s [m/128, k_blocks] row m_tile, b_s [ceil(n/128), k_blocks] rows 2 n_tile (+1 only when has_hi)
   const float* as_row = p.a_s + int64_t(m_tile) * p.k_blocks;
-  const float* bs_row = p.b_s + int64_t(n_tile) * p.k_blocks;
-  float acc[64];
+  const float* bs_row0 = p.b_s + int64_t(2 * n_tile) * p.k_blocks;
+  const float* bs_row1 = bs_row0 + p.k_blocks;
+  float acc0[64], acc1[64];
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+  for (int i = 0; i < 64; ++i) acc0[i] = acc1[i] = 0.0f;
   // float(s) without the conversion unit: as_float(0x4B400000 + s) == 1.5*2^23 + s exactly for |s| < 2^22 (a K-block sum
   // is at most 128^3 = 2^21 in magnitude), and subtracting 1.5*2^23 is exact, so this is the same value __int2float_rn gives
   // on the full-rate integer-add and FP32 pipes
   constexpr float kMagicF = 12582912.0f;
   constexpr int kMagicI = 0x4B400000;
   uint32_t ia[64];
-  for (int kb = 0; kb < p.k_blocks; ++kb) {
-    issue(ia, kb, false);
-    const float scale = __ldg(as_row + kb) * __ldg(bs_row + kb);
+  auto dequant = [&](float (&acc)[64], float scale) {
     wgmma_wait<0>();
     reg_fence(ia);
-    release(kb);
 #pragma unroll
     for (int i = 0; i < 64; ++i)
       acc[i] = __fmaf_rn(__fsub_rn(__int_as_float(static_cast<int>(ia[i]) + kMagicI), kMagicF), scale, acc[i]);
+  };
+  for (int kb = 0; kb < p.k_blocks; ++kb) {
+    wait_full(kb);
+    const float as = __ldg(as_row + kb);
+    issue(ia, kb, 0, false);
+    wgmma_commit();
+    dequant(acc0, as * __ldg(bs_row0 + kb));
+    if (has_hi) {
+      issue(ia, kb, 1, false);
+      wgmma_commit();
+      dequant(acc1, as * __ldg(bs_row1 + kb));
+    }
+    release(kb);
   }
 
   const bool act_gelu = p.act == 1;
   if (p.out_q != nullptr) {
-    // ---- fused a1: the tile is one 128x128 quant block (m_tile, n_tile).  y = the T-rounded value the plain epilogue
-    //      would store (rows >= m count as 0); amax over the block; q = sat_s8(rint(y*128/amax)).
-    uint32_t yw[32];
-    uint32_t amax2 = 0u;
+    // ---- fused a1: each half is one 128x128 quant block (m_tile, 2 n_tile + hf).  y = the T-rounded value the plain
+    //      epilogue would store (rows >= m count as 0); amax over the block; q = sat_s8(rint(y*128/amax)).
+    auto store_q = [&](const float (&acc)[64], int hf) {
+      const int64_t col_base = int64_t(n_tile) * BN + hf * BH + cq;
+      uint32_t yw[32];
+      uint32_t amax2 = 0u;
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int64_t col = col_base + 8 * j;
-      const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
+      for (int j = 0; j < BH / 8; ++j) {
+        const int64_t col = col_base + 8 * j;
+        const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint32_t y = F16Traits<T>::pack(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);   // T(acc)
-        if (bias != nullptr) y = F16Traits<T>::add2(y, bw);                            // T(T(acc) + bias)
-        if (act_gelu) y = F16Traits<T>::pack(gelu_tanh_approx(F16Traits<T>::lo(y)), gelu_tanh_approx(F16Traits<T>::hi(y)));
-        if ((h ? row1 : row0) >= p.m) y = 0u;
-        yw[2 * j + h] = y;
-        amax2 = F16Traits<T>::absmax2(amax2, y);
+        for (int h = 0; h < 2; ++h) {
+          uint32_t y = F16Traits<T>::pack(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);   // T(acc)
+          if (bias != nullptr) y = F16Traits<T>::add2(y, bw);                            // T(T(acc) + bias)
+          if (act_gelu) y = F16Traits<T>::pack(gelu_tanh_approx(F16Traits<T>::lo(y)), gelu_tanh_approx(F16Traits<T>::hi(y)));
+          if ((h ? row1 : row0) >= p.m) y = 0u;
+          yw[2 * j + h] = y;
+          amax2 = F16Traits<T>::absmax2(amax2, y);
+        }
       }
-    }
-    float amax = fmaxf(1e-8f, fmaxf(F16Traits<T>::lo(amax2), F16Traits<T>::hi(amax2)));
-    amax = warp_max(amax);
-    if (lane == 0) amax_x[warp] = amax;
-    named_bar_sync(1, kConsumerWarps * 32);
+      float amax = fmaxf(1e-8f, fmaxf(F16Traits<T>::lo(amax2), F16Traits<T>::hi(amax2)));
+      amax = warp_max(amax);
+      float* xch = amax_x + hf * kConsumerWarps;   // one exchange slot set per half: no reuse hazard between halves
+      if (lane == 0) xch[warp] = amax;
+      named_bar_sync(1, kConsumerWarps * 32);
 #pragma unroll
-    for (int w = 0; w < kConsumerWarps; ++w) amax = fmaxf(amax, amax_x[w]);
-    const float r = __fdiv_rn(128.0f, amax);
-    if (threadIdx.x == 0) p.out_s[int64_t(m_tile) * (p.n >> 7) + n_tile] = amax * 0.0078125f;
+      for (int w = 0; w < kConsumerWarps; ++w) amax = fmaxf(amax, xch[w]);
+      const float r = __fdiv_rn(128.0f, amax);
+      if (threadIdx.x == 0) p.out_s[int64_t(m_tile) * (p.n >> 7) + 2 * n_tile + hf] = amax * 0.0078125f;
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int64_t col = col_base + 8 * j;
+      for (int j = 0; j < BH / 8; ++j) {
+        const int64_t col = col_base + 8 * j;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const uint32_t y = yw[2 * j + h];
-        const int q0 = __float2int_rn(fminf(__fmul_rn(F16Traits<T>::lo(y), r), 127.0f));
-        const int q1 = __float2int_rn(fminf(__fmul_rn(F16Traits<T>::hi(y), r), 127.0f));
-        const int64_t row = h ? row1 : row0;
-        if (row < p.m)
-          *reinterpret_cast<uint16_t*>(p.out_q + row * p.n + col) = static_cast<uint16_t>((q0 & 0xFF) | ((q1 & 0xFF) << 8));
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t y = yw[2 * j + h];
+          const int q0 = __float2int_rn(fminf(__fmul_rn(F16Traits<T>::lo(y), r), 127.0f));
+          const int q1 = __float2int_rn(fminf(__fmul_rn(F16Traits<T>::hi(y), r), 127.0f));
+          const int64_t row = h ? row1 : row0;
+          if (row < p.m)
+            *reinterpret_cast<uint16_t*>(p.out_q + row * p.n + col) = static_cast<uint16_t>((q0 & 0xFF) | ((q1 & 0xFF) << 8));
+        }
       }
-    }
+    };
+    store_q(acc0, 0);
+    if (has_hi) store_q(acc1, 1);
     return;
   }
+  auto store = [&](const float (&acc)[64], int hf) {
+    const int64_t col_base = int64_t(n_tile) * BN + hf * BH + cq;
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const int64_t col = col_base + 8 * j;
-    if (col >= p.n) continue;
-    const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
-    const int64_t part = col / p.n_part;
-    T* cp = static_cast<T*>(p.c) + part * p.m * p.n_part + (col - part * p.n_part);
+    for (int j = 0; j < BH / 8; ++j) {
+      const int64_t col = col_base + 8 * j;
+      if (col >= p.n) continue;
+      const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
+      const int64_t part = col / p.n_part;
+      T* cp = static_cast<T*>(p.c) + part * p.m * p.n_part + (col - part * p.n_part);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      // T(acc) then the packed 16-bit add: one rounding each, exactly the module's `out + bias` on 16-bit tensors
-      uint32_t y = F16Traits<T>::pack(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-      if (bias != nullptr) y = F16Traits<T>::add2(y, bw);
-      if (act_gelu) y = F16Traits<T>::pack(gelu_precise(F16Traits<T>::lo(y)), gelu_precise(F16Traits<T>::hi(y)));
-      const int64_t row = h ? row1 : row0;
-      if (row < p.m) *reinterpret_cast<uint32_t*>(cp + row * p.n_part) = y;
+      for (int h = 0; h < 2; ++h) {
+        // T(acc) then the packed 16-bit add: one rounding each, exactly the module's `out + bias` on 16-bit tensors
+        uint32_t y = F16Traits<T>::pack(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        if (bias != nullptr) y = F16Traits<T>::add2(y, bw);
+        if (act_gelu) y = F16Traits<T>::pack(gelu_precise(F16Traits<T>::lo(y)), gelu_precise(F16Traits<T>::hi(y)));
+        const int64_t row = h ? row1 : row0;
+        if (row < p.m) *reinterpret_cast<uint32_t*>(cp + row * p.n_part) = y;
+      }
     }
-  }
+  };
+  store(acc0, 0);
+  if (has_hi) store(acc1, 1);
 }
 
 template <typename T, bool kRowScale>

@@ -33,7 +33,7 @@
 extern "C" {
 #endif
 
-#define TDB200_ABI_VERSION 1
+#define TDB200_ABI_VERSION 2
 
 #define TDB200_OK 0
 #define TDB200_ERR_INVALID_ARG (-1)  /* null pointer, bad size, misaligned buffer            */
@@ -150,102 +150,69 @@ int tdb200_rms_norm_rope_table(const void* x, int dtype, const float* w, const f
 
 /* ---------------------------------------------------------------------------------------------
  * a7-a10. SLA / SageSLA.  q, k, v, out are [b, l, h, d] contiguous 16-bit (the layout the module is
- * called with, SLA/core.py:181-183), d in {64, 128}.  Block sizes: BLKQ = 128 query rows, BLKK = 64 key rows
- * (the non-sm90 branch, SLA/core.py:191-193).  mblk = ceil(l/128), nblk = ceil(l/64).  The *_blocks entry points also
- * serve the sm90 branch's BLKQ = 64, BLKK = 128 (mblk = ceil(l/64), nblk = ceil(l/128)).
+ * called with, SLA/core.py:181-183), d in {64, 128}.
+ * Block families (blkq, blkk): (128, 64), the non-sm90 branch of SLA/core.py:191-193, or (64, 128), SpargeAttn's Hopper family
+ * (SLA/core.py:191-193, 226-229); any other pair returns TDB200_ERR_UNSUPPORTED.
+ * mblk = ceil(query rows / blkq), nblk = ceil(key rows / blkk).
+ * INT8 K layouts: head-major [b,h,lk,d] (tdb200_sla_quant_qk), or sequence-major [b,lk,h,d] (tdb200_sla_quant_k_seq), the layout
+ * in which sequence-parallel ranks all-gather their key rows.
  *
  * tdb200_sla_quant_qk   one pass over q [b,lq,h,d] and two over k [b,lk,h,d] (lq != lk when the query rows are one rank's
- *     sequence shard and k is the gathered key slab; mblk = ceil(lq/128), nblk = ceil(lk/64)):
+ *     sequence shard and k is the gathered key slab):
  *     kmean  [b,h,d]  fp32   = sum_l k / l  (T-rounded copy is what is subtracted, SLA/utils.py:56)
- *     q_i8   [b,h,l,d] int8, q_scale [b,h,mblk];  k_i8 [b,h,l,d] int8 of T(k - T(kmean)), k_scale [b,h,nblk]
- *                             scale = amax/127 + 1e-7, round half away from zero (SpargeAttn get_vanilla_qk_quant)
+ *     q_i8   [b,h,lq,d] int8 per blkq rows, q_scale [b,h,mblk];  k_i8 [b,h,lk,d] int8 of T(k - T(kmean)) per blkk rows,
+ *     k_scale [b,h,nblk]      scale = amax/127 + 1e-7, round half away from zero (SpargeAttn get_vanilla_qk_quant)
  *     q_pool [b,h,mblk,d] T,  k_pool [b,h,nblk,d] T   block means (SLA/utils.py:21-52; actual row count in the tail)
  *     q == NULL or k == NULL runs only the other half (the sequence-parallel path prepares Q while the K/V all-gather
- *     is still in flight).
+ *     is still in flight); the pair (blkq, blkk) must still be one of the two families.
  * tdb200_sla_block_map  pooled score T(q_pool . k_pool^T), top-`topk` per row (ties -> lowest index),
  *     sparse_map [b,h,mblk,nblk] int8 0/1 (SLA/utils.py:64-66) and lut [b,h,mblk,topk] int32 ascending block ids.
- * tdb200_sla_linear_moments   phi = softmax over d;  kv [b,h,d(v),d(k)] fp32 = sum_l v[l,:]^T phi(k)[l,:],
- *     ksum [b,h,d] fp32 = sum_l phi(k)[l,:]   (SLA/core.py:243-247).  Both must be zeroed by the caller
- *     (they are accumulated, so sequence shards can be summed with one all-reduce).
+ * tdb200_sla_linear_moments   phi = feature map of the keys: 0 softmax over d, 1 elu+1, 2 relu (SLA/core.py:57-73);
+ *     kv [b,h,d(v),d(k)] fp32 = sum_l v[l,:]^T phi(k)[l,:], ksum [b,h,d] fp32 = sum_l phi(k)[l,:]   (SLA/core.py:243-247).
+ *     Both must be zeroed by the caller (they are accumulated, so sequence shards can be summed with one all-reduce).
+ * tdb200_sla_project_moments  kvw [bh,d,d] T = T(proj_w [d,d] . kv [bh,d,d]): folds proj_l's weight (SLA/core.py:246
+ *     `self.proj_l(o_l)`) into the moment matrix so the fused kernel applies it with its last MMA; fp32 FMA chain over d_v.
  * tdb200_sla_attn_fwd   o = T( sparse_softmax_attention(q_i8,k_i8,v; lut) + proj( phi(q) kv / (1e-5 + phi(q).ksum) ) )
- *     kvw [b,h,d(out),d(k)] T = (proj_w . kv) so that proj is folded into the moment matrix; proj_b [d] fp32.
- *     The int8 QK^T, online softmax (exp2), PV, linear branch and merge run in one wgmma kernel.
+ *     q_i8 / q_scale / k_scale as tdb200_sla_quant_qk made them, lut [b,h,mblk,topk] of blkk-row key blocks (1 <= topk <= nblk),
+ *     kvw [b,h,d(out),d(k)] T = (proj_w . kv) so that proj is folded into the moment matrix, proj_b [d] fp32; `feature` is the
+ *     map the moments were built with.  The int8 QK^T, online softmax (exp2), PV, linear branch and merge run in one wgmma
+ *     kernel; with (64, 128) one CTA per 64-row query block runs two consumer warpgroups on alternate key blocks and merges
+ *     their softmax states.  k_seq_major != 0 reads k_i8 in the sequence-major layout [1,lk,h,d] (rows past lk may follow);
+ *     it is implemented for d = 128, the softmax map and b = 1, other calls return TDB200_ERR_UNSUPPORTED.
  * ------------------------------------------------------------------------------------------- */
 int tdb200_sla_quant_qk(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d,
                         float* kmean, int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale, void* q_pool,
-                        void* k_pool, void* stream);
+                        void* k_pool, int64_t blkq, int64_t blkk, void* stream);
 int tdb200_sla_block_map(const void* q_pool, const void* k_pool, int dtype, int64_t b, int64_t h, int64_t mblk,
                          int64_t nblk, int64_t d, int64_t topk, int8_t* sparse_map, int32_t* lut, void* stream);
 int tdb200_sla_linear_moments(const void* k, const void* v, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
-                              float* kv, float* ksum, void* stream);
-/* Same with the feature map of the linear branch selectable (0 softmax, 1 elu+1, 2 relu; SLA/core.py:57-73) and head dim
- * 64 or 128 (kv [b,h,d,d], ksum [b,h,d]). */
-int tdb200_sla_linear_moments_ex(const void* k, const void* v, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
-                                 int feature, float* kv, float* ksum, void* stream);
-/* kvw [bh,d,d] T = T(proj_w [d,d] . kv [bh,d,d]): folds proj_l's weight (SLA/core.py:246 `self.proj_l(o_l)`) into the moment
- * matrix so the fused kernel applies it with its last MMA; fp32 FMA chain over d_v. */
+                              int feature, float* kv, float* ksum, void* stream);
 int tdb200_sla_project_moments(const float* proj_w, const float* kv, int dtype, int64_t bh, int64_t d, void* kvw, void* stream);
 int tdb200_sla_attn_fwd(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
                         const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk, const void* kvw,
                         const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
-                        int64_t h, int64_t d, float sm_scale, void* stream);
+                        int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq, int64_t blkk,
+                        int k_seq_major, void* stream);
 /* Sequence-parallel form of the key half of tdb200_sla_quant_qk (reference: the context-parallel attention of
  * rcm/utils/a2a_cp.py:66-182 exchanges 16-bit K; here each rank quantises its own key rows and the INT8 tensor travels).
  *   tdb200_sla_kmean_partial  partial [b,h,ceil(l/128),d] fp32 = column sums of each 128-row chunk of k [b,l,h,d];
  *   tdb200_sla_kmean_final    kmean [b,h,d] = (fixed-order sum of `chunks` partials) / l_total  -- the reduction
- *                             tdb200_sla_quant_qk runs, so gathering every rank's partials reproduces its mean bit for bit;
- *   tdb200_sla_quant_k_seq    smoothed Sage INT8 of k's rows: k_i8 in the INPUT layout [b,l,h,d], k_scale [b,h,ceil(l/64)],
- *                             k_pool [b,h,ceil(l/64),d];
- *   tdb200_sla_attn_fwd_kseq  tdb200_sla_attn_fwd with k_i8 in that [b,lk,h,d] layout. */
+ *                             tdb200_sla_quant_qk runs, so gathering every rank's partials reproduces its mean bit for bit
+ *                             (the 128-row partials serve both block families);
+ *   tdb200_sla_quant_k_seq    smoothed Sage INT8 of k's rows per blkk rows, blkk = 64 or 128: k_i8 in the sequence-major
+ *                             layout [b,l,h,d], k_scale [b,h,ceil(l/blkk)], k_pool [b,h,ceil(l/blkk),d]. */
 int tdb200_sla_kmean_partial(const void* k, int dtype, int64_t b, int64_t l, int64_t h, int64_t d, float* partial, void* stream);
 int tdb200_sla_kmean_final(const float* partial, int64_t b, int64_t h, int64_t chunks, int64_t d, int64_t l_total, float* kmean,
                            void* stream);
 int tdb200_sla_quant_k_seq(const void* k, const float* kmean, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
-                           int8_t* k_i8, float* k_scale, void* k_pool, void* stream);
-int tdb200_sla_attn_fwd_kseq(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
-                             const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk, const void* kvw,
-                             const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
-                             int64_t h, int64_t d, float sm_scale, void* stream);
+                           int8_t* k_i8, float* k_scale, void* k_pool, int64_t blkk, void* stream);
 /* The non-quantised SLA path (reference: Triton _attn_fwd, turbodiffusion/SLA/kernel.py:33-82, used by SparseLinearAttention
  * when --attention_type sla): the same fused kernel with Q.K^T as a 16-bit tensor-core product on the un-quantised q, k
- * [b,l,h,d] (fp32 scores, exp2 softmax, P rounded to T before P.V, :60-73); no q/k scales, no key smoothing. */
+ * [b,l,h,d] (fp32 scores, exp2 softmax, P rounded to T before P.V, :60-73); no q/k scales, no key smoothing.
+ * d = 128, (blkq, blkk) = (128, 64), softmax map. */
 int tdb200_sla_attn_fwd_qk16(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
                              const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l,
                              int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream);
-/* Second-generation fused kernel (persistent tiles, two softmax threads per query row, linear branch folded into the
- * P.V accumulator); same arguments plus `feature`: 0 softmax, 1 elu+1, 2 relu feature map of the linear branch
- * (SLA/core.py:57-73; the moments must have been built with the same map). */
-int tdb200_sla_attn_fwd_v2(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
-                           const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk, const void* kvw,
-                           const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
-                           int64_t h, int64_t d, float sm_scale, int feature, void* stream);
-/* The SageSLA pair with the block geometry as an argument: (blkq, blkk) = (128, 64), the sizes of the entry points above, or
- * (64, 128), SpargeAttn's Hopper family (SLA/core.py:191-193, 226-229).  Any other pair returns TDB200_ERR_UNSUPPORTED.
- *   tdb200_sla_quant_qk_blocks  tdb200_sla_quant_qk with q pooled / quantised per blkq rows and smoothed k per blkk rows:
- *                               q_scale [b,h,ceil(lq/blkq)], q_pool [b,h,ceil(lq/blkq),d], k_scale [b,h,ceil(lk/blkk)],
- *                               k_pool [b,h,ceil(lk/blkk),d]; kmean and the code layouts are unchanged.
- *   tdb200_sla_attn_fwd_blocks  tdb200_sla_attn_fwd_v2 on those blocks (lut [b,h,ceil(l/blkq),topk] of blkk-row key blocks);
- *                               (128, 64) is tdb200_sla_attn_fwd_v2 itself.  With (64, 128) one CTA per 64-row query block
- *                               runs two consumer warpgroups on alternate key blocks and merges their softmax states. */
-int tdb200_sla_quant_qk_blocks(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d,
-                               float* kmean, int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale, void* q_pool,
-                               void* k_pool, int64_t blkq, int64_t blkk, void* stream);
-int tdb200_sla_attn_fwd_blocks(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
-                               const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk, const void* kvw,
-                               const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
-                               int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq, int64_t blkk, void* stream);
-/* The sequence-parallel key half on either block family (the gathered key mean and its 128-row partials serve both):
- *   tdb200_sla_quant_k_seq_blocks   tdb200_sla_quant_k_seq pooling / quantising per blkk rows, blkk = 64 or 128: k_i8 in the
- *                                   input layout [b,l,h,d], k_scale [b,h,ceil(l/blkk)], k_pool [b,h,ceil(l/blkk),d]; 64 is
- *                                   tdb200_sla_quant_k_seq itself.
- *   tdb200_sla_attn_fwd_kseq_blocks tdb200_sla_attn_fwd_kseq on (blkq, blkk) = (128, 64), which is that call itself, or (64, 128);
- *                                   d = 128, softmax map, b = 1, k_i8 in [1,lk,h,d].  Other pairs return TDB200_ERR_UNSUPPORTED. */
-int tdb200_sla_quant_k_seq_blocks(const void* k, const float* kmean, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
-                                  int8_t* k_i8, float* k_scale, void* k_pool, int64_t blkk, void* stream);
-int tdb200_sla_attn_fwd_kseq_blocks(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
-                                    const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk, const void* kvw,
-                                    const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
-                                    int64_t h, int64_t d, float sm_scale, int64_t blkq, int64_t blkk, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * a9' backward. Gradients of the block-sparse 16-bit attention (the sparse branch of SparseLinearAttention; reference: the

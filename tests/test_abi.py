@@ -40,7 +40,7 @@ def test_ctypes_binding_matches_header(libpath):
     from turbodiffusion_b200 import _lib
     assert sorted(_lib.exported_names()) == _declared()
     lib = _lib.lib()  # raises if any prototype names a missing symbol
-    assert lib.tdb200_abi_version() == 1
+    assert lib.tdb200_abi_version() == _lib.ABI_VERSION == 2
     assert lib.tdb200_last_error() is not None
 
 
@@ -88,28 +88,28 @@ def test_argument_validation_of_every_kernel_family(libpath):
         ("gemm epilogue", lambda: lib.tdb200_gemm_w8a8_ex(_p(), _p(), _p(), _p(), None, _p(), 0, 128, 128, 128, 9, None), INVALID, b"epilogue"),
         ("rowwise null", lambda: lib.tdb200_gemm_w8a8_rowwise(_p(), _p(), _p(), _p(), None, None, 0, 128, 128, 128, None), INVALID, b"null"),
         ("rowquant k%8", lambda: lib.tdb200_quant_int8_rowwise(_p(), 0, 4, 12, _p(), _p(), None), INVALID, b"shape"),
-        ("sla prep head dim", lambda: lib.tdb200_sla_quant_qk(_p(), _p(), 0, 1, 256, 256, 2, 96, _p(), _p(), _p(), _p(), _p(), _p(), _p(), None),
-         UNSUPPORTED, b"head dim"),
+        ("sla prep head dim", lambda: lib.tdb200_sla_quant_qk(_p(), _p(), 0, 1, 256, 256, 2, 96, _p(), _p(), _p(), _p(), _p(), _p(), _p(), 128,
+                                                              64, None), UNSUPPORTED, b"head dim"),
         ("block map topk", lambda: lib.tdb200_sla_block_map(_p(), _p(), 0, 1, 2, 4, 8, 128, 9, _p(), _p(), None), INVALID, b"topk"),
-        ("moments head dim", lambda: lib.tdb200_sla_linear_moments(_p(), _p(), 0, 1, 256, 2, 96, _p(), _p(), None), UNSUPPORTED, b"head dim"),
-        ("moments feature map", lambda: lib.tdb200_sla_linear_moments_ex(_p(), _p(), 0, 1, 256, 2, 64, 7, _p(), _p(), None), INVALID, b"feature"),
-        ("attn v2 head dim", lambda: lib.tdb200_sla_attn_fwd_v2(_p(), _p(), _p(), _p(), _p(), _p(), 0, _p(), 4, _p(), _p(), _p(), _p(), 1, 256,
-                                                                256, 2, 96, 0.088, 0, None), UNSUPPORTED, b"head dim"),
+        ("moments head dim", lambda: lib.tdb200_sla_linear_moments(_p(), _p(), 0, 1, 256, 2, 96, 0, _p(), _p(), None), UNSUPPORTED, b"head dim"),
+        ("moments feature map", lambda: lib.tdb200_sla_linear_moments(_p(), _p(), 0, 1, 256, 2, 64, 7, _p(), _p(), None), INVALID, b"feature"),
+        ("attn head dim", lambda: lib.tdb200_sla_attn_fwd(_p(), _p(), _p(), _p(), _p(), _p(), 0, _p(), 4, _p(), _p(), _p(), _p(), 1, 256,
+                                                          256, 2, 96, 0.088, 0, 128, 64, 0, None), UNSUPPORTED, b"head dim"),
         ("gelu quant k", lambda: lib.tdb200_gelu_quant_int8_block128(_p(), 0, 128, 100, _p(), _p(), None), UNSUPPORTED, b"multiple of 8"),
-        ("attn kseq batch", lambda: lib.tdb200_sla_attn_fwd_kseq(_p(), _p(), _p(), _p(), _p(), _p(), 0, _p(), 4, _p(), _p(), _p(), _p(), 2, 256,
-                                                                 256, 2, 128, 0.088, None), UNSUPPORTED, b"batch"),
+        ("attn sequence-major K batch", lambda: lib.tdb200_sla_attn_fwd(_p(), _p(), _p(), _p(), _p(), _p(), 0, _p(), 4, _p(), _p(), _p(), _p(),
+                                                                        2, 256, 256, 2, 128, 0.088, 0, 128, 64, 1, None), UNSUPPORTED, b"batch"),
         ("split parts", lambda: lib.tdb200_gemm_w8a8_split(_p(), _p(), _p(), _p(), None, _p(), 0, 128, 768, 128, 2, None), UNSUPPORTED,
          b"parts"),
         ("split null", lambda: lib.tdb200_gemm_w8a8_split(_p(), _p(), _p(), _p(), None, None, 0, 128, 512, 128, 2, None), INVALID, b"null"),
         ("kmean partial head dim", lambda: lib.tdb200_sla_kmean_partial(_p(), 0, 1, 256, 2, 96, _p(), None), UNSUPPORTED, b"head dim"),
         ("kmean final null", lambda: lib.tdb200_sla_kmean_final(None, 1, 2, 2, 128, 256, _p(), None), INVALID, b"null"),
-        ("quant k seq null", lambda: lib.tdb200_sla_quant_k_seq(_p(), None, 0, 1, 256, 2, 128, _p(), _p(), _p(), None), INVALID, b"null"),
+        ("quant k seq null", lambda: lib.tdb200_sla_quant_k_seq(_p(), None, 0, 1, 256, 2, 128, _p(), _p(), _p(), 64, None), INVALID, b"null"),
         ("project moments head dim", lambda: lib.tdb200_sla_project_moments(_p(), _p(), 0, 4, 96, _p(), None), UNSUPPORTED, b"head dim"),
         ("rope table null", lambda: lib.tdb200_rms_norm_rope_table(None, 0, _p(), _p(), _p(), 64, 2, 128, 1e-6, None), INVALID, b"null"),
         ("attn null", lambda: lib.tdb200_sla_attn_fwd(None, _p(), _p(), _p(), _p(), _p(), 0, _p(), 4, _p(), _p(), _p(), _p(), 1, 256, 256, 2,
-                                                      128, 0.088, None), INVALID, b"null"),
+                                                      128, 0.088, 0, 128, 64, 0, None), INVALID, b"null"),
         ("attn topk", lambda: lib.tdb200_sla_attn_fwd(_p(), _p(), _p(), _p(), _p(), _p(), 0, _p(), 9, _p(), _p(), _p(), _p(), 1, 256, 256, 2,
-                                                      128, 0.088, None), INVALID, b"topk"),
+                                                      128, 0.088, 0, 128, 64, 0, None), INVALID, b"topk"),
     ]
     for name, call, code, needle in cases:
         rc = call()

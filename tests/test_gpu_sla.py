@@ -439,7 +439,7 @@ def test_split_key_prep_equals_the_fused_one(cuda, l, h, d, shards):
 
 
 def test_attention_reads_sequence_major_int8_keys(cuda):
-    """tdb200_sla_attn_fwd_kseq (INT8 K in the gathered [B, Lk, H, D] layout, key rows padded past lk) == tdb200_sla_attn_fwd."""
+    """tdb200_sla_attn_fwd on INT8 K in the gathered [B, Lk, H, D] layout (k_seq_major, key rows padded past lk) == on head-major K."""
     from turbodiffusion_b200.SLA.core import attn_fwd, linear_moments
     from turbodiffusion_b200.SLA.utils import block_map_from_pools, quant_qk
     b, l, h, d = 1, 1000, 3, 128

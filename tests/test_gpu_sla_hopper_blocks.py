@@ -64,33 +64,6 @@ def test_quant_qk_hopper_blocks_codes_scales_pools(sm90, b, l, h, d, dtype):
     assert torch.equal(prep.k_i8.cpu(), k_i8), (prep.k_i8.cpu() != k_i8).sum()
 
 
-@pytest.mark.parametrize("d,feature", [(128, 0), (64, 1)])
-def test_default_family_through_the_block_entry_points(cuda, d, feature):
-    """(128, 64) through tdb200_sla_quant_qk_blocks / tdb200_sla_attn_fwd_blocks == tdb200_sla_quant_qk / _v2, bit for bit."""
-    from turbodiffusion_b200._lib import DTYPE_TAG, lib, ptr, stream_ptr
-    from turbodiffusion_b200.SLA.core import attn_fwd, linear_moments, project_moments
-    from turbodiffusion_b200.SLA.utils import block_map_from_pools, quant_qk
-    b, l, h = 2, 700, 3
-    q, k, v = (t.to(cuda) for t in _qkv(b, l, h, d, 11 + d))
-    prep = quant_qk(q, k)
-    ref = {n: torch.empty_like(getattr(prep, n)) for n in ("kmean", "q_i8", "q_scale", "k_i8", "k_scale", "q_pool", "k_pool")}
-    assert lib().tdb200_sla_quant_qk(ptr(q), ptr(k), DTYPE_TAG[q.dtype], b, l, l, h, d, *(ptr(ref[n]) for n in ref),
-                                     stream_ptr(cuda)) == 0
-    for n in ref:
-        assert torch.equal(getattr(prep, n), ref[n]), n
-    topk = 4
-    _, lut = block_map_from_pools(prep.q_pool, prep.k_pool, topk)
-    kv, ksum = linear_moments(k, v, feature)
-    kvw = project_moments(torch.randn(d, d, device=cuda) * 0.05, kv, q.dtype)
-    pb = torch.randn(d, device=cuda) * 0.05
-    got = attn_fwd(prep, v, q, lut, topk, kvw, ksum, pb, d ** -0.5, feature=feature)
-    want = torch.empty_like(q)
-    assert lib().tdb200_sla_attn_fwd_v2(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v), ptr(q),
-                                        DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(pb), ptr(want), b, l, l, h, d,
-                                        float(d ** -0.5), feature, stream_ptr(cuda)) == 0
-    assert torch.equal(got, want)
-
-
 def _check_topk(scores, sm, lt, topk):
     """`sm` is a top-k of `scores` up to one 16-bit ulp at the threshold; LUT ascending and equal to the map."""
     assert (sm.sum(-1) == topk).all()

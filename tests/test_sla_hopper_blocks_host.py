@@ -1,5 +1,5 @@
-"""CPU checks of the Hopper SageSLA block family (BLKQ=64, BLKK=128): argument validation of the *_blocks entry points, the
-served-arch switch and the sequence-parallel refusal under "sm90"."""
+"""CPU checks of the Hopper SageSLA block family (BLKQ=64, BLKK=128): argument validation of the block sizes and head-major
+shapes in tdb200_sla_quant_qk / tdb200_sla_attn_fwd, the served-arch switch and the sequence-parallel refusal under "sm90"."""
 import ctypes
 
 import pytest
@@ -17,13 +17,12 @@ def lib():
 
 
 def _quant(lib, d=128, blkq=64, blkk=128):
-    return lib.tdb200_sla_quant_qk_blocks(_p(), _p(), 0, 1, 256, 256, 2, d, _p(), _p(), _p(), _p(), _p(), _p(),
-                                          _p(), blkq, blkk, None)
+    return lib.tdb200_sla_quant_qk(_p(), _p(), 0, 1, 256, 256, 2, d, _p(), _p(), _p(), _p(), _p(), _p(), _p(), blkq, blkk, None)
 
 
 def _attn(lib, d=128, blkq=64, blkk=128, topk=1, q_i8=None, dtype=0):
-    return lib.tdb200_sla_attn_fwd_blocks(_p() if q_i8 is None else q_i8, _p(), _p(), _p(), _p(), _p(), dtype, _p(), topk, _p(),
-                                          _p(), _p(), _p(), 1, 256, 256, 2, d, 0.088, 0, blkq, blkk, None)
+    return lib.tdb200_sla_attn_fwd(_p() if q_i8 is None else q_i8, _p(), _p(), _p(), _p(), _p(), dtype, _p(), topk, _p(), _p(), _p(),
+                                   _p(), 1, 256, 256, 2, d, 0.088, 0, blkq, blkk, 0, None)
 
 
 def test_argument_validation_of_the_block_entry_points(lib):
@@ -32,8 +31,8 @@ def test_argument_validation_of_the_block_entry_points(lib):
         ("quant block pair", lambda: _quant(lib, blkq=64, blkk=64), UNSUPPORTED, b"block"),
         ("quant block pair 128x128", lambda: _quant(lib, blkq=128, blkk=128), UNSUPPORTED, b"block"),
         ("quant head dim", lambda: _quant(lib, d=96), UNSUPPORTED, b"head dim"),
-        ("quant null", lambda: lib.tdb200_sla_quant_qk_blocks(None, None, 0, 1, 256, 256, 2, 128, _p(), _p(), _p(), _p(), _p(),
-                                                               _p(), _p(), 64, 128, None), INVALID, b"null"),
+        ("quant null", lambda: lib.tdb200_sla_quant_qk(None, None, 0, 1, 256, 256, 2, 128, _p(), _p(), _p(), _p(), _p(), _p(), _p(),
+                                                        64, 128, None), INVALID, b"null"),
         ("attn block pair", lambda: _attn(lib, blkq=32, blkk=128), UNSUPPORTED, b"block"),
         ("attn head dim", lambda: _attn(lib, d=96), UNSUPPORTED, b"head dim"),
         ("attn head dim 128x64", lambda: _attn(lib, d=96, blkq=128, blkk=64), UNSUPPORTED, b"head dim"),

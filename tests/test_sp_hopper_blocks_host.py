@@ -1,6 +1,7 @@
-"""CPU checks of sequence parallelism on the Hopper SageSLA block family (BLKQ=64, BLKK=128): argument validation of the
-sequence-major entry points with a block size, the binding of the hooks to the family they were built for, and `gloo` runs of
-the dist.py plumbing at (64, 128) with the CPU oracle injected as the per-rank primitives."""
+"""CPU checks of sequence parallelism on the Hopper SageSLA block family (BLKQ=64, BLKK=128): argument validation of
+tdb200_sla_quant_k_seq and of tdb200_sla_attn_fwd on sequence-major K with either block family, the binding of the hooks to
+the family they were built for, and `gloo` runs of the dist.py plumbing at (64, 128) with the CPU oracle injected as the
+per-rank primitives."""
 import ctypes
 import os
 import socket
@@ -35,13 +36,12 @@ def lib():
 
 
 def _quant(lib, blkk=128, d=128, kmean=None):
-    return lib.tdb200_sla_quant_k_seq_blocks(_p(), _p() if kmean is None else kmean, 0, 1, 256, 2, d, _p(), _p(), _p(), blkk,
-                                             None)
+    return lib.tdb200_sla_quant_k_seq(_p(), _p() if kmean is None else kmean, 0, 1, 256, 2, d, _p(), _p(), _p(), blkk, None)
 
 
-def _attn(lib, blkq=BQ, blkk=BK, b=1, d=128, topk=1, q_i8=None, dtype=0):
-    return lib.tdb200_sla_attn_fwd_kseq_blocks(_p() if q_i8 is None else q_i8, _p(), _p(), _p(), _p(), _p(), dtype, _p(), topk,
-                                               _p(), _p(), _p(), _p(), b, 256, 256, 2, d, 0.088, blkq, blkk, None)
+def _attn(lib, blkq=BQ, blkk=BK, b=1, d=128, topk=1, q_i8=None, dtype=0, feature=0):
+    return lib.tdb200_sla_attn_fwd(_p() if q_i8 is None else q_i8, _p(), _p(), _p(), _p(), _p(), dtype, _p(), topk, _p(), _p(), _p(),
+                                   _p(), b, 256, 256, 2, d, 0.088, feature, blkq, blkk, 1, None)
 
 
 def test_argument_validation_of_the_sequence_major_block_entry_points(lib):
@@ -57,6 +57,7 @@ def test_argument_validation_of_the_sequence_major_block_entry_points(lib):
         ("attn batch 128x64", lambda: _attn(lib, b=2, blkq=128, blkk=64), UNSUPPORTED, b"batch"),
         ("attn head dim", lambda: _attn(lib, d=64), UNSUPPORTED, b"head dim"),
         ("attn head dim 128x64", lambda: _attn(lib, d=64, blkq=128, blkk=64), UNSUPPORTED, b"head dim"),
+        ("attn feature map", lambda: _attn(lib, feature=1), UNSUPPORTED, b"feature"),
         ("attn null", lambda: _attn(lib, q_i8=ctypes.c_void_p(0)), INVALID, b"null"),
         # lk = 256: nblk = 2 for 128-row key blocks, so topk = 3 is out of range ...
         ("attn topk follows blkk", lambda: _attn(lib, topk=3), INVALID, b"topk"),

@@ -30,8 +30,8 @@ def linear_moments(k: torch.Tensor, v: torch.Tensor, feature: int = 0):
     b, l, h, d = k.shape
     buf = torch.zeros(b * h * d * (d + 1), dtype=torch.float32, device=k.device)        # one fill for both accumulators
     kv, ksum = buf[: b * h * d * d].view(b, h, d, d), buf[b * h * d * d:].view(b, h, d)
-    check(lib().tdb200_sla_linear_moments_ex(ptr(k), ptr(v), DTYPE_TAG[k.dtype], b, l, h, d, feature, ptr(kv), ptr(ksum),
-                                             stream_ptr(k.device)), "sla_linear_moments")
+    check(lib().tdb200_sla_linear_moments(ptr(k), ptr(v), DTYPE_TAG[k.dtype], b, l, h, d, feature, ptr(kv), ptr(ksum),
+                                          stream_ptr(k.device)), "sla_linear_moments")
     return kv, ksum
 
 
@@ -62,18 +62,12 @@ def _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, featu
     b, l, h, d = q.shape
     lk = v.shape[1] if lk is None else lk
     out = torch.empty_like(q)
-    if getattr(prep, "k_seq_major", False):   # INT8 K in the gathered [B, Lk, H, D] layout (dist.py)
-        if d != 128 or feature != 0:
-            raise NotImplementedError("sequence-major INT8 K is served by the 128-wide softmax kernels only")
-        check(lib().tdb200_sla_attn_fwd_kseq_blocks(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v),
-                                                    ptr(q), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b),
-                                                    ptr(out), b, l, lk, h, d, float(sm_scale), blkq, blkk, stream_ptr(q.device)),
-              "sla_attn_fwd")
-    else:   # head-major INT8 K: head dims 64 and 128, every feature map, both block geometries
-        check(lib().tdb200_sla_attn_fwd_blocks(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v),
-                                               ptr(q), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b),
-                                               ptr(out), b, l, lk, h, d, float(sm_scale), feature, blkq, blkk,
-                                               stream_ptr(q.device)), "sla_attn_fwd")
+    k_seq_major = int(getattr(prep, "k_seq_major", False))   # INT8 K in the gathered [B, Lk, H, D] layout (dist.py)
+    if k_seq_major and (d != 128 or feature != 0):
+        raise NotImplementedError("sequence-major INT8 K is served by the 128-wide softmax kernels only")
+    check(lib().tdb200_sla_attn_fwd(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v), ptr(q),
+                                    DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b), ptr(out), b, l, lk, h, d,
+                                    float(sm_scale), feature, blkq, blkk, k_seq_major, stream_ptr(q.device)), "sla_attn_fwd")
     return out
 
 

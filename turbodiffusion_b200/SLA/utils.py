@@ -64,9 +64,9 @@ def quant_qk(q: torch.Tensor, k: torch.Tensor, lk: int = None, blkq: int = 128, 
     o.k_scale = torch.empty(b, h, nblk, dtype=torch.float32, device=dev)
     o.q_pool = torch.empty(b, h, mblk, d, dtype=q.dtype, device=dev)
     o.k_pool = torch.empty(b, h, nblk, d, dtype=q.dtype, device=dev)
-    check(lib().tdb200_sla_quant_qk_blocks(ptr(q), ptr(k), DTYPE_TAG[q.dtype], b, lq, lk, h, d, ptr(o.kmean), ptr(o.q_i8),
-                                           ptr(o.q_scale), ptr(o.k_i8), ptr(o.k_scale), ptr(o.q_pool), ptr(o.k_pool), blkq, blkk,
-                                           stream_ptr(dev)), "sla_quant_qk_blocks")
+    check(lib().tdb200_sla_quant_qk(ptr(q), ptr(k), DTYPE_TAG[q.dtype], b, lq, lk, h, d, ptr(o.kmean), ptr(o.q_i8), ptr(o.q_scale),
+                                    ptr(o.k_i8), ptr(o.k_scale), ptr(o.q_pool), ptr(o.k_pool), blkq, blkk, stream_ptr(dev)),
+          "sla_quant_qk")
     return o
 
 
@@ -81,9 +81,9 @@ def quant_q_only(q: torch.Tensor, blkq: int = 128) -> QKPrep:
     o.q_scale = torch.empty(b, h, o.mblk, dtype=torch.float32, device=dev)
     o.q_pool = torch.empty(b, h, o.mblk, d, dtype=q.dtype, device=dev)
     # the key block size only matters to the key half; any valid pair with this blkq serves
-    check(lib().tdb200_sla_quant_qk_blocks(ptr(q), None, DTYPE_TAG[q.dtype], b, lq, lq, h, d, None, ptr(o.q_i8), ptr(o.q_scale),
-                                           None, None, ptr(o.q_pool), None, blkq, 64 if blkq == 128 else 128, stream_ptr(dev)),
-          "sla_quant_qk_blocks", launches=1)
+    check(lib().tdb200_sla_quant_qk(ptr(q), None, DTYPE_TAG[q.dtype], b, lq, lq, h, d, None, ptr(o.q_i8), ptr(o.q_scale), None,
+                                    None, ptr(o.q_pool), None, blkq, 64 if blkq == 128 else 128, stream_ptr(dev)),
+          "sla_quant_qk", launches=1)
     return o
 
 
@@ -97,9 +97,9 @@ def quant_k_into(o: QKPrep, k: torch.Tensor, lk: int, blkk: int = 64) -> QKPrep:
     o.k_i8 = torch.empty(b, h, lk, d, dtype=torch.int8, device=dev)
     o.k_scale = torch.empty(b, h, o.nblk, dtype=torch.float32, device=dev)
     o.k_pool = torch.empty(b, h, o.nblk, d, dtype=k.dtype, device=dev)
-    check(lib().tdb200_sla_quant_qk_blocks(None, ptr(k), DTYPE_TAG[k.dtype], b, lk, lk, h, d, ptr(o.kmean), None, None,
-                                           ptr(o.k_i8), ptr(o.k_scale), None, ptr(o.k_pool), 128 if blkk == 64 else 64, blkk,
-                                           stream_ptr(dev)), "sla_quant_qk_blocks", launches=3)
+    check(lib().tdb200_sla_quant_qk(None, ptr(k), DTYPE_TAG[k.dtype], b, lk, lk, h, d, ptr(o.kmean), None, None, ptr(o.k_i8),
+                                    ptr(o.k_scale), None, ptr(o.k_pool), 128 if blkk == 64 else 64, blkk, stream_ptr(dev)),
+          "sla_quant_qk", launches=3)
     return o
 
 
@@ -134,8 +134,8 @@ def quant_k_seq(k: torch.Tensor, kmean: torch.Tensor, k_i8=None, blkk: int = 64)
     k_i8 = torch.empty(b, rows, h, d, dtype=torch.int8, device=k.device) if k_i8 is None else k_i8
     k_scale = torch.empty(b, h, nb, dtype=torch.float32, device=k.device)
     k_pool = torch.empty(b, h, nb, d, dtype=k.dtype, device=k.device)
-    check(lib().tdb200_sla_quant_k_seq_blocks(ptr(k), ptr(kmean), DTYPE_TAG[k.dtype], b, rows, h, d, ptr(k_i8), ptr(k_scale),
-                                              ptr(k_pool), blkk, stream_ptr(k.device)), "sla_quant_k_seq")
+    check(lib().tdb200_sla_quant_k_seq(ptr(k), ptr(kmean), DTYPE_TAG[k.dtype], b, rows, h, d, ptr(k_i8), ptr(k_scale),
+                                       ptr(k_pool), blkk, stream_ptr(k.device)), "sla_quant_k_seq")
     return k_i8, k_scale, k_pool
 
 

@@ -41,27 +41,16 @@ _PROTOS = {
     "tdb200_rope_interleaved": [_P, _I, _P, _P, _I64, _I64, _I64, _P],
     "tdb200_rms_norm_rope": [_P, _I, _P, _P, _P, _I64, _I64, _I64, _F, _P],
     "tdb200_rms_norm_rope_table": [_P, _I, _P, _P, _P, _I64, _I64, _I64, _F, _P],
-    "tdb200_sla_quant_qk": [_P, _P, _I, _I64, _I64, _I64, _I64, _I64, _P, _P, _P, _P, _P, _P, _P, _P],
+    "tdb200_sla_quant_qk": [_P, _P, _I, _I64, _I64, _I64, _I64, _I64, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _P],
     "tdb200_sla_block_map": [_P, _P, _I, _I64, _I64, _I64, _I64, _I64, _I64, _P, _P, _P],
-    "tdb200_sla_linear_moments": [_P, _P, _I, _I64, _I64, _I64, _I64, _P, _P, _P],
-    "tdb200_sla_linear_moments_ex": [_P, _P, _I, _I64, _I64, _I64, _I64, _I, _P, _P, _P],
+    "tdb200_sla_linear_moments": [_P, _P, _I, _I64, _I64, _I64, _I64, _I, _P, _P, _P],
     "tdb200_sla_attn_fwd": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F,
-                            _P],
-    "tdb200_sla_attn_fwd_kseq": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F,
-                                 _P],
+                            _I, _I64, _I64, _I, _P],
     "tdb200_sla_project_moments": [_P, _P, _I, _I64, _I64, _P, _P],
     "tdb200_sla_kmean_partial": [_P, _I, _I64, _I64, _I64, _I64, _P, _P],
     "tdb200_sla_kmean_final": [_P, _I64, _I64, _I64, _I64, _I64, _P, _P],
-    "tdb200_sla_quant_k_seq": [_P, _P, _I, _I64, _I64, _I64, _I64, _P, _P, _P, _P],
+    "tdb200_sla_quant_k_seq": [_P, _P, _I, _I64, _I64, _I64, _I64, _P, _P, _P, _I64, _P],
     "tdb200_sla_attn_fwd_qk16": [_P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F, _P],
-    "tdb200_sla_attn_fwd_v2": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F, _I,
-                               _P],
-    "tdb200_sla_quant_qk_blocks": [_P, _P, _I, _I64, _I64, _I64, _I64, _I64, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _P],
-    "tdb200_sla_attn_fwd_blocks": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F,
-                                   _I, _I64, _I64, _P],
-    "tdb200_sla_quant_k_seq_blocks": [_P, _P, _I, _I64, _I64, _I64, _I64, _P, _P, _P, _I64, _P],
-    "tdb200_sla_attn_fwd_kseq_blocks": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64,
-                                        _F, _I64, _I64, _P],
     "tdb200_sla_attn_fwd_qk16_lse": [_P, _P, _P, _I, _P, _I64, _P, _P, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_sla_attn_bwd_qk16": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_sla_attn_bwd_workspace_bytes": [_I64, _I64, _I64, _I64],
@@ -73,6 +62,7 @@ _PROTOS = {
     "tdb200_gemm_w8a8_rowwise": [_P, _P, _P, _P, _P, _P, _I, _I64, _I64, _I64, _P],
 }
 _RESTYPES = {"tdb200_last_error": c_char_p, "tdb200_sla_attn_bwd_workspace_bytes": c_int64}
+ABI_VERSION = 2   # TDB200_ABI_VERSION of include/tdb200.h, whose prototypes _PROTOS mirrors
 
 _lib = None
 
@@ -98,7 +88,7 @@ def lib() -> ctypes.CDLL:
             fn = getattr(handle, name)  # AttributeError if the library does not export a declared symbol
             fn.argtypes = argtypes
             fn.restype = _RESTYPES.get(name, c_int)
-        if handle.tdb200_abi_version() != 1:
+        if handle.tdb200_abi_version() != ABI_VERSION:
             raise Tdb200Error("libtdb200.so ABI version mismatch")
         _lib = _DeviceGuarded(handle)
     return _lib
@@ -134,7 +124,7 @@ class _DeviceGuarded:
 
 
 LAUNCHES = 0  # kernels launched through the C ABI (each entry point documents how many it enqueues)
-_KERNELS_PER_CALL = {"sla_quant_qk": 4, "sla_quant_qk_blocks": 4, "layernorm_modulate_quant": 2, "sla_attn_bwd_qk16": 4}  # upper bounds per entry point
+_KERNELS_PER_CALL = {"sla_quant_qk": 4, "layernorm_modulate_quant": 2, "sla_attn_bwd_qk16": 4}  # upper bounds per entry point
 
 
 def check(rc: int, what: str, launches: int = None) -> None:

@@ -16,9 +16,9 @@
 //   Q/K/KVW are K-major swizzled (128B rows, or 64B rows for 64-wide int8 heads).
 // The O accumulator is only rescaled when a row maximum grows by more than 2^8 (lazy rescale): P stays <= 256, which
 // bf16/fp32 hold exactly as well as P <= 1, and the final O / l normalisation is unchanged.
-// Entry points: tdb200_sla_attn_fwd (INT8 Q/K, head-major K), _kseq (INT8 K in [b, lk, h, d]), _qk16 (16-bit Q/K read from
-// the module layout [b, l, h, d], fp32 scores), _v2 (INT8, head dims 64 and 128, feature maps of the linear branch) and
-// _blocks (_v2 with the block geometry as an argument; 64 x 128 blocks run sla_attn_fwd_q64_kernel, further down).
+// Entry points: tdb200_sla_attn_fwd (INT8 Q/K, head dims 64 and 128, feature maps of the linear branch, K head-major or in
+// [b, lk, h, d], 128 x 64 blocks or 64 x 128 blocks in sla_attn_fwd_q64_kernel further down), _qk16 (16-bit Q/K read from the
+// module layout [b, l, h, d], fp32 scores) and _qk16_lse (its sparse branch and row log-sum-exp, for the backward).
 #include <type_traits>
 
 #include "common.cuh"
@@ -607,7 +607,7 @@ constexpr auto attn_kernel() {
 }
 
 // kQK16: 16-bit Q and K in [b, l, h, d]; otherwise INT8 Q [b*h, l, d] and INT8 K [b, h, lk, d] (or [b, lk, h, d] when k_seq_major).
-// kBQ x kBK: the block geometry, 128 x 64 (sla_attn_fwd_kernel) or 64 x 128 (sla_attn_fwd_q64_kernel, INT8 head-major K only).
+// kBQ x kBK: the block geometry, 128 x 64 (sla_attn_fwd_kernel) or 64 x 128 (sla_attn_fwd_q64_kernel, INT8 Q/K only).
 // kLse (16-bit 128 x 64 only): sparse branch and row log-sum-exp into `lse`; kvw, ksum and proj_b are not read.
 template <int HD, bool kQK16, int kBQ = BLKQ, int kBK = BLKK, bool kLse = false>
 int launch(const void* q_op, const float* q_scale, const void* k_op, const float* k_scale, const void* v, const void* q, int dtype,
@@ -709,53 +709,42 @@ int check_common(const void* q_op, const void* k_op, const void* v, const void* 
 
 }  // namespace
 
+// INT8 Q [b*h, l, d]; INT8 K head-major [b, h, lk, d] or, with k_seq_major, the [1, lk, h, d] slab sequence-parallel ranks
+// all-gather.  Both producers load K at (0, blk*BK, head, b) over the dims (d, lk, h, b), so the sequence-major layout is only a
+// different set of tensor-map strides.  (blkq, blkk) = (128, 64) runs sla_attn_fwd_kernel, (64, 128) sla_attn_fwd_q64_kernel.
 extern "C" int tdb200_sla_attn_fwd(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
                                    const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk,
                                    const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
-                                   int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  if (int rc = check_common(q_i8, k_i8, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
-  if (!q_scale || !k_scale) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: null pointer");
-  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (this kernel implements d=128)", (long long)d);
-  return launch<128, false>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, sm_scale, 0,
-                            false, stream);
-}
-
-// the same kernel reading INT8 K in the [b, lk, h, d] layout (tdb200_sla_quant_k_seq; what sequence-parallel ranks all-gather)
-extern "C" int tdb200_sla_attn_fwd_kseq(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
-                                        const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk,
-                                        const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
-                                        int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  if (int rc = check_common(q_i8, k_i8, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
-  if (!q_scale || !k_scale) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: null pointer");
-  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (this kernel implements d=128)", (long long)d);
-  if (b != 1)
-    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_kseq: batch %lld (the gathered [lk_pad, h, d] key slab is one sequence)", (long long)b);
-  return launch<128, false>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, sm_scale, 0,
-                            true, stream);
-}
-
-// tdb200_sla_attn_fwd_kseq with the block geometry chosen by the caller: (128, 64) is tdb200_sla_attn_fwd_kseq itself, (64, 128)
-// runs sla_attn_fwd_q64_kernel.  Its producer loads K at (0, blk*BK, head, b) over the dims (d, lk, h, b), so the sequence-major
-// layout is only a different set of tensor-map strides.
-extern "C" int tdb200_sla_attn_fwd_kseq_blocks(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
-                                               const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk,
-                                               const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
-                                               int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, int64_t blkq,
-                                               int64_t blkk, void* stream) {
+                                   int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq,
+                                   int64_t blkk, int k_seq_major, void* stream) {
   const bool hopper = blkq == kHopperBlkQ && blkk == kHopperBlkK;
   if (!hopper && !(blkq == BLKQ && blkk == BLKK))
-    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_kseq_blocks: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 128)",
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 128)",
                 (long long)blkq, (long long)blkk);
-  if (!hopper)
-    return tdb200_sla_attn_fwd_kseq(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, d,
-                                    sm_scale, stream);
   if (int rc = check_common(q_i8, k_i8, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
   if (!q_scale || !k_scale) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: null pointer");
-  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (this kernel implements d=128)", (long long)d);
-  if (b != 1)
-    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_kseq: batch %lld (the gathered [lk_pad, h, d] key slab is one sequence)", (long long)b);
-  return launch<128, false, kHopperBlkQ, kHopperBlkK>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out,
-                                                      b, l, lk, h, sm_scale, 0, true, stream);
+  if (k_seq_major) {
+    if (d != 128)
+      return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (sequence-major K is implemented for d=128)", (long long)d);
+    if (feature != 0)
+      return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: feature map tag %d (sequence-major K is implemented for softmax)", feature);
+    if (b != 1)
+      return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: batch %lld (the gathered [lk_pad, h, d] key slab is one sequence)", (long long)b);
+  } else {
+    if (d != 64 && d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (64 or 128, SLA/core.py:207)", (long long)d);
+    if (feature < 0 || feature > 2) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: feature map tag %d", feature);
+  }
+#define TDB_LAUNCH(HD, BQ, BK)                                                                                             \
+  return launch<HD, false, BQ, BK>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, \
+                                   sm_scale, feature, k_seq_major != 0, stream)
+  // the order of these instantiations is the order nvcc compiles the kernels in, which changes the code it emits for them
+  if (d == 128) {
+    if (!hopper) TDB_LAUNCH(128, BLKQ, BLKK);
+    TDB_LAUNCH(128, kHopperBlkQ, kHopperBlkK);
+  }
+  if (!hopper) TDB_LAUNCH(64, BLKQ, BLKK);
+  TDB_LAUNCH(64, kHopperBlkQ, kHopperBlkK);
+#undef TDB_LAUNCH
 }
 
 extern "C" int tdb200_sla_attn_fwd_qk16(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
@@ -776,45 +765,4 @@ extern "C" int tdb200_sla_attn_fwd_qk16_lse(const void* q, const void* k, const 
   if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_qk16_lse: head dim %lld (this kernel implements d=128)", (long long)d);
   return launch<128, true, BLKQ, BLKK, true>(q, nullptr, k, nullptr, v, q, dtype, lut, topk, nullptr, nullptr, nullptr, o_s, b, l, l, h,
                                              sm_scale, 0, false, stream, lse);
-}
-
-extern "C" int tdb200_sla_attn_fwd_v2(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
-                                      const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk,
-                                      const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
-                                      int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, int feature,
-                                      void* stream) {
-  if (int rc = check_common(q_i8, k_i8, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
-  if (!q_scale || !k_scale) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: null pointer");
-  if (d != 64 && d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (64 or 128, SLA/core.py:207)", (long long)d);
-  if (feature < 0 || feature > 2) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: feature map tag %d", feature);
-  if (d == 128)
-    return launch<128, false>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, sm_scale,
-                              feature, false, stream);
-  return launch<64, false>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, sm_scale,
-                           feature, false, stream);
-}
-
-// tdb200_sla_attn_fwd_v2 with the block geometry chosen by the caller: (blkq, blkk) = (128, 64) is tdb200_sla_attn_fwd_v2 itself,
-// (64, 128) runs sla_attn_fwd_q64_kernel (mblk = ceil(l/64), nblk = ceil(lk/128)).
-extern "C" int tdb200_sla_attn_fwd_blocks(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
-                                          const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk,
-                                          const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
-                                          int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, int feature,
-                                          int64_t blkq, int64_t blkk, void* stream) {
-  const bool hopper = blkq == kHopperBlkQ && blkk == kHopperBlkK;
-  if (!hopper && !(blkq == BLKQ && blkk == BLKK))
-    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_blocks: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 128)",
-                (long long)blkq, (long long)blkk);
-  if (!hopper)
-    return tdb200_sla_attn_fwd_v2(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, d,
-                                  sm_scale, feature, stream);
-  if (int rc = check_common(q_i8, k_i8, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
-  if (!q_scale || !k_scale) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: null pointer");
-  if (d != 64 && d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (64 or 128, SLA/core.py:207)", (long long)d);
-  if (feature < 0 || feature > 2) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: feature map tag %d", feature);
-  if (d == 128)
-    return launch<128, false, kHopperBlkQ, kHopperBlkK>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b,
-                                                        out, b, l, lk, h, sm_scale, feature, false, stream);
-  return launch<64, false, kHopperBlkQ, kHopperBlkK>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum, proj_b, out,
-                                                     b, l, lk, h, sm_scale, feature, false, stream);
 }

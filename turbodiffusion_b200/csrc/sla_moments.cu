@@ -216,8 +216,8 @@ sla_moments_kernel(const __grid_constant__ CUtensorMap tmap_v, MomParams p) {
 
 }  // namespace
 
-static int moments_impl(const void* k, const void* v, int dtype, int64_t b, int64_t l, int64_t h, int64_t d, int feature,
-                        float* kv, float* ksum, void* stream) {
+extern "C" int tdb200_sla_linear_moments(const void* k, const void* v, int dtype, int64_t b, int64_t l, int64_t h,
+                                         int64_t d, int feature, float* kv, float* ksum, void* stream) {
   using namespace tdb;
   if (!k || !v || !kv || !ksum) return fail(TDB200_ERR_INVALID_ARG, "sla_linear_moments: null pointer");
   if (b <= 0 || l <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_linear_moments: bad shape");
@@ -265,16 +265,6 @@ static int moments_impl(const void* k, const void* v, int dtype, int64_t b, int6
 #undef TDB_MOM2
 #undef TDB_MOM
   return fail(TDB200_ERR_UNSUPPORTED, "sla_linear_moments: dtype tag %d", dtype);
-}
-
-extern "C" int tdb200_sla_linear_moments(const void* k, const void* v, int dtype, int64_t b, int64_t l, int64_t h,
-                                         int64_t d, float* kv, float* ksum, void* stream) {
-  return moments_impl(k, v, dtype, b, l, h, d, 0, kv, ksum, stream);
-}
-
-extern "C" int tdb200_sla_linear_moments_ex(const void* k, const void* v, int dtype, int64_t b, int64_t l, int64_t h,
-                                            int64_t d, int feature, float* kv, float* ksum, void* stream) {
-  return moments_impl(k, v, dtype, b, l, h, d, feature, kv, ksum, stream);
 }
 
 // ---- kvw = T(proj_w . kv): the linear branch's output projection folded into the moment matrix (SLA/core.py:243-253:

@@ -217,10 +217,17 @@ int run(const void* q, const void* k, int64_t b, int64_t lq, int64_t l, int64_t 
   return TDB200_OK;
 }
 
-// (blkq, blkk) is (128, 64) or (64, 128); the callers check it
-int quant_qk(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int64_t l, int64_t h, int64_t d, float* kmean,
-             int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale, void* q_pool, void* k_pool, int64_t blkq, int64_t blkk,
-             void* stream) {
+}  // namespace
+
+// Q pooled / quantised per blkq rows, smoothed K per blkk rows, (blkq, blkk) = (128, 64) or (64, 128).  The key mean is the same
+// for both (its 128-row partials do not depend on the block size).
+extern "C" int tdb200_sla_quant_qk(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int64_t l, int64_t h,
+                                   int64_t d, float* kmean, int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale,
+                                   void* q_pool, void* k_pool, int64_t blkq, int64_t blkk, void* stream) {
+  using namespace tdb;
+  if (!((blkq == 128 && blkk == 64) || (blkq == 64 && blkk == 128)))
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_qk: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 128)",
+                (long long)blkq, (long long)blkk);
   if ((!q && !k) || (q && (!q_i8 || !q_scale || !q_pool)) || (k && (!kmean || !k_i8 || !k_scale || !k_pool)))
     return fail(TDB200_ERR_INVALID_ARG, "sla_quant_qk: null pointer");
   if (b <= 0 || l <= 0 || lq <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_quant_qk: bad shape");
@@ -243,26 +250,6 @@ int quant_qk(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int
   }
 #undef TDB_RUN
   return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_qk: dtype tag %d", dtype);
-}
-
-}  // namespace
-
-extern "C" int tdb200_sla_quant_qk(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int64_t l, int64_t h,
-                                   int64_t d, float* kmean, int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale,
-                                   void* q_pool, void* k_pool, void* stream) {
-  return quant_qk(q, k, dtype, b, lq, l, h, d, kmean, q_i8, q_scale, k_i8, k_scale, q_pool, k_pool, 128, 64, stream);
-}
-
-// tdb200_sla_quant_qk with the block geometry chosen by the caller: Q pooled / quantised per blkq rows, smoothed K per blkk rows,
-// (blkq, blkk) = (128, 64) or (64, 128).  The key mean is the same (its 128-row partials do not depend on the block size).
-extern "C" int tdb200_sla_quant_qk_blocks(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int64_t l, int64_t h,
-                                          int64_t d, float* kmean, int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale,
-                                          void* q_pool, void* k_pool, int64_t blkq, int64_t blkk, void* stream) {
-  using namespace tdb;
-  if (!((blkq == 128 && blkk == 64) || (blkq == 64 && blkk == 128)))
-    return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_qk_blocks: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 128)",
-                (long long)blkq, (long long)blkk);
-  return quant_qk(q, k, dtype, b, lq, l, h, d, kmean, q_i8, q_scale, k_i8, k_scale, q_pool, k_pool, blkq, blkk, stream);
 }
 
 // ---- the key half split in three, for sequence-parallel ranks (dist.py): each rank reduces ITS rows to 128-row partial sums,
@@ -295,11 +282,11 @@ extern "C" int tdb200_sla_kmean_final(const float* partial, int64_t b, int64_t h
   return check_launch("kmean_final_kernel");
 }
 
-extern "C" int tdb200_sla_quant_k_seq_blocks(const void* k, const float* kmean, int dtype, int64_t b, int64_t l, int64_t h,
-                                             int64_t d, int8_t* k_i8, float* k_scale, void* k_pool, int64_t blkk, void* stream) {
+extern "C" int tdb200_sla_quant_k_seq(const void* k, const float* kmean, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
+                                      int8_t* k_i8, float* k_scale, void* k_pool, int64_t blkk, void* stream) {
   using namespace tdb;
   if (blkk != 64 && blkk != 128)
-    return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_k_seq_blocks: key block size %lld (BLKK = 64 or 128)", (long long)blkk);
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_k_seq: key block size %lld (BLKK = 64 or 128)", (long long)blkk);
   if (!k || !kmean || !k_i8 || !k_scale || !k_pool) return fail(TDB200_ERR_INVALID_ARG, "sla_quant_k_seq: null pointer");
   if (b <= 0 || l <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_quant_k_seq: bad shape");
   if (d != 64 && d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_k_seq: head dim %lld (64 or 128)", (long long)d);
@@ -319,9 +306,4 @@ extern "C" int tdb200_sla_quant_k_seq_blocks(const void* k, const float* kmean, 
   }
 #undef TDB_RUN
   return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_k_seq: dtype tag %d", dtype);
-}
-
-extern "C" int tdb200_sla_quant_k_seq(const void* k, const float* kmean, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
-                                      int8_t* k_i8, float* k_scale, void* k_pool, void* stream) {
-  return tdb200_sla_quant_k_seq_blocks(k, kmean, dtype, b, l, h, d, k_i8, k_scale, k_pool, 64, stream);
 }

@@ -422,6 +422,10 @@ __device__ __forceinline__ void reg_dealloc() {
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// signal barrier `id` without waiting: the releasing side of an ordering handshake whose waiting side calls named_bar_sync
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 // ------------------------------------------------------------------------------------------
 // 128-bit global memory access helpers (streaming)

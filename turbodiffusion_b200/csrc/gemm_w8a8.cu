@@ -12,10 +12,11 @@
 //            L2, and pays the ring fill and the epilogue once per twice the work (DESIGN.md, a2).
 //   warpgroups 0-1  MMA + dequant + epilogue; warpgroup g owns output rows [64g, 64g+64) of the tile.  Per K-block and
 //            half: four wgmma.m64n128k32.s32.s8.s8 into one 64-register int32 staging accumulator, then the int -> float
-//            conversion and the FFMA with that half's block scale into the half's 64 fp32 registers; the two warpgroups'
-//            dequant and MMA phases interleave on the SM.  The accumulate flag is reset at every K-block because the
-//            reference rescales per K-block.  After the last K-block, per half: round to T, (+bias), (GELU), store.
-//            A half that lies entirely past n is not stored, and in the block-scale variant not multiplied either.
+//            conversion and the FFMA with that half's block scale into the half's 64 fp32 registers.  Both warpgroups
+//            issue together off the same full barrier, so their MMA phases and their dequant phases coincide; ordering
+//            them to alternate (ping-pong, -DTDB200_GEMM_PINGPONG) was measured slower (DESIGN.md, a2).  The
+//            accumulate flag is reset at every K-block because the reference rescales per K-block.  After the last
+//            K-block, per half: round to T, (+bias), (GELU), store.  A half that lies entirely past n is not stored, and in the block-scale variant not multiplied either.
 // Integer accumulation is exact and the fp32 FMA chain runs in ascending kb order, so the result is bit-identical
 // to the reference restatement (oracle.int8_linear) on the same int8 inputs.
 #include "common.cuh"
@@ -193,28 +194,47 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   float acc0[64], acc1[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc0[i] = acc1[i] = 0.0f;
-  // float(s) without the conversion unit: as_float(0x4B400000 + s) == 1.5*2^23 + s exactly for |s| < 2^22 (a K-block sum
-  // is at most 128^3 = 2^21 in magnitude), and subtracting 1.5*2^23 is exact, so this is the same value __int2float_rn gives
-  // on the full-rate integer-add and FP32 pipes
-  constexpr float kMagicF = 12582912.0f;
-  constexpr int kMagicI = 0x4B400000;
   uint32_t ia[64];
+  // float(s) is exact (a K-block sum is at most 128^3 = 2^21 in magnitude).  I2FP + FFMA is two instructions per value
+  // against three for the magic-number conversion (IADD, FADD, FFMA), and measured faster on the H100 (DESIGN.md, a2).
   auto dequant = [&](float (&acc)[64], float scale) {
     wgmma_wait<0>();
     reg_fence(ia);
 #pragma unroll
-    for (int i = 0; i < 64; ++i)
-      acc[i] = __fmaf_rn(__fsub_rn(__int_as_float(static_cast<int>(ia[i]) + kMagicI), kMagicF), scale, acc[i]);
+    for (int i = 0; i < 64; ++i) acc[i] = __fmaf_rn(__int2float_rn(static_cast<int>(ia[i])), scale, acc[i]);
   };
-  for (int kb = 0; kb < p.k_blocks; ++kb) {
+#ifdef TDB200_GEMM_PINGPONG
+  // Experimental ping-pong schedule (DESIGN.md, a2: measured slower, so not built by default).  A turn is one (K-block,
+  // half) of one warpgroup; turns are issued WG0 t0, WG1 t0, WG0 t1, WG1 t1, ...  Named barrier 2 gates WG0 (synced
+  // before its turns 1..T-1, arrived on by WG1 after issuing its turns 0..T-2), barrier 3 gates WG1 (synced before each
+  // of its T turns, arrived on by WG0 after issuing each of its T turns): the counts balance, so nothing is pending at
+  // exit.  Barrier 1 is the quantised epilogue's amax exchange.
+  const int last_turn = p.k_blocks * (has_hi ? 2 : 1) - 1;   // has_hi is CTA-uniform: both warpgroups have T turns
+  auto before_issue = [&](int t) {
+    if (wg == 1) named_bar_sync(3, kConsumerWarps * 32);
+    else if (t > 0) named_bar_sync(2, kConsumerWarps * 32);
+  };
+  auto after_commit = [&](int t) {
+    if (wg == 0) named_bar_arrive(3, kConsumerWarps * 32);
+    else if (t < last_turn) named_bar_arrive(2, kConsumerWarps * 32);
+  };
+#else
+  auto before_issue = [](int) {};
+  auto after_commit = [](int) {};
+#endif
+  for (int kb = 0, t = 0; kb < p.k_blocks; ++kb) {
     wait_full(kb);
     const float as = __ldg(as_row + kb);
+    before_issue(t);
     issue(ia, kb, 0, false);
     wgmma_commit();
+    after_commit(t++);
     dequant(acc0, as * __ldg(bs_row0 + kb));
     if (has_hi) {
+      before_issue(t);
       issue(ia, kb, 1, false);
       wgmma_commit();
+      after_commit(t++);
       dequant(acc1, as * __ldg(bs_row1 + kb));
     }
     release(kb);

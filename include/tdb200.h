@@ -206,30 +206,47 @@ int tdb200_sla_kmean_final(const float* partial, int64_t b, int64_t h, int64_t c
                            void* stream);
 int tdb200_sla_quant_k_seq(const void* k, const float* kmean, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
                            int8_t* k_i8, float* k_scale, void* k_pool, int64_t blkk, void* stream);
-/* The non-quantised SLA path (reference: Triton _attn_fwd, turbodiffusion/SLA/kernel.py:33-82, used by SparseLinearAttention
- * when --attention_type sla): the same fused kernel with Q.K^T as a 16-bit tensor-core product on the un-quantised q, k
- * [b,l,h,d] (fp32 scores, exp2 softmax, P rounded to T before P.V, :60-73); no q/k scales, no key smoothing.
- * d = 128, (blkq, blkk) = (128, 64), softmax map. */
+/* ---------------------------------------------------------------------------------------------
+ * a9'. The non-quantised SLA path (SparseLinearAttention, --attention_type sla; reference: the Triton _attn_fwd, its autograd
+ * function `_attention` and its backward, turbodiffusion/SLA/kernel.py:21-319).  Q.K^T is a 16-bit tensor-core product on the
+ * un-quantised q, k (fp32 scores, exp2 softmax, P rounded to T before P.V, :60-73); no q/k scales, no key smoothing.
+ * d = 128; q, k, v, out, o_s, d_o, dq, dk, dv are [b, l, h, d] contiguous 16-bit; lut [b,h,mblk,topk] int32 of distinct
+ * blkk-row key-block ids per row (1 <= topk <= nblk).
+ * Block sizes (blkq, blkk): (128, 64), the configuration TurboDiffusion's modify_model.py requests, or (64, 64), the module's
+ * default (the reference's BLOCK_M = 64 kernels); any other pair returns TDB200_ERR_UNSUPPORTED.  With (64, 64) one CTA per
+ * 64-row query block runs two consumer warpgroups on alternate key blocks and merges their softmax states (forward) or adds
+ * their dQ / dK / dV partials in a fixed order (backward).
+ *   tdb200_sla_attn16_fwd      o = T( sparse_softmax_attention(q,k,v; lut) + proj( phi(q) kv / (1e-5 + phi(q).ksum) ) ), with
+ *                              kvw, ksum, proj_b and `feature` as for tdb200_sla_attn_fwd (0 softmax, 1 elu+1, 2 relu).
+ *   tdb200_sla_attn16_fwd_lse  o_s = T(the softmax part alone) (no linear branch, no proj_b; lk = l) and lse [b,h,l] fp32 =
+ *                              m + log2(l) of the scores in the log2 domain (S * sm_scale * log2e): the training forward.
+ *   tdb200_sla_attn16_bwd      dq, dk, dv of o_s w.r.t. q, k, v for the incoming gradient d_o, given the forward's o_s and lse.
+ *                              P and dS are rounded to T only as MMA operands, accumulation is fp32, no atomics (bit-for-bit
+ *                              reproducible); key blocks no query block selected get zero dk / dv.  Four kernel launches and
+ *                              no host synchronisation, so the call can be captured in a CUDA graph.
+ *   tdb200_sla_attn16_bwd_workspace_bytes  host-only size of the workspace the backward needs (or a negative error code):
+ *                              delta [b,h,l] fp32, then the key-major index of the LUT: offsets [b*h, nblk+1], cursors
+ *                              [b*h, nblk] and entries [b*h, mblk*topk] int32, each 256-byte aligned (mblk = ceil(l / blkq)).
+ * Errors, all before any CUDA call: an unsupported block pair, d != 128 or a bad dtype tag -> TDB200_ERR_UNSUPPORTED; null pointer,
+ * bad shape, bad feature tag or topk outside [1, nblk] -> TDB200_ERR_INVALID_ARG; workspace_bytes below the size query ->
+ * TDB200_ERR_WORKSPACE.
+ * The four older names below are the same operations at (blkq, blkk) = (128, 64) (and the softmax map for the fused forward):
+ * each is one call of its general form, kept because existing callers link against them.
+ * ------------------------------------------------------------------------------------------- */
+int tdb200_sla_attn16_fwd(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
+                          const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
+                          int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq, int64_t blkk, void* stream);
+int tdb200_sla_attn16_fwd_lse(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk, void* o_s,
+                              float* lse, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale, int64_t blkq, int64_t blkk,
+                              void* stream);
+int tdb200_sla_attn16_bwd(const void* q, const void* k, const void* v, const void* o_s, const void* d_o, const float* lse,
+                          int dtype, const int32_t* lut, int64_t topk, void* dq, void* dk, void* dv, void* workspace,
+                          int64_t workspace_bytes, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale, int64_t blkq,
+                          int64_t blkk, void* stream);
+int64_t tdb200_sla_attn16_bwd_workspace_bytes(int64_t b, int64_t h, int64_t l, int64_t topk, int64_t blkq);
 int tdb200_sla_attn_fwd_qk16(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
                              const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l,
                              int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream);
-
-/* ---------------------------------------------------------------------------------------------
- * a9' backward. Gradients of the block-sparse 16-bit attention (the sparse branch of SparseLinearAttention; reference: the
- * autograd function `_attention`, SLA/kernel.py:240-319).  d = 128, BLKQ = 128, BLKK = 64, q/k/v/o_s/d_o/dq/dk/dv
- * [b, l, h, d] contiguous 16-bit (lk = l), lut [b,h,mblk,topk] int32 of distinct key-block ids per row.
- *   tdb200_sla_attn_fwd_qk16_lse  o_s = T(softmax part of tdb200_sla_attn_fwd_qk16) (no linear branch, no proj_b) and
- *                                 lse [b,h,l] fp32 = m + log2(l) of the scores in the log2 domain (S * sm_scale * log2e).
- *   tdb200_sla_attn_bwd_qk16      dq, dk, dv of o_s w.r.t. q, k, v for the incoming gradient d_o, given the forward's o_s and
- *                                 lse.  P and dS are rounded to T only as MMA operands, accumulation is fp32, no atomics
- *                                 (bit-for-bit reproducible); key blocks no query block selected get zero dk / dv.  Four kernel
- *                                 launches and no host synchronisation, so the call can be captured in a CUDA graph.
- *   tdb200_sla_attn_bwd_workspace_bytes  host-only size of the workspace the backward needs (or a negative error code):
- *                                 delta [b,h,l] fp32, then the key-major index of the LUT: offsets [b*h, nblk+1], cursors
- *                                 [b*h, nblk] and entries [b*h, mblk*topk] int32, each 256-byte aligned.
- * Errors: null pointer, bad shape or topk outside [1, nblk] -> TDB200_ERR_INVALID_ARG; d != 128 or a bad dtype tag ->
- * TDB200_ERR_UNSUPPORTED; workspace_bytes below the size query -> TDB200_ERR_WORKSPACE.
- * ------------------------------------------------------------------------------------------- */
 int tdb200_sla_attn_fwd_qk16_lse(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
                                  void* o_s, float* lse, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale, void* stream);
 int tdb200_sla_attn_bwd_qk16(const void* q, const void* k, const void* v, const void* o_s, const void* d_o, const float* lse,

@@ -15,7 +15,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .._lib import DTYPE_TAG, check, lib, ptr, require_cuda, stream_ptr
-from .utils import SAGE_BLOCKS, QKPrep, block_map_from_pools, get_block_map, get_cuda_arch, quant_qk  # noqa: F401
+from .utils import (SAGE_BLOCKS, QKPrep, block_map_from_pools, get_block_map, get_cuda_arch, quant_k_into,  # noqa: F401
+                    quant_q_only, quant_qk)
 
 SAGESLA_ENABLED = True   # the INT8 path is built in (no SpargeAttn dependency)
 SAGE2PP_ENABLED = True
@@ -71,58 +72,72 @@ def _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, featu
     return out
 
 
-def attn_fwd_qk16(q, k, v, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None):
-    """The non-quantised sparse attention (a9', SLA/kernel.py:33-82): 16-bit Q.K^T on the tensor cores, fp32 scores."""
+# The 16-bit attention serves 64-row key blocks with 128- or 64-row query blocks; `blkq` below is the query block size `lut`
+# was built with.
+BLKK16 = 64
+
+
+def attn_fwd_qk16(q, k, v, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, feature=0, blkq=128):
+    """The non-quantised sparse attention (a9', SLA/kernel.py:33-82): 16-bit Q.K^T on the tensor cores, fp32 scores, and the
+    linear branch with feature map `feature`."""
     b, l, h, d = q.shape
     lk = v.shape[1] if lk is None else lk
     out = torch.empty_like(q)
-    check(lib().tdb200_sla_attn_fwd_qk16(ptr(q), ptr(k), ptr(v), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum),
-                                         ptr(proj_b), ptr(out), b, l, lk, h, d, float(sm_scale), stream_ptr(q.device)),
-          "sla_attn_fwd_qk16")
+    check(lib().tdb200_sla_attn16_fwd(ptr(q), ptr(k), ptr(v), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b),
+                                      ptr(out), b, l, lk, h, d, float(sm_scale), feature, blkq, BLKK16, stream_ptr(q.device)),
+          "sla_attn16_fwd")
     return out
 
 
-def attn_fwd_qk16_lse(q, k, v, lut, topk, sm_scale):
+def attn_fwd_qk16_lse(q, k, v, lut, topk, sm_scale, blkq=128):
     """Sparse branch of attn_fwd_qk16 alone, for the training path: (o_s [B,L,H,D] in q.dtype, lse [B,H,L] fp32), lse being
     the row log-sum-exp of the scores in log2 units (scores scaled by sm_scale * log2(e)).  `lut` [B,H,Mblk,topk] int32."""
     b, l, h, d = q.shape
     o_s = torch.empty_like(q)
     lse = torch.empty(b, h, l, dtype=torch.float32, device=q.device)
-    check(lib().tdb200_sla_attn_fwd_qk16_lse(ptr(q), ptr(k), ptr(v), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(o_s), ptr(lse), b, l, h,
-                                             d, float(sm_scale), stream_ptr(q.device)), "sla_attn_fwd_qk16_lse")
+    check(lib().tdb200_sla_attn16_fwd_lse(ptr(q), ptr(k), ptr(v), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(o_s), ptr(lse), b, l, h, d,
+                                          float(sm_scale), blkq, BLKK16, stream_ptr(q.device)), "sla_attn16_fwd_lse")
     return o_s, lse
 
 
-def attn_bwd_qk16(q, k, v, o_s, d_o, lse, lut, topk, sm_scale):
+def attn_bwd_qk16(q, k, v, o_s, d_o, lse, lut, topk, sm_scale, blkq=128):
     """(dq, dk, dv) of attn_fwd_qk16_lse's o_s for the incoming gradient d_o; all [B,L,H,D] contiguous in q.dtype."""
     b, l, h, d = q.shape
     dq, dk, dv = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
-    nbytes = lib().tdb200_sla_attn_bwd_workspace_bytes(b, h, l, topk)
-    check(0 if nbytes >= 0 else nbytes, "sla_attn_bwd_workspace_bytes", launches=0)
+    nbytes = lib().tdb200_sla_attn16_bwd_workspace_bytes(b, h, l, topk, blkq)
+    check(0 if nbytes >= 0 else nbytes, "sla_attn16_bwd_workspace_bytes", launches=0)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
-    check(lib().tdb200_sla_attn_bwd_qk16(ptr(q), ptr(k), ptr(v), ptr(o_s), ptr(d_o), ptr(lse), DTYPE_TAG[q.dtype], ptr(lut), topk,
-                                         ptr(dq), ptr(dk), ptr(dv), ptr(ws), nbytes, b, l, h, d, float(sm_scale),
-                                         stream_ptr(q.device)), "sla_attn_bwd_qk16")
+    check(lib().tdb200_sla_attn16_bwd(ptr(q), ptr(k), ptr(v), ptr(o_s), ptr(d_o), ptr(lse), DTYPE_TAG[q.dtype], ptr(lut), topk,
+                                      ptr(dq), ptr(dk), ptr(dv), ptr(ws), nbytes, b, l, h, d, float(sm_scale), blkq, BLKK16,
+                                      stream_ptr(q.device)), "sla_attn16_bwd")
     return dq, dk, dv
 
 
 class SparseAttention16(torch.autograd.Function):
-    """o_s = block-sparse softmax attention of q, k, v ([B,L,H,D], 16-bit, d = 128) over `lut`'s key blocks, differentiable in
-    q, k and v (the reference's `_attention`, SLA/kernel.py:240-319)."""
+    """o_s = block-sparse softmax attention of q, k, v ([B,L,H,D], 16-bit, d = 128) over `lut`'s key blocks (`blkq`-row query
+    blocks, 64-row key blocks), differentiable in q, k and v (the reference's `_attention`, SLA/kernel.py:240-319)."""
 
     @staticmethod
-    def forward(ctx, q, k, v, lut, topk, sm_scale):
-        o_s, lse = attn_fwd_qk16_lse(q, k, v, lut, topk, sm_scale)
+    def forward(ctx, q, k, v, lut, topk, sm_scale, blkq=128):
+        o_s, lse = attn_fwd_qk16_lse(q, k, v, lut, topk, sm_scale, blkq)
         ctx.save_for_backward(q, k, v, o_s, lse, lut)
-        ctx.topk, ctx.sm_scale = topk, sm_scale
+        ctx.topk, ctx.sm_scale, ctx.blkq = topk, sm_scale, blkq
         return o_s
 
     @staticmethod
     def backward(ctx, d_o):
         q, k, v, o_s, lse, lut = ctx.saved_tensors
         d_o = d_o.to(q.dtype).contiguous()
-        dq, dk, dv = attn_bwd_qk16(q, k, v, o_s, d_o, lse, lut, ctx.topk, ctx.sm_scale)
-        return dq, dk, dv, None, None, None
+        dq, dk, dv = attn_bwd_qk16(q, k, v, o_s, d_o, lse, lut, ctx.topk, ctx.sm_scale, ctx.blkq)
+        return dq, dk, dv, None, None, None, None
+
+
+def select_prep(q, k, blkq, blkk):
+    """The pooled means (and Sage INT8 codes) block selection reads, for q, k [B, L, H, D]: quant_qk for the SageSLA families;
+    (64, 64), a pair tdb200_sla_quant_qk does not take, from its query half at blkq = 64 and its key half at blkk = 64."""
+    if (blkq, blkk) == (64, 64):
+        return quant_k_into(quant_q_only(q, blkq), k, k.shape[1], blkk)
+    return quant_qk(q, k, blkq=blkq, blkk=blkk)
 
 
 class _SLABase(nn.Module):
@@ -166,7 +181,7 @@ class _SLABase(nn.Module):
         if d not in (64, 128):
             raise AssertionError("headdim should be in [64, 128].")  # SLA/core.py:207
         blkq, blkk = self.block_sizes(q.device.index)
-        prep = quant_qk(q, k, blkq=blkq, blkk=blkk)
+        prep = select_prep(q, k, blkq, blkk)
         nblk = prep.nblk
         real_topk = min(nblk, int(self.topk * nblk))
         if real_topk < 1:
@@ -178,8 +193,9 @@ class _SLABase(nn.Module):
         kv, ksum = linear_moments(k, v, self.feature)
         # proj_l folded into the moments: (phi(q) KV / den) W^T + b == phi(q) (W KV^T)^T / den + b ; kv is [dv, dk]
         kvw = project_moments(self.proj_l.weight, kv, self.dtype)  # [B,H,d_out,d_k]
-        if not self.quantised_qk and d == 128 and self.feature == 0:
-            o = attn_fwd_qk16(q, k, v, lut, real_topk, kvw, ksum, self.proj_l.bias.float().contiguous(), d ** -0.5)
+        if not self.quantised_qk and d == 128 and (self.feature == 0 or blkq == 64):
+            o = attn_fwd_qk16(q, k, v, lut, real_topk, kvw, ksum, self.proj_l.bias.float().contiguous(), d ** -0.5,
+                              feature=self.feature, blkq=blkq)
         else:
             o = attn_fwd(prep, v, q, lut, real_topk, kvw, ksum, self.proj_l.bias.float().contiguous(), d ** -0.5,
                          feature=self.feature, blkq=blkq, blkk=blkk)
@@ -196,14 +212,15 @@ class _SLABase(nn.Module):
         dtype = q.dtype
         q, k, v = (t if (t.dtype == self.dtype and t.is_contiguous()) else t.to(self.dtype).contiguous() for t in (q, k, v))
         d = q.shape[-1]
+        blkq, blkk = self.block_sizes(q.device.index)
         with torch.no_grad():
-            prep = quant_qk(q.detach(), k.detach())
+            prep = select_prep(q.detach(), k.detach(), blkq, blkk)
             nblk = prep.nblk
             real_topk = max(1, min(nblk, int(self.topk * nblk)))
             sparse_map, lut = block_map_from_pools(prep.q_pool, prep.k_pool, real_topk)
         if getattr(self, "_keep_selection", None) is not None:
             self._keep_selection.update(lut=lut, sparse_map=sparse_map, topk=real_topk)
-        o_s = SparseAttention16.apply(q, k, v, lut, real_topk, d ** -0.5)
+        o_s = SparseAttention16.apply(q, k, v, lut, real_topk, d ** -0.5, blkq)
         qh, kh, vh = (t.transpose(1, 2) for t in (q, k, v))                       # [B, H, L, D] views
         c_q = self.feature_map_q(qh).contiguous().to(self.dtype)
         c_k = self.feature_map_k(kh).contiguous().to(self.dtype)
@@ -227,16 +244,22 @@ class _SLABase(nn.Module):
 
 
 class SparseLinearAttention(_SLABase):
-    """SLA/core.py:38-119: the non-quantised variant (`--attention_type sla`).  128-wide heads with the softmax feature map run
-    the fused kernel with a 16-bit Q.K^T (the arithmetic of the reference's Triton _attn_fwd, SLA/kernel.py:33-82); 64-wide
-    heads and the elu / relu maps are served by the INT8-QK kernel.  Block sizes are BLKQ=128, BLKK=64 (the configuration
-    modify_model.py:50 requests); other values are accepted for signature compatibility with a warning."""
+    """SLA/core.py:38-119: the non-quantised variant (`--attention_type sla`).  Block sizes (BLKQ, BLKK) = (128, 64) (the
+    configuration modify_model.py:50 requests) and, for 128-wide heads, the constructor's default (64, 64) are served as
+    the reference computes them.  128-wide heads run the fused kernel with a 16-bit Q.K^T (the arithmetic of the reference's
+    Triton _attn_fwd, SLA/kernel.py:21-82); at (128, 64) the elu / relu maps and 64-wide heads are served by the INT8-QK
+    kernel.  Other block sizes are accepted for signature compatibility with a warning and run as (128, 64)."""
     quantised_qk = False
+
+    def block_sizes(self, device_index):
+        """(BLKQ, BLKK) of this call: the constructor's pair where it is served, else (128, 64)."""
+        return (self.BLKQ, self.BLKK) if self._served else (128, 64)
 
     def __init__(self, head_dim, topk, feature_map="softmax", BLKQ=64, BLKK=64, use_bf16=True, tie_feature_map_qk=True):
         super().__init__(head_dim, topk, feature_map, use_bf16, tie_feature_map_qk)
         self.BLKQ, self.BLKK = BLKQ, BLKK
-        if (BLKQ, BLKK) != (128, 64):
+        self._served = (BLKQ, BLKK) == (128, 64) or ((BLKQ, BLKK) == (64, 64) and head_dim == 128)
+        if not self._served:
             import warnings
             warnings.warn(f"SparseLinearAttention(BLKQ={BLKQ}, BLKK={BLKK}): these kernels use 128-row query blocks and "
                           "64-row key blocks (the configuration TurboDiffusion's modify_model.py:50 requests); block "

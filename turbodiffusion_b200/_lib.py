@@ -54,6 +54,11 @@ _PROTOS = {
     "tdb200_sla_attn_fwd_qk16_lse": [_P, _P, _P, _I, _P, _I64, _P, _P, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_sla_attn_bwd_qk16": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_sla_attn_bwd_workspace_bytes": [_I64, _I64, _I64, _I64],
+    "tdb200_sla_attn16_fwd": [_P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F, _I, _I64, _I64, _P],
+    "tdb200_sla_attn16_fwd_lse": [_P, _P, _P, _I, _P, _I64, _P, _P, _I64, _I64, _I64, _I64, _F, _I64, _I64, _P],
+    "tdb200_sla_attn16_bwd": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F, _I64, _I64,
+                              _P],
+    "tdb200_sla_attn16_bwd_workspace_bytes": [_I64, _I64, _I64, _I64, _I64],
     "tdb200_ltx_modulated_rms_norm_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_ltx_modulate_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
     "tdb200_ltx_gated_residual_ada": [_P, _P, _I, _P, _P, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
@@ -61,7 +66,8 @@ _PROTOS = {
     "tdb200_quant_int8_rowwise": [_P, _I, _I64, _I64, _P, _P, _P],
     "tdb200_gemm_w8a8_rowwise": [_P, _P, _P, _P, _P, _P, _I, _I64, _I64, _I64, _P],
 }
-_RESTYPES = {"tdb200_last_error": c_char_p, "tdb200_sla_attn_bwd_workspace_bytes": c_int64}
+_RESTYPES = {"tdb200_last_error": c_char_p, "tdb200_sla_attn_bwd_workspace_bytes": c_int64,
+             "tdb200_sla_attn16_bwd_workspace_bytes": c_int64}
 ABI_VERSION = 2   # TDB200_ABI_VERSION of include/tdb200.h, whose prototypes _PROTOS mirrors
 
 _lib = None
@@ -124,7 +130,7 @@ class _DeviceGuarded:
 
 
 LAUNCHES = 0  # kernels launched through the C ABI (each entry point documents how many it enqueues)
-_KERNELS_PER_CALL = {"sla_quant_qk": 4, "layernorm_modulate_quant": 2, "sla_attn_bwd_qk16": 4}  # upper bounds per entry point
+_KERNELS_PER_CALL = {"sla_quant_qk": 4, "layernorm_modulate_quant": 2, "sla_attn16_bwd": 4}  # upper bounds per entry point
 
 
 def check(rc: int, what: str, launches: int = None) -> None:

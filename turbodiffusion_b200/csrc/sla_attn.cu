@@ -17,8 +17,9 @@
 // The O accumulator is only rescaled when a row maximum grows by more than 2^8 (lazy rescale): P stays <= 256, which
 // bf16/fp32 hold exactly as well as P <= 1, and the final O / l normalisation is unchanged.
 // Entry points: tdb200_sla_attn_fwd (INT8 Q/K, head dims 64 and 128, feature maps of the linear branch, K head-major or in
-// [b, lk, h, d], 128 x 64 blocks or 64 x 128 blocks in sla_attn_fwd_q64_kernel further down), _qk16 (16-bit Q/K read from the
-// module layout [b, l, h, d], fp32 scores) and _qk16_lse (its sparse branch and row log-sum-exp, for the backward).
+// [b, lk, h, d], 128 x 64 blocks or 64 x 128 blocks in sla_attn_fwd_q64_kernel further down), tdb200_sla_attn16_fwd (16-bit
+// Q/K read from the module layout [b, l, h, d], fp32 scores; 128 x 64 blocks, or 64 x 64 in sla_attn_fwd_q64k64_kernel) and
+// tdb200_sla_attn16_fwd_lse (its sparse branch and row log-sum-exp, for the backward).
 #include <type_traits>
 
 #include "common.cuh"
@@ -600,15 +601,233 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
   linear_branch_store<T, HD>(o, l_part, p, sbase + L::kOffW, int64_t(m_blk) * BQ + r_lo, cq, b, hh, bh);
 }
 
+// 16-bit Q.K^T on 64-row query blocks and 64-row key blocks: SparseLinearAttention's default geometry (the reference's
+// BLOCK_M = 64, BLOCK_N = 64 configuration of SLA/kernel.py:21-82).  The CTA of sla_attn_fwd_q64_kernel: a producer warpgroup
+// that gives its registers away, and two consumer warpgroups on the same 64 query rows taking alternate LUT entries, each with
+// its own online softmax on a 64 x 64 fp32 score tile (wgmma m64n64k16, Q and K K-major from shared memory; P rounded to T for
+// P.V as in sla_attn_fwd_kernel).  Warpgroup 1 hands its (m, l, O) to warpgroup 0 through the drained ring.  Without kLse
+// warpgroup 0 then runs the linear branch (every feature map) and the merge; with kLse it stores o_s and the row lse instead.
+constexpr int kSla16BlkQ = 64;
+template <typename T, bool kLse>
+__global__ void __launch_bounds__(kThreadsQ64, 1)
+sla_attn_fwd_q64k64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                           const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw, AttnParams p) {
+  constexpr int HD = 128, BQ = kSla16BlkQ, BK = BLKK;
+  using L = Lay<HD, true, BQ, BK>;
+  static_assert((HD / 2 + 4) * 128 * 4 <= kStages * (L::kKBytes + L::kVBytes), "merge buffer does not fit in the ring");
+  constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kOffBars);
+  uint16_t* s_lut = reinterpret_cast<uint16_t*>(smem + L::kOffLut);
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
+  const int bh = b * p.h + hh;
+  const int T_blocks = p.topk;
+
+  if (threadIdx.x == 0) {
+    mbar_init(&bars[kQ64QFull], 1);
+    for (int i = 0; i < kStages; ++i) {
+      for (int g = 0; g < 2; ++g) {
+        mbar_init(&bars[kQ64KFull + 2 * i + g], 1);
+        mbar_init(&bars[kQ64VFull + 2 * i + g], 1);
+      }
+      mbar_init(&bars[kQ64KEmpty + i], 4);
+      mbar_init(&bars[kQ64VEmpty + i], 4);
+    }
+    mbar_fence_init();
+  }
+  {
+    const int32_t* lut_row = p.lut + (int64_t(bh) * p.mblk + m_blk) * p.topk;
+    for (int i = threadIdx.x; i < T_blocks; i += kThreadsQ64) s_lut[i] = static_cast<uint16_t>(__ldg(lut_row + i));
+  }
+  __syncthreads();
+
+  if (warp >= kConsumerWarps) {
+    // =============================================================== TMA producer
+    reg_dealloc<kProducerRegsQ64>();
+    if (warp == kConsumerWarps && lane == 0) {
+      tma_prefetch_desc(&tmap_q);
+      tma_prefetch_desc(&tmap_k);
+      tma_prefetch_desc(&tmap_v);
+      if constexpr (!kLse) tma_prefetch_desc(&tmap_kvw);
+      mbar_expect_tx(&bars[kQ64QFull], L::kQBytes + (kLse ? 0 : L::kWBytes));
+#pragma unroll
+      for (int c = 0; c < HD / 64; ++c)
+        tma_load_4d(smem + L::kOffQ + c * (BQ * 128), &tmap_q, &bars[kQ64QFull], c * 64, hh, m_blk * BQ, b);
+      if constexpr (!kLse) {
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c)
+          tma_load_4d(smem + L::kOffW + c * (HD * 128), &tmap_kvw, &bars[kQ64QFull], c * 64, 0, bh, 0);
+      }
+      for (int j = 0; j < T_blocks; ++j) {
+        const int st = j % kStages;
+        const uint32_t ph = ((j / kStages) & 1) ^ 1;
+        const int blk = s_lut[j];
+        uint64_t* kfull = &bars[q64_full(kQ64KFull, j)];
+        uint64_t* vfull = &bars[q64_full(kQ64VFull, j)];
+        mbar_wait(&bars[kQ64KEmpty + st], ph);
+        mbar_expect_tx(kfull, L::kKBytes);
+        uint8_t* sk = smem + L::kOffK + st * L::kKBytes;
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c) tma_load_4d(sk + c * (BK * 128), &tmap_k, kfull, c * 64, hh, blk * BK, b);
+        mbar_wait(&bars[kQ64VEmpty + st], ph);
+        mbar_expect_tx(vfull, L::kVBytes);
+        uint8_t* sv = smem + L::kOffV + st * L::kVBytes;
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c) tma_load_4d(sv + c * (BK * 128), &tmap_v, vfull, c * 64, hh, blk * BK, b);
+      }
+    }
+    return;
+  }
+
+  // =============================================================== consumer warpgroups (same 64 rows, alternate LUT entries)
+  reg_alloc<kConsumerRegsQ64>();
+  const int wg = warp >> 2, w4 = warp & 3;
+  const int r_lo = w4 * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const uint32_t sbase = smem_u32(smem);
+  const float sc = p.sm_scale * kLog2e;
+
+  float o[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+  float m_used[2] = {-INFINITY, -INFINITY}, l_part[2] = {0.f, 0.f};  // a warpgroup without entries keeps m = -inf, l = 0
+
+  mbar_wait(&bars[kQ64QFull], 0);
+  for (int j = wg; j < T_blocks; j += 2) {
+    const int st = j % kStages;
+    const uint32_t ph = (j / (2 * kStages)) & 1;        // phase j / 6 of this warpgroup's full barriers of slot st
+    const int valid = p.lk - s_lut[j] * BK;             // < 64 only in the ragged last key block
+
+    // ---- S = Q.K^T over this entry's 64 keys
+    float s[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s[i] = 0.f;
+    mbar_wait(&bars[q64_full(kQ64KFull, j)], ph);
+    const uint32_t sk = sbase + L::kOffK + st * L::kKBytes;
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks) {
+      const uint64_t qd = make_desc_kmajor_sw128(sbase + L::kOffQ + (ks >> 2) * (BQ * 128)) + uint64_t((ks & 3) * 2);
+      const uint64_t kd = make_desc_kmajor_sw128(sk + (ks >> 2) * (BK * 128)) + uint64_t((ks & 3) * 2);
+      wgmma_f16_ss<64, kBF16>(s, qd, kd, ks > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s[i] *= sc;
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars[kQ64KEmpty + st]);
+
+    if (valid < BK) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if (8 * (i >> 2) + cq + (i & 1) >= valid) s[i] = -INFINITY;
+    }
+    // ---- row maxima and the lazy rescale, as in sla_attn_fwd_kernel
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if (((i >> 1) & 1) == h) mx = fmaxf(mx, s[i]);
+      mx = quad_max(mx);
+      if (j == wg) {
+        m_used[h] = mx;
+      } else if (mx > m_used[h] + kRescaleThreshold) {
+        const float alpha = fast_exp2(m_used[h] - mx);
+#pragma unroll
+        for (int i = 0; i < HD / 2; ++i)
+          if (((i >> 1) & 1) == h) o[i] *= alpha;
+        l_part[h] *= alpha;
+        m_used[h] = mx;
+      }
+    }
+    uint32_t pa[BK / 16][4];
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int h = (i >> 1) & 1;
+      const float p0 = fast_exp2(s[i] - m_used[h]), p1 = fast_exp2(s[i + 1] - m_used[h]);
+      l_part[h] += p0 + p1;
+      pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0, p1);
+    }
+
+    // ---- O += P.V  (V: [64 keys x HD], MN-major; +16 keys = +2048 B per K step)
+    mbar_wait(&bars[q64_full(kQ64VFull, j)], ph);
+    const uint64_t vdesc = make_desc_mnmajor_sw128(sbase + L::kOffV + st * L::kVBytes, BK * 128);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(o, pa[kk], vdesc + uint64_t(kk * 128));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk) reg_fence(pa[kk]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars[kQ64VEmpty + st]);
+  }
+
+  // ---- merge, as in sla_attn_fwd_q64_kernel: warpgroup 1's state through the drained ring, [value][thread]
+  float* xchg = reinterpret_cast<float*>(smem + L::kOffK) + (threadIdx.x & 127);
+  named_bar_sync(1, 256);
+  if (wg == 1) {
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) xchg[i * 128] = o[i];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      xchg[(HD / 2 + h) * 128] = m_used[h];
+      xchg[(HD / 2 + 2 + h) * 128] = l_part[h];
+    }
+  }
+  named_bar_sync(1, 256);
+  if (wg == 1) return;
+  float a0[2], a1[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {  // warpgroup 0 always has entry 0, so its maximum is finite and an empty state drops out
+    const float m1 = xchg[(HD / 2 + h) * 128], l1 = xchg[(HD / 2 + 2 + h) * 128];
+    const float mx = fmaxf(m_used[h], m1);
+    a0[h] = fast_exp2(m_used[h] - mx);
+    a1[h] = fast_exp2(m1 - mx);
+    l_part[h] = fmaf(l_part[h], a0[h], l1 * a1[h]);
+    m_used[h] = mx;
+  }
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) {
+    const int h = (i >> 1) & 1;
+    o[i] = fmaf(o[i], a0[h], xchg[i * 128] * a1[h]);
+  }
+  const int64_t qrow0 = int64_t(m_blk) * BQ + r_lo;
+  if constexpr (kLse) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t qr = qrow0 + 8 * h;
+      if (qr >= p.l) continue;
+      const float l_tot = quad_sum(l_part[h]), inv_l = 1.0f / l_tot;
+      if ((lane & 3) == 0) p.lse[int64_t(bh) * p.l + qr] = m_used[h] + __log2f(l_tot);
+      T* orow = static_cast<T*>(p.out) + ((int64_t(b) * p.l + qr) * p.h + hh) * HD;
+#pragma unroll
+      for (int c = 0; c < HD / 8; ++c)
+        *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) = F16Traits<T>::pack(o[4 * c + 2 * h] * inv_l, o[4 * c + 2 * h + 1] * inv_l);
+    }
+  } else {
+    linear_branch_store<T, HD>(o, l_part, p, sbase + L::kOffW, qrow0, cq, b, hh, bh);
+  }
+}
+
 template <typename T, int HD, bool kQK16, int kBQ, bool kLse>
 constexpr auto attn_kernel() {
-  if constexpr (kBQ == kHopperBlkQ) return sla_attn_fwd_q64_kernel<T, HD>;
+  if constexpr (kQK16 && kBQ == kSla16BlkQ) return sla_attn_fwd_q64k64_kernel<T, kLse>;
+  else if constexpr (kBQ == kHopperBlkQ) return sla_attn_fwd_q64_kernel<T, HD>;
   else return sla_attn_fwd_kernel<T, HD, kQK16, kLse>;
 }
 
 // kQK16: 16-bit Q and K in [b, l, h, d]; otherwise INT8 Q [b*h, l, d] and INT8 K [b, h, lk, d] (or [b, lk, h, d] when k_seq_major).
-// kBQ x kBK: the block geometry, 128 x 64 (sla_attn_fwd_kernel) or 64 x 128 (sla_attn_fwd_q64_kernel, INT8 Q/K only).
-// kLse (16-bit 128 x 64 only): sparse branch and row log-sum-exp into `lse`; kvw, ksum and proj_b are not read.
+// kBQ x kBK: the block geometry, 128 x 64 (sla_attn_fwd_kernel), 64 x 128 (sla_attn_fwd_q64_kernel, INT8 Q/K only) or
+// 64 x 64 (sla_attn_fwd_q64k64_kernel, 16-bit Q/K only).
+// kLse (16-bit only): sparse branch and row log-sum-exp into `lse`; kvw, ksum and proj_b are not read.
 template <int HD, bool kQK16, int kBQ = BLKQ, int kBK = BLKK, bool kLse = false>
 int launch(const void* q_op, const float* q_scale, const void* k_op, const float* k_scale, const void* v, const void* q, int dtype,
            const int32_t* lut, int64_t topk, const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
@@ -747,22 +966,61 @@ extern "C" int tdb200_sla_attn_fwd(const int8_t* q_i8, const float* q_scale, con
 #undef TDB_LAUNCH
 }
 
+namespace {
+int check_blocks16(const char* what, int64_t blkq, int64_t blkk) {
+  if ((blkq == BLKQ || blkq == kSla16BlkQ) && blkk == BLKK) return 0;
+  return fail(TDB200_ERR_UNSUPPORTED, "%s: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 64)", what, (long long)blkq,
+              (long long)blkk);
+}
+
+// The four 16-bit kernels, instantiated in this order: the (128, 64) ones first, because nvcc's output depends on the order.
+int launch16(bool with_lse, int64_t blkq, const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
+             const void* kvw, const float* ksum, const float* proj_b, void* out, float* lse, int64_t b, int64_t l, int64_t lk,
+             int64_t h, float sm_scale, int feature, void* stream) {
+#define TDB_LAUNCH16(BQ, LSE)                                                                                                  \
+  return launch<128, true, BQ, BLKK, LSE>(q, nullptr, k, nullptr, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, \
+                                          sm_scale, feature, false, stream, lse)
+  if (blkq == BLKQ) {
+    if (!with_lse) TDB_LAUNCH16(BLKQ, false);
+    TDB_LAUNCH16(BLKQ, true);
+  }
+  if (!with_lse) TDB_LAUNCH16(kSla16BlkQ, false);
+  TDB_LAUNCH16(kSla16BlkQ, true);
+#undef TDB_LAUNCH16
+}
+}  // namespace
+
+// 16-bit Q/K read from the module layout: (blkq, blkk) = (128, 64) runs sla_attn_fwd_kernel, (64, 64) sla_attn_fwd_q64k64_kernel.
+extern "C" int tdb200_sla_attn16_fwd(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
+                                     const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l,
+                                     int64_t lk, int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq, int64_t blkk,
+                                     void* stream) {
+  if (int rc = check_blocks16("sla_attn16_fwd", blkq, blkk)) return rc;
+  if (int rc = check_common(q, k, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (this kernel implements d=128)", (long long)d);
+  if (feature < 0 || feature > 2) return fail(TDB200_ERR_INVALID_ARG, "sla_attn16_fwd: feature map tag %d", feature);
+  return launch16(false, blkq, q, k, v, dtype, lut, topk, kvw, ksum, proj_b, out, nullptr, b, l, lk, h, sm_scale, feature, stream);
+}
+
+// The sparse branch of tdb200_sla_attn16_fwd with its row log-sum-exp, the forward half of the training path.
+extern "C" int tdb200_sla_attn16_fwd_lse(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
+                                         void* o_s, float* lse, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale,
+                                         int64_t blkq, int64_t blkk, void* stream) {
+  if (int rc = check_blocks16("sla_attn16_fwd_lse", blkq, blkk)) return rc;
+  if (!q || !k || !v || !lut || !o_s || !lse) return fail(TDB200_ERR_INVALID_ARG, "sla_attn16_fwd_lse: null pointer");
+  if (b <= 0 || l <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_attn16_fwd_lse: bad shape");
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn16_fwd_lse: head dim %lld (this kernel implements d=128)", (long long)d);
+  return launch16(true, blkq, q, k, v, dtype, lut, topk, nullptr, nullptr, nullptr, o_s, lse, b, l, l, h, sm_scale, 0, stream);
+}
+
 extern "C" int tdb200_sla_attn_fwd_qk16(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
                                         const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
                                         int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  if (int rc = check_common(q, k, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
-  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: head dim %lld (this kernel implements d=128)", (long long)d);
-  return launch<128, true>(q, nullptr, k, nullptr, v, q, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, sm_scale, 0, false,
-                           stream);
+  return tdb200_sla_attn16_fwd(q, k, v, dtype, lut, topk, kvw, ksum, proj_b, out, b, l, lk, h, d, sm_scale, 0, BLKQ, BLKK, stream);
 }
 
-// The sparse branch of tdb200_sla_attn_fwd_qk16 with its row log-sum-exp, the forward half of the training path.
 extern "C" int tdb200_sla_attn_fwd_qk16_lse(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
                                             void* o_s, float* lse, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale,
                                             void* stream) {
-  if (!q || !k || !v || !lut || !o_s || !lse) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd_qk16_lse: null pointer");
-  if (b <= 0 || l <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd_qk16_lse: bad shape");
-  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_qk16_lse: head dim %lld (this kernel implements d=128)", (long long)d);
-  return launch<128, true, BLKQ, BLKK, true>(q, nullptr, k, nullptr, v, q, dtype, lut, topk, nullptr, nullptr, nullptr, o_s, b, l, l, h,
-                                             sm_scale, 0, false, stream, lse);
+  return tdb200_sla_attn16_fwd_lse(q, k, v, dtype, lut, topk, o_s, lse, b, l, h, d, sm_scale, BLKQ, BLKK, stream);
 }

@@ -1,8 +1,9 @@
 // Backward of the block-sparse 16-bit attention (the sparse branch of SparseLinearAttention; reference: the autograd function
 // `_attention`, SLA/kernel.py:240-319, whose backward runs _attn_bwd_preprocess / _attn_bwd_dq / _attn_bwd_dkdv, :85-237).
-// Block geometry of the forward: BLKQ = 128 query rows, BLKK = 64 key rows, 128-wide heads, q/k/v/o/dO/dq/dk/dv in the module
-// layout [b, l, h, d].  The forward (sla_attn.cu, kLse) leaves o_s = T(O / l) and lse = m + log2(l) in the log2 domain, so that
-// P = exp2(S * sm_scale * log2e - lse) is recomputed exactly as the forward normalised it.
+// Block geometry of the forward: BLKQ = 128 (or 64: the _q64 kernels further down) query rows, BLKK = 64 key rows, 128-wide
+// heads, q/k/v/o/dO/dq/dk/dv in the module layout [b, l, h, d].  The forward (sla_attn.cu, kLse) leaves o_s = T(O / l) and
+// lse = m + log2(l) in the log2 domain, so that P = exp2(S * sm_scale * log2e - lse) is recomputed exactly as the forward
+// normalised it.
 //
 //   sla_bwd_delta_kernel      delta[b,h,row] = sum_d T(dO) * T(o_s), fp32
 //   sla_bwd_kmajor_index_kernel  the LUT transposed: for every (b, h, key block) the ascending list of the query blocks that
@@ -466,13 +467,382 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   store_rows<T>(dv, 1.0f, p.dv, row0, p.l, p.h, hh, b, cq);
 }
 
+// ------------------------------------------------------------------------------------------------ 64-row query blocks
+// The backward of sla_attn_fwd_q64k64_kernel (BLKQ = 64, BLKK = 64).  Both kernels run a producer warpgroup (setmaxnreg hands
+// its registers to the consumers) and two consumer warpgroups that take alternate entries of the streamed list, so a 64-row
+// query block is never split: each warpgroup keeps its own fp32 partial, and warpgroup 1 hands it to warpgroup 0 through the
+// drained ring, which adds the two in a fixed order and stores.
+constexpr int BLKQ64 = 64;
+constexpr int kThreads64 = 3 * 128;
+constexpr uint32_t kProducerRegs64 = 40, kConsumerRegs64 = 232;   // 128 * 40 + 256 * 232 <= 65536
+
+// dQ: one CTA per (64-row query block, head, batch); Q_i and dO_i resident, K_j / V_j streamed over the LUT row through a
+// 3-stage ring.  Ring slot st serves entries st, st+3, ..., which alternate between the warpgroups, so every slot has one
+// full barrier per warpgroup (entry j completes phase j / 6 of barrier (j % 3, j % 2); see sla_attn_fwd_q64_kernel).
+namespace dq64 {
+constexpr int kStages = 3;
+constexpr uint32_t kTileQ = BLKQ64 * HD * 2, kTileK = BLKK * HD * 2;   // 16 KB each
+constexpr uint32_t kOffQ = 0, kOffDO = kTileQ, kOffK = 2 * kTileQ, kOffV = kOffK + kStages * kTileK;
+constexpr uint32_t kOffBars = kOffV + kStages * kTileK, kOffLut = kOffBars + 256;
+enum Bar { kQFull = 0, kKFull = 1 /*3 x 2*/, kKEmpty = 7 /*3*/, kVFull = 10 /*3 x 2*/, kVEmpty = 16 /*3*/ };
+static_assert((kVEmpty + kStages) * 8 <= 256, "barriers exceed their shared-memory slot");
+static_assert(HD / 2 * 128 * 4 <= kStages * kTileK, "partial dQ does not fit in the K ring");
+__device__ __forceinline__ int full(int base, int j) { return base + 2 * (j % kStages) + (j & 1); }
+}  // namespace dq64
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads64, 1)
+sla_bwd_dq_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
+                      const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v, BwdParams p) {
+  using namespace dq64;
+  constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
+  uint16_t* s_lut = reinterpret_cast<uint16_t*>(smem + kOffLut);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
+  const int bh = b * p.h + hh;
+
+  if (threadIdx.x == 0) {
+    mbar_init(&bars[kQFull], 1);
+    for (int i = 0; i < kStages; ++i) {
+      for (int g = 0; g < 2; ++g) {
+        mbar_init(&bars[kKFull + 2 * i + g], 1);
+        mbar_init(&bars[kVFull + 2 * i + g], 1);
+      }
+      mbar_init(&bars[kKEmpty + i], 4);
+      mbar_init(&bars[kVEmpty + i], 4);
+    }
+    mbar_fence_init();
+  }
+  {
+    const int32_t* lut_row = p.lut + (int64_t(bh) * p.mblk + m_blk) * p.topk;
+    for (int i = threadIdx.x; i < p.topk; i += kThreads64) s_lut[i] = static_cast<uint16_t>(__ldg(lut_row + i));
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // =============================================================== TMA producer
+    reg_dealloc<kProducerRegs64>();
+    if (warp == 8 && lane == 0) {
+      tma_prefetch_desc(&tmap_q);
+      tma_prefetch_desc(&tmap_do);
+      tma_prefetch_desc(&tmap_k);
+      tma_prefetch_desc(&tmap_v);
+      mbar_expect_tx(&bars[kQFull], 2 * kTileQ);
+#pragma unroll
+      for (int c = 0; c < HD / 64; ++c) {
+        tma_load_4d(smem + kOffQ + c * (BLKQ64 * 128), &tmap_q, &bars[kQFull], c * 64, hh, m_blk * BLKQ64, b);
+        tma_load_4d(smem + kOffDO + c * (BLKQ64 * 128), &tmap_do, &bars[kQFull], c * 64, hh, m_blk * BLKQ64, b);
+      }
+      for (int j = 0; j < p.topk; ++j) {
+        const int st = j % kStages;
+        const uint32_t ph = ((j / kStages) & 1) ^ 1;
+        const int blk = s_lut[j];
+        uint64_t* kfull = &bars[full(kKFull, j)];
+        uint64_t* vfull = &bars[full(kVFull, j)];
+        mbar_wait(&bars[kKEmpty + st], ph);
+        mbar_expect_tx(kfull, kTileK);
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c)
+          tma_load_4d(smem + kOffK + st * kTileK + c * (BLKK * 128), &tmap_k, kfull, c * 64, hh, blk * BLKK, b);
+        mbar_wait(&bars[kVEmpty + st], ph);
+        mbar_expect_tx(vfull, kTileK);
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c)
+          tma_load_4d(smem + kOffV + st * kTileK + c * (BLKK * 128), &tmap_v, vfull, c * 64, hh, blk * BLKK, b);
+      }
+    }
+    return;
+  }
+
+  // =============================================================== consumer warpgroups (same 64 rows, alternate LUT entries)
+  reg_alloc<kConsumerRegs64>();
+  const int wg = warp >> 2, w4 = warp & 3;
+  const int r_lo = w4 * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const uint32_t sbase = smem_u32(smem);
+  const float sc = p.sm_scale * kLog2e;
+  float lse[2], dlt[2];
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    const int64_t r = int64_t(m_blk) * BLKQ64 + r_lo + 8 * hf;
+    lse[hf] = r < p.l ? __ldg(p.lse + int64_t(bh) * p.l + r) : INFINITY;
+    dlt[hf] = r < p.l ? __ldg(p.delta + int64_t(bh) * p.l + r) : 0.f;
+  }
+  float acc[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) acc[i] = 0.f;
+
+  mbar_wait(&bars[kQFull], 0);
+  for (int j = wg; j < p.topk; j += 2) {
+    const int st = j % kStages;
+    const uint32_t ph = (j / (2 * kStages)) & 1;
+    const int valid = p.l - s_lut[j] * BLKK;
+    const uint32_t sk = sbase + kOffK + st * kTileK, sv = sbase + kOffV + st * kTileK;
+
+    // ---- S = Q.K^T and dP = dO.V^T (all operands K-major over d)
+    float s[32], dp[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s[i] = dp[i] = 0.f;
+    mbar_wait(&bars[full(kKFull, j)], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks) {
+      const uint64_t qd = make_desc_kmajor_sw128(sbase + kOffQ + (ks >> 2) * (BLKQ64 * 128)) + uint64_t((ks & 3) * 2);
+      const uint64_t kd = make_desc_kmajor_sw128(sk + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
+      wgmma_f16_ss<64, kBF16>(s, qd, kd, ks > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    mbar_wait(&bars[full(kVFull, j)], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks) {
+      const uint64_t gd = make_desc_kmajor_sw128(sbase + kOffDO + (ks >> 2) * (BLKQ64 * 128)) + uint64_t((ks & 3) * 2);
+      const uint64_t vd = make_desc_kmajor_sw128(sv + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
+      wgmma_f16_ss<64, kBF16>(dp, gd, vd, ks > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    reg_fence(dp);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars[kVEmpty + st]);
+
+    // ---- P = exp2(S sc - lse) (columns past l masked), dS = P o (dP - delta), rounded to T into the A fragments
+    uint32_t da[BLKK / 16][4];
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int hf = (i >> 1) & 1, col = 8 * (i >> 2) + cq;
+      const float p0 = col < valid ? fast_exp2(fmaf(s[i], sc, -lse[hf])) : 0.f;
+      const float p1 = col + 1 < valid ? fast_exp2(fmaf(s[i + 1], sc, -lse[hf])) : 0.f;
+      da[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0 * (dp[i] - dlt[hf]), p1 * (dp[i + 1] - dlt[hf]));
+    }
+    // ---- dQ += dS.K  (K as the MN-major operand; +16 keys = +2048 B per K step)
+    const uint64_t kmn = make_desc_mnmajor_sw128(sk, BLKK * 128);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BLKK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(acc, da[kk], kmn + uint64_t(kk * 128));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(acc);
+#pragma unroll
+    for (int kk = 0; kk < BLKK / 16; ++kk) reg_fence(da[kk]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars[kKEmpty + st]);
+  }
+
+  // ---- dQ = partial of warpgroup 0 + partial of warpgroup 1, through the drained K ring ([value][thread] layout)
+  float* xchg = reinterpret_cast<float*>(smem + kOffK) + (threadIdx.x & 127);
+  named_bar_sync(1, 256);
+  if (wg == 1) {
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) xchg[i * 128] = acc[i];
+  }
+  named_bar_sync(1, 256);
+  if (wg == 1) return;
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) acc[i] += xchg[i * 128];
+  store_rows<T>(acc, p.sm_scale, p.dq, int64_t(m_blk) * BLKQ64 + r_lo, p.l, p.h, hh, b, cq);
+}
+
+// dK / dV: sla_bwd_dkdv_kernel with each list entry one 64-row query block, taken by warpgroup j % 2.  With four ring stages
+// slot j % 4 is only ever used by warpgroup j % 2, so every slot's barriers are consumed by one warpgroup, in order, and each
+// warpgroup has its next (Q_i, dO_i) pair in flight while it computes.
+namespace dkv64 {
+constexpr int kStages = 4;
+constexpr uint32_t kTileQ = BLKQ64 * HD * 2, kTileK = BLKK * HD * 2;
+constexpr uint32_t kOffK = 0, kOffV = kTileK, kOffQ = 2 * kTileK, kOffDO = kOffQ + kStages * kTileQ;
+constexpr uint32_t kOffStats = kOffDO + kStages * kTileQ;             // [warpgroup][buffer][lse 64 | delta 64] fp32
+constexpr uint32_t kOffBars = kOffStats + 2 * 2 * 128 * 4;
+constexpr uint32_t kSmem = kOffBars + 128;
+enum Bar { kKVFull = 0, kFull = 1 /*4*/, kEmpty = 5 /*4*/ };
+static_assert((kEmpty + kStages) * 8 <= 128, "barriers exceed their shared-memory slot");
+static_assert(HD * 128 * 4 <= 2 * kStages * kTileQ, "partial dK / dV do not fit in the ring");
+}  // namespace dkv64
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads64, 1)
+sla_bwd_dkdv_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
+                        const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v, BwdParams p) {
+  using namespace dkv64;
+  constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
+  const int bh = b * p.h + hh;
+  const int32_t* kv_off = p.kv_off + int64_t(bh) * (p.nblk + 1);
+  const int32_t* list = p.kv_idx + int64_t(bh) * p.mblk * p.topk + __ldg(kv_off + n_blk);
+  const int n_list = __ldg(kv_off + n_blk + 1) - __ldg(kv_off + n_blk);
+
+  if (n_list == 0) {  // no query block selected this key block: its gradients are zero (the outputs are not pre-zeroed)
+    for (int e = threadIdx.x; e < BLKK * HD / 8; e += kThreads64) {
+      const int64_t r = int64_t(n_blk) * BLKK + e / (HD / 8);
+      if (r >= p.l) break;
+      const int64_t o = ((int64_t(b) * p.l + r) * p.h + hh) * HD + (e % (HD / 8)) * 8;
+      stg_v4(static_cast<T*>(p.dk) + o, make_uint4(0, 0, 0, 0));
+      stg_v4(static_cast<T*>(p.dv) + o, make_uint4(0, 0, 0, 0));
+    }
+    return;
+  }
+  if (threadIdx.x == 0) {
+    mbar_init(&bars[kKVFull], 1);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&bars[kFull + i], 1);
+      mbar_init(&bars[kEmpty + i], 4);   // the four warps of warpgroup i % 2
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // =============================================================== TMA producer
+    reg_dealloc<kProducerRegs64>();
+    if (warp == 8 && lane == 0) {
+      tma_prefetch_desc(&tmap_q);
+      tma_prefetch_desc(&tmap_do);
+      tma_prefetch_desc(&tmap_k);
+      tma_prefetch_desc(&tmap_v);
+      mbar_expect_tx(&bars[kKVFull], 2 * kTileK);
+#pragma unroll
+      for (int c = 0; c < HD / 64; ++c) {
+        tma_load_4d(smem + kOffK + c * (BLKK * 128), &tmap_k, &bars[kKVFull], c * 64, hh, n_blk * BLKK, b);
+        tma_load_4d(smem + kOffV + c * (BLKK * 128), &tmap_v, &bars[kKVFull], c * 64, hh, n_blk * BLKK, b);
+      }
+      for (int j = 0; j < n_list; ++j) {
+        const int st = j % kStages;
+        const uint32_t ph = ((j / kStages) & 1) ^ 1;
+        const int qb = __ldg(list + j);
+        mbar_wait(&bars[kEmpty + st], ph);
+        mbar_expect_tx(&bars[kFull + st], 2 * kTileQ);
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c) {
+          tma_load_4d(smem + kOffQ + st * kTileQ + c * (BLKQ64 * 128), &tmap_q, &bars[kFull + st], c * 64, hh, qb * BLKQ64, b);
+          tma_load_4d(smem + kOffDO + st * kTileQ + c * (BLKQ64 * 128), &tmap_do, &bars[kFull + st], c * 64, hh, qb * BLKQ64, b);
+        }
+      }
+    }
+    return;
+  }
+
+  // =============================================================== consumer warpgroups (alternate list entries)
+  reg_alloc<kConsumerRegs64>();
+  const int wg = warp >> 2, w4 = warp & 3, t = threadIdx.x & 127;
+  const int kr_lo = w4 * 16 + (lane >> 2);   // key rows kr_lo, kr_lo + 8 of the block
+  const int cq = 2 * (lane & 3);
+  const uint32_t sbase = smem_u32(smem);
+  const float sc = p.sm_scale * kLog2e;
+  float* stats = reinterpret_cast<float*>(smem + kOffStats) + wg * 256;
+  float dk[HD / 2], dv[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) dk[i] = dv[i] = 0.f;
+
+  mbar_wait(&bars[kKVFull], 0);
+  for (int j = wg, it = 0; j < n_list; j += 2, ++it) {
+    const int st = j % kStages;
+    const uint32_t ph = (j / kStages) & 1;
+    const int qb = __ldg(list + j);
+    // ---- lse / delta of the block's 64 query rows; query rows >= l: P = 0 and delta = 0
+    float* sb = stats + (it & 1) * 128;
+    {
+      const int64_t r = int64_t(qb) * BLKQ64 + (t & 63);
+      const bool in = r < p.l;
+      sb[t] = t < 64 ? (in ? __ldg(p.lse + int64_t(bh) * p.l + r) : INFINITY) : (in ? __ldg(p.delta + int64_t(bh) * p.l + r) : 0.f);
+    }
+    named_bar_sync(1 + wg, 128);
+
+    // ---- S^T = K.Q^T and dP^T = V.dO^T (all operands K-major over d)
+    const uint32_t sq = sbase + kOffQ + st * kTileQ, sg = sbase + kOffDO + st * kTileQ;
+    float s[32], dp[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s[i] = dp[i] = 0.f;
+    mbar_wait(&bars[kFull + st], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks) {
+      const uint64_t kd = make_desc_kmajor_sw128(sbase + kOffK + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
+      const uint64_t qd = make_desc_kmajor_sw128(sq + (ks >> 2) * (BLKQ64 * 128)) + uint64_t((ks & 3) * 2);
+      wgmma_f16_ss<64, kBF16>(s, kd, qd, ks > 0 ? 1u : 0u);
+    }
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks) {
+      const uint64_t vd = make_desc_kmajor_sw128(sbase + kOffV + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
+      const uint64_t gd = make_desc_kmajor_sw128(sg + (ks >> 2) * (BLKQ64 * 128)) + uint64_t((ks & 3) * 2);
+      wgmma_f16_ss<64, kBF16>(dp, vd, gd, ks > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    reg_fence(dp);
+
+    // ---- P^T rounded to T; dV += P^T.dO with dO as the MN-major operand (+16 rows = +2048 B per K step).
+    //      Key rows >= l only reach dK / dV rows that are never stored, so they need no mask.
+    uint32_t pa[4][4], da[4][4];
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const float2 ls = *reinterpret_cast<const float2*>(sb + 8 * (i >> 2) + cq);
+      s[i] = fast_exp2(fmaf(s[i], sc, -ls.x));
+      s[i + 1] = fast_exp2(fmaf(s[i + 1], sc, -ls.y));
+      pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(s[i], s[i + 1]);
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_f16_rs<HD, kBF16, 1>(dv, pa[kk], make_desc_mnmajor_sw128(sg, BLKQ64 * 128) + uint64_t(kk * 128));
+    wgmma_commit();
+    // ---- dS^T = P^T o (dP^T - delta) rounded to T; dK += dS^T.Q
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const float2 dl = *reinterpret_cast<const float2*>(sb + 64 + 8 * (i >> 2) + cq);
+      da[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(s[i] * (dp[i] - dl.x), s[i + 1] * (dp[i + 1] - dl.y));
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_f16_rs<HD, kBF16, 1>(dk, da[kk], make_desc_mnmajor_sw128(sq, BLKQ64 * 128) + uint64_t(kk * 128));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(dv);
+    reg_fence(dk);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      reg_fence(pa[kk]);
+      reg_fence(da[kk]);
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars[kEmpty + st]);
+  }
+
+  // ---- warpgroup 1's partials -> warpgroup 0 through the Q / dO ring (every slot consumed); [value][thread] layout
+  float* xchg = reinterpret_cast<float*>(smem + kOffQ) + t;
+  named_bar_sync(3, 256);
+  if (wg == 1) {
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) {
+      xchg[i * 128] = dk[i];
+      xchg[(HD / 2 + i) * 128] = dv[i];
+    }
+  }
+  named_bar_sync(3, 256);
+  if (wg == 1) return;
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) {
+    dk[i] += xchg[i * 128];
+    dv[i] += xchg[(HD / 2 + i) * 128];
+  }
+  const int64_t row0 = int64_t(n_blk) * BLKK + kr_lo;
+  store_rows<T>(dk, p.sm_scale, p.dk, row0, p.l, p.h, hh, b, cq);
+  store_rows<T>(dv, 1.0f, p.dv, row0, p.l, p.h, hh, b, cq);
+}
+
 // ------------------------------------------------------------------------------------------------ host
 struct WsLayout {
   size_t delta, kv_off, cursor, kv_idx, total;
 };
 size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
-WsLayout ws_layout(int64_t b, int64_t h, int64_t l, int64_t topk) {
-  const int64_t mblk = cdiv64(l, BLKQ), nblk = cdiv64(l, BLKK), bh = b * h;
+WsLayout ws_layout(int64_t b, int64_t h, int64_t l, int64_t topk, int64_t blkq) {
+  const int64_t mblk = cdiv64(l, blkq), nblk = cdiv64(l, BLKK), bh = b * h;
   WsLayout w;
   w.delta = 0;
   w.kv_off = w.delta + align256(size_t(bh * l) * 4);
@@ -490,12 +860,12 @@ int tmap_rows(CUtensorMap* m, const void* base, CUtensorMapDataType t16, int64_t
   return make_tmap_4d(m, base, t16, 2, dims, str, box);
 }
 
-template <typename T>
+template <typename T, int kBQ>
 int launch_bwd(const void* q, const void* k, const void* v, const void* o_s, const void* d_o, const float* lse, const int32_t* lut,
                int64_t topk, void* dq, void* dk, void* dv, uint8_t* ws, int64_t b, int64_t l, int64_t h, float sm_scale,
                cudaStream_t st) {
-  const int64_t mblk = cdiv64(l, BLKQ), nblk = cdiv64(l, BLKK);
-  const WsLayout w = ws_layout(b, h, l, topk);
+  const int64_t mblk = cdiv64(l, kBQ), nblk = cdiv64(l, BLKK);
+  const WsLayout w = ws_layout(b, h, l, topk, kBQ);
   float* delta = reinterpret_cast<float*>(ws + w.delta);
   int32_t* kv_off = reinterpret_cast<int32_t*>(ws + w.kv_off);
   int32_t* cursor = reinterpret_cast<int32_t*>(ws + w.cursor);
@@ -503,8 +873,8 @@ int launch_bwd(const void* q, const void* k, const void* v, const void* o_s, con
   const CUtensorMapDataType t16 = std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                                                         : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUtensorMap tq, tdo, tk, tv;
-  if (int rc = tmap_rows(&tq, q, t16, b, l, h, BLKQ)) return rc;
-  if (int rc = tmap_rows(&tdo, d_o, t16, b, l, h, BLKQ)) return rc;
+  if (int rc = tmap_rows(&tq, q, t16, b, l, h, kBQ)) return rc;
+  if (int rc = tmap_rows(&tdo, d_o, t16, b, l, h, kBQ)) return rc;
   if (int rc = tmap_rows(&tk, k, t16, b, l, h, BLKK)) return rc;
   if (int rc = tmap_rows(&tv, v, t16, b, l, h, BLKK)) return rc;
 
@@ -531,53 +901,84 @@ int launch_bwd(const void* q, const void* k, const void* v, const void* o_s, con
   p.topk = int(topk);
   p.sm_scale = sm_scale;
 
-  const size_t smem_dq = 1024 + dq::kOffLut + ((size_t(topk) * 2 + 15) & ~size_t(15));
-  if (int rc = check_cuda(cudaFuncSetAttribute(sla_bwd_dq_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_dq)),
+  constexpr bool kQ64 = kBQ == BLKQ64;
+  const auto dq_kern = kQ64 ? sla_bwd_dq_q64_kernel<T> : sla_bwd_dq_kernel<T>;
+  const auto dkdv_kern = kQ64 ? sla_bwd_dkdv_q64_kernel<T> : sla_bwd_dkdv_kernel<T>;
+  const int threads_dq = kQ64 ? kThreads64 : dq::kThreads, threads_kv = kQ64 ? kThreads64 : dkv::kThreads;
+  const size_t smem_dq = 1024 + (kQ64 ? dq64::kOffLut : dq::kOffLut) + ((size_t(topk) * 2 + 15) & ~size_t(15));
+  if (int rc = check_cuda(cudaFuncSetAttribute(dq_kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_dq)),
                           "cudaFuncSetAttribute(sla_bwd_dq)"))
     return rc;
-  sla_bwd_dq_kernel<T><<<dim3(unsigned(mblk), unsigned(h), unsigned(b)), dq::kThreads, smem_dq, st>>>(tq, tdo, tk, tv, p);
+  dq_kern<<<dim3(unsigned(mblk), unsigned(h), unsigned(b)), threads_dq, smem_dq, st>>>(tq, tdo, tk, tv, p);
   if (int rc = check_launch("sla_bwd_dq_kernel")) return rc;
 
-  const size_t smem_kv = 1024 + dkv::kSmem;
-  if (int rc = check_cuda(cudaFuncSetAttribute(sla_bwd_dkdv_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_kv)),
+  const size_t smem_kv = 1024 + (kQ64 ? dkv64::kSmem : dkv::kSmem);
+  if (int rc = check_cuda(cudaFuncSetAttribute(dkdv_kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_kv)),
                           "cudaFuncSetAttribute(sla_bwd_dkdv)"))
     return rc;
-  sla_bwd_dkdv_kernel<T><<<dim3(unsigned(nblk), unsigned(h), unsigned(b)), dkv::kThreads, smem_kv, st>>>(tq, tdo, tk, tv, p);
+  dkdv_kern<<<dim3(unsigned(nblk), unsigned(h), unsigned(b)), threads_kv, smem_kv, st>>>(tq, tdo, tk, tv, p);
   return check_launch("sla_bwd_dkdv_kernel");
+}
+
+int check_blkq(const char* what, int64_t blkq, int64_t blkk) {
+  if ((blkq == BLKQ || blkq == BLKQ64) && blkk == BLKK) return 0;
+  return fail(TDB200_ERR_UNSUPPORTED, "%s: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 64)", what, (long long)blkq,
+              (long long)blkk);
 }
 
 }  // namespace
 
-extern "C" int64_t tdb200_sla_attn_bwd_workspace_bytes(int64_t b, int64_t h, int64_t l, int64_t topk) {
+extern "C" int64_t tdb200_sla_attn16_bwd_workspace_bytes(int64_t b, int64_t h, int64_t l, int64_t topk, int64_t blkq) {
+  if (int rc = check_blkq("sla_attn16_bwd_workspace_bytes", blkq, BLKK)) return rc;
   if (b <= 0 || h <= 0 || l <= 0 || topk <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_bwd_workspace_bytes: bad shape");
-  return int64_t(ws_layout(b, h, l, topk).total);
+  return int64_t(ws_layout(b, h, l, topk, blkq).total);
+}
+
+// (blkq, blkk) = (128, 64) runs sla_bwd_dq_kernel / sla_bwd_dkdv_kernel, (64, 64) their _q64 forms.
+extern "C" int tdb200_sla_attn16_bwd(const void* q, const void* k, const void* v, const void* o_s, const void* d_o, const float* lse,
+                                     int dtype, const int32_t* lut, int64_t topk, void* dq, void* dk, void* dv, void* workspace,
+                                     int64_t workspace_bytes, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale,
+                                     int64_t blkq, int64_t blkk, void* stream) {
+  if (int rc = check_blkq("sla_attn16_bwd", blkq, blkk)) return rc;
+  if (!q || !k || !v || !o_s || !d_o || !lse || !lut || !dq || !dk || !dv || !workspace)
+    return fail(TDB200_ERR_INVALID_ARG, "sla_attn16_bwd: null pointer");
+  if (b <= 0 || l <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_attn16_bwd: bad shape");
+  const int64_t mblk = cdiv64(l, blkq), nblk = cdiv64(l, BLKK);
+  if (topk <= 0 || topk > nblk)
+    return fail(TDB200_ERR_INVALID_ARG, "sla_attn16_bwd: topk=%lld outside [1, %lld]", (long long)topk, (long long)nblk);
+  if (d != HD) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn16_bwd: head dim %lld (this kernel implements d=128)", (long long)d);
+  if (dtype != TDB200_DTYPE_BF16 && dtype != TDB200_DTYPE_FP16)
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn16_bwd: dtype tag %d", dtype);
+  if (nblk > 65535 || h > 65535 || b > 65535 || b * h * mblk * topk > 0x7FFFFFFF)
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn16_bwd: dimension too large");
+  if (1024 + (blkq == BLKQ ? dq::kOffLut : dq64::kOffLut) + ((size_t(topk) * 2 + 15) & ~size_t(15)) > 227 * 1024)
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn16_bwd: topk=%lld too large for on-chip LUT", (long long)topk);
+  const int64_t need = int64_t(ws_layout(b, h, l, topk, blkq).total);
+  if (workspace_bytes < need)
+    return fail(TDB200_ERR_WORKSPACE, "sla_attn16_bwd: workspace of %lld bytes, %lld needed", (long long)workspace_bytes,
+                (long long)need);
+  if (int rc = require_sm90()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  // the (128, 64) kernels are instantiated first: nvcc's output for them depends on the order
+  if (blkq == BLKQ) {
+    if (dtype == TDB200_DTYPE_BF16)
+      return launch_bwd<__nv_bfloat16, BLKQ>(q, k, v, o_s, d_o, lse, lut, topk, dq, dk, dv, ws, b, l, h, sm_scale, st);
+    return launch_bwd<__half, BLKQ>(q, k, v, o_s, d_o, lse, lut, topk, dq, dk, dv, ws, b, l, h, sm_scale, st);
+  }
+  if (dtype == TDB200_DTYPE_BF16)
+    return launch_bwd<__nv_bfloat16, BLKQ64>(q, k, v, o_s, d_o, lse, lut, topk, dq, dk, dv, ws, b, l, h, sm_scale, st);
+  return launch_bwd<__half, BLKQ64>(q, k, v, o_s, d_o, lse, lut, topk, dq, dk, dv, ws, b, l, h, sm_scale, st);
+}
+
+extern "C" int64_t tdb200_sla_attn_bwd_workspace_bytes(int64_t b, int64_t h, int64_t l, int64_t topk) {
+  return tdb200_sla_attn16_bwd_workspace_bytes(b, h, l, topk, BLKQ);
 }
 
 extern "C" int tdb200_sla_attn_bwd_qk16(const void* q, const void* k, const void* v, const void* o_s, const void* d_o, const float* lse,
                                         int dtype, const int32_t* lut, int64_t topk, void* dq, void* dk, void* dv, void* workspace,
                                         int64_t workspace_bytes, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale,
                                         void* stream) {
-  if (!q || !k || !v || !o_s || !d_o || !lse || !lut || !dq || !dk || !dv || !workspace)
-    return fail(TDB200_ERR_INVALID_ARG, "sla_attn_bwd_qk16: null pointer");
-  if (b <= 0 || l <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_bwd_qk16: bad shape");
-  const int64_t mblk = cdiv64(l, BLKQ), nblk = cdiv64(l, BLKK);
-  if (topk <= 0 || topk > nblk)
-    return fail(TDB200_ERR_INVALID_ARG, "sla_attn_bwd_qk16: topk=%lld outside [1, %lld]", (long long)topk, (long long)nblk);
-  if (d != HD) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_bwd_qk16: head dim %lld (this kernel implements d=128)", (long long)d);
-  if (dtype != TDB200_DTYPE_BF16 && dtype != TDB200_DTYPE_FP16)
-    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_bwd_qk16: dtype tag %d", dtype);
-  if (nblk > 65535 || h > 65535 || b > 65535 || b * h * mblk * topk > 0x7FFFFFFF)
-    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_bwd_qk16: dimension too large");
-  if (1024 + dq::kOffLut + ((size_t(topk) * 2 + 15) & ~size_t(15)) > 227 * 1024)
-    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_bwd_qk16: topk=%lld too large for on-chip LUT", (long long)topk);
-  const int64_t need = int64_t(ws_layout(b, h, l, topk).total);
-  if (workspace_bytes < need)
-    return fail(TDB200_ERR_WORKSPACE, "sla_attn_bwd_qk16: workspace of %lld bytes, %lld needed", (long long)workspace_bytes,
-                (long long)need);
-  if (int rc = require_sm90()) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  if (dtype == TDB200_DTYPE_BF16)
-    return launch_bwd<__nv_bfloat16>(q, k, v, o_s, d_o, lse, lut, topk, dq, dk, dv, ws, b, l, h, sm_scale, st);
-  return launch_bwd<__half>(q, k, v, o_s, d_o, lse, lut, topk, dq, dk, dv, ws, b, l, h, sm_scale, st);
+  return tdb200_sla_attn16_bwd(q, k, v, o_s, d_o, lse, dtype, lut, topk, dq, dk, dv, workspace, workspace_bytes, b, l, h, d, sm_scale,
+                               BLKQ, BLKK, stream);
 }

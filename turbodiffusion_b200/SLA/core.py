@@ -14,7 +14,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from .._lib import DTYPE_TAG, check, lib, ptr, require_cuda, stream_ptr
+from .. import _ops
+from .._lib import require_cuda
 from .utils import (SAGE_BLOCKS, QKPrep, block_map_from_pools, get_block_map, get_cuda_arch, quant_k_into,  # noqa: F401
                     quant_q_only, quant_qk)
 
@@ -29,11 +30,8 @@ def linear_moments(k: torch.Tensor, v: torch.Tensor, feature: int = 0):
     """kv [B,H,D(v),D(k)] fp32, ksum [B,H,D] fp32 of the local keys (accumulated: add shards / all-reduce).  D in {64, 128};
     `feature`: 0 softmax over D, 1 elu+1, 2 relu."""
     b, l, h, d = k.shape
-    buf = torch.zeros(b * h * d * (d + 1), dtype=torch.float32, device=k.device)        # one fill for both accumulators
-    kv, ksum = buf[: b * h * d * d].view(b, h, d, d), buf[b * h * d * d:].view(b, h, d)
-    check(lib().tdb200_sla_linear_moments(ptr(k), ptr(v), DTYPE_TAG[k.dtype], b, l, h, d, feature, ptr(kv), ptr(ksum),
-                                          stream_ptr(k.device)), "sla_linear_moments")
-    return kv, ksum
+    buf = _ops.sla_linear_moments(k, v, feature)        # both accumulators in one buffer: one fill
+    return buf[: b * h * d * d].view(b, h, d, d), buf[b * h * d * d:].view(b, h, d)
 
 
 def project_moments(proj_w: torch.Tensor, kv: torch.Tensor, dtype) -> torch.Tensor:
@@ -41,10 +39,7 @@ def project_moments(proj_w: torch.Tensor, kv: torch.Tensor, dtype) -> torch.Tens
     b, h, d, _ = kv.shape
     w = proj_w if (proj_w.dtype == torch.float32 and proj_w.is_contiguous()) else proj_w.float().contiguous()
     assert kv.dtype == torch.float32 and kv.is_contiguous() and w.shape == (d, d)
-    out = torch.empty(b, h, d, d, dtype=dtype, device=kv.device)
-    check(lib().tdb200_sla_project_moments(ptr(w), ptr(kv), DTYPE_TAG[dtype], b * h, d, ptr(out), stream_ptr(kv.device)),
-          "sla_project_moments")
-    return out
+    return _ops.sla_project_moments(w, kv, dtype)
 
 
 ATTN_TIMER = None  # bench.py installs a callable(h, mblk, topk, d) -> context manager to time the fused-attention launches
@@ -60,76 +55,42 @@ def attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, featur
 
 
 def _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, feature=0, blkq=128, blkk=64):
-    b, l, h, d = q.shape
+    d = q.shape[3]
     lk = v.shape[1] if lk is None else lk
-    out = torch.empty_like(q)
-    k_seq_major = int(getattr(prep, "k_seq_major", False))   # INT8 K in the gathered [B, Lk, H, D] layout (dist.py)
+    k_seq_major = bool(getattr(prep, "k_seq_major", False))   # INT8 K in the gathered [B, Lk, H, D] layout (dist.py)
     if k_seq_major and (d != 128 or feature != 0):
         raise NotImplementedError("sequence-major INT8 K is served by the 128-wide softmax kernels only")
-    check(lib().tdb200_sla_attn_fwd(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v), ptr(q),
-                                    DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b), ptr(out), b, l, lk, h, d,
-                                    float(sm_scale), feature, blkq, blkk, k_seq_major, stream_ptr(q.device)), "sla_attn_fwd")
-    return out
+    return _ops.sla_attn_fwd(prep.q_i8, prep.q_scale, prep.k_i8, prep.k_scale, v, q, lut, topk, kvw, ksum, proj_b,
+                             float(sm_scale), lk, feature, blkq, blkk, k_seq_major)
 
 
-# The 16-bit attention serves 64-row key blocks with 128- or 64-row query blocks; `blkq` below is the query block size `lut`
-# was built with.
-BLKK16 = 64
+# The 16-bit attention serves 64-row key blocks (_ops.BLKK16) with 128- or 64-row query blocks; `blkq` below is the query
+# block size `lut` was built with.
 
 
 def attn_fwd_qk16(q, k, v, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, feature=0, blkq=128):
     """The non-quantised sparse attention (a9', SLA/kernel.py:33-82): 16-bit Q.K^T on the tensor cores, fp32 scores, and the
     linear branch with feature map `feature`."""
-    b, l, h, d = q.shape
     lk = v.shape[1] if lk is None else lk
-    out = torch.empty_like(q)
-    check(lib().tdb200_sla_attn16_fwd(ptr(q), ptr(k), ptr(v), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b),
-                                      ptr(out), b, l, lk, h, d, float(sm_scale), feature, blkq, BLKK16, stream_ptr(q.device)),
-          "sla_attn16_fwd")
-    return out
+    return _ops.sla_attn16_fwd(q, k, v, lut, topk, kvw, ksum, proj_b, float(sm_scale), lk, feature, blkq)
 
 
 def attn_fwd_qk16_lse(q, k, v, lut, topk, sm_scale, blkq=128):
     """Sparse branch of attn_fwd_qk16 alone, for the training path: (o_s [B,L,H,D] in q.dtype, lse [B,H,L] fp32), lse being
-    the row log-sum-exp of the scores in log2 units (scores scaled by sm_scale * log2(e)).  `lut` [B,H,Mblk,topk] int32."""
-    b, l, h, d = q.shape
-    o_s = torch.empty_like(q)
-    lse = torch.empty(b, h, l, dtype=torch.float32, device=q.device)
-    check(lib().tdb200_sla_attn16_fwd_lse(ptr(q), ptr(k), ptr(v), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(o_s), ptr(lse), b, l, h, d,
-                                          float(sm_scale), blkq, BLKK16, stream_ptr(q.device)), "sla_attn16_fwd_lse")
-    return o_s, lse
+    the row log-sum-exp of the scores in log2 units (scores scaled by sm_scale * log2(e)).  `lut` [B,H,Mblk,topk] int32.
+    Differentiable in q, k and v through o_s (the backward is attn_bwd_qk16)."""
+    return _ops.sla_attn16_fwd_lse(q, k, v, lut, topk, float(sm_scale), blkq)
 
 
 def attn_bwd_qk16(q, k, v, o_s, d_o, lse, lut, topk, sm_scale, blkq=128):
     """(dq, dk, dv) of attn_fwd_qk16_lse's o_s for the incoming gradient d_o; all [B,L,H,D] contiguous in q.dtype."""
-    b, l, h, d = q.shape
-    dq, dk, dv = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
-    nbytes = lib().tdb200_sla_attn16_bwd_workspace_bytes(b, h, l, topk, blkq)
-    check(0 if nbytes >= 0 else nbytes, "sla_attn16_bwd_workspace_bytes", launches=0)
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
-    check(lib().tdb200_sla_attn16_bwd(ptr(q), ptr(k), ptr(v), ptr(o_s), ptr(d_o), ptr(lse), DTYPE_TAG[q.dtype], ptr(lut), topk,
-                                      ptr(dq), ptr(dk), ptr(dv), ptr(ws), nbytes, b, l, h, d, float(sm_scale), blkq, BLKK16,
-                                      stream_ptr(q.device)), "sla_attn16_bwd")
-    return dq, dk, dv
+    return _ops.sla_attn16_bwd(q, k, v, o_s, d_o, lse, lut, topk, float(sm_scale), blkq)
 
 
-class SparseAttention16(torch.autograd.Function):
+def sparse_attention16(q, k, v, lut, topk, sm_scale, blkq=128):
     """o_s = block-sparse softmax attention of q, k, v ([B,L,H,D], 16-bit, d = 128) over `lut`'s key blocks (`blkq`-row query
     blocks, 64-row key blocks), differentiable in q, k and v (the reference's `_attention`, SLA/kernel.py:240-319)."""
-
-    @staticmethod
-    def forward(ctx, q, k, v, lut, topk, sm_scale, blkq=128):
-        o_s, lse = attn_fwd_qk16_lse(q, k, v, lut, topk, sm_scale, blkq)
-        ctx.save_for_backward(q, k, v, o_s, lse, lut)
-        ctx.topk, ctx.sm_scale, ctx.blkq = topk, sm_scale, blkq
-        return o_s
-
-    @staticmethod
-    def backward(ctx, d_o):
-        q, k, v, o_s, lse, lut = ctx.saved_tensors
-        d_o = d_o.to(q.dtype).contiguous()
-        dq, dk, dv = attn_bwd_qk16(q, k, v, o_s, d_o, lse, lut, ctx.topk, ctx.sm_scale, ctx.blkq)
-        return dq, dk, dv, None, None, None, None
+    return attn_fwd_qk16_lse(q, k, v, lut, topk, sm_scale, blkq)[0]
 
 
 def select_prep(q, k, blkq, blkk):
@@ -192,19 +153,19 @@ class _SLABase(nn.Module):
             self._keep_selection.update(lut=lut, sparse_map=sparse_map, topk=real_topk)
         kv, ksum = linear_moments(k, v, self.feature)
         # proj_l folded into the moments: (phi(q) KV / den) W^T + b == phi(q) (W KV^T)^T / den + b ; kv is [dv, dk]
-        kvw = project_moments(self.proj_l.weight, kv, self.dtype)  # [B,H,d_out,d_k]
+        # forward-only kernels: proj_l enters as data (detached), so the output carries no autograd history
+        kvw = project_moments(self.proj_l.weight.detach(), kv, self.dtype)  # [B,H,d_out,d_k]
+        proj_b = self.proj_l.bias.detach().float().contiguous()
         if not self.quantised_qk and d == 128 and (self.feature == 0 or blkq == 64):
-            o = attn_fwd_qk16(q, k, v, lut, real_topk, kvw, ksum, self.proj_l.bias.float().contiguous(), d ** -0.5,
-                              feature=self.feature, blkq=blkq)
+            o = attn_fwd_qk16(q, k, v, lut, real_topk, kvw, ksum, proj_b, d ** -0.5, feature=self.feature, blkq=blkq)
         else:
-            o = attn_fwd(prep, v, q, lut, real_topk, kvw, ksum, self.proj_l.bias.float().contiguous(), d ** -0.5,
-                         feature=self.feature, blkq=blkq, blkk=blkk)
+            o = attn_fwd(prep, v, q, lut, real_topk, kvw, ksum, proj_b, d ** -0.5, feature=self.feature, blkq=blkq, blkk=blkk)
         o = o if o.dtype == dtype else o.to(dtype)
         return (o, real_topk / nblk) if return_sparsity else o
 
     def _forward_train(self, q, k, v, return_sparsity):
         """The reference's SparseLinearAttention.forward (SLA/core.py:81-119) with autograd: the same block selection as the
-        fused path, the sparse branch through SparseAttention16, the linear branch and proj_l in torch at the reference's
+        fused path, the sparse branch through sparse_attention16, the linear branch and proj_l in torch at the reference's
         rounding points (feature maps -> dtype, bmm in dtype, proj_l evaluated in dtype as under its autocast)."""
         if q.shape[-1] != 128:
             raise NotImplementedError(f"SparseLinearAttention backward: head dim {q.shape[-1]}; gradients are served for d = 128")
@@ -220,7 +181,7 @@ class _SLABase(nn.Module):
             sparse_map, lut = block_map_from_pools(prep.q_pool, prep.k_pool, real_topk)
         if getattr(self, "_keep_selection", None) is not None:
             self._keep_selection.update(lut=lut, sparse_map=sparse_map, topk=real_topk)
-        o_s = SparseAttention16.apply(q, k, v, lut, real_topk, d ** -0.5, blkq)
+        o_s = sparse_attention16(q, k, v, lut, real_topk, d ** -0.5, blkq)
         qh, kh, vh = (t.transpose(1, 2) for t in (q, k, v))                       # [B, H, L, D] views
         c_q = self.feature_map_q(qh).contiguous().to(self.dtype)
         c_k = self.feature_map_k(kh).contiguous().to(self.dtype)

@@ -3,6 +3,7 @@ from __future__ import annotations
 
 import torch
 
+from .. import _ops
 from .._lib import DTYPE_TAG, check, lib, ptr, require_cuda, stream_ptr
 
 
@@ -53,53 +54,26 @@ def quant_qk(q: torch.Tensor, k: torch.Tensor, lk: int = None, blkq: int = 128, 
     lk = k.shape[1] if lk is None else lk
     assert k.shape[0] == b and k.shape[2:] == q.shape[2:] and lk <= k.shape[1]
     assert q.is_contiguous() and k.is_contiguous() and (b == 1 or lk == k.shape[1])
-    dev = q.device
-    mblk, nblk = cdiv(lq, blkq), cdiv(lk, blkk)
     o = QKPrep()
-    o.mblk, o.nblk = mblk, nblk
-    o.kmean = torch.empty(b, h, d, dtype=torch.float32, device=dev)
-    o.q_i8 = torch.empty(b, h, lq, d, dtype=torch.int8, device=dev)
-    o.k_i8 = torch.empty(b, h, lk, d, dtype=torch.int8, device=dev)
-    o.q_scale = torch.empty(b, h, mblk, dtype=torch.float32, device=dev)
-    o.k_scale = torch.empty(b, h, nblk, dtype=torch.float32, device=dev)
-    o.q_pool = torch.empty(b, h, mblk, d, dtype=q.dtype, device=dev)
-    o.k_pool = torch.empty(b, h, nblk, d, dtype=q.dtype, device=dev)
-    check(lib().tdb200_sla_quant_qk(ptr(q), ptr(k), DTYPE_TAG[q.dtype], b, lq, lk, h, d, ptr(o.kmean), ptr(o.q_i8), ptr(o.q_scale),
-                                    ptr(o.k_i8), ptr(o.k_scale), ptr(o.q_pool), ptr(o.k_pool), blkq, blkk, stream_ptr(dev)),
-          "sla_quant_qk")
+    o.mblk, o.nblk, o.k_seq_major = cdiv(lq, blkq), cdiv(lk, blkk), False
+    o.kmean, o.q_i8, o.q_scale, o.k_i8, o.k_scale, o.q_pool, o.k_pool = _ops.sla_quant_qk(q, k, lk, blkq, blkk)
     return o
 
 
 def quant_q_only(q: torch.Tensor, blkq: int = 128) -> QKPrep:
     """The query half of quant_qk (pooled means + Sage INT8 of q); fill in the key half later with quant_k_into()."""
     require_cuda(q)
-    b, lq, h, d = q.shape
-    dev = q.device
     o = QKPrep()
-    o.mblk = cdiv(lq, blkq)
-    o.q_i8 = torch.empty(b, h, lq, d, dtype=torch.int8, device=dev)
-    o.q_scale = torch.empty(b, h, o.mblk, dtype=torch.float32, device=dev)
-    o.q_pool = torch.empty(b, h, o.mblk, d, dtype=q.dtype, device=dev)
-    # the key block size only matters to the key half; any valid pair with this blkq serves
-    check(lib().tdb200_sla_quant_qk(ptr(q), None, DTYPE_TAG[q.dtype], b, lq, lq, h, d, None, ptr(o.q_i8), ptr(o.q_scale), None,
-                                    None, ptr(o.q_pool), None, blkq, 64 if blkq == 128 else 128, stream_ptr(dev)),
-          "sla_quant_qk", launches=1)
+    o.mblk, o.k_seq_major = cdiv(q.shape[1], blkq), False
+    o.q_i8, o.q_scale, o.q_pool = _ops.sla_quant_q(q, blkq)
     return o
 
 
 def quant_k_into(o: QKPrep, k: torch.Tensor, lk: int, blkk: int = 64) -> QKPrep:
     """The key half of quant_qk on the first `lk` rows of k [B, >=lk, H, D]."""
     require_cuda(k)
-    b, _, h, d = k.shape
-    dev = k.device
     o.nblk = cdiv(lk, blkk)
-    o.kmean = torch.empty(b, h, d, dtype=torch.float32, device=dev)
-    o.k_i8 = torch.empty(b, h, lk, d, dtype=torch.int8, device=dev)
-    o.k_scale = torch.empty(b, h, o.nblk, dtype=torch.float32, device=dev)
-    o.k_pool = torch.empty(b, h, o.nblk, d, dtype=k.dtype, device=dev)
-    check(lib().tdb200_sla_quant_qk(None, ptr(k), DTYPE_TAG[k.dtype], b, lk, lk, h, d, ptr(o.kmean), None, None, ptr(o.k_i8),
-                                    ptr(o.k_scale), None, ptr(o.k_pool), 128 if blkk == 64 else 64, blkk, stream_ptr(dev)),
-          "sla_quant_qk", launches=3)
+    o.kmean, o.k_i8, o.k_scale, o.k_pool = _ops.sla_quant_k(k, lk, blkk)
     return o
 
 
@@ -141,13 +115,7 @@ def quant_k_seq(k: torch.Tensor, kmean: torch.Tensor, k_i8=None, blkk: int = 64)
 
 def block_map_from_pools(q_pool: torch.Tensor, k_pool: torch.Tensor, topk: int):
     """Pooled score + top-k (SLA/utils.py:59-66).  Returns (sparse_map int8 [B,H,Mblk,Nblk], lut int32 ascending)."""
-    b, h, mblk, d = q_pool.shape
-    nblk = k_pool.shape[2]
-    sparse_map = torch.empty(b, h, mblk, nblk, dtype=torch.int8, device=q_pool.device)
-    lut = torch.empty(b, h, mblk, topk, dtype=torch.int32, device=q_pool.device)
-    check(lib().tdb200_sla_block_map(ptr(q_pool), ptr(k_pool), DTYPE_TAG[q_pool.dtype], b, h, mblk, nblk, d, topk,
-                                     ptr(sparse_map), ptr(lut), stream_ptr(q_pool.device)), "sla_block_map")
-    return sparse_map, lut
+    return _ops.sla_block_map(q_pool, k_pool, topk)
 
 
 def mean_pool(x: torch.Tensor, BLK: int) -> torch.Tensor:

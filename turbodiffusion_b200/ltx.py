@@ -7,7 +7,8 @@ from __future__ import annotations
 
 import torch
 
-from ._lib import DTYPE_TAG, check, lib, ptr, require_cuda, stream_ptr
+from . import _ops
+from ._lib import DTYPE_TAG, require_cuda
 
 
 def _prep(x, table, timestep, num_ada):
@@ -15,46 +16,28 @@ def _prep(x, table, timestep, num_ada):
     assert x.dim() == 3 and x.dtype in DTYPE_TAG
     b, t, n = x.shape
     ts = timestep.reshape(b, -1, num_ada * n).to(x.dtype).contiguous()
-    return x.contiguous(), table.float().contiguous(), ts, b, t, ts.shape[1], n
+    return x.contiguous(), table.float().contiguous(), ts
 
 
 def modulated_rms_norm_from_ada(x, scale_shift_table, timestep, scale_index, shift_index, num_ada_params, eps):
-    x, tab, ts, b, t, tt, n = _prep(x, scale_shift_table, timestep, num_ada_params)
-    y = torch.empty_like(x)
-    check(lib().tdb200_ltx_modulated_rms_norm_ada(ptr(x), DTYPE_TAG[x.dtype], ptr(tab), ptr(ts), scale_index, shift_index,
-                                                  num_ada_params, ptr(y), b, t, tt, n, float(eps), stream_ptr(x.device)),
-          "ltx_modulated_rms_norm_ada")
-    return y
+    x, tab, ts = _prep(x, scale_shift_table, timestep, num_ada_params)
+    return _ops.ltx_modulated_rms_norm_ada(x, tab, ts, scale_index, shift_index, num_ada_params, float(eps))
 
 
 def modulate_from_ada(x, scale_shift_table, timestep, scale_index, shift_index, num_ada_params):
-    x, tab, ts, b, t, tt, n = _prep(x, scale_shift_table, timestep, num_ada_params)
-    y = torch.empty_like(x)
-    check(lib().tdb200_ltx_modulate_ada(ptr(x), DTYPE_TAG[x.dtype], ptr(tab), ptr(ts), scale_index, shift_index,
-                                        num_ada_params, ptr(y), b, t, tt, n, stream_ptr(x.device)), "ltx_modulate_ada")
-    return y
+    x, tab, ts = _prep(x, scale_shift_table, timestep, num_ada_params)
+    return _ops.ltx_modulate_ada(x, tab, ts, scale_index, shift_index, num_ada_params)
 
 
 def gated_residual_from_ada(x, residual, scale_shift_table, timestep, gate_index, num_ada_params):
-    x, tab, ts, b, t, tt, n = _prep(x, scale_shift_table, timestep, num_ada_params)
-    residual = residual.to(x.dtype).contiguous()
-    y = torch.empty_like(x)
-    check(lib().tdb200_ltx_gated_residual_ada(ptr(x), ptr(residual), DTYPE_TAG[x.dtype], ptr(tab), ptr(ts), gate_index,
-                                              num_ada_params, ptr(y), b, t, tt, n, stream_ptr(x.device)),
-          "ltx_gated_residual_ada")
-    return y
+    x, tab, ts = _prep(x, scale_shift_table, timestep, num_ada_params)
+    return _ops.ltx_gated_residual_ada(x, residual.to(x.dtype).contiguous(), tab, ts, gate_index, num_ada_params)
 
 
 def apply_split_rotary_emb(x, cos_freqs, sin_freqs):
     """x [B, T, H*D] (or [B, T, H, D]); cos/sin [B, H, T, D/2]  (ltx_core/model/transformer/rope.py:42-60)."""
     require_cuda(x, cos_freqs, sin_freqs)
-    b, h, t, half = cos_freqs.shape
-    xc = x.contiguous()
-    y = torch.empty_like(xc)
-    c, s = cos_freqs.to(x.dtype).contiguous(), sin_freqs.to(x.dtype).contiguous()
-    check(lib().tdb200_ltx_split_rope(ptr(xc), ptr(c), ptr(s), DTYPE_TAG[x.dtype], ptr(y), b, t, h, 2 * half,
-                                      stream_ptr(x.device)), "ltx_split_rope")
-    return y
+    return _ops.ltx_split_rope(x.contiguous(), cos_freqs.to(x.dtype).contiguous(), sin_freqs.to(x.dtype).contiguous())
 
 
 # ------------------------------------------------------------------------------------------------ per-row post-scale W8A8
@@ -62,11 +45,12 @@ def row_quant_int8(x: torch.Tensor, out_q: torch.Tensor = None, out_s: torch.Ten
     """ltx_distillation/tilelang_w8a8.py:39-75: x [M,K] bf16/fp16 -> (int8 [M,K], fp32 scale [M])."""
     require_cuda(x)
     assert x.dim() == 2 and x.is_contiguous() and x.dtype in DTYPE_TAG
+    if out_q is None and out_s is None:
+        return _ops.quant_int8_rowwise(x)
     m, k = x.shape
     q = torch.empty((m, k), dtype=torch.int8, device=x.device) if out_q is None else out_q
     s = torch.empty((m,), dtype=torch.float32, device=x.device) if out_s is None else out_s
-    check(lib().tdb200_quant_int8_rowwise(ptr(x), DTYPE_TAG[x.dtype], m, k, ptr(q), ptr(s), stream_ptr(x.device)),
-          "quant_int8_rowwise")
+    _ops.quant_int8_rowwise_out(x, q, s)
     return q, s
 
 
@@ -74,14 +58,9 @@ def gemm_int8_post_scale_bias(x_q, x_s, w_q, w_s, bias, out_dtype=torch.bfloat16
     """_tl_gemm_int8_post_scale_bias (tilelang_w8a8.py:78-117): C = acc_int32 * sA[i] * sB[j] + bias[j], evaluated as the
     reference's compiled kernel does: fma(float(acc) * sA[i], sB[j], bias[j]) (see tools/tilelang_epilogue_probe.py)."""
     require_cuda(x_q, x_s, w_q, w_s, bias)
-    m, k = x_q.shape
-    n = w_q.shape[0]
-    y = torch.empty((m, n), dtype=out_dtype, device=x_q.device)
     if bias is not None and bias.dtype != out_dtype:
         bias = bias.to(out_dtype)
-    check(lib().tdb200_gemm_w8a8_rowwise(ptr(x_q), ptr(x_s), ptr(w_q), ptr(w_s), ptr(bias), ptr(y), DTYPE_TAG[out_dtype],
-                                         m, n, k, stream_ptr(x_q.device)), "gemm_w8a8_rowwise")
-    return y
+    return _ops.gemm_w8a8_rowwise(x_q, x_s, w_q, w_s, bias, out_dtype)
 
 
 class PostScaleInt8Linear(torch.nn.Module):

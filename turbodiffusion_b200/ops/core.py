@@ -13,7 +13,8 @@ from typing import Optional, Tuple
 import torch
 import torch.nn as nn
 
-from .._lib import DTYPE_TAG, check, lib, ptr, require_cuda, stream_ptr
+from .. import _ops
+from .._lib import DTYPE_TAG, require_cuda
 from ..turbo_diffusion_ops import quant_cuda, gemm_cuda, gemm_cuda_swizzle_bias
 
 
@@ -65,8 +66,7 @@ def rmsnorm(x: torch.Tensor, w: torch.Tensor, eps: float) -> torch.Tensor:
     if x2.dtype != torch.float32:
         raise RuntimeError("rmsnorm expects an fp32 input (the module casts with x.float())")
     y = torch.empty_like(x2)
-    check(lib().tdb200_rms_norm_f32(ptr(x2), ptr(w.float()), ptr(y), x2.shape[0], x2.shape[1], float(eps),
-                                    stream_ptr(x.device)), "rmsnorm")
+    _ops.rms_norm_f32(x2, w.float(), float(eps), y)
     return y.reshape(x.shape)
 
 
@@ -81,9 +81,7 @@ def layernorm(x, w, b, eps, elementwise_affine=True):
     if x2.dtype != torch.float32:
         raise RuntimeError("layernorm expects an fp32 input (the module casts with x.float())")
     y = torch.empty_like(x2)
-    check(lib().tdb200_layer_norm_f32(ptr(x2), ptr(None if w is None else w.float()),
-                                      ptr(None if b is None else b.float()), ptr(y), x2.shape[0], x2.shape[1],
-                                      float(eps), stream_ptr(x.device)), "layernorm")
+    _ops.layer_norm_f32(x2, None if w is None else w.float(), None if b is None else b.float(), float(eps), y)
     return y.reshape(x.shape)
 
 
@@ -211,13 +209,10 @@ def fast_rmsnorm(x: torch.Tensor, w: torch.Tensor, eps: float) -> torch.Tensor:
     x2 = _rows16(x)
     if x2 is None:  # fp32 input: the reference entry point
         return rmsnorm(x.float().contiguous(), w, eps).to(x.dtype)
-    y = torch.empty_like(x2)
     if x2.numel() == 0:          # empty batch: nothing to launch (an empty tensor has no data pointer to hand to the C ABI)
-        return y.reshape(x.shape)
+        return torch.empty_like(x2).reshape(x.shape)
     w = _f32(w, x2.shape[1], "fast_rmsnorm weight")
-    check(lib().tdb200_rms_norm(ptr(x2), DTYPE_TAG[x.dtype], ptr(w), ptr(y), x2.shape[0], x2.shape[1],
-                                float(eps), stream_ptr(x.device)), "fast_rmsnorm")
-    return y.reshape(x.shape)
+    return _ops.rms_norm(x2, w, float(eps)).reshape(x.shape)
 
 
 def fast_layernorm(x, w, b, eps) -> torch.Tensor:
@@ -225,13 +220,10 @@ def fast_layernorm(x, w, b, eps) -> torch.Tensor:
     x2 = _rows16(x)
     if x2 is None:
         return layernorm(x.float().contiguous(), w, b, eps, w is not None).to(x.dtype)
-    y = torch.empty_like(x2)
     if x2.numel() == 0:
-        return y.reshape(x.shape)
+        return torch.empty_like(x2).reshape(x.shape)
     w, b = _f32(w, x2.shape[1], "fast_layernorm weight"), _f32(b, x2.shape[1], "fast_layernorm bias")
-    check(lib().tdb200_layer_norm(ptr(x2), DTYPE_TAG[x.dtype], ptr(w), ptr(b), ptr(y), x2.shape[0], x2.shape[1], float(eps),
-                                  stream_ptr(x.device)), "fast_layernorm")
-    return y.reshape(x.shape)
+    return _ops.layer_norm(x2, w, b, float(eps)).reshape(x.shape)
 
 
 def layernorm_modulate(x: torch.Tensor, scale: torch.Tensor, shift: torch.Tensor, eps: float) -> torch.Tensor:
@@ -239,10 +231,7 @@ def layernorm_modulate(x: torch.Tensor, scale: torch.Tensor, shift: torch.Tensor
     x2 = _rows16(x)
     assert x2 is not None, "layernorm_modulate expects a bf16/fp16 input"
     scale, shift = _f32(scale, x2.shape[1], "layernorm_modulate scale"), _f32(shift, x2.shape[1], "layernorm_modulate shift")
-    y = torch.empty_like(x2)
-    check(lib().tdb200_layer_norm_modulate(ptr(x2), DTYPE_TAG[x.dtype], ptr(scale), ptr(shift), ptr(y), x2.shape[0],
-                                           x2.shape[1], float(eps), stream_ptr(x.device)), "layernorm_modulate")
-    return y.reshape(x.shape)
+    return _ops.layer_norm_modulate(x2, scale, shift, float(eps)).reshape(x.shape)
 
 
 def layernorm_modulate_quant(x: torch.Tensor, scale: torch.Tensor, shift: torch.Tensor, eps: float):
@@ -251,33 +240,21 @@ def layernorm_modulate_quant(x: torch.Tensor, scale: torch.Tensor, shift: torch.
     assert x2 is not None
     m, n = x2.shape
     scale, shift = _f32(scale, n, "layernorm_modulate_quant scale"), _f32(shift, n, "layernorm_modulate_quant shift")
-    q = torch.empty((m, n), dtype=torch.int8, device=x.device)
-    s = torch.empty((cdiv(m, 128), cdiv(n, 128)), dtype=torch.float32, device=x.device)
-    stats = torch.empty((2 * m,), dtype=torch.float32, device=x.device)
-    check(lib().tdb200_layer_norm_modulate_quant(ptr(x2), DTYPE_TAG[x.dtype], ptr(scale), ptr(shift), ptr(q), ptr(s),
-                                                 ptr(stats), m, n, float(eps), stream_ptr(x.device)),
-          "layernorm_modulate_quant")
-    return q, s
+    return _ops.layer_norm_modulate_quant(x2, scale, shift, float(eps))
 
 
 def gate_residual(x: torch.Tensor, y: torch.Tensor, gate: torch.Tensor) -> torch.Tensor:
     """x + y * gate.type_as(x)  — rcm/networks/wan2pt1.py:405-406, gate fp32 [dim]."""
     x2, y2 = _rows16(x), _rows16(y)
     gate = _f32(gate, x2.shape[1], "gate_residual gate")
-    out = torch.empty_like(x2)
-    check(lib().tdb200_gate_residual(ptr(x2), ptr(y2), ptr(gate), ptr(out), DTYPE_TAG[x.dtype], x2.shape[0],
-                                     x2.shape[1], stream_ptr(x.device)), "gate_residual")
-    return out.reshape(x.shape)
+    return _ops.gate_residual(x2, y2, gate).reshape(x.shape)
 
 
 def gate_residual_stats(x: torch.Tensor, y: torch.Tensor, gate: Optional[torch.Tensor], eps: float):
     """(x + y * gate.type_as(x)  [gate None: x + y],  row statistics of that result for the next LayerNorm)."""
     x2, y2 = _rows16(x), _rows16(y)
     gate = _f32(gate, x2.shape[1], "gate_residual_stats gate")
-    out = torch.empty_like(x2)
-    stats = torch.empty((2 * x2.shape[0],), dtype=torch.float32, device=x.device)
-    check(lib().tdb200_gate_residual_stats(ptr(x2), ptr(y2), ptr(gate), ptr(out), ptr(stats), DTYPE_TAG[x.dtype],
-                                           x2.shape[0], x2.shape[1], float(eps), stream_ptr(x.device)), "gate_residual_stats")
+    out, stats = _ops.gate_residual_stats(x2, y2, gate, float(eps))
     return out.reshape(x.shape), stats
 
 
@@ -287,12 +264,7 @@ def layernorm_modulate_quant_from_stats(x: torch.Tensor, stats: torch.Tensor, sc
     m, n = x2.shape
     scale, shift = _f32(scale, n, "layernorm_modulate_quant_from_stats scale"), _f32(shift, n, "layernorm_modulate_quant_from_stats shift")
     stats = _f32(stats, 2 * m, "layernorm_modulate_quant_from_stats stats")
-    q = torch.empty((m, n), dtype=torch.int8, device=x.device)
-    s = torch.empty((cdiv(m, 128), cdiv(n, 128)), dtype=torch.float32, device=x.device)
-    check(lib().tdb200_layer_norm_modulate_quant_stats(ptr(x2), DTYPE_TAG[x.dtype], ptr(stats), ptr(scale), ptr(shift),
-                                                       ptr(q), ptr(s), m, n, stream_ptr(x.device)),
-          "layernorm_modulate_quant_from_stats")
-    return q, s
+    return _ops.layer_norm_modulate_quant_stats(x2, stats, scale, shift)
 
 
 def rope_interleaved(x: torch.Tensor, angles: torch.Tensor) -> torch.Tensor:
@@ -300,13 +272,10 @@ def rope_interleaved(x: torch.Tensor, angles: torch.Tensor) -> torch.Tensor:
     require_cuda(x, angles)
     l, h, d = x.shape[-3:]
     xc = x.contiguous()
-    y = torch.empty_like(xc)
     rows = xc.numel() // (h * d)
     assert rows == angles.shape[0], "one angle row per token row"
     angles = _f32(angles, rows * (d // 2), "rope_interleaved angles")
-    check(lib().tdb200_rope_interleaved(ptr(xc), DTYPE_TAG[x.dtype], ptr(angles), ptr(y), rows, h, d,
-                                        stream_ptr(x.device)), "rope_interleaved")
-    return y
+    return _ops.rope_interleaved(xc, angles)
 
 
 _ROPE_TABLES = {}   # id(angles) -> (weakref to the angle tensor, its _version, (cos, sin) table [L, D/2, 2] fp32)
@@ -315,17 +284,25 @@ ROPE_TABLE = os.environ.get("TDB200_ROPE_TABLE", "1") != "0"   # "0": evaluate s
 
 def rope_cos_sin(angles: torch.Tensor) -> torch.Tensor:
     """(cos, sin) of an angle tensor [L, D/2] as one fp32 table [L, D/2, 2], built once per tensor (and per in-place version of
-    it) and reused by every rmsnorm_rope call that is handed the same angles: all heads, q and k, every layer of a step."""
+    it) and reused by every rmsnorm_rope call that is handed the same angles: all heads, q and k, every layer of a step.
+    Under torch.compile the table is computed from the traced angles instead (the identity/version cache cannot be traced);
+    the compiler folds the identical computations of one graph into one."""
+    if torch.compiler.is_compiling():
+        return _cos_sin(angles)
     key = id(angles)
     hit = _ROPE_TABLES.get(key)
     if hit is not None and hit[0]() is angles and hit[1] == angles._version:
         return hit[2]
     if len(_ROPE_TABLES) >= 16:
         _ROPE_TABLES.clear()
-    a = angles.detach().float()
-    table = torch.stack((torch.cos(a), torch.sin(a)), dim=-1).contiguous()
+    table = _cos_sin(angles)
     _ROPE_TABLES[key] = (weakref.ref(angles), angles._version, table)
     return table
+
+
+def _cos_sin(angles: torch.Tensor) -> torch.Tensor:
+    a = angles.detach().float()
+    return torch.stack((torch.cos(a), torch.sin(a)), dim=-1).contiguous()
 
 
 def rmsnorm_rope(x: torch.Tensor, w: torch.Tensor, angles: torch.Tensor, eps: float, heads: int) -> torch.Tensor:
@@ -334,17 +311,12 @@ def rmsnorm_rope(x: torch.Tensor, w: torch.Tensor, angles: torch.Tensor, eps: fl
     xc = x.contiguous()
     l, hd = xc.shape
     w = _f32(w, hd, "rmsnorm_rope weight")
-    y = torch.empty_like(xc)
     if ROPE_TABLE:
         if angles.numel() != l * (hd // heads // 2):
             raise ValueError("rmsnorm_rope angles: expected [L, head_dim/2]")
-        check(lib().tdb200_rms_norm_rope_table(ptr(xc), DTYPE_TAG[x.dtype], ptr(w), ptr(rope_cos_sin(angles)), ptr(y), l, heads,
-                                               hd // heads, float(eps), stream_ptr(x.device)), "rmsnorm_rope")
-        return y
+        return _ops.rms_norm_rope_table(xc, w, rope_cos_sin(angles), float(eps), heads)
     angles = _f32(angles, l * (hd // heads // 2), "rmsnorm_rope angles")
-    check(lib().tdb200_rms_norm_rope(ptr(xc), DTYPE_TAG[x.dtype], ptr(w), ptr(angles), ptr(y), l, heads, hd // heads,
-                                     float(eps), stream_ptr(x.device)), "rmsnorm_rope")
-    return y
+    return _ops.rms_norm_rope(xc, w, angles, float(eps), heads)
 
 
 def wan_rope_angles(t: int, h: int, w: int, head_dim: int, device=None) -> torch.Tensor:

@@ -14,8 +14,8 @@ from typing import Optional, Tuple
 
 import torch
 
-from . import _lib
-from ._lib import DTYPE_TAG, check, lib, ptr, require_cuda, stream_ptr
+from . import _ops
+from ._lib import DTYPE_TAG, require_cuda
 
 
 def _cdiv(a, b):
@@ -31,15 +31,14 @@ def quant_cuda(x: torch.Tensor, out_q: Optional[torch.Tensor] = None,
         raise RuntimeError("Unsupported input data type for quant_cuda (bf16/fp16 only).")  # quant.cu:64-67
     if x.dim() != 2 or not x.is_contiguous():
         raise RuntimeError("quant_cuda expects a contiguous 2-D tensor")
+    if out_q is None and out_s is None:
+        return _ops.quant_int8_block128(x)
     m, k = x.shape
     if out_q is None:
         out_q = torch.empty((m, k), dtype=torch.int8, device=x.device)
     if out_s is None:
         out_s = torch.empty((_cdiv(m, 128), _cdiv(k, 128)), dtype=torch.float32, device=x.device)
-    if m == 0 or k == 0:         # empty batch: nothing to launch (an empty tensor has no data pointer to hand to the C ABI)
-        return out_q, out_s
-    check(lib().tdb200_quant_int8_block128(ptr(x), DTYPE_TAG[x.dtype], m, k, ptr(out_q), ptr(out_s),
-                                           stream_ptr(x.device)), "quant_cuda")
+    _ops.quant_int8_block128_out(x, out_q, out_s)
     return out_q, out_s
 
 
@@ -48,12 +47,7 @@ def gelu_quant_cuda(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     require_cuda(x)
     if x.dtype not in DTYPE_TAG or x.dim() != 2 or not x.is_contiguous():
         raise RuntimeError("gelu_quant_cuda expects a contiguous 2-D bf16/fp16 tensor")
-    m, k = x.shape
-    out_q = torch.empty((m, k), dtype=torch.int8, device=x.device)
-    out_s = torch.empty((_cdiv(m, 128), _cdiv(k, 128)), dtype=torch.float32, device=x.device)
-    check(lib().tdb200_gelu_quant_int8_block128(ptr(x), DTYPE_TAG[x.dtype], m, k, ptr(out_q), ptr(out_s),
-                                                stream_ptr(x.device)), "gelu_quant_cuda")
-    return out_q, out_s
+    return _ops.gelu_quant_int8_block128(x)
 
 
 GEMM_TIMER = None  # bench.py installs a callable(m, n, k) -> context manager to time GEMM launches with CUDA events
@@ -75,11 +69,7 @@ def _gemm_impl(a_q, a_s, b_q, b_s, c, bias, epilogue: int = 0):
             raise RuntimeError("gemm_cuda expects contiguous tensors")
     if bias is not None and bias.dtype != c.dtype:
         bias = bias.to(c.dtype)
-    m, n, k = a_q.size(0), b_q.size(0), b_q.size(1)  # gemm.cu:37-39
-    if m == 0 or n == 0:
-        return
-    check(lib().tdb200_gemm_w8a8_ex(ptr(a_q), ptr(a_s), ptr(b_q), ptr(b_s), ptr(bias), ptr(c), DTYPE_TAG[c.dtype], m,
-                                    n, k, epilogue, stream_ptr(c.device)), "gemm_cuda")
+    _ops.gemm_w8a8(a_q, a_s, b_q, b_s, bias, epilogue, c)   # M, N, K = a_q.size(0), b_q.size(0), b_q.size(1) (gemm.cu:37-39)
 
 
 def gemm_cuda(a_q, a_s, b_q, b_s, c) -> None:
@@ -106,29 +96,19 @@ def gemm_cuda_split(a_q, a_s, b_q, b_s, bias, out_dtype, parts: int):
     """One GEMM against `parts` row-concatenated projection weights (b_q [parts*n, k], b_s, bias); returns the outputs as a
     [parts, m, n] tensor of separate contiguous matrices (each bit-identical to its own gemm_cuda_swizzle_bias call)."""
     require_cuda(a_q, a_s, b_q, b_s, bias)
-    m, n, k = a_q.size(0), b_q.size(0), b_q.size(1)
-    c = torch.empty((parts, m, n // parts), dtype=out_dtype, device=a_q.device)
     if bias is not None and bias.dtype != out_dtype:
         bias = bias.to(out_dtype)
-    with (GEMM_TIMER(m, n, k) if GEMM_TIMER is not None else contextlib.nullcontext()):
-        check(lib().tdb200_gemm_w8a8_split(ptr(a_q), ptr(a_s), ptr(b_q), ptr(b_s), ptr(bias), ptr(c), DTYPE_TAG[out_dtype],
-                                           m, n, k, parts, stream_ptr(a_q.device)), "gemm_cuda_split")
-    return c
+    with (GEMM_TIMER(a_q.size(0), b_q.size(0), b_q.size(1)) if GEMM_TIMER is not None else contextlib.nullcontext()):
+        return _ops.gemm_w8a8_split(a_q, a_s, b_q, b_s, bias, out_dtype, parts)
 
 
 def gemm_cuda_quant_out(a_q, a_s, b_q, b_s, bias, mid_dtype, gelu: bool = False):
     """(q, s) = quant_cuda(act(gemm + bias)) in one kernel; the 16-bit activation never reaches HBM."""
     require_cuda(a_q, a_s, b_q, b_s, bias)
-    m, n, k = a_q.size(0), b_q.size(0), b_q.size(1)
-    q = torch.empty((m, n), dtype=torch.int8, device=a_q.device)
-    s = torch.empty((_cdiv(m, 128), _cdiv(n, 128)), dtype=torch.float32, device=a_q.device)
     if bias is not None and bias.dtype != mid_dtype:
         bias = bias.to(mid_dtype)
-    with (GEMM_TIMER(m, n, k) if GEMM_TIMER is not None else contextlib.nullcontext()):
-        check(lib().tdb200_gemm_w8a8_quant_out(ptr(a_q), ptr(a_s), ptr(b_q), ptr(b_s), ptr(bias), ptr(q), ptr(s),
-                                               DTYPE_TAG[mid_dtype], m, n, k, 1 if gelu else 0, stream_ptr(a_q.device)),
-              "gemm_cuda_quant_out")
-    return q, s
+    with (GEMM_TIMER(a_q.size(0), b_q.size(0), b_q.size(1)) if GEMM_TIMER is not None else contextlib.nullcontext()):
+        return _ops.gemm_w8a8_quant_out(a_q, a_s, b_q, b_s, bias, mid_dtype, bool(gelu))
 
 
 def rms_norm_cuda(x: torch.Tensor, eps: float, w: Optional[torch.Tensor] = None,
@@ -139,8 +119,7 @@ def rms_norm_cuda(x: torch.Tensor, eps: float, w: Optional[torch.Tensor] = None,
         raise RuntimeError("rms_norm_cuda expects a contiguous fp32 [M,N] tensor")
     if out is None:
         out = torch.empty_like(x)
-    check(lib().tdb200_rms_norm_f32(ptr(x), ptr(w), ptr(out), x.shape[0], x.shape[1], float(eps),
-                                    stream_ptr(x.device)), "rms_norm_cuda")
+    _ops.rms_norm_f32(x, w, float(eps), out)
     return out
 
 
@@ -152,6 +131,5 @@ def layer_norm_cuda(x: torch.Tensor, eps: float, w: Optional[torch.Tensor] = Non
         raise RuntimeError("layer_norm_cuda expects a contiguous fp32 [M,N] tensor")
     if out is None:
         out = torch.empty_like(x)
-    check(lib().tdb200_layer_norm_f32(ptr(x), ptr(w), ptr(b), ptr(out), x.shape[0], x.shape[1], float(eps),
-                                      stream_ptr(x.device)), "layer_norm_cuda")
+    _ops.layer_norm_f32(x, w, b, float(eps), out)
     return out

@@ -123,31 +123,3 @@ def test_launch_accounting_counts_every_abi_call():
     with pytest.raises(_lib.Tdb200Error, match=r"boom failed \(code -1\)"):
         _lib.check(-1, "boom")
 
-
-def test_attention_poly_exp2_experiment_coefficients():
-    """The build-time experiment TDB_ATTN_POLY_EXP2 (csrc/sla_attn.cu poly_exp2_x2) is emulated here with the coefficients
-    parsed from the source: magic-add rounding, cubic on [-0.5, 0.5], exponent patched in by a shift-add.  It must stay
-    within 1e-4 of exp2 over the whole range the kernel can feed it (clamp at -125, lazy-rescale bound +8)."""
-    import re
-    import numpy as np
-    src = open(os.path.join(ROOT, "turbodiffusion_b200", "csrc", "sla_attn.cu")).read()
-    if "poly_exp2_x2(float2 x)" not in src:
-        pytest.skip("the polynomial exp2 is not part of the current attention kernel")
-    body = src[src.index("poly_exp2_x2(float2 x)"):src.index("#endif", src.index("poly_exp2_x2(float2 x)"))]
-    hexes = re.findall(r"(0x1\.[0-9a-f]+p-?\d+)f", body)
-    c3, c2, c1, c0 = [np.float32(float.fromhex(h)) for h in (hexes[0], hexes[2], hexes[4], hexes[6])]
-    x = np.concatenate([np.linspace(-125, 8, 400001), [-1e9, -125.5, -0.5, 0.5, 0.0, 8.0]]).astype(np.float32)
-    x = np.maximum(x, np.float32(-125))
-    magic = np.float32(12582912.0)
-    r = (x + magic).astype(np.float32)
-    f = (x - (r - magic).astype(np.float32)).astype(np.float32)
-
-    def fma(a, b, c):
-        return (a.astype(np.float64) * b.astype(np.float64) + np.float64(c)).astype(np.float32)
-
-    p = fma(fma(fma(f, np.full_like(f, c3), c2), f, c1), f, c0)
-    bits = (p.view(np.int32).astype(np.int64) + ((r.view(np.int32).astype(np.int64) << 23) & 0xFFFFFFFF)) & 0xFFFFFFFF
-    out = bits.astype(np.uint32).view(np.float32)
-    assert np.isfinite(out).all() and (np.abs(f) <= 0.5).all()
-    rel = np.abs(out.astype(np.float64) / np.exp2(x.astype(np.float64)) - 1)
-    assert rel.max() < 1e-4, rel.max()

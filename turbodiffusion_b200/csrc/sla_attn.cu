@@ -1,12 +1,14 @@
-// a9 + a10. Fused SageSLA attention forward for one (128-row query block, head, batch) per CTA:
+// a9 + a10. Fused SageSLA attention forward for one (query block, head, batch) per CTA:
 //   block-sparse INT8 Q.K^T -> online softmax (exp2) -> 16-bit P.V, then the linear branch phi(Q).KVW / (eps + phi(Q).ksum)
 //   folded into the same accumulator, all in one wgmma kernel.
 //   reference: Sage call site turbodiffusion/SLA/core.py:231-235 (arithmetic in third-party SpargeAttn, unpinned);
 //   the in-tree statement of the same attention is the Triton kernel SLA/kernel.py:33-82 (tail masking :57-62, exp2 with
 //   qk_scale*log2e :60, row sum from unrounded P :71, P cast before P.V :73); linear branch + merge SLA/core.py:243-253.
 //
-// CTA = 2 consumer warpgroups + 1 TMA warp.  Warpgroup g owns query rows [64g, 64g+64) of the block; every thread holds two
-//   rows of the fragments (common.cuh): S[64 x 64] in 32 registers (wgmma m64n64, A = Q and B = K from shared memory),
+// Two kernels: sla_attn_fwd_kernel on 128-row query blocks (2 consumer warpgroups + 1 TMA warp; warpgroup g owns query rows
+//   [64g, 64g+64) of the block), and sla_attn_fwd_q64_kernel on 64-row query blocks (the entry-split CTA of sla_attn.cuh).
+//   Both run the same per-entry steps on a warpgroup's 64 rows, and every thread holds two rows of the fragments
+//   (common.cuh): S[64 x BK] in BK/2 registers (wgmma m64nBK, A = Q and B = K from shared memory),
 //   P converted in registers straight into the A fragments of P.V (wgmma m64nHD, A from registers, B = V MN-major from
 //   shared memory, so no transposed copy of V is ever materialised), and the O accumulator [64 x HD] in HD/2 registers.
 //   Row maxima / sums are reduced across the four lanes that share a row.
@@ -17,27 +19,29 @@
 // The O accumulator is only rescaled when a row maximum grows by more than 2^8 (lazy rescale): P stays <= 256, which
 // bf16/fp32 hold exactly as well as P <= 1, and the final O / l normalisation is unchanged.
 // Entry points: tdb200_sla_attn_fwd (INT8 Q/K, head dims 64 and 128, feature maps of the linear branch, K head-major or in
-// [b, lk, h, d], 128 x 64 blocks or 64 x 128 blocks in sla_attn_fwd_q64_kernel further down), tdb200_sla_attn16_fwd (16-bit
-// Q/K read from the module layout [b, l, h, d], fp32 scores; 128 x 64 blocks, or 64 x 64 in sla_attn_fwd_q64k64_kernel) and
-// tdb200_sla_attn16_fwd_lse (its sparse branch and row log-sum-exp, for the backward).
+// [b, lk, h, d], 128 x 64 blocks or 64 x 128 blocks), tdb200_sla_attn16_fwd (16-bit Q/K read from the module layout
+// [b, l, h, d], fp32 scores; 128 x 64 or 64 x 64 blocks) and tdb200_sla_attn16_fwd_lse (its sparse branch and row
+// log-sum-exp, for the backward).
 #include <type_traits>
 
-#include "common.cuh"
+#include "sla_attn.cuh"
 #include "host_common.h"
 
 namespace {
 using namespace tdb;
 
 constexpr int BLKQ = 128, BLKK = 64;
+constexpr int kBlkQ64 = 64, kHopperBlkK = 128;   // the 64-row query blocks; 128-row key blocks of the INT8 Hopper family
 constexpr int kConsumerWarps = 8;
 constexpr int kThreads = kConsumerWarps * 32 + 32;
 constexpr int kStages = 3;
+static_assert(kStages == split::kStages, "the 64-row kernel uses the entry-split rings");
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kRescaleThreshold = 8.0f;  // log2 domain
 
 template <int HD, bool kQK16, int kBQ = BLKQ, int kBK = BLKK>
 struct Lay {
-  static constexpr uint32_t kQBytes = kQK16 ? kBQ * HD * 2 : kBQ * HD;     // 16-bit: HD/64 chunks of [128 rows x 128 B]
+  static constexpr uint32_t kQBytes = kQK16 ? kBQ * HD * 2 : kBQ * HD;     // 16-bit: HD/64 chunks of [kBQ rows x 128 B]
   static constexpr uint32_t kKBytes = kQK16 ? kBK * HD * 2 : kBK * HD;
   static constexpr uint32_t kVBytes = kBK * HD * 2;                        // HD/64 boxes of [kBK keys x 128 B]
   static constexpr uint32_t kWBytes = HD * HD * 2;                         // HD/64 d_k chunks of [HD rows x 128 B]
@@ -48,6 +52,7 @@ struct Lay {
   static constexpr uint32_t kOffBars = kOffW + kWBytes;
   static constexpr uint32_t kOffLut = kOffBars + 256;
 };
+static_assert(split::kNumBars * 8 <= 256, "barriers exceed their shared-memory slot");
 
 struct AttnParams {
   const float* q_scale;   // [b,h,mblk]
@@ -77,6 +82,118 @@ __device__ __forceinline__ float quad_max(float v) {
 __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+// ---- The per-entry steps of every forward kernel, on one warpgroup's 64 query rows.  Each thread holds rows r and r + 8 of
+//      the tiles (fragment layout, common.cuh); cq is its column pair offset inside every 8-column slice.
+
+// S = Q.K^T over the BK keys of one ring slot, scaled by sc into the log2 domain.  INT8: scores are int32 dot products (sc
+// folds in q_scale * k_scale), Q and K rows of HD bytes with a 128-byte swizzle for 128-wide heads and a 64-byte one for
+// 64-wide heads.  16-bit: fp32 scores, Q and K in HD/64 chunks of 128-byte rows, q_chunk bytes apart for Q.
+template <bool kQK16, int HD, int BK, bool kBF16>
+__device__ __forceinline__ void score_tile(float (&s)[BK / 2], uint32_t sq, uint32_t q_chunk, uint32_t sk, float sc) {
+  if constexpr (kQK16) {
+#pragma unroll
+    for (int i = 0; i < BK / 2; ++i) s[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < HD / 16; ++ks) {  // K = 16 elements per MMA: chunk ks/4, +32 bytes per step inside the chunk
+      const uint64_t qd = make_desc_kmajor_sw128(sq + (ks >> 2) * q_chunk) + uint64_t((ks & 3) * 2);
+      const uint64_t kd = make_desc_kmajor_sw128(sk + (ks >> 2) * (BK * 128)) + uint64_t((ks & 3) * 2);
+      wgmma_f16_ss<BK, kBF16>(s, qd, kd, ks > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+#pragma unroll
+    for (int i = 0; i < BK / 2; ++i) s[i] *= sc;
+  } else {
+    uint32_t si[BK / 2];
+#pragma unroll
+    for (int i = 0; i < BK / 2; ++i) si[i] = 0u;
+    const uint64_t qdesc = HD == 128 ? make_desc_kmajor_sw128(sq) : make_desc_kmajor_sw64(sq);
+    const uint64_t kdesc = HD == 128 ? make_desc_kmajor_sw128(sk) : make_desc_kmajor_sw64(sk);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < HD / 32; ++ks)
+      wgmma_i8_ss<BK>(si, qdesc + uint64_t(ks * 2), kdesc + uint64_t(ks * 2), ks > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(si);
+#pragma unroll
+    for (int i = 0; i < BK / 2; ++i) s[i] = static_cast<float>(static_cast<int>(si[i])) * sc;
+  }
+}
+
+// One online-softmax step: key columns from `valid` on do not exist (the ragged last key block), then the row maxima and the
+// lazy rescale of O and the row sums (per row: alpha == 1 exactly where the maximum is kept), then P = exp2(s - m_used) into
+// the A fragments of P.V.  The row sum is taken from the unrounded P, the tensor core gets P rounded to T.  `first`: the first
+// entry of this warpgroup, which sets the maxima.
+template <typename T, int HD, int BK>
+__device__ __forceinline__ void softmax_step(float (&s)[BK / 2], float (&o)[HD / 2], float (&m_used)[2], float (&l_part)[2],
+                                             uint32_t (&pa)[BK / 16][4], int valid, int cq, bool first) {
+  if (valid < BK) {
+#pragma unroll
+    for (int i = 0; i < BK / 2; ++i)
+      if (8 * (i >> 2) + cq + (i & 1) >= valid) s[i] = -INFINITY;
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float mx = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < BK / 2; ++i)
+      if (((i >> 1) & 1) == h) mx = fmaxf(mx, s[i]);
+    mx = quad_max(mx);
+    if (first) {
+      m_used[h] = mx;
+    } else if (mx > m_used[h] + kRescaleThreshold) {
+      const float alpha = fast_exp2(m_used[h] - mx);
+#pragma unroll
+      for (int i = 0; i < HD / 2; ++i)
+        if (((i >> 1) & 1) == h) o[i] *= alpha;
+      l_part[h] *= alpha;
+      m_used[h] = mx;
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < BK / 2; i += 2) {
+    const int h = (i >> 1) & 1;
+    const float p0 = fast_exp2(s[i] - m_used[h]), p1 = fast_exp2(s[i + 1] - m_used[h]);
+    l_part[h] += p0 + p1;
+    pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0, p1);
+  }
+}
+
+// O += P.V  (V: [BK keys x HD], HD/64 MN-major chunks of BK x 128 B, so no transposed copy of V; +16 keys = +2048 B per K step)
+template <int HD, int BK, bool kBF16>
+__device__ __forceinline__ void pv_step(float (&o)[HD / 2], uint32_t (&pa)[BK / 16][4], uint32_t sv) {
+  const uint64_t vdesc = make_desc_mnmajor_sw128(sv, BK * 128);
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < BK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(o, pa[kk], vdesc + uint64_t(kk * 128));
+  wgmma_commit();
+  wgmma_wait<0>();
+  reg_fence(o);
+#pragma unroll
+  for (int kk = 0; kk < BK / 16; ++kk) reg_fence(pa[kk]);
+}
+
+// kLse epilogue: out = T(O / l) and lse[b,h,row] = m_used + log2(l), the row log-sum-exp of the scores in the kernel's log2
+// domain, for rows qrow0 + {0, 8}.
+template <typename T, int HD>
+__device__ __forceinline__ void store_o_lse(const float (&o)[HD / 2], const float (&m_used)[2], const float (&l_part)[2],
+                                            const AttnParams& p, int64_t qrow0, int cq, int b, int hh, int bh) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t qr = qrow0 + 8 * h;
+    if (qr >= p.l) continue;
+    const float l_tot = quad_sum(l_part[h]), inv_l = 1.0f / l_tot;
+    if (cq == 0) p.lse[int64_t(bh) * p.l + qr] = m_used[h] + __log2f(l_tot);
+    T* orow = static_cast<T*>(p.out) + ((int64_t(b) * p.l + qr) * p.h + hh) * HD;
+#pragma unroll
+    for (int c = 0; c < HD / 8; ++c)
+      *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) = F16Traits<T>::pack(o[4 * c + 2 * h] * inv_l, o[4 * c + 2 * h + 1] * inv_l);
+  }
 }
 
 // After the last key block, for the 64 query rows of one warpgroup (rows qrow0 + {0, 8} for this thread): the linear branch
@@ -166,8 +283,8 @@ __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const fl
   }
 }
 
-// kLse: the sparse branch alone for the training path (sla_attn_bwd.cu): out = T(O / l) and lse[b,h,row] = m_used + log2(l),
-// the row log-sum-exp of the scores in the kernel's log2 domain (scaled by sm_scale * log2e).  No KVW load, no linear branch.
+// 128-row query blocks.  CTA = 2 consumer warpgroups + 1 TMA warp; warpgroup g owns query rows [64g, 64g+64) of the block.
+// kLse: the sparse branch alone for the training path (sla_attn_bwd.cu): store_o_lse instead of the KVW load and the linear branch.
 template <typename T, int HD, bool kQK16, bool kLse = false>
 __global__ void __launch_bounds__(kThreads, 1)
 sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
@@ -256,7 +373,6 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   const int r_lo = wg * 64 + w4 * 16 + (lane >> 2);   // rows r_lo and r_lo + 8 of the block (fragment layout, common.cuh)
   const int cq = 2 * (lane & 3);                       // column pair offset inside every 8-column slice
   const uint32_t sbase = smem_u32(smem);
-  // INT8 path: scores are int32 dot products scaled by q_scale * k_scale; 16-bit path: fp32 scores.  Both in the log2 domain.
   const float qsc = (kQK16 ? 1.0f : __ldg(p.q_scale + int64_t(bh) * p.mblk + m_blk)) * p.sm_scale * kLog2e;
 
   float o[HD / 2];
@@ -272,407 +388,101 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     const float sc = qsc * s_ksc[j];
     const int valid = p.lk - blk * BLKK;                // < 64 only in the ragged last key block
 
-    // ---- S = Q.K^T for this warpgroup's 64 rows
-    float s[32];
+    float s[BLKK / 2];
     mbar_wait(&bars[kKFull + st], ph);
-    const uint32_t sk = sbase + L::kOffK + st * L::kKBytes;
-    if constexpr (kQK16) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) s[i] = 0.f;
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < HD / 16; ++ks) {  // K = 16 elements per MMA: chunk ks/4, +32 bytes per step inside the chunk
-        const uint64_t qd = make_desc_kmajor_sw128(sbase + L::kOffQ + (ks >> 2) * (BLKQ * 128) + wg * (64 * 128)) + uint64_t((ks & 3) * 2);
-        const uint64_t kd = make_desc_kmajor_sw128(sk + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
-        wgmma_f16_ss<64, kBF16>(s, qd, kd, ks > 0 ? 1u : 0u);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      reg_fence(s);
-#pragma unroll
-      for (int i = 0; i < 32; ++i) s[i] *= sc;
-    } else {
-      uint32_t si[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) si[i] = 0u;
-      // int8 rows are HD bytes: 128-byte swizzle for 128-wide heads, 64-byte swizzle for 64-wide heads
-      const uint32_t qa = sbase + L::kOffQ + wg * (64 * HD);
-      const uint64_t qdesc = HD == 128 ? make_desc_kmajor_sw128(qa) : make_desc_kmajor_sw64(qa);
-      const uint64_t kdesc = HD == 128 ? make_desc_kmajor_sw128(sk) : make_desc_kmajor_sw64(sk);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < HD / 32; ++ks)
-        wgmma_i8_ss<64>(si, qdesc + uint64_t(ks * 2), kdesc + uint64_t(ks * 2), ks > 0 ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<0>();
-      reg_fence(si);
-#pragma unroll
-      for (int i = 0; i < 32; ++i) s[i] = static_cast<float>(static_cast<int>(si[i])) * sc;
-    }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars[kKEmpty + st]);
-
-    // ---- ragged last key block: columns past lk do not exist
-    if (valid < BLKK) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (8 * (i >> 2) + cq + (i & 1) >= valid) s[i] = -INFINITY;
-    }
-    // ---- row maxima and the lazy rescale of the O accumulator (per row: alpha == 1 exactly where the maximum is kept)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float mx = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (((i >> 1) & 1) == h) mx = fmaxf(mx, s[i]);
-      mx = quad_max(mx);
-      if (j == 0) {
-        m_used[h] = mx;
-      } else if (mx > m_used[h] + kRescaleThreshold) {
-        const float alpha = fast_exp2(m_used[h] - mx);
-#pragma unroll
-        for (int i = 0; i < HD / 2; ++i)
-          if (((i >> 1) & 1) == h) o[i] *= alpha;
-        l_part[h] *= alpha;
-        m_used[h] = mx;
-      }
-    }
-    // ---- P = exp2(s - m_used); the row sum is taken from the unrounded P, the tensor core gets P rounded to T
+    score_tile<kQK16, HD, BLKK, kBF16>(s, sbase + L::kOffQ + wg * (64 * HD), BLKQ * 128, sbase + L::kOffK + st * L::kKBytes, sc);
+    warp_release(&bars[kKEmpty + st], lane);
     uint32_t pa[BLKK / 16][4];
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const int h = (i >> 1) & 1;
-      const float p0 = fast_exp2(s[i] - m_used[h]), p1 = fast_exp2(s[i + 1] - m_used[h]);
-      l_part[h] += p0 + p1;
-      pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0, p1);
-    }
-
-    // ---- O += P.V  (V: [64 keys x HD] rows, MN-major operand; +16 keys = +2048 B per K step)
+    softmax_step<T, HD, BLKK>(s, o, m_used, l_part, pa, valid, cq, j == 0);
     mbar_wait(&bars[kVFull + st], ph);
-    const uint64_t vdesc = make_desc_mnmajor_sw128(sbase + L::kOffV + st * L::kVBytes, BLKK * 128);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < BLKK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(o, pa[kk], vdesc + uint64_t(kk * 128));
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(o);
-#pragma unroll
-    for (int kk = 0; kk < BLKK / 16; ++kk) reg_fence(pa[kk]);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars[kVEmpty + st]);
+    pv_step<HD, BLKK, kBF16>(o, pa, sbase + L::kOffV + st * L::kVBytes);
+    warp_release(&bars[kVEmpty + st], lane);
   }
   if constexpr (kLse) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int64_t qr = int64_t(m_blk) * BLKQ + r_lo + 8 * h;
-      if (qr >= p.l) continue;
-      const float l_tot = quad_sum(l_part[h]), inv_l = 1.0f / l_tot;
-      if ((lane & 3) == 0) p.lse[int64_t(bh) * p.l + qr] = m_used[h] + __log2f(l_tot);
-      T* orow = static_cast<T*>(p.out) + ((int64_t(b) * p.l + qr) * p.h + hh) * HD;
-#pragma unroll
-      for (int c = 0; c < HD / 8; ++c)
-        *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) = F16Traits<T>::pack(o[4 * c + 2 * h] * inv_l, o[4 * c + 2 * h + 1] * inv_l);
-    }
+    store_o_lse<T, HD>(o, m_used, l_part, p, int64_t(m_blk) * BLKQ + r_lo, cq, b, hh, bh);
   } else {
     linear_branch_store<T, HD>(o, l_part, p, sbase + L::kOffW, int64_t(m_blk) * BLKQ + r_lo, cq, b, hh, bh);
   }
 }
 
-// SpargeAttn's Hopper block geometry (SLA/core.py:191-193, 226-229 on sm90): BLKQ = 64 query rows, BLKK = 128 key rows.
-// CTA = (64-row query block, head, batch); both consumer warpgroups work on the SAME 64 query rows and split the block's LUT
-// entries (warpgroup g takes entries j = g mod 2, the producer streams all of them through one ring), each running its own
-// online softmax on a 64 x 128 score tile (wgmma m64n128k32: 64 int32 / fp32 registers), so one warpgroup's softmax overlaps
-// the other's MMAs.  After both loops warpgroup 1 hands its (m, l, O) to warpgroup 0 through the drained K/V ring; warpgroup 0
-// merges the two states and runs the linear branch and the output once (linear_branch_store).
-// The producer is a whole warpgroup (one warp issues the TMA loads) so that setmaxnreg can move registers to the consumers:
-// O (64) + S (64) + P (32) fp32 registers per thread do not fit in the 168 a 384-thread CTA starts with.
-constexpr int kHopperBlkQ = 64, kHopperBlkK = 128;
-constexpr int kThreadsQ64 = 3 * 128;
-constexpr uint32_t kProducerRegsQ64 = 40, kConsumerRegsQ64 = 232;   // 128 * 40 + 256 * 232 <= 65536
-
-// Ring slot st serves entries st, st+3, st+6, ..., which alternate between the two warpgroups.  One full barrier per slot would
-// let a warpgroup skip a phase (the other warpgroup's entry), and try_wait.parity cannot tell phase n from phase n-2, so the
-// wait could pass while the skipped entry's load is still landing.  Each slot therefore has one full barrier per warpgroup:
-// entry j completes phase j / 6 of barrier (j % 3, j % 2), and warpgroup j % 2 consumes that barrier's phases in order.  The
-// empty barriers stay per slot: the producer waits on every phase in order, and the four warps of the entry's warpgroup
-// arrive only after its load, i.e. after the previous phase completed.
-enum BarQ64 { kQ64QFull = 0, kQ64KFull = 1 /*3 x 2*/, kQ64KEmpty = 7 /*3*/, kQ64VFull = 10 /*3 x 2*/, kQ64VEmpty = 16 /*3*/ };
-__device__ __forceinline__ int q64_full(int base, int j) { return base + 2 * (j % kStages) + (j & 1); }
-
-template <typename T, int HD>
-__global__ void __launch_bounds__(kThreadsQ64, 1)
+// 64-row query blocks, on the entry-split schedule (sla_attn.cuh): both consumer warpgroups work on the same 64 query rows and
+// take alternate LUT entries, each running its own online softmax, so one warpgroup's softmax overlaps the other's MMAs.  The
+// producer is a whole warpgroup so that setmaxnreg can move registers to the consumers: at BK = 128, O (64) + S (64) + P (32)
+// fp32 registers per thread do not fit in the 168 a 384-thread CTA starts with.  Two block families:
+//   INT8 Q/K, BK = 128: SpargeAttn's Hopper block geometry (SLA/core.py:191-193, 226-229 on sm90); wgmma m64n128k32.
+//   16-bit Q/K, BK = 64: SparseLinearAttention's default geometry (the reference's BLOCK_M = 64, BLOCK_N = 64 configuration
+//   of SLA/kernel.py:21-82); wgmma m64n64k16 into fp32.
+// After both loops warpgroup 1 hands its (m, l, O) to warpgroup 0, which merges the two states and then runs the linear
+// branch and the output (linear_branch_store), or with kLse stores o_s and the row lse.
+template <typename T, int HD, bool kQK16, int BK, bool kLse>
+__global__ void __launch_bounds__(split::kThreads, 1)
 sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                         const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw, AttnParams p) {
-  constexpr int BQ = kHopperBlkQ, BK = kHopperBlkK;
-  using L = Lay<HD, false, BQ, BK>;
-  // exchange of warpgroup 1's state: HD/2 accumulator registers + m_used[2] + l_part[2] per thread, over the K and V rings
+  constexpr int BQ = kBlkQ64;
+  using L = Lay<HD, kQK16, BQ, BK>;
+  // hand-off of warpgroup 1's state: HD/2 accumulator registers + m_used[2] + l_part[2] per thread, over the K and V rings
   static_assert((HD / 2 + 4) * 128 * 4 <= kStages * (L::kKBytes + L::kVBytes), "merge buffer does not fit in the ring");
   constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kOffBars);
   uint16_t* s_lut = reinterpret_cast<uint16_t*>(smem + L::kOffLut);
-  float* s_ksc = reinterpret_cast<float*>(smem + L::kOffLut + ((p.topk * 2 + 15) & ~15));
+  float* s_ksc = reinterpret_cast<float*>(smem + L::kOffLut + ((p.topk * 2 + 15) & ~15));  // INT8 only
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
   const int bh = b * p.h + hh;
   const int T_blocks = p.topk;
 
-  static_assert((kQ64VEmpty + kStages) * 8 <= 256, "barriers exceed their shared-memory slot");
-  if (threadIdx.x == 0) {
-    mbar_init(&bars[kQ64QFull], 1);
-    for (int i = 0; i < kStages; ++i) {  // each use of a ring slot is consumed by the four warps of one warpgroup
-      for (int g = 0; g < 2; ++g) {
-        mbar_init(&bars[kQ64KFull + 2 * i + g], 1);
-        mbar_init(&bars[kQ64VFull + 2 * i + g], 1);
-      }
-      mbar_init(&bars[kQ64KEmpty + i], 4);
-      mbar_init(&bars[kQ64VEmpty + i], 4);
-    }
-    mbar_fence_init();
-  }
+  if (threadIdx.x == 0) split::init_barriers(bars);
   {
     const int32_t* lut_row = p.lut + (int64_t(bh) * p.mblk + m_blk) * p.topk;
     const float* ksc_row = p.k_scale + int64_t(bh) * p.nblk;
-    for (int i = threadIdx.x; i < T_blocks; i += kThreadsQ64) {
+    for (int i = threadIdx.x; i < T_blocks; i += split::kThreads) {
       const int blk = __ldg(lut_row + i);
       s_lut[i] = static_cast<uint16_t>(blk);
-      s_ksc[i] = __ldg(ksc_row + blk);
+      if constexpr (!kQK16) s_ksc[i] = __ldg(ksc_row + blk);
     }
   }
   __syncthreads();
 
   if (warp >= kConsumerWarps) {
     // =============================================================== TMA producer
-    reg_dealloc<kProducerRegsQ64>();
-    if (warp == kConsumerWarps && lane == 0) {
-      tma_prefetch_desc(&tmap_q);
-      tma_prefetch_desc(&tmap_k);
-      tma_prefetch_desc(&tmap_v);
-      tma_prefetch_desc(&tmap_kvw);
-      mbar_expect_tx(&bars[kQ64QFull], L::kQBytes + L::kWBytes);
-      tma_load_4d(smem + L::kOffQ, &tmap_q, &bars[kQ64QFull], 0, m_blk * BQ, bh, 0);
-#pragma unroll
-      for (int c = 0; c < HD / 64; ++c)
-        tma_load_4d(smem + L::kOffW + c * (HD * 128), &tmap_kvw, &bars[kQ64QFull], c * 64, 0, bh, 0);
-      for (int j = 0; j < T_blocks; ++j) {
-        const int st = j % kStages;
-        const uint32_t ph = ((j / kStages) & 1) ^ 1;
-        const int blk = s_lut[j];
-        uint64_t* kfull = &bars[q64_full(kQ64KFull, j)];
-        uint64_t* vfull = &bars[q64_full(kQ64VFull, j)];
-        mbar_wait(&bars[kQ64KEmpty + st], ph);
-        mbar_expect_tx(kfull, L::kKBytes);
-        tma_load_4d(smem + L::kOffK + st * L::kKBytes, &tmap_k, kfull, 0, blk * BK, hh, b);
-        mbar_wait(&bars[kQ64VEmpty + st], ph);
-        mbar_expect_tx(vfull, L::kVBytes);
-        uint8_t* sv = smem + L::kOffV + st * L::kVBytes;
-#pragma unroll
-        for (int c = 0; c < HD / 64; ++c)
-          tma_load_4d(sv + c * (BK * 128), &tmap_v, vfull, c * 64, hh, blk * BK, b);
-      }
-    }
-    return;
-  }
-
-  // =============================================================== consumer warpgroups (same 64 rows, alternate LUT entries)
-  reg_alloc<kConsumerRegsQ64>();
-  const int wg = warp >> 2, w4 = warp & 3;
-  const int r_lo = w4 * 16 + (lane >> 2);
-  const int cq = 2 * (lane & 3);
-  const uint32_t sbase = smem_u32(smem);
-  const float qsc = __ldg(p.q_scale + int64_t(bh) * p.mblk + m_blk) * p.sm_scale * kLog2e;
-  const uint64_t qdesc = HD == 128 ? make_desc_kmajor_sw128(sbase + L::kOffQ) : make_desc_kmajor_sw64(sbase + L::kOffQ);
-
-  float o[HD / 2];
-#pragma unroll
-  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
-  float m_used[2] = {-INFINITY, -INFINITY}, l_part[2] = {0.f, 0.f};  // a warpgroup without entries keeps m = -inf, l = 0
-
-  mbar_wait(&bars[kQ64QFull], 0);
-  for (int j = wg; j < T_blocks; j += 2) {
-    const int st = j % kStages;
-    const uint32_t ph = (j / (2 * kStages)) & 1;        // phase j / 6 of this warpgroup's full barriers of slot st
-    const int blk = s_lut[j];
-    const float sc = qsc * s_ksc[j];
-    const int valid = p.lk - blk * BK;                  // < 128 only in the ragged last key block
-
-    // ---- S = Q.K^T over this entry's 128 keys
-    float s[64];
-    {
-      uint32_t si[64];
-#pragma unroll
-      for (int i = 0; i < 64; ++i) si[i] = 0u;
-      mbar_wait(&bars[q64_full(kQ64KFull, j)], ph);
-      const uint32_t sk = sbase + L::kOffK + st * L::kKBytes;
-      const uint64_t kdesc = HD == 128 ? make_desc_kmajor_sw128(sk) : make_desc_kmajor_sw64(sk);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < HD / 32; ++ks)
-        wgmma_i8_ss<128>(si, qdesc + uint64_t(ks * 2), kdesc + uint64_t(ks * 2), ks > 0 ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<0>();
-      reg_fence(si);
-#pragma unroll
-      for (int i = 0; i < 64; ++i) s[i] = static_cast<float>(static_cast<int>(si[i])) * sc;
-    }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars[kQ64KEmpty + st]);
-
-    // ---- ragged last key block (fewer than 64 valid keys masks a whole half of the tile)
-    if (valid < BK) {
-#pragma unroll
-      for (int i = 0; i < 64; ++i)
-        if (8 * (i >> 2) + cq + (i & 1) >= valid) s[i] = -INFINITY;
-    }
-    // ---- row maxima and the lazy rescale, as in sla_attn_fwd_kernel
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float mx = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < 64; ++i)
-        if (((i >> 1) & 1) == h) mx = fmaxf(mx, s[i]);
-      mx = quad_max(mx);
-      if (j == wg) {
-        m_used[h] = mx;
-      } else if (mx > m_used[h] + kRescaleThreshold) {
-        const float alpha = fast_exp2(m_used[h] - mx);
-#pragma unroll
-        for (int i = 0; i < HD / 2; ++i)
-          if (((i >> 1) & 1) == h) o[i] *= alpha;
-        l_part[h] *= alpha;
-        m_used[h] = mx;
-      }
-    }
-    uint32_t pa[BK / 16][4];
-#pragma unroll
-    for (int i = 0; i < 64; i += 2) {
-      const int h = (i >> 1) & 1;
-      const float p0 = fast_exp2(s[i] - m_used[h]), p1 = fast_exp2(s[i + 1] - m_used[h]);
-      l_part[h] += p0 + p1;
-      pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0, p1);
-    }
-
-    // ---- O += P.V  (V: [128 keys x HD], HD/64 MN-major chunks of 128 x 128 B; +16 keys = +2048 B per K step)
-    mbar_wait(&bars[q64_full(kQ64VFull, j)], ph);
-    const uint64_t vdesc = make_desc_mnmajor_sw128(sbase + L::kOffV + st * L::kVBytes, BK * 128);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < BK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(o, pa[kk], vdesc + uint64_t(kk * 128));
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(o);
-#pragma unroll
-    for (int kk = 0; kk < BK / 16; ++kk) reg_fence(pa[kk]);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars[kQ64VEmpty + st]);
-  }
-
-  // ---- merge: every ring slot has been consumed once both loops are done, so the ring holds warpgroup 1's state.  Thread t of
-  //      warpgroup 0 and thread t of warpgroup 1 own the same fragment positions; the buffer is [value][thread], conflict-free.
-  float* xchg = reinterpret_cast<float*>(smem + L::kOffK) + (threadIdx.x & 127);
-  named_bar_sync(1, 256);
-  if (wg == 1) {
-#pragma unroll
-    for (int i = 0; i < HD / 2; ++i) xchg[i * 128] = o[i];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      xchg[(HD / 2 + h) * 128] = m_used[h];
-      xchg[(HD / 2 + 2 + h) * 128] = l_part[h];
-    }
-  }
-  named_bar_sync(1, 256);
-  if (wg == 1) return;
-  float a0[2], a1[2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {  // warpgroup 0 always has entry 0, so its maximum is finite and exp2(-inf - m) = 0 drops an empty state
-    const float m1 = xchg[(HD / 2 + h) * 128], l1 = xchg[(HD / 2 + 2 + h) * 128];
-    const float mx = fmaxf(m_used[h], m1);
-    a0[h] = fast_exp2(m_used[h] - mx);
-    a1[h] = fast_exp2(m1 - mx);
-    l_part[h] = fmaf(l_part[h], a0[h], l1 * a1[h]);
-  }
-#pragma unroll
-  for (int i = 0; i < HD / 2; ++i) {
-    const int h = (i >> 1) & 1;
-    o[i] = fmaf(o[i], a0[h], xchg[i * 128] * a1[h]);
-  }
-  linear_branch_store<T, HD>(o, l_part, p, sbase + L::kOffW, int64_t(m_blk) * BQ + r_lo, cq, b, hh, bh);
-}
-
-// 16-bit Q.K^T on 64-row query blocks and 64-row key blocks: SparseLinearAttention's default geometry (the reference's
-// BLOCK_M = 64, BLOCK_N = 64 configuration of SLA/kernel.py:21-82).  The CTA of sla_attn_fwd_q64_kernel: a producer warpgroup
-// that gives its registers away, and two consumer warpgroups on the same 64 query rows taking alternate LUT entries, each with
-// its own online softmax on a 64 x 64 fp32 score tile (wgmma m64n64k16, Q and K K-major from shared memory; P rounded to T for
-// P.V as in sla_attn_fwd_kernel).  Warpgroup 1 hands its (m, l, O) to warpgroup 0 through the drained ring.  Without kLse
-// warpgroup 0 then runs the linear branch (every feature map) and the merge; with kLse it stores o_s and the row lse instead.
-constexpr int kSla16BlkQ = 64;
-template <typename T, bool kLse>
-__global__ void __launch_bounds__(kThreadsQ64, 1)
-sla_attn_fwd_q64k64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                           const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw, AttnParams p) {
-  constexpr int HD = 128, BQ = kSla16BlkQ, BK = BLKK;
-  using L = Lay<HD, true, BQ, BK>;
-  static_assert((HD / 2 + 4) * 128 * 4 <= kStages * (L::kKBytes + L::kVBytes), "merge buffer does not fit in the ring");
-  constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kOffBars);
-  uint16_t* s_lut = reinterpret_cast<uint16_t*>(smem + L::kOffLut);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
-  const int bh = b * p.h + hh;
-  const int T_blocks = p.topk;
-
-  if (threadIdx.x == 0) {
-    mbar_init(&bars[kQ64QFull], 1);
-    for (int i = 0; i < kStages; ++i) {
-      for (int g = 0; g < 2; ++g) {
-        mbar_init(&bars[kQ64KFull + 2 * i + g], 1);
-        mbar_init(&bars[kQ64VFull + 2 * i + g], 1);
-      }
-      mbar_init(&bars[kQ64KEmpty + i], 4);
-      mbar_init(&bars[kQ64VEmpty + i], 4);
-    }
-    mbar_fence_init();
-  }
-  {
-    const int32_t* lut_row = p.lut + (int64_t(bh) * p.mblk + m_blk) * p.topk;
-    for (int i = threadIdx.x; i < T_blocks; i += kThreadsQ64) s_lut[i] = static_cast<uint16_t>(__ldg(lut_row + i));
-  }
-  __syncthreads();
-
-  if (warp >= kConsumerWarps) {
-    // =============================================================== TMA producer
-    reg_dealloc<kProducerRegsQ64>();
+    reg_dealloc<split::kProducerRegs>();
     if (warp == kConsumerWarps && lane == 0) {
       tma_prefetch_desc(&tmap_q);
       tma_prefetch_desc(&tmap_k);
       tma_prefetch_desc(&tmap_v);
       if constexpr (!kLse) tma_prefetch_desc(&tmap_kvw);
-      mbar_expect_tx(&bars[kQ64QFull], L::kQBytes + (kLse ? 0 : L::kWBytes));
+      mbar_expect_tx(&bars[split::kQFull], L::kQBytes + (kLse ? 0 : L::kWBytes));
+      if constexpr (kQK16) {
 #pragma unroll
-      for (int c = 0; c < HD / 64; ++c)
-        tma_load_4d(smem + L::kOffQ + c * (BQ * 128), &tmap_q, &bars[kQ64QFull], c * 64, hh, m_blk * BQ, b);
+        for (int c = 0; c < HD / 64; ++c)
+          tma_load_4d(smem + L::kOffQ + c * (BQ * 128), &tmap_q, &bars[split::kQFull], c * 64, hh, m_blk * BQ, b);
+      } else {
+        tma_load_4d(smem + L::kOffQ, &tmap_q, &bars[split::kQFull], 0, m_blk * BQ, bh, 0);
+      }
       if constexpr (!kLse) {
 #pragma unroll
         for (int c = 0; c < HD / 64; ++c)
-          tma_load_4d(smem + L::kOffW + c * (HD * 128), &tmap_kvw, &bars[kQ64QFull], c * 64, 0, bh, 0);
+          tma_load_4d(smem + L::kOffW + c * (HD * 128), &tmap_kvw, &bars[split::kQFull], c * 64, 0, bh, 0);
       }
       for (int j = 0; j < T_blocks; ++j) {
         const int st = j % kStages;
         const uint32_t ph = ((j / kStages) & 1) ^ 1;
         const int blk = s_lut[j];
-        uint64_t* kfull = &bars[q64_full(kQ64KFull, j)];
-        uint64_t* vfull = &bars[q64_full(kQ64VFull, j)];
-        mbar_wait(&bars[kQ64KEmpty + st], ph);
+        uint64_t* kfull = &bars[split::full(split::kKFull, j)];
+        uint64_t* vfull = &bars[split::full(split::kVFull, j)];
+        mbar_wait(&bars[split::kKEmpty + st], ph);
         mbar_expect_tx(kfull, L::kKBytes);
         uint8_t* sk = smem + L::kOffK + st * L::kKBytes;
+        if constexpr (kQK16) {
 #pragma unroll
-        for (int c = 0; c < HD / 64; ++c) tma_load_4d(sk + c * (BK * 128), &tmap_k, kfull, c * 64, hh, blk * BK, b);
-        mbar_wait(&bars[kQ64VEmpty + st], ph);
+          for (int c = 0; c < HD / 64; ++c) tma_load_4d(sk + c * (BK * 128), &tmap_k, kfull, c * 64, hh, blk * BK, b);
+        } else {
+          tma_load_4d(sk, &tmap_k, kfull, 0, blk * BK, hh, b);
+        }
+        mbar_wait(&bars[split::kVEmpty + st], ph);
         mbar_expect_tx(vfull, L::kVBytes);
         uint8_t* sv = smem + L::kOffV + st * L::kVBytes;
 #pragma unroll
@@ -683,111 +493,51 @@ sla_attn_fwd_q64k64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __g
   }
 
   // =============================================================== consumer warpgroups (same 64 rows, alternate LUT entries)
-  reg_alloc<kConsumerRegsQ64>();
+  reg_alloc<split::kConsumerRegs>();
   const int wg = warp >> 2, w4 = warp & 3;
   const int r_lo = w4 * 16 + (lane >> 2);
   const int cq = 2 * (lane & 3);
   const uint32_t sbase = smem_u32(smem);
-  const float sc = p.sm_scale * kLog2e;
+  const float qsc = kQK16 ? p.sm_scale * kLog2e : __ldg(p.q_scale + int64_t(bh) * p.mblk + m_blk) * p.sm_scale * kLog2e;
 
   float o[HD / 2];
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
   float m_used[2] = {-INFINITY, -INFINITY}, l_part[2] = {0.f, 0.f};  // a warpgroup without entries keeps m = -inf, l = 0
 
-  mbar_wait(&bars[kQ64QFull], 0);
+  mbar_wait(&bars[split::kQFull], 0);
   for (int j = wg; j < T_blocks; j += 2) {
     const int st = j % kStages;
-    const uint32_t ph = (j / (2 * kStages)) & 1;        // phase j / 6 of this warpgroup's full barriers of slot st
-    const int valid = p.lk - s_lut[j] * BK;             // < 64 only in the ragged last key block
+    const uint32_t ph = split::full_phase(j);
+    const int blk = s_lut[j];
+    const float sc = kQK16 ? qsc : qsc * s_ksc[j];
+    const int valid = p.lk - blk * BK;                  // < BK only in the ragged last key block
 
-    // ---- S = Q.K^T over this entry's 64 keys
-    float s[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) s[i] = 0.f;
-    mbar_wait(&bars[q64_full(kQ64KFull, j)], ph);
-    const uint32_t sk = sbase + L::kOffK + st * L::kKBytes;
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < HD / 16; ++ks) {
-      const uint64_t qd = make_desc_kmajor_sw128(sbase + L::kOffQ + (ks >> 2) * (BQ * 128)) + uint64_t((ks & 3) * 2);
-      const uint64_t kd = make_desc_kmajor_sw128(sk + (ks >> 2) * (BK * 128)) + uint64_t((ks & 3) * 2);
-      wgmma_f16_ss<64, kBF16>(s, qd, kd, ks > 0 ? 1u : 0u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(s);
-#pragma unroll
-    for (int i = 0; i < 32; ++i) s[i] *= sc;
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars[kQ64KEmpty + st]);
-
-    if (valid < BK) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (8 * (i >> 2) + cq + (i & 1) >= valid) s[i] = -INFINITY;
-    }
-    // ---- row maxima and the lazy rescale, as in sla_attn_fwd_kernel
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float mx = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (((i >> 1) & 1) == h) mx = fmaxf(mx, s[i]);
-      mx = quad_max(mx);
-      if (j == wg) {
-        m_used[h] = mx;
-      } else if (mx > m_used[h] + kRescaleThreshold) {
-        const float alpha = fast_exp2(m_used[h] - mx);
-#pragma unroll
-        for (int i = 0; i < HD / 2; ++i)
-          if (((i >> 1) & 1) == h) o[i] *= alpha;
-        l_part[h] *= alpha;
-        m_used[h] = mx;
-      }
-    }
+    float s[BK / 2];
+    mbar_wait(&bars[split::full(split::kKFull, j)], ph);
+    score_tile<kQK16, HD, BK, kBF16>(s, sbase + L::kOffQ, BQ * 128, sbase + L::kOffK + st * L::kKBytes, sc);
+    warp_release(&bars[split::kKEmpty + st], lane);
     uint32_t pa[BK / 16][4];
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const int h = (i >> 1) & 1;
-      const float p0 = fast_exp2(s[i] - m_used[h]), p1 = fast_exp2(s[i + 1] - m_used[h]);
-      l_part[h] += p0 + p1;
-      pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0, p1);
-    }
-
-    // ---- O += P.V  (V: [64 keys x HD], MN-major; +16 keys = +2048 B per K step)
-    mbar_wait(&bars[q64_full(kQ64VFull, j)], ph);
-    const uint64_t vdesc = make_desc_mnmajor_sw128(sbase + L::kOffV + st * L::kVBytes, BK * 128);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < BK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(o, pa[kk], vdesc + uint64_t(kk * 128));
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(o);
-#pragma unroll
-    for (int kk = 0; kk < BK / 16; ++kk) reg_fence(pa[kk]);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars[kQ64VEmpty + st]);
+    softmax_step<T, HD, BK>(s, o, m_used, l_part, pa, valid, cq, j == wg);
+    mbar_wait(&bars[split::full(split::kVFull, j)], ph);
+    pv_step<HD, BK, kBF16>(o, pa, sbase + L::kOffV + st * L::kVBytes);
+    warp_release(&bars[split::kVEmpty + st], lane);
   }
 
-  // ---- merge, as in sla_attn_fwd_q64_kernel: warpgroup 1's state through the drained ring, [value][thread]
-  float* xchg = reinterpret_cast<float*>(smem + L::kOffK) + (threadIdx.x & 127);
-  named_bar_sync(1, 256);
-  if (wg == 1) {
+  const Handoff x = handoff_wg1_to_wg0(smem + L::kOffK, wg, 1, [&](const Handoff& x) {
 #pragma unroll
-    for (int i = 0; i < HD / 2; ++i) xchg[i * 128] = o[i];
+    for (int i = 0; i < HD / 2; ++i) x[i] = o[i];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      xchg[(HD / 2 + h) * 128] = m_used[h];
-      xchg[(HD / 2 + 2 + h) * 128] = l_part[h];
+      x[HD / 2 + h] = m_used[h];
+      x[HD / 2 + 2 + h] = l_part[h];
     }
-  }
-  named_bar_sync(1, 256);
+  });
   if (wg == 1) return;
   float a0[2], a1[2];
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {  // warpgroup 0 always has entry 0, so its maximum is finite and an empty state drops out
-    const float m1 = xchg[(HD / 2 + h) * 128], l1 = xchg[(HD / 2 + 2 + h) * 128];
+  for (int h = 0; h < 2; ++h) {  // warpgroup 0 always has entry 0, so its maximum is finite and exp2(-inf - m) = 0 drops an empty state
+    const float m1 = x[HD / 2 + h], l1 = x[HD / 2 + 2 + h];
     const float mx = fmaxf(m_used[h], m1);
     a0[h] = fast_exp2(m_used[h] - mx);
     a1[h] = fast_exp2(m1 - mx);
@@ -797,36 +547,25 @@ sla_attn_fwd_q64k64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __g
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) {
     const int h = (i >> 1) & 1;
-    o[i] = fmaf(o[i], a0[h], xchg[i * 128] * a1[h]);
+    o[i] = fmaf(o[i], a0[h], x[i] * a1[h]);
   }
   const int64_t qrow0 = int64_t(m_blk) * BQ + r_lo;
   if constexpr (kLse) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int64_t qr = qrow0 + 8 * h;
-      if (qr >= p.l) continue;
-      const float l_tot = quad_sum(l_part[h]), inv_l = 1.0f / l_tot;
-      if ((lane & 3) == 0) p.lse[int64_t(bh) * p.l + qr] = m_used[h] + __log2f(l_tot);
-      T* orow = static_cast<T*>(p.out) + ((int64_t(b) * p.l + qr) * p.h + hh) * HD;
-#pragma unroll
-      for (int c = 0; c < HD / 8; ++c)
-        *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) = F16Traits<T>::pack(o[4 * c + 2 * h] * inv_l, o[4 * c + 2 * h + 1] * inv_l);
-    }
+    store_o_lse<T, HD>(o, m_used, l_part, p, qrow0, cq, b, hh, bh);
   } else {
     linear_branch_store<T, HD>(o, l_part, p, sbase + L::kOffW, qrow0, cq, b, hh, bh);
   }
 }
 
-template <typename T, int HD, bool kQK16, int kBQ, bool kLse>
+template <typename T, int HD, bool kQK16, int kBQ, int kBK, bool kLse>
 constexpr auto attn_kernel() {
-  if constexpr (kQK16 && kBQ == kSla16BlkQ) return sla_attn_fwd_q64k64_kernel<T, kLse>;
-  else if constexpr (kBQ == kHopperBlkQ) return sla_attn_fwd_q64_kernel<T, HD>;
+  if constexpr (kBQ == kBlkQ64) return sla_attn_fwd_q64_kernel<T, HD, kQK16, kBK, kLse>;
   else return sla_attn_fwd_kernel<T, HD, kQK16, kLse>;
 }
 
 // kQK16: 16-bit Q and K in [b, l, h, d]; otherwise INT8 Q [b*h, l, d] and INT8 K [b, h, lk, d] (or [b, lk, h, d] when k_seq_major).
-// kBQ x kBK: the block geometry, 128 x 64 (sla_attn_fwd_kernel), 64 x 128 (sla_attn_fwd_q64_kernel, INT8 Q/K only) or
-// 64 x 64 (sla_attn_fwd_q64k64_kernel, 16-bit Q/K only).
+// kBQ x kBK: the block geometry, 128 x 64 (sla_attn_fwd_kernel), or with sla_attn_fwd_q64_kernel 64 x 128 (INT8 Q/K only)
+// or 64 x 64 (16-bit Q/K only).
 // kLse (16-bit only): sparse branch and row log-sum-exp into `lse`; kvw, ksum and proj_b are not read.
 template <int HD, bool kQK16, int kBQ = BLKQ, int kBK = BLKK, bool kLse = false>
 int launch(const void* q_op, const float* q_scale, const void* k_op, const float* k_scale, const void* v, const void* q, int dtype,
@@ -902,11 +641,11 @@ int launch(const void* q_op, const float* q_scale, const void* k_op, const float
   p.sm_scale = sm_scale;
   p.lse = lse;
   dim3 grid(static_cast<unsigned>(mblk), static_cast<unsigned>(h), static_cast<unsigned>(b));
-  const int threads = kBQ == kHopperBlkQ ? kThreadsQ64 : kThreads;
+  const int threads = kBQ == kBlkQ64 ? split::kThreads : kThreads;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define TDB_ATTN(T)                                                                                                   \
   do {                                                                                                                \
-    const auto kern = attn_kernel<T, HD, kQK16, kBQ, kLse>();                                                               \
+    const auto kern = attn_kernel<T, HD, kQK16, kBQ, kBK, kLse>();                                                               \
     if (int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), \
                             "cudaFuncSetAttribute(sla_attn)"))                                                        \
       return rc;                                                                                                      \
@@ -936,7 +675,7 @@ extern "C" int tdb200_sla_attn_fwd(const int8_t* q_i8, const float* q_scale, con
                                    const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
                                    int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq,
                                    int64_t blkk, int k_seq_major, void* stream) {
-  const bool hopper = blkq == kHopperBlkQ && blkk == kHopperBlkK;
+  const bool hopper = blkq == kBlkQ64 && blkk == kHopperBlkK;
   if (!hopper && !(blkq == BLKQ && blkk == BLKK))
     return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 128)",
                 (long long)blkq, (long long)blkk);
@@ -959,16 +698,16 @@ extern "C" int tdb200_sla_attn_fwd(const int8_t* q_i8, const float* q_scale, con
   // the order of these instantiations is the order nvcc compiles the kernels in, which changes the code it emits for them
   if (d == 128) {
     if (!hopper) TDB_LAUNCH(128, BLKQ, BLKK);
-    TDB_LAUNCH(128, kHopperBlkQ, kHopperBlkK);
+    TDB_LAUNCH(128, kBlkQ64, kHopperBlkK);
   }
   if (!hopper) TDB_LAUNCH(64, BLKQ, BLKK);
-  TDB_LAUNCH(64, kHopperBlkQ, kHopperBlkK);
+  TDB_LAUNCH(64, kBlkQ64, kHopperBlkK);
 #undef TDB_LAUNCH
 }
 
 namespace {
 int check_blocks16(const char* what, int64_t blkq, int64_t blkk) {
-  if ((blkq == BLKQ || blkq == kSla16BlkQ) && blkk == BLKK) return 0;
+  if ((blkq == BLKQ || blkq == kBlkQ64) && blkk == BLKK) return 0;
   return fail(TDB200_ERR_UNSUPPORTED, "%s: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 64)", what, (long long)blkq,
               (long long)blkk);
 }
@@ -984,13 +723,13 @@ int launch16(bool with_lse, int64_t blkq, const void* q, const void* k, const vo
     if (!with_lse) TDB_LAUNCH16(BLKQ, false);
     TDB_LAUNCH16(BLKQ, true);
   }
-  if (!with_lse) TDB_LAUNCH16(kSla16BlkQ, false);
-  TDB_LAUNCH16(kSla16BlkQ, true);
+  if (!with_lse) TDB_LAUNCH16(kBlkQ64, false);
+  TDB_LAUNCH16(kBlkQ64, true);
 #undef TDB_LAUNCH16
 }
 }  // namespace
 
-// 16-bit Q/K read from the module layout: (blkq, blkk) = (128, 64) runs sla_attn_fwd_kernel, (64, 64) sla_attn_fwd_q64k64_kernel.
+// 16-bit Q/K read from the module layout: (blkq, blkk) = (128, 64) runs sla_attn_fwd_kernel, (64, 64) sla_attn_fwd_q64_kernel.
 extern "C" int tdb200_sla_attn16_fwd(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
                                      const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l,
                                      int64_t lk, int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq, int64_t blkk,

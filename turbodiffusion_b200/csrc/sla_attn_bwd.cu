@@ -1,6 +1,6 @@
 // Backward of the block-sparse 16-bit attention (the sparse branch of SparseLinearAttention; reference: the autograd function
 // `_attention`, SLA/kernel.py:240-319, whose backward runs _attn_bwd_preprocess / _attn_bwd_dq / _attn_bwd_dkdv, :85-237).
-// Block geometry of the forward: BLKQ = 128 (or 64: the _q64 kernels further down) query rows, BLKK = 64 key rows, 128-wide
+// Block geometry of the forward: BLKQ = 128 (or 64) query rows, BLKK = 64 key rows, 128-wide
 // heads, q/k/v/o/dO/dq/dk/dv in the module layout [b, l, h, d].  The forward (sla_attn.cu, kLse) leaves o_s = T(O / l) and
 // lse = m + log2(l) in the log2 domain, so that P = exp2(S * sm_scale * log2e - lse) is recomputed exactly as the forward
 // normalised it.
@@ -10,8 +10,10 @@
 //                                selected it (CSR offsets + entries), built on the device without a host synchronisation
 //   sla_bwd_dq_kernel         one CTA per (query block, head, batch): Q_i and dO_i resident, K_j / V_j streamed over the LUT row;
 //                             S = Q.K^T, dP = dO.V^T, dS = P o (dP - delta), dQ += dS.K  (K tile as the MN-major operand)
+//   sla_bwd_dq_q64_kernel     the same on 64-row query blocks, on the entry-split schedule of sla_attn.cuh
 //   sla_bwd_dkdv_kernel       one CTA per (key block, head, batch): K_j and V_j resident, (Q_i, dO_i) streamed over the key
-//                             block's list; S^T = K.Q^T, dP^T = V.dO^T, dV += P^T.dO, dK += dS^T.Q  (Q / dO tiles MN-major)
+//                             block's list; S^T = K.Q^T, dP^T = V.dO^T, dV += P^T.dO, dK += dS^T.Q  (Q / dO tiles MN-major);
+//                             one template for both query-block heights
 //
 // Rounding points (FlashAttention-2's): P and dS are formed in fp32 and rounded to T only as MMA operands; dQ, dK, dV accumulate
 // in fp32 registers and are rounded to T once.  No floating-point atomics: every output element is written by one thread in a
@@ -19,13 +21,13 @@
 // lse = +inf (P = 0) and delta = 0 explicitly, because TMA zero-fill gives their scores, not their statistics.
 #include <type_traits>
 
-#include "common.cuh"
+#include "sla_attn.cuh"
 #include "host_common.h"
 
 namespace {
 using namespace tdb;
 
-constexpr int HD = 128, BLKQ = 128, BLKK = 64;
+constexpr int HD = 128, BLKQ = 128, BLKQ64 = 64, BLKK = 64;
 constexpr float kLog2e = 1.4426950408889634f;
 
 struct BwdParams {
@@ -143,7 +145,7 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
   using namespace dq;
   constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // 1024-aligned, stays a shared-space pointer
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
   uint16_t* s_lut = reinterpret_cast<uint16_t*>(smem + kOffLut);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -276,32 +278,40 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
 }
 
 // ------------------------------------------------------------------------------------------------ dK / dV
-// CTA = a producer warpgroup (one warp issues TMA; setmaxnreg hands its registers to the consumers) + 2 consumer warpgroups.
-// Both consumers work on the same 64 key rows; warpgroup g takes query rows [64g, 64g + 64) of every streamed query block:
-// S^T and dP^T are 64 x 64 tiles (32 registers each), the partial dK and dV 64 x 128 (64 + 64).  The 128 lse / delta values
-// of a query block are staged in shared memory per warpgroup (double-buffered, one named barrier per step).  At the end
-// warpgroup 1 hands its partials to warpgroup 0 through the drained ring, which adds them (fixed order) and stores.
-namespace dkv {
-constexpr int kThreads = 3 * 128, kStages = 2;
-constexpr uint32_t kProducerRegs = 40, kConsumerRegs = 232;   // 128 * 40 + 256 * 232 <= 65536
-constexpr uint32_t kTileQ = BLKQ * HD * 2, kTileK = BLKK * HD * 2;
-constexpr uint32_t kOffK = 0, kOffV = kTileK, kOffQ = 2 * kTileK, kOffDO = kOffQ + kStages * kTileQ;
-constexpr uint32_t kOffStats = kOffDO + kStages * kTileQ;             // [warpgroup][buffer][lse 64 | delta 64] fp32
-constexpr uint32_t kOffBars = kOffStats + 2 * 2 * 128 * 4;
-constexpr uint32_t kSmem = kOffBars + 64;
-enum Bar { kKVFull = 0, kFull = 1 /*2*/, kEmpty = 3 /*2*/ };
-static_assert(HD * 128 * 4 <= 2 * kStages * kTileQ, "partial dK / dV do not fit in the ring");
-}  // namespace dkv
+// CTA = a producer warpgroup (one warp issues TMA; setmaxnreg hands its registers to the consumers) + 2 consumer warpgroups, both
+// on the same 64 key rows; K_j and V_j resident, (Q_i, dO_i) streamed over the key block's list.  Per streamed 64-row query slab
+// S^T and dP^T are 64 x 64 tiles (32 registers each); the partial dK and dV are 64 x 128 (64 + 64).  The lse / delta values of
+// a slab are staged in shared memory per warpgroup (double-buffered, one named barrier per step).  At the end warpgroup 1 hands
+// its partials to warpgroup 0, which adds them (fixed order) and stores.
+//   kBQ = 128: warpgroup g takes query rows [64g, 64g + 64) of every list entry through a 2-stage ring whose stages both
+//              warpgroups read.
+//   kBQ = 64:  each list entry is one 64-row query block, taken by warpgroup j % 2.  With four ring stages slot j % 4 is only
+//              ever used by warpgroup j % 2, so every slot's barriers are consumed by one warpgroup, in order, and each
+//              warpgroup has its next (Q_i, dO_i) pair in flight while it computes.
+template <int kBQ>
+struct Dkv {
+  static constexpr bool kSplit = kBQ == BLKQ64;
+  static constexpr int kStages = kSplit ? 4 : 2;
+  static constexpr uint32_t kTileQ = kBQ * HD * 2, kTileK = BLKK * HD * 2;
+  static constexpr uint32_t kOffK = 0, kOffV = kTileK, kOffQ = 2 * kTileK, kOffDO = kOffQ + kStages * kTileQ;
+  static constexpr uint32_t kOffStats = kOffDO + kStages * kTileQ;             // [warpgroup][buffer][lse 64 | delta 64] fp32
+  static constexpr uint32_t kOffBars = kOffStats + 2 * 2 * 128 * 4;
+  static constexpr uint32_t kSmem = kOffBars + (kSplit ? 128 : 64);
+  enum Bar { kKVFull = 0, kFull = 1 /*kStages*/, kEmpty = 1 + kStages /*kStages*/ };
+  static_assert((kEmpty + kStages) * 8 <= kSmem - kOffBars, "barriers exceed their shared-memory slot");
+  static_assert(HD * 128 * 4 <= 2 * kStages * kTileQ, "partial dK / dV do not fit in the ring");
+};
 
-template <typename T>
-__global__ void __launch_bounds__(dkv::kThreads, 1)
+template <typename T, int kBQ>
+__global__ void __launch_bounds__(split::kThreads, 1)
 sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
                     const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v, BwdParams p) {
-  using namespace dkv;
+  using L = Dkv<kBQ>;
+  constexpr int kStages = L::kStages;
   constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kOffBars);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
   const int bh = b * p.h + hh;
@@ -310,7 +320,7 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   const int n_list = __ldg(kv_off + n_blk + 1) - __ldg(kv_off + n_blk);
 
   if (n_list == 0) {  // no query block selected this key block: its gradients are zero (the outputs are not pre-zeroed)
-    for (int e = threadIdx.x; e < BLKK * HD / 8; e += kThreads) {
+    for (int e = threadIdx.x; e < BLKK * HD / 8; e += split::kThreads) {
       const int64_t r = int64_t(n_blk) * BLKK + e / (HD / 8);
       if (r >= p.l) break;
       const int64_t o = ((int64_t(b) * p.l + r) * p.h + hh) * HD + (e % (HD / 8)) * 8;
@@ -320,10 +330,10 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     return;
   }
   if (threadIdx.x == 0) {
-    mbar_init(&bars[kKVFull], 1);
+    mbar_init(&bars[L::kKVFull], 1);
     for (int i = 0; i < kStages; ++i) {
-      mbar_init(&bars[kFull + i], 1);
-      mbar_init(&bars[kEmpty + i], 8);   // both consumer warpgroups read every stage
+      mbar_init(&bars[L::kFull + i], 1);
+      mbar_init(&bars[L::kEmpty + i], L::kSplit ? 4 : 8);   // the four warps of warpgroup i % 2, or both warpgroups
     }
     mbar_fence_init();
   }
@@ -331,28 +341,28 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 
   if (warp >= 8) {
     // =============================================================== TMA producer
-    reg_dealloc<kProducerRegs>();
+    reg_dealloc<split::kProducerRegs>();
     if (warp == 8 && lane == 0) {
       tma_prefetch_desc(&tmap_q);
       tma_prefetch_desc(&tmap_do);
       tma_prefetch_desc(&tmap_k);
       tma_prefetch_desc(&tmap_v);
-      mbar_expect_tx(&bars[kKVFull], 2 * kTileK);
+      mbar_expect_tx(&bars[L::kKVFull], 2 * L::kTileK);
 #pragma unroll
       for (int c = 0; c < HD / 64; ++c) {
-        tma_load_4d(smem + kOffK + c * (BLKK * 128), &tmap_k, &bars[kKVFull], c * 64, hh, n_blk * BLKK, b);
-        tma_load_4d(smem + kOffV + c * (BLKK * 128), &tmap_v, &bars[kKVFull], c * 64, hh, n_blk * BLKK, b);
+        tma_load_4d(smem + L::kOffK + c * (BLKK * 128), &tmap_k, &bars[L::kKVFull], c * 64, hh, n_blk * BLKK, b);
+        tma_load_4d(smem + L::kOffV + c * (BLKK * 128), &tmap_v, &bars[L::kKVFull], c * 64, hh, n_blk * BLKK, b);
       }
       for (int j = 0; j < n_list; ++j) {
         const int st = j % kStages;
         const uint32_t ph = ((j / kStages) & 1) ^ 1;
         const int qb = __ldg(list + j);
-        mbar_wait(&bars[kEmpty + st], ph);
-        mbar_expect_tx(&bars[kFull + st], 2 * kTileQ);
+        mbar_wait(&bars[L::kEmpty + st], ph);
+        mbar_expect_tx(&bars[L::kFull + st], 2 * L::kTileQ);
 #pragma unroll
         for (int c = 0; c < HD / 64; ++c) {
-          tma_load_4d(smem + kOffQ + st * kTileQ + c * (BLKQ * 128), &tmap_q, &bars[kFull + st], c * 64, hh, qb * BLKQ, b);
-          tma_load_4d(smem + kOffDO + st * kTileQ + c * (BLKQ * 128), &tmap_do, &bars[kFull + st], c * 64, hh, qb * BLKQ, b);
+          tma_load_4d(smem + L::kOffQ + st * L::kTileQ + c * (kBQ * 128), &tmap_q, &bars[L::kFull + st], c * 64, hh, qb * kBQ, b);
+          tma_load_4d(smem + L::kOffDO + st * L::kTileQ + c * (kBQ * 128), &tmap_do, &bars[L::kFull + st], c * 64, hh, qb * kBQ, b);
         }
       }
     }
@@ -360,48 +370,49 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   }
 
   // =============================================================== consumer warpgroups
-  reg_alloc<kConsumerRegs>();
+  reg_alloc<split::kConsumerRegs>();
   const int wg = warp >> 2, w4 = warp & 3, t = threadIdx.x & 127;
   const int kr_lo = w4 * 16 + (lane >> 2);   // key rows kr_lo, kr_lo + 8 of the block
   const int cq = 2 * (lane & 3);
   const uint32_t sbase = smem_u32(smem);
   const float sc = p.sm_scale * kLog2e;
-  float* stats = reinterpret_cast<float*>(smem + kOffStats) + wg * 256;
+  const int q0 = L::kSplit ? 0 : wg * 64;    // this warpgroup's first row of a streamed query block
+  float* stats = reinterpret_cast<float*>(smem + L::kOffStats) + wg * 256;
   float dk[HD / 2], dv[HD / 2];
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) dk[i] = dv[i] = 0.f;
 
-  mbar_wait(&bars[kKVFull], 0);
-  for (int j = 0; j < n_list; ++j) {
+  mbar_wait(&bars[L::kKVFull], 0);
+  for (int j = L::kSplit ? wg : 0, it = 0; j < n_list; j += L::kSplit ? 2 : 1, ++it) {
     const int st = j % kStages;
     const uint32_t ph = (j / kStages) & 1;
     const int qb = __ldg(list + j);
     // ---- lse / delta of this warpgroup's 64 query rows; query rows >= l: P = 0 and delta = 0
-    float* sb = stats + (j & 1) * 128;
+    float* sb = stats + ((L::kSplit ? it : j) & 1) * 128;
     {
-      const int64_t r = int64_t(qb) * BLKQ + wg * 64 + (t & 63);
+      const int64_t r = int64_t(qb) * kBQ + q0 + (t & 63);
       const bool in = r < p.l;
       sb[t] = t < 64 ? (in ? __ldg(p.lse + int64_t(bh) * p.l + r) : INFINITY) : (in ? __ldg(p.delta + int64_t(bh) * p.l + r) : 0.f);
     }
     named_bar_sync(1 + wg, 128);
 
     // ---- S^T = K.Q^T and dP^T = V.dO^T over this warpgroup's 64 query rows (all operands K-major over d)
-    const uint32_t sq = sbase + kOffQ + st * kTileQ + wg * (64 * 128), sg = sbase + kOffDO + st * kTileQ + wg * (64 * 128);
+    const uint32_t sq = sbase + L::kOffQ + st * L::kTileQ + q0 * 128, sg = sbase + L::kOffDO + st * L::kTileQ + q0 * 128;
     float s[32], dp[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) s[i] = dp[i] = 0.f;
-    mbar_wait(&bars[kFull + st], ph);
+    mbar_wait(&bars[L::kFull + st], ph);
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < HD / 16; ++ks) {
-      const uint64_t kd = make_desc_kmajor_sw128(sbase + kOffK + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
-      const uint64_t qd = make_desc_kmajor_sw128(sq + (ks >> 2) * (BLKQ * 128)) + uint64_t((ks & 3) * 2);
+      const uint64_t kd = make_desc_kmajor_sw128(sbase + L::kOffK + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
+      const uint64_t qd = make_desc_kmajor_sw128(sq + (ks >> 2) * (kBQ * 128)) + uint64_t((ks & 3) * 2);
       wgmma_f16_ss<64, kBF16>(s, kd, qd, ks > 0 ? 1u : 0u);
     }
 #pragma unroll
     for (int ks = 0; ks < HD / 16; ++ks) {
-      const uint64_t vd = make_desc_kmajor_sw128(sbase + kOffV + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
-      const uint64_t gd = make_desc_kmajor_sw128(sg + (ks >> 2) * (BLKQ * 128)) + uint64_t((ks & 3) * 2);
+      const uint64_t vd = make_desc_kmajor_sw128(sbase + L::kOffV + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
+      const uint64_t gd = make_desc_kmajor_sw128(sg + (ks >> 2) * (kBQ * 128)) + uint64_t((ks & 3) * 2);
       wgmma_f16_ss<64, kBF16>(dp, vd, gd, ks > 0 ? 1u : 0u);
     }
     wgmma_commit();
@@ -421,7 +432,7 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     }
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) wgmma_f16_rs<HD, kBF16, 1>(dv, pa[kk], make_desc_mnmajor_sw128(sg, BLKQ * 128) + uint64_t(kk * 128));
+    for (int kk = 0; kk < 4; ++kk) wgmma_f16_rs<HD, kBF16, 1>(dv, pa[kk], make_desc_mnmajor_sw128(sg, kBQ * 128) + uint64_t(kk * 128));
     wgmma_commit();
     // ---- dS^T = P^T o (dP^T - delta) rounded to T; dK += dS^T.Q
 #pragma unroll
@@ -431,7 +442,7 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     }
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) wgmma_f16_rs<HD, kBF16, 1>(dk, da[kk], make_desc_mnmajor_sw128(sq, BLKQ * 128) + uint64_t(kk * 128));
+    for (int kk = 0; kk < 4; ++kk) wgmma_f16_rs<HD, kBF16, 1>(dk, da[kk], make_desc_mnmajor_sw128(sq, kBQ * 128) + uint64_t(kk * 128));
     wgmma_commit();
     wgmma_wait<0>();
     reg_fence(dv);
@@ -441,60 +452,47 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
       reg_fence(pa[kk]);
       reg_fence(da[kk]);
     }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars[kEmpty + st]);
+    warp_release(&bars[L::kEmpty + st], lane);
   }
 
-  // ---- warpgroup 1's partials -> warpgroup 0 through the ring (every stage has been consumed by both); [value][thread] layout
-  float* xchg = reinterpret_cast<float*>(smem + kOffQ) + t;
-  named_bar_sync(3, 256);
-  if (wg == 1) {
+  // ---- warpgroup 1's partials -> warpgroup 0 through the Q / dO ring, which both warpgroups have drained
+  const Handoff x = handoff_wg1_to_wg0(smem + L::kOffQ, wg, 3, [&](const Handoff& x) {
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) {
-      xchg[i * 128] = dk[i];
-      xchg[(HD / 2 + i) * 128] = dv[i];
+      x[i] = dk[i];
+      x[HD / 2 + i] = dv[i];
     }
-  }
-  named_bar_sync(3, 256);
+  });
   if (wg == 1) return;
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) {
-    dk[i] += xchg[i * 128];
-    dv[i] += xchg[(HD / 2 + i) * 128];
+    dk[i] += x[i];
+    dv[i] += x[HD / 2 + i];
   }
   const int64_t row0 = int64_t(n_blk) * BLKK + kr_lo;
   store_rows<T>(dk, p.sm_scale, p.dk, row0, p.l, p.h, hh, b, cq);
   store_rows<T>(dv, 1.0f, p.dv, row0, p.l, p.h, hh, b, cq);
 }
 
-// ------------------------------------------------------------------------------------------------ 64-row query blocks
-// The backward of sla_attn_fwd_q64k64_kernel (BLKQ = 64, BLKK = 64).  Both kernels run a producer warpgroup (setmaxnreg hands
-// its registers to the consumers) and two consumer warpgroups that take alternate entries of the streamed list, so a 64-row
-// query block is never split: each warpgroup keeps its own fp32 partial, and warpgroup 1 hands it to warpgroup 0 through the
-// drained ring, which adds the two in a fixed order and stores.
-constexpr int BLKQ64 = 64;
-constexpr int kThreads64 = 3 * 128;
-constexpr uint32_t kProducerRegs64 = 40, kConsumerRegs64 = 232;   // 128 * 40 + 256 * 232 <= 65536
-
-// dQ: one CTA per (64-row query block, head, batch); Q_i and dO_i resident, K_j / V_j streamed over the LUT row through a
-// 3-stage ring.  Ring slot st serves entries st, st+3, ..., which alternate between the warpgroups, so every slot has one
-// full barrier per warpgroup (entry j completes phase j / 6 of barrier (j % 3, j % 2); see sla_attn_fwd_q64_kernel).
+// ------------------------------------------------------------------------------------------------ dQ on 64-row query blocks
+// The backward of the 64 x 64 forward, on the entry-split schedule (sla_attn.cuh): one CTA per (64-row query block, head,
+// batch); Q_i and dO_i resident, K_j / V_j streamed over the LUT row, the two consumer warpgroups take alternate entries with
+// the per-entry arithmetic of sla_bwd_dq_kernel.  Each keeps its own fp32 partial, and warpgroup 0 adds warpgroup 1's in a
+// fixed order before storing.
 namespace dq64 {
-constexpr int kStages = 3;
 constexpr uint32_t kTileQ = BLKQ64 * HD * 2, kTileK = BLKK * HD * 2;   // 16 KB each
-constexpr uint32_t kOffQ = 0, kOffDO = kTileQ, kOffK = 2 * kTileQ, kOffV = kOffK + kStages * kTileK;
-constexpr uint32_t kOffBars = kOffV + kStages * kTileK, kOffLut = kOffBars + 256;
-enum Bar { kQFull = 0, kKFull = 1 /*3 x 2*/, kKEmpty = 7 /*3*/, kVFull = 10 /*3 x 2*/, kVEmpty = 16 /*3*/ };
-static_assert((kVEmpty + kStages) * 8 <= 256, "barriers exceed their shared-memory slot");
-static_assert(HD / 2 * 128 * 4 <= kStages * kTileK, "partial dQ does not fit in the K ring");
-__device__ __forceinline__ int full(int base, int j) { return base + 2 * (j % kStages) + (j & 1); }
+constexpr uint32_t kOffQ = 0, kOffDO = kTileQ, kOffK = 2 * kTileQ, kOffV = kOffK + split::kStages * kTileK;
+constexpr uint32_t kOffBars = kOffV + split::kStages * kTileK, kOffLut = kOffBars + 256;
+static_assert(split::kNumBars * 8 <= 256, "barriers exceed their shared-memory slot");
+static_assert(HD / 2 * 128 * 4 <= split::kStages * kTileK, "partial dQ does not fit in the K ring");
 }  // namespace dq64
 
 template <typename T>
-__global__ void __launch_bounds__(kThreads64, 1)
+__global__ void __launch_bounds__(split::kThreads, 1)
 sla_bwd_dq_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
                       const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v, BwdParams p) {
   using namespace dq64;
+  using namespace split;
   constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -504,27 +502,16 @@ sla_bwd_dq_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
   const int bh = b * p.h + hh;
 
-  if (threadIdx.x == 0) {
-    mbar_init(&bars[kQFull], 1);
-    for (int i = 0; i < kStages; ++i) {
-      for (int g = 0; g < 2; ++g) {
-        mbar_init(&bars[kKFull + 2 * i + g], 1);
-        mbar_init(&bars[kVFull + 2 * i + g], 1);
-      }
-      mbar_init(&bars[kKEmpty + i], 4);
-      mbar_init(&bars[kVEmpty + i], 4);
-    }
-    mbar_fence_init();
-  }
+  if (threadIdx.x == 0) init_barriers(bars);
   {
     const int32_t* lut_row = p.lut + (int64_t(bh) * p.mblk + m_blk) * p.topk;
-    for (int i = threadIdx.x; i < p.topk; i += kThreads64) s_lut[i] = static_cast<uint16_t>(__ldg(lut_row + i));
+    for (int i = threadIdx.x; i < p.topk; i += split::kThreads) s_lut[i] = static_cast<uint16_t>(__ldg(lut_row + i));
   }
   __syncthreads();
 
   if (warp >= 8) {
     // =============================================================== TMA producer
-    reg_dealloc<kProducerRegs64>();
+    reg_dealloc<kProducerRegs>();
     if (warp == 8 && lane == 0) {
       tma_prefetch_desc(&tmap_q);
       tma_prefetch_desc(&tmap_do);
@@ -558,7 +545,7 @@ sla_bwd_dq_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   }
 
   // =============================================================== consumer warpgroups (same 64 rows, alternate LUT entries)
-  reg_alloc<kConsumerRegs64>();
+  reg_alloc<kConsumerRegs>();
   const int wg = warp >> 2, w4 = warp & 3;
   const int r_lo = w4 * 16 + (lane >> 2);
   const int cq = 2 * (lane & 3);
@@ -578,7 +565,7 @@ sla_bwd_dq_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   mbar_wait(&bars[kQFull], 0);
   for (int j = wg; j < p.topk; j += 2) {
     const int st = j % kStages;
-    const uint32_t ph = (j / (2 * kStages)) & 1;
+    const uint32_t ph = full_phase(j);
     const int valid = p.l - s_lut[j] * BLKK;
     const uint32_t sk = sbase + kOffK + st * kTileK, sv = sbase + kOffV + st * kTileK;
 
@@ -633,207 +620,15 @@ sla_bwd_dq_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     if (lane == 0) mbar_arrive(&bars[kKEmpty + st]);
   }
 
-  // ---- dQ = partial of warpgroup 0 + partial of warpgroup 1, through the drained K ring ([value][thread] layout)
-  float* xchg = reinterpret_cast<float*>(smem + kOffK) + (threadIdx.x & 127);
-  named_bar_sync(1, 256);
-  if (wg == 1) {
+  // ---- dQ = partial of warpgroup 0 + partial of warpgroup 1, through the drained K ring
+  const Handoff x = handoff_wg1_to_wg0(smem + kOffK, wg, 1, [&](const Handoff& x) {
 #pragma unroll
-    for (int i = 0; i < HD / 2; ++i) xchg[i * 128] = acc[i];
-  }
-  named_bar_sync(1, 256);
+    for (int i = 0; i < HD / 2; ++i) x[i] = acc[i];
+  });
   if (wg == 1) return;
 #pragma unroll
-  for (int i = 0; i < HD / 2; ++i) acc[i] += xchg[i * 128];
+  for (int i = 0; i < HD / 2; ++i) acc[i] += x[i];
   store_rows<T>(acc, p.sm_scale, p.dq, int64_t(m_blk) * BLKQ64 + r_lo, p.l, p.h, hh, b, cq);
-}
-
-// dK / dV: sla_bwd_dkdv_kernel with each list entry one 64-row query block, taken by warpgroup j % 2.  With four ring stages
-// slot j % 4 is only ever used by warpgroup j % 2, so every slot's barriers are consumed by one warpgroup, in order, and each
-// warpgroup has its next (Q_i, dO_i) pair in flight while it computes.
-namespace dkv64 {
-constexpr int kStages = 4;
-constexpr uint32_t kTileQ = BLKQ64 * HD * 2, kTileK = BLKK * HD * 2;
-constexpr uint32_t kOffK = 0, kOffV = kTileK, kOffQ = 2 * kTileK, kOffDO = kOffQ + kStages * kTileQ;
-constexpr uint32_t kOffStats = kOffDO + kStages * kTileQ;             // [warpgroup][buffer][lse 64 | delta 64] fp32
-constexpr uint32_t kOffBars = kOffStats + 2 * 2 * 128 * 4;
-constexpr uint32_t kSmem = kOffBars + 128;
-enum Bar { kKVFull = 0, kFull = 1 /*4*/, kEmpty = 5 /*4*/ };
-static_assert((kEmpty + kStages) * 8 <= 128, "barriers exceed their shared-memory slot");
-static_assert(HD * 128 * 4 <= 2 * kStages * kTileQ, "partial dK / dV do not fit in the ring");
-}  // namespace dkv64
-
-template <typename T>
-__global__ void __launch_bounds__(kThreads64, 1)
-sla_bwd_dkdv_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
-                        const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v, BwdParams p) {
-  using namespace dkv64;
-  constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
-  const int bh = b * p.h + hh;
-  const int32_t* kv_off = p.kv_off + int64_t(bh) * (p.nblk + 1);
-  const int32_t* list = p.kv_idx + int64_t(bh) * p.mblk * p.topk + __ldg(kv_off + n_blk);
-  const int n_list = __ldg(kv_off + n_blk + 1) - __ldg(kv_off + n_blk);
-
-  if (n_list == 0) {  // no query block selected this key block: its gradients are zero (the outputs are not pre-zeroed)
-    for (int e = threadIdx.x; e < BLKK * HD / 8; e += kThreads64) {
-      const int64_t r = int64_t(n_blk) * BLKK + e / (HD / 8);
-      if (r >= p.l) break;
-      const int64_t o = ((int64_t(b) * p.l + r) * p.h + hh) * HD + (e % (HD / 8)) * 8;
-      stg_v4(static_cast<T*>(p.dk) + o, make_uint4(0, 0, 0, 0));
-      stg_v4(static_cast<T*>(p.dv) + o, make_uint4(0, 0, 0, 0));
-    }
-    return;
-  }
-  if (threadIdx.x == 0) {
-    mbar_init(&bars[kKVFull], 1);
-    for (int i = 0; i < kStages; ++i) {
-      mbar_init(&bars[kFull + i], 1);
-      mbar_init(&bars[kEmpty + i], 4);   // the four warps of warpgroup i % 2
-    }
-    mbar_fence_init();
-  }
-  __syncthreads();
-
-  if (warp >= 8) {
-    // =============================================================== TMA producer
-    reg_dealloc<kProducerRegs64>();
-    if (warp == 8 && lane == 0) {
-      tma_prefetch_desc(&tmap_q);
-      tma_prefetch_desc(&tmap_do);
-      tma_prefetch_desc(&tmap_k);
-      tma_prefetch_desc(&tmap_v);
-      mbar_expect_tx(&bars[kKVFull], 2 * kTileK);
-#pragma unroll
-      for (int c = 0; c < HD / 64; ++c) {
-        tma_load_4d(smem + kOffK + c * (BLKK * 128), &tmap_k, &bars[kKVFull], c * 64, hh, n_blk * BLKK, b);
-        tma_load_4d(smem + kOffV + c * (BLKK * 128), &tmap_v, &bars[kKVFull], c * 64, hh, n_blk * BLKK, b);
-      }
-      for (int j = 0; j < n_list; ++j) {
-        const int st = j % kStages;
-        const uint32_t ph = ((j / kStages) & 1) ^ 1;
-        const int qb = __ldg(list + j);
-        mbar_wait(&bars[kEmpty + st], ph);
-        mbar_expect_tx(&bars[kFull + st], 2 * kTileQ);
-#pragma unroll
-        for (int c = 0; c < HD / 64; ++c) {
-          tma_load_4d(smem + kOffQ + st * kTileQ + c * (BLKQ64 * 128), &tmap_q, &bars[kFull + st], c * 64, hh, qb * BLKQ64, b);
-          tma_load_4d(smem + kOffDO + st * kTileQ + c * (BLKQ64 * 128), &tmap_do, &bars[kFull + st], c * 64, hh, qb * BLKQ64, b);
-        }
-      }
-    }
-    return;
-  }
-
-  // =============================================================== consumer warpgroups (alternate list entries)
-  reg_alloc<kConsumerRegs64>();
-  const int wg = warp >> 2, w4 = warp & 3, t = threadIdx.x & 127;
-  const int kr_lo = w4 * 16 + (lane >> 2);   // key rows kr_lo, kr_lo + 8 of the block
-  const int cq = 2 * (lane & 3);
-  const uint32_t sbase = smem_u32(smem);
-  const float sc = p.sm_scale * kLog2e;
-  float* stats = reinterpret_cast<float*>(smem + kOffStats) + wg * 256;
-  float dk[HD / 2], dv[HD / 2];
-#pragma unroll
-  for (int i = 0; i < HD / 2; ++i) dk[i] = dv[i] = 0.f;
-
-  mbar_wait(&bars[kKVFull], 0);
-  for (int j = wg, it = 0; j < n_list; j += 2, ++it) {
-    const int st = j % kStages;
-    const uint32_t ph = (j / kStages) & 1;
-    const int qb = __ldg(list + j);
-    // ---- lse / delta of the block's 64 query rows; query rows >= l: P = 0 and delta = 0
-    float* sb = stats + (it & 1) * 128;
-    {
-      const int64_t r = int64_t(qb) * BLKQ64 + (t & 63);
-      const bool in = r < p.l;
-      sb[t] = t < 64 ? (in ? __ldg(p.lse + int64_t(bh) * p.l + r) : INFINITY) : (in ? __ldg(p.delta + int64_t(bh) * p.l + r) : 0.f);
-    }
-    named_bar_sync(1 + wg, 128);
-
-    // ---- S^T = K.Q^T and dP^T = V.dO^T (all operands K-major over d)
-    const uint32_t sq = sbase + kOffQ + st * kTileQ, sg = sbase + kOffDO + st * kTileQ;
-    float s[32], dp[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) s[i] = dp[i] = 0.f;
-    mbar_wait(&bars[kFull + st], ph);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < HD / 16; ++ks) {
-      const uint64_t kd = make_desc_kmajor_sw128(sbase + kOffK + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
-      const uint64_t qd = make_desc_kmajor_sw128(sq + (ks >> 2) * (BLKQ64 * 128)) + uint64_t((ks & 3) * 2);
-      wgmma_f16_ss<64, kBF16>(s, kd, qd, ks > 0 ? 1u : 0u);
-    }
-#pragma unroll
-    for (int ks = 0; ks < HD / 16; ++ks) {
-      const uint64_t vd = make_desc_kmajor_sw128(sbase + kOffV + (ks >> 2) * (BLKK * 128)) + uint64_t((ks & 3) * 2);
-      const uint64_t gd = make_desc_kmajor_sw128(sg + (ks >> 2) * (BLKQ64 * 128)) + uint64_t((ks & 3) * 2);
-      wgmma_f16_ss<64, kBF16>(dp, vd, gd, ks > 0 ? 1u : 0u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(s);
-    reg_fence(dp);
-
-    // ---- P^T rounded to T; dV += P^T.dO with dO as the MN-major operand (+16 rows = +2048 B per K step).
-    //      Key rows >= l only reach dK / dV rows that are never stored, so they need no mask.
-    uint32_t pa[4][4], da[4][4];
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const float2 ls = *reinterpret_cast<const float2*>(sb + 8 * (i >> 2) + cq);
-      s[i] = fast_exp2(fmaf(s[i], sc, -ls.x));
-      s[i + 1] = fast_exp2(fmaf(s[i + 1], sc, -ls.y));
-      pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(s[i], s[i + 1]);
-    }
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) wgmma_f16_rs<HD, kBF16, 1>(dv, pa[kk], make_desc_mnmajor_sw128(sg, BLKQ64 * 128) + uint64_t(kk * 128));
-    wgmma_commit();
-    // ---- dS^T = P^T o (dP^T - delta) rounded to T; dK += dS^T.Q
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const float2 dl = *reinterpret_cast<const float2*>(sb + 64 + 8 * (i >> 2) + cq);
-      da[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(s[i] * (dp[i] - dl.x), s[i + 1] * (dp[i + 1] - dl.y));
-    }
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) wgmma_f16_rs<HD, kBF16, 1>(dk, da[kk], make_desc_mnmajor_sw128(sq, BLKQ64 * 128) + uint64_t(kk * 128));
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(dv);
-    reg_fence(dk);
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      reg_fence(pa[kk]);
-      reg_fence(da[kk]);
-    }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars[kEmpty + st]);
-  }
-
-  // ---- warpgroup 1's partials -> warpgroup 0 through the Q / dO ring (every slot consumed); [value][thread] layout
-  float* xchg = reinterpret_cast<float*>(smem + kOffQ) + t;
-  named_bar_sync(3, 256);
-  if (wg == 1) {
-#pragma unroll
-    for (int i = 0; i < HD / 2; ++i) {
-      xchg[i * 128] = dk[i];
-      xchg[(HD / 2 + i) * 128] = dv[i];
-    }
-  }
-  named_bar_sync(3, 256);
-  if (wg == 1) return;
-#pragma unroll
-  for (int i = 0; i < HD / 2; ++i) {
-    dk[i] += xchg[i * 128];
-    dv[i] += xchg[(HD / 2 + i) * 128];
-  }
-  const int64_t row0 = int64_t(n_blk) * BLKK + kr_lo;
-  store_rows<T>(dk, p.sm_scale, p.dk, row0, p.l, p.h, hh, b, cq);
-  store_rows<T>(dv, 1.0f, p.dv, row0, p.l, p.h, hh, b, cq);
 }
 
 // ------------------------------------------------------------------------------------------------ host
@@ -903,8 +698,8 @@ int launch_bwd(const void* q, const void* k, const void* v, const void* o_s, con
 
   constexpr bool kQ64 = kBQ == BLKQ64;
   const auto dq_kern = kQ64 ? sla_bwd_dq_q64_kernel<T> : sla_bwd_dq_kernel<T>;
-  const auto dkdv_kern = kQ64 ? sla_bwd_dkdv_q64_kernel<T> : sla_bwd_dkdv_kernel<T>;
-  const int threads_dq = kQ64 ? kThreads64 : dq::kThreads, threads_kv = kQ64 ? kThreads64 : dkv::kThreads;
+  const auto dkdv_kern = sla_bwd_dkdv_kernel<T, kBQ>;
+  const int threads_dq = kQ64 ? split::kThreads : dq::kThreads;
   const size_t smem_dq = 1024 + (kQ64 ? dq64::kOffLut : dq::kOffLut) + ((size_t(topk) * 2 + 15) & ~size_t(15));
   if (int rc = check_cuda(cudaFuncSetAttribute(dq_kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_dq)),
                           "cudaFuncSetAttribute(sla_bwd_dq)"))
@@ -912,11 +707,11 @@ int launch_bwd(const void* q, const void* k, const void* v, const void* o_s, con
   dq_kern<<<dim3(unsigned(mblk), unsigned(h), unsigned(b)), threads_dq, smem_dq, st>>>(tq, tdo, tk, tv, p);
   if (int rc = check_launch("sla_bwd_dq_kernel")) return rc;
 
-  const size_t smem_kv = 1024 + (kQ64 ? dkv64::kSmem : dkv::kSmem);
+  const size_t smem_kv = 1024 + Dkv<kBQ>::kSmem;
   if (int rc = check_cuda(cudaFuncSetAttribute(dkdv_kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_kv)),
                           "cudaFuncSetAttribute(sla_bwd_dkdv)"))
     return rc;
-  dkdv_kern<<<dim3(unsigned(nblk), unsigned(h), unsigned(b)), threads_kv, smem_kv, st>>>(tq, tdo, tk, tv, p);
+  dkdv_kern<<<dim3(unsigned(nblk), unsigned(h), unsigned(b)), split::kThreads, smem_kv, st>>>(tq, tdo, tk, tv, p);
   return check_launch("sla_bwd_dkdv_kernel");
 }
 
@@ -934,7 +729,8 @@ extern "C" int64_t tdb200_sla_attn16_bwd_workspace_bytes(int64_t b, int64_t h, i
   return int64_t(ws_layout(b, h, l, topk, blkq).total);
 }
 
-// (blkq, blkk) = (128, 64) runs sla_bwd_dq_kernel / sla_bwd_dkdv_kernel, (64, 64) their _q64 forms.
+// (blkq, blkk) = (128, 64) runs sla_bwd_dq_kernel / sla_bwd_dkdv_kernel<T, 128>, (64, 64) sla_bwd_dq_q64_kernel /
+// sla_bwd_dkdv_kernel<T, 64>.
 extern "C" int tdb200_sla_attn16_bwd(const void* q, const void* k, const void* v, const void* o_s, const void* d_o, const float* lse,
                                      int dtype, const int32_t* lut, int64_t topk, void* dq, void* dk, void* dv, void* workspace,
                                      int64_t workspace_bytes, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale,

@@ -169,7 +169,12 @@ int tdb200_rms_norm_rope_table(const void* x, int dtype, const float* w, const f
  *     sparse_map [b,h,mblk,nblk] int8 0/1 (SLA/utils.py:64-66) and lut [b,h,mblk,topk] int32 ascending block ids.
  * tdb200_sla_linear_moments   phi = feature map of the keys: 0 softmax over d, 1 elu+1, 2 relu (SLA/core.py:57-73);
  *     kv [b,h,d(v),d(k)] fp32 = sum_l v[l,:]^T phi(k)[l,:], ksum [b,h,d] fp32 = sum_l phi(k)[l,:]   (SLA/core.py:243-247).
- *     Both must be zeroed by the caller (they are accumulated, so sequence shards can be summed with one all-reduce).
+ *     Both must be zeroed by the caller (they are accumulated, so sequence shards can be summed with one all-reduce);
+ *     each element receives one plain add of the call's total, so a second launch into the same buffer gives fp32(t + t).
+ *     Reproducible: the bits of one (b, h) depend only on that head's k, v, l, d, feature map and dtype, not on the run,
+ *     the GPU's SM count, the number of heads or batch entries in the call, or other work on the device.  The 128-row
+ *     tiles are split over min(ceil(l/128), 8) CTAs of one thread-block cluster, whose partials are summed in split order
+ *     without floating-point atomics.
  * tdb200_sla_project_moments  kvw [bh,d,d] T = T(proj_w [d,d] . kv [bh,d,d]): folds proj_l's weight (SLA/core.py:246
  *     `self.proj_l(o_l)`) into the moment matrix so the fused kernel applies it with its last MMA; fp32 FMA chain over d_v.
  * tdb200_sla_attn_fwd   o = T( sparse_softmax_attention(q_i8,k_i8,v; lut) + proj( phi(q) kv / (1e-5 + phi(q).ksum) ) )

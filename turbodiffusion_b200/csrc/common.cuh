@@ -143,6 +143,25 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// distributed shared memory: the word(s) at this CTA's shared address `saddr`, read from CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t dsmem_addr(uint32_t saddr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
+  return r;
+}
+__device__ __forceinline__ float4 ld_dsmem_v4(uint32_t saddr, uint32_t rank) {
+  float4 v;
+  asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+               : "r"(dsmem_addr(saddr, rank))
+               : "memory");
+  return v;
+}
+__device__ __forceinline__ float ld_dsmem_f32(uint32_t saddr, uint32_t rank) {
+  float v;
+  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(dsmem_addr(saddr, rank)) : "memory");
+  return v;
+}
 
 // ------------------------------------------------------------------------------------------
 // wgmma (sm_90a warpgroup MMA): shared-memory matrix descriptors

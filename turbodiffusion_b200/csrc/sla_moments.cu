@@ -2,8 +2,18 @@
 //   phi = softmax over the head dim (rounded to the 16-bit type),
 //   kv[b,h,dv,dk] += sum_l v[l,dv] * phi(k)[l,dk]        (stored transposed: rows = value channel, cols = key channel)
 //   ksum[b,h,dk]  += sum_l phi(k)[l,dk]
-// Both outputs are ACCUMULATED in fp32 with red.global.add (caller zeroes them), so sequence shards and the split-L
-// CTAs of one GPU combine by plain addition (and one all-reduce across GPUs).
+// Both outputs are ACCUMULATED in fp32 (caller zeroes them): every element receives exactly one plain add of this call's
+// total, so sequence shards combine by plain addition (and one all-reduce across GPUs), and two launches into the same
+// buffer give exactly fp32(t + t).
+//
+// Reproducibility: the bits of kv and ksum of one (b, h) depend only on that head's k, v, l, d, feature map and dtype.
+// They do not depend on the run, the GPU's SM count, the number of heads or batch entries in the call, or other work on
+// the device.  There are no floating-point atomics.  The tiles ceil(l/128) are split over S = min(tiles, kMaxSplits) CTAs
+// (split s owns tiles s, s+S, s+2S, ...), a function of the tile count alone.  Those S CTAs form one thread-block cluster
+// along grid.y.  After the last tile each CTA stages its fp32 partial kv (and its two ksum row halves, folded lower half
+// first) in its own shared memory, in the V ring that is free by then.  After a cluster barrier, CTA r reduces its slice
+// of the elements over distributed shared memory in split order 0, 1, ..., S-1 and adds the total to global memory, so
+// each element has one writer and one summation order.
 //
 // CTA = 2 warpgroups, 128 key rows per tile.  Two threads per key row (each owns 64 of its 128 channels): load the row,
 // feature map (softmax over D with MUFU ex2), write phi(k) into shared memory in the MN-major 128B-swizzled operand layout;
@@ -33,6 +43,12 @@ constexpr uint32_t kOffPhi = kVStages * kOperandBytes;
 constexpr uint32_t kOffBars = kOffPhi + kOperandBytes;    // 128 KB
 constexpr size_t kSmemBytes = 1024 + kOffBars + 128;
 constexpr float kLog2e = 1.4426950408889634f;
+// Split CTAs per (head or head pair, b): the cluster size, at most 8 (portable).  12 heads x 8 = 96 CTAs fill one wave
+// on an H100 (two 8-CTA clusters per GPC).
+constexpr int kMaxSplits = 8;
+// Partials staged after the last tile, in the V ring: kv [D*D] fp32 (a pair uses the first 2*64*64), then ksum [2][128]
+constexpr uint32_t kOffPartKsum = D * D * 4;
+static_assert(kOffPartKsum + 2 * 128 * 4 <= kOffPhi - kOffV, "the staged partials must fit in the V ring");
 
 struct MomParams {
   const void* k;
@@ -42,10 +58,6 @@ struct MomParams {
   int hd;        // 128, or 64 (two heads per 128-wide row; `h` is then the number of REAL heads, grid.x = ceil(h/2) pairs)
   int feature;   // 0 softmax, 1 elu+1, 2 relu
 };
-
-__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
-  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
-}
 
 template <typename T, bool kPair>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -60,8 +72,7 @@ sla_moments_kernel(const __grid_constant__ CUtensorMap tmap_v, MomParams p) {
   const int head0 = kPair ? 2 * hh : hh;                           // first real head of this CTA
   const bool second_ok = !kPair || head0 + 1 < p.h;                // odd head count: the last pair has one real head
   const int64_t row_elems = int64_t(p.h) * p.hd;                   // elements per token row of k / v
-  const int my_tiles = (p.tiles - split + p.splits - 1) / p.splits;  // tiles split, split+splits, ...
-  if (my_tiles <= 0) return;   // more splits than tiles
+  const int my_tiles = (p.tiles - split + p.splits - 1) / p.splits;  // tiles split, split+splits, ...; >= 1 (splits <= tiles)
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kVStages; ++i) mbar_init(&vfull[i], 1);
@@ -191,27 +202,61 @@ sla_moments_kernel(const __grid_constant__ CUtensorMap tmap_v, MomParams p) {
   }
   wgmma_wait<0>();
   reg_fence(acc);
+  __syncthreads();   // both warpgroups' MMAs have retired: the V ring is free for the partials
+  // ---- stage this CTA's partials.  kv in the layout of its global block: a 128-wide head's [dv][dk] rows 64wg.., or a
+  // pair's two [64][64] blocks one after the other (accumulator rows = value channels, fragment layout in common.cuh).
+  // ksum: thread t's sum over key rows 64(t/128).. of channel t % 128 (head0's channel, or a pair's channel c-64 of head0+1).
+  float* const part = reinterpret_cast<float*>(smem + kOffV);
   {
-    // thread t holds key channel t % 128 of the 128-wide row: head0's channel, or (pairs) channel c-64 of head0+1
-    const int col = threadIdx.x & 127;
-    if (!kPair) {
-      atomicAdd(p.ksum + (int64_t(b) * p.h + head0) * D + col, ksum_acc);
-    } else if (col < 64 || second_ok) {
-      atomicAdd(p.ksum + (int64_t(b) * p.h + head0 + (col >> 6)) * 64 + (col & 63), ksum_acc);
-    }
-  }
-  // ---- kv: accumulator rows = value channels, columns = key channels (fragment layout, common.cuh)
-  const int w4 = warp & 3;
-  const int dv_lo = w4 * 16 + (lane >> 2), cq = 2 * (lane & 3);
-  if (!kPair || wg == 0 || second_ok) {
-    float* dst = kPair ? p.kv + (int64_t(b) * p.h + head0 + wg) * 64 * 64
-                       : p.kv + (int64_t(b) * p.h + head0) * D * D + int64_t(wg) * 64 * D;
+    const int w4 = warp & 3;
+    const int dv_lo = w4 * 16 + (lane >> 2), cq = 2 * (lane & 3);
+    float* const mine = part + wg * 64 * N;
 #pragma unroll
     for (int j = 0; j < N / 8; ++j)
 #pragma unroll
       for (int h2 = 0; h2 < 2; ++h2)
-        red_add_v2(dst + int64_t(dv_lo + 8 * h2) * N + 8 * j + cq, acc[4 * j + 2 * h2], acc[4 * j + 2 * h2 + 1]);
+        *reinterpret_cast<float2*>(mine + (dv_lo + 8 * h2) * N + 8 * j + cq) =
+            make_float2(acc[4 * j + 2 * h2], acc[4 * j + 2 * h2 + 1]);
+    part[kOffPartKsum / 4 + threadIdx.x] = ksum_acc;
   }
+  cluster_sync_all();   // every split's partials are staged and visible across the cluster
+  // ---- reduce: CTA `rank` owns every S-th run of kThreads float4 chunks; each element is summed over splits 0..S-1
+  {
+    const uint32_t rank = cluster_ctarank(), S = p.splits;
+    const uint32_t spart = smem_u32(part);
+    const int64_t bh0 = int64_t(b) * p.h + head0;
+    constexpr int kChunks = (kPair ? 2 * 64 * 64 : D * D) / 4;
+    const int live_chunks = second_ok ? kChunks : kChunks / 2;   // odd head count: the last pair's second head is absent
+    float4* const dst = reinterpret_cast<float4*>(p.kv + bh0 * (kPair ? 64 * 64 : D * D));
+    // all S loads of an element are issued before the first add, so the remote reads overlap
+    for (int c = int(rank) * kThreads + threadIdx.x; c < live_chunks; c += S * kThreads) {
+      float4 g = dst[c];
+      float4 u[kMaxSplits];
+#pragma unroll
+      for (uint32_t s = 0; s < kMaxSplits; ++s)
+        if (s < S) u[s] = ld_dsmem_v4(spart + c * 16, s);
+      float4 t = u[0];
+#pragma unroll
+      for (uint32_t s = 1; s < kMaxSplits; ++s)
+        if (s < S) { t.x += u[s].x; t.y += u[s].y; t.z += u[s].z; t.w += u[s].w; }
+      g.x += t.x; g.y += t.y; g.z += t.z; g.w += t.w;
+      dst[c] = g;
+    }
+    const int live_cols = second_ok ? 128 : 64;
+    for (int c = int(rank) * kThreads + threadIdx.x; c < live_cols; c += S * kThreads) {
+      const uint32_t a = spart + kOffPartKsum + c * 4;
+      float u[kMaxSplits][2];
+#pragma unroll
+      for (uint32_t s = 0; s < kMaxSplits; ++s)
+        if (s < S) { u[s][0] = ld_dsmem_f32(a, s); u[s][1] = ld_dsmem_f32(a + 128 * 4, s); }
+      float t = u[0][0] + u[0][1];
+#pragma unroll
+      for (uint32_t s = 1; s < kMaxSplits; ++s)
+        if (s < S) t += u[s][0] + u[s][1];
+      p.ksum[bh0 * p.hd + c] += t;   // a pair's channels 64.. are head0+1's, which follow head0's 64 in ksum
+    }
+  }
+  cluster_sync_all();   // no CTA leaves while another still reads its shared memory
 }
 
 }  // namespace
@@ -244,20 +289,26 @@ extern "C" int tdb200_sla_linear_moments(const void* k, const void* v, int dtype
   p.hd = int(d);
   p.feature = feature;
   p.tiles = int(cdiv64(l, kRowsPerTile));
-  int splits = sm_count() / int(b * units);
-  if (splits < 1) splits = 1;
-  if (splits > p.tiles) splits = p.tiles;
-  p.splits = splits;
-  dim3 grid(static_cast<unsigned>(units), splits, static_cast<unsigned>(b));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  p.splits = p.tiles < kMaxSplits ? p.tiles : kMaxSplits;   // the tile count alone decides the summation order
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(static_cast<unsigned>(units), static_cast<unsigned>(p.splits), static_cast<unsigned>(b));
+  cfg.blockDim = dim3(kThreads);
+  cfg.dynamicSmemBytes = kSmemBytes;
+  cfg.stream = static_cast<cudaStream_t>(stream);
+  cudaLaunchAttribute cluster;
+  cluster.id = cudaLaunchAttributeClusterDimension;
+  cluster.val.clusterDim.x = 1;
+  cluster.val.clusterDim.y = static_cast<unsigned>(p.splits);   // the split CTAs of one (head or pair, b)
+  cluster.val.clusterDim.z = 1;
+  cfg.attrs = &cluster;
+  cfg.numAttrs = 1;
 #define TDB_MOM2(T, PAIR)                                                                                          \
   do {                                                                                                              \
     static bool attr_done[64] = {false};                                                                            \
     if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(sla_moments_kernel<T, PAIR>), kSmemBytes, attr_done, \
                                            "cudaFuncSetAttribute(sla_moments)"))                                   \
       return rc;                                                                                                    \
-    sla_moments_kernel<T, PAIR><<<grid, kThreads, kSmemBytes, st>>>(tv, p);                                         \
-    return check_launch("sla_moments_kernel");                                                                      \
+    return check_cuda(cudaLaunchKernelEx(&cfg, sla_moments_kernel<T, PAIR>, tv, p), "sla_moments_kernel");          \
   } while (0)
 #define TDB_MOM(T) do { if (d == 64) { TDB_MOM2(T, true); } else { TDB_MOM2(T, false); } } while (0)
   if (dtype == TDB200_DTYPE_BF16) TDB_MOM(__nv_bfloat16);

@@ -3,20 +3,27 @@
 //
 //   c[i,j] = T( fma-chain over kb of  float(int32 dot of K-block kb) * (a_s[i/128,kb]*b_s[j/128,kb]) )  [+ bias]
 //
-// Design (one CTA per 128x256 output tile, 128-deep K-blocks; the tile is one 128-row block of the activation scale grid
-// and two 128-column blocks ("halves") of the weight scale grid):
+// Design (128x256 output tiles, 128-deep K-blocks; a tile is one 128-row block of the activation scale grid and two
+// 128-column blocks ("halves") of the weight scale grid).  The kernel is persistent: min(tiles, SMs) CTAs, one per SM, and
+// CTA b works through tiles b, b + grid, b + 2 grid, ... with tile id = m_tile * n_tiles + n_tile, so the CTAs running
+// together share A rows and a few B tiles in L2.  Producer and consumers derive that sequence on their own (no scheduler,
+// no atomics); barriers, the register split and the tensor-map prefetch are paid once per CTA.  A GEMM with fewer tiles
+// than SMs is one tile per CTA.
 //   warpgroup 2  TMA producer (one thread of warp 8; setmaxnreg gives its registers to the consumers, whose two fp32
 //            accumulators and int32 staging accumulator do not fit in the 168 a 384-thread CTA starts with): A tile
 //            [128 rows x 128 B] and B tile [256 rows x 128 B] per K-block, 128B-swizzled, 4-stage ring, mbarrier
 //            complete_tx.  The wide tile does twice the MMA work of a 128x128 one for 1.5x the operand bytes pulled from
-//            L2, and pays the ring fill and the epilogue once per twice the work (DESIGN.md, a2).
+//            L2.  Ring slot and phase come from one K-block counter that runs on across tiles, so the next tile's first
+//            loads are issued as soon as slots free up: during the consumers' last K-blocks and their epilogue.
 //   warpgroups 0-1  MMA + dequant + epilogue; warpgroup g owns output rows [64g, 64g+64) of the tile.  Per K-block and
 //            half: four wgmma.m64n128k32.s32.s8.s8 into one 64-register int32 staging accumulator, then the int -> float
 //            conversion and the FFMA with that half's block scale into the half's 64 fp32 registers.  Both warpgroups
-//            issue together off the same full barrier, so their MMA phases and their dequant phases coincide; ordering
-//            them to alternate (ping-pong, -DTDB200_GEMM_PINGPONG) was measured slower (DESIGN.md, a2).  The
-//            accumulate flag is reset at every K-block because the reference rescales per K-block.  After the last
-//            K-block, per half: round to T, (+bias), (GELU), store.  A half that lies entirely past n is not stored, and in the block-scale variant not multiplied either.
+//            issue off the same full barrier; ordering them to alternate (ping-pong) was measured slower (DESIGN.md,
+//            a2).  The accumulate flag is reset at every K-block because the reference rescales per K-block.  After the
+//            last K-block, per half: round to T, (+bias), (GELU), store.  A half that lies entirely past n is not stored,
+//            and in the block-scale variant not multiplied either.  Each warpgroup loops over the tiles on its own with
+//            the same running K-block counter; only the quantised epilogue's amax exchange makes the two meet, so
+//            otherwise one warpgroup's epilogue overlaps the other's MMAs once they drift apart.
 // Integer accumulation is exact and the fp32 FMA chain runs in ascending kb order, so the result is bit-identical
 // to the reference restatement (oracle.int8_linear) on the same int8 inputs.
 #include "common.cuh"
@@ -35,7 +42,7 @@ constexpr uint32_t kProducerRegs = 40, kConsumerRegs = 232;   // 128 * 40 + 256 
 constexpr uint32_t kATile = BM * BK;                 // 16 KB
 constexpr uint32_t kBTile = BN * BK;                 // 32 KB: half h at +16 KB h
 constexpr uint32_t kStageBytes = kATile + kBTile;
-constexpr size_t kSmemBytes = 1024 + size_t(kStages) * kStageBytes + 256 /*barriers + amax exchange*/;
+constexpr size_t kSmemBytes = 1024 + size_t(kStages) * kStageBytes + 256 /*barriers 64 B + amax exchange 128 B*/;
 
 struct GemmParams {
   const float* a_s;
@@ -44,6 +51,8 @@ struct GemmParams {
   void* c;
   int64_t m, n, k;
   int k_blocks;
+  int n_tiles;    // 256-column tiles per 128-row tile
+  int tiles;      // ceil(m / 128) * n_tiles
   int act;        // 0 none, 1 GELU(tanh) applied to the T-rounded (acc [+ bias]) value, result rounded to T again
   int8_t* out_q;  // when non-NULL: emit quant_int8_block128(T output) instead of the T output itself
   float* out_s;   // [ceil(m/128), n/128]
@@ -82,11 +91,10 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + size_t(kStages) * kStageBytes);
   uint64_t* full_bar = bars;                // [kStages]  TMA -> MMA
   uint64_t* empty_bar = bars + kStages;     // [kStages]  MMA -> TMA (one arrival per consumer warp)
-  float* amax_x = reinterpret_cast<float*>(bars + 2 * kStages);  // [2][kConsumerWarps] block-amax exchange per half
+  float* amax_x = reinterpret_cast<float*>(bars + 2 * kStages);  // [2][2][kConsumerWarps] block-amax exchange: tile parity, half
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int n_tile = blockIdx.x, m_tile = blockIdx.y;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kStages; ++i) {
@@ -103,13 +111,17 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     if (warp == kConsumerWarps && lane == 0) {
       tma_prefetch_desc(&tmap_a);
       tma_prefetch_desc(&tmap_b);
-      for (int kb = 0; kb < p.k_blocks; ++kb) {
-        const uint32_t stage = kb % kStages, phase = (kb / kStages) & 1u;
-        mbar_wait(&empty_bar[stage], phase ^ 1u);
-        uint8_t* sa = smem + size_t(stage) * kStageBytes;
-        mbar_expect_tx(&full_bar[stage], kStageBytes);
-        tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * BK, m_tile * BM);
-        tma_load_2d(sa + kATile, &tmap_b, &full_bar[stage], kb * BK, n_tile * BN);
+      uint32_t it = 0;   // K-blocks loaded so far, over all tiles; only it % (2 kStages) matters, so wrap-around is harmless
+      for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
+        const int n_tile = tile % p.n_tiles, m_tile = tile / p.n_tiles;
+        for (int kb = 0; kb < p.k_blocks; ++kb, ++it) {
+          const uint32_t stage = it % kStages, phase = (it / kStages) & 1u;
+          mbar_wait(&empty_bar[stage], phase ^ 1u);
+          uint8_t* sa = smem + size_t(stage) * kStageBytes;
+          mbar_expect_tx(&full_bar[stage], kStageBytes);
+          tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * BK, m_tile * BM);
+          tma_load_2d(sa + kATile, &tmap_b, &full_bar[stage], kb * BK, n_tile * BN);
+        }
       }
     }
     return;
@@ -119,10 +131,11 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   reg_alloc<kConsumerRegs>();
   const int wg = warp >> 2, w4 = warp & 3;
   const uint32_t sbase = smem_u32(smem);
-  // the four K=32 steps of K-block kb against half `h` of the B tile into `d` (onto its contents when `acc_in`); the caller
-  // has waited on the stage's full barrier and commits the group
-  auto issue = [&](uint32_t (&d)[64], int kb, int h, bool acc_in) {
-    const uint32_t sa = sbase + (kb % kStages) * kStageBytes;
+  // `it` below counts this CTA's K-blocks over all its tiles, as the producer does: it names the ring slot and its phase.
+  // The four K=32 steps of K-block `it` against half `h` of the B tile into `d` (onto its contents when `acc_in`); the
+  // caller has waited on the stage's full barrier and commits the group
+  auto issue = [&](uint32_t (&d)[64], uint32_t it, int h, bool acc_in) {
+    const uint32_t sa = sbase + (it % kStages) * kStageBytes;
     const uint64_t adesc = make_desc_kmajor_sw128(sa + wg * (64 * 128));
     const uint64_t bdesc = make_desc_kmajor_sw128(sa + kATile + h * (BH * BK));
     wgmma_fence();
@@ -130,198 +143,187 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     for (int ks = 0; ks < BK / 32; ++ks)  // +32 bytes (one K=32 int8 slice) inside the 128B swizzle row: +2 in 16-byte units
       wgmma_i8_ss<BH>(d, adesc + uint64_t(ks * 2), bdesc + uint64_t(ks * 2), (ks > 0 || acc_in) ? 1u : 0u);
   };
-  auto wait_full = [&](int kb) { mbar_wait(&full_bar[kb % kStages], (kb / kStages) & 1u); };
-  auto release = [&](int kb) {
+  auto wait_full = [&](uint32_t it) { mbar_wait(&full_bar[it % kStages], (it / kStages) & 1u); };
+  auto release = [&](uint32_t it) {
     __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[kb % kStages]);
+    if (lane == 0) mbar_arrive(&empty_bar[it % kStages]);
   };
 
   // fragment coordinates (common.cuh): register i holds row r_lo + 8 ((i >> 1) & 1), column 8 (i >> 2) + cq + (i & 1)
   const int r_lo = wg * 64 + w4 * 16 + (lane >> 2);
   const int cq = 2 * (lane & 3);
-  const int64_t row0 = int64_t(m_tile) * BM + r_lo, row1 = row0 + 8;
   const T* bias = static_cast<const T*>(p.bias);
-  // the second half holds at least one column < n (CTA-uniform)
-  const bool has_hi = int64_t(n_tile) * BN + BH < p.n;
+  const bool act_gelu = p.act == 1;
 
-  if constexpr (kRowScale) {
-    uint32_t ia0[64], ia1[64];
-    // K-block kb's MMAs chain onto kb-1's in flight (same accumulators, in order): wait only for kb-1 to free its slot,
-    // so the tensor pipe does not drain at every K-block of a long K
-    for (int kb = 0; kb < p.k_blocks; ++kb) {
-      wait_full(kb);
-      issue(ia0, kb, 0, kb > 0);
-      issue(ia1, kb, 1, kb > 0);   // unconditional: a wgmma under a branch costs an injected warpgroup.arrive per K-block
-      wgmma_commit();
-      if (kb > 0) {
-        wgmma_wait<1>();
-        release(kb - 1);
+  uint32_t it0 = 0;       // the running K-block count at the start of the tile
+  uint32_t parity = 0;    // of this CTA's tile count: selects the amax exchange slots
+  for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x, it0 += p.k_blocks, parity ^= 1u) {
+    const int n_tile = tile % p.n_tiles, m_tile = tile / p.n_tiles;
+    const int64_t row0 = int64_t(m_tile) * BM + r_lo, row1 = row0 + 8;
+    // the second half holds at least one column < n (CTA-uniform)
+    const bool has_hi = int64_t(n_tile) * BN + BH < p.n;
+
+    if constexpr (kRowScale) {
+      uint32_t ia0[64], ia1[64];
+      // K-block kb's MMAs chain onto kb-1's in flight (same accumulators, in order): wait only for kb-1 to free its slot,
+      // so the tensor pipe does not drain at every K-block of a long K
+      for (int kb = 0; kb < p.k_blocks; ++kb) {
+        wait_full(it0 + kb);
+        issue(ia0, it0 + kb, 0, kb > 0);
+        issue(ia1, it0 + kb, 1, kb > 0);   // unconditional: a wgmma under a branch costs an injected warpgroup.arrive per K-block
+        wgmma_commit();
+        if (kb > 0) {
+          wgmma_wait<1>();
+          release(it0 + kb - 1);
+        }
       }
+      wgmma_wait<0>();
+      release(it0 + p.k_blocks - 1);   // the producer refills the last slot for the next tile during this epilogue
+      reg_fence(ia0);
+      reg_fence(ia1);
+      // c = T(fma(float(acc) * a_s[row], b_s[col], bias[col])): the reference's TileLang epilogue compiles (nvcc default
+      // -fmad) to I2FP, FMUL, FFMA per element (tools/tilelang_epilogue_probe.py)
+      const float sa0 = row0 < p.m ? __ldg(p.a_s + row0) : 0.f, sa1 = row1 < p.m ? __ldg(p.a_s + row1) : 0.f;
+      auto store = [&](const uint32_t (&ia)[64], int hf) {
+        const int64_t col_base = int64_t(n_tile) * BN + hf * BH + cq;
+#pragma unroll
+        for (int j = 0; j < BH / 8; ++j) {
+          const int64_t col = col_base + 8 * j;
+          if (col >= p.n) continue;
+          const float sb0 = __ldg(p.b_s + col), sb1 = __ldg(p.b_s + col + 1);
+          const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float sa = h ? sa1 : sa0;
+            const float y0 = __fmaf_rn(__fmul_rn(__int2float_rn(static_cast<int>(ia[4 * j + 2 * h])), sa), sb0, F16Traits<T>::lo(bw));
+            const float y1 = __fmaf_rn(__fmul_rn(__int2float_rn(static_cast<int>(ia[4 * j + 2 * h + 1])), sa), sb1, F16Traits<T>::hi(bw));
+            const int64_t row = h ? row1 : row0;
+            if (row < p.m) *reinterpret_cast<uint32_t*>(static_cast<T*>(p.c) + row * p.n + col) = F16Traits<T>::pack(y0, y1);
+          }
+        }
+      };
+      store(ia0, 0);
+      if (has_hi) store(ia1, 1);
+      continue;
     }
-    wgmma_wait<0>();
-    reg_fence(ia0);
-    reg_fence(ia1);
-    // c = T(fma(float(acc) * a_s[row], b_s[col], bias[col])): the reference's TileLang epilogue compiles (nvcc default
-    // -fmad) to I2FP, FMUL, FFMA per element (tools/tilelang_epilogue_probe.py)
-    const float sa0 = row0 < p.m ? __ldg(p.a_s + row0) : 0.f, sa1 = row1 < p.m ? __ldg(p.a_s + row1) : 0.f;
-    auto store = [&](const uint32_t (&ia)[64], int hf) {
+
+    // block scales: a_s [m/128, k_blocks] row m_tile, b_s [ceil(n/128), k_blocks] rows 2 n_tile (+1 only when has_hi)
+    const float* as_row = p.a_s + int64_t(m_tile) * p.k_blocks;
+    const float* bs_row0 = p.b_s + int64_t(2 * n_tile) * p.k_blocks;
+    const float* bs_row1 = bs_row0 + p.k_blocks;
+    float acc0[64], acc1[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc0[i] = acc1[i] = 0.0f;
+    uint32_t ia[64];
+    // float(s) is exact (a K-block sum is at most 128^3 = 2^21 in magnitude).  I2FP + FFMA is two instructions per value
+    // against three for the magic-number conversion (IADD, FADD, FFMA), and measured faster on the H100 (DESIGN.md, a2).
+    auto dequant = [&](float (&acc)[64], float scale) {
+      wgmma_wait<0>();
+      reg_fence(ia);
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = __fmaf_rn(__int2float_rn(static_cast<int>(ia[i])), scale, acc[i]);
+    };
+    for (int kb = 0; kb < p.k_blocks; ++kb) {
+      wait_full(it0 + kb);
+      const float as = __ldg(as_row + kb);
+      issue(ia, it0 + kb, 0, false);
+      wgmma_commit();
+      dequant(acc0, as * __ldg(bs_row0 + kb));
+      if (has_hi) {
+        issue(ia, it0 + kb, 1, false);
+        wgmma_commit();
+        dequant(acc1, as * __ldg(bs_row1 + kb));
+      }
+      release(it0 + kb);
+    }
+
+    if (p.out_q != nullptr) {
+      // ---- fused a1: each half is one 128x128 quant block (m_tile, 2 n_tile + hf).  y = the T-rounded value the plain
+      //      epilogue would store (rows >= m count as 0); amax over the block; q = sat_s8(rint(y*128/amax)).
+      auto store_q = [&](const float (&acc)[64], int hf) {
+        const int64_t col_base = int64_t(n_tile) * BN + hf * BH + cq;
+        uint32_t yw[32];
+        uint32_t amax2 = 0u;
+#pragma unroll
+        for (int j = 0; j < BH / 8; ++j) {
+          const int64_t col = col_base + 8 * j;
+          const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            uint32_t y = F16Traits<T>::pack(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);   // T(acc)
+            if (bias != nullptr) y = F16Traits<T>::add2(y, bw);                            // T(T(acc) + bias)
+            if (act_gelu) y = F16Traits<T>::pack(gelu_tanh_approx(F16Traits<T>::lo(y)), gelu_tanh_approx(F16Traits<T>::hi(y)));
+            if ((h ? row1 : row0) >= p.m) y = 0u;
+            yw[2 * j + h] = y;
+            amax2 = F16Traits<T>::absmax2(amax2, y);
+          }
+        }
+        float amax = fmaxf(1e-8f, fmaxf(F16Traits<T>::lo(amax2), F16Traits<T>::hi(amax2)));
+        amax = warp_max(amax);
+        // One slot set per (tile parity, half).  A set is rewritten two tiles later, and every warp passes the barrier of
+        // the tile in between, after its reads here, before any warp can get there.  One set per half alone would not
+        // do: a tile without a second half has a single barrier, so a warp still reading its slots could be overtaken
+        // by the next tile's write to the same ones.  The parity bit costs 64 bytes and no extra barrier.
+        float* xch = amax_x + (parity * 2 + hf) * kConsumerWarps;
+        if (lane == 0) xch[warp] = amax;
+        named_bar_sync(1, kConsumerWarps * 32);
+#pragma unroll
+        for (int w = 0; w < kConsumerWarps; ++w) amax = fmaxf(amax, xch[w]);
+        const float r = __fdiv_rn(128.0f, amax);
+        if (threadIdx.x == 0) p.out_s[int64_t(m_tile) * (p.n >> 7) + 2 * n_tile + hf] = amax * 0.0078125f;
+#pragma unroll
+        for (int j = 0; j < BH / 8; ++j) {
+          const int64_t col = col_base + 8 * j;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t y = yw[2 * j + h];
+            const int q0 = __float2int_rn(fminf(__fmul_rn(F16Traits<T>::lo(y), r), 127.0f));
+            const int q1 = __float2int_rn(fminf(__fmul_rn(F16Traits<T>::hi(y), r), 127.0f));
+            const int64_t row = h ? row1 : row0;
+            if (row < p.m)
+              *reinterpret_cast<uint16_t*>(p.out_q + row * p.n + col) = static_cast<uint16_t>((q0 & 0xFF) | ((q1 & 0xFF) << 8));
+          }
+        }
+      };
+      store_q(acc0, 0);
+      if (has_hi) store_q(acc1, 1);
+      continue;
+    }
+    // a tile lies inside one output part (n_part is n itself or a multiple of 256): one division per tile, not per column
+    const int part = n_tile * BN / p.n_part;
+    T* c_part = static_cast<T*>(p.c) + int64_t(part) * p.m * p.n_part - int64_t(part) * p.n_part;
+    auto store = [&](const float (&acc)[64], int hf) {
       const int64_t col_base = int64_t(n_tile) * BN + hf * BH + cq;
 #pragma unroll
       for (int j = 0; j < BH / 8; ++j) {
         const int64_t col = col_base + 8 * j;
         if (col >= p.n) continue;
-        const float sb0 = __ldg(p.b_s + col), sb1 = __ldg(p.b_s + col + 1);
         const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
+        T* cp = c_part + col;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const float sa = h ? sa1 : sa0;
-          const float y0 = __fmaf_rn(__fmul_rn(__int2float_rn(static_cast<int>(ia[4 * j + 2 * h])), sa), sb0, F16Traits<T>::lo(bw));
-          const float y1 = __fmaf_rn(__fmul_rn(__int2float_rn(static_cast<int>(ia[4 * j + 2 * h + 1])), sa), sb1, F16Traits<T>::hi(bw));
+          // T(acc) then the packed 16-bit add: one rounding each, exactly the module's `out + bias` on 16-bit tensors
+          uint32_t y = F16Traits<T>::pack(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+          if (bias != nullptr) y = F16Traits<T>::add2(y, bw);
+          if (act_gelu) y = F16Traits<T>::pack(gelu_precise(F16Traits<T>::lo(y)), gelu_precise(F16Traits<T>::hi(y)));
           const int64_t row = h ? row1 : row0;
-          if (row < p.m) *reinterpret_cast<uint32_t*>(static_cast<T*>(p.c) + row * p.n + col) = F16Traits<T>::pack(y0, y1);
+          if (row < p.m) *reinterpret_cast<uint32_t*>(cp + row * p.n_part) = y;
         }
       }
     };
-    store(ia0, 0);
-    if (has_hi) store(ia1, 1);
-    return;
+    store(acc0, 0);
+    if (has_hi) store(acc1, 1);
   }
-
-  // block scales: a_s [m/128, k_blocks] row m_tile, b_s [ceil(n/128), k_blocks] rows 2 n_tile (+1 only when has_hi)
-  const float* as_row = p.a_s + int64_t(m_tile) * p.k_blocks;
-  const float* bs_row0 = p.b_s + int64_t(2 * n_tile) * p.k_blocks;
-  const float* bs_row1 = bs_row0 + p.k_blocks;
-  float acc0[64], acc1[64];
-#pragma unroll
-  for (int i = 0; i < 64; ++i) acc0[i] = acc1[i] = 0.0f;
-  uint32_t ia[64];
-  // float(s) is exact (a K-block sum is at most 128^3 = 2^21 in magnitude).  I2FP + FFMA is two instructions per value
-  // against three for the magic-number conversion (IADD, FADD, FFMA), and measured faster on the H100 (DESIGN.md, a2).
-  auto dequant = [&](float (&acc)[64], float scale) {
-    wgmma_wait<0>();
-    reg_fence(ia);
-#pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = __fmaf_rn(__int2float_rn(static_cast<int>(ia[i])), scale, acc[i]);
-  };
-#ifdef TDB200_GEMM_PINGPONG
-  // Experimental ping-pong schedule (DESIGN.md, a2: measured slower, so not built by default).  A turn is one (K-block,
-  // half) of one warpgroup; turns are issued WG0 t0, WG1 t0, WG0 t1, WG1 t1, ...  Named barrier 2 gates WG0 (synced
-  // before its turns 1..T-1, arrived on by WG1 after issuing its turns 0..T-2), barrier 3 gates WG1 (synced before each
-  // of its T turns, arrived on by WG0 after issuing each of its T turns): the counts balance, so nothing is pending at
-  // exit.  Barrier 1 is the quantised epilogue's amax exchange.
-  const int last_turn = p.k_blocks * (has_hi ? 2 : 1) - 1;   // has_hi is CTA-uniform: both warpgroups have T turns
-  auto before_issue = [&](int t) {
-    if (wg == 1) named_bar_sync(3, kConsumerWarps * 32);
-    else if (t > 0) named_bar_sync(2, kConsumerWarps * 32);
-  };
-  auto after_commit = [&](int t) {
-    if (wg == 0) named_bar_arrive(3, kConsumerWarps * 32);
-    else if (t < last_turn) named_bar_arrive(2, kConsumerWarps * 32);
-  };
-#else
-  auto before_issue = [](int) {};
-  auto after_commit = [](int) {};
-#endif
-  for (int kb = 0, t = 0; kb < p.k_blocks; ++kb) {
-    wait_full(kb);
-    const float as = __ldg(as_row + kb);
-    before_issue(t);
-    issue(ia, kb, 0, false);
-    wgmma_commit();
-    after_commit(t++);
-    dequant(acc0, as * __ldg(bs_row0 + kb));
-    if (has_hi) {
-      before_issue(t);
-      issue(ia, kb, 1, false);
-      wgmma_commit();
-      after_commit(t++);
-      dequant(acc1, as * __ldg(bs_row1 + kb));
-    }
-    release(kb);
-  }
-
-  const bool act_gelu = p.act == 1;
-  if (p.out_q != nullptr) {
-    // ---- fused a1: each half is one 128x128 quant block (m_tile, 2 n_tile + hf).  y = the T-rounded value the plain
-    //      epilogue would store (rows >= m count as 0); amax over the block; q = sat_s8(rint(y*128/amax)).
-    auto store_q = [&](const float (&acc)[64], int hf) {
-      const int64_t col_base = int64_t(n_tile) * BN + hf * BH + cq;
-      uint32_t yw[32];
-      uint32_t amax2 = 0u;
-#pragma unroll
-      for (int j = 0; j < BH / 8; ++j) {
-        const int64_t col = col_base + 8 * j;
-        const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          uint32_t y = F16Traits<T>::pack(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);   // T(acc)
-          if (bias != nullptr) y = F16Traits<T>::add2(y, bw);                            // T(T(acc) + bias)
-          if (act_gelu) y = F16Traits<T>::pack(gelu_tanh_approx(F16Traits<T>::lo(y)), gelu_tanh_approx(F16Traits<T>::hi(y)));
-          if ((h ? row1 : row0) >= p.m) y = 0u;
-          yw[2 * j + h] = y;
-          amax2 = F16Traits<T>::absmax2(amax2, y);
-        }
-      }
-      float amax = fmaxf(1e-8f, fmaxf(F16Traits<T>::lo(amax2), F16Traits<T>::hi(amax2)));
-      amax = warp_max(amax);
-      float* xch = amax_x + hf * kConsumerWarps;   // one exchange slot set per half: no reuse hazard between halves
-      if (lane == 0) xch[warp] = amax;
-      named_bar_sync(1, kConsumerWarps * 32);
-#pragma unroll
-      for (int w = 0; w < kConsumerWarps; ++w) amax = fmaxf(amax, xch[w]);
-      const float r = __fdiv_rn(128.0f, amax);
-      if (threadIdx.x == 0) p.out_s[int64_t(m_tile) * (p.n >> 7) + 2 * n_tile + hf] = amax * 0.0078125f;
-#pragma unroll
-      for (int j = 0; j < BH / 8; ++j) {
-        const int64_t col = col_base + 8 * j;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const uint32_t y = yw[2 * j + h];
-          const int q0 = __float2int_rn(fminf(__fmul_rn(F16Traits<T>::lo(y), r), 127.0f));
-          const int q1 = __float2int_rn(fminf(__fmul_rn(F16Traits<T>::hi(y), r), 127.0f));
-          const int64_t row = h ? row1 : row0;
-          if (row < p.m)
-            *reinterpret_cast<uint16_t*>(p.out_q + row * p.n + col) = static_cast<uint16_t>((q0 & 0xFF) | ((q1 & 0xFF) << 8));
-        }
-      }
-    };
-    store_q(acc0, 0);
-    if (has_hi) store_q(acc1, 1);
-    return;
-  }
-  auto store = [&](const float (&acc)[64], int hf) {
-    const int64_t col_base = int64_t(n_tile) * BN + hf * BH + cq;
-#pragma unroll
-    for (int j = 0; j < BH / 8; ++j) {
-      const int64_t col = col_base + 8 * j;
-      if (col >= p.n) continue;
-      const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
-      const int64_t part = col / p.n_part;
-      T* cp = static_cast<T*>(p.c) + part * p.m * p.n_part + (col - part * p.n_part);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        // T(acc) then the packed 16-bit add: one rounding each, exactly the module's `out + bias` on 16-bit tensors
-        uint32_t y = F16Traits<T>::pack(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-        if (bias != nullptr) y = F16Traits<T>::add2(y, bw);
-        if (act_gelu) y = F16Traits<T>::pack(gelu_precise(F16Traits<T>::lo(y)), gelu_precise(F16Traits<T>::hi(y)));
-        const int64_t row = h ? row1 : row0;
-        if (row < p.m) *reinterpret_cast<uint32_t*>(cp + row * p.n_part) = y;
-      }
-    }
-  };
-  store(acc0, 0);
-  if (has_hi) store(acc1, 1);
 }
 
 template <typename T, bool kRowScale>
-int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int64_t m_tiles, int64_t n_tiles,
-           cudaStream_t st) {
+int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st) {
   auto kern = gemm_w8a8_kernel<T, kRowScale>;
   static bool attr_done[64] = {false};
   if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), kSmemBytes, attr_done,
                                          "cudaFuncSetAttribute(gemm_w8a8)"))
     return rc;
-  kern<<<dim3(static_cast<unsigned>(n_tiles), static_cast<unsigned>(m_tiles)), kThreads, kSmemBytes, st>>>(ta, tb, p);
+  kern<<<std::min(p.tiles, sm_count()), kThreads, kSmemBytes, st>>>(ta, tb, p);
   return check_launch("gemm_w8a8_kernel");
 }
 
@@ -392,7 +394,8 @@ static int gemm_impl(const int8_t* a_q, const float* a_s, const int8_t* b_q, con
   if (int rc = require_sm90()) return rc;
 
   const int64_t m_tiles = cdiv64(m, BM), n_tiles = cdiv64(n, BN);
-  if (m_tiles > 65535) return fail(TDB200_ERR_UNSUPPORTED, "gemm_w8a8: m=%lld exceeds %d rows", (long long)m, 65535 * BM);
+  if (m_tiles * n_tiles > (int64_t(1) << 30))   // int tile ids, with room for the grid stride past the last one
+    return fail(TDB200_ERR_UNSUPPORTED, "gemm_w8a8: m=%lld x n=%lld exceeds 2^30 output tiles", (long long)m, (long long)n);
   if (c_dtype != TDB200_DTYPE_BF16 && c_dtype != TDB200_DTYPE_FP16)
     return fail(TDB200_ERR_UNSUPPORTED, "gemm_w8a8: output dtype tag %d (bf16/fp16 only, gemm.cu:41-65)", c_dtype);
   CUtensorMap ta, tb;
@@ -414,12 +417,14 @@ static int gemm_impl(const int8_t* a_q, const float* a_s, const int8_t* b_q, con
   p.out_s = out_s;
   p.n_part = static_cast<int>(n / parts);
   p.k_blocks = static_cast<int>(k / BK);
+  p.n_tiles = static_cast<int>(n_tiles);
+  p.tiles = static_cast<int>(m_tiles * n_tiles);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (row_scale) {
     if (k > 16384 * 8) return fail(TDB200_ERR_UNSUPPORTED, "gemm_w8a8_rowwise: k too large for int32 accumulation");
-    if (c_dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16, true>(ta, tb, p, m_tiles, n_tiles, st);
-    return launch<__half, true>(ta, tb, p, m_tiles, n_tiles, st);
+    if (c_dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16, true>(ta, tb, p, st);
+    return launch<__half, true>(ta, tb, p, st);
   }
-  if (c_dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16, false>(ta, tb, p, m_tiles, n_tiles, st);
-  return launch<__half, false>(ta, tb, p, m_tiles, n_tiles, st);
+  if (c_dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16, false>(ta, tb, p, st);
+  return launch<__half, false>(ta, tb, p, st);
 }

@@ -14,6 +14,7 @@
  *   SLA.utils.get_block_map               turbodiffusion/SLA/utils.py:55-67           -> tdb200_sla_block_map
  *   spas_sage_attn get_vanilla_qk_quant   call site turbodiffusion/SLA/core.py:200-203 -> tdb200_sla_quant_qk
  *   Sage block-sparse attention + linear  turbodiffusion/SLA/core.py:231-253          -> tdb200_sla_linear_moments, tdb200_sla_attn_fwd
+ *   attention (dense SDPA / FlashAttention) turbodiffusion/rcm/utils/attention.py:120-167 -> tdb200_attn_dense_fwd
  *
  * Conventions
  *   - plain pointers and sizes; all pointers are DEVICE pointers unless stated; no allocation inside;
@@ -258,6 +259,24 @@ int tdb200_sla_attn_bwd_qk16(const void* q, const void* k, const void* v, const 
                              int dtype, const int32_t* lut, int64_t topk, void* dq, void* dk, void* dv, void* workspace,
                              int64_t workspace_bytes, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale, void* stream);
 int64_t tdb200_sla_attn_bwd_workspace_bytes(int64_t b, int64_t h, int64_t l, int64_t topk);
+
+/* ---------------------------------------------------------------------------------------------
+ * f1. Dense softmax attention, forward only: the block's cross-attention over the text tokens and `--attention_type original`
+ * (reference: the `attention` wrapper over FlashAttention / F.scaled_dot_product_attention, turbodiffusion/rcm/utils/attention.py:120-167,
+ * without its dropout, causal, window and variable-length arguments, which the denoise path leaves at their defaults).
+ *   out = T( softmax(q . k^T * sm_scale) . v )   per (batch, head)
+ * q, out [b, lq, h, d] and k, v [b, lk, h, d], contiguous 16-bit of type `dtype`, 16-byte aligned, read and written in place
+ * (row stride h*d: the [l, h*d] output of a projection GEMM is consumed as it is, no transposed copies).  lq and lk are
+ * independent and need not be multiples of anything: key columns >= lk are masked to -inf and query rows >= lq are not stored.
+ * Arithmetic, that of tdb200_sla_attn16_fwd's softmax part: S by wgmma into fp32, scores scaled by sm_scale * log2(e), online
+ * softmax with exp2 over 128-key tiles in ascending order, the row sum from the unrounded P, P rounded to T as the operand of
+ * P.V, fp32 accumulation, one rounding of O / l to T.  No atomics: the bits of a (batch, head) depend only on its own q, k, v.
+ * d = 128 only (d = 64 returns TDB200_ERR_UNSUPPORTED).  One kernel launch, no host synchronisation (capturable in a CUDA graph).
+ * Errors, all before any CUDA call: null or misaligned pointer, non-positive b, lq, lk, h or d -> TDB200_ERR_INVALID_ARG; bad
+ * dtype tag, d != 128, b or h above 65535, lq*h*d or lk*h*d of 2^39 elements or more -> TDB200_ERR_UNSUPPORTED.
+ * ------------------------------------------------------------------------------------------- */
+int tdb200_attn_dense_fwd(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq, int64_t lk,
+                          int64_t h, int64_t d, float sm_scale, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * a12. LTX-2 (TurboT2AV) prologue variants   (ltx_core/model/transformer/transformer.py:21-94; Triton fast path

@@ -1,0 +1,195 @@
+// Dense softmax attention forward, out = softmax(q.k^T * sm_scale).v, for 16-bit q [b, lq, h, d] and k, v [b, lk, h, d] read
+// in place through 4-D TMA tensor maps (the cross-attention over the text tokens, and the dense baseline of the SLA kernels).
+//   reference: the 'original' attention of rcm/utils/attention.py:120-167 (F.scaled_dot_product_attention / FlashAttention).
+// The arithmetic is the 16-bit SLA kernel's, step for step (sla_attn.cuh): S by wgmma into fp32, scores scaled by
+// sm_scale * log2e, exp2 online softmax with the lazy rescale, the row sum from the unrounded P, P rounded to T as the register
+// A operand of P.V, fp32 accumulation, out = T(O / l).
+//
+// One CTA per (128-row query block, head, batch): a producer warpgroup (one thread issues the TMA loads; setmaxnreg hands its
+// registers to the consumers) and two consumer warpgroups, warpgroup g owning query rows [64g, 64g + 64) of the block.  What the
+// sparse kernels carry and dense attention does not need is gone: key blocks are visited in order, so there is no LUT in shared
+// memory and no LUT read in the producer, no KVW tile and no linear-branch epilogue.  The shared memory that frees goes to
+// 128-row key tiles (wgmma.m64n128k16 scores: half the softmax rounds and barrier trips of a 64-row tile, which needs the
+// 232 registers setmaxnreg gives a consumer thread: O 64 + S 64 + P 32) on a 3-stage K ring and a 3-stage V ring:
+// Q 32 KB + 3 x (K 32 KB + V 32 KB) = 224 KB.  128 query rows per CTA, not 64: K and V do not fit on chip next to Q
+// (128 KB each per head at lk = 512), so every CTA streams all of K and V from L2, and 128 rows halve that traffic per FLOP.
+// Key columns >= lk are masked to -inf (their K and V rows are TMA zero fill, whatever memory holds there) and query rows >= lq
+// are not stored, so lq and lk need not be multiples of anything.  Every output row is written by one warpgroup that visits the
+// key tiles in ascending order: no atomics, and the bits of a (batch, head) depend only on its own q, k, v.
+#include <type_traits>
+
+#include "sla_attn.cuh"
+#include "host_common.h"
+
+namespace {
+using namespace tdb;
+
+constexpr int HD = 128, BQ = 128, BK = 128;
+constexpr int kStages = 3;
+constexpr int kConsumerWarps = 8;
+constexpr uint32_t kQBytes = BQ * HD * 2;      // HD/64 chunks of [BQ rows x 128 B]
+constexpr uint32_t kTileBytes = BK * HD * 2;   // K and V alike: HD/64 chunks of [BK keys x 128 B]
+constexpr uint32_t kOffQ = 0;
+constexpr uint32_t kOffK = kOffQ + kQBytes;
+constexpr uint32_t kOffV = kOffK + kStages * kTileBytes;
+constexpr uint32_t kOffBars = kOffV + kStages * kTileBytes;
+constexpr size_t kSmemBytes = 1024 + kOffBars + 256;   // 1024: the tiles are aligned inside the dynamic allocation
+static_assert(kSmemBytes <= 227 * 1024, "shared memory of the dense attention kernel");
+
+// both warpgroups consume every tile, so a slot has one full barrier and its empty barrier counts their eight warps
+enum Bar { kQFull = 0, kKFull = 1, kKEmpty = kKFull + kStages, kVFull = kKEmpty + kStages, kVEmpty = kVFull + kStages,
+           kNumBars = kVEmpty + kStages };
+static_assert(kNumBars * 8 <= 256, "barriers exceed their shared-memory slot");
+
+struct DenseParams {
+  void* out;   // [b, lq, h, d] T
+  int lq, lk, h;
+  float sm_scale;
+};
+
+template <typename T>
+__global__ void __launch_bounds__(split::kThreads, 1)
+dense_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                      const __grid_constant__ CUtensorMap tmap_v, DenseParams p) {
+  constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // 1024-aligned, stays a shared-space pointer
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
+  const int n_tiles = (p.lk + BK - 1) / BK;
+
+  if (threadIdx.x == 0) {
+    mbar_init(&bars[kQFull], 1);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&bars[kKFull + i], 1);
+      mbar_init(&bars[kKEmpty + i], kConsumerWarps);
+      mbar_init(&bars[kVFull + i], 1);
+      mbar_init(&bars[kVEmpty + i], kConsumerWarps);
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp >= kConsumerWarps) {
+    // =============================================================== TMA producer
+    reg_dealloc<split::kProducerRegs>();
+    if (warp == kConsumerWarps && lane == 0) {
+      tma_prefetch_desc(&tmap_q);
+      tma_prefetch_desc(&tmap_k);
+      tma_prefetch_desc(&tmap_v);
+      mbar_expect_tx(&bars[kQFull], kQBytes);
+#pragma unroll
+      for (int c = 0; c < HD / 64; ++c)
+        tma_load_4d(smem + kOffQ + c * (BQ * 128), &tmap_q, &bars[kQFull], c * 64, hh, m_blk * BQ, b);
+      for (int j = 0; j < n_tiles; ++j) {
+        const int st = j % kStages;
+        const uint32_t ph = ((j / kStages) & 1) ^ 1;
+        mbar_wait(&bars[kKEmpty + st], ph);
+        mbar_expect_tx(&bars[kKFull + st], kTileBytes);
+        uint8_t* sk = smem + kOffK + st * kTileBytes;
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c) tma_load_4d(sk + c * (BK * 128), &tmap_k, &bars[kKFull + st], c * 64, hh, j * BK, b);
+        mbar_wait(&bars[kVEmpty + st], ph);
+        mbar_expect_tx(&bars[kVFull + st], kTileBytes);
+        uint8_t* sv = smem + kOffV + st * kTileBytes;
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c) tma_load_4d(sv + c * (BK * 128), &tmap_v, &bars[kVFull + st], c * 64, hh, j * BK, b);
+      }
+    }
+    return;
+  }
+
+  // =============================================================== consumer warpgroups (64 query rows each, every key tile)
+  reg_alloc<split::kConsumerRegs>();
+  const int wg = warp >> 2, w4 = warp & 3;
+  const int r_lo = wg * 64 + w4 * 16 + (lane >> 2);   // rows r_lo and r_lo + 8 of the block (fragment layout, common.cuh)
+  const int cq = 2 * (lane & 3);                       // column pair offset inside every 8-column slice
+  const uint32_t sbase = smem_u32(smem);
+  const float sc = p.sm_scale * kLog2e;
+
+  float o[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+  float m_used[2] = {-INFINITY, -INFINITY}, l_part[2] = {0.f, 0.f};  // l_part: this thread's columns of the row sum
+
+  mbar_wait(&bars[kQFull], 0);
+  for (int j = 0; j < n_tiles; ++j) {
+    const int st = j % kStages;
+    const uint32_t ph = (j / kStages) & 1;
+
+    float s[BK / 2];
+    mbar_wait(&bars[kKFull + st], ph);
+    score_tile<true, HD, BK, kBF16>(s, sbase + kOffQ + wg * (64 * 128), BQ * 128, sbase + kOffK + st * kTileBytes, sc);
+    warp_release(&bars[kKEmpty + st], lane);
+    uint32_t pa[BK / 16][4];
+    softmax_step<T, HD, BK>(s, o, m_used, l_part, pa, p.lk - j * BK, cq, j == 0);   // valid < BK only in the ragged last tile
+    mbar_wait(&bars[kVFull + st], ph);
+    pv_step<HD, BK, kBF16>(o, pa, sbase + kOffV + st * kTileBytes);
+    warp_release(&bars[kVEmpty + st], lane);
+  }
+
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float l_tot = quad_sum(l_part[h]);   // all four lanes of a row take part, stored or not
+    const int64_t qr = int64_t(m_blk) * BQ + r_lo + 8 * h;
+    if (qr >= p.lq) continue;
+    store_o_row<T, HD>(static_cast<T*>(p.out) + ((int64_t(b) * p.lq + qr) * p.h + hh) * HD, o, h, 1.0f / l_tot, cq);
+  }
+}
+
+template <typename T>
+int launch(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const DenseParams& p, dim3 grid, cudaStream_t st) {
+  static bool smem_set[64];
+  const auto kern = dense_attn_fwd_kernel<T>;
+  if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), kSmemBytes, smem_set, "cudaFuncSetAttribute(dense_attn)"))
+    return rc;
+  kern<<<grid, split::kThreads, kSmemBytes, st>>>(tq, tk, tv, p);
+  return check_launch("dense_attn_fwd_kernel");
+}
+
+}  // namespace
+
+extern "C" int tdb200_attn_dense_fwd(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq,
+                                     int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
+  if (!q || !k || !v || !out) return fail(TDB200_ERR_INVALID_ARG, "attn_dense_fwd: null pointer");
+  if (b <= 0 || lq <= 0 || lk <= 0 || h <= 0 || d <= 0)
+    return fail(TDB200_ERR_INVALID_ARG, "attn_dense_fwd: bad shape (b=%lld, lq=%lld, lk=%lld, h=%lld, d=%lld)", (long long)b,
+                (long long)lq, (long long)lk, (long long)h, (long long)d);
+  if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out))
+    return fail(TDB200_ERR_INVALID_ARG, "attn_dense_fwd: q, k, v and out must be 16-byte aligned");
+  if (dtype != TDB200_DTYPE_BF16 && dtype != TDB200_DTYPE_FP16) return fail(TDB200_ERR_UNSUPPORTED, "attn_dense_fwd: dtype tag %d", dtype);
+  if (d != HD) return fail(TDB200_ERR_UNSUPPORTED, "attn_dense_fwd: head dim %lld (this kernel implements d=128)", (long long)d);
+  // grid (query blocks, h, b); int32 TMA coordinates; tensor-map strides below 2^40 bytes
+  constexpr int64_t kMaxStride = int64_t(1) << 40;
+  if (h > 65535 || b > 65535 || lq > 0x7FFFFFFF || lk > 0x7FFFFFFF || lq * h * d * 2 >= kMaxStride || lk * h * d * 2 >= kMaxStride)
+    return fail(TDB200_ERR_UNSUPPORTED, "attn_dense_fwd: dimension too large (b, h <= 65535; lq * h * d and lk * h * d below 2^39)");
+  if (int rc = require_sm90()) return rc;
+
+  const CUtensorMapDataType t16 = dtype == TDB200_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUtensorMap tq, tk, tv;
+  {
+    const uint64_t dims[4] = {uint64_t(d), uint64_t(h), uint64_t(lq), uint64_t(b)};
+    const uint64_t str[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(lq * h * d * 2)};
+    const uint32_t box[4] = {64, 1, BQ, 1};
+    if (int rc = make_tmap_4d(&tq, q, t16, 2, dims, str, box)) return rc;
+  }
+  {
+    const uint64_t dims[4] = {uint64_t(d), uint64_t(h), uint64_t(lk), uint64_t(b)};
+    const uint64_t str[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(lk * h * d * 2)};
+    const uint32_t box[4] = {64, 1, BK, 1};
+    if (int rc = make_tmap_4d(&tk, k, t16, 2, dims, str, box)) return rc;
+    if (int rc = make_tmap_4d(&tv, v, t16, 2, dims, str, box)) return rc;
+  }
+  DenseParams p;
+  p.out = out;
+  p.lq = int(lq);
+  p.lk = int(lk);
+  p.h = int(h);
+  p.sm_scale = sm_scale;
+  const dim3 grid(static_cast<unsigned>(cdiv64(lq, BQ)), static_cast<unsigned>(h), static_cast<unsigned>(b));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16>(tq, tk, tv, p, grid, st);
+  return launch<__half>(tq, tk, tv, p, grid, st);
+}

@@ -36,8 +36,6 @@ constexpr int kConsumerWarps = 8;
 constexpr int kThreads = kConsumerWarps * 32 + 32;
 constexpr int kStages = 3;
 static_assert(kStages == split::kStages, "the 64-row kernel uses the entry-split rings");
-constexpr float kLog2e = 1.4426950408889634f;
-constexpr float kRescaleThreshold = 8.0f;  // log2 domain
 
 template <int HD, bool kQK16, int kBQ = BLKQ, int kBK = BLKK>
 struct Lay {
@@ -75,108 +73,6 @@ __device__ __forceinline__ float feat(float x, float off_log2, int feature) {
   if (feature == 1) return x > 0.f ? x + 1.0f : fast_exp2(x * kLog2e);
   return fmaxf(x, 0.f);
 }
-__device__ __forceinline__ float quad_max(float v) {
-  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
-  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
-}
-__device__ __forceinline__ float quad_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  return v + __shfl_xor_sync(0xffffffffu, v, 2);
-}
-
-// ---- The per-entry steps of every forward kernel, on one warpgroup's 64 query rows.  Each thread holds rows r and r + 8 of
-//      the tiles (fragment layout, common.cuh); cq is its column pair offset inside every 8-column slice.
-
-// S = Q.K^T over the BK keys of one ring slot, scaled by sc into the log2 domain.  INT8: scores are int32 dot products (sc
-// folds in q_scale * k_scale), Q and K rows of HD bytes with a 128-byte swizzle for 128-wide heads and a 64-byte one for
-// 64-wide heads.  16-bit: fp32 scores, Q and K in HD/64 chunks of 128-byte rows, q_chunk bytes apart for Q.
-template <bool kQK16, int HD, int BK, bool kBF16>
-__device__ __forceinline__ void score_tile(float (&s)[BK / 2], uint32_t sq, uint32_t q_chunk, uint32_t sk, float sc) {
-  if constexpr (kQK16) {
-#pragma unroll
-    for (int i = 0; i < BK / 2; ++i) s[i] = 0.f;
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < HD / 16; ++ks) {  // K = 16 elements per MMA: chunk ks/4, +32 bytes per step inside the chunk
-      const uint64_t qd = make_desc_kmajor_sw128(sq + (ks >> 2) * q_chunk) + uint64_t((ks & 3) * 2);
-      const uint64_t kd = make_desc_kmajor_sw128(sk + (ks >> 2) * (BK * 128)) + uint64_t((ks & 3) * 2);
-      wgmma_f16_ss<BK, kBF16>(s, qd, kd, ks > 0 ? 1u : 0u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(s);
-#pragma unroll
-    for (int i = 0; i < BK / 2; ++i) s[i] *= sc;
-  } else {
-    uint32_t si[BK / 2];
-#pragma unroll
-    for (int i = 0; i < BK / 2; ++i) si[i] = 0u;
-    const uint64_t qdesc = HD == 128 ? make_desc_kmajor_sw128(sq) : make_desc_kmajor_sw64(sq);
-    const uint64_t kdesc = HD == 128 ? make_desc_kmajor_sw128(sk) : make_desc_kmajor_sw64(sk);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < HD / 32; ++ks)
-      wgmma_i8_ss<BK>(si, qdesc + uint64_t(ks * 2), kdesc + uint64_t(ks * 2), ks > 0 ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(si);
-#pragma unroll
-    for (int i = 0; i < BK / 2; ++i) s[i] = static_cast<float>(static_cast<int>(si[i])) * sc;
-  }
-}
-
-// One online-softmax step: key columns from `valid` on do not exist (the ragged last key block), then the row maxima and the
-// lazy rescale of O and the row sums (per row: alpha == 1 exactly where the maximum is kept), then P = exp2(s - m_used) into
-// the A fragments of P.V.  The row sum is taken from the unrounded P, the tensor core gets P rounded to T.  `first`: the first
-// entry of this warpgroup, which sets the maxima.
-template <typename T, int HD, int BK>
-__device__ __forceinline__ void softmax_step(float (&s)[BK / 2], float (&o)[HD / 2], float (&m_used)[2], float (&l_part)[2],
-                                             uint32_t (&pa)[BK / 16][4], int valid, int cq, bool first) {
-  if (valid < BK) {
-#pragma unroll
-    for (int i = 0; i < BK / 2; ++i)
-      if (8 * (i >> 2) + cq + (i & 1) >= valid) s[i] = -INFINITY;
-  }
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    float mx = -INFINITY;
-#pragma unroll
-    for (int i = 0; i < BK / 2; ++i)
-      if (((i >> 1) & 1) == h) mx = fmaxf(mx, s[i]);
-    mx = quad_max(mx);
-    if (first) {
-      m_used[h] = mx;
-    } else if (mx > m_used[h] + kRescaleThreshold) {
-      const float alpha = fast_exp2(m_used[h] - mx);
-#pragma unroll
-      for (int i = 0; i < HD / 2; ++i)
-        if (((i >> 1) & 1) == h) o[i] *= alpha;
-      l_part[h] *= alpha;
-      m_used[h] = mx;
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < BK / 2; i += 2) {
-    const int h = (i >> 1) & 1;
-    const float p0 = fast_exp2(s[i] - m_used[h]), p1 = fast_exp2(s[i + 1] - m_used[h]);
-    l_part[h] += p0 + p1;
-    pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0, p1);
-  }
-}
-
-// O += P.V  (V: [BK keys x HD], HD/64 MN-major chunks of BK x 128 B, so no transposed copy of V; +16 keys = +2048 B per K step)
-template <int HD, int BK, bool kBF16>
-__device__ __forceinline__ void pv_step(float (&o)[HD / 2], uint32_t (&pa)[BK / 16][4], uint32_t sv) {
-  const uint64_t vdesc = make_desc_mnmajor_sw128(sv, BK * 128);
-  wgmma_fence();
-#pragma unroll
-  for (int kk = 0; kk < BK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(o, pa[kk], vdesc + uint64_t(kk * 128));
-  wgmma_commit();
-  wgmma_wait<0>();
-  reg_fence(o);
-#pragma unroll
-  for (int kk = 0; kk < BK / 16; ++kk) reg_fence(pa[kk]);
-}
 
 // kLse epilogue: out = T(O / l) and lse[b,h,row] = m_used + log2(l), the row log-sum-exp of the scores in the kernel's log2
 // domain, for rows qrow0 + {0, 8}.
@@ -189,10 +85,7 @@ __device__ __forceinline__ void store_o_lse(const float (&o)[HD / 2], const floa
     if (qr >= p.l) continue;
     const float l_tot = quad_sum(l_part[h]), inv_l = 1.0f / l_tot;
     if (cq == 0) p.lse[int64_t(bh) * p.l + qr] = m_used[h] + __log2f(l_tot);
-    T* orow = static_cast<T*>(p.out) + ((int64_t(b) * p.l + qr) * p.h + hh) * HD;
-#pragma unroll
-    for (int c = 0; c < HD / 8; ++c)
-      *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) = F16Traits<T>::pack(o[4 * c + 2 * h] * inv_l, o[4 * c + 2 * h + 1] * inv_l);
+    store_o_row<T, HD>(static_cast<T*>(p.out) + ((int64_t(b) * p.l + qr) * p.h + hh) * HD, o, h, inv_l, cq);
   }
 }
 

@@ -28,7 +28,6 @@ namespace {
 using namespace tdb;
 
 constexpr int HD = 128, BLKQ = 128, BLKQ64 = 64, BLKK = 64;
-constexpr float kLog2e = 1.4426950408889634f;
 
 struct BwdParams {
   const float* lse;        // [b,h,l]

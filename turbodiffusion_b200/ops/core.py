@@ -14,7 +14,7 @@ import torch
 import torch.nn as nn
 
 from .. import _ops
-from .._lib import DTYPE_TAG, require_cuda
+from .._lib import DTYPE_TAG, check, lib, ptr, require_cuda, stream_ptr
 from ..turbo_diffusion_ops import quant_cuda, gemm_cuda, gemm_cuda_swizzle_bias
 
 
@@ -333,3 +333,22 @@ def wan_rope_angles(t: int, h: int, w: int, head_dim: int, device=None) -> torch
     out = torch.cat([ft[:, None, None, :].expand(t, h, w, -1), fh[None, :, None, :].expand(t, h, w, -1),
                      fw[None, None, :, :].expand(t, h, w, -1)], dim=-1).reshape(t * h * w, head_dim // 2).float().contiguous()
     return out if device is None else out.to(device)
+
+
+def dense_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, sm_scale: Optional[float] = None) -> torch.Tensor:
+    """softmax(q.k^T * sm_scale).v per (batch, head), the reference's dense attention (rcm/utils/attention.py:120-167):
+    q [B, Lq, H, D], k and v [B, Lk, H, D], D = 128, any Lq and Lk; returns [B, Lq, H, D] in q's dtype.  bf16 / fp16 inputs run
+    in their own type, any other float type in bf16.  sm_scale defaults to D ** -0.5.  One kernel on the current stream
+    (tdb200_attn_dense_fwd), the arithmetic of the 16-bit SLA kernel.  Forward only, and not a `tdb200::` operator: eager use."""
+    require_cuda(q, k, v)
+    if q.dim() != 4 or k.shape != v.shape or k.dim() != 4 or (q.shape[0], *q.shape[2:]) != (k.shape[0], *k.shape[2:]):
+        raise ValueError(f"dense_attention: q [B, Lq, H, D] and k, v [B, Lk, H, D] expected, got {tuple(q.shape)}, "
+                         f"{tuple(k.shape)}, {tuple(v.shape)}")
+    dtype = q.dtype if q.dtype in DTYPE_TAG else torch.bfloat16
+    qc, kc, vc = (t.to(dtype).contiguous() for t in (q, k, v))
+    b, lq, h, d = qc.shape
+    out = torch.empty_like(qc)
+    check(lib().tdb200_attn_dense_fwd(ptr(qc), ptr(kc), ptr(vc), DTYPE_TAG[dtype], ptr(out), b, lq, kc.shape[1], h, d,
+                                      float(d ** -0.5 if sm_scale is None else sm_scale), stream_ptr(qc.device)),
+          "attn_dense_fwd")
+    return out.to(q.dtype)

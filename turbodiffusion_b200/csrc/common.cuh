@@ -131,6 +131,11 @@ template <int kKeep>
 __device__ __forceinline__ void tma_store_wait_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(kKeep) : "memory");
 }
+// all but the newest kKeep store groups of this thread have completed (their global writes included)
+template <int kKeep>
+__device__ __forceinline__ void tma_store_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(kKeep) : "memory");
+}
 
 // ------------------------------------------------------------------------------------------
 // thread-block clusters

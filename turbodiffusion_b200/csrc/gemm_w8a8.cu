@@ -24,6 +24,13 @@
 //            and in the block-scale variant not multiplied either.  Each warpgroup loops over the tiles on its own with
 //            the same running K-block counter; only the quantised epilogue's amax exchange makes the two meet, so
 //            otherwise one warpgroup's epilogue overlaps the other's MMAs once they drift apart.
+//   The store: each consumer warpgroup writes its 64 rows of a half into its own 16 KB shared-memory buffer (after the
+//            ring: 4 x 48 KB + 2 x 16 KB + barriers = 230,656 B of the 232,448 B opt-in), in the 128B-swizzled layout of
+//            a TMA box, and one of its threads stores the boxes with cp.async.bulk.tensor: whole 128-byte lines instead
+//            of 4,096 partial-sector STGs per tile, issued asynchronously, so the warpgroup goes on to its next tile's
+//            MMAs while they drain.  The buffer is waited on (wait_group.read) only before it is written again.  The
+//            output tensor maps clip rows >= m, columns >= n and a split output's parts, so the epilogue has no
+//            per-element predicates.
 // Integer accumulation is exact and the fp32 FMA chain runs in ascending kb order, so the result is bit-identical
 // to the reference restatement (oracle.int8_linear) on the same int8 inputs.
 #include "common.cuh"
@@ -42,7 +49,11 @@ constexpr uint32_t kProducerRegs = 40, kConsumerRegs = 232;   // 128 * 40 + 256 
 constexpr uint32_t kATile = BM * BK;                 // 16 KB
 constexpr uint32_t kBTile = BN * BK;                 // 32 KB: half h at +16 KB h
 constexpr uint32_t kStageBytes = kATile + kBTile;
-constexpr size_t kSmemBytes = 1024 + size_t(kStages) * kStageBytes + 256 /*barriers 64 B + amax exchange 128 B*/;
+constexpr uint32_t kOutBox = 64 * 128;               // one 128B-swizzled TMA store box: 64 rows x 128 B
+constexpr uint32_t kOutWg = 2 * kOutBox;             // a warpgroup's staging buffer: 64 rows x one half in 16 bits
+constexpr size_t kSmemBytes =
+    1024 + size_t(kStages) * kStageBytes + 2 * kOutWg + 256 /*barriers 64 B + amax exchange 128 B*/;   // 230,656 B
+static_assert(kSmemBytes <= 232448, "over the sm_90 opt-in shared memory per block");
 
 struct GemmParams {
   const float* a_s;
@@ -85,10 +96,12 @@ __device__ __forceinline__ float gelu_precise(float x) {
 // c = T(float(acc) * a_s[i] * b_s[j] + bias[j]).
 template <typename T, bool kRowScale>
 __global__ void __launch_bounds__(kThreads, 1)
-gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, GemmParams p) {
+gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                 const __grid_constant__ CUtensorMap tmap_c, GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // 1024-aligned, stays a shared-space pointer
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + size_t(kStages) * kStageBytes);
+  uint8_t* out_stage = smem + size_t(kStages) * kStageBytes;                      // [2 warpgroups][kOutWg]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(out_stage + 2 * kOutWg);
   uint64_t* full_bar = bars;                // [kStages]  TMA -> MMA
   uint64_t* empty_bar = bars + kStages;     // [kStages]  MMA -> TMA (one arrival per consumer warp)
   float* amax_x = reinterpret_cast<float*>(bars + 2 * kStages);  // [2][2][kConsumerWarps] block-amax exchange: tile parity, half
@@ -155,6 +168,39 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const T* bias = static_cast<const T*>(p.bias);
   const bool act_gelu = p.act == 1;
 
+  // Output staging.  Warpgroup wg's buffer holds its 64 rows of one half: two {64 columns x 64 rows} boxes of T, or for
+  // the int8 output one {128 B x 64 rows} box per half, each in the 128B-swizzled layout of the TMA map: row r at 128 r,
+  // its 16-byte chunk c at chunk c ^ (r & 7).  A warp's store of one register covers 8 rows x 16 bytes that land in 8
+  // different chunks, so it is free of bank conflicts.  One thread per warpgroup issues the TMA stores; the bulk groups it
+  // commits are its own, so it alone can wait for them, and the warpgroup's named barrier passes that on.
+  uint8_t* const stage_wg = out_stage + wg * kOutWg;
+  const bool issuer = (threadIdx.x & 127) == 0;
+  const uint32_t wg_bar = 2 + wg;   // barrier 0 is __syncthreads, 1 the amax exchange of both warpgroups
+  const int32_t row_wg = wg * 64;   // + m_tile * BM: the first output row of this warpgroup's boxes
+  // byte offset of (row 8 h + the thread's fragment row, byte column bc < 128) inside a box
+  auto box_off = [&](int h, int bc) -> uint32_t {
+    return uint32_t(w4 * 16 + 8 * h + (lane >> 2)) * 128u + ((((bc >> 4) ^ (lane >> 2)) << 4) | (bc & 15));
+  };
+  if (issuer) tma_prefetch_desc(&tmap_c);
+  // one half of 16-bit output, yw[2 j + h] = the T pair at fragment row h, columns 8 j + cq (+1), stored at column `col`
+  // of output part `part`; the map clips rows >= m and columns >= n_part
+  auto store16 = [&](const uint32_t (&yw)[BH / 4], int32_t col, int32_t row, int32_t part) {
+    if (issuer) tma_store_wait_read<0>();   // the previous half's boxes have left the buffer
+    named_bar_sync(wg_bar, 128);
+#pragma unroll
+    for (int j = 0; j < BH / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        *reinterpret_cast<uint32_t*>(stage_wg + (j >> 3) * kOutBox + box_off(h, 16 * (j & 7) + 2 * cq)) = yw[2 * j + h];
+    fence_proxy_async_smem();
+    named_bar_sync(wg_bar, 128);
+    if (issuer) {
+      tma_store_4d(&tmap_c, stage_wg, col, row, part, 0);
+      tma_store_4d(&tmap_c, stage_wg + kOutBox, col + 64, row, part, 0);
+      tma_store_commit();
+    }
+  };
+
   uint32_t it0 = 0;       // the running K-block count at the start of the tile
   uint32_t parity = 0;    // of this CTA's tile count: selects the amax exchange slots
   for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x, it0 += p.k_blocks, parity ^= 1u) {
@@ -186,21 +232,22 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       const float sa0 = row0 < p.m ? __ldg(p.a_s + row0) : 0.f, sa1 = row1 < p.m ? __ldg(p.a_s + row1) : 0.f;
       auto store = [&](const uint32_t (&ia)[64], int hf) {
         const int64_t col_base = int64_t(n_tile) * BN + hf * BH + cq;
+        uint32_t yw[BH / 4];
 #pragma unroll
         for (int j = 0; j < BH / 8; ++j) {
           const int64_t col = col_base + 8 * j;
-          if (col >= p.n) continue;
-          const float sb0 = __ldg(p.b_s + col), sb1 = __ldg(p.b_s + col + 1);
-          const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
+          const bool in = col < p.n;   // columns >= n are clipped by the store
+          const float sb0 = in ? __ldg(p.b_s + col) : 0.f, sb1 = in ? __ldg(p.b_s + col + 1) : 0.f;
+          const uint32_t bw = bias != nullptr && in ? __ldg(reinterpret_cast<const unsigned int*>(bias + col)) : 0u;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const float sa = h ? sa1 : sa0;
             const float y0 = __fmaf_rn(__fmul_rn(__int2float_rn(static_cast<int>(ia[4 * j + 2 * h])), sa), sb0, F16Traits<T>::lo(bw));
             const float y1 = __fmaf_rn(__fmul_rn(__int2float_rn(static_cast<int>(ia[4 * j + 2 * h + 1])), sa), sb1, F16Traits<T>::hi(bw));
-            const int64_t row = h ? row1 : row0;
-            if (row < p.m) *reinterpret_cast<uint32_t*>(static_cast<T*>(p.c) + row * p.n + col) = F16Traits<T>::pack(y0, y1);
+            yw[2 * j + h] = F16Traits<T>::pack(y0, y1);
           }
         }
+        store16(yw, n_tile * BN + hf * BH, m_tile * BM + row_wg, 0);
       };
       store(ia0, 0);
       if (has_hi) store(ia1, 1);
@@ -266,23 +313,30 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         // by the next tile's write to the same ones.  The parity bit costs 64 bytes and no extra barrier.
         float* xch = amax_x + (parity * 2 + hf) * kConsumerWarps;
         if (lane == 0) xch[warp] = amax;
+        // Both halves' codes fit in the buffer (8 KB each), so only the first half waits, for the previous tile's boxes,
+        // and the exchange barrier tells the warpgroup.
+        if (issuer && hf == 0) tma_store_wait_read<0>();
         named_bar_sync(1, kConsumerWarps * 32);
 #pragma unroll
         for (int w = 0; w < kConsumerWarps; ++w) amax = fmaxf(amax, xch[w]);
         const float r = __fdiv_rn(128.0f, amax);
         if (threadIdx.x == 0) p.out_s[int64_t(m_tile) * (p.n >> 7) + 2 * n_tile + hf] = amax * 0.0078125f;
+        uint8_t* const box = stage_wg + hf * kOutBox;
 #pragma unroll
         for (int j = 0; j < BH / 8; ++j) {
-          const int64_t col = col_base + 8 * j;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const uint32_t y = yw[2 * j + h];
             const int q0 = __float2int_rn(fminf(__fmul_rn(F16Traits<T>::lo(y), r), 127.0f));
             const int q1 = __float2int_rn(fminf(__fmul_rn(F16Traits<T>::hi(y), r), 127.0f));
-            const int64_t row = h ? row1 : row0;
-            if (row < p.m)
-              *reinterpret_cast<uint16_t*>(p.out_q + row * p.n + col) = static_cast<uint16_t>((q0 & 0xFF) | ((q1 & 0xFF) << 8));
+            *reinterpret_cast<uint16_t*>(box + box_off(h, 8 * j + cq)) = static_cast<uint16_t>((q0 & 0xFF) | ((q1 & 0xFF) << 8));
           }
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(wg_bar, 128);
+        if (issuer) {   // rows >= m are clipped by the map
+          tma_store_2d(&tmap_c, box, n_tile * BN + hf * BH, m_tile * BM + row_wg);
+          tma_store_commit();
         }
       };
       store_q(acc0, 0);
@@ -291,39 +345,43 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     }
     // a tile lies inside one output part (n_part is n itself or a multiple of 256): one division per tile, not per column
     const int part = n_tile * BN / p.n_part;
-    T* c_part = static_cast<T*>(p.c) + int64_t(part) * p.m * p.n_part - int64_t(part) * p.n_part;
     auto store = [&](const float (&acc)[64], int hf) {
       const int64_t col_base = int64_t(n_tile) * BN + hf * BH + cq;
+      // all of the half's bias words are loaded before any value is staged
+      uint32_t bw[BH / 8];
 #pragma unroll
       for (int j = 0; j < BH / 8; ++j) {
         const int64_t col = col_base + 8 * j;
-        if (col >= p.n) continue;
-        const uint32_t bw = bias != nullptr ? *reinterpret_cast<const uint32_t*>(bias + col) : 0u;
-        T* cp = c_part + col;
+        bw[j] = bias != nullptr && col < p.n ? __ldg(reinterpret_cast<const unsigned int*>(bias + col)) : 0u;
+      }
+      uint32_t yw[BH / 4];
+#pragma unroll
+      for (int j = 0; j < BH / 8; ++j) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           // T(acc) then the packed 16-bit add: one rounding each, exactly the module's `out + bias` on 16-bit tensors
           uint32_t y = F16Traits<T>::pack(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-          if (bias != nullptr) y = F16Traits<T>::add2(y, bw);
+          if (bias != nullptr) y = F16Traits<T>::add2(y, bw[j]);
           if (act_gelu) y = F16Traits<T>::pack(gelu_precise(F16Traits<T>::lo(y)), gelu_precise(F16Traits<T>::hi(y)));
-          const int64_t row = h ? row1 : row0;
-          if (row < p.m) *reinterpret_cast<uint32_t*>(cp + row * p.n_part) = y;
+          yw[2 * j + h] = y;
         }
       }
+      store16(yw, n_tile * BN + hf * BH - part * p.n_part, m_tile * BM + row_wg, part);
     };
     store(acc0, 0);
     if (has_hi) store(acc1, 1);
   }
+  if (issuer) tma_store_wait<0>();   // the staging buffers must outlive the stores that read them
 }
 
 template <typename T, bool kRowScale>
-int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st) {
+int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const GemmParams& p, cudaStream_t st) {
   auto kern = gemm_w8a8_kernel<T, kRowScale>;
   static bool attr_done[64] = {false};
   if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), kSmemBytes, attr_done,
                                          "cudaFuncSetAttribute(gemm_w8a8)"))
     return rc;
-  kern<<<std::min(p.tiles, sm_count()), kThreads, kSmemBytes, st>>>(ta, tb, p);
+  kern<<<std::min(p.tiles, sm_count()), kThreads, kSmemBytes, st>>>(ta, tb, tc, p);
   return check_launch("gemm_w8a8_kernel");
 }
 
@@ -403,6 +461,20 @@ static int gemm_impl(const int8_t* a_q, const float* a_s, const int8_t* b_q, con
     return rc;
   if (int rc = make_tmap_2d(&tb, b_q, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, uint64_t(k), uint64_t(n), uint64_t(k), BK, BN))
     return rc;
+  // the output, stored from 64-row boxes: int8 codes [m, n] in 128-byte boxes, or the 16-bit c as (n_part, m, parts) in
+  // 64-column boxes, so that a part's last rows and the columns past n are clipped rather than written into the next
+  CUtensorMap tc;
+  if (out_q) {
+    if (int rc = make_tmap_2d(&tc, out_q, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, uint64_t(n), uint64_t(m), uint64_t(n), 128, 64))
+      return rc;
+  } else {
+    const uint64_t np = uint64_t(n / parts);
+    const uint64_t dims[4] = {np, uint64_t(m), uint64_t(parts), 1};
+    const uint64_t strides[3] = {2 * np, 2 * np * uint64_t(m), 2 * uint64_t(n) * uint64_t(m)};
+    const uint32_t box[4] = {64, 64, 1, 1};
+    const CUtensorMapDataType t16 = c_dtype == TDB200_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    if (int rc = make_tmap_4d(&tc, c, t16, 2, dims, strides, box)) return rc;
+  }
 
   GemmParams p;
   p.a_s = a_s;
@@ -422,9 +494,9 @@ static int gemm_impl(const int8_t* a_q, const float* a_s, const int8_t* b_q, con
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (row_scale) {
     if (k > 16384 * 8) return fail(TDB200_ERR_UNSUPPORTED, "gemm_w8a8_rowwise: k too large for int32 accumulation");
-    if (c_dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16, true>(ta, tb, p, st);
-    return launch<__half, true>(ta, tb, p, st);
+    if (c_dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16, true>(ta, tb, tc, p, st);
+    return launch<__half, true>(ta, tb, tc, p, st);
   }
-  if (c_dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16, false>(ta, tb, p, st);
-  return launch<__half, false>(ta, tb, p, st);
+  if (c_dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16, false>(ta, tb, tc, p, st);
+  return launch<__half, false>(ta, tb, tc, p, st);
 }

@@ -15,6 +15,7 @@
  *   spas_sage_attn get_vanilla_qk_quant   call site turbodiffusion/SLA/core.py:200-203 -> tdb200_sla_quant_qk
  *   Sage block-sparse attention + linear  turbodiffusion/SLA/core.py:231-253          -> tdb200_sla_linear_moments, tdb200_sla_attn_fwd
  *   attention (dense SDPA / FlashAttention) turbodiffusion/rcm/utils/attention.py:120-167 -> tdb200_attn_dense_fwd
+ *   JVP flash attention (rCM distillation) turbodiffusion/rcm/networks/wan2pt1_jvp.py -> tdb200_attn_dense_jvp
  *
  * Conventions
  *   - plain pointers and sizes; all pointers are DEVICE pointers unless stated; no allocation inside;
@@ -277,6 +278,25 @@ int64_t tdb200_sla_attn_bwd_workspace_bytes(int64_t b, int64_t h, int64_t l, int
  * ------------------------------------------------------------------------------------------- */
 int tdb200_attn_dense_fwd(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq, int64_t lk,
                           int64_t h, int64_t d, float sm_scale, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * f1 JVP. Forward-mode derivative of the dense attention above (rCM distillation's tangent pass, reference
+ * turbodiffusion/rcm/networks/wan2pt1_jvp.py): the attention output and its tangent for tangents q_t, k_t, v_t, in one kernel.
+ *   S = sm_scale q.k^T,  S_t = sm_scale (q_t.k^T + q.k_t^T),  P = softmax(S),  out = T(P.v)
+ *   out_t = T( sum_j P_j S_t,j v_j - (sum_j P_j S_t,j) out + P.v_t )   per (batch, head) and query row
+ * q, q_t, out, out_t [b, lq, h, d] and k, v, k_t, v_t [b, lk, h, d], contiguous 16-bit of type `dtype` (tangents included),
+ * 16-byte aligned, read and written in place; key columns >= lk are masked and query rows >= lq are stored to neither output.
+ * Arithmetic: the online softmax of tdb200_attn_dense_fwd over 64-key tiles, with two more accumulators per row,
+ * A = sum p (S_t v + v_t) and mu = sum p S_t, rescaled with O and l; l and mu sum the unrounded p and p S_t, the tensor core
+ * gets p and p S_t rounded to T; out = T(O / l), out_t = T((A - (mu / l) O) / l).  No atomics: the bits of a (batch, head)
+ * depend only on its own inputs.  d = 128 only.  One kernel launch, no workspace, no host synchronisation.
+ * Errors, all before any CUDA call: any of the eight pointers null or misaligned, non-positive b, lq, lk, h or d ->
+ * TDB200_ERR_INVALID_ARG; bad dtype tag, d != 128, b or h above 65535, lq*h*d or lk*h*d of 2^39 elements or more ->
+ * TDB200_ERR_UNSUPPORTED.
+ * ------------------------------------------------------------------------------------------- */
+int tdb200_attn_dense_jvp(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                          int dtype, void* out, void* out_t, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d,
+                          float sm_scale, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * a12. LTX-2 (TurboT2AV) prologue variants   (ltx_core/model/transformer/transformer.py:21-94; Triton fast path

@@ -149,6 +149,252 @@ int launch(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, 
   return check_launch("dense_attn_fwd_kernel");
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Forward-mode derivative (JVP): o = softmax(S).v and its tangent od for tangents qd, kd, vd of q, k, v, with S = c q.k^T and
+// Sd = c (qd.k^T + q.kd^T), c = sm_scale:
+//   od = sum_j P_j Sd_j v_j - (sum_j P_j Sd_j) o + P.vd.
+// With the online softmax and p = exp2(s - m) unnormalised, each warpgroup row keeps l = sum p and O = sum p v as the forward
+// does, plus A = sum p (Sd v + vd) and mu = sum p Sd; the lazy rescale scales all four, and at the end o = O / l and
+// od = (A - (mu / l) O) / l.  Per 64-key tile: S by wgmma and the softmax, which leaves p in fp32 in S's registers; then Sd as
+// one commit group (O 64 + A 64 + p 32 + Sd 32 fp32 registers per thread at the peak; issuing S and Sd together so that the
+// softmax overlaps Sd's MMAs spilled); l and mu sum the unrounded p and p Sd, the tensor core gets p and
+// p Sd rounded to T; then O += P.V, A += (P Sd).V and A += P.Vd as one commit group.
+// CTA per (128-row query block, head, batch), the forward's warp roles.  Shared memory: Q and Qd resident (64 KB), a 2-stage
+// (K, Kd) ring and a 2-stage (V, Vd) ring of 32 KB per stage: 192 KB.  A third stage of both rings would need 256 KB.
+namespace jvp {
+constexpr int BK = 64;
+constexpr int kStages = 2;
+constexpr uint32_t kQBytes = BQ * HD * 2;           // Q and Qd alike
+constexpr uint32_t kHalfBytes = BK * HD * 2;        // one of K, Kd, V, Vd: HD/64 chunks of [BK keys x 128 B]
+constexpr uint32_t kStageBytes = 2 * kHalfBytes;    // (K, Kd) or (V, Vd)
+constexpr uint32_t kOffQ = 0, kOffQd = kQBytes;
+constexpr uint32_t kOffK = 2 * kQBytes;
+constexpr uint32_t kOffV = kOffK + kStages * kStageBytes;
+constexpr uint32_t kOffBars = kOffV + kStages * kStageBytes;
+constexpr size_t kSmemBytes = 1024 + kOffBars + 256;
+static_assert(kSmemBytes <= 227 * 1024, "shared memory of the dense attention JVP kernel");
+
+enum Bar { kQFull = 0, kKFull = 1, kKEmpty = kKFull + kStages, kVFull = kKEmpty + kStages, kVEmpty = kVFull + kStages,
+           kNumBars = kVEmpty + kStages };
+static_assert(kNumBars * 8 <= 256, "barriers exceed their shared-memory slot");
+
+struct Params {
+  void* out;     // [b, lq, h, d] T
+  void* out_t;   // [b, lq, h, d] T
+  int lq, lk, h;
+  float sm_scale;
+};
+
+// d (+)= Q.K^T over one 64-key tile: Q rows at sq (HD/64 chunks kQBytes/2 apart), K at sk (chunks BK * 128 bytes apart)
+template <bool kBF16>
+__device__ __forceinline__ void qk_mmas(float (&d)[BK / 2], uint32_t sq, uint32_t sk, bool accumulate) {
+#pragma unroll
+  for (int ks = 0; ks < HD / 16; ++ks) {
+    const uint64_t qd = make_desc_kmajor_sw128(sq + (ks >> 2) * (BQ * 128)) + uint64_t((ks & 3) * 2);
+    const uint64_t kd = make_desc_kmajor_sw128(sk + (ks >> 2) * (BK * 128)) + uint64_t((ks & 3) * 2);
+    wgmma_f16_ss<BK, kBF16>(d, qd, kd, (accumulate || ks > 0) ? 1u : 0u);
+  }
+}
+
+// softmax_step's masking, maxima and lazy rescale, with A and mu rescaled beside O and l; leaves p = exp2(s - m_used) in s
+__device__ __forceinline__ void softmax_step_jvp(float (&s)[BK / 2], float (&o)[HD / 2], float (&a)[HD / 2], float (&m_used)[2],
+                                                 float (&l_part)[2], float (&mu_part)[2], int valid, int cq, bool first) {
+  if (valid < BK) {
+#pragma unroll
+    for (int i = 0; i < BK / 2; ++i)
+      if (8 * (i >> 2) + cq + (i & 1) >= valid) s[i] = -INFINITY;
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float mx = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < BK / 2; ++i)
+      if (((i >> 1) & 1) == h) mx = fmaxf(mx, s[i]);
+    mx = quad_max(mx);
+    if (first) {
+      m_used[h] = mx;
+    } else if (mx > m_used[h] + kRescaleThreshold) {
+      const float alpha = fast_exp2(m_used[h] - mx);
+#pragma unroll
+      for (int i = 0; i < HD / 2; ++i)
+        if (((i >> 1) & 1) == h) {
+          o[i] *= alpha;
+          a[i] *= alpha;
+        }
+      l_part[h] *= alpha;
+      mu_part[h] *= alpha;
+      m_used[h] = mx;
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < BK / 2; i += 2) {
+    const int h = (i >> 1) & 1;
+    s[i] = fast_exp2(s[i] - m_used[h]);
+    s[i + 1] = fast_exp2(s[i + 1] - m_used[h]);
+    l_part[h] += s[i] + s[i + 1];
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(split::kThreads, 1)
+dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                      const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_qt,
+                      const __grid_constant__ CUtensorMap tmap_kt, const __grid_constant__ CUtensorMap tmap_vt, Params p) {
+  constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
+  const int n_tiles = (p.lk + BK - 1) / BK;
+
+  if (threadIdx.x == 0) {
+    mbar_init(&bars[kQFull], 1);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&bars[kKFull + i], 1);
+      mbar_init(&bars[kKEmpty + i], kConsumerWarps);
+      mbar_init(&bars[kVFull + i], 1);
+      mbar_init(&bars[kVEmpty + i], kConsumerWarps);
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp >= kConsumerWarps) {
+    // =============================================================== TMA producer
+    reg_dealloc<split::kProducerRegs>();
+    if (warp == kConsumerWarps && lane == 0) {
+      tma_prefetch_desc(&tmap_q);
+      tma_prefetch_desc(&tmap_qt);
+      tma_prefetch_desc(&tmap_k);
+      tma_prefetch_desc(&tmap_kt);
+      tma_prefetch_desc(&tmap_v);
+      tma_prefetch_desc(&tmap_vt);
+      mbar_expect_tx(&bars[kQFull], 2 * kQBytes);
+#pragma unroll
+      for (int c = 0; c < HD / 64; ++c) {
+        tma_load_4d(smem + kOffQ + c * (BQ * 128), &tmap_q, &bars[kQFull], c * 64, hh, m_blk * BQ, b);
+        tma_load_4d(smem + kOffQd + c * (BQ * 128), &tmap_qt, &bars[kQFull], c * 64, hh, m_blk * BQ, b);
+      }
+      for (int j = 0; j < n_tiles; ++j) {
+        const int st = j % kStages;
+        const uint32_t ph = ((j / kStages) & 1) ^ 1;
+        mbar_wait(&bars[kKEmpty + st], ph);
+        mbar_expect_tx(&bars[kKFull + st], kStageBytes);
+        uint8_t* sk = smem + kOffK + st * kStageBytes;
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c) {
+          tma_load_4d(sk + c * (BK * 128), &tmap_k, &bars[kKFull + st], c * 64, hh, j * BK, b);
+          tma_load_4d(sk + kHalfBytes + c * (BK * 128), &tmap_kt, &bars[kKFull + st], c * 64, hh, j * BK, b);
+        }
+        mbar_wait(&bars[kVEmpty + st], ph);
+        mbar_expect_tx(&bars[kVFull + st], kStageBytes);
+        uint8_t* sv = smem + kOffV + st * kStageBytes;
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c) {
+          tma_load_4d(sv + c * (BK * 128), &tmap_v, &bars[kVFull + st], c * 64, hh, j * BK, b);
+          tma_load_4d(sv + kHalfBytes + c * (BK * 128), &tmap_vt, &bars[kVFull + st], c * 64, hh, j * BK, b);
+        }
+      }
+    }
+    return;
+  }
+
+  // =============================================================== consumer warpgroups (64 query rows each, every key tile)
+  reg_alloc<split::kConsumerRegs>();
+  const int wg = warp >> 2, w4 = warp & 3;
+  const int r_lo = wg * 64 + w4 * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const uint32_t sbase = smem_u32(smem);
+  const uint32_t sq = sbase + kOffQ + wg * (64 * 128), sqd = sbase + kOffQd + wg * (64 * 128);
+  const float sc = p.sm_scale * kLog2e;
+
+  float o[HD / 2], a[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) o[i] = a[i] = 0.f;
+  float m_used[2] = {-INFINITY, -INFINITY}, l_part[2] = {0.f, 0.f}, mu_part[2] = {0.f, 0.f};
+
+  mbar_wait(&bars[kQFull], 0);
+  for (int j = 0; j < n_tiles; ++j) {
+    const int st = j % kStages;
+    const uint32_t ph = (j / kStages) & 1;
+    const uint32_t sk = sbase + kOffK + st * kStageBytes, sv = sbase + kOffV + st * kStageBytes;
+
+    float s[BK / 2], sd[BK / 2];
+    mbar_wait(&bars[kKFull + st], ph);
+    score_tile<true, HD, BK, kBF16>(s, sq, BQ * 128, sk, sc);
+    softmax_step_jvp(s, o, a, m_used, l_part, mu_part, p.lk - j * BK, cq, j == 0);   // s := p
+#pragma unroll
+    for (int i = 0; i < BK / 2; ++i) sd[i] = 0.f;
+    wgmma_fence();
+    qk_mmas<kBF16>(sd, sqd, sk, false);               // Sd / c = Qd.K^T + Q.Kd^T
+    qk_mmas<kBF16>(sd, sq, sk + kHalfBytes, true);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(sd);
+    warp_release(&bars[kKEmpty + st], lane);
+
+    uint32_t pa[BK / 16][4], pda[BK / 16][4];        // P and P * Sd rounded to T: the A operands of the products
+#pragma unroll
+    for (int i = 0; i < BK / 2; i += 2) {
+      const int h = (i >> 1) & 1;
+      const float x0 = s[i] * (sd[i] * p.sm_scale), x1 = s[i + 1] * (sd[i + 1] * p.sm_scale);   // Sd in natural-log units
+      mu_part[h] += x0 + x1;
+      pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(s[i], s[i + 1]);
+      pda[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(x0, x1);
+    }
+
+    mbar_wait(&bars[kVFull + st], ph);
+    const uint64_t vdesc = make_desc_mnmajor_sw128(sv, BK * 128), vddesc = make_desc_mnmajor_sw128(sv + kHalfBytes, BK * 128);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(o, pa[kk], vdesc + uint64_t(kk * 128));
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(a, pda[kk], vdesc + uint64_t(kk * 128));
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(a, pa[kk], vddesc + uint64_t(kk * 128));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    reg_fence(a);
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk) {
+      reg_fence(pa[kk]);
+      reg_fence(pda[kk]);
+    }
+    warp_release(&bars[kVEmpty + st], lane);
+  }
+
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float l_tot = quad_sum(l_part[h]), mu_tot = quad_sum(mu_part[h]);   // all four lanes of a row take part
+    const int64_t qr = int64_t(m_blk) * BQ + r_lo + 8 * h;
+    if (qr >= p.lq) continue;
+    const int64_t row = ((int64_t(b) * p.lq + qr) * p.h + hh) * HD;
+    const float inv_l = 1.0f / l_tot, mu_l = mu_tot * inv_l;
+    store_o_row<T, HD>(static_cast<T*>(p.out) + row, o, h, inv_l, cq);
+    T* trow = static_cast<T*>(p.out_t) + row;
+#pragma unroll
+    for (int c = 0; c < HD / 8; ++c) {
+      const int i = 4 * c + 2 * h;
+      *reinterpret_cast<uint32_t*>(trow + 8 * c + cq) =
+          F16Traits<T>::pack(fmaf(-mu_l, o[i], a[i]) * inv_l, fmaf(-mu_l, o[i + 1], a[i + 1]) * inv_l);
+    }
+  }
+}
+
+template <typename T>
+int launch(const CUtensorMap (&tm)[6], const Params& p, dim3 grid, cudaStream_t st) {
+  static bool smem_set[64];
+  const auto kern = dense_attn_jvp_kernel<T>;
+  if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), kSmemBytes, smem_set, "cudaFuncSetAttribute(dense_attn_jvp)"))
+    return rc;
+  kern<<<grid, split::kThreads, kSmemBytes, st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p);
+  return check_launch("dense_attn_jvp_kernel");
+}
+}  // namespace jvp
+
 }  // namespace
 
 extern "C" int tdb200_attn_dense_fwd(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq,
@@ -192,4 +438,52 @@ extern "C" int tdb200_attn_dense_fwd(const void* q, const void* k, const void* v
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16>(tq, tk, tv, p, grid, st);
   return launch<__half>(tq, tk, tv, p, grid, st);
+}
+
+extern "C" int tdb200_attn_dense_jvp(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
+                                     const void* v_t, int dtype, void* out, void* out_t, int64_t b, int64_t lq, int64_t lk,
+                                     int64_t h, int64_t d, float sm_scale, void* stream) {
+  if (!q || !k || !v || !q_t || !k_t || !v_t || !out || !out_t) return fail(TDB200_ERR_INVALID_ARG, "attn_dense_jvp: null pointer");
+  if (b <= 0 || lq <= 0 || lk <= 0 || h <= 0 || d <= 0)
+    return fail(TDB200_ERR_INVALID_ARG, "attn_dense_jvp: bad shape (b=%lld, lq=%lld, lk=%lld, h=%lld, d=%lld)", (long long)b,
+                (long long)lq, (long long)lk, (long long)h, (long long)d);
+  if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(q_t) || !aligned16(k_t) || !aligned16(v_t) ||
+      !aligned16(out) || !aligned16(out_t))
+    return fail(TDB200_ERR_INVALID_ARG, "attn_dense_jvp: q, k, v, their tangents, out and out_t must be 16-byte aligned");
+  if (dtype != TDB200_DTYPE_BF16 && dtype != TDB200_DTYPE_FP16) return fail(TDB200_ERR_UNSUPPORTED, "attn_dense_jvp: dtype tag %d", dtype);
+  if (d != HD) return fail(TDB200_ERR_UNSUPPORTED, "attn_dense_jvp: head dim %lld (this kernel implements d=128)", (long long)d);
+  constexpr int64_t kMaxStride = int64_t(1) << 40;
+  if (h > 65535 || b > 65535 || lq > 0x7FFFFFFF || lk > 0x7FFFFFFF || lq * h * d * 2 >= kMaxStride || lk * h * d * 2 >= kMaxStride)
+    return fail(TDB200_ERR_UNSUPPORTED, "attn_dense_jvp: dimension too large (b, h <= 65535; lq * h * d and lk * h * d below 2^39)");
+  if (int rc = require_sm90()) return rc;
+
+  const CUtensorMapDataType t16 = dtype == TDB200_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUtensorMap tm[6];   // q, k, v, q_t, k_t, v_t
+  {
+    const uint64_t dims[4] = {uint64_t(d), uint64_t(h), uint64_t(lq), uint64_t(b)};
+    const uint64_t str[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(lq * h * d * 2)};
+    const uint32_t box[4] = {64, 1, BQ, 1};
+    if (int rc = make_tmap_4d(&tm[0], q, t16, 2, dims, str, box)) return rc;
+    if (int rc = make_tmap_4d(&tm[3], q_t, t16, 2, dims, str, box)) return rc;
+  }
+  {
+    const uint64_t dims[4] = {uint64_t(d), uint64_t(h), uint64_t(lk), uint64_t(b)};
+    const uint64_t str[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(lk * h * d * 2)};
+    const uint32_t box[4] = {64, 1, jvp::BK, 1};
+    if (int rc = make_tmap_4d(&tm[1], k, t16, 2, dims, str, box)) return rc;
+    if (int rc = make_tmap_4d(&tm[2], v, t16, 2, dims, str, box)) return rc;
+    if (int rc = make_tmap_4d(&tm[4], k_t, t16, 2, dims, str, box)) return rc;
+    if (int rc = make_tmap_4d(&tm[5], v_t, t16, 2, dims, str, box)) return rc;
+  }
+  jvp::Params p;
+  p.out = out;
+  p.out_t = out_t;
+  p.lq = int(lq);
+  p.lk = int(lk);
+  p.h = int(h);
+  p.sm_scale = sm_scale;
+  const dim3 grid(static_cast<unsigned>(cdiv64(lq, BQ)), static_cast<unsigned>(h), static_cast<unsigned>(b));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (dtype == TDB200_DTYPE_BF16) return jvp::launch<__nv_bfloat16>(tm, p, grid, st);
+  return jvp::launch<__half>(tm, p, grid, st);
 }

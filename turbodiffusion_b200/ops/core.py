@@ -352,3 +352,27 @@ def dense_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, sm_scale:
                                       float(d ** -0.5 if sm_scale is None else sm_scale), stream_ptr(qc.device)),
           "attn_dense_fwd")
     return out.to(q.dtype)
+
+
+def dense_attention_jvp(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, q_t: torch.Tensor, k_t: torch.Tensor,
+                        v_t: torch.Tensor, sm_scale: Optional[float] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """dense_attention(q, k, v) and its forward-mode derivative along the tangents (q_t, k_t, v_t), from one kernel
+    (tdb200_attn_dense_jvp): (out, out_t) with out_t = sum_j P_j S_t,j v_j - (sum_j P_j S_t,j) out + P.v_t, S_t =
+    sm_scale (q_t.k^T + q.k_t^T).  Shapes and dtype rules as dense_attention; each tangent has its primal's shape and runs in
+    the primal's 16-bit type.  Both outputs are [B, Lq, H, D] in q's dtype.  Not a `tdb200::` operator: eager use."""
+    require_cuda(q, k, v, q_t, k_t, v_t)
+    if q.dim() != 4 or k.shape != v.shape or k.dim() != 4 or (q.shape[0], *q.shape[2:]) != (k.shape[0], *k.shape[2:]):
+        raise ValueError(f"dense_attention_jvp: q [B, Lq, H, D] and k, v [B, Lk, H, D] expected, got {tuple(q.shape)}, "
+                         f"{tuple(k.shape)}, {tuple(v.shape)}")
+    for name, t, primal in (("q_t", q_t, q), ("k_t", k_t, k), ("v_t", v_t, v)):
+        if t.shape != primal.shape:
+            raise ValueError(f"dense_attention_jvp: {name} {tuple(t.shape)} must have its primal's shape {tuple(primal.shape)}")
+    dtype = q.dtype if q.dtype in DTYPE_TAG else torch.bfloat16
+    qc, kc, vc, qtc, ktc, vtc = (t.to(dtype).contiguous() for t in (q, k, v, q_t, k_t, v_t))
+    b, lq, h, d = qc.shape
+    out, out_t = torch.empty_like(qc), torch.empty_like(qc)
+    check(lib().tdb200_attn_dense_jvp(ptr(qc), ptr(kc), ptr(vc), ptr(qtc), ptr(ktc), ptr(vtc), DTYPE_TAG[dtype], ptr(out),
+                                      ptr(out_t), b, lq, kc.shape[1], h, d, float(d ** -0.5 if sm_scale is None else sm_scale),
+                                      stream_ptr(qc.device)),
+          "attn_dense_jvp")
+    return out.to(q.dtype), out_t.to(q.dtype)

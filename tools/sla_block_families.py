@@ -20,6 +20,14 @@ pooling of its rows), its Q prep and block map and the fused attention of its qu
 ("allgather"; the fused attention alone is "allgather_attn"); in the Ulysses mode the single-GPU pipeline on its H/N heads
 (rank 0 takes the extra head of an uneven split).  The collectives and their overlap with compute are not timed.  One JSON
 line per (shape, N, family).
+
+    python tools/sla_block_families.py --baseline-lib PATH [--shape ...]
+
+compares this tree's libtdb200.so with another build of the same C ABI (for example the parent commit's), loaded side by
+side: at each shape the fused attention of both INT8 families, the 16-bit (128, 64) forward and its lse forward are called
+through the C entry points on the same inputs, the two builds alternating call by call in a rotating order.  Per leg and build:
+median, 10th and 90th percentile of the call time.  Every output of the two builds (out, and lse for the lse forward) is
+compared byte for byte; the script exits non-zero if any leg differs.
 """
 from __future__ import annotations
 
@@ -143,6 +151,113 @@ def run_shape(name, ratio, iters, warmup):
     return rows
 
 
+def _load_build(path):
+    """The attention entry points of the libtdb200.so at `path`, typed from this tree's prototypes."""
+    import ctypes
+    from turbodiffusion_b200 import _lib
+    handle = ctypes.CDLL(path)
+    fns = {}
+    for name in ("tdb200_sla_attn_fwd", "tdb200_sla_attn16_fwd", "tdb200_sla_attn16_fwd_lse"):
+        fn = getattr(handle, name)
+        fn.argtypes = _lib._PROTOS[name]
+        fn.restype = ctypes.c_int
+        fns[name] = fn
+    return fns
+
+
+def _build_legs(fns, q, k, v, ratio):
+    """Per leg, a call of one build's entry point and the output buffers it writes (fresh for this build)."""
+    from turbodiffusion_b200._lib import DTYPE_TAG, ptr
+    from turbodiffusion_b200.SLA.core import linear_moments, project_moments
+    from turbodiffusion_b200.SLA.utils import block_map_from_pools, quant_qk
+    b, l, h, d = q.shape
+    g = torch.Generator(device="cuda").manual_seed(1)
+    w = torch.randn(d, d, generator=g, device="cuda") * 0.05
+    pb = (torch.randn(d, generator=g, device="cuda") * 0.05).contiguous()
+    kv, ksum = linear_moments(k, v)
+    kvw = project_moments(w, kv, q.dtype)
+    stream = torch.cuda.current_stream().cuda_stream
+    tag, sm_scale = DTYPE_TAG[q.dtype], d ** -0.5
+    legs = {}
+
+    def check(rc, what):
+        if rc != 0:
+            raise RuntimeError(f"{what} returned {rc}")
+
+    for fam, (blkq, blkk) in (("sm100", (128, 64)), ("sm90", (64, 128))):
+        prep = quant_qk(q, k, blkq=blkq, blkk=blkk)
+        topk = max(1, min(prep.nblk, int(ratio * prep.nblk)))
+        _, lut = block_map_from_pools(prep.q_pool, prep.k_pool, topk)
+        out = torch.empty_like(q)
+
+        def call(prep=prep, lut=lut, topk=topk, out=out, blkq=blkq, blkk=blkk):
+            check(fns["tdb200_sla_attn_fwd"](ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v), ptr(q),
+                                             tag, ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(pb), ptr(out), b, l, l, h, d, sm_scale,
+                                             0, blkq, blkk, 0, stream), "tdb200_sla_attn_fwd")
+        legs[fam] = {"call": call, "outputs": [out], "mblk": prep.mblk, "topk": topk, "blkq": blkq, "blkk": blkk}
+        if fam == "sm100":   # the 16-bit (128, 64) kernels on the same 128 x 64 block list
+            out16, o_s = torch.empty_like(q), torch.empty_like(q)
+            lse = torch.empty(b, h, l, dtype=torch.float32, device=q.device)
+
+            def call16(lut=lut, topk=topk):
+                check(fns["tdb200_sla_attn16_fwd"](ptr(q), ptr(k), ptr(v), tag, ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(pb),
+                                                   ptr(out16), b, l, l, h, d, sm_scale, 0, 128, 64, stream), "tdb200_sla_attn16_fwd")
+
+            def call16_lse(lut=lut, topk=topk):
+                check(fns["tdb200_sla_attn16_fwd_lse"](ptr(q), ptr(k), ptr(v), tag, ptr(lut), topk, ptr(o_s), ptr(lse), b, l, h, d,
+                                                       sm_scale, 128, 64, stream), "tdb200_sla_attn16_fwd_lse")
+            common = {"mblk": prep.mblk, "topk": topk, "blkq": 128, "blkk": 64}
+            legs["attn16"] = {"call": call16, "outputs": [out16], **common}
+            legs["attn16_lse"] = {"call": call16_lse, "outputs": [o_s, lse], **common}
+    return legs
+
+
+def _pct(xs, f):
+    xs = sorted(xs)
+    return xs[min(len(xs) - 1, int(round(f * (len(xs) - 1))))]
+
+
+def run_builds(name, ratio, iters, warmup, baseline_lib):
+    """This tree's build against `baseline_lib`, leg by leg, alternated call by call; returns (rows, all outputs identical)."""
+    from turbodiffusion_b200 import _lib
+    l, h, d = SHAPES[name]
+    g = torch.Generator(device="cuda").manual_seed(0)
+    q, k, v = (torch.randn(1, l, h, d, generator=g, device="cuda").bfloat16() for _ in range(3))
+    k += torch.randn(1, 1, h, d, generator=g, device="cuda").bfloat16() * 2
+    builds = {"this": _load_build(_lib.LIB_PATH), "baseline": _load_build(baseline_lib)}
+    legs = {bn: _build_legs(fns, q, k, v, ratio) for bn, fns in builds.items()}
+    names = list(legs["this"])
+    calls = [(leg, bn) for leg in names for bn in builds]
+    times = {c: [] for c in calls}
+    clocks = {}
+    for i in range(warmup + iters):
+        if i == warmup:
+            clocks["sm_clock_throttle_before"] = clock_state()
+        r = i % len(calls)
+        for leg, bn in calls[r:] + calls[:r]:
+            t = _timed(legs[bn][leg]["call"])
+            if i >= warmup:
+                times[(leg, bn)].append(t)
+    clocks["sm_clock_throttle_after"] = clock_state()
+    rows, same_all = [], True
+    for leg in names:
+        f = legs["this"][leg]
+        same = all(torch.equal(a.view(torch.uint8), b_.view(torch.uint8))
+                   for a, b_ in zip(legs["this"][leg]["outputs"], legs["baseline"][leg]["outputs"]))
+        same_all &= same
+        flops = h * f["mblk"] * f["topk"] * 4 * f["blkq"] * f["blkk"] * d
+        row = {"shape": name, "L": l, "heads": h, "head_dim": d, "leg": leg, "blkq": f["blkq"], "blkk": f["blkk"], "topk": f["topk"],
+               "outputs_byte_identical": same, "calls": iters, **clocks}
+        for bn in builds:
+            ts = times[(leg, bn)]
+            med = statistics.median(ts)
+            row[bn] = {"ms_median": round(med, 4), "ms_p10": round(_pct(ts, 0.1), 4), "ms_p90": round(_pct(ts, 0.9), 4),
+                       "tflops": round(flops / med / 1e9, 1)}
+        row["median_ratio_this_over_baseline"] = round(row["this"]["ms_median"] / row["baseline"]["ms_median"], 4)
+        rows.append(row)
+    return rows, same_all
+
+
 def setup_rank0(arch, q, k, v, ratio, world):
     """Rank 0's share of one sequence-parallel layer on `world` GPUs (dist.py), on one family's blocks, built from the real
     per-rank primitives.  The gathered slab rank 0 attends over is made here from the whole sequence; the split key prep
@@ -245,6 +360,8 @@ def main():
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--topk", type=float, default=0.1)
+    ap.add_argument("--baseline-lib", default=None,
+                    help="another libtdb200.so with the same C ABI: time it against this tree's build and compare the outputs")
     ap.add_argument("--ranks", default=None,
                     help="comma-separated world sizes, e.g. 1,2,4,8: time rank 0's share of a sequence-parallel layer instead")
     args = ap.parse_args()
@@ -257,6 +374,19 @@ def main():
         raise SystemExit("sla_block_families.py measures on a CUDA device; none is available")
     if args.iters < 50:
         raise SystemExit("--iters: the medians are taken over at least 50 calls")
+    if args.baseline_lib is not None:
+        from turbodiffusion_b200 import _lib
+        print(json.dumps({**device_info(), "builds": {"this": _lib.LIB_PATH, "baseline": os.path.abspath(args.baseline_lib)}}),
+              flush=True)
+        identical = True
+        for name in (["A", "B"] if args.shape == "both" else [args.shape]):
+            rows, same = run_builds(name, args.topk, args.iters, args.warmup, os.path.abspath(args.baseline_lib))
+            identical &= same
+            for row in rows:
+                print(json.dumps(row), flush=True)
+        if not identical:
+            raise SystemExit("the two builds' outputs differ")
+        return
     print(json.dumps(device_info()), flush=True)
     for name in (["A", "B"] if args.shape == "both" else [args.shape]):
         rows = run_shape(name, args.topk, args.iters, args.warmup) if ranks is None else \

@@ -10,6 +10,8 @@
 #include <cuda_fp16.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace tdb {
 
 // ------------------------------------------------------------------------------------------
@@ -219,14 +221,18 @@ __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory");
 }
 // Ties registers written (or read) by an in-flight wgmma to a point after wgmma_wait: the compiler may neither read
-// an accumulator before it nor reuse an A-fragment register ahead of it.
+// an accumulator before it nor reuse an A-fragment register ahead of it.  Each register is pinned in its own type: pinning a
+// float through a uint32_t alias makes nvcc emit mov copies of the accumulator around the asm, and ptxas, seeing non-wgmma
+// reads of an in-flight accumulator, then serialises every wgmma of the kernel (warning C7514).
 template <typename R, int N>
 __device__ __forceinline__ void reg_fence(R (&r)[N]) {
+  static_assert(std::is_same<R, float>::value || std::is_same<R, uint32_t>::value, "reg_fence: float or uint32_t registers");
 #pragma unroll
   for (int i = 0; i < N; ++i) {
-    if constexpr (sizeof(R) == 4) {
-      uint32_t* u = reinterpret_cast<uint32_t*>(&r[i]);
-      asm volatile("" : "+r"(*u)::"memory");
+    if constexpr (std::is_same<R, float>::value) {
+      asm volatile("" : "+f"(r[i])::"memory");
+    } else {
+      asm volatile("" : "+r"(r[i])::"memory");
     }
   }
 }

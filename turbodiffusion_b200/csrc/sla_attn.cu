@@ -273,22 +273,45 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
   float m_used[2] = {-INFINITY, -INFINITY}, l_part[2] = {0.f, 0.f};  // l_part: this thread's columns of the row sum
 
+  // Software pipeline, per warpgroup (the FA3 order): S_{j+1} = Q.K_{j+1}^T and O += P_j.V_j are issued back to back as two
+  // commit groups, and the softmax of S_{j+1} runs while P_j.V_j is still on the tensor core.  Per element the steps and their
+  // order are those of softmax_step and pv_step: l is scaled before it adds an entry's P, O is scaled after the previous P.V
+  // retired and before this one, and the entries accumulate in LUT order.  Every P.V retires inside its own iteration: with one
+  // still in flight across the loop's back edge, ptxas no longer proves which group a wait retires and serialises every wgmma
+  // of the kernel (C7514).
+  const uint32_t sq = sbase + L::kOffQ + wg * (64 * HD);
+  ScoreAcc<kQK16> sacc[BLKK / 2];   // S_{j+1} in flight
+  float s[BLKK / 2];                // S_j, then P_j
+  uint32_t pa[BLKK / 16][4];        // P_j, read by the P.V in flight
+  bool rescale[2];
+  float alpha[2];
   mbar_wait(&bars[kQFull], 0);
+  mbar_wait(&bars[kKFull], 0);
+  score_issue<kQK16, HD, BLKK, kBF16>(sacc, sq, BLKQ * 128, sbase + L::kOffK);
+  wgmma_wait<0>();
+  score_finish<kQK16, BLKK>(sacc, s, qsc * s_ksc[0]);
+  warp_release(&bars[kKEmpty], lane);
+  // valid < 64 only in the ragged last key block
+  softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, p.lk - int(s_lut[0]) * BLKK, cq, true);
   for (int j = 0; j < T_blocks; ++j) {
-    const int st = j % kStages;
-    const uint32_t ph = (j / kStages) & 1;
-    const int blk = s_lut[j];
-    const float sc = qsc * s_ksc[j];
-    const int valid = p.lk - blk * BLKK;                // < 64 only in the ragged last key block
-
-    float s[BLKK / 2];
-    mbar_wait(&bars[kKFull + st], ph);
-    score_tile<kQK16, HD, BLKK, kBF16>(s, sbase + L::kOffQ + wg * (64 * HD), BLKQ * 128, sbase + L::kOffK + st * L::kKBytes, sc);
-    warp_release(&bars[kKEmpty + st], lane);
-    uint32_t pa[BLKK / 16][4];
-    softmax_step<T, HD, BLKK>(s, o, m_used, l_part, pa, valid, cq, j == 0);
-    mbar_wait(&bars[kVFull + st], ph);
-    pv_step<HD, BLKK, kBF16>(o, pa, sbase + L::kOffV + st * L::kVBytes);
+    const int st = j % kStages, st1 = (j + 1) % kStages;
+    const bool next = j + 1 < T_blocks;
+    if (next) {
+      mbar_wait(&bars[kKFull + st1], ((j + 1) / kStages) & 1);
+      score_issue<kQK16, HD, BLKK, kBF16>(sacc, sq, BLKQ * 128, sbase + L::kOffK + st1 * L::kKBytes);
+    }
+    rescale_o<HD>(o, rescale, alpha);
+    pack_p<T, BLKK>(s, pa);
+    mbar_wait(&bars[kVFull + st], (j / kStages) & 1);
+    pv_issue<HD, BLKK, kBF16>(o, pa, sbase + L::kOffV + st * L::kVBytes);
+    wgmma_wait<1>();                                    // S_{j+1} retired, P_j.V_j may still run
+    if (next) {
+      score_finish<kQK16, BLKK>(sacc, s, qsc * s_ksc[j + 1]);
+      warp_release(&bars[kKEmpty + st1], lane);
+      softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, p.lk - int(s_lut[j + 1]) * BLKK, cq, false);
+    }
+    wgmma_wait<0>();
+    pv_fence<HD, BLKK>(o, pa);
     warp_release(&bars[kVEmpty + st], lane);
   }
   if constexpr (kLse) {

@@ -37,51 +37,69 @@ __device__ __forceinline__ float quad_sum(float v) {
 // ---- The per-entry steps of every forward kernel (sla_attn.cu, dense_attn.cu), on one warpgroup's 64 query rows.  Each thread
 //      holds rows r and r + 8 of the tiles (fragment layout, common.cuh); cq is its column pair offset inside every 8-column slice.
 
-// S = Q.K^T over the BK keys of one ring slot, scaled by sc into the log2 domain.  INT8: scores are int32 dot products (sc
-// folds in q_scale * k_scale), Q and K rows of HD bytes with a 128-byte swizzle for 128-wide heads and a 64-byte one for
-// 64-wide heads.  16-bit: fp32 scores, Q and K in HD/64 chunks of 128-byte rows, q_chunk bytes apart for Q.
+// The raw score accumulator of S = Q.K^T: int32 dot products for INT8 Q/K, fp32 for 16-bit Q/K.
+template <bool kQK16>
+using ScoreAcc = std::conditional_t<kQK16, float, uint32_t>;
+
+// Issue S = Q.K^T over the BK keys of one ring slot into acc, as one commit group.  INT8: Q and K rows of HD bytes with a
+// 128-byte swizzle for 128-wide heads and a 64-byte one for 64-wide heads.  16-bit: Q and K in HD/64 chunks of 128-byte rows,
+// q_chunk bytes apart for Q.  acc must not be touched until the group has retired and score_finish has fenced it.
 template <bool kQK16, int HD, int BK, bool kBF16>
-__device__ __forceinline__ void score_tile(float (&s)[BK / 2], uint32_t sq, uint32_t q_chunk, uint32_t sk, float sc) {
-  if constexpr (kQK16) {
+__device__ __forceinline__ void score_issue(ScoreAcc<kQK16> (&acc)[BK / 2], uint32_t sq, uint32_t q_chunk, uint32_t sk) {
 #pragma unroll
-    for (int i = 0; i < BK / 2; ++i) s[i] = 0.f;
+  for (int i = 0; i < BK / 2; ++i) acc[i] = 0;
+  if constexpr (kQK16) {
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < HD / 16; ++ks) {  // K = 16 elements per MMA: chunk ks/4, +32 bytes per step inside the chunk
       const uint64_t qd = make_desc_kmajor_sw128(sq + (ks >> 2) * q_chunk) + uint64_t((ks & 3) * 2);
       const uint64_t kd = make_desc_kmajor_sw128(sk + (ks >> 2) * (BK * 128)) + uint64_t((ks & 3) * 2);
-      wgmma_f16_ss<BK, kBF16>(s, qd, kd, ks > 0 ? 1u : 0u);
+      wgmma_f16_ss<BK, kBF16>(acc, qd, kd, ks > 0 ? 1u : 0u);
     }
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(s);
-#pragma unroll
-    for (int i = 0; i < BK / 2; ++i) s[i] *= sc;
   } else {
-    uint32_t si[BK / 2];
-#pragma unroll
-    for (int i = 0; i < BK / 2; ++i) si[i] = 0u;
     const uint64_t qdesc = HD == 128 ? make_desc_kmajor_sw128(sq) : make_desc_kmajor_sw64(sq);
     const uint64_t kdesc = HD == 128 ? make_desc_kmajor_sw128(sk) : make_desc_kmajor_sw64(sk);
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < HD / 32; ++ks)
-      wgmma_i8_ss<BK>(si, qdesc + uint64_t(ks * 2), kdesc + uint64_t(ks * 2), ks > 0 ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(si);
+      wgmma_i8_ss<BK>(acc, qdesc + uint64_t(ks * 2), kdesc + uint64_t(ks * 2), ks > 0 ? 1u : 0u);
+  }
+  wgmma_commit();
+}
+
+// Once score_issue's group has retired: s = acc scaled by sc into the log2 domain (INT8: sc folds in q_scale * k_scale).
+template <bool kQK16, int BK>
+__device__ __forceinline__ void score_finish(ScoreAcc<kQK16> (&acc)[BK / 2], float (&s)[BK / 2], float sc) {
+  reg_fence(acc);
 #pragma unroll
-    for (int i = 0; i < BK / 2; ++i) s[i] = static_cast<float>(static_cast<int>(si[i])) * sc;
+  for (int i = 0; i < BK / 2; ++i) {
+    if constexpr (kQK16) s[i] = acc[i] * sc;
+    else s[i] = static_cast<float>(static_cast<int>(acc[i])) * sc;
   }
 }
 
-// One online-softmax step: key columns from `valid` on do not exist (the ragged last key block), then the row maxima and the
-// lazy rescale of O and the row sums (per row: alpha == 1 exactly where the maximum is kept), then P = exp2(s - m_used) into
-// the A fragments of P.V.  The row sum is taken from the unrounded P, the tensor core gets P rounded to T.  `first`: the first
-// entry of this warpgroup, which sets the maxima.
-template <typename T, int HD, int BK>
-__device__ __forceinline__ void softmax_step(float (&s)[BK / 2], float (&o)[HD / 2], float (&m_used)[2], float (&l_part)[2],
-                                             uint32_t (&pa)[BK / 16][4], int valid, int cq, bool first) {
+// S = Q.K^T over the BK keys of one ring slot, scaled by sc into the log2 domain, with nothing else in flight.
+template <bool kQK16, int HD, int BK, bool kBF16>
+__device__ __forceinline__ void score_tile(float (&s)[BK / 2], uint32_t sq, uint32_t q_chunk, uint32_t sk, float sc) {
+  if constexpr (kQK16) {   // the fp32 accumulator is s itself
+    score_issue<kQK16, HD, BK, kBF16>(s, sq, q_chunk, sk);
+    wgmma_wait<0>();
+    score_finish<kQK16, BK>(s, s, sc);
+  } else {
+    uint32_t si[BK / 2];
+    score_issue<kQK16, HD, BK, kBF16>(si, sq, q_chunk, sk);
+    wgmma_wait<0>();
+    score_finish<kQK16, BK>(si, s, sc);
+  }
+}
+
+// The part of one online-softmax step that does not touch O: key columns from `valid` on do not exist (the ragged last key
+// block), then the row maxima, the lazy rescale of the row sums (per row half h: rescale[h] where the maximum grew by more than
+// the threshold, O to be scaled by alpha[h]; elsewhere the maximum is kept and O stays as it is), then P = exp2(s - m_used),
+// left unrounded in s, and its row sums.  `first`: the first entry of this warpgroup, which sets the maxima.
+template <int BK>
+__device__ __forceinline__ void softmax_p(float (&s)[BK / 2], float (&m_used)[2], float (&l_part)[2], bool (&rescale)[2],
+                                          float (&alpha)[2], int valid, int cq, bool first) {
   if (valid < BK) {
 #pragma unroll
     for (int i = 0; i < BK / 2; ++i)
@@ -94,38 +112,80 @@ __device__ __forceinline__ void softmax_step(float (&s)[BK / 2], float (&o)[HD /
     for (int i = 0; i < BK / 2; ++i)
       if (((i >> 1) & 1) == h) mx = fmaxf(mx, s[i]);
     mx = quad_max(mx);
+    rescale[h] = false;
+    alpha[h] = 1.0f;
     if (first) {
       m_used[h] = mx;
     } else if (mx > m_used[h] + kRescaleThreshold) {
-      const float alpha = fast_exp2(m_used[h] - mx);
-#pragma unroll
-      for (int i = 0; i < HD / 2; ++i)
-        if (((i >> 1) & 1) == h) o[i] *= alpha;
-      l_part[h] *= alpha;
+      alpha[h] = fast_exp2(m_used[h] - mx);
+      rescale[h] = true;
+      l_part[h] *= alpha[h];
       m_used[h] = mx;
     }
   }
 #pragma unroll
   for (int i = 0; i < BK / 2; i += 2) {
     const int h = (i >> 1) & 1;
-    const float p0 = fast_exp2(s[i] - m_used[h]), p1 = fast_exp2(s[i + 1] - m_used[h]);
-    l_part[h] += p0 + p1;
-    pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0, p1);
+    s[i] = fast_exp2(s[i] - m_used[h]);
+    s[i + 1] = fast_exp2(s[i + 1] - m_used[h]);
+    l_part[h] += s[i] + s[i + 1];
   }
 }
 
-// O += P.V  (V: [BK keys x HD], HD/64 MN-major chunks of BK x 128 B, so no transposed copy of V; +16 keys = +2048 B per K step)
+// The O part of the step: the lazy rescale softmax_p decided.  O must hold every earlier entry's P.V.
+template <int HD>
+__device__ __forceinline__ void rescale_o(float (&o)[HD / 2], const bool (&rescale)[2], const float (&alpha)[2]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (rescale[h]) {
+#pragma unroll
+      for (int i = 0; i < HD / 2; ++i)
+        if (((i >> 1) & 1) == h) o[i] *= alpha[h];
+    }
+  }
+}
+
+// P rounded to T into the A fragments of P.V (the row sums were taken from the unrounded P)
+template <typename T, int BK>
+__device__ __forceinline__ void pack_p(const float (&p)[BK / 2], uint32_t (&pa)[BK / 16][4]) {
+#pragma unroll
+  for (int i = 0; i < BK / 2; i += 2) pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p[i], p[i + 1]);
+}
+
+// One online-softmax step, with no P.V in flight: softmax_p, the rescale of O, and P into the A fragments of P.V.
+template <typename T, int HD, int BK>
+__device__ __forceinline__ void softmax_step(float (&s)[BK / 2], float (&o)[HD / 2], float (&m_used)[2], float (&l_part)[2],
+                                             uint32_t (&pa)[BK / 16][4], int valid, int cq, bool first) {
+  bool rescale[2];
+  float alpha[2];
+  softmax_p<BK>(s, m_used, l_part, rescale, alpha, valid, cq, first);
+  rescale_o<HD>(o, rescale, alpha);
+  pack_p<T, BK>(s, pa);
+}
+
+// Issue O += P.V as one commit group (V: [BK keys x HD], HD/64 MN-major chunks of BK x 128 B, so no transposed copy of V;
+// +16 keys = +2048 B per K step).  o and pa must not be touched until the group has retired and pv_fence has run.
 template <int HD, int BK, bool kBF16>
-__device__ __forceinline__ void pv_step(float (&o)[HD / 2], uint32_t (&pa)[BK / 16][4], uint32_t sv) {
+__device__ __forceinline__ void pv_issue(float (&o)[HD / 2], uint32_t (&pa)[BK / 16][4], uint32_t sv) {
   const uint64_t vdesc = make_desc_mnmajor_sw128(sv, BK * 128);
   wgmma_fence();
 #pragma unroll
   for (int kk = 0; kk < BK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(o, pa[kk], vdesc + uint64_t(kk * 128));
   wgmma_commit();
-  wgmma_wait<0>();
+}
+template <int HD, int BK>
+__device__ __forceinline__ void pv_fence(float (&o)[HD / 2], uint32_t (&pa)[BK / 16][4]) {
   reg_fence(o);
 #pragma unroll
   for (int kk = 0; kk < BK / 16; ++kk) reg_fence(pa[kk]);
+}
+
+// O += P.V, waited for
+template <int HD, int BK, bool kBF16>
+__device__ __forceinline__ void pv_step(float (&o)[HD / 2], uint32_t (&pa)[BK / 16][4], uint32_t sv) {
+  pv_issue<HD, BK, kBF16>(o, pa, sv);
+  wgmma_wait<0>();
+  pv_fence<HD, BK>(o, pa);
 }
 
 // columns 8 c + cq + {0, 1} of one output row = T(O / l), from row half h (rows r and r + 8) of this thread's O fragment

@@ -16,6 +16,7 @@
  *   Sage block-sparse attention + linear  turbodiffusion/SLA/core.py:231-253          -> tdb200_sla_linear_moments, tdb200_sla_attn_fwd
  *   attention (dense SDPA / FlashAttention) turbodiffusion/rcm/utils/attention.py:120-167 -> tdb200_attn_dense_fwd
  *   JVP flash attention (rCM distillation) turbodiffusion/rcm/networks/wan2pt1_jvp.py -> tdb200_attn_dense_jvp
+ *   backward of the dense attention and of the JVP's primal                          -> tdb200_attn_dense_bwd
  *
  * Conventions
  *   - plain pointers and sizes; all pointers are DEVICE pointers unless stated; no allocation inside;
@@ -297,6 +298,43 @@ int tdb200_attn_dense_fwd(const void* q, const void* k, const void* v, int dtype
 int tdb200_attn_dense_jvp(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
                           int dtype, void* out, void* out_t, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d,
                           float sm_scale, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * f1 backward. Gradients of the dense attention above, for training through tdb200_attn_dense_fwd or the primal output of
+ * tdb200_attn_dense_jvp (rCM / sCM distillation differentiates through out; out_t is a stop-gradient target).
+ *   tdb200_attn_dense_fwd_lse  tdb200_attn_dense_fwd, plus lse [b, h, lq] fp32 = m + log2(l): the row log-sum-exp of the scores
+ *                              in the log2 domain (S * sm_scale * log2e), m the row maximum the lazy rescale last used.
+ *   tdb200_attn_dense_jvp_lse  tdb200_attn_dense_jvp, plus the same lse of the primal.
+ *                              out (and out_t) are bit-identical to those of the entry points without lse: the arithmetic is
+ *                              the same, only the store of lse is added.  Argument checks as theirs, plus lse null or not
+ *                              4-byte aligned -> TDB200_ERR_INVALID_ARG.
+ *   tdb200_attn_dense_bwd      dq [b, lq, h, d], dk and dv [b, lk, h, d] of out for the incoming gradient d_out [b, lq, h, d],
+ *                              given q, k, v, the forward's out and lse.  FlashAttention-2's backward on 128-row query and
+ *                              64-row key tiles: P = exp2(S * sm_scale * log2e - lse) and dS = P o (dO.V^T - delta) with
+ *                              delta = rowsum(dO o out) in fp32, rounded to T only as MMA operands; fp32 accumulation, dq, dk
+ *                              and dv rounded to T once.  Key columns >= lk are masked; rows >= lq of dq and rows >= lk of dk
+ *                              and dv are not written.  No atomics: every output row is written by one thread in a fixed
+ *                              order, so the gradients are bit-for-bit reproducible.  Three kernel launches (delta, dq,
+ *                              dk/dv), no host synchronisation, so the call can be captured in a CUDA graph.
+ *   tdb200_attn_dense_bwd_workspace_bytes  host-only size of the workspace the backward needs, delta [b, h, lq] fp32 (or a
+ *                              negative error code: non-positive sizes -> TDB200_ERR_INVALID_ARG, sizes past the limits
+ *                              below -> TDB200_ERR_UNSUPPORTED).
+ * All tensors contiguous 16-bit of type `dtype` except lse (fp32); d = 128 only.
+ * Errors of tdb200_attn_dense_bwd, all before any CUDA call: any pointer null, q, k, v, out, d_out, dq, dk or dv not 16-byte
+ * aligned, lse or workspace not 4-byte aligned, non-positive b, lq, lk, h or d -> TDB200_ERR_INVALID_ARG; bad dtype tag,
+ * d != 128, b or h above 65535, lq*h*d or lk*h*d of 2^39 elements or more, or b*lq*h above 8 * (2^31 - 1) rows (the delta
+ * kernel's grid: a tighter limit than the forward's) -> TDB200_ERR_UNSUPPORTED; workspace_bytes below the size query ->
+ * TDB200_ERR_WORKSPACE.
+ * ------------------------------------------------------------------------------------------- */
+int tdb200_attn_dense_fwd_lse(const void* q, const void* k, const void* v, int dtype, void* out, float* lse, int64_t b, int64_t lq,
+                              int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream);
+int tdb200_attn_dense_jvp_lse(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                              int dtype, void* out, void* out_t, float* lse, int64_t b, int64_t lq, int64_t lk, int64_t h,
+                              int64_t d, float sm_scale, void* stream);
+int tdb200_attn_dense_bwd(const void* q, const void* k, const void* v, const void* out, const void* d_out, const float* lse,
+                          int dtype, void* dq, void* dk, void* dv, void* workspace, int64_t workspace_bytes, int64_t b, int64_t lq,
+                          int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream);
+int64_t tdb200_attn_dense_bwd_workspace_bytes(int64_t b, int64_t h, int64_t lq);
 
 /* ---------------------------------------------------------------------------------------------
  * a12. LTX-2 (TurboT2AV) prologue variants   (ltx_core/model/transformer/transformer.py:21-94; Triton fast path

@@ -61,6 +61,10 @@ _PROTOS = {
     "tdb200_sla_attn16_bwd_workspace_bytes": [_I64, _I64, _I64, _I64, _I64],
     "tdb200_attn_dense_fwd": [_P, _P, _P, _I, _P, _I64, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_attn_dense_jvp": [_P, _P, _P, _P, _P, _P, _I, _P, _P, _I64, _I64, _I64, _I64, _I64, _F, _P],
+    "tdb200_attn_dense_fwd_lse": [_P, _P, _P, _I, _P, _P, _I64, _I64, _I64, _I64, _I64, _F, _P],
+    "tdb200_attn_dense_jvp_lse": [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F, _P],
+    "tdb200_attn_dense_bwd": [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _I64, _F, _P],
+    "tdb200_attn_dense_bwd_workspace_bytes": [_I64, _I64, _I64],
     "tdb200_ltx_modulated_rms_norm_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_ltx_modulate_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
     "tdb200_ltx_gated_residual_ada": [_P, _P, _I, _P, _P, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
@@ -69,7 +73,7 @@ _PROTOS = {
     "tdb200_gemm_w8a8_rowwise": [_P, _P, _P, _P, _P, _P, _I, _I64, _I64, _I64, _P],
 }
 _RESTYPES = {"tdb200_last_error": c_char_p, "tdb200_sla_attn_bwd_workspace_bytes": c_int64,
-             "tdb200_sla_attn16_bwd_workspace_bytes": c_int64}
+             "tdb200_sla_attn16_bwd_workspace_bytes": c_int64, "tdb200_attn_dense_bwd_workspace_bytes": c_int64}
 ABI_VERSION = 2   # TDB200_ABI_VERSION of include/tdb200.h, whose prototypes _PROTOS mirrors
 
 _lib = None
@@ -132,7 +136,7 @@ class _DeviceGuarded:
 
 
 LAUNCHES = 0  # kernels launched through the C ABI (each entry point documents how many it enqueues)
-_KERNELS_PER_CALL = {"sla_quant_qk": 4, "layernorm_modulate_quant": 2, "sla_attn16_bwd": 4}  # upper bounds per entry point
+_KERNELS_PER_CALL = {"sla_quant_qk": 4, "layernorm_modulate_quant": 2, "sla_attn16_bwd": 4, "attn_dense_bwd": 3}  # upper bounds per entry point
 
 
 def check(rc: int, what: str, launches: int = None) -> None:

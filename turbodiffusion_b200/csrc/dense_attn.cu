@@ -42,12 +42,15 @@ enum Bar { kQFull = 0, kKFull = 1, kKEmpty = kKFull + kStages, kVFull = kKEmpty 
 static_assert(kNumBars * 8 <= 256, "barriers exceed their shared-memory slot");
 
 struct DenseParams {
-  void* out;   // [b, lq, h, d] T
+  void* out;    // [b, lq, h, d] T
+  float* lse;   // [b, h, lq] fp32, log2 domain (kLse only)
   int lq, lk, h;
   float sm_scale;
 };
 
-template <typename T>
+// kLse: also lse[b, h, row] = m_used + log2(l), the row log-sum-exp of the scores in the log2 domain with m_used the maximum the
+// lazy rescale last used (tdb200_sla_attn16_fwd_lse's convention), for the backward (sla_attn_bwd.cu) to recompute P from.
+template <typename T, bool kLse>
 __global__ void __launch_bounds__(split::kThreads, 1)
 dense_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                       const __grid_constant__ CUtensorMap tmap_v, DenseParams p) {
@@ -135,14 +138,16 @@ dense_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     const float l_tot = quad_sum(l_part[h]);   // all four lanes of a row take part, stored or not
     const int64_t qr = int64_t(m_blk) * BQ + r_lo + 8 * h;
     if (qr >= p.lq) continue;
+    if constexpr (kLse)
+      if (cq == 0) p.lse[(int64_t(b) * p.h + hh) * p.lq + qr] = m_used[h] + __log2f(l_tot);
     store_o_row<T, HD>(static_cast<T*>(p.out) + ((int64_t(b) * p.lq + qr) * p.h + hh) * HD, o, h, 1.0f / l_tot, cq);
   }
 }
 
-template <typename T>
+template <typename T, bool kLse>
 int launch(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const DenseParams& p, dim3 grid, cudaStream_t st) {
   static bool smem_set[64];
-  const auto kern = dense_attn_fwd_kernel<T>;
+  const auto kern = dense_attn_fwd_kernel<T, kLse>;
   if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), kSmemBytes, smem_set, "cudaFuncSetAttribute(dense_attn)"))
     return rc;
   kern<<<grid, split::kThreads, kSmemBytes, st>>>(tq, tk, tv, p);
@@ -181,6 +186,7 @@ static_assert(kNumBars * 8 <= 256, "barriers exceed their shared-memory slot");
 struct Params {
   void* out;     // [b, lq, h, d] T
   void* out_t;   // [b, lq, h, d] T
+  float* lse;    // [b, h, lq] fp32, log2 domain (kLse only)
   int lq, lk, h;
   float sm_scale;
 };
@@ -235,7 +241,8 @@ __device__ __forceinline__ void softmax_step_jvp(float (&s)[BK / 2], float (&o)[
   }
 }
 
-template <typename T>
+// kLse: also the row lse of the primal, as dense_attn_fwd_kernel<T, true> stores it
+template <typename T, bool kLse>
 __global__ void __launch_bounds__(split::kThreads, 1)
 dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                       const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_qt,
@@ -372,6 +379,8 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     const int64_t qr = int64_t(m_blk) * BQ + r_lo + 8 * h;
     if (qr >= p.lq) continue;
     const int64_t row = ((int64_t(b) * p.lq + qr) * p.h + hh) * HD;
+    if constexpr (kLse)
+      if (cq == 0) p.lse[(int64_t(b) * p.h + hh) * p.lq + qr] = m_used[h] + __log2f(l_tot);
     const float inv_l = 1.0f / l_tot, mu_l = mu_tot * inv_l;
     store_o_row<T, HD>(static_cast<T*>(p.out) + row, o, h, inv_l, cq);
     T* trow = static_cast<T*>(p.out_t) + row;
@@ -384,10 +393,10 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   }
 }
 
-template <typename T>
+template <typename T, bool kLse>
 int launch(const CUtensorMap (&tm)[6], const Params& p, dim3 grid, cudaStream_t st) {
   static bool smem_set[64];
-  const auto kern = dense_attn_jvp_kernel<T>;
+  const auto kern = dense_attn_jvp_kernel<T, kLse>;
   if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), kSmemBytes, smem_set, "cudaFuncSetAttribute(dense_attn_jvp)"))
     return rc;
   kern<<<grid, split::kThreads, kSmemBytes, st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p);
@@ -395,95 +404,102 @@ int launch(const CUtensorMap (&tm)[6], const Params& p, dim3 grid, cudaStream_t 
 }
 }  // namespace jvp
 
-}  // namespace
+// [b, l, h, HD] 16-bit tensor, boxes of 64 columns x `rows` sequence rows of one head
+int tmap16(CUtensorMap* m, const void* base, int dtype, int64_t b, int64_t l, int64_t h, uint32_t rows) {
+  const CUtensorMapDataType t16 = dtype == TDB200_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const uint64_t dims[4] = {uint64_t(HD), uint64_t(h), uint64_t(l), uint64_t(b)};
+  const uint64_t str[3] = {uint64_t(HD * 2), uint64_t(h * HD * 2), uint64_t(l * h * HD * 2)};
+  const uint32_t box[4] = {64, 1, rows, 1};
+  return make_tmap_4d(m, base, t16, 2, dims, str, box);
+}
 
-extern "C" int tdb200_attn_dense_fwd(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq,
-                                     int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  if (!q || !k || !v || !out) return fail(TDB200_ERR_INVALID_ARG, "attn_dense_fwd: null pointer");
-  if (b <= 0 || lq <= 0 || lk <= 0 || h <= 0 || d <= 0)
-    return fail(TDB200_ERR_INVALID_ARG, "attn_dense_fwd: bad shape (b=%lld, lq=%lld, lk=%lld, h=%lld, d=%lld)", (long long)b,
-                (long long)lq, (long long)lk, (long long)h, (long long)d);
+bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
+
+// tdb200_attn_dense_fwd (lse null) and tdb200_attn_dense_fwd_lse; `what` prefixes the messages
+int dense_fwd(const char* what, const void* q, const void* k, const void* v, int dtype, void* out, float* lse, bool with_lse,
+              int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
+  if (!q || !k || !v || !out || (with_lse && !lse)) return fail(TDB200_ERR_INVALID_ARG, "%s: null pointer", what);
+  if (int rc = dense_attn_shape(what, b, lq, lk, h, d)) return rc;
   if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out))
-    return fail(TDB200_ERR_INVALID_ARG, "attn_dense_fwd: q, k, v and out must be 16-byte aligned");
-  if (dtype != TDB200_DTYPE_BF16 && dtype != TDB200_DTYPE_FP16) return fail(TDB200_ERR_UNSUPPORTED, "attn_dense_fwd: dtype tag %d", dtype);
-  if (d != HD) return fail(TDB200_ERR_UNSUPPORTED, "attn_dense_fwd: head dim %lld (this kernel implements d=128)", (long long)d);
-  // grid (query blocks, h, b); int32 TMA coordinates; tensor-map strides below 2^40 bytes
-  constexpr int64_t kMaxStride = int64_t(1) << 40;
-  if (h > 65535 || b > 65535 || lq > 0x7FFFFFFF || lk > 0x7FFFFFFF || lq * h * d * 2 >= kMaxStride || lk * h * d * 2 >= kMaxStride)
-    return fail(TDB200_ERR_UNSUPPORTED, "attn_dense_fwd: dimension too large (b, h <= 65535; lq * h * d and lk * h * d below 2^39)");
+    return fail(TDB200_ERR_INVALID_ARG, "%s: q, k, v and out must be 16-byte aligned", what);
+  if (with_lse && !aligned4(lse)) return fail(TDB200_ERR_INVALID_ARG, "%s: lse must be 4-byte aligned", what);
+  if (int rc = dense_attn_limits(what, dtype, b, lq, lk, h, d)) return rc;
   if (int rc = require_sm90()) return rc;
 
-  const CUtensorMapDataType t16 = dtype == TDB200_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUtensorMap tq, tk, tv;
-  {
-    const uint64_t dims[4] = {uint64_t(d), uint64_t(h), uint64_t(lq), uint64_t(b)};
-    const uint64_t str[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(lq * h * d * 2)};
-    const uint32_t box[4] = {64, 1, BQ, 1};
-    if (int rc = make_tmap_4d(&tq, q, t16, 2, dims, str, box)) return rc;
-  }
-  {
-    const uint64_t dims[4] = {uint64_t(d), uint64_t(h), uint64_t(lk), uint64_t(b)};
-    const uint64_t str[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(lk * h * d * 2)};
-    const uint32_t box[4] = {64, 1, BK, 1};
-    if (int rc = make_tmap_4d(&tk, k, t16, 2, dims, str, box)) return rc;
-    if (int rc = make_tmap_4d(&tv, v, t16, 2, dims, str, box)) return rc;
-  }
+  if (int rc = tmap16(&tq, q, dtype, b, lq, h, BQ)) return rc;
+  if (int rc = tmap16(&tk, k, dtype, b, lk, h, BK)) return rc;
+  if (int rc = tmap16(&tv, v, dtype, b, lk, h, BK)) return rc;
   DenseParams p;
   p.out = out;
+  p.lse = lse;
   p.lq = int(lq);
   p.lk = int(lk);
   p.h = int(h);
   p.sm_scale = sm_scale;
   const dim3 grid(static_cast<unsigned>(cdiv64(lq, BQ)), static_cast<unsigned>(h), static_cast<unsigned>(b));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (dtype == TDB200_DTYPE_BF16) return launch<__nv_bfloat16>(tq, tk, tv, p, grid, st);
-  return launch<__half>(tq, tk, tv, p, grid, st);
+  const bool bf16 = dtype == TDB200_DTYPE_BF16;
+  if (!with_lse) return bf16 ? launch<__nv_bfloat16, false>(tq, tk, tv, p, grid, st) : launch<__half, false>(tq, tk, tv, p, grid, st);
+  return bf16 ? launch<__nv_bfloat16, true>(tq, tk, tv, p, grid, st) : launch<__half, true>(tq, tk, tv, p, grid, st);
+}
+
+// tdb200_attn_dense_jvp (lse null) and tdb200_attn_dense_jvp_lse
+int dense_jvp(const char* what, const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+              int dtype, void* out, void* out_t, float* lse, bool with_lse, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d,
+              float sm_scale, void* stream) {
+  if (!q || !k || !v || !q_t || !k_t || !v_t || !out || !out_t || (with_lse && !lse))
+    return fail(TDB200_ERR_INVALID_ARG, "%s: null pointer", what);
+  if (int rc = dense_attn_shape(what, b, lq, lk, h, d)) return rc;
+  if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(q_t) || !aligned16(k_t) || !aligned16(v_t) ||
+      !aligned16(out) || !aligned16(out_t))
+    return fail(TDB200_ERR_INVALID_ARG, "%s: q, k, v, their tangents, out and out_t must be 16-byte aligned", what);
+  if (with_lse && !aligned4(lse)) return fail(TDB200_ERR_INVALID_ARG, "%s: lse must be 4-byte aligned", what);
+  if (int rc = dense_attn_limits(what, dtype, b, lq, lk, h, d)) return rc;
+  if (int rc = require_sm90()) return rc;
+
+  CUtensorMap tm[6];   // q, k, v, q_t, k_t, v_t
+  if (int rc = tmap16(&tm[0], q, dtype, b, lq, h, BQ)) return rc;
+  if (int rc = tmap16(&tm[3], q_t, dtype, b, lq, h, BQ)) return rc;
+  if (int rc = tmap16(&tm[1], k, dtype, b, lk, h, jvp::BK)) return rc;
+  if (int rc = tmap16(&tm[2], v, dtype, b, lk, h, jvp::BK)) return rc;
+  if (int rc = tmap16(&tm[4], k_t, dtype, b, lk, h, jvp::BK)) return rc;
+  if (int rc = tmap16(&tm[5], v_t, dtype, b, lk, h, jvp::BK)) return rc;
+  jvp::Params p;
+  p.out = out;
+  p.out_t = out_t;
+  p.lse = lse;
+  p.lq = int(lq);
+  p.lk = int(lk);
+  p.h = int(h);
+  p.sm_scale = sm_scale;
+  const dim3 grid(static_cast<unsigned>(cdiv64(lq, BQ)), static_cast<unsigned>(h), static_cast<unsigned>(b));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool bf16 = dtype == TDB200_DTYPE_BF16;
+  if (!with_lse) return bf16 ? jvp::launch<__nv_bfloat16, false>(tm, p, grid, st) : jvp::launch<__half, false>(tm, p, grid, st);
+  return bf16 ? jvp::launch<__nv_bfloat16, true>(tm, p, grid, st) : jvp::launch<__half, true>(tm, p, grid, st);
+}
+
+}  // namespace
+
+extern "C" int tdb200_attn_dense_fwd(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq,
+                                     int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
+  return dense_fwd("attn_dense_fwd", q, k, v, dtype, out, nullptr, false, b, lq, lk, h, d, sm_scale, stream);
+}
+
+extern "C" int tdb200_attn_dense_fwd_lse(const void* q, const void* k, const void* v, int dtype, void* out, float* lse, int64_t b,
+                                         int64_t lq, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
+  return dense_fwd("attn_dense_fwd_lse", q, k, v, dtype, out, lse, true, b, lq, lk, h, d, sm_scale, stream);
 }
 
 extern "C" int tdb200_attn_dense_jvp(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
                                      const void* v_t, int dtype, void* out, void* out_t, int64_t b, int64_t lq, int64_t lk,
                                      int64_t h, int64_t d, float sm_scale, void* stream) {
-  if (!q || !k || !v || !q_t || !k_t || !v_t || !out || !out_t) return fail(TDB200_ERR_INVALID_ARG, "attn_dense_jvp: null pointer");
-  if (b <= 0 || lq <= 0 || lk <= 0 || h <= 0 || d <= 0)
-    return fail(TDB200_ERR_INVALID_ARG, "attn_dense_jvp: bad shape (b=%lld, lq=%lld, lk=%lld, h=%lld, d=%lld)", (long long)b,
-                (long long)lq, (long long)lk, (long long)h, (long long)d);
-  if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(q_t) || !aligned16(k_t) || !aligned16(v_t) ||
-      !aligned16(out) || !aligned16(out_t))
-    return fail(TDB200_ERR_INVALID_ARG, "attn_dense_jvp: q, k, v, their tangents, out and out_t must be 16-byte aligned");
-  if (dtype != TDB200_DTYPE_BF16 && dtype != TDB200_DTYPE_FP16) return fail(TDB200_ERR_UNSUPPORTED, "attn_dense_jvp: dtype tag %d", dtype);
-  if (d != HD) return fail(TDB200_ERR_UNSUPPORTED, "attn_dense_jvp: head dim %lld (this kernel implements d=128)", (long long)d);
-  constexpr int64_t kMaxStride = int64_t(1) << 40;
-  if (h > 65535 || b > 65535 || lq > 0x7FFFFFFF || lk > 0x7FFFFFFF || lq * h * d * 2 >= kMaxStride || lk * h * d * 2 >= kMaxStride)
-    return fail(TDB200_ERR_UNSUPPORTED, "attn_dense_jvp: dimension too large (b, h <= 65535; lq * h * d and lk * h * d below 2^39)");
-  if (int rc = require_sm90()) return rc;
+  return dense_jvp("attn_dense_jvp", q, k, v, q_t, k_t, v_t, dtype, out, out_t, nullptr, false, b, lq, lk, h, d, sm_scale, stream);
+}
 
-  const CUtensorMapDataType t16 = dtype == TDB200_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  CUtensorMap tm[6];   // q, k, v, q_t, k_t, v_t
-  {
-    const uint64_t dims[4] = {uint64_t(d), uint64_t(h), uint64_t(lq), uint64_t(b)};
-    const uint64_t str[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(lq * h * d * 2)};
-    const uint32_t box[4] = {64, 1, BQ, 1};
-    if (int rc = make_tmap_4d(&tm[0], q, t16, 2, dims, str, box)) return rc;
-    if (int rc = make_tmap_4d(&tm[3], q_t, t16, 2, dims, str, box)) return rc;
-  }
-  {
-    const uint64_t dims[4] = {uint64_t(d), uint64_t(h), uint64_t(lk), uint64_t(b)};
-    const uint64_t str[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(lk * h * d * 2)};
-    const uint32_t box[4] = {64, 1, jvp::BK, 1};
-    if (int rc = make_tmap_4d(&tm[1], k, t16, 2, dims, str, box)) return rc;
-    if (int rc = make_tmap_4d(&tm[2], v, t16, 2, dims, str, box)) return rc;
-    if (int rc = make_tmap_4d(&tm[4], k_t, t16, 2, dims, str, box)) return rc;
-    if (int rc = make_tmap_4d(&tm[5], v_t, t16, 2, dims, str, box)) return rc;
-  }
-  jvp::Params p;
-  p.out = out;
-  p.out_t = out_t;
-  p.lq = int(lq);
-  p.lk = int(lk);
-  p.h = int(h);
-  p.sm_scale = sm_scale;
-  const dim3 grid(static_cast<unsigned>(cdiv64(lq, BQ)), static_cast<unsigned>(h), static_cast<unsigned>(b));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (dtype == TDB200_DTYPE_BF16) return jvp::launch<__nv_bfloat16>(tm, p, grid, st);
-  return jvp::launch<__half>(tm, p, grid, st);
+extern "C" int tdb200_attn_dense_jvp_lse(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
+                                         const void* v_t, int dtype, void* out, void* out_t, float* lse, int64_t b, int64_t lq,
+                                         int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
+  return dense_jvp("attn_dense_jvp_lse", q, k, v, q_t, k_t, v_t, dtype, out, out_t, lse, true, b, lq, lk, h, d, sm_scale, stream);
 }

@@ -164,6 +164,21 @@ int make_tmap_4d(CUtensorMap* out, const void* base, CUtensorMapDataType dtype, 
   return encode(out, dtype, 4, base, dims, strides_bytes, box, swizzle_bytes);
 }
 
+int dense_attn_shape(const char* what, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d) {
+  if (b > 0 && lq > 0 && lk > 0 && h > 0 && d > 0) return 0;
+  return fail(TDB200_ERR_INVALID_ARG, "%s: bad shape (b=%lld, lq=%lld, lk=%lld, h=%lld, d=%lld)", what, (long long)b, (long long)lq,
+              (long long)lk, (long long)h, (long long)d);
+}
+
+int dense_attn_limits(const char* what, int dtype, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d) {
+  if (dtype != TDB200_DTYPE_BF16 && dtype != TDB200_DTYPE_FP16) return fail(TDB200_ERR_UNSUPPORTED, "%s: dtype tag %d", what, dtype);
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "%s: head dim %lld (this kernel implements d=128)", what, (long long)d);
+  constexpr int64_t kMaxStride = int64_t(1) << 40;
+  if (h > 65535 || b > 65535 || lq > 0x7FFFFFFF || lk > 0x7FFFFFFF || lq * h * d * 2 >= kMaxStride || lk * h * d * 2 >= kMaxStride)
+    return fail(TDB200_ERR_UNSUPPORTED, "%s: dimension too large (b, h <= 65535; lq * h * d and lk * h * d below 2^39)", what);
+  return 0;
+}
+
 }  // namespace tdb
 
 namespace tdb {

@@ -41,4 +41,11 @@ int set_max_dynamic_smem_once(const void* func, size_t bytes, bool* done_per_dev
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
+// The size checks the dense attention entry points share (dense_attn.cu, sla_attn_bwd.cu), messages prefixed with `what`.
+// dense_attn_shape: non-positive b, lq, lk, h or d -> TDB200_ERR_INVALID_ARG.  dense_attn_limits: a bad dtype tag, d != 128,
+// b or h above 65535 (grid y and z), lq or lk above 2^31 - 1 (int32 TMA coordinates), lq*h*d or lk*h*d of 2^39 elements or
+// more (tensor-map strides below 2^40 bytes) -> TDB200_ERR_UNSUPPORTED.
+int dense_attn_shape(const char* what, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d);
+int dense_attn_limits(const char* what, int dtype, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d);
+
 }  // namespace tdb

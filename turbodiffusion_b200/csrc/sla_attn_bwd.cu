@@ -15,9 +15,14 @@
 //                             block's list; S^T = K.Q^T, dP^T = V.dO^T, dV += P^T.dO, dK += dS^T.Q  (Q / dO tiles MN-major);
 //                             one template for both query-block heights
 //
+// Dense attention (tdb200_attn_dense_bwd, the backward of dense_attn.cu's kLse forwards, lq != lk allowed) runs the delta
+// kernel and the 128-row dQ and dK/dV kernels with kDense: the dQ CTA visits every 64-key tile and the dK/dV CTA every 128-row
+// query block, in ascending order, with no LUT staging, no index read and no index kernel.  kDense is a compile-time choice
+// that only replaces where a block id comes from; the per-tile arithmetic is the same instructions.
+//
 // Rounding points (FlashAttention-2's): P and dS are formed in fp32 and rounded to T only as MMA operands; dQ, dK, dV accumulate
 // in fp32 registers and are rounded to T once.  No floating-point atomics: every output element is written by one thread in a
-// fixed order, so the gradients are bit-for-bit reproducible.  Key columns >= l are masked to -inf; query rows >= l get
+// fixed order, so the gradients are bit-for-bit reproducible.  Key columns >= lk are masked to -inf; query rows >= lq get
 // lse = +inf (P = 0) and delta = 0 explicitly, because TMA zero-fill gives their scores, not their statistics.
 #include <type_traits>
 
@@ -30,15 +35,17 @@ using namespace tdb;
 constexpr int HD = 128, BLKQ = 128, BLKQ64 = 64, BLKK = 64;
 
 struct BwdParams {
-  const float* lse;        // [b,h,l]
-  const float* delta;      // [b,h,l]
-  const int32_t* lut;      // [b,h,mblk,topk]       (dQ)
-  const int32_t* kv_off;   // [b*h, nblk+1]          (dK/dV: CSR offsets into kv_idx)
+  const float* lse;        // [b,h,lq]
+  const float* delta;      // [b,h,lq]
+  const int32_t* lut;      // [b,h,mblk,topk]       (dQ; not read by the dense kernels)
+  const int32_t* kv_off;   // [b*h, nblk+1]          (dK/dV: CSR offsets into kv_idx; not read by the dense kernels)
   const int32_t* kv_idx;   // [b*h, mblk*topk]
-  void* dq;                // [b,l,h,d] T
-  void* dk;
+  void* dq;                // [b,lq,h,d] T
+  void* dk;                // [b,lk,h,d] T
   void* dv;
-  int l, h, mblk, nblk, topk;
+  int lq, lk;              // query and key lengths (lq = lk = l for SLA)
+  int h, mblk, nblk;       // mblk / nblk: query / key blocks
+  int topk;                // key blocks per query block (dense: nblk)
   float sm_scale;
 };
 
@@ -137,7 +144,7 @@ constexpr uint32_t kOffBars = kOffV + kStages * kTileK, kOffLut = kOffBars + 256
 enum Bar { kQFull = 0, kKFull = 1, kKEmpty = 4, kVFull = 7, kVEmpty = 10 };
 }  // namespace dq
 
-template <typename T>
+template <typename T, bool kDense = false>
 __global__ void __launch_bounds__(dq::kThreads, 1)
 sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
                   const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v, BwdParams p) {
@@ -161,7 +168,7 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
     }
     mbar_fence_init();
   }
-  {
+  if constexpr (!kDense) {
     const int32_t* lut_row = p.lut + (int64_t(bh) * p.mblk + m_blk) * p.topk;
     for (int i = threadIdx.x; i < p.topk; i += kThreads) s_lut[i] = static_cast<uint16_t>(__ldg(lut_row + i));
   }
@@ -183,7 +190,7 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
       for (int j = 0; j < p.topk; ++j) {
         const int st = j % kStages;
         const uint32_t ph = ((j / kStages) & 1) ^ 1;
-        const int blk = s_lut[j];
+        const int blk = kDense ? j : s_lut[j];
         mbar_wait(&bars[kKEmpty + st], ph);
         mbar_expect_tx(&bars[kKFull + st], kTileK);
 #pragma unroll
@@ -209,8 +216,8 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     const int64_t r = int64_t(m_blk) * BLKQ + r_lo + 8 * hf;
-    lse[hf] = r < p.l ? __ldg(p.lse + int64_t(bh) * p.l + r) : INFINITY;
-    dlt[hf] = r < p.l ? __ldg(p.delta + int64_t(bh) * p.l + r) : 0.f;
+    lse[hf] = r < p.lq ? __ldg(p.lse + int64_t(bh) * p.lq + r) : INFINITY;
+    dlt[hf] = r < p.lq ? __ldg(p.delta + int64_t(bh) * p.lq + r) : 0.f;
   }
   float acc[HD / 2];
 #pragma unroll
@@ -220,7 +227,7 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
   for (int j = 0; j < p.topk; ++j) {
     const int st = j % kStages;
     const uint32_t ph = (j / kStages) & 1;
-    const int valid = p.l - s_lut[j] * BLKK;
+    const int valid = p.lk - (kDense ? j : s_lut[j]) * BLKK;
     const uint32_t sk = sbase + kOffK + st * kTileK, sv = sbase + kOffV + st * kTileK;
 
     // ---- S = Q.K^T and dP = dO.V^T for this warpgroup's 64 rows (all operands K-major over d)
@@ -273,7 +280,7 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
     __syncwarp();
     if (lane == 0) mbar_arrive(&bars[kKEmpty + st]);
   }
-  store_rows<T>(acc, p.sm_scale, p.dq, int64_t(m_blk) * BLKQ + r_lo, p.l, p.h, hh, b, cq);
+  store_rows<T>(acc, p.sm_scale, p.dq, int64_t(m_blk) * BLKQ + r_lo, p.lq, p.h, hh, b, cq);
 }
 
 // ------------------------------------------------------------------------------------------------ dK / dV
@@ -301,7 +308,7 @@ struct Dkv {
   static_assert(HD * 128 * 4 <= 2 * kStages * kTileQ, "partial dK / dV do not fit in the ring");
 };
 
-template <typename T, int kBQ>
+template <typename T, int kBQ, bool kDense = false>
 __global__ void __launch_bounds__(split::kThreads, 1)
 sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
                     const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v, BwdParams p) {
@@ -314,15 +321,19 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
   const int bh = b * p.h + hh;
-  const int32_t* kv_off = p.kv_off + int64_t(bh) * (p.nblk + 1);
-  const int32_t* list = p.kv_idx + int64_t(bh) * p.mblk * p.topk + __ldg(kv_off + n_blk);
-  const int n_list = __ldg(kv_off + n_blk + 1) - __ldg(kv_off + n_blk);
+  const int32_t* list = nullptr;   // the query blocks of this key block: list[j], or (kDense) j for every j < mblk
+  int n_list = p.mblk;
+  if constexpr (!kDense) {
+    const int32_t* kv_off = p.kv_off + int64_t(bh) * (p.nblk + 1);
+    list = p.kv_idx + int64_t(bh) * p.mblk * p.topk + __ldg(kv_off + n_blk);
+    n_list = __ldg(kv_off + n_blk + 1) - __ldg(kv_off + n_blk);
+  }
 
   if (n_list == 0) {  // no query block selected this key block: its gradients are zero (the outputs are not pre-zeroed)
     for (int e = threadIdx.x; e < BLKK * HD / 8; e += split::kThreads) {
       const int64_t r = int64_t(n_blk) * BLKK + e / (HD / 8);
-      if (r >= p.l) break;
-      const int64_t o = ((int64_t(b) * p.l + r) * p.h + hh) * HD + (e % (HD / 8)) * 8;
+      if (r >= p.lk) break;
+      const int64_t o = ((int64_t(b) * p.lk + r) * p.h + hh) * HD + (e % (HD / 8)) * 8;
       stg_v4(static_cast<T*>(p.dk) + o, make_uint4(0, 0, 0, 0));
       stg_v4(static_cast<T*>(p.dv) + o, make_uint4(0, 0, 0, 0));
     }
@@ -355,7 +366,7 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
       for (int j = 0; j < n_list; ++j) {
         const int st = j % kStages;
         const uint32_t ph = ((j / kStages) & 1) ^ 1;
-        const int qb = __ldg(list + j);
+        const int qb = kDense ? j : __ldg(list + j);
         mbar_wait(&bars[L::kEmpty + st], ph);
         mbar_expect_tx(&bars[L::kFull + st], 2 * L::kTileQ);
 #pragma unroll
@@ -385,13 +396,13 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   for (int j = L::kSplit ? wg : 0, it = 0; j < n_list; j += L::kSplit ? 2 : 1, ++it) {
     const int st = j % kStages;
     const uint32_t ph = (j / kStages) & 1;
-    const int qb = __ldg(list + j);
-    // ---- lse / delta of this warpgroup's 64 query rows; query rows >= l: P = 0 and delta = 0
+    const int qb = kDense ? j : __ldg(list + j);
+    // ---- lse / delta of this warpgroup's 64 query rows; query rows >= lq: P = 0 and delta = 0
     float* sb = stats + ((L::kSplit ? it : j) & 1) * 128;
     {
       const int64_t r = int64_t(qb) * kBQ + q0 + (t & 63);
-      const bool in = r < p.l;
-      sb[t] = t < 64 ? (in ? __ldg(p.lse + int64_t(bh) * p.l + r) : INFINITY) : (in ? __ldg(p.delta + int64_t(bh) * p.l + r) : 0.f);
+      const bool in = r < p.lq;
+      sb[t] = t < 64 ? (in ? __ldg(p.lse + int64_t(bh) * p.lq + r) : INFINITY) : (in ? __ldg(p.delta + int64_t(bh) * p.lq + r) : 0.f);
     }
     named_bar_sync(1 + wg, 128);
 
@@ -420,7 +431,7 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     reg_fence(dp);
 
     // ---- P^T (columns = query rows) rounded to T; dV += P^T.dO with dO as the MN-major operand (+16 rows = +2048 B per K step).
-    //      Key rows >= l only reach dK / dV rows that are never stored, so they need no mask.
+    //      Key rows >= lk only reach dK / dV rows that are never stored, so they need no mask.
     uint32_t pa[4][4], da[4][4];
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
@@ -469,8 +480,8 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     dv[i] += x[HD / 2 + i];
   }
   const int64_t row0 = int64_t(n_blk) * BLKK + kr_lo;
-  store_rows<T>(dk, p.sm_scale, p.dk, row0, p.l, p.h, hh, b, cq);
-  store_rows<T>(dv, 1.0f, p.dv, row0, p.l, p.h, hh, b, cq);
+  store_rows<T>(dk, p.sm_scale, p.dk, row0, p.lk, p.h, hh, b, cq);
+  store_rows<T>(dv, 1.0f, p.dv, row0, p.lk, p.h, hh, b, cq);
 }
 
 // ------------------------------------------------------------------------------------------------ dQ on 64-row query blocks
@@ -554,8 +565,8 @@ sla_bwd_dq_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     const int64_t r = int64_t(m_blk) * BLKQ64 + r_lo + 8 * hf;
-    lse[hf] = r < p.l ? __ldg(p.lse + int64_t(bh) * p.l + r) : INFINITY;
-    dlt[hf] = r < p.l ? __ldg(p.delta + int64_t(bh) * p.l + r) : 0.f;
+    lse[hf] = r < p.lq ? __ldg(p.lse + int64_t(bh) * p.lq + r) : INFINITY;
+    dlt[hf] = r < p.lq ? __ldg(p.delta + int64_t(bh) * p.lq + r) : 0.f;
   }
   float acc[HD / 2];
 #pragma unroll
@@ -565,7 +576,7 @@ sla_bwd_dq_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   for (int j = wg; j < p.topk; j += 2) {
     const int st = j % kStages;
     const uint32_t ph = full_phase(j);
-    const int valid = p.l - s_lut[j] * BLKK;
+    const int valid = p.lk - s_lut[j] * BLKK;
     const uint32_t sk = sbase + kOffK + st * kTileK, sv = sbase + kOffV + st * kTileK;
 
     // ---- S = Q.K^T and dP = dO.V^T (all operands K-major over d)
@@ -627,7 +638,7 @@ sla_bwd_dq_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   if (wg == 1) return;
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) acc[i] += x[i];
-  store_rows<T>(acc, p.sm_scale, p.dq, int64_t(m_blk) * BLKQ64 + r_lo, p.l, p.h, hh, b, cq);
+  store_rows<T>(acc, p.sm_scale, p.dq, int64_t(m_blk) * BLKQ64 + r_lo, p.lq, p.h, hh, b, cq);
 }
 
 // ------------------------------------------------------------------------------------------------ host
@@ -688,7 +699,7 @@ int launch_bwd(const void* q, const void* k, const void* v, const void* o_s, con
   p.dq = dq;
   p.dk = dk;
   p.dv = dv;
-  p.l = int(l);
+  p.lq = p.lk = int(l);
   p.h = int(h);
   p.mblk = int(mblk);
   p.nblk = int(nblk);
@@ -776,4 +787,99 @@ extern "C" int tdb200_sla_attn_bwd_qk16(const void* q, const void* k, const void
                                         void* stream) {
   return tdb200_sla_attn16_bwd(q, k, v, o_s, d_o, lse, dtype, lut, topk, dq, dk, dv, workspace, workspace_bytes, b, l, h, d, sm_scale,
                                BLKQ, BLKK, stream);
+}
+
+// ------------------------------------------------------------------------------------------------ dense attention
+namespace {
+
+// The delta kernel's grid has one 8-row CTA per 8 rows of [b, lq, h], and grid.x stops at 2^31 - 1.
+constexpr int64_t kMaxDenseRows = int64_t(8) * 0x7FFFFFFF;
+
+bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
+
+// delta kernel, then dQ over every key tile and dK / dV over every 128-row query block (no index kernel)
+template <typename T>
+int launch_dense_bwd(const void* q, const void* k, const void* v, const void* out, const void* d_out, const float* lse, void* dq,
+                     void* dk, void* dv, float* delta, int64_t b, int64_t lq, int64_t lk, int64_t h, float sm_scale,
+                     cudaStream_t st) {
+  const CUtensorMapDataType t16 = std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                                        : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUtensorMap tq, tdo, tk, tv;
+  if (int rc = tmap_rows(&tq, q, t16, b, lq, h, BLKQ)) return rc;
+  if (int rc = tmap_rows(&tdo, d_out, t16, b, lq, h, BLKQ)) return rc;
+  if (int rc = tmap_rows(&tk, k, t16, b, lk, h, BLKK)) return rc;
+  if (int rc = tmap_rows(&tv, v, t16, b, lk, h, BLKK)) return rc;
+
+  const int64_t rows = b * lq * h;
+  sla_bwd_delta_kernel<T><<<unsigned(cdiv64(rows, 8)), 256, 0, st>>>(static_cast<const T*>(out), static_cast<const T*>(d_out), delta,
+                                                                       rows, int(lq), int(h));
+  if (int rc = check_launch("sla_bwd_delta_kernel")) return rc;
+
+  BwdParams p = {};
+  p.lse = lse;
+  p.delta = delta;
+  p.dq = dq;
+  p.dk = dk;
+  p.dv = dv;
+  p.lq = int(lq);
+  p.lk = int(lk);
+  p.h = int(h);
+  p.mblk = int(cdiv64(lq, BLKQ));
+  p.nblk = int(cdiv64(lk, BLKK));
+  p.topk = p.nblk;
+  p.sm_scale = sm_scale;
+
+  static bool smem_set_dq[64], smem_set_kv[64];
+  const auto dq_kern = sla_bwd_dq_kernel<T, true>;
+  const auto dkdv_kern = sla_bwd_dkdv_kernel<T, BLKQ, true>;
+  const size_t smem_dq = 1024 + dq::kOffLut, smem_kv = 1024 + Dkv<BLKQ>::kSmem;
+  if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(dq_kern), smem_dq, smem_set_dq, "cudaFuncSetAttribute(dense_bwd_dq)"))
+    return rc;
+  dq_kern<<<dim3(unsigned(p.mblk), unsigned(h), unsigned(b)), dq::kThreads, smem_dq, st>>>(tq, tdo, tk, tv, p);
+  if (int rc = check_launch("sla_bwd_dq_kernel")) return rc;
+  if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(dkdv_kern), smem_kv, smem_set_kv, "cudaFuncSetAttribute(dense_bwd_dkdv)"))
+    return rc;
+  dkdv_kern<<<dim3(unsigned(p.nblk), unsigned(h), unsigned(b)), split::kThreads, smem_kv, st>>>(tq, tdo, tk, tv, p);
+  return check_launch("sla_bwd_dkdv_kernel");
+}
+
+}  // namespace
+
+extern "C" int64_t tdb200_attn_dense_bwd_workspace_bytes(int64_t b, int64_t h, int64_t lq) {
+  if (b <= 0 || h <= 0 || lq <= 0)
+    return fail(TDB200_ERR_INVALID_ARG, "attn_dense_bwd_workspace_bytes: bad shape (b=%lld, h=%lld, lq=%lld)", (long long)b,
+                (long long)h, (long long)lq);
+  if (b > 65535 || h > 65535 || lq > 0x7FFFFFFF || b * h * lq > kMaxDenseRows)
+    return fail(TDB200_ERR_UNSUPPORTED, "attn_dense_bwd_workspace_bytes: dimension too large (b, h <= 65535; b * lq * h <= 8 * (2^31 - 1))");
+  return b * h * lq * int64_t(sizeof(float));
+}
+
+extern "C" int tdb200_attn_dense_bwd(const void* q, const void* k, const void* v, const void* out, const void* d_out, const float* lse,
+                                     int dtype, void* dq, void* dk, void* dv, void* workspace, int64_t workspace_bytes, int64_t b,
+                                     int64_t lq, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
+  const char* what = "attn_dense_bwd";
+  if (!q || !k || !v || !out || !d_out || !lse || !dq || !dk || !dv || !workspace)
+    return fail(TDB200_ERR_INVALID_ARG, "%s: null pointer", what);
+  if (int rc = dense_attn_shape(what, b, lq, lk, h, d)) return rc;
+  if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out) || !aligned16(d_out) || !aligned16(dq) || !aligned16(dk) ||
+      !aligned16(dv))
+    return fail(TDB200_ERR_INVALID_ARG, "%s: q, k, v, out, d_out, dq, dk and dv must be 16-byte aligned", what);
+  if (!aligned4(lse) || !aligned4(workspace)) return fail(TDB200_ERR_INVALID_ARG, "%s: lse and workspace must be 4-byte aligned", what);
+  if (int rc = dense_attn_limits(what, dtype, b, lq, lk, h, d)) return rc;
+  if (b * lq * h > kMaxDenseRows)
+    return fail(TDB200_ERR_UNSUPPORTED, "%s: dimension too large (b * lq * h above 8 * (2^31 - 1), the delta kernel's grid)", what);
+  const int64_t need = tdb200_attn_dense_bwd_workspace_bytes(b, h, lq);
+  if (workspace_bytes < need)
+    return fail(TDB200_ERR_WORKSPACE, "%s: workspace of %lld bytes, %lld needed", what, (long long)workspace_bytes, (long long)need);
+  if (int rc = require_sm90()) return rc;
+  // Autograd calls a backward from a worker thread of its own, on which no runtime call may yet have made the device's
+  // primary context current; the tensor maps are encoded through the driver API, which needs one.
+  int dev = 0;
+  if (int rc = check_cuda(cudaGetDevice(&dev), "cudaGetDevice")) return rc;
+  if (int rc = check_cuda(cudaSetDevice(dev), "cudaSetDevice")) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  float* delta = static_cast<float*>(workspace);
+  if (dtype == TDB200_DTYPE_BF16)
+    return launch_dense_bwd<__nv_bfloat16>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, h, sm_scale, st);
+  return launch_dense_bwd<__half>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, h, sm_scale, st);
 }

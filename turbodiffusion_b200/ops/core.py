@@ -335,21 +335,94 @@ def wan_rope_angles(t: int, h: int, w: int, head_dim: int, device=None) -> torch
     return out if device is None else out.to(device)
 
 
+def _dense_args(what, q, k, v):
+    if q.dim() != 4 or k.shape != v.shape or k.dim() != 4 or (q.shape[0], *q.shape[2:]) != (k.shape[0], *k.shape[2:]):
+        raise ValueError(f"{what}: q [B, Lq, H, D] and k, v [B, Lk, H, D] expected, got {tuple(q.shape)}, "
+                         f"{tuple(k.shape)}, {tuple(v.shape)}")
+    return q.dtype if q.dtype in DTYPE_TAG else torch.bfloat16
+
+
+def _needs_grad(*tensors) -> bool:
+    """The training path's rule, the SLA modules' too: grad mode on and a primal input that requires grad."""
+    return torch.is_grad_enabled() and any(t.requires_grad for t in tensors)
+
+
+def _dense_bwd(ctx, d_out):
+    """(dq, dk, dv) from tdb200_attn_dense_bwd, for the tensors the lse forward saved."""
+    q, k, v, out, lse = ctx.saved_tensors
+    b, lq, h, d = q.shape
+    lk = k.shape[1]
+    d_out = d_out.to(q.dtype).contiguous()
+    dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+    nbytes = lib().tdb200_attn_dense_bwd_workspace_bytes(b, h, lq)
+    check(0 if nbytes >= 0 else nbytes, "attn_dense_bwd_workspace_bytes", launches=0)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
+    check(lib().tdb200_attn_dense_bwd(ptr(q), ptr(k), ptr(v), ptr(out), ptr(d_out), ptr(lse), DTYPE_TAG[q.dtype], ptr(dq), ptr(dk),
+                                      ptr(dv), ptr(ws), nbytes, b, lq, lk, h, d, ctx.sm_scale, stream_ptr(q.device)),
+          "attn_dense_bwd")
+    return dq, dk, dv
+
+
+class _DenseAttention(torch.autograd.Function):
+    """dense_attention's training path on 16-bit contiguous q, k, v: the lse forward, and the dense backward."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, sm_scale):
+        b, lq, h, d = q.shape
+        out = torch.empty_like(q)
+        lse = torch.empty(b, h, lq, dtype=torch.float32, device=q.device)
+        check(lib().tdb200_attn_dense_fwd_lse(ptr(q), ptr(k), ptr(v), DTYPE_TAG[q.dtype], ptr(out), ptr(lse), b, lq, k.shape[1], h, d,
+                                              sm_scale, stream_ptr(q.device)), "attn_dense_fwd_lse")
+        ctx.save_for_backward(q, k, v, out, lse)
+        ctx.sm_scale = sm_scale
+        return out
+
+    @staticmethod
+    def backward(ctx, d_out):
+        return (*_dense_bwd(ctx, d_out), None)
+
+
+class _DenseAttentionJvp(torch.autograd.Function):
+    """dense_attention_jvp's training path: out differentiable in q, k and v; out_t, and the tangents, carry no gradient."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, q_t, k_t, v_t, sm_scale):
+        b, lq, h, d = q.shape
+        out, out_t = torch.empty_like(q), torch.empty_like(q)
+        lse = torch.empty(b, h, lq, dtype=torch.float32, device=q.device)
+        check(lib().tdb200_attn_dense_jvp_lse(ptr(q), ptr(k), ptr(v), ptr(q_t), ptr(k_t), ptr(v_t), DTYPE_TAG[q.dtype], ptr(out),
+                                              ptr(out_t), ptr(lse), b, lq, k.shape[1], h, d, sm_scale, stream_ptr(q.device)),
+              "attn_dense_jvp_lse")
+        ctx.mark_non_differentiable(out_t)
+        ctx.set_materialize_grads(False)    # out_t's gradient is never used: no zero tensor for it
+        ctx.save_for_backward(q, k, v, out, lse)
+        ctx.sm_scale = sm_scale
+        return out, out_t
+
+    @staticmethod
+    def backward(ctx, d_out, d_out_t):
+        if d_out is None:
+            return (None,) * 7
+        return (*_dense_bwd(ctx, d_out), None, None, None, None)
+
+
 def dense_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, sm_scale: Optional[float] = None) -> torch.Tensor:
     """softmax(q.k^T * sm_scale).v per (batch, head), the reference's dense attention (rcm/utils/attention.py:120-167):
     q [B, Lq, H, D], k and v [B, Lk, H, D], D = 128, any Lq and Lk; returns [B, Lq, H, D] in q's dtype.  bf16 / fp16 inputs run
     in their own type, any other float type in bf16.  sm_scale defaults to D ** -0.5.  One kernel on the current stream
-    (tdb200_attn_dense_fwd), the arithmetic of the 16-bit SLA kernel.  Forward only, and not a `tdb200::` operator: eager use."""
+    (tdb200_attn_dense_fwd), the arithmetic of the 16-bit SLA kernel.  With grad enabled and any of q, k, v requiring grad the
+    output is differentiable: the forward also stores the row lse (tdb200_attn_dense_fwd_lse, the same output bits) and the
+    backward is tdb200_attn_dense_bwd.  Not a `tdb200::` operator: eager use."""
     require_cuda(q, k, v)
-    if q.dim() != 4 or k.shape != v.shape or k.dim() != 4 or (q.shape[0], *q.shape[2:]) != (k.shape[0], *k.shape[2:]):
-        raise ValueError(f"dense_attention: q [B, Lq, H, D] and k, v [B, Lk, H, D] expected, got {tuple(q.shape)}, "
-                         f"{tuple(k.shape)}, {tuple(v.shape)}")
-    dtype = q.dtype if q.dtype in DTYPE_TAG else torch.bfloat16
+    dtype = _dense_args("dense_attention", q, k, v)
     qc, kc, vc = (t.to(dtype).contiguous() for t in (q, k, v))
     b, lq, h, d = qc.shape
+    sm_scale = float(d ** -0.5 if sm_scale is None else sm_scale)
+    if _needs_grad(q, k, v):
+        return _DenseAttention.apply(qc, kc, vc, sm_scale).to(q.dtype)
     out = torch.empty_like(qc)
-    check(lib().tdb200_attn_dense_fwd(ptr(qc), ptr(kc), ptr(vc), DTYPE_TAG[dtype], ptr(out), b, lq, kc.shape[1], h, d,
-                                      float(d ** -0.5 if sm_scale is None else sm_scale), stream_ptr(qc.device)),
+    check(lib().tdb200_attn_dense_fwd(ptr(qc), ptr(kc), ptr(vc), DTYPE_TAG[dtype], ptr(out), b, lq, kc.shape[1], h, d, sm_scale,
+                                      stream_ptr(qc.device)),
           "attn_dense_fwd")
     return out.to(q.dtype)
 
@@ -359,20 +432,23 @@ def dense_attention_jvp(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, q_t: 
     """dense_attention(q, k, v) and its forward-mode derivative along the tangents (q_t, k_t, v_t), from one kernel
     (tdb200_attn_dense_jvp): (out, out_t) with out_t = sum_j P_j S_t,j v_j - (sum_j P_j S_t,j) out + P.v_t, S_t =
     sm_scale (q_t.k^T + q.k_t^T).  Shapes and dtype rules as dense_attention; each tangent has its primal's shape and runs in
-    the primal's 16-bit type.  Both outputs are [B, Lq, H, D] in q's dtype.  Not a `tdb200::` operator: eager use."""
+    the primal's 16-bit type.  Both outputs are [B, Lq, H, D] in q's dtype.  With grad enabled and any of q, k, v requiring
+    grad, out is differentiable in q, k and v (tdb200_attn_dense_jvp_lse, the same bits, then tdb200_attn_dense_bwd), as a
+    consistency-distillation loss needs; out_t never carries a gradient (a stop-gradient target) and the tangents get none.
+    Not a `tdb200::` operator: eager use."""
     require_cuda(q, k, v, q_t, k_t, v_t)
-    if q.dim() != 4 or k.shape != v.shape or k.dim() != 4 or (q.shape[0], *q.shape[2:]) != (k.shape[0], *k.shape[2:]):
-        raise ValueError(f"dense_attention_jvp: q [B, Lq, H, D] and k, v [B, Lk, H, D] expected, got {tuple(q.shape)}, "
-                         f"{tuple(k.shape)}, {tuple(v.shape)}")
+    dtype = _dense_args("dense_attention_jvp", q, k, v)
     for name, t, primal in (("q_t", q_t, q), ("k_t", k_t, k), ("v_t", v_t, v)):
         if t.shape != primal.shape:
             raise ValueError(f"dense_attention_jvp: {name} {tuple(t.shape)} must have its primal's shape {tuple(primal.shape)}")
-    dtype = q.dtype if q.dtype in DTYPE_TAG else torch.bfloat16
     qc, kc, vc, qtc, ktc, vtc = (t.to(dtype).contiguous() for t in (q, k, v, q_t, k_t, v_t))
     b, lq, h, d = qc.shape
+    sm_scale = float(d ** -0.5 if sm_scale is None else sm_scale)
+    if _needs_grad(q, k, v):
+        out, out_t = _DenseAttentionJvp.apply(qc, kc, vc, qtc, ktc, vtc, sm_scale)
+        return out.to(q.dtype), out_t.to(q.dtype)
     out, out_t = torch.empty_like(qc), torch.empty_like(qc)
     check(lib().tdb200_attn_dense_jvp(ptr(qc), ptr(kc), ptr(vc), ptr(qtc), ptr(ktc), ptr(vtc), DTYPE_TAG[dtype], ptr(out),
-                                      ptr(out_t), b, lq, kc.shape[1], h, d, float(d ** -0.5 if sm_scale is None else sm_scale),
-                                      stream_ptr(qc.device)),
+                                      ptr(out_t), b, lq, kc.shape[1], h, d, sm_scale, stream_ptr(qc.device)),
           "attn_dense_jvp")
     return out.to(q.dtype), out_t.to(q.dtype)

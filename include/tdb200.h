@@ -337,6 +337,31 @@ int tdb200_attn_dense_bwd(const void* q, const void* k, const void* v, const voi
 int64_t tdb200_attn_dense_bwd_workspace_bytes(int64_t b, int64_t h, int64_t lq);
 
 /* ---------------------------------------------------------------------------------------------
+ * a9' JVP. Forward-mode derivative of the sparse softmax branch of a9' (SparseLinearAttention.forward_jvp, the tangent pass of
+ * rCM / sCM distillation through sparse attention): the f1 JVP restricted to the key blocks lut[b, h, m, :] lists.
+ *   o_s   = T( softmax over the listed keys of S ) . v                      (tdb200_sla_attn16_fwd_lse's o_s: no linear branch)
+ *   o_s_t = T( sum_j P_j S_t,j v_j - (sum_j P_j S_t,j) o_s + P.v_t )          j over the listed keys, S_t as for f1 JVP
+ * q, k, v, their tangents, o_s and o_s_t [b, l, h, d] contiguous 16-bit of type `dtype`, 16-byte aligned, read and written in
+ * place; lut [b, h, ceil(l / blkq), topk] int32 of distinct key-block ids (1 <= topk <= nblk = ceil(l / blkk)), 4-byte aligned.
+ * (blkq, blkk) = (128, 64) only: the f1 JVP kernel's 128-row query block over 64-key tiles, its tile ids read from the LUT in list
+ * order.  Keys >= l are masked, rows >= l are stored to neither output.  The arithmetic is tdb200_attn_dense_jvp's, step for step,
+ * so on an ascending LUT listing every key block the outputs are its bits.  d = 128.  One kernel launch, no workspace, no host
+ * synchronisation; no atomics, so the bits of a (batch, head) depend only on its own inputs.
+ *   tdb200_sla_attn16_jvp_lse  also lse [b, h, l] fp32 = m + log2(l) in log2 units, the convention tdb200_sla_attn16_bwd reads,
+ *                              so the gradient of o_s goes through the existing SLA backward.
+ * Errors, all before any CUDA call: (blkq, blkk) other than (128, 64) -> TDB200_ERR_UNSUPPORTED ((64, 64) included: its CTA holds
+ * one 64-row query block); any pointer null, a 16-bit tensor not 16-byte aligned, lut or lse not 4-byte aligned, non-positive b,
+ * l, h or d, topk outside [1, nblk] -> TDB200_ERR_INVALID_ARG; bad dtype tag, d != 128, the size limits of f1, topk above 8640
+ * (the LUT row is staged in shared memory) -> TDB200_ERR_UNSUPPORTED.
+ * ------------------------------------------------------------------------------------------- */
+int tdb200_sla_attn16_jvp(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                          int dtype, const int32_t* lut, int64_t topk, void* o_s, void* o_s_t, int64_t b, int64_t l, int64_t h,
+                          int64_t d, float sm_scale, int64_t blkq, int64_t blkk, void* stream);
+int tdb200_sla_attn16_jvp_lse(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                              int dtype, const int32_t* lut, int64_t topk, void* o_s, void* o_s_t, float* lse, int64_t b, int64_t l,
+                              int64_t h, int64_t d, float sm_scale, int64_t blkq, int64_t blkk, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * a12. LTX-2 (TurboT2AV) prologue variants   (ltx_core/model/transformer/transformer.py:21-94; Triton fast path
  *      ltx_distillation/fast_norm_kernels.py:388-473).  x, y, residual [b, tokens, n] 16-bit; table [num_ada, n] fp32;
  *      timestep [b, ts_tokens, num_ada*n] 16-bit with ts_tokens in {1, tokens}; ada value i = table[i] + timestep[.., i, :].

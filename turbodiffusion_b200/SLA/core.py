@@ -11,11 +11,12 @@ from __future__ import annotations
 
 
 import torch
+import torch.autograd.forward_ad as fwAD
 import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import _ops
-from .._lib import require_cuda
+from .._lib import DTYPE_TAG, check, lib, ptr, require_cuda, stream_ptr
 from .utils import (SAGE_BLOCKS, QKPrep, block_map_from_pools, get_block_map, get_cuda_arch, quant_k_into,  # noqa: F401
                     quant_q_only, quant_qk)
 
@@ -91,6 +92,63 @@ def sparse_attention16(q, k, v, lut, topk, sm_scale, blkq=128):
     """o_s = block-sparse softmax attention of q, k, v ([B,L,H,D], 16-bit, d = 128) over `lut`'s key blocks (`blkq`-row query
     blocks, 64-row key blocks), differentiable in q, k and v (the reference's `_attention`, SLA/kernel.py:240-319)."""
     return attn_fwd_qk16_lse(q, k, v, lut, topk, sm_scale, blkq)[0]
+
+
+def _jvp_call(q, k, v, q_t, k_t, v_t, lut, topk, sm_scale, blkq, with_lse):
+    b, l, h, d = q.shape
+    o_s, o_s_t = torch.empty_like(q), torch.empty_like(q)
+    if not with_lse:
+        check(lib().tdb200_sla_attn16_jvp(ptr(q), ptr(k), ptr(v), ptr(q_t), ptr(k_t), ptr(v_t), DTYPE_TAG[q.dtype], ptr(lut), topk,
+                                          ptr(o_s), ptr(o_s_t), b, l, h, d, sm_scale, blkq, _ops.BLKK16, stream_ptr(q.device)),
+              "sla_attn16_jvp")
+        return o_s, o_s_t, None
+    lse = torch.empty(b, h, l, dtype=torch.float32, device=q.device)
+    check(lib().tdb200_sla_attn16_jvp_lse(ptr(q), ptr(k), ptr(v), ptr(q_t), ptr(k_t), ptr(v_t), DTYPE_TAG[q.dtype], ptr(lut), topk,
+                                          ptr(o_s), ptr(o_s_t), ptr(lse), b, l, h, d, sm_scale, blkq, _ops.BLKK16,
+                                          stream_ptr(q.device)),
+          "sla_attn16_jvp_lse")
+    return o_s, o_s_t, lse
+
+
+def attn_jvp_qk16(q, k, v, q_t, k_t, v_t, lut, topk, sm_scale, blkq=128):
+    """(o_s, o_s_t): attn_fwd_qk16_lse's o_s and its forward-mode derivative along the tangents (q_t, k_t, v_t), the softmax
+    restricted to `lut`'s key blocks held fixed (tdb200_sla_attn16_jvp, one kernel).  All [B,L,H,D] contiguous in q.dtype,
+    d = 128, (blkq, blkk) = (128, 64).  Eager: not a `tdb200::` operator, no autograd."""
+    return _jvp_call(q, k, v, q_t, k_t, v_t, lut, topk, float(sm_scale), blkq, False)[:2]
+
+
+class _SparseAttention16Jvp(torch.autograd.Function):
+    """sparse_attention16_jvp's training path: o_s differentiable in q, k and v through the SLA backward (attn_bwd_qk16, fed
+    the lse of tdb200_sla_attn16_jvp_lse); o_s_t, and the tangents, carry no gradient."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, q_t, k_t, v_t, lut, topk, sm_scale, blkq):
+        o_s, o_s_t, lse = _jvp_call(q, k, v, q_t, k_t, v_t, lut, topk, sm_scale, blkq, True)
+        ctx.mark_non_differentiable(o_s_t)
+        ctx.set_materialize_grads(False)    # o_s_t's gradient is never used: no zero tensor for it
+        ctx.save_for_backward(q, k, v, o_s, lse, lut)
+        ctx.topk, ctx.sm_scale, ctx.blkq = topk, sm_scale, blkq
+        return o_s, o_s_t
+
+    @staticmethod
+    def backward(ctx, d_o, d_o_t):
+        if d_o is None:
+            return (None,) * 10
+        q, k, v, o_s, lse, lut = ctx.saved_tensors
+        dq, dk, dv = attn_bwd_qk16(q, k, v, o_s, d_o.to(q.dtype).contiguous(), lse, lut, ctx.topk, ctx.sm_scale, ctx.blkq)
+        return dq, dk, dv, None, None, None, None, None, None, None
+
+
+def sparse_attention16_jvp(q, k, v, q_t, k_t, v_t, lut, topk, sm_scale, blkq=128):
+    """(o_s, o_s_t): sparse_attention16's o_s and its tangent along (q_t, k_t, v_t) with the block selection `lut` held fixed
+    (it is piecewise constant in q, k).  q, k, v and the tangents [B,L,H,D] contiguous 16-bit of one dtype, d = 128, blkq = 128.
+    With grad enabled and any of q, k, v requiring grad, o_s is differentiable in q, k and v (the same bits, plus the row lse the
+    SLA backward reads); o_s_t never carries a gradient (a stop-gradient target) and the tangents get none."""
+    sm_scale = float(sm_scale)
+    q_t, k_t, v_t = q_t.detach(), k_t.detach(), v_t.detach()
+    if torch.is_grad_enabled() and any(t.requires_grad for t in (q, k, v)):
+        return _SparseAttention16Jvp.apply(q, k, v, q_t, k_t, v_t, lut, topk, sm_scale, blkq)
+    return attn_jvp_qk16(q, k, v, q_t, k_t, v_t, lut, topk, sm_scale, blkq)
 
 
 def select_prep(q, k, blkq, blkk):
@@ -182,6 +240,13 @@ class _SLABase(nn.Module):
         if getattr(self, "_keep_selection", None) is not None:
             self._keep_selection.update(lut=lut, sparse_map=sparse_map, topk=real_topk)
         o_s = sparse_attention16(q, k, v, lut, real_topk, d ** -0.5, blkq)
+        o = (o_s + self._linear_branch(q, k, v)).to(dtype).contiguous()
+        return (o, real_topk / nblk) if return_sparsity else o
+
+    def _linear_branch(self, q, k, v):
+        """proj_l(phi(q) (phi(k)^T v) / (1e-5 + phi(q).sum phi(k))) as [B, L, H, D] in self.dtype, in torch at the reference's
+        rounding points (SLA/core.py:104-117): feature maps -> dtype, bmm in dtype, proj_l evaluated in dtype as under its
+        autocast."""
         qh, kh, vh = (t.transpose(1, 2) for t in (q, k, v))                       # [B, H, L, D] views
         c_q = self.feature_map_q(qh).contiguous().to(self.dtype)
         c_k = self.feature_map_k(kh).contiguous().to(self.dtype)
@@ -189,8 +254,48 @@ class _SLABase(nn.Module):
         ksum = torch.sum(c_k, dim=-2, keepdim=True)
         o_l = (c_q @ kvsum) / (1e-5 + (c_q * ksum).sum(dim=-1, keepdim=True))
         o_l = F.linear(o_l.to(self.dtype), self.proj_l.weight.to(self.dtype), self.proj_l.bias.to(self.dtype))
-        o = (o_s + o_l.transpose(1, 2)).to(dtype).contiguous()
-        return (o, real_topk / nblk) if return_sparsity else o
+        return o_l.transpose(1, 2)
+
+    def forward_jvp(self, q, k, v, q_t, k_t, v_t, return_sparsity=False):
+        """forward(q, k, v) and its forward-mode derivative along the tangents (q_t, k_t, v_t): (o, o_t), both [B, L, H, D] in
+        q.dtype (plus the sparsity with return_sparsity), for the tangent pass of rCM / sCM consistency distillation.
+        The block selection is forward's, computed from the primal q, k; the tangent holds it fixed (it is piecewise constant).
+        The sparse branch is one kernel (sparse_attention16_jvp); the linear branch and proj_l are _forward_train's torch ops,
+        their tangent by torch forward-mode AD.  o is differentiable in q, k, v and proj_l as _forward_train's output is; o_t
+        never carries a gradient and the tangents get none.  Served for SparseLinearAttention with d = 128 and
+        (BLKQ, BLKK) = (128, 64); every other call raises NotImplementedError before any CUDA work.  Eager only: under
+        torch.compile it is a graph break, and it is not hooked into torch.func.jvp / forward_ad."""
+        if self.quantised_qk:
+            raise NotImplementedError("forward_jvp: SageSparseLinearAttention is inference-only (as in the reference); "
+                                      "use SparseLinearAttention")
+        if q.shape[-1] != 128:
+            raise NotImplementedError(f"forward_jvp: head dim {q.shape[-1]}; the sparse attention JVP is served for d = 128")
+        if (self.BLKQ, self.BLKK) != (128, 64):
+            raise NotImplementedError(f"forward_jvp: block sizes (BLKQ, BLKK) = ({self.BLKQ}, {self.BLKK}); the sparse attention "
+                                      "JVP is served for (128, 64)")
+        for name, t, primal in (("q_t", q_t, q), ("k_t", k_t, k), ("v_t", v_t, v)):
+            if t.shape != primal.shape:
+                raise ValueError(f"forward_jvp: {name} {tuple(t.shape)} must have its primal's shape {tuple(primal.shape)}")
+        require_cuda(q, k, v, q_t, k_t, v_t)
+        dtype = q.dtype
+        q, k, v = (t if (t.dtype == self.dtype and t.is_contiguous()) else t.to(self.dtype).contiguous() for t in (q, k, v))
+        q_t, k_t, v_t = (t.detach().to(self.dtype).contiguous() for t in (q_t, k_t, v_t))
+        d = q.shape[-1]
+        blkq, blkk = 128, 64
+        with torch.no_grad():
+            prep = select_prep(q.detach(), k.detach(), blkq, blkk)
+            nblk = prep.nblk
+            real_topk = max(1, min(nblk, int(self.topk * nblk)))
+            sparse_map, lut = block_map_from_pools(prep.q_pool, prep.k_pool, real_topk)
+        if getattr(self, "_keep_selection", None) is not None:
+            self._keep_selection.update(lut=lut, sparse_map=sparse_map, topk=real_topk)
+        o_s, o_s_t = sparse_attention16_jvp(q, k, v, q_t, k_t, v_t, lut, real_topk, d ** -0.5, blkq)
+        with fwAD.dual_level():
+            o_l = self._linear_branch(fwAD.make_dual(q, q_t), fwAD.make_dual(k, k_t), fwAD.make_dual(v, v_t))
+            o_l, o_l_t = fwAD.unpack_dual(o_l)
+        o = (o_s + o_l).to(dtype).contiguous()
+        o_t = (o_s_t + o_l_t.detach()).to(dtype).contiguous()
+        return (o, o_t, real_topk / nblk) if return_sparsity else (o, o_t)
 
     def forward_with_lut(self, q, k, v):
         """forward() that also returns the block selection it used: (o, {"lut": int32 [B,H,Mblk,topk] ascending key-block

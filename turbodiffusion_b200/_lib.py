@@ -65,6 +65,8 @@ _PROTOS = {
     "tdb200_attn_dense_jvp_lse": [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_attn_dense_bwd": [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_attn_dense_bwd_workspace_bytes": [_I64, _I64, _I64],
+    "tdb200_sla_attn16_jvp": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _I64, _I64, _I64, _I64, _F, _I64, _I64, _P],
+    "tdb200_sla_attn16_jvp_lse": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _I64, _I64, _I64, _I64, _F, _I64, _I64, _P],
     "tdb200_ltx_modulated_rms_norm_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_ltx_modulate_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
     "tdb200_ltx_gated_residual_ada": [_P, _P, _I, _P, _P, _I, _I, _P, _I64, _I64, _I64, _I64, _P],

@@ -166,6 +166,11 @@ int launch(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, 
 // p Sd rounded to T; then O += P.V, A += (P Sd).V and A += P.Vd as one commit group.
 // CTA per (128-row query block, head, batch), the forward's warp roles.  Shared memory: Q and Qd resident (64 KB), a 2-stage
 // (K, Kd) ring and a 2-stage (V, Vd) ring of 32 KB per stage: 192 KB.  A third stage of both rings would need 256 KB.
+// kSparse (tdb200_sla_attn16_jvp): the same kernel over the key blocks lut[b, h, m, :] lists, in list order, instead of tiles
+// 0 .. ceil(lk / 64) - 1; the 64-key tile is the SLA key block (BLKK = 64), the 128-row query block its BLKQ = 128.  The LUT row
+// is staged in shared memory behind the barriers (4 * topk bytes) and the producer and the consumers read the same ids from it;
+// keys are masked by their absolute column, blk * 64 + c >= lk.  Only the source of the tile index changes, so on an ascending
+// LUT listing every key block the sparse kernel computes the dense one's bits.
 namespace jvp {
 constexpr int BK = 64;
 constexpr int kStages = 2;
@@ -178,6 +183,9 @@ constexpr uint32_t kOffV = kOffK + kStages * kStageBytes;
 constexpr uint32_t kOffBars = kOffV + kStages * kStageBytes;
 constexpr size_t kSmemBytes = 1024 + kOffBars + 256;
 static_assert(kSmemBytes <= 227 * 1024, "shared memory of the dense attention JVP kernel");
+constexpr uint32_t kOffLut = kOffBars + 256;                        // kSparse: the CTA's LUT row, int32 [topk]
+constexpr size_t kSparseSmemMax = 227 * 1024;
+constexpr int64_t kMaxLutIds = (kSparseSmemMax - kSmemBytes) / 4;   // 8640 ids: topk of any l up to 552,960 keys
 
 enum Bar { kQFull = 0, kKFull = 1, kKEmpty = kKFull + kStages, kVFull = kKEmpty + kStages, kVEmpty = kVFull + kStages,
            kNumBars = kVEmpty + kStages };
@@ -189,6 +197,8 @@ struct Params {
   float* lse;    // [b, h, lq] fp32, log2 domain (kLse only)
   int lq, lk, h;
   float sm_scale;
+  const int32_t* lut;   // [b, h, mblk, topk] key-block ids (kSparse only)
+  int topk, mblk;
 };
 
 // d (+)= Q.K^T over one 64-key tile: Q rows at sq (HD/64 chunks kQBytes/2 apart), K at sk (chunks BK * 128 bytes apart)
@@ -242,7 +252,7 @@ __device__ __forceinline__ void softmax_step_jvp(float (&s)[BK / 2], float (&o)[
 }
 
 // kLse: also the row lse of the primal, as dense_attn_fwd_kernel<T, true> stores it
-template <typename T, bool kLse>
+template <typename T, bool kLse, bool kSparse = false>
 __global__ void __launch_bounds__(split::kThreads, 1)
 dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                       const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_qt,
@@ -251,10 +261,11 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
+  int32_t* s_lut = reinterpret_cast<int32_t*>(smem + kOffLut);   // kSparse only
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
-  const int n_tiles = (p.lk + BK - 1) / BK;
+  const int n_tiles = kSparse ? p.topk : (p.lk + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
     mbar_init(&bars[kQFull], 1);
@@ -265,6 +276,10 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
       mbar_init(&bars[kVEmpty + i], kConsumerWarps);
     }
     mbar_fence_init();
+  }
+  if constexpr (kSparse) {
+    const int32_t* lut_row = p.lut + ((int64_t(b) * p.h + hh) * p.mblk + m_blk) * p.topk;
+    for (int i = threadIdx.x; i < p.topk; i += split::kThreads) s_lut[i] = __ldg(lut_row + i);
   }
   __syncthreads();
 
@@ -287,21 +302,22 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
       for (int j = 0; j < n_tiles; ++j) {
         const int st = j % kStages;
         const uint32_t ph = ((j / kStages) & 1) ^ 1;
+        const int key0 = (kSparse ? s_lut[j] : j) * BK;
         mbar_wait(&bars[kKEmpty + st], ph);
         mbar_expect_tx(&bars[kKFull + st], kStageBytes);
         uint8_t* sk = smem + kOffK + st * kStageBytes;
 #pragma unroll
         for (int c = 0; c < HD / 64; ++c) {
-          tma_load_4d(sk + c * (BK * 128), &tmap_k, &bars[kKFull + st], c * 64, hh, j * BK, b);
-          tma_load_4d(sk + kHalfBytes + c * (BK * 128), &tmap_kt, &bars[kKFull + st], c * 64, hh, j * BK, b);
+          tma_load_4d(sk + c * (BK * 128), &tmap_k, &bars[kKFull + st], c * 64, hh, key0, b);
+          tma_load_4d(sk + kHalfBytes + c * (BK * 128), &tmap_kt, &bars[kKFull + st], c * 64, hh, key0, b);
         }
         mbar_wait(&bars[kVEmpty + st], ph);
         mbar_expect_tx(&bars[kVFull + st], kStageBytes);
         uint8_t* sv = smem + kOffV + st * kStageBytes;
 #pragma unroll
         for (int c = 0; c < HD / 64; ++c) {
-          tma_load_4d(sv + c * (BK * 128), &tmap_v, &bars[kVFull + st], c * 64, hh, j * BK, b);
-          tma_load_4d(sv + kHalfBytes + c * (BK * 128), &tmap_vt, &bars[kVFull + st], c * 64, hh, j * BK, b);
+          tma_load_4d(sv + c * (BK * 128), &tmap_v, &bars[kVFull + st], c * 64, hh, key0, b);
+          tma_load_4d(sv + kHalfBytes + c * (BK * 128), &tmap_vt, &bars[kVFull + st], c * 64, hh, key0, b);
         }
       }
     }
@@ -331,7 +347,7 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     float s[BK / 2], sd[BK / 2];
     mbar_wait(&bars[kKFull + st], ph);
     score_tile<true, HD, BK, kBF16>(s, sq, BQ * 128, sk, sc);
-    softmax_step_jvp(s, o, a, m_used, l_part, mu_part, p.lk - j * BK, cq, j == 0);   // s := p
+    softmax_step_jvp(s, o, a, m_used, l_part, mu_part, p.lk - (kSparse ? s_lut[j] : j) * BK, cq, j == 0);   // s := p
 #pragma unroll
     for (int i = 0; i < BK / 2; ++i) sd[i] = 0.f;
     wgmma_fence();
@@ -401,6 +417,18 @@ int launch(const CUtensorMap (&tm)[6], const Params& p, dim3 grid, cudaStream_t 
     return rc;
   kern<<<grid, split::kThreads, kSmemBytes, st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p);
   return check_launch("dense_attn_jvp_kernel");
+}
+
+// kSparse: the dynamic shared memory grows by the LUT row, so the attribute is set once to the largest size any topk may use
+template <typename T, bool kLse>
+int launch_sparse(const CUtensorMap (&tm)[6], const Params& p, dim3 grid, cudaStream_t st) {
+  static bool smem_set[64];
+  const auto kern = dense_attn_jvp_kernel<T, kLse, true>;
+  if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), kSparseSmemMax, smem_set,
+                                         "cudaFuncSetAttribute(sla_attn16_jvp)"))
+    return rc;
+  kern<<<grid, split::kThreads, kSmemBytes + 4 * size_t(p.topk), st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p);
+  return check_launch("sla_attn16_jvp_kernel");
 }
 }  // namespace jvp
 
@@ -480,6 +508,55 @@ int dense_jvp(const char* what, const void* q, const void* k, const void* v, con
   return bf16 ? jvp::launch<__nv_bfloat16, true>(tm, p, grid, st) : jvp::launch<__half, true>(tm, p, grid, st);
 }
 
+// tdb200_sla_attn16_jvp (lse null) and tdb200_sla_attn16_jvp_lse: the JVP kernel over the LUT's key blocks, lq = lk = l
+int sla_jvp(const char* what, const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+            int dtype, const int32_t* lut, int64_t topk, void* o_s, void* o_s_t, float* lse, bool with_lse, int64_t b, int64_t l,
+            int64_t h, int64_t d, float sm_scale, int64_t blkq, int64_t blkk, void* stream) {
+  if (blkq != BQ || blkk != jvp::BK)
+    return fail(TDB200_ERR_UNSUPPORTED, "%s: block sizes (%lld, %lld) (the JVP serves BLKQ x BLKK = 128 x 64)", what,
+                (long long)blkq, (long long)blkk);
+  if (!q || !k || !v || !q_t || !k_t || !v_t || !lut || !o_s || !o_s_t || (with_lse && !lse))
+    return fail(TDB200_ERR_INVALID_ARG, "%s: null pointer", what);
+  if (int rc = dense_attn_shape(what, b, l, l, h, d)) return rc;
+  if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(q_t) || !aligned16(k_t) || !aligned16(v_t) ||
+      !aligned16(o_s) || !aligned16(o_s_t))
+    return fail(TDB200_ERR_INVALID_ARG, "%s: q, k, v, their tangents, o_s and o_s_t must be 16-byte aligned", what);
+  if (!aligned4(lut) || (with_lse && !aligned4(lse))) return fail(TDB200_ERR_INVALID_ARG, "%s: lut and lse must be 4-byte aligned", what);
+  const int64_t nblk = cdiv64(l, jvp::BK);
+  if (topk <= 0 || topk > nblk)
+    return fail(TDB200_ERR_INVALID_ARG, "%s: topk=%lld outside [1, %lld]", what, (long long)topk, (long long)nblk);
+  if (int rc = dense_attn_limits(what, dtype, b, l, l, h, d)) return rc;
+  if (topk > jvp::kMaxLutIds)
+    return fail(TDB200_ERR_UNSUPPORTED, "%s: topk=%lld too large for the on-chip LUT (at most %lld)", what, (long long)topk,
+                (long long)jvp::kMaxLutIds);
+  if (int rc = require_sm90()) return rc;
+
+  CUtensorMap tm[6];   // q, k, v, q_t, k_t, v_t
+  if (int rc = tmap16(&tm[0], q, dtype, b, l, h, BQ)) return rc;
+  if (int rc = tmap16(&tm[3], q_t, dtype, b, l, h, BQ)) return rc;
+  if (int rc = tmap16(&tm[1], k, dtype, b, l, h, jvp::BK)) return rc;
+  if (int rc = tmap16(&tm[2], v, dtype, b, l, h, jvp::BK)) return rc;
+  if (int rc = tmap16(&tm[4], k_t, dtype, b, l, h, jvp::BK)) return rc;
+  if (int rc = tmap16(&tm[5], v_t, dtype, b, l, h, jvp::BK)) return rc;
+  jvp::Params p;
+  p.out = o_s;
+  p.out_t = o_s_t;
+  p.lse = lse;
+  p.lq = int(l);
+  p.lk = int(l);
+  p.h = int(h);
+  p.sm_scale = sm_scale;
+  p.lut = lut;
+  p.topk = int(topk);
+  p.mblk = int(cdiv64(l, BQ));
+  const dim3 grid(static_cast<unsigned>(p.mblk), static_cast<unsigned>(h), static_cast<unsigned>(b));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool bf16 = dtype == TDB200_DTYPE_BF16;
+  if (!with_lse)
+    return bf16 ? jvp::launch_sparse<__nv_bfloat16, false>(tm, p, grid, st) : jvp::launch_sparse<__half, false>(tm, p, grid, st);
+  return bf16 ? jvp::launch_sparse<__nv_bfloat16, true>(tm, p, grid, st) : jvp::launch_sparse<__half, true>(tm, p, grid, st);
+}
+
 }  // namespace
 
 extern "C" int tdb200_attn_dense_fwd(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq,
@@ -502,4 +579,19 @@ extern "C" int tdb200_attn_dense_jvp_lse(const void* q, const void* k, const voi
                                          const void* v_t, int dtype, void* out, void* out_t, float* lse, int64_t b, int64_t lq,
                                          int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
   return dense_jvp("attn_dense_jvp_lse", q, k, v, q_t, k_t, v_t, dtype, out, out_t, lse, true, b, lq, lk, h, d, sm_scale, stream);
+}
+
+extern "C" int tdb200_sla_attn16_jvp(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                                     int dtype, const int32_t* lut, int64_t topk, void* o_s, void* o_s_t, int64_t b, int64_t l,
+                                     int64_t h, int64_t d, float sm_scale, int64_t blkq, int64_t blkk, void* stream) {
+  return sla_jvp("sla_attn16_jvp", q, k, v, q_t, k_t, v_t, dtype, lut, topk, o_s, o_s_t, nullptr, false, b, l, h, d, sm_scale, blkq,
+                 blkk, stream);
+}
+
+extern "C" int tdb200_sla_attn16_jvp_lse(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
+                                         const void* v_t, int dtype, const int32_t* lut, int64_t topk, void* o_s, void* o_s_t,
+                                         float* lse, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale, int64_t blkq,
+                                         int64_t blkk, void* stream) {
+  return sla_jvp("sla_attn16_jvp_lse", q, k, v, q_t, k_t, v_t, dtype, lut, topk, o_s, o_s_t, lse, true, b, l, h, d, sm_scale, blkq,
+                 blkk, stream);
 }

@@ -362,6 +362,28 @@ int tdb200_sla_attn16_jvp_lse(const void* q, const void* k, const void* v, const
                               int64_t h, int64_t d, float sm_scale, int64_t blkq, int64_t blkk, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Tangents alone, from a saved primal: the forward-mode rules of ops.dense_attention and SparseLinearAttention.forward
+ * (torch.func.jvp / torch.autograd.forward_ad), whose primal the lse forward has already computed.
+ *   tdb200_attn_dense_tangent  out_t of f1 JVP for tangents q_t, k_t, v_t, given out and lse of tdb200_attn_dense_fwd_lse on the
+ *                              same q, k, v.  Shapes, layouts and argument checks as tdb200_attn_dense_jvp_lse, with out and lse
+ *                              read instead of written.
+ *   tdb200_sla_attn16_tangent  o_s_t of a9' JVP over the same lut, given o_s and lse of tdb200_sla_attn16_fwd_lse (blkq = 128).
+ *                              Shapes, layouts and argument checks as tdb200_sla_attn16_jvp_lse, with o_s and lse read.
+ * lse [b, h, lq] is the log2-domain row log-sum-exp, so P = exp2(S * sm_scale * log2e - lse) is the softmax without an online
+ * pass or a rescale:
+ *   out_t = T( (P o S_t).v + P.v_t - rowsum(P o S_t) out ),   S_t = sm_scale (q_t.k^T + q.k_t^T)
+ * The tensor core gets P and P o S_t rounded to T; the row sum is of the unrounded P o S_t; the last term reads the rounded out.
+ * f1 JVP's CTA and rings, 64-key tiles, keys >= lk masked; rows >= lq read no lse and are not stored.  No atomics, one kernel
+ * launch, no workspace, no host synchronisation.
+ * ------------------------------------------------------------------------------------------- */
+int tdb200_attn_dense_tangent(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                              const void* out, const float* lse, int dtype, void* out_t, int64_t b, int64_t lq, int64_t lk,
+                              int64_t h, int64_t d, float sm_scale, void* stream);
+int tdb200_sla_attn16_tangent(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                              const void* o_s, const float* lse, int dtype, const int32_t* lut, int64_t topk, void* o_s_t, int64_t b,
+                              int64_t l, int64_t h, int64_t d, float sm_scale, int64_t blkq, int64_t blkk, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * a12. LTX-2 (TurboT2AV) prologue variants   (ltx_core/model/transformer/transformer.py:21-94; Triton fast path
  *      ltx_distillation/fast_norm_kernels.py:388-473).  x, y, residual [b, tokens, n] 16-bit; table [num_ada, n] fp32;
  *      timestep [b, ts_tokens, num_ada*n] 16-bit with ts_tokens in {1, tokens}; ada value i = table[i] + timestep[.., i, :].

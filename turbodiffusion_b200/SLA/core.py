@@ -16,7 +16,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import _ops
-from .._lib import DTYPE_TAG, check, lib, ptr, require_cuda, stream_ptr
+from .._lib import DTYPE_TAG, check, has_tangent, lib, plain, ptr, require_cuda, stream_ptr
 from .utils import (SAGE_BLOCKS, QKPrep, block_map_from_pools, get_block_map, get_cuda_arch, quant_k_into,  # noqa: F401
                     quant_q_only, quant_qk)
 
@@ -151,6 +151,57 @@ def sparse_attention16_jvp(q, k, v, q_t, k_t, v_t, lut, topk, sm_scale, blkq=128
     return attn_jvp_qk16(q, k, v, q_t, k_t, v_t, lut, topk, sm_scale, blkq)
 
 
+class _SparseAttention16AD(torch.autograd.Function):
+    """SparseLinearAttention.forward's sparse branch for q, k, v of which one carries a forward-mode tangent: the block
+    selection from the primal q, k ((BLKQ, BLKK) = (128, 64), `topk` blocks per row; `module`'s _keep_selection, if set,
+    receives it: passed as the module, since torch.func rebuilds a dict argument), then
+    attn_fwd_qk16_lse once; jvp = tdb200_sla_attn16_tangent from the saved o_s and lse with the selection held fixed (missing
+    tangents are zeros); backward = attn_bwd_qk16.  lse and lut are outputs only so that setup_context can save them.  The
+    tangent carries no gradient."""
+
+    @staticmethod
+    def forward(q, k, v, topk, sm_scale, module):
+        prep = select_prep(q, k, 128, _ops.BLKK16)
+        sparse_map, lut = block_map_from_pools(prep.q_pool, prep.k_pool, topk)
+        keep = getattr(module, "_keep_selection", None)
+        if keep is not None:
+            keep.update(lut=lut, sparse_map=sparse_map, topk=topk)
+        o_s, lse = attn_fwd_qk16_lse(q, k, v, lut, topk, sm_scale, 128)
+        return o_s, lse, lut
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        q, k, v, topk, sm_scale, _ = inputs
+        o_s, lse, lut = output
+        ctx.mark_non_differentiable(lse, lut)
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(q, k, v, o_s, lse, lut)
+        ctx.save_for_forward(q, k, v, o_s, lse, lut)
+        ctx.topk, ctx.sm_scale = topk, sm_scale
+
+    @staticmethod
+    def jvp(ctx, q_t, k_t, v_t, *_):
+        with torch._C._DisableFuncTorch():
+            q, k, v, o_s, lse, lut = (plain(t) for t in ctx.saved_tensors)
+            q_t, k_t, v_t = (torch.zeros_like(p) if t is None else plain(t).detach().to(p.dtype).contiguous()
+                             for t, p in ((q_t, q), (k_t, k), (v_t, v)))
+            b, l, h, d = q.shape
+            o_s_t = torch.empty_like(q)
+            check(lib().tdb200_sla_attn16_tangent(ptr(q), ptr(k), ptr(v), ptr(q_t), ptr(k_t), ptr(v_t), ptr(o_s), ptr(lse),
+                                                  DTYPE_TAG[q.dtype], ptr(lut), ctx.topk, ptr(o_s_t), b, l, h, d, ctx.sm_scale, 128,
+                                                  _ops.BLKK16, stream_ptr(q.device)),
+                  "sla_attn16_tangent")
+        return o_s_t, None, None
+
+    @staticmethod
+    def backward(ctx, d_o, d_lse, d_lut):
+        if d_o is None:
+            return (None,) * 6
+        q, k, v, o_s, lse, lut = ctx.saved_tensors
+        dq, dk, dv = attn_bwd_qk16(q, k, v, o_s, d_o.to(q.dtype).contiguous(), lse, lut, ctx.topk, ctx.sm_scale, 128)
+        return dq, dk, dv, None, None, None
+
+
 def select_prep(q, k, blkq, blkk):
     """The pooled means (and Sage INT8 codes) block selection reads, for q, k [B, L, H, D]: quant_qk for the SageSLA families;
     (64, 64), a pair tdb200_sla_quant_qk does not take, from its query half at blkq = 64 and its key half at blkk = 64."""
@@ -190,7 +241,10 @@ class _SLABase(nn.Module):
     def forward(self, q, k, v, return_sparsity=False):
         """q,k,v [B, L, H, D] (any float dtype), D in {64, 128} (SLA/core.py:207) -> [B, L, H, D] in q.dtype.
         SparseLinearAttention with grad enabled and any of q, k, v requiring grad takes the differentiable training path
-        (_forward_train); every other call runs the fused forward-only kernels."""
+        (_forward_train); every other call runs the fused forward-only kernels.  When any of q, k, v carries a forward-mode
+        tangent (torch.func.jvp, torch.autograd.forward_ad), the call takes _forward_ad, whose output carries the tangent."""
+        if has_tangent(q, k, v):
+            return self._forward_ad(q, k, v, return_sparsity)
         if not self.quantised_qk and torch.is_grad_enabled() and any(t.requires_grad for t in (q, k, v)):
             return self._forward_train(q, k, v, return_sparsity)
         require_cuda(q, k, v)
@@ -243,6 +297,34 @@ class _SLABase(nn.Module):
         o = (o_s + self._linear_branch(q, k, v)).to(dtype).contiguous()
         return (o, real_topk / nblk) if return_sparsity else o
 
+    def _forward_ad(self, q, k, v, return_sparsity):
+        """forward() with a forward-AD rule: _forward_train's composition, the sparse branch through _SparseAttention16AD
+        (one primal forward with the training op's bits; its tangent by tdb200_sla_attn16_tangent with the block selection
+        held fixed; its backward the training op's) and the linear branch and proj_l in torch, whose forward AD gives their
+        tangent (under torch.func.jvp torch's jvp rules for those ops may round differently from the plain ops).  Served
+        where forward_jvp is; other calls raise NotImplementedError before any CUDA work."""
+        self._refuse_unserved_jvp("forward with a forward-mode tangent", q.shape[-1])
+        require_cuda(q, k, v)
+        dtype = q.dtype
+        q, k, v = (t if (t.dtype == self.dtype and t.is_contiguous()) else t.to(self.dtype).contiguous() for t in (q, k, v))
+        b, l, h, d = q.shape
+        nblk = (l + _ops.BLKK16 - 1) // _ops.BLKK16
+        real_topk = max(1, min(nblk, int(self.topk * nblk)))
+        o_s = _SparseAttention16AD.apply(q, k, v, real_topk, d ** -0.5, self)[0]
+        o = (o_s + self._linear_branch(q, k, v)).to(dtype).contiguous()
+        return (o, real_topk / nblk) if return_sparsity else o
+
+    def _refuse_unserved_jvp(self, what, d):
+        """NotImplementedError for the calls the sparse attention JVP and tangent kernels do not serve"""
+        if self.quantised_qk:
+            raise NotImplementedError(f"{what}: SageSparseLinearAttention is inference-only (as in the reference); "
+                                      "use SparseLinearAttention")
+        if d != 128:
+            raise NotImplementedError(f"{what}: head dim {d}; the sparse attention JVP is served for d = 128")
+        if (self.BLKQ, self.BLKK) != (128, 64):
+            raise NotImplementedError(f"{what}: block sizes (BLKQ, BLKK) = ({self.BLKQ}, {self.BLKK}); the sparse attention "
+                                      "JVP is served for (128, 64)")
+
     def _linear_branch(self, q, k, v):
         """proj_l(phi(q) (phi(k)^T v) / (1e-5 + phi(q).sum phi(k))) as [B, L, H, D] in self.dtype, in torch at the reference's
         rounding points (SLA/core.py:104-117): feature maps -> dtype, bmm in dtype, proj_l evaluated in dtype as under its
@@ -264,15 +346,9 @@ class _SLABase(nn.Module):
         their tangent by torch forward-mode AD.  o is differentiable in q, k, v and proj_l as _forward_train's output is; o_t
         never carries a gradient and the tangents get none.  Served for SparseLinearAttention with d = 128 and
         (BLKQ, BLKK) = (128, 64); every other call raises NotImplementedError before any CUDA work.  Eager only: under
-        torch.compile it is a graph break, and it is not hooked into torch.func.jvp / forward_ad."""
-        if self.quantised_qk:
-            raise NotImplementedError("forward_jvp: SageSparseLinearAttention is inference-only (as in the reference); "
-                                      "use SparseLinearAttention")
-        if q.shape[-1] != 128:
-            raise NotImplementedError(f"forward_jvp: head dim {q.shape[-1]}; the sparse attention JVP is served for d = 128")
-        if (self.BLKQ, self.BLKK) != (128, 64):
-            raise NotImplementedError(f"forward_jvp: block sizes (BLKQ, BLKK) = ({self.BLKQ}, {self.BLKK}); the sparse attention "
-                                      "JVP is served for (128, 64)")
+        torch.compile it is a graph break.  The same tangent is what forward() carries under torch.func.jvp / forward_ad
+        (_forward_ad); this is the explicit-tangent form of it."""
+        self._refuse_unserved_jvp("forward_jvp", q.shape[-1])
         for name, t, primal in (("q_t", q_t, q), ("k_t", k_t, k), ("v_t", v_t, v)):
             if t.shape != primal.shape:
                 raise ValueError(f"forward_jvp: {name} {tuple(t.shape)} must have its primal's shape {tuple(primal.shape)}")

@@ -9,6 +9,7 @@ import os
 from ctypes import c_char_p, c_float, c_int, c_int64, c_void_p
 
 import torch
+import torch.autograd.forward_ad as fwAD
 
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(PKG_DIR, "libtdb200.so")
@@ -67,6 +68,8 @@ _PROTOS = {
     "tdb200_attn_dense_bwd_workspace_bytes": [_I64, _I64, _I64],
     "tdb200_sla_attn16_jvp": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _I64, _I64, _I64, _I64, _F, _I64, _I64, _P],
     "tdb200_sla_attn16_jvp_lse": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _I64, _I64, _I64, _I64, _F, _I64, _I64, _P],
+    "tdb200_attn_dense_tangent": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I64, _I64, _I64, _I64, _I64, _F, _P],
+    "tdb200_sla_attn16_tangent": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _I64, _I64, _I64, _I64, _F, _I64, _I64, _P],
     "tdb200_ltx_modulated_rms_norm_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_ltx_modulate_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
     "tdb200_ltx_gated_residual_ada": [_P, _P, _I, _P, _P, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
@@ -159,6 +162,23 @@ def stream_ptr(device=None) -> int:
 
 def ptr(t):
     return 0 if t is None else t.data_ptr()
+
+
+def has_tangent(*tensors) -> bool:
+    """Any of the tensors carries a forward-mode tangent: a dual tensor at the current torch.autograd.forward_ad level, or an
+    input of torch.func.jvp (which runs on a forward_ad level of its own).  False while torch.compile traces."""
+    if torch.compiler.is_compiling():
+        return False
+    return any(t is not None and fwAD.unpack_dual(t).tangent is not None for t in tensors)
+
+
+def plain(t):
+    """The tensor under any torch.func wrappers: the same values, with a data pointer for the C ABI.  A forward-AD rule's jvp
+    sees its saved tensors and tangents wrapped at the torch.func.jvp level; it reads them through this, under
+    torch._C._DisableFuncTorch() so that the tensors it allocates are plain as well."""
+    while t is not None and torch._C._functorch.is_functorch_wrapped_tensor(t):
+        t = torch._C._functorch.get_unwrapped(t)
+    return t
 
 
 def require_cuda(*tensors) -> None:

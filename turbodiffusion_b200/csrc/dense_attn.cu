@@ -430,6 +430,192 @@ int launch_sparse(const CUtensorMap (&tm)[6], const Params& p, dim3 grid, cudaSt
   kern<<<grid, split::kThreads, kSmemBytes + 4 * size_t(p.topk), st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p);
   return check_launch("sla_attn16_jvp_kernel");
 }
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// Tangent alone, from the primal's saved out and lse (tdb200_attn_dense_tangent, tdb200_sla_attn16_tangent): the forward-AD rule
+// of the attention operators, whose primal the lse forward has already computed.  lse being the row's log-sum-exp of the
+// log2-domain scores, P = exp2(s - lse) is the normalised softmax itself, so there is no online softmax and no rescale:
+//   od = (P o Sd).V + P.Vd - rowsum(P o Sd) out.
+// Per 64-key tile: S, P (keys >= lk masked), Sd as one commit group; mu sums the unrounded P Sd, the tensor core gets P and
+// P Sd rounded to T; then A += (P Sd).V + P.Vd as one commit group.  The epilogue reads the forward's rounded out for the last
+// term, which saves the product O = P.V.  Five products per tile against the JVP kernel's six; warp roles, shared memory,
+// the rings and kSparse as dense_attn_jvp_kernel's.  Query rows >= lq read no lse and store nothing (their P is 0).
+// p.out and p.lse are inputs here.  The set-up and the producer are dense_attn_jvp_kernel's, written out again: moved into a
+// shared function they changed that kernel's register allocation.
+template <typename T, bool kSparse>
+__global__ void __launch_bounds__(split::kThreads, 1)
+attn_tangent_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                    const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_qt,
+                    const __grid_constant__ CUtensorMap tmap_kt, const __grid_constant__ CUtensorMap tmap_vt, Params p) {
+  constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBars);
+  int32_t* s_lut = reinterpret_cast<int32_t*>(smem + kOffLut);   // kSparse only
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
+  const int n_tiles = kSparse ? p.topk : (p.lk + BK - 1) / BK;
+
+  if (threadIdx.x == 0) {
+    mbar_init(&bars[kQFull], 1);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&bars[kKFull + i], 1);
+      mbar_init(&bars[kKEmpty + i], kConsumerWarps);
+      mbar_init(&bars[kVFull + i], 1);
+      mbar_init(&bars[kVEmpty + i], kConsumerWarps);
+    }
+    mbar_fence_init();
+  }
+  if constexpr (kSparse) {
+    const int32_t* lut_row = p.lut + ((int64_t(b) * p.h + hh) * p.mblk + m_blk) * p.topk;
+    for (int i = threadIdx.x; i < p.topk; i += split::kThreads) s_lut[i] = __ldg(lut_row + i);
+  }
+  __syncthreads();
+
+  if (warp >= kConsumerWarps) {
+    // =============================================================== TMA producer (dense_attn_jvp_kernel's)
+    reg_dealloc<split::kProducerRegs>();
+    if (warp == kConsumerWarps && lane == 0) {
+      tma_prefetch_desc(&tmap_q);
+      tma_prefetch_desc(&tmap_qt);
+      tma_prefetch_desc(&tmap_k);
+      tma_prefetch_desc(&tmap_kt);
+      tma_prefetch_desc(&tmap_v);
+      tma_prefetch_desc(&tmap_vt);
+      mbar_expect_tx(&bars[kQFull], 2 * kQBytes);
+#pragma unroll
+      for (int c = 0; c < HD / 64; ++c) {
+        tma_load_4d(smem + kOffQ + c * (BQ * 128), &tmap_q, &bars[kQFull], c * 64, hh, m_blk * BQ, b);
+        tma_load_4d(smem + kOffQd + c * (BQ * 128), &tmap_qt, &bars[kQFull], c * 64, hh, m_blk * BQ, b);
+      }
+      for (int j = 0; j < n_tiles; ++j) {
+        const int st = j % kStages;
+        const uint32_t ph = ((j / kStages) & 1) ^ 1;
+        const int key0 = (kSparse ? s_lut[j] : j) * BK;
+        mbar_wait(&bars[kKEmpty + st], ph);
+        mbar_expect_tx(&bars[kKFull + st], kStageBytes);
+        uint8_t* sk = smem + kOffK + st * kStageBytes;
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c) {
+          tma_load_4d(sk + c * (BK * 128), &tmap_k, &bars[kKFull + st], c * 64, hh, key0, b);
+          tma_load_4d(sk + kHalfBytes + c * (BK * 128), &tmap_kt, &bars[kKFull + st], c * 64, hh, key0, b);
+        }
+        mbar_wait(&bars[kVEmpty + st], ph);
+        mbar_expect_tx(&bars[kVFull + st], kStageBytes);
+        uint8_t* sv = smem + kOffV + st * kStageBytes;
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c) {
+          tma_load_4d(sv + c * (BK * 128), &tmap_v, &bars[kVFull + st], c * 64, hh, key0, b);
+          tma_load_4d(sv + kHalfBytes + c * (BK * 128), &tmap_vt, &bars[kVFull + st], c * 64, hh, key0, b);
+        }
+      }
+    }
+    return;
+  }
+
+  reg_alloc<split::kConsumerRegs>();
+  const int wg = warp >> 2, w4 = warp & 3;
+  const int r_lo = wg * 64 + w4 * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const uint32_t sbase = smem_u32(smem);
+  const uint32_t sq = sbase + kOffQ + wg * (64 * 128), sqd = sbase + kOffQd + wg * (64 * 128);
+  const float sc = p.sm_scale * kLog2e;
+
+  float lse[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t qr = int64_t(m_blk) * BQ + r_lo + 8 * h;
+    lse[h] = qr < p.lq ? p.lse[(int64_t(b) * p.h + hh) * p.lq + qr] : INFINITY;
+  }
+  float a[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) a[i] = 0.f;
+  float mu_part[2] = {0.f, 0.f};
+
+  mbar_wait(&bars[kQFull], 0);
+  for (int j = 0; j < n_tiles; ++j) {
+    const int st = j % kStages;
+    const uint32_t ph = (j / kStages) & 1;
+    const uint32_t sk = sbase + kOffK + st * kStageBytes, sv = sbase + kOffV + st * kStageBytes;
+
+    float s[BK / 2], sd[BK / 2];
+    mbar_wait(&bars[kKFull + st], ph);
+    score_tile<true, HD, BK, kBF16>(s, sq, BQ * 128, sk, sc);
+    const int valid = p.lk - (kSparse ? s_lut[j] : j) * BK;
+#pragma unroll
+    for (int i = 0; i < BK / 2; ++i) {
+      const float x = s[i] - lse[(i >> 1) & 1];
+      s[i] = valid < BK && 8 * (i >> 2) + cq + (i & 1) >= valid ? 0.f : fast_exp2(x);   // s := P
+    }
+#pragma unroll
+    for (int i = 0; i < BK / 2; ++i) sd[i] = 0.f;
+    wgmma_fence();
+    qk_mmas<kBF16>(sd, sqd, sk, false);               // Sd / c = Qd.K^T + Q.Kd^T
+    qk_mmas<kBF16>(sd, sq, sk + kHalfBytes, true);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(sd);
+    warp_release(&bars[kKEmpty + st], lane);
+
+    uint32_t pa[BK / 16][4], pda[BK / 16][4];        // P and P * Sd rounded to T: the A operands of the products
+#pragma unroll
+    for (int i = 0; i < BK / 2; i += 2) {
+      const int h = (i >> 1) & 1;
+      const float x0 = s[i] * (sd[i] * p.sm_scale), x1 = s[i + 1] * (sd[i + 1] * p.sm_scale);
+      mu_part[h] += x0 + x1;
+      pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(s[i], s[i + 1]);
+      pda[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(x0, x1);
+    }
+
+    mbar_wait(&bars[kVFull + st], ph);
+    const uint64_t vdesc = make_desc_mnmajor_sw128(sv, BK * 128), vddesc = make_desc_mnmajor_sw128(sv + kHalfBytes, BK * 128);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(a, pda[kk], vdesc + uint64_t(kk * 128));
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk) wgmma_f16_rs<HD, kBF16, 1>(a, pa[kk], vddesc + uint64_t(kk * 128));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(a);
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk) {
+      reg_fence(pa[kk]);
+      reg_fence(pda[kk]);
+    }
+    warp_release(&bars[kVEmpty + st], lane);
+  }
+
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float mu = quad_sum(mu_part[h]);   // all four lanes of a row take part
+    const int64_t qr = int64_t(m_blk) * BQ + r_lo + 8 * h;
+    if (qr >= p.lq) continue;
+    const int64_t row = ((int64_t(b) * p.lq + qr) * p.h + hh) * HD;
+    const T* orow = static_cast<const T*>(p.out) + row;
+    T* trow = static_cast<T*>(p.out_t) + row;
+#pragma unroll
+    for (int c = 0; c < HD / 8; ++c) {
+      const int i = 4 * c + 2 * h;
+      const uint32_t ow = *reinterpret_cast<const uint32_t*>(orow + 8 * c + cq);
+      *reinterpret_cast<uint32_t*>(trow + 8 * c + cq) =
+          F16Traits<T>::pack(fmaf(-mu, F16Traits<T>::lo(ow), a[i]), fmaf(-mu, F16Traits<T>::hi(ow), a[i + 1]));
+    }
+  }
+}
+
+// kSparse: the dynamic shared memory grows by the LUT row, as for launch_sparse
+template <typename T, bool kSparse>
+int launch_tangent(const CUtensorMap (&tm)[6], const Params& p, dim3 grid, cudaStream_t st) {
+  static bool smem_set[64];
+  const auto kern = attn_tangent_kernel<T, kSparse>;
+  const size_t smem_max = kSparse ? kSparseSmemMax : kSmemBytes;
+  if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), smem_max, smem_set,
+                                         kSparse ? "cudaFuncSetAttribute(sla_attn16_tangent)" : "cudaFuncSetAttribute(attn_dense_tangent)"))
+    return rc;
+  kern<<<grid, split::kThreads, kSmemBytes + (kSparse ? 4 * size_t(p.topk) : 0), st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p);
+  return check_launch(kSparse ? "sla_attn16_tangent_kernel" : "attn_dense_tangent_kernel");
+}
 }  // namespace jvp
 
 // [b, l, h, HD] 16-bit tensor, boxes of 64 columns x `rows` sequence rows of one head
@@ -472,10 +658,10 @@ int dense_fwd(const char* what, const void* q, const void* k, const void* v, int
   return bf16 ? launch<__nv_bfloat16, true>(tq, tk, tv, p, grid, st) : launch<__half, true>(tq, tk, tv, p, grid, st);
 }
 
-// tdb200_attn_dense_jvp (lse null) and tdb200_attn_dense_jvp_lse
+// tdb200_attn_dense_jvp (lse null), tdb200_attn_dense_jvp_lse and, `tangent`, tdb200_attn_dense_tangent (out and lse inputs)
 int dense_jvp(const char* what, const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
               int dtype, void* out, void* out_t, float* lse, bool with_lse, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d,
-              float sm_scale, void* stream) {
+              float sm_scale, void* stream, bool tangent = false) {
   if (!q || !k || !v || !q_t || !k_t || !v_t || !out || !out_t || (with_lse && !lse))
     return fail(TDB200_ERR_INVALID_ARG, "%s: null pointer", what);
   if (int rc = dense_attn_shape(what, b, lq, lk, h, d)) return rc;
@@ -504,14 +690,17 @@ int dense_jvp(const char* what, const void* q, const void* k, const void* v, con
   const dim3 grid(static_cast<unsigned>(cdiv64(lq, BQ)), static_cast<unsigned>(h), static_cast<unsigned>(b));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool bf16 = dtype == TDB200_DTYPE_BF16;
+  if (tangent)
+    return bf16 ? jvp::launch_tangent<__nv_bfloat16, false>(tm, p, grid, st) : jvp::launch_tangent<__half, false>(tm, p, grid, st);
   if (!with_lse) return bf16 ? jvp::launch<__nv_bfloat16, false>(tm, p, grid, st) : jvp::launch<__half, false>(tm, p, grid, st);
   return bf16 ? jvp::launch<__nv_bfloat16, true>(tm, p, grid, st) : jvp::launch<__half, true>(tm, p, grid, st);
 }
 
-// tdb200_sla_attn16_jvp (lse null) and tdb200_sla_attn16_jvp_lse: the JVP kernel over the LUT's key blocks, lq = lk = l
+// tdb200_sla_attn16_jvp (lse null) and tdb200_sla_attn16_jvp_lse: the JVP kernel over the LUT's key blocks, lq = lk = l;
+// `tangent`: tdb200_sla_attn16_tangent, the tangent kernel over them (o_s and lse inputs)
 int sla_jvp(const char* what, const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
             int dtype, const int32_t* lut, int64_t topk, void* o_s, void* o_s_t, float* lse, bool with_lse, int64_t b, int64_t l,
-            int64_t h, int64_t d, float sm_scale, int64_t blkq, int64_t blkk, void* stream) {
+            int64_t h, int64_t d, float sm_scale, int64_t blkq, int64_t blkk, void* stream, bool tangent = false) {
   if (blkq != BQ || blkk != jvp::BK)
     return fail(TDB200_ERR_UNSUPPORTED, "%s: block sizes (%lld, %lld) (the JVP serves BLKQ x BLKK = 128 x 64)", what,
                 (long long)blkq, (long long)blkk);
@@ -552,6 +741,8 @@ int sla_jvp(const char* what, const void* q, const void* k, const void* v, const
   const dim3 grid(static_cast<unsigned>(p.mblk), static_cast<unsigned>(h), static_cast<unsigned>(b));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool bf16 = dtype == TDB200_DTYPE_BF16;
+  if (tangent)
+    return bf16 ? jvp::launch_tangent<__nv_bfloat16, true>(tm, p, grid, st) : jvp::launch_tangent<__half, true>(tm, p, grid, st);
   if (!with_lse)
     return bf16 ? jvp::launch_sparse<__nv_bfloat16, false>(tm, p, grid, st) : jvp::launch_sparse<__half, false>(tm, p, grid, st);
   return bf16 ? jvp::launch_sparse<__nv_bfloat16, true>(tm, p, grid, st) : jvp::launch_sparse<__half, true>(tm, p, grid, st);
@@ -594,4 +785,19 @@ extern "C" int tdb200_sla_attn16_jvp_lse(const void* q, const void* k, const voi
                                          int64_t blkk, void* stream) {
   return sla_jvp("sla_attn16_jvp_lse", q, k, v, q_t, k_t, v_t, dtype, lut, topk, o_s, o_s_t, lse, true, b, l, h, d, sm_scale, blkq,
                  blkk, stream);
+}
+
+extern "C" int tdb200_attn_dense_tangent(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
+                                         const void* v_t, const void* out, const float* lse, int dtype, void* out_t, int64_t b,
+                                         int64_t lq, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
+  return dense_jvp("attn_dense_tangent", q, k, v, q_t, k_t, v_t, dtype, const_cast<void*>(out), out_t, const_cast<float*>(lse), true,
+                   b, lq, lk, h, d, sm_scale, stream, true);
+}
+
+extern "C" int tdb200_sla_attn16_tangent(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
+                                         const void* v_t, const void* o_s, const float* lse, int dtype, const int32_t* lut,
+                                         int64_t topk, void* o_s_t, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale,
+                                         int64_t blkq, int64_t blkk, void* stream) {
+  return sla_jvp("sla_attn16_tangent", q, k, v, q_t, k_t, v_t, dtype, lut, topk, const_cast<void*>(o_s), o_s_t, const_cast<float*>(lse),
+                 true, b, l, h, d, sm_scale, blkq, blkk, stream, true);
 }

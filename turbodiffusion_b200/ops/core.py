@@ -14,7 +14,7 @@ import torch
 import torch.nn as nn
 
 from .. import _ops
-from .._lib import DTYPE_TAG, check, lib, ptr, require_cuda, stream_ptr
+from .._lib import DTYPE_TAG, check, has_tangent, lib, plain, ptr, require_cuda, stream_ptr
 from ..turbo_diffusion_ops import quant_cuda, gemm_cuda, gemm_cuda_swizzle_bias
 
 
@@ -406,18 +406,67 @@ class _DenseAttentionJvp(torch.autograd.Function):
         return (*_dense_bwd(ctx, d_out), None, None, None, None)
 
 
+class _DenseAttentionAD(torch.autograd.Function):
+    """dense_attention with a forward-AD rule, for q, k, v of which one carries a tangent (torch.func.jvp, forward_ad): the lse
+    forward once; jvp = tdb200_attn_dense_tangent from the saved out and lse (missing tangents are zeros); backward = the dense
+    backward.  lse is an output only so that setup_context can save it.  The tangent carries no gradient."""
+
+    @staticmethod
+    def forward(q, k, v, sm_scale):
+        b, lq, h, d = q.shape
+        out = torch.empty_like(q)
+        lse = torch.empty(b, h, lq, dtype=torch.float32, device=q.device)
+        check(lib().tdb200_attn_dense_fwd_lse(ptr(q), ptr(k), ptr(v), DTYPE_TAG[q.dtype], ptr(out), ptr(lse), b, lq, k.shape[1], h, d,
+                                              sm_scale, stream_ptr(q.device)), "attn_dense_fwd_lse")
+        return out, lse
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        q, k, v, sm_scale = inputs
+        out, lse = output
+        ctx.mark_non_differentiable(lse)
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(q, k, v, out, lse)
+        ctx.save_for_forward(q, k, v, out, lse)
+        ctx.sm_scale = sm_scale
+
+    @staticmethod
+    def jvp(ctx, q_t, k_t, v_t, _):
+        with torch._C._DisableFuncTorch():
+            q, k, v, out, lse = (plain(t) for t in ctx.saved_tensors)
+            q_t, k_t, v_t = (torch.zeros_like(p) if t is None else plain(t).detach().to(p.dtype).contiguous()
+                             for t, p in ((q_t, q), (k_t, k), (v_t, v)))
+            b, lq, h, d = q.shape
+            out_t = torch.empty_like(q)
+            check(lib().tdb200_attn_dense_tangent(ptr(q), ptr(k), ptr(v), ptr(q_t), ptr(k_t), ptr(v_t), ptr(out), ptr(lse),
+                                                  DTYPE_TAG[q.dtype], ptr(out_t), b, lq, k.shape[1], h, d, ctx.sm_scale,
+                                                  stream_ptr(q.device)), "attn_dense_tangent")
+        return out_t, None
+
+    @staticmethod
+    def backward(ctx, d_out, d_lse):
+        if d_out is None:
+            return None, None, None, None
+        return (*_dense_bwd(ctx, d_out), None)
+
+
 def dense_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, sm_scale: Optional[float] = None) -> torch.Tensor:
     """softmax(q.k^T * sm_scale).v per (batch, head), the reference's dense attention (rcm/utils/attention.py:120-167):
     q [B, Lq, H, D], k and v [B, Lk, H, D], D = 128, any Lq and Lk; returns [B, Lq, H, D] in q's dtype.  bf16 / fp16 inputs run
     in their own type, any other float type in bf16.  sm_scale defaults to D ** -0.5.  One kernel on the current stream
     (tdb200_attn_dense_fwd), the arithmetic of the 16-bit SLA kernel.  With grad enabled and any of q, k, v requiring grad the
     output is differentiable: the forward also stores the row lse (tdb200_attn_dense_fwd_lse, the same output bits) and the
-    backward is tdb200_attn_dense_bwd.  Not a `tdb200::` operator: eager use."""
+    backward is tdb200_attn_dense_bwd.  Forward-mode AD (torch.func.jvp, torch.autograd.forward_ad): when any of q, k, v
+    carries a tangent, the output carries out_t = dense_attention_jvp's tangent, computed by tdb200_attn_dense_tangent from the
+    lse forward's out and lse, so the primal runs once and has these bits; out_t carries no gradient.  Not a `tdb200::`
+    operator: eager use."""
     require_cuda(q, k, v)
     dtype = _dense_args("dense_attention", q, k, v)
     qc, kc, vc = (t.to(dtype).contiguous() for t in (q, k, v))
     b, lq, h, d = qc.shape
     sm_scale = float(d ** -0.5 if sm_scale is None else sm_scale)
+    if has_tangent(q, k, v):
+        return _DenseAttentionAD.apply(qc, kc, vc, sm_scale)[0].to(q.dtype)
     if _needs_grad(q, k, v):
         return _DenseAttention.apply(qc, kc, vc, sm_scale).to(q.dtype)
     out = torch.empty_like(qc)

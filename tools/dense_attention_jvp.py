@@ -1,7 +1,7 @@
-"""Time the dense attention JVP operator (ops.dense_attention_jvp, the dense_attn_jvp_kernel) on one GPU, bf16, against the
-dense forward and the cheapest torch JVP that runs, at the shapes the models run attention at.
+"""Time the dense attention JVP operator (ops.dense_attention_jvp, the dense_attn_jvp_kernel) on one GPU, bf16 (or fp16 with
+--dtype fp16), against the dense forward and the cheapest torch JVP that runs, at the shapes the models run attention at.
 
-    python tools/dense_attention_jvp.py [--iters 60] [--warmup 10] [--only NAME] [--out-dir DIR]
+    python tools/dense_attention_jvp.py [--iters 60] [--warmup 10] [--only NAME] [--dtype bf16|fp16] [--out-dir DIR]
 
 Shapes (queries x keys, heads x head dim):
   A-cross   32760 x 512,   12 x 128   Wan2.1-1.3B at 480p, cross-attention over the text tokens
@@ -46,12 +46,13 @@ def _attn(q, k, v, sm_scale):
     return (torch.softmax(s, -1) @ v.transpose(1, 2)).transpose(1, 2)
 
 
-def run_shape(name, iters, warmup, out_dir):
+def run_shape(name, iters, warmup, out_dir, dtype="bf16"):
     from turbodiffusion_b200 import ops
     lq, lk, h = SHAPES[name]
     g = torch.Generator(device="cuda").manual_seed(0)
-    q, q_t = (torch.randn(1, lq, h, D, device="cuda", generator=g).bfloat16() for _ in range(2))
-    k, v, k_t, v_t = (torch.randn(1, lk, h, D, device="cuda", generator=g).bfloat16() for _ in range(4))
+    dt = {"bf16": torch.bfloat16, "fp16": torch.float16}[dtype]
+    q, q_t = (torch.randn(1, lq, h, D, device="cuda", generator=g).to(dt) for _ in range(2))
+    k, v, k_t, v_t = (torch.randn(1, lk, h, D, device="cuda", generator=g).to(dt) for _ in range(4))
     sm_scale = D ** -0.5
     legs = {"dense_attention_jvp": lambda: ops.dense_attention_jvp(q, k, v, q_t, k_t, v_t, sm_scale),
             "dense_attention": lambda: ops.dense_attention(q, k, v, sm_scale),
@@ -60,7 +61,7 @@ def run_shape(name, iters, warmup, out_dir):
     torch.cuda.empty_cache()
     score_bytes = 4 * h * lq * lk * 2
     free = torch.cuda.mem_get_info()[0]
-    row = {"shape": name, "Lq": lq, "Lk": lk, "heads": h, "head_dim": D, "dtype": "bf16"}
+    row = {"shape": name, "Lq": lq, "Lk": lk, "heads": h, "head_dim": D, "dtype": dtype}
     if score_bytes < 0.8 * free:
         legs["torch_func_jvp"] = lambda: torch.func.jvp(lambda a, b, c: _attn(a, b, c, sm_scale), (q, k, v), (q_t, k_t, v_t))
     else:
@@ -94,6 +95,7 @@ def main():
     ap.add_argument("--iters", type=int, default=60)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--only", choices=tuple(SHAPES), default=None)
+    ap.add_argument("--dtype", choices=("bf16", "fp16"), default="bf16")
     ap.add_argument("--out-dir", default=None, help="where the profiler traces go (default: a new temporary directory)")
     args = ap.parse_args()
     if args.iters < 50:
@@ -104,7 +106,7 @@ def main():
     os.makedirs(out_dir, exist_ok=True)
     print(json.dumps({**device_info(), "torch": torch.__version__, "traces": out_dir}), flush=True)
     for name in ((args.only,) if args.only else SHAPES):
-        print(json.dumps(run_shape(name, args.iters, args.warmup, out_dir)), flush=True)
+        print(json.dumps(run_shape(name, args.iters, args.warmup, out_dir, args.dtype)), flush=True)
 
 
 if __name__ == "__main__":

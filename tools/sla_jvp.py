@@ -1,7 +1,7 @@
-"""Time the sparse attention JVP (tdb200_sla_attn16_jvp, SparseLinearAttention.forward_jvp) on one GPU, bf16, against the
-sparse forward and the dense JVP on the same inputs, at the shapes the models run sparse attention at.
+"""Time the sparse attention JVP (tdb200_sla_attn16_jvp, SparseLinearAttention.forward_jvp) on one GPU, bf16 (or fp16 with
+--dtype fp16), against the sparse forward and the dense JVP on the same inputs, at the shapes the models run sparse attention at.
 
-    python tools/sla_jvp.py [--iters 50] [--warmup 5] [--only NAME]
+    python tools/sla_jvp.py [--iters 50] [--warmup 5] [--only NAME] [--dtype bf16|fp16]
 
 Shapes (tokens, heads x head dim, top-k ratio of the 64-key blocks):
   A   32760, 12 x 128, 0.1 and 0.15   Wan2.1-1.3B at 480p (51 and 76 of 512 key blocks)
@@ -43,7 +43,7 @@ def _lut(h, l, topk, seed):
     return ids.view(1, h, mblk, topk).int().contiguous()
 
 
-def run_row(name, ratio, with_dense, iters, warmup):
+def run_row(name, ratio, with_dense, iters, warmup, dtype="bf16"):
     from turbodiffusion_b200 import ops
     from turbodiffusion_b200.SLA import SparseLinearAttention
     from turbodiffusion_b200.SLA.core import attn_fwd_qk16_lse, attn_jvp_qk16
@@ -51,10 +51,11 @@ def run_row(name, ratio, with_dense, iters, warmup):
     mblk, nblk = (l + BLKQ - 1) // BLKQ, (l + BLKK - 1) // BLKK
     topk = int(ratio * nblk)
     g = torch.Generator(device="cuda").manual_seed(0)
-    q, k, v, q_t, k_t, v_t = (torch.randn(1, l, h, D, device="cuda", generator=g).bfloat16() for _ in range(6))
+    dt = {"bf16": torch.bfloat16, "fp16": torch.float16}[dtype]
+    q, k, v, q_t, k_t, v_t = (torch.randn(1, l, h, D, device="cuda", generator=g).to(dt) for _ in range(6))
     lut = _lut(h, l, topk, seed=1)
     sm = D ** -0.5
-    mod = SparseLinearAttention(D, ratio, BLKQ=BLKQ, BLKK=BLKK).cuda()
+    mod = SparseLinearAttention(D, ratio, BLKQ=BLKQ, BLKK=BLKK, use_bf16=dtype == "bf16").cuda()
     with torch.no_grad():
         mod.proj_l.weight.normal_(0, 0.05)
         mod.proj_l.bias.normal_(0, 0.05)
@@ -82,7 +83,7 @@ def run_row(name, ratio, with_dense, iters, warmup):
         legs["dense_jvp"] = lambda: ops.dense_attention_jvp(q, k, v, q_t, k_t, v_t, sm)
     sparse_flop = h * mblk * topk * BLKQ * BLKK * D
     flop = {"sla_jvp": 12 * sparse_flop, "sla_fwd_lse": 4 * sparse_flop, "dense_jvp": 12 * h * l * l * D}
-    row = {"shape": name, "L": l, "heads": h, "head_dim": D, "dtype": "bf16", "topk_ratio": ratio, "topk": topk, "nblk": nblk,
+    row = {"shape": name, "L": l, "heads": h, "head_dim": D, "dtype": dtype, "topk_ratio": ratio, "topk": topk, "nblk": nblk,
            "topk_over_nblk": round(topk / nblk, 4)}
     for _ in range(warmup):
         for fn in legs.values():
@@ -108,6 +109,7 @@ def main():
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--only", choices=tuple(SHAPES), default=None)
+    ap.add_argument("--dtype", choices=("bf16", "fp16"), default="bf16")
     args = ap.parse_args()
     if args.iters < 50:
         ap.error("--iters: at least 50 timed calls per leg")
@@ -116,7 +118,7 @@ def main():
     print(json.dumps({**device_info(), "torch": torch.__version__}), flush=True)
     for name in ((args.only,) if args.only else SHAPES):
         for i, ratio in enumerate(SHAPES[name][2]):
-            print(json.dumps(run_row(name, ratio, i == 0, args.iters, args.warmup)), flush=True)
+            print(json.dumps(run_row(name, ratio, i == 0, args.iters, args.warmup, args.dtype)), flush=True)
             torch.cuda.empty_cache()
 
 

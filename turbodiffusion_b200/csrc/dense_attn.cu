@@ -212,9 +212,12 @@ __device__ __forceinline__ void qk_mmas(float (&d)[BK / 2], uint32_t sq, uint32_
   }
 }
 
-// softmax_step's masking, maxima and lazy rescale, with A and mu rescaled beside O and l; leaves p = exp2(s - m_used) in s
+// softmax_step's masking, maxima and lazy rescale, with A and mu rescaled beside O and l; leaves p = exp2(s - m_used) in s.
+// kRunMax (fp16): also m_run, the row's running maximum, for the overflow rescale of dense_attn_jvp_kernel.
+template <bool kRunMax>
 __device__ __forceinline__ void softmax_step_jvp(float (&s)[BK / 2], float (&o)[HD / 2], float (&a)[HD / 2], float (&m_used)[2],
-                                                 float (&l_part)[2], float (&mu_part)[2], int valid, int cq, bool first) {
+                                                 float (&m_run)[2], float (&l_part)[2], float (&mu_part)[2], int valid, int cq,
+                                                 bool first) {
   if (valid < BK) {
 #pragma unroll
     for (int i = 0; i < BK / 2; ++i)
@@ -241,6 +244,7 @@ __device__ __forceinline__ void softmax_step_jvp(float (&s)[BK / 2], float (&o)[
       mu_part[h] *= alpha;
       m_used[h] = mx;
     }
+    if constexpr (kRunMax) m_run[h] = first ? mx : fmaxf(m_run[h], mx);
   }
 #pragma unroll
   for (int i = 0; i < BK / 2; i += 2) {
@@ -336,7 +340,7 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   float o[HD / 2], a[HD / 2];
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) o[i] = a[i] = 0.f;
-  float m_used[2] = {-INFINITY, -INFINITY}, l_part[2] = {0.f, 0.f}, mu_part[2] = {0.f, 0.f};
+  float m_used[2] = {-INFINITY, -INFINITY}, m_run[2], l_part[2] = {0.f, 0.f}, mu_part[2] = {0.f, 0.f};
 
   mbar_wait(&bars[kQFull], 0);
   for (int j = 0; j < n_tiles; ++j) {
@@ -347,7 +351,8 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     float s[BK / 2], sd[BK / 2];
     mbar_wait(&bars[kKFull + st], ph);
     score_tile<true, HD, BK, kBF16>(s, sq, BQ * 128, sk, sc);
-    softmax_step_jvp(s, o, a, m_used, l_part, mu_part, p.lk - (kSparse ? s_lut[j] : j) * BK, cq, j == 0);   // s := p
+    softmax_step_jvp<!kBF16>(s, o, a, m_used, m_run, l_part, mu_part, p.lk - (kSparse ? s_lut[j] : j) * BK, cq,
+                             j == 0);   // s := p
 #pragma unroll
     for (int i = 0; i < BK / 2; ++i) sd[i] = 0.f;
     wgmma_fence();
@@ -358,11 +363,45 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     reg_fence(sd);
     warp_release(&bars[kKEmpty + st], lane);
 
+    // fp16: p reaches 2^kRescaleThreshold between lazy rescales, so p * Sd rounded to fp16 overflows from |Sd| ~ 256 on, where
+    // the normalised P * Sd is still far inside fp16's range.  In a row where some |p * Sd| of the tile would round to inf, the
+    // kernel rescales O, A, l and mu onto the running maximum first (a rescale the lazy rule skipped): then p <= 1 and
+    // |p * Sd| <= |Sd|, P * Sd's range.  Other rows, and every row of an input whose tangent did not overflow, keep their bits.
+    if constexpr (!kBF16) {
+#pragma unroll
+      for (int i = 0; i < BK / 2; ++i) sd[i] = s[i] * (sd[i] * p.sm_scale);   // sd := p * Sd, Sd in natural-log units
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float xm = 0.f;
+#pragma unroll
+        for (int i = 0; i < BK / 2; ++i)
+          if (((i >> 1) & 1) == h) xm = fmaxf(xm, fabsf(sd[i]));
+        if (quad_max(xm) > 65504.0f) {
+          const float alpha = fast_exp2(m_used[h] - m_run[h]);
+#pragma unroll
+          for (int i = 0; i < HD / 2; ++i)
+            if (((i >> 1) & 1) == h) {
+              o[i] *= alpha;
+              a[i] *= alpha;
+            }
+#pragma unroll
+          for (int i = 0; i < BK / 2; ++i)
+            if (((i >> 1) & 1) == h) {
+              s[i] *= alpha;
+              sd[i] *= alpha;
+            }
+          l_part[h] *= alpha;   // this tile's p are already in it
+          mu_part[h] *= alpha;
+          m_used[h] = m_run[h];
+        }
+      }
+    }
     uint32_t pa[BK / 16][4], pda[BK / 16][4];        // P and P * Sd rounded to T: the A operands of the products
 #pragma unroll
     for (int i = 0; i < BK / 2; i += 2) {
       const int h = (i >> 1) & 1;
-      const float x0 = s[i] * (sd[i] * p.sm_scale), x1 = s[i + 1] * (sd[i + 1] * p.sm_scale);   // Sd in natural-log units
+      const float x0 = kBF16 ? s[i] * (sd[i] * p.sm_scale) : sd[i];   // Sd in natural-log units
+      const float x1 = kBF16 ? s[i + 1] * (sd[i + 1] * p.sm_scale) : sd[i + 1];
       mu_part[h] += x0 + x1;
       pa[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(s[i], s[i + 1]);
       pda[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(x0, x1);

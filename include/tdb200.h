@@ -187,6 +187,12 @@ int tdb200_rms_norm_rope_table(const void* x, int dtype, const float* w, const f
  *     kernel; with (64, 128) one CTA per 64-row query block runs two consumer warpgroups on alternate key blocks and merges
  *     their softmax states.  k_seq_major != 0 reads k_i8 in the sequence-major layout [1,lk,h,d] (rows past lk may follow);
  *     it is implemented for d = 128, the softmax map and b = 1, other calls return TDB200_ERR_UNSUPPORTED.
+ *     Range: the linear branch enters as one more MMA whose 16-bit operand is A = phi(q) * l / den (l the unnormalised
+ *     softmax row sum).  In fp16 a row whose max A lies outside [2^-6, 2^15) runs that MMA on A and the accumulator scaled by
+ *     one power of two (and divides it out in the store), so dead relu channels (den = 1e-5), outlier channels and long
+ *     peaked rows neither overflow nor go subnormal; other rows, and every bf16 call, are unchanged.  kvw itself must fit in T:
+ *     proj_w . kv grows with l * E[phi(k)] * mean(v), and in fp16 it overflows first (for example relu at l = 75600 with a
+ *     modest mean in v); the caller's T(proj_w . kv) is what the kernel multiplies.
  * ------------------------------------------------------------------------------------------- */
 int tdb200_sla_quant_qk(const void* q, const void* k, int dtype, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d,
                         float* kmean, int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale, void* q_pool,
@@ -225,7 +231,8 @@ int tdb200_sla_quant_k_seq(const void* k, const float* kmean, int dtype, int64_t
  * 64-row query block runs two consumer warpgroups on alternate key blocks and merges their softmax states (forward) or adds
  * their dQ / dK / dV partials in a fixed order (backward).
  *   tdb200_sla_attn16_fwd      o = T( sparse_softmax_attention(q,k,v; lut) + proj( phi(q) kv / (1e-5 + phi(q).ksum) ) ), with
- *                              kvw, ksum, proj_b and `feature` as for tdb200_sla_attn_fwd (0 softmax, 1 elu+1, 2 relu).
+ *                              kvw, ksum, proj_b and `feature` as for tdb200_sla_attn_fwd (0 softmax, 1 elu+1, 2 relu), and
+ *                              the same fp16 range of the linear-branch operand and limit on kvw.
  *   tdb200_sla_attn16_fwd_lse  o_s = T(the softmax part alone) (no linear branch, no proj_b; lk = l) and lse [b,h,l] fp32 =
  *                              m + log2(l) of the scores in the log2 domain (S * sm_scale * log2e): the training forward.
  *   tdb200_sla_attn16_bwd      dq, dk, dv of o_s w.r.t. q, k, v for the incoming gradient d_o, given the forward's o_s and lse.

@@ -1,7 +1,7 @@
 """Compare the two SageSLA block families on one GPU: BLKQ=128 / BLKK=64 (the Sage2++ family, served as "sm100") and
 BLKQ=64 / BLKK=128 (SpargeAttn's Hopper family, served as "sm90").
 
-    python tools/sla_block_families.py [--shape A|B|both] [--iters 50] [--warmup 10] [--topk 0.1]
+    python tools/sla_block_families.py [--shape A|B|both] [--iters 50] [--warmup 10] [--topk 0.1] [--dtype bf16|fp16]
 
 Both families run in the same process and are timed with CUDA events, call by call, in an order that rotates every
 iteration (so no timing always follows the same predecessor): the whole SageSparseLinearAttention forward, the fused
@@ -24,10 +24,13 @@ line per (shape, N, family).
     python tools/sla_block_families.py --baseline-lib PATH [--shape ...]
 
 compares this tree's libtdb200.so with another build of the same C ABI (for example the parent commit's), loaded side by
-side: at each shape the fused attention of both INT8 families, the 16-bit (128, 64) forward and its lse forward are called
-through the C entry points on the same inputs, the two builds alternating call by call in a rotating order.  Per leg and build:
+side: at each shape the fused attention of both INT8 families, the 16-bit (128, 64) forward and its lse forward, and the
+16-bit (64, 64) forward are called through the C entry points on the same inputs, the two builds alternating call by call in
+a rotating order.  Per leg and build:
 median, 10th and 90th percentile of the call time.  Every output of the two builds (out, and lse for the lse forward) is
 compared byte for byte; the script exits non-zero if any leg differs.
+
+--dtype (bf16 by default) is the type of q, k, v, the output and every 16-bit MMA operand, in all three modes.
 """
 from __future__ import annotations
 
@@ -73,9 +76,9 @@ def _timed(fn):
     return start.elapsed_time(end)
 
 
-def _module(d, ratio, device):
+def _module(d, ratio, device, dtype=torch.bfloat16):
     from turbodiffusion_b200.SLA import SageSparseLinearAttention
-    mod = SageSparseLinearAttention(d, ratio).to(device)
+    mod = SageSparseLinearAttention(d, ratio, use_bf16=dtype == torch.bfloat16).to(device)
     with torch.no_grad():
         mod.proj_l.weight.normal_(0, 0.05)
         mod.proj_l.bias.normal_(0, 0.05)
@@ -88,7 +91,7 @@ def setup(arch, q, k, v, ratio):
     from turbodiffusion_b200.SLA.utils import block_map_from_pools, quant_qk, set_served_arch
     set_served_arch(arch)
     d = q.shape[-1]
-    mod = _module(d, ratio, q.device)
+    mod = _module(d, ratio, q.device, q.dtype)
     blkq, blkk = mod.block_sizes(q.device.index)
     prep = quant_qk(q, k, blkq=blkq, blkk=blkk)
     topk = max(1, min(prep.nblk, int(ratio * prep.nblk)))
@@ -111,12 +114,22 @@ def setup(arch, q, k, v, ratio):
     return {"blkq": blkq, "blkk": blkk, "mblk": prep.mblk, "topk": topk, "attn": attn, "forward": forward, "prep": prep_only}
 
 
-def run_shape(name, ratio, iters, warmup):
-    from turbodiffusion_b200.SLA.utils import set_served_arch
+DTYPES = {"bf16": torch.bfloat16, "fp16": torch.float16}
+
+
+def inputs(name, dtype):
+    """Seeded q, k, v [1, L, H, D] of shape `name` in `dtype`, keys with a shared offset per head."""
     l, h, d = SHAPES[name]
     g = torch.Generator(device="cuda").manual_seed(0)
-    q, k, v = (torch.randn(1, l, h, d, generator=g, device="cuda").bfloat16() for _ in range(3))
-    k += torch.randn(1, 1, h, d, generator=g, device="cuda").bfloat16() * 2
+    q, k, v = (torch.randn(1, l, h, d, generator=g, device="cuda").to(dtype) for _ in range(3))
+    k += torch.randn(1, 1, h, d, generator=g, device="cuda").to(dtype) * 2
+    return q, k, v
+
+
+def run_shape(name, ratio, iters, warmup, dtype):
+    from turbodiffusion_b200.SLA.utils import set_served_arch
+    l, h, d = SHAPES[name]
+    q, k, v = inputs(name, dtype)
     prev = set_served_arch("sm100")
     try:
         fams = {arch: setup(arch, q, k, v, ratio) for arch in FAMILIES}
@@ -141,7 +154,7 @@ def run_shape(name, ratio, iters, warmup):
         f = fams[arch]
         attn_ms = statistics.median(times[arch]["attn"])
         flops = h * f["mblk"] * f["topk"] * 4 * f["blkq"] * f["blkk"] * d
-        rows.append({"shape": name, "L": l, "heads": h, "head_dim": d, "family": arch, "blkq": f["blkq"], "blkk": f["blkk"],
+        rows.append({"shape": name, "L": l, "heads": h, "head_dim": d, "dtype": str(q.dtype)[6:], "family": arch, "blkq": f["blkq"], "blkk": f["blkk"],
                      "topk": f["topk"], "keys_per_query": round(f["topk"] * f["blkk"] / l, 4),
                      "attn_ms_median": round(attn_ms, 4), "attn_tflops": round(flops / attn_ms / 1e9, 1),
                      "forward_ms_median": round(statistics.median(times[arch]["forward"]), 4),
@@ -169,6 +182,7 @@ def _build_legs(fns, q, k, v, ratio):
     """Per leg, a call of one build's entry point and the output buffers it writes (fresh for this build)."""
     from turbodiffusion_b200._lib import DTYPE_TAG, ptr
     from turbodiffusion_b200.SLA.core import linear_moments, project_moments
+    from turbodiffusion_b200.SLA.core import select_prep
     from turbodiffusion_b200.SLA.utils import block_map_from_pools, quant_qk
     b, l, h, d = q.shape
     g = torch.Generator(device="cuda").manual_seed(1)
@@ -209,6 +223,15 @@ def _build_legs(fns, q, k, v, ratio):
             common = {"mblk": prep.mblk, "topk": topk, "blkq": 128, "blkk": 64}
             legs["attn16"] = {"call": call16, "outputs": [out16], **common}
             legs["attn16_lse"] = {"call": call16_lse, "outputs": [o_s, lse], **common}
+    prep = select_prep(q, k, 64, 64)      # the 16-bit (64, 64) forward on its own selection
+    topk = max(1, min(prep.nblk, int(ratio * prep.nblk)))
+    _, lut = block_map_from_pools(prep.q_pool, prep.k_pool, topk)
+    out64 = torch.empty_like(q)
+
+    def call16_q64(lut=lut, topk=topk):
+        check(fns["tdb200_sla_attn16_fwd"](ptr(q), ptr(k), ptr(v), tag, ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(pb), ptr(out64),
+                                           b, l, l, h, d, sm_scale, 0, 64, 64, stream), "tdb200_sla_attn16_fwd")
+    legs["attn16_q64"] = {"call": call16_q64, "outputs": [out64], "mblk": prep.mblk, "topk": topk, "blkq": 64, "blkk": 64}
     return legs
 
 
@@ -217,13 +240,11 @@ def _pct(xs, f):
     return xs[min(len(xs) - 1, int(round(f * (len(xs) - 1))))]
 
 
-def run_builds(name, ratio, iters, warmup, baseline_lib):
+def run_builds(name, ratio, iters, warmup, baseline_lib, dtype):
     """This tree's build against `baseline_lib`, leg by leg, alternated call by call; returns (rows, all outputs identical)."""
     from turbodiffusion_b200 import _lib
     l, h, d = SHAPES[name]
-    g = torch.Generator(device="cuda").manual_seed(0)
-    q, k, v = (torch.randn(1, l, h, d, generator=g, device="cuda").bfloat16() for _ in range(3))
-    k += torch.randn(1, 1, h, d, generator=g, device="cuda").bfloat16() * 2
+    q, k, v = inputs(name, dtype)
     builds = {"this": _load_build(_lib.LIB_PATH), "baseline": _load_build(baseline_lib)}
     legs = {bn: _build_legs(fns, q, k, v, ratio) for bn, fns in builds.items()}
     names = list(legs["this"])
@@ -246,7 +267,7 @@ def run_builds(name, ratio, iters, warmup, baseline_lib):
                    for a, b_ in zip(legs["this"][leg]["outputs"], legs["baseline"][leg]["outputs"]))
         same_all &= same
         flops = h * f["mblk"] * f["topk"] * 4 * f["blkq"] * f["blkk"] * d
-        row = {"shape": name, "L": l, "heads": h, "head_dim": d, "leg": leg, "blkq": f["blkq"], "blkk": f["blkk"], "topk": f["topk"],
+        row = {"shape": name, "L": l, "heads": h, "head_dim": d, "dtype": str(dtype)[6:], "leg": leg, "blkq": f["blkq"], "blkk": f["blkk"], "topk": f["topk"],
                "outputs_byte_identical": same, "calls": iters, **clocks}
         for bn in builds:
             ts = times[(leg, bn)]
@@ -267,7 +288,7 @@ def setup_rank0(arch, q, k, v, ratio, world):
     from turbodiffusion_b200.SLA.utils import block_map_from_pools, kmean_from_partials, kmean_partials, quant_k_seq, set_served_arch
     set_served_arch(arch)
     _, l, h, d = q.shape
-    mod = _module(d, ratio, q.device)
+    mod = _module(d, ratio, q.device, q.dtype)
     gp, up = GpuPrimitives(mod, arch), UlyssesGpuPrims(mod, arch)
     blkq, blkk = gp.blkq, gp.blkk
     begin, end, rows_pad = shard_rows(l, world, 0)
@@ -305,13 +326,11 @@ def setup_rank0(arch, q, k, v, ratio, world):
             "allgather": allgather, "allgather_attn": allgather_attn, "ulysses": ulysses}
 
 
-def run_ranks(name, ratio, iters, warmup, ranks):
+def run_ranks(name, ratio, iters, warmup, ranks, dtype):
     """Rank 0's share per family for each world size; collectives are not timed."""
     from turbodiffusion_b200.SLA.utils import set_served_arch
     l, h, d = SHAPES[name]
-    g = torch.Generator(device="cuda").manual_seed(0)
-    q, k, v = (torch.randn(1, l, h, d, generator=g, device="cuda").bfloat16() for _ in range(3))
-    k += torch.randn(1, 1, h, d, generator=g, device="cuda").bfloat16() * 2
+    q, k, v = inputs(name, dtype)
     rows = []
     prev = set_served_arch("sm100")
     try:
@@ -360,6 +379,7 @@ def main():
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--topk", type=float, default=0.1)
+    ap.add_argument("--dtype", default="bf16", choices=sorted(DTYPES))
     ap.add_argument("--baseline-lib", default=None,
                     help="another libtdb200.so with the same C ABI: time it against this tree's build and compare the outputs")
     ap.add_argument("--ranks", default=None,
@@ -380,7 +400,8 @@ def main():
               flush=True)
         identical = True
         for name in (["A", "B"] if args.shape == "both" else [args.shape]):
-            rows, same = run_builds(name, args.topk, args.iters, args.warmup, os.path.abspath(args.baseline_lib))
+            rows, same = run_builds(name, args.topk, args.iters, args.warmup, os.path.abspath(args.baseline_lib),
+                                    DTYPES[args.dtype])
             identical &= same
             for row in rows:
                 print(json.dumps(row), flush=True)
@@ -389,8 +410,8 @@ def main():
         return
     print(json.dumps(device_info()), flush=True)
     for name in (["A", "B"] if args.shape == "both" else [args.shape]):
-        rows = run_shape(name, args.topk, args.iters, args.warmup) if ranks is None else \
-            run_ranks(name, args.topk, args.iters, args.warmup, ranks)
+        rows = run_shape(name, args.topk, args.iters, args.warmup, DTYPES[args.dtype]) if ranks is None else \
+            run_ranks(name, args.topk, args.iters, args.warmup, ranks, DTYPES[args.dtype])
         for row in rows:
             print(json.dumps(row), flush=True)
 

@@ -1,7 +1,7 @@
-"""Time SparseLinearAttention (16-bit Q.K^T, bf16) at its two served block geometries, (BLKQ, BLKK) = (128, 64) and the
+"""Time SparseLinearAttention (16-bit Q.K^T) at its two served block geometries, (BLKQ, BLKK) = (128, 64) and the
 constructor's default (64, 64), on one GPU.
 
-    python tools/sla_q64_16bit.py [--shape A|B|both] [--topk 0.1] [--iters 20] [--warmup 5]
+    python tools/sla_q64_16bit.py [--shape A|B|both] [--topk 0.1] [--iters 20] [--warmup 5] [--dtype bf16|fp16]
 
 Per shape and geometry, in one run, geometries alternated call by call, CUDA events, medians over --iters calls:
   * the module's inference forward (no grad: block selection, linear moments, fused attention) and its block-selection prep
@@ -11,7 +11,8 @@ Per shape and geometry, in one run, geometries alternated call by call, CUDA eve
     of its own (mean device time per launch).
 FLOPs (Mblk = ceil(L / BLKQ), topk = int(r * ceil(L / BLKK))): F = H * Mblk * topk * 4 * BLKQ * BLKK * D for a forward; the dQ
 kernel executes 1.5 F (S, dP, dQ), the dK/dV kernel 2.0 F (S, dP, dV, dK).  One JSON line with the device name and power
-limit, then one per shape; the SM clock and throttle reasons are read before and after each shape's timed window.
+limit, then one per shape; the SM clock and throttle reasons are read before and after each shape's timed window.  --dtype
+(bf16 by default) is the type of q, k, v, the module and its output.
 """
 from __future__ import annotations
 
@@ -27,7 +28,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from sla_backward import _median_ms  # noqa: E402
-from sla_block_families import SHAPES, clock_state, device_info  # noqa: E402
+from sla_block_families import DTYPES, SHAPES, clock_state, device_info  # noqa: E402
 
 GEOMETRIES = ((128, 64), (64, 64))
 
@@ -48,18 +49,18 @@ def _kernel_times(fn, iters):
     return out
 
 
-def run_shape(name, topk_ratio, iters, warmup):
+def run_shape(name, topk_ratio, iters, warmup, dtype):
     from turbodiffusion_b200.SLA import SparseLinearAttention
     from turbodiffusion_b200.SLA.core import block_map_from_pools, select_prep
     l, h, d = SHAPES[name]
     dev = torch.device("cuda:0")
     g = torch.Generator(device=dev).manual_seed(0)
-    q, k, v = (torch.randn(1, l, h, d, device=dev, generator=g, dtype=torch.bfloat16) for _ in range(3))
-    gout = torch.randn(q.shape, device=dev, generator=g, dtype=torch.bfloat16)
+    q, k, v = (torch.randn(1, l, h, d, device=dev, generator=g, dtype=dtype) for _ in range(3))
+    gout = torch.randn(q.shape, device=dev, generator=g, dtype=dtype)
     qg, kg, vg = (t.clone().requires_grad_() for t in (q, k, v))
     legs = {}
     for blkq, blkk in GEOMETRIES:
-        mod = SparseLinearAttention(d, topk_ratio, BLKQ=blkq, BLKK=blkk).to(dev)
+        mod = SparseLinearAttention(d, topk_ratio, BLKQ=blkq, BLKK=blkk, use_bf16=dtype == torch.bfloat16).to(dev)
         _, sel = mod.forward_with_lut(q, k, v)
         topk = sel["topk"]
         state = {}
@@ -84,7 +85,7 @@ def run_shape(name, topk_ratio, iters, warmup):
         for leg in legs.values():
             leg["infer"](), leg["prep"](), leg["train_fwd"](), leg["train_bwd"]()
     torch.cuda.synchronize()
-    row = {"shape": name, "L": l, "heads": h, "head_dim": d, "topk_ratio": topk_ratio, "sm_clock_throttle_before": clock_state()}
+    row = {"shape": name, "L": l, "heads": h, "head_dim": d, "dtype": str(dtype)[6:], "topk_ratio": topk_ratio, "sm_clock_throttle_before": clock_state()}
     for _ in range(iters):
         for leg in legs.values():
             for n in ("infer", "prep", "train_fwd", "train_bwd"):
@@ -124,12 +125,13 @@ def main():
     ap.add_argument("--topk", type=float, default=0.1)
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--dtype", default="bf16", choices=sorted(DTYPES))
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("sla_q64_16bit.py measures on the GPU; no CUDA device found")
     print(json.dumps(device_info()), flush=True)
     for name in (("A", "B") if args.shape == "both" else (args.shape,)):
-        print(json.dumps(run_shape(name, args.topk, args.iters, args.warmup)), flush=True)
+        print(json.dumps(run_shape(name, args.topk, args.iters, args.warmup, DTYPES[args.dtype])), flush=True)
 
 
 if __name__ == "__main__":

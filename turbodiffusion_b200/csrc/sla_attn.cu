@@ -113,6 +113,14 @@ __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const fl
     }
   }
   const float* ks = p.ksum + int64_t(bh) * HD;
+  // fp16: A is rounded to T only as the MMA operand, and its range follows l / den, not the output's: a relu channel dead on
+  // every key (ksum_j = 0, den = 1e-5) puts A_j near 1e5 * l, inf against a KVW column of zeros (inf * 0 = NaN), a large
+  // shared channel lifts max A past 65504, and peaked rows over long sequences make every A subnormal (below 2^-14).  A row
+  // whose max A lies outside [2^-6, 2^15) runs the product on A * 2^sc, O * 2^sc and stores with 1 / l * 2^-sc, sc chosen
+  // to put max A near 2^14.  |sc| <= 64, so the three scalings are exact in fp32: O <= l max|v| < 2^42 times 2^64 stays
+  // finite, 1/l in [2^-27, 1] stays normal, and O elements that 2^-64 would take below fp32's normal range are < 2^-62, far
+  // under fp16's last subnormal after the division by l >= 1.  Other rows keep sc = 0 and their bits.
+  float out_scale[2] = {1.f, 1.f};
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     float off = 0.f;
@@ -125,7 +133,7 @@ __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const fl
           qm = fmaxf(qm, fmaxf(F16Traits<T>::lo(qa[kk][h + 2 * u]), F16Traits<T>::hi(qa[kk][h + 2 * u])));
       off = quad_max(qm) * kLog2e;
     }
-    float e = 0.f, f = 0.f;
+    float e = 0.f, f = 0.f, fm = 0.f;
 #pragma unroll
     for (int kk = 0; kk < HD / 16; ++kk)
 #pragma unroll
@@ -135,11 +143,24 @@ __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const fl
         const float a0 = feat(F16Traits<T>::lo(w), off, p.feature), a1 = feat(F16Traits<T>::hi(w), off, p.feature);
         e += a0 + a1;
         f = fmaf(a0, k2.x, fmaf(a1, k2.y, f));
+        if constexpr (!kBF16) fm = fmaxf(fm, fmaxf(a0, a1));   // every feature map is >= 0
       }
     const float E = quad_sum(e), F = quad_sum(f);
     const float inv_e = p.feature == 0 ? 1.0f / E : 1.0f;
     const float den = 1e-5f + F * inv_e;
-    const float cscale = inv_e * l_tot[h] / den;
+    float cscale = inv_e * l_tot[h] / den;
+    if constexpr (!kBF16) {
+      const float amax = quad_max(fm) * cscale;   // = max_j A_j before rounding (rounding is monotone)
+      if ((amax > 0.f && amax < 0x1p-6f) || amax >= 0x1p15f) {
+        const int sc = min(64, max(-64, 14 - ((__float_as_int(amax) >> 23) - 127)));
+        const float up = __int_as_float((127 + sc) << 23);
+        cscale *= up;
+#pragma unroll
+        for (int i = 0; i < HD / 2; ++i)
+          if (((i >> 1) & 1) == h) o[i] *= up;
+        out_scale[h] = __int_as_float((127 - sc) << 23);
+      }
+    }
 #pragma unroll
     for (int kk = 0; kk < HD / 16; ++kk)
 #pragma unroll
@@ -165,7 +186,7 @@ __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const fl
   for (int h = 0; h < 2; ++h) {
     const int64_t qr = qrow0 + 8 * h;
     if (qr >= p.l) continue;
-    const float inv_l = 1.0f / l_tot[h];
+    const float inv_l = kBF16 ? 1.0f / l_tot[h] : 1.0f / l_tot[h] * out_scale[h];
     T* orow = static_cast<T*>(p.out) + ((int64_t(b) * p.l + qr) * p.h + hh) * HD;
 #pragma unroll
     for (int c = 0; c < HD / 8; ++c) {

@@ -207,6 +207,43 @@ int tdb200_sla_attn_fwd(const int8_t* q_i8, const float* q_scale, const int8_t* 
                         const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
                         int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq, int64_t blkk,
                         int k_seq_major, void* stream);
+/* SparseLinearAttention's linear branch and proj_l for training (reference SLA/core.py:104-117), per (batch, head), phi the
+ * feature map `feature` (0 softmax over d, 1 elu+1, 2 relu), c = T(phi(x)), kv = M^T [b,h,d(v),d(k)] and ksum = s [b,h,d] fp32
+ * from tdb200_sla_linear_moments of the same k, v and feature:
+ *   tdb200_sla_linear_fwd   den_i = 1e-5 + c_q,i . s,  u_i = c_q,i M / den_i,  o_l,i = T(u_i proj_w^T + proj_b)
+ *   tdb200_sla_linear_bwd   for d_o = dL/do_l: dq, dk, dv (T) and dproj_w [d,d], dproj_b [d] (fp32, summed over b, h and l) of
+ *                           the forward above, from q, k, v, kv and ksum (nothing of l's size is saved by the forward)
+ *   tdb200_sla_linear_bwd_workspace_bytes  host-only size of the backward's workspace (or a negative error code): three
+ *                           [b,l,h,d] 16-bit operands, per-64-row partials of ds and dproj_b, split partials of dM and dproj_w,
+ *                           dM and ds, each 256-byte aligned.
+ *   tdb200_sla_linear_tangent  o_l_t = T(udot proj_w^T), the forward's tangent along q_t, k_t, v_t (proj_w, proj_b fixed):
+ *                           Mdot = sum_j (cdot_k,j^T v_j + c_k,j^T v_t,j), sdot = sum_j cdot_k,j with cdot = J_phi . x_t,
+ *                           udot_i = (cdot_q,i M + c_q,i Mdot) / den_i - u_i (cdot_q,i . s + c_q,i . sdot) / den_i.
+ *                           J_phi: softmax c (x_t - c . x_t); elu+1 1 where x > 0, else e^x; relu 1[x > 0].  Five launches.
+ *   tdb200_sla_linear_tangent_workspace_bytes  its workspace: c_k and cdot_k [b,l,h,d] 16-bit, per-64-row partials of sdot,
+ *                           split partials of Mdot, Mdot and sdot, each 256-byte aligned.
+ * q, k, v, d_o, o_l, dq, dk, dv [b,l,h,d] contiguous 16-bit of type `dtype`; proj_w [d(out),d(in)] and proj_b [d] fp32.
+ * Rounding points: c_q and c_k to T; cdot (fp32) to T as MMA operands, sdot from the fp32 cdot; M, Mdot and dM (fp32) to
+ * T as MMA operands after a power-of-two scale per (b, h) that puts their largest magnitude in [2^14, 2^15); udot,
+ * proj_w, u, g and du to T as MMA operands; dM's row operands c_q,i 2^e and du_i/den_i 2^-e
+ * to T with e splitting the two rows' exponents; everything else, den, e_i, s and ds included, fp32.  Products are 16-bit
+ * tensor-core MMAs with fp32 accumulation.  Every reduction over rows, heads and batch entries is summed in a fixed order
+ * without atomics: the results are bit-reproducible, and a (batch, head)'s o_l, dq, dk and dv depend only on its own inputs.
+ * The forward is one launch, the backward eight, the tangent five; neither synchronises the host, so both can be captured in a CUDA graph.
+ * Errors, all before any CUDA call: null or misaligned (16 B) pointer, non-positive b, l, h or d -> TDB200_ERR_INVALID_ARG;
+ * d != 128, bad dtype or feature tag, b*h above 65535, l*h*d of 2^39 elements or more -> TDB200_ERR_UNSUPPORTED;
+ * workspace_bytes below the size query -> TDB200_ERR_WORKSPACE. */
+int tdb200_sla_linear_fwd(const void* q, const float* kv, const float* ksum, const float* proj_w, const float* proj_b, int dtype,
+                          int feature, void* o_l, int64_t b, int64_t l, int64_t h, int64_t d, void* stream);
+int tdb200_sla_linear_bwd(const void* q, const void* k, const void* v, const void* d_o, const float* kv, const float* ksum,
+                          const float* proj_w, int dtype, int feature, void* dq, void* dk, void* dv, float* dproj_w,
+                          float* dproj_b, void* workspace, int64_t workspace_bytes, int64_t b, int64_t l, int64_t h, int64_t d,
+                          void* stream);
+int64_t tdb200_sla_linear_bwd_workspace_bytes(int64_t b, int64_t h, int64_t l, int64_t d);
+int tdb200_sla_linear_tangent(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                              const float* kv, const float* ksum, const float* proj_w, int dtype, int feature, void* o_l_t,
+                              void* workspace, int64_t workspace_bytes, int64_t b, int64_t l, int64_t h, int64_t d, void* stream);
+int64_t tdb200_sla_linear_tangent_workspace_bytes(int64_t b, int64_t h, int64_t l, int64_t d);
 /* Sequence-parallel form of the key half of tdb200_sla_quant_qk (reference: the context-parallel attention of
  * rcm/utils/a2a_cp.py:66-182 exchanges 16-bit K; here each rank quantises its own key rows and the INT8 tensor travels).
  *   tdb200_sla_kmean_partial  partial [b,h,ceil(l/128),d] fp32 = column sums of each 128-row chunk of k [b,l,h,d];

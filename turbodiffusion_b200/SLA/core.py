@@ -16,6 +16,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import _ops
+from . import utils as _utils
 from .._lib import DTYPE_TAG, check, has_tangent, lib, plain, ptr, require_cuda, stream_ptr
 from .utils import (SAGE_BLOCKS, QKPrep, block_map_from_pools, get_block_map, get_cuda_arch, quant_k_into,  # noqa: F401
                     quant_q_only, quant_qk)
@@ -202,6 +203,84 @@ class _SparseAttention16AD(torch.autograd.Function):
         return dq, dk, dv, None, None, None
 
 
+def _linear_args(q, k, v, proj_w, proj_b, feature, what):
+    feature = FEATURE_TAG[feature] if isinstance(feature, str) else int(feature)
+    if q.shape[-1] != 128:
+        raise NotImplementedError(f"{what}: head dim {q.shape[-1]}; the linear-branch kernels serve d = 128")
+    if not (q.dtype == k.dtype == v.dtype and q.dtype in (torch.bfloat16, torch.float16)):
+        raise ValueError(f"{what}: q, k, v must share one 16-bit dtype, got {q.dtype}, {k.dtype}, {v.dtype}")
+    if not (q.shape == k.shape == v.shape):
+        raise ValueError(f"{what}: q, k, v shapes differ: {tuple(q.shape)}, {tuple(k.shape)}, {tuple(v.shape)}")
+    if has_tangent(proj_w, proj_b):
+        raise NotImplementedError(f"{what}: proj_w / proj_b carry a forward-mode tangent; the tangent kernels hold them "
+                                  "fixed (SparseLinearAttention takes its torch branch for such calls)")
+    require_cuda(q, k, v, proj_w, proj_b)
+    return feature, proj_w.float().contiguous(), proj_b.float().contiguous()
+
+
+def _linear_tangent(q, k, v, q_t, k_t, v_t, mom, w, feature):
+    q_t, k_t, v_t = (torch.zeros_like(p) if t is None else t.detach().to(p.dtype).contiguous()
+                     for t, p in ((q_t, q), (k_t, k), (v_t, v)))
+    return _ops.sla_linear_tangent(q, k, v, q_t, k_t, v_t, mom, w, feature)
+
+
+class _LinearBranchAD(torch.autograd.Function):
+    """linear_branch for q, k, v of which one carries a forward-mode tangent: the forward operator once (its bits), jvp =
+    tdb200_sla_linear_tangent from the saved moments (missing tangents are zeros), backward = tdb200_sla_linear_bwd."""
+
+    @staticmethod
+    def forward(q, k, v, w, b, feature):
+        return _ops.sla_linear_fwd(q, k, v, w, b, feature)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        q, k, v, w, b, feature = inputs
+        ctx.mark_non_differentiable(output[1])
+        ctx.save_for_backward(q, k, v, w, output[1])
+        ctx.save_for_forward(q, k, v, w, output[1])
+        ctx.feature = feature
+
+    @staticmethod
+    def jvp(ctx, q_t, k_t, v_t, *_):
+        with torch._C._DisableFuncTorch():
+            q, k, v, w, mom = (plain(t) for t in ctx.saved_tensors)
+            o_t = _linear_tangent(q, k, v, plain(q_t), plain(k_t), plain(v_t), mom, w, ctx.feature)
+        return o_t, None
+
+    @staticmethod
+    def backward(ctx, d_o, d_mom):
+        q, k, v, w, mom = ctx.saved_tensors
+        dq, dk, dv, dw, db = _ops.sla_linear_bwd(q, k, v, d_o.to(q.dtype).contiguous(), mom, w, ctx.feature)
+        return dq, dk, dv, dw, db, None
+
+
+def linear_branch(q, k, v, proj_w, proj_b, feature="softmax"):
+    """SparseLinearAttention's linear branch and proj_l as CUDA kernels: o_l [B, L, H, D] in q.dtype,
+    o_l,i = T(u_i proj_w^T + proj_b) with u_i = phi(q_i) M / (1e-5 + phi(q_i).s), M = sum_j phi(k_j)^T v_j, s = sum_j phi(k_j).
+    q, k, v [B, L, H, 128] of one 16-bit dtype; proj_w [128, 128], proj_b [128] (fp32: proj_l's parameters); `feature` is
+    "softmax", "elu" or "relu" (or its tag 0, 1, 2).  Differentiable in all five inputs (tdb200_sla_linear_bwd; the gradients
+    of proj_w and proj_b are fp32 sums over batch, heads and rows, in a fixed order).  When q, k or v carries a forward-mode
+    tangent (torch.func.jvp, forward_ad) the output carries its tangent from tdb200_sla_linear_tangent; proj_w and proj_b
+    must carry none (NotImplementedError).  Rounding points: include/tdb200.h."""
+    feature, w, b = _linear_args(q, k, v, proj_w, proj_b, feature, "linear_branch")
+    if has_tangent(q, k, v):
+        return _LinearBranchAD.apply(q.contiguous(), k.contiguous(), v.contiguous(), w, b, feature)[0]
+    q, k, v = (t.contiguous() for t in (q, k, v))
+    return _ops.sla_linear_fwd(q, k, v, w, b, feature)[0]
+
+
+def linear_branch_jvp(q, k, v, q_t, k_t, v_t, proj_w, proj_b, feature="softmax"):
+    """(o_l, o_l_t): linear_branch and its forward-mode derivative along (q_t, k_t, v_t), proj_w and proj_b held fixed.
+    o_l is differentiable as linear_branch's is (the same forward kernel, so the same bits with and without grad); o_l_t
+    carries no gradient and the tangents get none."""
+    feature, w, b = _linear_args(q, k, v, proj_w, proj_b, feature, "linear_branch_jvp")
+    q, k, v = (t.contiguous() for t in (q, k, v))
+    o_l, mom = _ops.sla_linear_fwd(q, k, v, w, b, feature)
+    with torch.no_grad():
+        o_t = _linear_tangent(q, k, v, q_t, k_t, v_t, mom.detach(), w.detach(), feature)
+    return o_l, o_t
+
+
 def select_prep(q, k, blkq, blkk):
     """The pooled means (and Sage INT8 codes) block selection reads, for q, k [B, L, H, D]: quant_qk for the SageSLA families;
     (64, 64), a pair tdb200_sla_quant_qk does not take, from its query half at blkq = 64 and its key half at blkk = 64."""
@@ -278,7 +357,8 @@ class _SLABase(nn.Module):
     def _forward_train(self, q, k, v, return_sparsity):
         """The reference's SparseLinearAttention.forward (SLA/core.py:81-119) with autograd: the same block selection as the
         fused path, the sparse branch through sparse_attention16, the linear branch and proj_l in torch at the reference's
-        rounding points (feature maps -> dtype, bmm in dtype, proj_l evaluated in dtype as under its autocast)."""
+        rounding points (feature maps -> dtype, bmm in dtype, proj_l evaluated in dtype as under its autocast), or, with
+        SLA.utils.set_linear_branch("fused"), through linear_branch's CUDA kernels."""
         if q.shape[-1] != 128:
             raise NotImplementedError(f"SparseLinearAttention backward: head dim {q.shape[-1]}; gradients are served for d = 128")
         require_cuda(q, k, v)
@@ -294,7 +374,8 @@ class _SLABase(nn.Module):
         if getattr(self, "_keep_selection", None) is not None:
             self._keep_selection.update(lut=lut, sparse_map=sparse_map, topk=real_topk)
         o_s = sparse_attention16(q, k, v, lut, real_topk, d ** -0.5, blkq)
-        o = (o_s + self._linear_branch(q, k, v)).to(dtype).contiguous()
+        o_l = linear_branch(q, k, v, *self._proj, self.feature) if self._fused_linear() else self._linear_branch(q, k, v)
+        o = (o_s + o_l).to(dtype).contiguous()
         return (o, real_topk / nblk) if return_sparsity else o
 
     def _forward_ad(self, q, k, v, return_sparsity):
@@ -311,7 +392,8 @@ class _SLABase(nn.Module):
         nblk = (l + _ops.BLKK16 - 1) // _ops.BLKK16
         real_topk = max(1, min(nblk, int(self.topk * nblk)))
         o_s = _SparseAttention16AD.apply(q, k, v, real_topk, d ** -0.5, self)[0]
-        o = (o_s + self._linear_branch(q, k, v)).to(dtype).contiguous()
+        o_l = linear_branch(q, k, v, *self._proj, self.feature) if self._fused_linear() else self._linear_branch(q, k, v)
+        o = (o_s + o_l).to(dtype).contiguous()
         return (o, real_topk / nblk) if return_sparsity else o
 
     def _refuse_unserved_jvp(self, what, d):
@@ -324,6 +406,15 @@ class _SLABase(nn.Module):
         if (self.BLKQ, self.BLKK) != (128, 64):
             raise NotImplementedError(f"{what}: block sizes (BLKQ, BLKK) = ({self.BLKQ}, {self.BLKK}); the sparse attention "
                                       "JVP is served for (128, 64)")
+
+    @property
+    def _proj(self):
+        return self.proj_l.weight, self.proj_l.bias
+
+    def _fused_linear(self):
+        """The linear branch of this call runs on the CUDA kernels: "fused" is selected (SLA.utils.set_linear_branch) and
+        proj_l's parameters carry no forward-mode tangent (those calls take the torch branch, whose forward AD covers them)."""
+        return _utils.LINEAR_BRANCH == "fused" and not has_tangent(*self._proj)
 
     def _linear_branch(self, q, k, v):
         """proj_l(phi(q) (phi(k)^T v) / (1e-5 + phi(q).sum phi(k))) as [B, L, H, D] in self.dtype, in torch at the reference's
@@ -366,6 +457,11 @@ class _SLABase(nn.Module):
         if getattr(self, "_keep_selection", None) is not None:
             self._keep_selection.update(lut=lut, sparse_map=sparse_map, topk=real_topk)
         o_s, o_s_t = sparse_attention16_jvp(q, k, v, q_t, k_t, v_t, lut, real_topk, d ** -0.5, blkq)
+        if self._fused_linear():
+            o_l, o_l_t = linear_branch_jvp(q, k, v, q_t, k_t, v_t, *self._proj, self.feature)
+            o = (o_s + o_l).to(dtype).contiguous()
+            o_t = (o_s_t + o_l_t).to(dtype).contiguous()
+            return (o, o_t, real_topk / nblk) if return_sparsity else (o, o_t)
         with fwAD.dual_level():
             o_l = self._linear_branch(fwAD.make_dual(q, q_t), fwAD.make_dual(k, k_t), fwAD.make_dual(v, v_t))
             o_l, o_l_t = fwAD.unpack_dual(o_l)

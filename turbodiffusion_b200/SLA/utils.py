@@ -29,6 +29,23 @@ def set_served_arch(arch: str) -> str:
     return prev
 
 
+# SparseLinearAttention's linear branch in training (see set_linear_branch).
+LINEAR_BRANCH = "reference"
+LINEAR_BRANCHES = ("reference", "fused")
+
+
+def set_linear_branch(name: str) -> str:
+    """Select how SparseLinearAttention's training forward computes the linear branch and proj_l: "reference" (the default,
+    torch ops at the reference's rounding points, SLA/core.py:104-117) or "fused" (SLA.core.linear_branch: the CUDA forward
+    and backward of tdb200_sla_linear_fwd / _bwd).  Read at every call; returns the previous value.  Calls that carry a
+    forward-mode tangent (forward_jvp, torch.func.jvp, forward_ad) take the reference branch under either setting."""
+    global LINEAR_BRANCH
+    if name not in LINEAR_BRANCHES:
+        raise ValueError(f"linear branch must be one of {list(LINEAR_BRANCHES)}, got {name!r}")
+    prev, LINEAR_BRANCH = LINEAR_BRANCH, name
+    return prev
+
+
 def get_cuda_arch(device_index):
     """SLA/utils.py:70-71.  The reference (SLA/core.py:191-193, 211-235) and the LTX client (acceleration.py:286-378) use this
     value only to choose a SpargeAttn kernel family and its block sizes: sm80/86/87 -> fp16-V kernels, sm90 -> the

@@ -48,6 +48,11 @@ _PROTOS = {
     "tdb200_sla_attn_fwd": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F,
                             _I, _I64, _I64, _I, _P],
     "tdb200_sla_project_moments": [_P, _P, _I, _I64, _I64, _P, _P],
+    "tdb200_sla_linear_fwd": [_P, _P, _P, _P, _P, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
+    "tdb200_sla_linear_bwd": [_P, _P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _P],
+    "tdb200_sla_linear_bwd_workspace_bytes": [_I64, _I64, _I64, _I64],
+    "tdb200_sla_linear_tangent": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _I64, _I64, _I64, _I64, _I64, _P],
+    "tdb200_sla_linear_tangent_workspace_bytes": [_I64, _I64, _I64, _I64],
     "tdb200_sla_kmean_partial": [_P, _I, _I64, _I64, _I64, _I64, _P, _P],
     "tdb200_sla_kmean_final": [_P, _I64, _I64, _I64, _I64, _I64, _P, _P],
     "tdb200_sla_quant_k_seq": [_P, _P, _I, _I64, _I64, _I64, _I64, _P, _P, _P, _I64, _P],
@@ -78,7 +83,8 @@ _PROTOS = {
     "tdb200_gemm_w8a8_rowwise": [_P, _P, _P, _P, _P, _P, _I, _I64, _I64, _I64, _P],
 }
 _RESTYPES = {"tdb200_last_error": c_char_p, "tdb200_sla_attn_bwd_workspace_bytes": c_int64,
-             "tdb200_sla_attn16_bwd_workspace_bytes": c_int64, "tdb200_attn_dense_bwd_workspace_bytes": c_int64}
+             "tdb200_sla_attn16_bwd_workspace_bytes": c_int64, "tdb200_attn_dense_bwd_workspace_bytes": c_int64,
+             "tdb200_sla_linear_bwd_workspace_bytes": c_int64, "tdb200_sla_linear_tangent_workspace_bytes": c_int64}
 ABI_VERSION = 2   # TDB200_ABI_VERSION of include/tdb200.h, whose prototypes _PROTOS mirrors
 
 _lib = None
@@ -141,7 +147,8 @@ class _DeviceGuarded:
 
 
 LAUNCHES = 0  # kernels launched through the C ABI (each entry point documents how many it enqueues)
-_KERNELS_PER_CALL = {"sla_quant_qk": 4, "layernorm_modulate_quant": 2, "sla_attn16_bwd": 4, "attn_dense_bwd": 3}  # upper bounds per entry point
+_KERNELS_PER_CALL = {"sla_quant_qk": 4, "layernorm_modulate_quant": 2, "sla_attn16_bwd": 4, "attn_dense_bwd": 3,
+                     "sla_linear_bwd": 8, "sla_linear_tangent": 5}  # upper bounds per entry point
 
 
 def check(rc: int, what: str, launches: int = None) -> None:

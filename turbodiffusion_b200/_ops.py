@@ -23,12 +23,12 @@ def _cdiv(a, b):
     return (a + b - 1) // b
 
 
-def _op(schema: str, cuda, fake):
+def _op(schema: str, cuda, fake, lib=LIB, ns="tdb200"):
     name = schema.split("(", 1)[0]
-    LIB.define(schema)
-    LIB.impl(name, cuda, "CUDA")
-    torch.library.register_fake("tdb200::" + name, fake, lib=LIB)
-    return getattr(torch.ops.tdb200, name).default
+    lib.define(schema)
+    lib.impl(name, cuda, "CUDA")
+    torch.library.register_fake(f"{ns}::{name}", fake, lib=lib)
+    return getattr(getattr(torch.ops, ns), name).default
 
 
 def _like(x, shape=None, dtype=None):
@@ -531,3 +531,80 @@ def _attn16_backward(ctx, d_o, d_lse):
 
 
 torch.library.register_autograd("tdb200::sla_attn16_fwd_lse", _attn16_backward, setup_context=_attn16_setup_context, lib=LIB)
+
+
+# ------------------------------------------------------------------------------------------------ SLA linear branch (training)
+# In a namespace of their own: the tdb200:: set is the one tests/test_compile_host.py pairs one-to-one with its fake-kernel
+# cases; these two have theirs in tests/test_sla_linear_branch_host.py.
+LIB_LINEAR = torch.library.Library("tdb200_linear", "DEF")
+def _linear_fwd_fake(q, k, v, w, bias, feature):
+    return _like(q), _moments_fake(k, v, feature)
+
+
+def _linear_fwd_cuda(q, k, v, w, bias, feature):
+    """(o_l, the moments buffer of sla_linear_moments): the buffer (kv, ksum) is what the backward reads."""
+    b, l, h, d = q.shape
+    mom = _moments_cuda(k, v, feature)
+    o_l = _like(q)
+    check(lib().tdb200_sla_linear_fwd(ptr(q), ptr(mom), ptr(mom) + 4 * b * h * d * d, ptr(w), ptr(bias), DTYPE_TAG[q.dtype],
+                                      feature, ptr(o_l), b, l, h, d, stream_ptr(q.device)), "sla_linear_fwd")
+    return o_l, mom
+
+
+sla_linear_fwd = _op("sla_linear_fwd(Tensor q, Tensor k, Tensor v, Tensor w, Tensor bias, int feature) -> (Tensor, Tensor)",
+                     _linear_fwd_cuda, _linear_fwd_fake, LIB_LINEAR, "tdb200_linear")
+
+
+def _linear_bwd_fake(q, k, v, d_o, mom, w, feature):
+    return _like(q), _like(q), _like(q), _like(w), _like(w, shape=(w.shape[0],))
+
+
+def _linear_bwd_cuda(q, k, v, d_o, mom, w, feature):
+    b, l, h, d = q.shape
+    dq, dk, dv, dw, db = _linear_bwd_fake(q, k, v, d_o, mom, w, feature)
+    nbytes = lib().tdb200_sla_linear_bwd_workspace_bytes(b, h, l, d)
+    check(0 if nbytes >= 0 else nbytes, "sla_linear_bwd_workspace_bytes", launches=0)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
+    check(lib().tdb200_sla_linear_bwd(ptr(q), ptr(k), ptr(v), ptr(d_o), ptr(mom), ptr(mom) + 4 * b * h * d * d, ptr(w),
+                                      DTYPE_TAG[q.dtype], feature, ptr(dq), ptr(dk), ptr(dv), ptr(dw), ptr(db), ptr(ws), nbytes,
+                                      b, l, h, d, stream_ptr(q.device)), "sla_linear_bwd")
+    return dq, dk, dv, dw, db
+
+
+sla_linear_bwd = _op("sla_linear_bwd(Tensor q, Tensor k, Tensor v, Tensor d_o, Tensor mom, Tensor w, int feature) "
+                     "-> (Tensor, Tensor, Tensor, Tensor, Tensor)", _linear_bwd_cuda, _linear_bwd_fake, LIB_LINEAR,
+                     "tdb200_linear")
+
+
+def _linear_tangent_cuda(q, k, v, q_t, k_t, v_t, mom, w, feature):
+    b, l, h, d = q.shape
+    o_t = _like(q)
+    nbytes = lib().tdb200_sla_linear_tangent_workspace_bytes(b, h, l, d)
+    check(0 if nbytes >= 0 else nbytes, "sla_linear_tangent_workspace_bytes", launches=0)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
+    check(lib().tdb200_sla_linear_tangent(ptr(q), ptr(k), ptr(v), ptr(q_t), ptr(k_t), ptr(v_t), ptr(mom),
+                                          ptr(mom) + 4 * b * h * d * d, ptr(w), DTYPE_TAG[q.dtype], feature, ptr(o_t), ptr(ws),
+                                          nbytes, b, l, h, d, stream_ptr(q.device)), "sla_linear_tangent")
+    return o_t
+
+
+sla_linear_tangent = _op("sla_linear_tangent(Tensor q, Tensor k, Tensor v, Tensor q_t, Tensor k_t, Tensor v_t, Tensor mom, "
+                         "Tensor w, int feature) -> Tensor", _linear_tangent_cuda, lambda q, *rest: _like(q), LIB_LINEAR,
+                         "tdb200_linear")
+
+
+def _linear_setup_context(ctx, inputs, output):
+    q, k, v, w, bias, feature = inputs
+    ctx.save_for_backward(q, k, v, w, output[1])
+    ctx.feature = feature
+
+
+def _linear_backward(ctx, d_o, d_mom):
+    """Gradients of o_l in q, k, v, proj_w and proj_b; the moments buffer is a by-product, not differentiated."""
+    q, k, v, w, mom = ctx.saved_tensors
+    dq, dk, dv, dw, db = sla_linear_bwd(q, k, v, d_o.to(q.dtype).contiguous(), mom, w, ctx.feature)
+    return dq, dk, dv, dw, db, None
+
+
+torch.library.register_autograd("tdb200_linear::sla_linear_fwd", _linear_backward, setup_context=_linear_setup_context,
+                                lib=LIB_LINEAR)

@@ -14,8 +14,9 @@
 //   Row maxima / sums are reduced across the four lanes that share a row.
 //   After the last key block the linear branch adds A.KVW^T to O with A = phi(q) * l / den in registers, so that
 //   O / l = softmax part + phi(q).KVW^T / den, and out = O / l + proj_b.
-// Shared memory: Q | K ring | V ring (3 stages each; K and V released per warp as soon as their MMA retired) | KVW.
-//   Q/K/KVW are K-major swizzled (128B rows, or 64B rows for 64-wide int8 heads).
+// Shared memory: Q | K ring | V ring (3 stages each; K and V released per warp as soon as their MMA retired) | KVW, and for
+//   INT8 Q/K the 16-bit query rows, loaded with Q and read by the linear branch, whose rows each warp then overwrites with
+//   its 16 output rows for a TMA store.  Q/K/KVW are K-major swizzled (128B rows, or 64B rows for 64-wide int8 heads).
 // The O accumulator is only rescaled when a row maximum grows by more than 2^8 (lazy rescale): P stays <= 256, which
 // bf16/fp32 hold exactly as well as P <= 1, and the final O / l normalisation is unchanged.
 // Entry points: tdb200_sla_attn_fwd (INT8 Q/K, head dims 64 and 128, feature maps of the linear branch, K head-major or in
@@ -43,11 +44,14 @@ struct Lay {
   static constexpr uint32_t kKBytes = kQK16 ? kBK * HD * 2 : kBK * HD;
   static constexpr uint32_t kVBytes = kBK * HD * 2;                        // HD/64 boxes of [kBK keys x 128 B]
   static constexpr uint32_t kWBytes = HD * HD * 2;                         // HD/64 d_k chunks of [HD rows x 128 B]
+  // INT8 only: the 16-bit query rows for phi(q), HD/64 chunks of [kBQ rows x 128 B], then the output rows staged for TMA
+  static constexpr uint32_t kQ16Bytes = kQK16 ? 0 : kBQ * HD * 2;
   static constexpr uint32_t kOffQ = 0;
   static constexpr uint32_t kOffK = kOffQ + kQBytes;
   static constexpr uint32_t kOffV = kOffK + kStages * kKBytes;
   static constexpr uint32_t kOffW = kOffV + kStages * kVBytes;
-  static constexpr uint32_t kOffBars = kOffW + kWBytes;
+  static constexpr uint32_t kOffQ16 = kOffW + kWBytes;
+  static constexpr uint32_t kOffBars = kOffQ16 + kQ16Bytes;
   static constexpr uint32_t kOffLut = kOffBars + 256;
 };
 static_assert(split::kNumBars * 8 <= 256, "barriers exceed their shared-memory slot");
@@ -89,27 +93,57 @@ __device__ __forceinline__ void store_o_lse(const float (&o)[HD / 2], const floa
   }
 }
 
+// The INT8 kernels' 16 query rows of one warp in shared memory: the 16-bit query rows TMA loaded with the Q barrier, HD/64
+// chunks of [16 rows x 128 B] `chunk` bytes apart in the 128-byte swizzle, which the output rows overwrite and a TMA store
+// (map `tmap_out`, boxes of 64 columns x 16 rows at query row `row`) writes out.
+struct RowTile {
+  uint8_t* smem;
+  uint32_t chunk;
+  const CUtensorMap* tmap_out;
+  int32_t row;
+};
+
+__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
+}
+__device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+
 // After the last key block, for the 64 query rows of one warpgroup (rows qrow0 + {0, 8} for this thread): the linear branch
 // adds A.KVW^T to O, then out = T( O / l + proj_b ).  kvw_smem: the KVW tile (K-major, swizzled like Q).
-template <typename T, int HD>
+// kTile (the INT8 kernels): the query rows are read from and the output rows written through the warp's RowTile, and rows
+// >= l are clipped by the tensor map; otherwise the query rows are read from and the output rows stored to global memory.
+template <typename T, int HD, bool kTile = false>
 __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const float (&l_part)[2], const AttnParams& p,
-                                                    uint32_t kvw_smem, int64_t qrow0, int cq, int b, int hh, int bh) {
+                                                    uint32_t kvw_smem, int64_t qrow0, int cq, int b, int hh, int bh,
+                                                    const RowTile& tile = RowTile{}) {
   constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
   const float l_tot[2] = {quad_sum(l_part[0]), quad_sum(l_part[1])};
+  const int lane = threadIdx.x & 31;
+  const uint32_t tile_s = smem_u32(tile.smem);
 
   // ---- linear branch operand (SLA/core.py:243).  f_j = feature map numerator of the query row:
   //      E = sum f_j, F = sum f_j * ksum_j;  phi_j = f_j / E (softmax) or f_j;  den = 1e-5 + sum_j phi_j ksum_j;
   //      A_j = T(phi_j * l / den), so that O + A.KVW^T = l * (O/l + phi.KVW^T/den).
   //      This thread holds, for each K=16 step kk, the column pairs 16 kk + cq and 16 kk + 8 + cq of its two rows.
   uint32_t qa[HD / 16][4];
+  if constexpr (kTile) {   // lane i addresses row (i & 7) + 8 ((i >> 3) & 1), 16-byte column unit i >> 4 of each K = 16 step
+    const int r = (lane & 7) + 8 * ((lane >> 3) & 1);
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int64_t qr = qrow0 + 8 * h;
-    const T* qrow = static_cast<const T*>(p.q) + ((int64_t(b) * p.l + (qr < p.l ? qr : p.l - 1)) * p.h + hh) * HD;
+    for (int kk = 0; kk < HD / 16; ++kk)
+      ldsm_x4(qa[kk], tile_s + (kk >> 2) * tile.chunk + r * 128 + ((((kk & 3) * 2 + (lane >> 4)) ^ (lane & 7)) << 4));
+  } else {
 #pragma unroll
-    for (int kk = 0; kk < HD / 16; ++kk) {
-      qa[kk][h] = __ldg(reinterpret_cast<const unsigned int*>(qrow + 16 * kk + cq));
-      qa[kk][2 + h] = __ldg(reinterpret_cast<const unsigned int*>(qrow + 16 * kk + 8 + cq));
+    for (int h = 0; h < 2; ++h) {
+      const int64_t qr = qrow0 + 8 * h;
+      const T* qrow = static_cast<const T*>(p.q) + ((int64_t(b) * p.l + (qr < p.l ? qr : p.l - 1)) * p.h + hh) * HD;
+#pragma unroll
+      for (int kk = 0; kk < HD / 16; ++kk) {
+        qa[kk][h] = __ldg(reinterpret_cast<const unsigned int*>(qrow + 16 * kk + cq));
+        qa[kk][2 + h] = __ldg(reinterpret_cast<const unsigned int*>(qrow + 16 * kk + 8 + cq));
+      }
     }
   }
   const float* ks = p.ksum + int64_t(bh) * HD;
@@ -182,17 +216,40 @@ __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const fl
   for (int kk = 0; kk < HD / 16; ++kk) reg_fence(qa[kk]);
 
   // ---- out = T( O / l + proj_b )
+  if constexpr (kTile) {   // this thread's rows lane / 4 + {0, 8} of the tile, over the query rows it was read from
+    __syncwarp();
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int64_t qr = qrow0 + 8 * h;
-    if (qr >= p.l) continue;
-    const float inv_l = kBF16 ? 1.0f / l_tot[h] : 1.0f / l_tot[h] * out_scale[h];
-    T* orow = static_cast<T*>(p.out) + ((int64_t(b) * p.l + qr) * p.h + hh) * HD;
+    for (int h = 0; h < 2; ++h) {
+      const float inv_l = kBF16 ? 1.0f / l_tot[h] : 1.0f / l_tot[h] * out_scale[h];
+      const uint32_t row_s = tile_s + ((lane >> 2) + 8 * h) * 128 + 2 * cq;
 #pragma unroll
-    for (int c = 0; c < HD / 8; ++c) {
-      const float2 pb = __ldg(reinterpret_cast<const float2*>(p.proj_b + 8 * c + cq));
-      *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) =
-          F16Traits<T>::pack(fmaf(o[4 * c + 2 * h], inv_l, pb.x), fmaf(o[4 * c + 2 * h + 1], inv_l, pb.y));
+      for (int c = 0; c < HD / 8; ++c) {
+        const float2 pb = __ldg(reinterpret_cast<const float2*>(p.proj_b + 8 * c + cq));
+        sts_u32(row_s + (c >> 3) * tile.chunk + (((c & 7) ^ (lane >> 2)) << 4),
+                F16Traits<T>::pack(fmaf(o[4 * c + 2 * h], inv_l, pb.x), fmaf(o[4 * c + 2 * h + 1], inv_l, pb.y)));
+      }
+    }
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+#pragma unroll
+      for (int c = 0; c < HD / 64; ++c) tma_store_4d(tile.tmap_out, tile.smem + c * tile.chunk, c * 64, hh, tile.row, b);
+      tma_store_commit();
+      tma_store_wait_read<0>();   // the shared memory stays the CTA's until the copy has read it
+    }
+  } else {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t qr = qrow0 + 8 * h;
+      if (qr >= p.l) continue;
+      const float inv_l = kBF16 ? 1.0f / l_tot[h] : 1.0f / l_tot[h] * out_scale[h];
+      T* orow = static_cast<T*>(p.out) + ((int64_t(b) * p.l + qr) * p.h + hh) * HD;
+#pragma unroll
+      for (int c = 0; c < HD / 8; ++c) {
+        const float2 pb = __ldg(reinterpret_cast<const float2*>(p.proj_b + 8 * c + cq));
+        *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) =
+            F16Traits<T>::pack(fmaf(o[4 * c + 2 * h], inv_l, pb.x), fmaf(o[4 * c + 2 * h + 1], inv_l, pb.y));
+      }
     }
   }
 }
@@ -202,7 +259,8 @@ __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const fl
 template <typename T, int HD, bool kQK16, bool kLse = false>
 __global__ void __launch_bounds__(kThreads, 1)
 sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                    const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw, AttnParams p) {
+                    const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw, AttnParams p,
+                    const __grid_constant__ CUtensorMap tmap_q16, const __grid_constant__ CUtensorMap tmap_out) {
   using L = Lay<HD, kQK16>;
   constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
@@ -244,13 +302,18 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
       tma_prefetch_desc(&tmap_k);
       tma_prefetch_desc(&tmap_v);
       if constexpr (!kLse) tma_prefetch_desc(&tmap_kvw);
-      mbar_expect_tx(&bars[kQFull], L::kQBytes + (kLse ? 0 : L::kWBytes));
+      mbar_expect_tx(&bars[kQFull], L::kQBytes + (kLse ? 0 : L::kWBytes) + L::kQ16Bytes);
       if constexpr (kQK16) {  // 16-bit Q rows from [B,L,H,D]: HD/64 chunks of 128 rows x 128 B
 #pragma unroll
         for (int c = 0; c < HD / 64; ++c)
           tma_load_4d(smem + L::kOffQ + c * (BLKQ * 128), &tmap_q, &bars[kQFull], c * 64, hh, m_blk * BLKQ, b);
       } else {
+        tma_prefetch_desc(&tmap_q16);
+        tma_prefetch_desc(&tmap_out);
         tma_load_4d(smem + L::kOffQ, &tmap_q, &bars[kQFull], 0, m_blk * BLKQ, bh, 0);
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c)  // the same rows in 16 bits, for phi(q)
+          tma_load_4d(smem + L::kOffQ16 + c * (BLKQ * 128), &tmap_q16, &bars[kQFull], c * 64, hh, m_blk * BLKQ, b);
       }
       if constexpr (!kLse) {
 #pragma unroll
@@ -310,10 +373,15 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   mbar_wait(&bars[kKFull], 0);
   score_issue<kQK16, HD, BLKK, kBF16>(sacc, sq, BLKQ * 128, sbase + L::kOffK);
   wgmma_wait<0>();
-  score_finish<kQK16, BLKK>(sacc, s, qsc * s_ksc[0]);
-  warp_release(&bars[kKEmpty], lane);
   // valid < 64 only in the ragged last key block
-  softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, p.lk - int(s_lut[0]) * BLKK, cq, true);
+  if constexpr (kQK16) {
+    score_finish<kQK16, BLKK>(sacc, s, qsc * s_ksc[0]);
+    warp_release(&bars[kKEmpty], lane);
+    softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, p.lk - int(s_lut[0]) * BLKK, cq, true);
+  } else {
+    warp_release(&bars[kKEmpty], lane);
+    softmax_p_i8<BLKK>(sacc, s, qsc * s_ksc[0], m_used, l_part, rescale, alpha, p.lk - int(s_lut[0]) * BLKK, cq, true);
+  }
   for (int j = 0; j < T_blocks; ++j) {
     const int st = j % kStages, st1 = (j + 1) % kStages;
     const bool next = j + 1 < T_blocks;
@@ -327,9 +395,15 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     pv_issue<HD, BLKK, kBF16>(o, pa, sbase + L::kOffV + st * L::kVBytes);
     wgmma_wait<1>();                                    // S_{j+1} retired, P_j.V_j may still run
     if (next) {
-      score_finish<kQK16, BLKK>(sacc, s, qsc * s_ksc[j + 1]);
-      warp_release(&bars[kKEmpty + st1], lane);
-      softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, p.lk - int(s_lut[j + 1]) * BLKK, cq, false);
+      if constexpr (kQK16) {
+        score_finish<kQK16, BLKK>(sacc, s, qsc * s_ksc[j + 1]);
+        warp_release(&bars[kKEmpty + st1], lane);
+        softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, p.lk - int(s_lut[j + 1]) * BLKK, cq, false);
+      } else {
+        warp_release(&bars[kKEmpty + st1], lane);
+        softmax_p_i8<BLKK>(sacc, s, qsc * s_ksc[j + 1], m_used, l_part, rescale, alpha, p.lk - int(s_lut[j + 1]) * BLKK, cq,
+                           false);
+      }
     }
     wgmma_wait<0>();
     pv_fence<HD, BLKK>(o, pa);
@@ -337,8 +411,12 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   }
   if constexpr (kLse) {
     store_o_lse<T, HD>(o, m_used, l_part, p, int64_t(m_blk) * BLKQ + r_lo, cq, b, hh, bh);
-  } else {
+  } else if constexpr (kQK16) {
     linear_branch_store<T, HD>(o, l_part, p, sbase + L::kOffW, int64_t(m_blk) * BLKQ + r_lo, cq, b, hh, bh);
+  } else {
+    const int row16 = wg * 64 + w4 * 16;   // this warp's 16 rows of the block
+    const RowTile tile{smem + L::kOffQ16 + row16 * 128, BLKQ * 128, &tmap_out, m_blk * BLKQ + row16};
+    linear_branch_store<T, HD, true>(o, l_part, p, sbase + L::kOffW, int64_t(m_blk) * BLKQ + r_lo, cq, b, hh, bh, tile);
   }
 }
 
@@ -354,7 +432,8 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 template <typename T, int HD, bool kQK16, int BK, bool kLse>
 __global__ void __launch_bounds__(split::kThreads, 1)
 sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                        const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw, AttnParams p) {
+                        const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw, AttnParams p,
+                        const __grid_constant__ CUtensorMap tmap_q16, const __grid_constant__ CUtensorMap tmap_out) {
   constexpr int BQ = kBlkQ64;
   using L = Lay<HD, kQK16, BQ, BK>;
   // hand-off of warpgroup 1's state: HD/2 accumulator registers + m_used[2] + l_part[2] per thread, over the K and V rings
@@ -391,13 +470,18 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
       tma_prefetch_desc(&tmap_k);
       tma_prefetch_desc(&tmap_v);
       if constexpr (!kLse) tma_prefetch_desc(&tmap_kvw);
-      mbar_expect_tx(&bars[split::kQFull], L::kQBytes + (kLse ? 0 : L::kWBytes));
+      mbar_expect_tx(&bars[split::kQFull], L::kQBytes + (kLse ? 0 : L::kWBytes) + L::kQ16Bytes);
       if constexpr (kQK16) {
 #pragma unroll
         for (int c = 0; c < HD / 64; ++c)
           tma_load_4d(smem + L::kOffQ + c * (BQ * 128), &tmap_q, &bars[split::kQFull], c * 64, hh, m_blk * BQ, b);
       } else {
+        tma_prefetch_desc(&tmap_q16);
+        tma_prefetch_desc(&tmap_out);
         tma_load_4d(smem + L::kOffQ, &tmap_q, &bars[split::kQFull], 0, m_blk * BQ, bh, 0);
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c)
+          tma_load_4d(smem + L::kOffQ16 + c * (BQ * 128), &tmap_q16, &bars[split::kQFull], c * 64, hh, m_blk * BQ, b);
       }
       if constexpr (!kLse) {
 #pragma unroll
@@ -451,11 +535,23 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
     const int valid = p.lk - blk * BK;                  // < BK only in the ragged last key block
 
     float s[BK / 2];
-    mbar_wait(&bars[split::full(split::kKFull, j)], ph);
-    score_tile<kQK16, HD, BK, kBF16>(s, sbase + L::kOffQ, BQ * 128, sbase + L::kOffK + st * L::kKBytes, sc);
-    warp_release(&bars[split::kKEmpty + st], lane);
     uint32_t pa[BK / 16][4];
-    softmax_step<T, HD, BK>(s, o, m_used, l_part, pa, valid, cq, j == wg);
+    mbar_wait(&bars[split::full(split::kKFull, j)], ph);
+    if constexpr (kQK16) {
+      score_tile<kQK16, HD, BK, kBF16>(s, sbase + L::kOffQ, BQ * 128, sbase + L::kOffK + st * L::kKBytes, sc);
+      warp_release(&bars[split::kKEmpty + st], lane);
+      softmax_step<T, HD, BK>(s, o, m_used, l_part, pa, valid, cq, j == wg);
+    } else {
+      uint32_t si[BK / 2];
+      score_issue<kQK16, HD, BK, kBF16>(si, sbase + L::kOffQ, BQ * 128, sbase + L::kOffK + st * L::kKBytes);
+      wgmma_wait<0>();
+      warp_release(&bars[split::kKEmpty + st], lane);
+      bool rescale[2];
+      float alpha[2];
+      softmax_p_i8<BK>(si, s, sc, m_used, l_part, rescale, alpha, valid, cq, j == wg);
+      rescale_o<HD>(o, rescale, alpha);
+      pack_p<T, BK>(s, pa);
+    }
     mbar_wait(&bars[split::full(split::kVFull, j)], ph);
     pv_step<HD, BK, kBF16>(o, pa, sbase + L::kOffV + st * L::kVBytes);
     warp_release(&bars[split::kVEmpty + st], lane);
@@ -489,8 +585,11 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
   const int64_t qrow0 = int64_t(m_blk) * BQ + r_lo;
   if constexpr (kLse) {
     store_o_lse<T, HD>(o, m_used, l_part, p, qrow0, cq, b, hh, bh);
-  } else {
+  } else if constexpr (kQK16) {
     linear_branch_store<T, HD>(o, l_part, p, sbase + L::kOffW, qrow0, cq, b, hh, bh);
+  } else {
+    const RowTile tile{smem + L::kOffQ16 + w4 * 16 * 128, BQ * 128, &tmap_out, m_blk * BQ + w4 * 16};
+    linear_branch_store<T, HD, true>(o, l_part, p, sbase + L::kOffW, qrow0, cq, b, hh, bh, tile);
   }
 }
 
@@ -521,7 +620,7 @@ int launch(const void* q_op, const float* q_scale, const void* k_op, const float
 
   const CUtensorMapDataType t16 = dtype == TDB200_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const int sw8 = HD == 128 ? 128 : 64;
-  CUtensorMap tq, tk, tv, tw;
+  CUtensorMap tq, tk, tv, tw, tq16, tout;
   if (kQK16) {  // 16-bit Q / K rows in the module layout [b, l, h, d]
     const uint64_t dq[4] = {uint64_t(d), uint64_t(h), uint64_t(l), uint64_t(b)};
     const uint64_t sq[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(l * h * d * 2)};
@@ -551,6 +650,15 @@ int launch(const void* q_op, const float* q_scale, const void* k_op, const float
     const uint64_t str[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(lk * h * d * 2)};
     const uint32_t box[4] = {64, 1, kBK, 1};
     if (int rc = make_tmap_4d(&tv, v, t16, 2, dims, str, box)) return rc;
+  }
+  if (kQK16) {
+    tq16 = tout = tv;  // not read
+  } else {  // INT8: the 16-bit query rows for phi(q), and the output, both [b, l, h, d] in 16-bit boxes of 64 columns
+    const uint64_t dims[4] = {uint64_t(d), uint64_t(h), uint64_t(l), uint64_t(b)};
+    const uint64_t str[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(l * h * d * 2)};
+    const uint32_t bq[4] = {64, 1, kBQ, 1}, bo[4] = {64, 1, 16, 1};
+    if (int rc = make_tmap_4d(&tq16, q, t16, 2, dims, str, bq)) return rc;
+    if (int rc = make_tmap_4d(&tout, out, t16, 2, dims, str, bo)) return rc;
   }
   if (kLse) {
     tw = tv;  // not read
@@ -586,7 +694,7 @@ int launch(const void* q_op, const float* q_scale, const void* k_op, const float
     if (int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), \
                             "cudaFuncSetAttribute(sla_attn)"))                                                        \
       return rc;                                                                                                      \
-    kern<<<grid, threads, smem, st>>>(tq, tk, tv, tw, p);                                                             \
+    kern<<<grid, threads, smem, st>>>(tq, tk, tv, tw, p, tq16, tout);                                                 \
     return check_launch("sla_attn_fwd_kernel");                                                                       \
   } while (0)
   if (dtype == TDB200_DTYPE_BF16) TDB_ATTN(__nv_bfloat16);

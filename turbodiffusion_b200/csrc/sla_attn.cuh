@@ -132,6 +132,58 @@ __device__ __forceinline__ void softmax_p(float (&s)[BK / 2], float (&m_used)[2]
   }
 }
 
+// softmax_p for INT8 Q/K, straight from score_issue's int32 accumulator once its group has retired: p = P, unrounded, for the
+// scores s = float(acc) * sc.  sc >= 0 and rounding is monotone, so the row maxima are taken on the integers (IMNMX) and
+// float(max) * sc is the maximum softmax_p finds.  Each exponent argument keeps softmax_p's two roundings, s and then s - m,
+// so every bit of P, l and O is softmax_p's (one FFMA instead is faster, but its last-bit changes do not stay last-bit
+// after the INT8 quantisation of the next layer's input; DESIGN.md).  The ragged last key block masks the float argument to
+// -inf as softmax_p does (an INT_MIN score times a small sc minus m would not underflow exp2).  kRagged: the block has columns
+// from `valid` on.  Full blocks run their own instantiation without the per-column test: written as one path, ptxas
+// predicates the test into every element of every block.
+template <int BK, bool kRagged>
+__device__ __forceinline__ void softmax_p_i8_cols(uint32_t (&acc)[BK / 2], float (&p)[BK / 2], float sc, float (&m_used)[2],
+                                                  float (&l_part)[2], bool (&rescale)[2], float (&alpha)[2], int valid, int cq,
+                                                  bool first) {
+  auto dead = [&](int i) { return kRagged && 8 * (i >> 2) + cq + (i & 1) >= valid; };
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    int imx = INT_MIN;   // every row has a valid column in its quad
+#pragma unroll
+    for (int i = 0; i < BK / 2; ++i)
+      if (((i >> 1) & 1) == h && !dead(i)) imx = max(imx, static_cast<int>(acc[i]));
+    imx = max(imx, __shfl_xor_sync(0xffffffffu, imx, 1));
+    imx = max(imx, __shfl_xor_sync(0xffffffffu, imx, 2));
+    const float mx = static_cast<float>(imx) * sc;
+    rescale[h] = false;
+    alpha[h] = 1.0f;
+    if (first) {
+      m_used[h] = mx;
+    } else if (mx > m_used[h] + kRescaleThreshold) {
+      alpha[h] = fast_exp2(m_used[h] - mx);
+      rescale[h] = true;
+      l_part[h] *= alpha[h];
+      m_used[h] = mx;
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < BK / 2; i += 2) {
+    const int h = (i >> 1) & 1;
+    const float x0 = __fsub_rn(__fmul_rn(static_cast<float>(static_cast<int>(acc[i])), sc), m_used[h]);
+    const float x1 = __fsub_rn(__fmul_rn(static_cast<float>(static_cast<int>(acc[i + 1])), sc), m_used[h]);
+    p[i] = fast_exp2(dead(i) ? -INFINITY : x0);
+    p[i + 1] = fast_exp2(dead(i + 1) ? -INFINITY : x1);
+    l_part[h] += p[i] + p[i + 1];
+  }
+}
+template <int BK>
+__device__ __forceinline__ void softmax_p_i8(uint32_t (&acc)[BK / 2], float (&p)[BK / 2], float sc, float (&m_used)[2],
+                                             float (&l_part)[2], bool (&rescale)[2], float (&alpha)[2], int valid, int cq,
+                                             bool first) {
+  reg_fence(acc);
+  if (valid < BK) softmax_p_i8_cols<BK, true>(acc, p, sc, m_used, l_part, rescale, alpha, valid, cq, first);
+  else softmax_p_i8_cols<BK, false>(acc, p, sc, m_used, l_part, rescale, alpha, valid, cq, first);
+}
+
 // The O part of the step: the lazy rescale softmax_p decided.  O must hold every earlier entry's P.V.
 template <int HD>
 __device__ __forceinline__ void rescale_o(float (&o)[HD / 2], const bool (&rescale)[2], const float (&alpha)[2]) {

@@ -207,6 +207,31 @@ int tdb200_sla_attn_fwd(const int8_t* q_i8, const float* q_scale, const int8_t* 
                         const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
                         int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq, int64_t blkk,
                         int k_seq_major, void* stream);
+/* SageSLA with FP8 P.V (SageAttention2's arithmetic: e4m3 P and V, per-channel V scales), an option beside the 16-bit P.V of
+ * tdb200_sla_attn_fwd; d = 128 only.
+ * tdb200_sla_quant_v_fp8  v [b,l,h,d] 16-bit (`dtype`) -> v_scale [b,h,d] fp32 and v_fp8 [b,h,d,l_pad] e4m3 codes, l_pad =
+ *     ceil(l / blkk) * blkk (blkk = 64 or 128, the key block of the attention call).  v_scale = max(amax over all l rows of the
+ *     channel, 2^-64) / 448, an IEEE division; codes = e4m3(v / v_scale), IEEE division then round to nearest even, saturated to
+ *     +-448 (what torch's float32 -> float8_e4m3fn cast gives for these values).  Keys l..l_pad-1 are zero codes.  Inside every
+ *     32-key group the keys are stored permuted for the kernel's register fragment: position 16 u + 4 t + j holds key
+ *     16 u + 8 (j >> 1) + 2 t + (j & 1).  A memset and three kernels on `stream`; the scales are order-independent (a max), so
+ *     both outputs are bit-reproducible.
+ * tdb200_sla_attn_fwd_fp8v  tdb200_sla_attn_fwd with `v` replaced by v_fp8 / v_scale from tdb200_sla_quant_v_fp8 over the lk keys
+ *     with the same blkk.  P (fp32, unrounded, <= 2^8 under the lazy rescale) is rounded to e4m3 as the MMA operand with the
+ *     scale 2^0; the row sum l is taken from the unrounded P as in tdb200_sla_attn_fwd.  Each key block's P.V is one chain of
+ *     e4m3 x e4m3 wgmma (whose accumulation is narrower than fp32), added to O in fp32; the softmax part is O * v_scale[d] / l; the linear branch, its fp16 range scaling and the output store
+ *     are tdb200_sla_attn_fwd's.  Both block families and k_seq_major as there.
+ * Errors, all before any CUDA call: null pointer, non-positive b, l, lk, h or d, or (tdb200_sla_quant_v_fp8: any buffer,
+ * tdb200_sla_attn_fwd_fp8v: v_fp8, v_scale) not 16-byte aligned -> TDB200_ERR_INVALID_ARG, as are a bad feature tag and topk
+ * outside [1, nblk]; d != 128, block sizes other than (128, 64) and (64, 128) (blkk other than 64 and 128), a bad dtype tag,
+ * b or h above 65535, sequence-major K with another feature map than softmax or b != 1 -> TDB200_ERR_UNSUPPORTED. */
+int tdb200_sla_quant_v_fp8(const void* v, int dtype, int64_t b, int64_t l, int64_t h, int64_t d, int64_t blkk, uint8_t* v_fp8,
+                           float* v_scale, void* stream);
+int tdb200_sla_attn_fwd_fp8v(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
+                             const uint8_t* v_fp8, const float* v_scale, const void* q, int dtype, const int32_t* lut,
+                             int64_t topk, const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
+                             int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq,
+                             int64_t blkk, int k_seq_major, void* stream);
 /* SparseLinearAttention's linear branch and proj_l for training (reference SLA/core.py:104-117), per (batch, head), phi the
  * feature map `feature` (0 softmax over d, 1 elu+1, 2 relu), c = T(phi(x)), kv = M^T [b,h,d(v),d(k)] and ksum = s [b,h,d] fp32
  * from tdb200_sla_linear_moments of the same k, v and feature:

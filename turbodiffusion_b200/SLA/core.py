@@ -47,21 +47,29 @@ def project_moments(proj_w: torch.Tensor, kv: torch.Tensor, dtype) -> torch.Tens
 ATTN_TIMER = None  # bench.py installs a callable(h, mblk, topk, d) -> context manager to time the fused-attention launches
 
 
-def attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, feature=0, blkq=128, blkk=64):
-    """(blkq, blkk): the block sizes `prep` and `lut` were built with, (128, 64) or (64, 128)."""
+def attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, feature=0, blkq=128, blkk=64, fp8_v=False):
+    """(blkq, blkk): the block sizes `prep` and `lut` were built with, (128, 64) or (64, 128).  fp8_v: P.V on e4m3 P and V
+    (tdb200_sla_quant_v_fp8 of the first lk rows of v, then tdb200_sla_attn_fwd_fp8v; d = 128)."""
     if ATTN_TIMER is not None:
         # bench.py counts H*Mblk*topk*4*128*64*D FLOPs: exact for both families, BLKQ*BLKK = 8192 in each
         with ATTN_TIMER(q.shape[2] * q.shape[0], (q.shape[1] + blkq - 1) // blkq, topk, q.shape[3]):
-            return _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk, feature, blkq, blkk)
-    return _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk, feature, blkq, blkk)
+            return _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk, feature, blkq, blkk, fp8_v)
+    return _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk, feature, blkq, blkk, fp8_v)
 
 
-def _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, feature=0, blkq=128, blkk=64):
+def _attn_fwd(prep, v, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk=None, feature=0, blkq=128, blkk=64, fp8_v=False):
     d = q.shape[3]
     lk = v.shape[1] if lk is None else lk
     k_seq_major = bool(getattr(prep, "k_seq_major", False))   # INT8 K in the gathered [B, Lk, H, D] layout (dist.py)
     if k_seq_major and (d != 128 or feature != 0):
         raise NotImplementedError("sequence-major INT8 K is served by the 128-wide softmax kernels only")
+    if fp8_v:
+        if d != 128:
+            raise NotImplementedError(f"FP8 P.V (SLA.utils.set_sage_pv('fp8')): head dim {d}; it is served for d = 128")
+        assert v.is_contiguous() and (v.shape[0] == 1 or v.shape[1] == lk)
+        v_fp8, v_scale = _ops.sla_quant_v_fp8(v, lk, blkk)
+        return _ops.sla_attn_fwd_fp8v(prep.q_i8, prep.q_scale, prep.k_i8, prep.k_scale, v_fp8, v_scale, q, lut, topk, kvw, ksum,
+                                      proj_b, float(sm_scale), lk, feature, blkq, blkk, k_seq_major)
     return _ops.sla_attn_fwd(prep.q_i8, prep.q_scale, prep.k_i8, prep.k_scale, v, q, lut, topk, kvw, ksum, proj_b,
                              float(sm_scale), lk, feature, blkq, blkk, k_seq_major)
 
@@ -326,6 +334,10 @@ class _SLABase(nn.Module):
             return self._forward_ad(q, k, v, return_sparsity)
         if not self.quantised_qk and torch.is_grad_enabled() and any(t.requires_grad for t in (q, k, v)):
             return self._forward_train(q, k, v, return_sparsity)
+        fp8_v = self.quantised_qk and _utils.SAGE_PV == "fp8"   # SageSparseLinearAttention under SLA.utils.set_sage_pv("fp8")
+        if fp8_v and q.shape[-1] != 128:
+            raise NotImplementedError(f"SageSparseLinearAttention with FP8 P.V (SLA.utils.set_sage_pv('fp8')): head dim "
+                                      f"{q.shape[-1]}; FP8 P.V is served for d = 128")
         require_cuda(q, k, v)
         dtype = q.dtype
         q, k, v = (t if (t.dtype == self.dtype and t.is_contiguous()) else t.to(self.dtype).contiguous() for t in (q, k, v))
@@ -350,7 +362,8 @@ class _SLABase(nn.Module):
         if not self.quantised_qk and d == 128 and (self.feature == 0 or blkq == 64):
             o = attn_fwd_qk16(q, k, v, lut, real_topk, kvw, ksum, proj_b, d ** -0.5, feature=self.feature, blkq=blkq)
         else:
-            o = attn_fwd(prep, v, q, lut, real_topk, kvw, ksum, proj_b, d ** -0.5, feature=self.feature, blkq=blkq, blkk=blkk)
+            o = attn_fwd(prep, v, q, lut, real_topk, kvw, ksum, proj_b, d ** -0.5, feature=self.feature, blkq=blkq, blkk=blkk,
+                         fp8_v=fp8_v)
         o = o if o.dtype == dtype else o.to(dtype)
         return (o, real_topk / nblk) if return_sparsity else o
 
@@ -562,7 +575,11 @@ fused = _FusedShim()
 
 def _sparse_only_attn(q_int8, k_int8, v_fp8, o, lut, q_scale, k_scale, sm_scale, blkq, blkk):
     """Sparse (softmax) branch only: o [B,H,L,D] <- block-sparse INT8-QK attention over the LUT's key blocks, the linear
-    branch switched off (zero moments, zero bias).  Same kernel as SageSparseLinearAttention.forward."""
+    branch switched off (zero moments, zero bias).  Same kernel as SageSparseLinearAttention.forward, with its P.V setting
+    (SLA.utils.set_sage_pv): under "fp8" the 16-bit V is quantised by tdb200_sla_quant_v_fp8 (d = 128 only)."""
+    fp8_v = _utils.SAGE_PV == "fp8"
+    if fp8_v and q_int8.shape[-1] != 128:
+        raise NotImplementedError(f"FP8 P.V (SLA.utils.set_sage_pv('fp8')): head dim {q_int8.shape[-1]}; it is served for d = 128")
     v = getattr(v_fp8, "_tdb200_src", None)
     if v is None:
         raise RuntimeError("this adapter needs the 16-bit V that SLA.core.fused.* was called with")
@@ -577,7 +594,7 @@ def _sparse_only_attn(q_int8, k_int8, v_fp8, o, lut, q_scale, k_scale, sm_scale,
     ksum = torch.ones(b, h, d, dtype=torch.float32, device=v.device)
     pb = torch.zeros(d, dtype=torch.float32, device=v.device)
     out = attn_fwd(prep, vt, qz, lut, lut.shape[-1], kvw, ksum, pb, sm_scale if sm_scale is not None else d ** -0.5, lk=lk,
-                   blkq=blkq, blkk=blkk)
+                   blkq=blkq, blkk=blkk, fp8_v=fp8_v)
     o.copy_(out.transpose(1, 2))
     return o
 

@@ -1,6 +1,8 @@
 """Mirror of turbodiffusion/SLA/utils.py: mean_pool, get_block_map, get_cuda_arch (H100 implementation)."""
 from __future__ import annotations
 
+import os
+
 import torch
 
 from .. import _ops
@@ -43,6 +45,33 @@ def set_linear_branch(name: str) -> str:
     if name not in LINEAR_BRANCHES:
         raise ValueError(f"linear branch must be one of {list(LINEAR_BRANCHES)}, got {name!r}")
     prev, LINEAR_BRANCH = LINEAR_BRANCH, name
+    return prev
+
+
+# SageSparseLinearAttention's P.V arithmetic (see set_sage_pv).
+SAGE_PV_MODES = ("bf16", "fp8")
+
+
+def _sage_pv_default():
+    mode = os.environ.get("TDB200_SAGE_PV") or "bf16"
+    if mode not in SAGE_PV_MODES:
+        raise ValueError(f"TDB200_SAGE_PV must be one of {list(SAGE_PV_MODES)}, got {mode!r}")
+    return mode
+
+
+SAGE_PV = _sage_pv_default()
+
+
+def set_sage_pv(mode: str) -> str:
+    """Select SageSparseLinearAttention's P.V: "bf16" (16-bit P and V, the default unless the environment variable
+    TDB200_SAGE_PV names the other) or "fp8" (SageAttention2's arithmetic: e4m3 P and V with per-channel V scales,
+    tdb200_sla_quant_v_fp8 + tdb200_sla_attn_fwd_fp8v; both block families, d = 128 only).  Read at every call, by the module
+    and by the LTX adapters in SLA.core; returns the previous value.  Under "fp8", 64-wide heads raise NotImplementedError, and
+    so do sequence parallelism's install and hooks (dist.py)."""
+    global SAGE_PV
+    if mode not in SAGE_PV_MODES:
+        raise ValueError(f"sage P.V must be one of {list(SAGE_PV_MODES)}, got {mode!r}")
+    prev, SAGE_PV = SAGE_PV, mode
     return prev
 
 

@@ -47,6 +47,9 @@ _PROTOS = {
     "tdb200_sla_linear_moments": [_P, _P, _I, _I64, _I64, _I64, _I64, _I, _P, _P, _P],
     "tdb200_sla_attn_fwd": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F,
                             _I, _I64, _I64, _I, _P],
+    "tdb200_sla_quant_v_fp8": [_P, _I, _I64, _I64, _I64, _I64, _I64, _P, _P, _P],
+    "tdb200_sla_attn_fwd_fp8v": [_P, _P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _F,
+                                 _I, _I64, _I64, _I, _P],
     "tdb200_sla_project_moments": [_P, _P, _I, _I64, _I64, _P, _P],
     "tdb200_sla_linear_fwd": [_P, _P, _P, _P, _P, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
     "tdb200_sla_linear_bwd": [_P, _P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _P],
@@ -148,7 +151,7 @@ class _DeviceGuarded:
 
 LAUNCHES = 0  # kernels launched through the C ABI (each entry point documents how many it enqueues)
 _KERNELS_PER_CALL = {"sla_quant_qk": 4, "layernorm_modulate_quant": 2, "sla_attn16_bwd": 4, "attn_dense_bwd": 3,
-                     "sla_linear_bwd": 8, "sla_linear_tangent": 5}  # upper bounds per entry point
+                     "sla_linear_bwd": 8, "sla_linear_tangent": 5, "sla_quant_v_fp8": 4}  # upper bounds per entry point
 
 
 def check(rc: int, what: str, launches: int = None) -> None:

@@ -608,3 +608,43 @@ def _linear_backward(ctx, d_o, d_mom):
 
 torch.library.register_autograd("tdb200_linear::sla_linear_fwd", _linear_backward, setup_context=_linear_setup_context,
                                 lib=LIB_LINEAR)
+
+
+# ------------------------------------------------------------------------------------------------ SageSLA with FP8 P.V
+# In a namespace of their own, like tdb200_linear::; their fake-kernel cases are in tests/test_sla_fp8_pv_host.py.
+LIB_FP8 = torch.library.Library("tdb200_fp8", "DEF")
+
+
+def _quant_v_fp8_fake(v, lk, blkk):
+    b, _, h, d = v.shape
+    return (torch.empty(b, h, d, _cdiv(lk, blkk) * blkk, dtype=torch.uint8, device=v.device),
+            torch.empty(b, h, d, dtype=torch.float32, device=v.device))
+
+
+def _quant_v_fp8_cuda(v, lk, blkk):
+    b, _, h, d = v.shape
+    v_fp8, v_scale = _quant_v_fp8_fake(v, lk, blkk)
+    check(lib().tdb200_sla_quant_v_fp8(ptr(v), DTYPE_TAG[v.dtype], b, lk, h, d, blkk, ptr(v_fp8), ptr(v_scale),
+                                       stream_ptr(v.device)), "sla_quant_v_fp8")
+    return v_fp8, v_scale
+
+
+sla_quant_v_fp8 = _op("sla_quant_v_fp8(Tensor v, int lk, int blkk) -> (Tensor, Tensor)", _quant_v_fp8_cuda, _quant_v_fp8_fake,
+                      LIB_FP8, "tdb200_fp8")
+
+
+def _attn_fwd_fp8v_cuda(q_i8, q_scale, k_i8, k_scale, v_fp8, v_scale, q, lut, topk, kvw, ksum, proj_b, sm_scale, lk, feature,
+                        blkq, blkk, k_seq_major):
+    b, l, h, d = q.shape
+    out = _like(q)
+    check(lib().tdb200_sla_attn_fwd_fp8v(ptr(q_i8), ptr(q_scale), ptr(k_i8), ptr(k_scale), ptr(v_fp8), ptr(v_scale), ptr(q),
+                                         DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b), ptr(out), b, l, lk, h,
+                                         d, sm_scale, feature, blkq, blkk, int(k_seq_major), stream_ptr(q.device)),
+          "sla_attn_fwd_fp8v")
+    return out
+
+
+sla_attn_fwd_fp8v = _op("sla_attn_fwd_fp8v(Tensor q_i8, Tensor q_scale, Tensor k_i8, Tensor k_scale, Tensor v_fp8, "
+                        "Tensor v_scale, Tensor q, Tensor lut, int topk, Tensor kvw, Tensor ksum, Tensor proj_b, float sm_scale, "
+                        "int lk, int feature, int blkq, int blkk, bool k_seq_major) -> Tensor", _attn_fwd_fp8v_cuda,
+                        lambda q_i8, q_scale, k_i8, k_scale, v_fp8, v_scale, q, *rest: _like(q), LIB_FP8, "tdb200_fp8")

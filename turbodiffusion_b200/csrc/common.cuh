@@ -458,7 +458,24 @@ __device__ __forceinline__ void wgmma_f16_rs<128, false, 1>(float (&d)[64], cons
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc)
       : "memory");
 }
-
+// D[64 x N] (+)= A[64 x 32] (registers) . B[32 x N] (shared memory, K-major), e4m3 x e4m3 -> fp32 (accumulated by the tensor
+// core at less than fp32 precision: keep the chains short and sum them on the FMA pipe).  The A fragment of one K = 32
+// step: a[0] = (row l/4, k 4(l%4)+{0..3}), a[1] = (row l/4+8, same k), a[2] = (row l/4, k+16), a[3] = (row l/4+8, k+16),
+// byte j of a register holding k + j.
+template <int N>
+__device__ __forceinline__ void wgmma_e4m3_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_e4m3_rs<128>(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
+      : "memory");
+}
 
 // ------------------------------------------------------------------------------------------
 // register re-distribution between warpgroups (all 4 warps of a warpgroup must execute it)
@@ -558,6 +575,18 @@ __device__ __forceinline__ uint32_t pack4_s8_rne(float a, float b, float c, floa
   const uint32_t lo = __byte_perm(ia, ib, 0x0040);   // byte0 = ia.b0, byte1 = ib.b0
   const uint32_t hi = __byte_perm(ic, id, 0x0040);
   return __byte_perm(lo, hi, 0x5410);                // ia.b0 | ib.b0 << 8 | ic.b0 << 16 | id.b0 << 24
+}
+
+// four fp32 -> four e4m3 codes (round to nearest even, saturated to +-448), a in the lowest byte
+__device__ __forceinline__ uint32_t pack4_e4m3(float a, float b, float c, float d) {
+  uint32_t r;
+  asm("{\n\t.reg .b16 lo, hi;\n\t"
+      "cvt.rn.satfinite.e4m3x2.f32 lo, %2, %1;\n\t"
+      "cvt.rn.satfinite.e4m3x2.f32 hi, %4, %3;\n\t"
+      "mov.b32 %0, {lo, hi};\n\t}"
+      : "=r"(r)
+      : "f"(a), "f"(b), "f"(c), "f"(d));
+  return r;
 }
 
 // lane-wise f32x2 arithmetic, each lane rounded to nearest like the scalar instruction

@@ -38,11 +38,11 @@ constexpr int kThreads = kConsumerWarps * 32 + 32;
 constexpr int kStages = 3;
 static_assert(kStages == split::kStages, "the 64-row kernel uses the entry-split rings");
 
-template <int HD, bool kQK16, int kBQ = BLKQ, int kBK = BLKK>
+template <int HD, bool kQK16, int kBQ = BLKQ, int kBK = BLKK, bool kF8V = false>
 struct Lay {
   static constexpr uint32_t kQBytes = kQK16 ? kBQ * HD * 2 : kBQ * HD;     // 16-bit: HD/64 chunks of [kBQ rows x 128 B]
   static constexpr uint32_t kKBytes = kQK16 ? kBK * HD * 2 : kBK * HD;
-  static constexpr uint32_t kVBytes = kBK * HD * 2;                        // HD/64 boxes of [kBK keys x 128 B]
+  static constexpr uint32_t kVBytes = kF8V ? kBK * HD : kBK * HD * 2;      // HD/64 boxes of [kBK keys x 128 B]; e4m3: [HD x kBK B]
   static constexpr uint32_t kWBytes = HD * HD * 2;                         // HD/64 d_k chunks of [HD rows x 128 B]
   // INT8 only: the 16-bit query rows for phi(q), HD/64 chunks of [kBQ rows x 128 B], then the output rows staged for TMA
   static constexpr uint32_t kQ16Bytes = kQK16 ? 0 : kBQ * HD * 2;
@@ -67,6 +67,7 @@ struct AttnParams {
   int l, lk, h, mblk, nblk, topk, feature;  // feature: 0 softmax, 1 elu+1, 2 relu (SLA/core.py:57-73)
   float sm_scale;
   float* lse;             // [b,h,l] fp32, log2 domain (kLse kernels only)
+  const float* v_scale;   // [b,h,d] fp32 (kF8V kernels only)
 };
 
 enum Bar { kQFull = 0, kKFull = 1 /*3*/, kKEmpty = 4 /*3*/, kVFull = 7 /*3*/, kVEmpty = 10 /*3*/, kNumBars = 13 };
@@ -256,12 +257,14 @@ __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const fl
 
 // 128-row query blocks.  CTA = 2 consumer warpgroups + 1 TMA warp; warpgroup g owns query rows [64g, 64g+64) of the block.
 // kLse: the sparse branch alone for the training path (sla_attn_bwd.cu): store_o_lse instead of the KVW load and the linear branch.
-template <typename T, int HD, bool kQK16, bool kLse = false>
+// kF8V (INT8 Q/K, HD = 128): e4m3 P.V on the [b, h, d, lk_pad] codes of tdb200_sla_quant_v_fp8 (PvOps), unscaled by v_scale.
+template <typename T, int HD, bool kQK16, bool kLse = false, bool kF8V = false>
 __global__ void __launch_bounds__(kThreads, 1)
 sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                     const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw, AttnParams p,
                     const __grid_constant__ CUtensorMap tmap_q16, const __grid_constant__ CUtensorMap tmap_out) {
-  using L = Lay<HD, kQK16>;
+  using L = Lay<HD, kQK16, BLKQ, BLKK, kF8V>;
+  using PV = PvOps<T, HD, BLKK, kF8V>;
   constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // 1024-aligned, stays a shared-space pointer
@@ -337,9 +340,13 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
         mbar_wait(&bars[kVEmpty + st], ph);
         mbar_expect_tx(&bars[kVFull + st], L::kVBytes);
         uint8_t* sv = smem + L::kOffV + st * L::kVBytes;
+        if constexpr (kF8V) {
+          tma_load_4d(sv, &tmap_v, &bars[kVFull + st], blk * BLKK, 0, hh, b);
+        } else {
 #pragma unroll
-        for (int c = 0; c < HD / 64; ++c)
-          tma_load_4d(sv + c * (BLKK * 128), &tmap_v, &bars[kVFull + st], c * 64, hh, blk * BLKK, b);
+          for (int c = 0; c < HD / 64; ++c)
+            tma_load_4d(sv + c * (BLKK * 128), &tmap_v, &bars[kVFull + st], c * 64, hh, blk * BLKK, b);
+        }
       }
     }
     return;
@@ -366,49 +373,69 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   const uint32_t sq = sbase + L::kOffQ + wg * (64 * HD);
   ScoreAcc<kQK16> sacc[BLKK / 2];   // S_{j+1} in flight
   float s[BLKK / 2];                // S_j, then P_j
-  uint32_t pa[BLKK / 16][4];        // P_j, read by the P.V in flight
+  typename PV::Frag pa;             // P_j, read by the P.V in flight
+  typename PV::Acc pacc;            // kF8V: P_j.V_j alone, added to O once retired
   bool rescale[2];
   float alpha[2];
   mbar_wait(&bars[kQFull], 0);
-  mbar_wait(&bars[kKFull], 0);
-  score_issue<kQK16, HD, BLKK, kBF16>(sacc, sq, BLKQ * 128, sbase + L::kOffK);
-  wgmma_wait<0>();
-  // valid < 64 only in the ragged last key block
-  if constexpr (kQK16) {
-    score_finish<kQK16, BLKK>(sacc, s, qsc * s_ksc[0]);
-    warp_release(&bars[kKEmpty], lane);
-    softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, p.lk - int(s_lut[0]) * BLKK, cq, true);
+  if constexpr (kF8V) {
+    // e4m3 P.V gives each block's P.V an accumulator of its own (PvOps), and that beside O, S_{j+1} and P_j does not fit in
+    // this kernel's 168 registers: the steps of an entry run one after the other, as in the 64-row kernel.
+    for (int j = 0; j < T_blocks; ++j) {
+      const int st = j % kStages;
+      mbar_wait(&bars[kKFull + st], (j / kStages) & 1);
+      score_issue<kQK16, HD, BLKK, kBF16>(sacc, sq, BLKQ * 128, sbase + L::kOffK + st * L::kKBytes);
+      wgmma_wait<0>();
+      warp_release(&bars[kKEmpty + st], lane);
+      softmax_p_i8<BLKK>(sacc, s, qsc * s_ksc[j], m_used, l_part, rescale, alpha, p.lk - int(s_lut[j]) * BLKK, cq, j == 0);
+      rescale_o<HD>(o, rescale, alpha);
+      PV::pack(s, pa);
+      mbar_wait(&bars[kVFull + st], (j / kStages) & 1);
+      PV::step(o, pacc, pa, sbase + L::kOffV + st * L::kVBytes);
+      warp_release(&bars[kVEmpty + st], lane);
+    }
   } else {
-    warp_release(&bars[kKEmpty], lane);
-    softmax_p_i8<BLKK>(sacc, s, qsc * s_ksc[0], m_used, l_part, rescale, alpha, p.lk - int(s_lut[0]) * BLKK, cq, true);
-  }
-  for (int j = 0; j < T_blocks; ++j) {
-    const int st = j % kStages, st1 = (j + 1) % kStages;
-    const bool next = j + 1 < T_blocks;
-    if (next) {
-      mbar_wait(&bars[kKFull + st1], ((j + 1) / kStages) & 1);
-      score_issue<kQK16, HD, BLKK, kBF16>(sacc, sq, BLKQ * 128, sbase + L::kOffK + st1 * L::kKBytes);
-    }
-    rescale_o<HD>(o, rescale, alpha);
-    pack_p<T, BLKK>(s, pa);
-    mbar_wait(&bars[kVFull + st], (j / kStages) & 1);
-    pv_issue<HD, BLKK, kBF16>(o, pa, sbase + L::kOffV + st * L::kVBytes);
-    wgmma_wait<1>();                                    // S_{j+1} retired, P_j.V_j may still run
-    if (next) {
-      if constexpr (kQK16) {
-        score_finish<kQK16, BLKK>(sacc, s, qsc * s_ksc[j + 1]);
-        warp_release(&bars[kKEmpty + st1], lane);
-        softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, p.lk - int(s_lut[j + 1]) * BLKK, cq, false);
-      } else {
-        warp_release(&bars[kKEmpty + st1], lane);
-        softmax_p_i8<BLKK>(sacc, s, qsc * s_ksc[j + 1], m_used, l_part, rescale, alpha, p.lk - int(s_lut[j + 1]) * BLKK, cq,
-                           false);
-      }
-    }
+    mbar_wait(&bars[kKFull], 0);
+    score_issue<kQK16, HD, BLKK, kBF16>(sacc, sq, BLKQ * 128, sbase + L::kOffK);
     wgmma_wait<0>();
-    pv_fence<HD, BLKK>(o, pa);
-    warp_release(&bars[kVEmpty + st], lane);
+    // valid < 64 only in the ragged last key block
+    if constexpr (kQK16) {
+      score_finish<kQK16, BLKK>(sacc, s, qsc * s_ksc[0]);
+      warp_release(&bars[kKEmpty], lane);
+      softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, p.lk - int(s_lut[0]) * BLKK, cq, true);
+    } else {
+      warp_release(&bars[kKEmpty], lane);
+      softmax_p_i8<BLKK>(sacc, s, qsc * s_ksc[0], m_used, l_part, rescale, alpha, p.lk - int(s_lut[0]) * BLKK, cq, true);
+    }
+    for (int j = 0; j < T_blocks; ++j) {
+      const int st = j % kStages, st1 = (j + 1) % kStages;
+      const bool next = j + 1 < T_blocks;
+      if (next) {
+        mbar_wait(&bars[kKFull + st1], ((j + 1) / kStages) & 1);
+        score_issue<kQK16, HD, BLKK, kBF16>(sacc, sq, BLKQ * 128, sbase + L::kOffK + st1 * L::kKBytes);
+      }
+      rescale_o<HD>(o, rescale, alpha);
+      PV::pack(s, pa);
+      mbar_wait(&bars[kVFull + st], (j / kStages) & 1);
+      PV::issue(o, pacc, pa, sbase + L::kOffV + st * L::kVBytes);
+      wgmma_wait<1>();                                    // S_{j+1} retired, P_j.V_j may still run
+      if (next) {
+        if constexpr (kQK16) {
+          score_finish<kQK16, BLKK>(sacc, s, qsc * s_ksc[j + 1]);
+          warp_release(&bars[kKEmpty + st1], lane);
+          softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, p.lk - int(s_lut[j + 1]) * BLKK, cq, false);
+        } else {
+          warp_release(&bars[kKEmpty + st1], lane);
+          softmax_p_i8<BLKK>(sacc, s, qsc * s_ksc[j + 1], m_used, l_part, rescale, alpha, p.lk - int(s_lut[j + 1]) * BLKK, cq,
+                             false);
+        }
+      }
+      wgmma_wait<0>();
+      PV::fence(o, pacc, pa);
+      warp_release(&bars[kVEmpty + st], lane);
+    }
   }
+  if constexpr (kF8V) unscale_o_f8v<HD>(o, p.v_scale + int64_t(bh) * HD, cq);
   if constexpr (kLse) {
     store_o_lse<T, HD>(o, m_used, l_part, p, int64_t(m_blk) * BLKQ + r_lo, cq, b, hh, bh);
   } else if constexpr (kQK16) {
@@ -429,13 +456,14 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 //   of SLA/kernel.py:21-82); wgmma m64n64k16 into fp32.
 // After both loops warpgroup 1 hands its (m, l, O) to warpgroup 0, which merges the two states and then runs the linear
 // branch and the output (linear_branch_store), or with kLse stores o_s and the row lse.
-template <typename T, int HD, bool kQK16, int BK, bool kLse>
+template <typename T, int HD, bool kQK16, int BK, bool kLse, bool kF8V = false>
 __global__ void __launch_bounds__(split::kThreads, 1)
 sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                         const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw, AttnParams p,
                         const __grid_constant__ CUtensorMap tmap_q16, const __grid_constant__ CUtensorMap tmap_out) {
   constexpr int BQ = kBlkQ64;
-  using L = Lay<HD, kQK16, BQ, BK>;
+  using L = Lay<HD, kQK16, BQ, BK, kF8V>;
+  using PV = PvOps<T, HD, BK, kF8V>;
   // hand-off of warpgroup 1's state: HD/2 accumulator registers + m_used[2] + l_part[2] per thread, over the K and V rings
   static_assert((HD / 2 + 4) * 128 * 4 <= kStages * (L::kKBytes + L::kVBytes), "merge buffer does not fit in the ring");
   constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
@@ -506,8 +534,12 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
         mbar_wait(&bars[split::kVEmpty + st], ph);
         mbar_expect_tx(vfull, L::kVBytes);
         uint8_t* sv = smem + L::kOffV + st * L::kVBytes;
+        if constexpr (kF8V) {
+          tma_load_4d(sv, &tmap_v, vfull, blk * BK, 0, hh, b);
+        } else {
 #pragma unroll
-        for (int c = 0; c < HD / 64; ++c) tma_load_4d(sv + c * (BK * 128), &tmap_v, vfull, c * 64, hh, blk * BK, b);
+          for (int c = 0; c < HD / 64; ++c) tma_load_4d(sv + c * (BK * 128), &tmap_v, vfull, c * 64, hh, blk * BK, b);
+        }
       }
     }
     return;
@@ -535,7 +567,8 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
     const int valid = p.lk - blk * BK;                  // < BK only in the ragged last key block
 
     float s[BK / 2];
-    uint32_t pa[BK / 16][4];
+    typename PV::Frag pa;
+    typename PV::Acc pacc;
     mbar_wait(&bars[split::full(split::kKFull, j)], ph);
     if constexpr (kQK16) {
       score_tile<kQK16, HD, BK, kBF16>(s, sbase + L::kOffQ, BQ * 128, sbase + L::kOffK + st * L::kKBytes, sc);
@@ -550,10 +583,10 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
       float alpha[2];
       softmax_p_i8<BK>(si, s, sc, m_used, l_part, rescale, alpha, valid, cq, j == wg);
       rescale_o<HD>(o, rescale, alpha);
-      pack_p<T, BK>(s, pa);
+      PV::pack(s, pa);
     }
     mbar_wait(&bars[split::full(split::kVFull, j)], ph);
-    pv_step<HD, BK, kBF16>(o, pa, sbase + L::kOffV + st * L::kVBytes);
+    PV::step(o, pacc, pa, sbase + L::kOffV + st * L::kVBytes);
     warp_release(&bars[split::kVEmpty + st], lane);
   }
 
@@ -582,6 +615,7 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
     const int h = (i >> 1) & 1;
     o[i] = fmaf(o[i], a0[h], x[i] * a1[h]);
   }
+  if constexpr (kF8V) unscale_o_f8v<HD>(o, p.v_scale + int64_t(bh) * HD, cq);
   const int64_t qrow0 = int64_t(m_blk) * BQ + r_lo;
   if constexpr (kLse) {
     store_o_lse<T, HD>(o, m_used, l_part, p, qrow0, cq, b, hh, bh);
@@ -593,21 +627,29 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
   }
 }
 
-template <typename T, int HD, bool kQK16, int kBQ, int kBK, bool kLse>
+template <typename T, int HD, bool kQK16, int kBQ, int kBK, bool kLse, bool kF8V>
 constexpr auto attn_kernel() {
-  if constexpr (kBQ == kBlkQ64) return sla_attn_fwd_q64_kernel<T, HD, kQK16, kBK, kLse>;
-  else return sla_attn_fwd_kernel<T, HD, kQK16, kLse>;
+  if constexpr (kF8V) {
+    if constexpr (kBQ == kBlkQ64) return sla_attn_fwd_q64_kernel<T, HD, kQK16, kBK, kLse, true>;
+    else return sla_attn_fwd_kernel<T, HD, kQK16, kLse, true>;
+  } else {
+    if constexpr (kBQ == kBlkQ64) return sla_attn_fwd_q64_kernel<T, HD, kQK16, kBK, kLse>;
+    else return sla_attn_fwd_kernel<T, HD, kQK16, kLse>;
+  }
 }
 
 // kQK16: 16-bit Q and K in [b, l, h, d]; otherwise INT8 Q [b*h, l, d] and INT8 K [b, h, lk, d] (or [b, lk, h, d] when k_seq_major).
 // kBQ x kBK: the block geometry, 128 x 64 (sla_attn_fwd_kernel), or with sla_attn_fwd_q64_kernel 64 x 128 (INT8 Q/K only)
 // or 64 x 64 (16-bit Q/K only).
 // kLse (16-bit only): sparse branch and row log-sum-exp into `lse`; kvw, ksum and proj_b are not read.
-template <int HD, bool kQK16, int kBQ = BLKQ, int kBK = BLKK, bool kLse = false>
+// kF8V (INT8 only, HD = 128): v is tdb200_sla_quant_v_fp8's e4m3 [b, h, d, lk_pad] with lk_pad = ceil(lk / kBK) * kBK, and
+// v_scale its [b, h, d] channel scales.
+template <int HD, bool kQK16, int kBQ = BLKQ, int kBK = BLKK, bool kLse = false, bool kF8V = false>
 int launch(const void* q_op, const float* q_scale, const void* k_op, const float* k_scale, const void* v, const void* q, int dtype,
            const int32_t* lut, int64_t topk, const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
-           int64_t l, int64_t lk, int64_t h, float sm_scale, int feature, bool k_seq_major, void* stream, float* lse = nullptr) {
-  using L = Lay<HD, kQK16, kBQ, kBK>;
+           int64_t l, int64_t lk, int64_t h, float sm_scale, int feature, bool k_seq_major, void* stream, float* lse = nullptr,
+           const float* v_scale = nullptr) {
+  using L = Lay<HD, kQK16, kBQ, kBK, kF8V>;
   const int64_t d = HD;
   const int64_t mblk = cdiv64(l, kBQ), nblk = cdiv64(lk, kBK);
   if (topk <= 0 || topk > nblk) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd: topk=%lld outside [1, %lld]", (long long)topk, (long long)nblk);
@@ -645,7 +687,13 @@ int launch(const void* q_op, const float* q_scale, const void* k_op, const float
       if (int rc = make_tmap_4d(&tk, k_op, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, dims, str, box, sw8)) return rc;
     }
   }
-  {
+  if (kF8V) {   // [kBK keys x HD channels] boxes of the transposed codes, key-block rows of kBK bytes
+    const uint64_t lk_pad = uint64_t(nblk * kBK);
+    const uint64_t dims[4] = {lk_pad, uint64_t(d), uint64_t(h), uint64_t(b)};
+    const uint64_t str[3] = {lk_pad, uint64_t(d) * lk_pad, uint64_t(h * d) * lk_pad};
+    const uint32_t box[4] = {uint32_t(kBK), uint32_t(HD), 1, 1};
+    if (int rc = make_tmap_4d(&tv, v, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, dims, str, box, kBK)) return rc;
+  } else {
     const uint64_t dims[4] = {uint64_t(d), uint64_t(h), uint64_t(lk), uint64_t(b)};
     const uint64_t str[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(lk * h * d * 2)};
     const uint32_t box[4] = {64, 1, kBK, 1};
@@ -685,12 +733,13 @@ int launch(const void* q_op, const float* q_scale, const void* k_op, const float
   p.feature = feature;
   p.sm_scale = sm_scale;
   p.lse = lse;
+  p.v_scale = v_scale;
   dim3 grid(static_cast<unsigned>(mblk), static_cast<unsigned>(h), static_cast<unsigned>(b));
   const int threads = kBQ == kBlkQ64 ? split::kThreads : kThreads;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define TDB_ATTN(T)                                                                                                   \
   do {                                                                                                                \
-    const auto kern = attn_kernel<T, HD, kQK16, kBQ, kBK, kLse>();                                                               \
+    const auto kern = attn_kernel<T, HD, kQK16, kBQ, kBK, kLse, kF8V>();                                                        \
     if (int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), \
                             "cudaFuncSetAttribute(sla_attn)"))                                                        \
       return rc;                                                                                                      \
@@ -807,4 +856,34 @@ extern "C" int tdb200_sla_attn_fwd_qk16_lse(const void* q, const void* k, const 
                                             void* o_s, float* lse, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale,
                                             void* stream) {
   return tdb200_sla_attn16_fwd_lse(q, k, v, dtype, lut, topk, o_s, lse, b, l, h, d, sm_scale, BLKQ, BLKK, stream);
+}
+
+// tdb200_sla_attn_fwd with e4m3 P.V: v_fp8 / v_scale from tdb200_sla_quant_v_fp8 with the same blkk.  Its kernels are instantiated
+// here, after every 16-bit-V kernel of this file, so that those compile as they did without them.
+extern "C" int tdb200_sla_attn_fwd_fp8v(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
+                                        const uint8_t* v_fp8, const float* v_scale, const void* q, int dtype, const int32_t* lut,
+                                        int64_t topk, const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
+                                        int64_t l, int64_t lk, int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq,
+                                        int64_t blkk, int k_seq_major, void* stream) {
+  const bool hopper = blkq == kBlkQ64 && blkk == kHopperBlkK;
+  if (!hopper && !(blkq == BLKQ && blkk == BLKK))
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_fp8v: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 128)",
+                (long long)blkq, (long long)blkk);
+  if (int rc = check_common(q_i8, k_i8, v_fp8, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
+  if (!q_scale || !k_scale || !v_scale) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd_fp8v: null pointer");
+  if (!aligned16(v_fp8) || !aligned16(v_scale))
+    return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd_fp8v: v_fp8 and v_scale must be 16-byte aligned");
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_fp8v: head dim %lld (FP8 P.V is implemented for d=128)", (long long)d);
+  if (feature < 0 || feature > 2) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd_fp8v: feature map tag %d", feature);
+  if (k_seq_major && feature != 0)
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_fp8v: feature map tag %d (sequence-major K is implemented for softmax)", feature);
+  if (k_seq_major && b != 1)
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_fp8v: batch %lld (the gathered [lk_pad, h, d] key slab is one sequence)",
+                (long long)b);
+  if (!hopper)
+    return launch<128, false, BLKQ, BLKK, false, true>(q_i8, q_scale, k_i8, k_scale, v_fp8, q, dtype, lut, topk, kvw, ksum, proj_b,
+                                                       out, b, l, lk, h, sm_scale, feature, k_seq_major != 0, stream, nullptr, v_scale);
+  return launch<128, false, kBlkQ64, kHopperBlkK, false, true>(q_i8, q_scale, k_i8, k_scale, v_fp8, q, dtype, lut, topk, kvw, ksum,
+                                                               proj_b, out, b, l, lk, h, sm_scale, feature, k_seq_major != 0, stream,
+                                                               nullptr, v_scale);
 }

@@ -240,6 +240,89 @@ __device__ __forceinline__ void pv_step(float (&o)[HD / 2], uint32_t (&pa)[BK / 
   pv_fence<HD, BK>(o, pa);
 }
 
+// ---- P.V with e4m3 P and V (the SageSLA kernels' FP8 option, tdb200_sla_attn_fwd_fp8v).  V arrives as codes of V / v_scale
+//      in tiles of [HD channels x BK keys], K-major (the only B layout e4m3 wgmma takes), rows of BK bytes in the 128-byte
+//      (BK = 128) or 64-byte (BK = 64) swizzle.  The A fragment of one K = 32 step holds, per row, the 4-byte groups k 4 (l%4)
+//      + {0..3} (a[0], a[1]: rows l/4, l/4 + 8) and 16 + 4 (l%4) + {0..3} (a[2], a[3]); the score accumulator holds keys
+//      8 c + 2 (l%4) + {0, 1}.  tdb200_sla_quant_v_fp8 stores the keys of every 32-key group in the order that makes the two
+//      agree (position 16 u + 4 t + j holds key 16 u + 8 (j >> 1) + 2 t + (j & 1)), so P packs into the fragment in registers
+//      without any exchange between lanes.
+// P is rounded to e4m3 times kF8PScale: p <= 2^8 under the lazy rescale, and 2^0 is the largest power of two that keeps
+// 2^8 s <= 448 (e4m3's largest finite value); a larger one would saturate the p in (224, 256], a smaller one would only push
+// more small p below e4m3's smallest normal, 2^-6.
+constexpr float kF8PScale = 1.0f;
+
+// The P.V step of one key block, for 16-bit P and V (kF8V = false: pack_p / pv_issue / pv_fence, straight into O) or e4m3 P
+// and V.  issue starts the block's P.V, fence (once it has retired) leaves O holding it; Acc is the block's own accumulator.
+template <typename T, int HD, int BK, bool kF8V>
+struct PvOps {
+  static constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
+  static constexpr int kSteps = BK / 16;   // A fragments: one per K = 16 step
+  using Frag = uint32_t[kSteps][4];
+  struct Acc {};
+  static __device__ __forceinline__ void pack(const float (&p)[BK / 2], Frag& pa) { pack_p<T, BK>(p, pa); }
+  static __device__ __forceinline__ void issue(float (&o)[HD / 2], Acc&, Frag& pa, uint32_t sv) { pv_issue<HD, BK, kBF16>(o, pa, sv); }
+  static __device__ __forceinline__ void fence(float (&o)[HD / 2], Acc&, Frag& pa) { pv_fence<HD, BK>(o, pa); }
+  static __device__ __forceinline__ void step(float (&o)[HD / 2], Acc&, Frag& pa, uint32_t sv) { pv_step<HD, BK, kBF16>(o, pa, sv); }
+};
+template <typename T, int HD, int BK>
+struct PvOps<T, HD, BK, true> {
+  static_assert(HD == 128 && (BK == 64 || BK == 128), "e4m3 P.V: 128 channels, 64- or 128-key blocks");
+  static constexpr int kSteps = BK / 32;   // one per K = 32 step
+  using Frag = uint32_t[kSteps][4];
+  // The e4m3 wgmma accumulates at less than fp32 precision, so over a whole key list O would lose the small terms of every
+  // block (the rel-L2 error grew with the list: 5-12 % against float64 at 50-120 blocks).  Each block's P.V therefore
+  // starts a fresh accumulator of BK / 32 MMAs, added to O in fp32 once it has retired (SageAttention2's two-level
+  // accumulation).
+  using Acc = float[HD / 2];
+  static __device__ __forceinline__ void pack(const float (&p)[BK / 2], Frag& pa) {
+#pragma unroll
+    for (int kk = 0; kk < kSteps; ++kk)
+#pragma unroll
+      for (int u = 0; u < 2; ++u)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int i = 4 * (4 * kk + 2 * u) + 2 * h;   // accumulator slices 4 kk + 2 u and + 1, row half h
+          pa[kk][2 * u + h] = pack4_e4m3(p[i] * kF8PScale, p[i + 1] * kF8PScale, p[i + 4] * kF8PScale, p[i + 5] * kF8PScale);
+        }
+  }
+  static __device__ __forceinline__ void issue(float (&)[HD / 2], Acc& acc, Frag& pa, uint32_t sv) {
+    const uint64_t vdesc = BK == 128 ? make_desc_kmajor_sw128(sv) : make_desc_kmajor_sw64(sv);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kSteps; ++kk)   // +32 bytes per K step; the first one overwrites acc
+      wgmma_e4m3_rs<HD>(acc, pa[kk], vdesc + uint64_t(kk * 2), kk > 0 ? 1u : 0u);
+    wgmma_commit();
+  }
+  static __device__ __forceinline__ void fence(float (&o)[HD / 2], Acc& acc, Frag& pa) {
+    reg_fence(acc);
+#pragma unroll
+    for (int kk = 0; kk < kSteps; ++kk) reg_fence(pa[kk]);
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) o[i] += acc[i];
+  }
+  static __device__ __forceinline__ void step(float (&o)[HD / 2], Acc& acc, Frag& pa, uint32_t sv) {
+    issue(o, acc, pa, sv);
+    wgmma_wait<0>();
+    fence(o, acc, pa);
+  }
+};
+
+// After the last e4m3 P.V: O = sum e4m3(p kF8PScale) e4m3(v / v_scale) back in the units of P.V, column by column
+// (v_scale: this head's [HD] channel scales).
+template <int HD>
+__device__ __forceinline__ void unscale_o_f8v(float (&o)[HD / 2], const float* v_scale, int cq) {
+#pragma unroll
+  for (int c = 0; c < HD / 8; ++c) {
+    const float2 s = __ldg(reinterpret_cast<const float2*>(v_scale + 8 * c + cq));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      o[4 * c + 2 * h] *= s.x * (1.0f / kF8PScale);
+      o[4 * c + 2 * h + 1] *= s.y * (1.0f / kF8PScale);
+    }
+  }
+}
+
 // columns 8 c + cq + {0, 1} of one output row = T(O / l), from row half h (rows r and r + 8) of this thread's O fragment
 template <typename T, int HD>
 __device__ __forceinline__ void store_o_row(T* orow, const float (&o)[HD / 2], int h, float inv_l, int cq) {

@@ -307,3 +307,119 @@ extern "C" int tdb200_sla_quant_k_seq(const void* k, const float* kmean, int dty
 #undef TDB_RUN
   return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_k_seq: dtype tag %d", dtype);
 }
+
+// ---- e4m3 V for the SageSLA kernels' FP8 P.V (tdb200_sla_attn_fwd_fp8v) ----------------------------------------------------
+// Two passes over v [b, l, h, d]: the per-channel amax over all l rows (order-independent, so the scales are reproducible),
+// then codes of v / v_scale, transposed to [b, h, d, l_pad] with each 32-key group in the order the attention kernel's e4m3
+// A fragment needs (sla_attn.cuh, PvOps): the permutation costs nothing here, since this pass gathers every output byte from a
+// staged tile anyway, and saves the kernel a byte exchange between lanes for every P.V.
+namespace {
+constexpr int kVAmaxRows = 256;             // rows per CTA of the amax pass
+constexpr float kE4m3Max = 448.0f;
+constexpr float kVAmaxFloor = 0x1p-64f;     // an all-zero channel gets a finite, normal scale (and zero codes)
+
+// amax[b, h, d] (fp32 bits, non-negative, so integer max is float max) over rows [kVAmaxRows * blockIdx.x, +kVAmaxRows)
+template <typename T>
+__global__ void __launch_bounds__(256) v_amax_kernel(const T* __restrict__ v, unsigned int* __restrict__ amax, int64_t l, int hd) {
+  const int b = blockIdx.y;
+  const int64_t row0 = int64_t(blockIdx.x) * kVAmaxRows;
+  const int rows = l - row0 < kVAmaxRows ? static_cast<int>(l - row0) : kVAmaxRows;
+  for (int cv = threadIdx.x; cv < hd / 8; cv += 256) {
+    uint32_t m[4] = {0u, 0u, 0u, 0u};
+    const T* src = v + (int64_t(b) * l + row0) * hd + cv * 8;
+#pragma unroll 8
+    for (int r = 0; r < rows; ++r) {
+      const uint4 raw = ldg_nc_v4(src + int64_t(r) * hd);
+      m[0] = F16Traits<T>::absmax2(m[0], raw.x);
+      m[1] = F16Traits<T>::absmax2(m[1], raw.y);
+      m[2] = F16Traits<T>::absmax2(m[2], raw.z);
+      m[3] = F16Traits<T>::absmax2(m[3], raw.w);
+    }
+    unsigned int* dst = amax + int64_t(b) * hd + cv * 8;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      atomicMax(dst + 2 * j, __float_as_uint(F16Traits<T>::lo(m[j])));
+      atomicMax(dst + 2 * j + 1, __float_as_uint(F16Traits<T>::hi(m[j])));
+    }
+  }
+}
+
+// in place: amax -> v_scale = max(amax, floor) / 448
+__global__ void v_scale_kernel(float* __restrict__ scale, int64_t n) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i < n) scale[i] = __fdiv_rn(fmaxf(scale[i], kVAmaxFloor), kE4m3Max);
+}
+
+// one [BK keys x 128 channels] tile of one (b, h): rows >= l are zero.  Position 16 u + 4 t + j of every 32-key group holds key
+// 16 u + 8 (j >> 1) + 2 t + (j & 1).
+template <typename T, int BK>
+__global__ void __launch_bounds__(256) v_quant_fp8_kernel(const T* __restrict__ v, const float* __restrict__ scale,
+                                                          uint8_t* __restrict__ v_fp8, int64_t l, int h, int64_t l_pad) {
+  constexpr int D = 128;
+  __shared__ __align__(16) uint16_t tile[BK][D];
+  const int blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
+  for (int c = threadIdx.x; c < BK * D / 8; c += 256) {   // 16 chunks of 16 bytes per key row
+    const int r = c / (D / 8), cc = c % (D / 8);
+    const int64_t row = int64_t(blk) * BK + r;
+    uint4 raw = make_uint4(0u, 0u, 0u, 0u);
+    if (row < l) raw = ldg_nc_v4(v + ((int64_t(b) * l + row) * h + hh) * D + cc * 8);
+    *reinterpret_cast<uint4*>(&tile[r][cc * 8]) = raw;
+  }
+  __syncthreads();
+  const int dch = threadIdx.x & (D - 1);                   // a warp reads 32 channels of one key row: no bank conflict
+  const float s = __ldg(scale + (int64_t(b) * h + hh) * D + dch);
+  uint8_t* dst = v_fp8 + ((int64_t(b) * h + hh) * D + dch) * l_pad + int64_t(blk) * BK;
+  for (int g = threadIdx.x >> 7; g < BK / 16; g += 2) {     // 16 output positions per store
+    float x[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int pos = 16 * g + i;
+      const int key = (pos & ~15) | (((pos >> 1) & 1) << 3) | (((pos >> 2) & 3) << 1) | (pos & 1);
+      uint16_t bits = tile[key][dch];
+      x[i] = __fdiv_rn(F16Traits<T>::lo(bits), s);
+    }
+    uint4 out;
+    out.x = pack4_e4m3(x[0], x[1], x[2], x[3]);
+    out.y = pack4_e4m3(x[4], x[5], x[6], x[7]);
+    out.z = pack4_e4m3(x[8], x[9], x[10], x[11]);
+    out.w = pack4_e4m3(x[12], x[13], x[14], x[15]);
+    *reinterpret_cast<uint4*>(dst + 16 * g) = out;
+  }
+}
+
+template <typename T>
+int run_quant_v_fp8(const void* v, int64_t b, int64_t l, int64_t h, int64_t blkk, uint8_t* v_fp8, float* v_scale, cudaStream_t st) {
+  const int64_t nblk = cdiv64(l, blkk), n = b * h * 128;
+  if (int rc = check_cuda(cudaMemsetAsync(v_scale, 0, size_t(n) * 4, st), "cudaMemsetAsync(v_scale)")) return rc;
+  v_amax_kernel<T><<<dim3(static_cast<unsigned>(cdiv64(l, kVAmaxRows)), static_cast<unsigned>(b)), 256, 0, st>>>(
+      static_cast<const T*>(v), reinterpret_cast<unsigned int*>(v_scale), l, static_cast<int>(h * 128));
+  if (int rc = check_launch("v_amax_kernel")) return rc;
+  v_scale_kernel<<<static_cast<unsigned>(cdiv64(n, 256)), 256, 0, st>>>(v_scale, n);
+  if (int rc = check_launch("v_scale_kernel")) return rc;
+  const dim3 grid(static_cast<unsigned>(nblk), static_cast<unsigned>(h), static_cast<unsigned>(b));
+  if (blkk == 128)
+    v_quant_fp8_kernel<T, 128><<<grid, 256, 0, st>>>(static_cast<const T*>(v), v_scale, v_fp8, l, static_cast<int>(h), nblk * 128);
+  else
+    v_quant_fp8_kernel<T, 64><<<grid, 256, 0, st>>>(static_cast<const T*>(v), v_scale, v_fp8, l, static_cast<int>(h), nblk * 64);
+  return check_launch("v_quant_fp8_kernel");
+}
+}  // namespace
+
+extern "C" int tdb200_sla_quant_v_fp8(const void* v, int dtype, int64_t b, int64_t l, int64_t h, int64_t d, int64_t blkk,
+                                      uint8_t* v_fp8, float* v_scale, void* stream) {
+  using namespace tdb;
+  if (blkk != 64 && blkk != 128)
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_v_fp8: key block size %lld (BLKK = 64 or 128)", (long long)blkk);
+  if (!v || !v_fp8 || !v_scale) return fail(TDB200_ERR_INVALID_ARG, "sla_quant_v_fp8: null pointer");
+  if (b <= 0 || l <= 0 || h <= 0 || d <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_quant_v_fp8: bad shape");
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_v_fp8: head dim %lld (FP8 P.V is implemented for d=128)", (long long)d);
+  if (dtype != TDB200_DTYPE_BF16 && dtype != TDB200_DTYPE_FP16) return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_v_fp8: dtype tag %d", dtype);
+  if (h > 65535 || b > 65535 || cdiv64(l, blkk) > 0x7FFFFFFF || int64_t(1) * l * h * d * 2 >= (int64_t(1) << 40))
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_v_fp8: dimension too large (b, h <= 65535; l * h * d below 2^39)");
+  if (!aligned16(v) || !aligned16(v_fp8) || !aligned16(v_scale))
+    return fail(TDB200_ERR_INVALID_ARG, "sla_quant_v_fp8: buffers must be 16-byte aligned");
+  if (int rc = require_sm90()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (dtype == TDB200_DTYPE_BF16) return run_quant_v_fp8<__nv_bfloat16>(v, b, l, h, blkk, v_fp8, v_scale, st);
+  return run_quant_v_fp8<__half>(v, b, l, h, blkk, v_fp8, v_scale, st);
+}

@@ -55,7 +55,11 @@ def sage_blocks(sage_arch: str):
 
 def require_served_arch(sage_arch: str) -> None:
     """Refuse, at install and at every hook call, to run `sage_arch`'s block sizes while a single GPU would run the other
-    family's (SLA.utils.set_served_arch)."""
+    family's (SLA.utils.set_served_arch), and to run at all while SageSLA's P.V is FP8 (SLA.utils.set_sage_pv): the hooks
+    serve the 16-bit P.V only, so the ranks would compute other arithmetic than a single GPU."""
+    if sla_utils.SAGE_PV != "bf16":
+        raise NotImplementedError(f"sequence parallelism runs SageSLA with 16-bit P.V; SLA.utils.set_sage_pv is "
+                                  f"{sla_utils.SAGE_PV!r}, and a single GPU would compute with FP8 P.V: select 'bf16'")
     served = sla_utils.SERVED_ARCH
     if served != sage_arch:
         bq, bk = sla_utils.SAGE_BLOCKS[sage_arch]

@@ -1,13 +1,23 @@
 """Closed-form backward of the block-sparse softmax attention (oracle/td_oracle.py `sparse_attention`), in float64: the
 reference for the SparseLinearAttention backward kernels (csrc/sla_attn_bwd.cu).  FlashAttention-2's formulation with the
 row statistics of the forward: lse (log2 units) and delta = rowsum(dO * O).  Test infrastructure only.  Tensors are
-[B, H, L, D] like td_oracle.sparse_attention; lut [B, H, Mblk, topk] key-block ids."""
+[B, H, L, D] like td_oracle.sparse_attention; lut [B, H, Mblk, topk] key-block ids.
+
+The second half holds what the 16-bit GPU tests share, on the module layout [B, L, H, D] and on whatever device the tensors
+live: the large-score and entry-split input builders, the long-list inputs, and the closed-form dQ / dK / dV of one block
+given float64 (or any) lse and delta."""
 from __future__ import annotations
 
 import math
 from typing import Optional, Tuple
 
 import torch
+
+D, BK = 128, 64
+SM = D ** -0.5
+LOG2E = 1.0 / math.log(2.0)
+F64 = torch.float64
+U = torch.ones(D) / D ** 0.5                      # the direction the magnitude ramps of the input builders live on
 
 
 def cdiv(a: int, b: int) -> int:
@@ -76,3 +86,115 @@ def sparse_attention_bwd_dkdv(q, k, v, d_o, lut, lse, delta, bi: int, hi: int, n
         dv += times * (p.t() @ gb)
         dk += times * sm_scale * (ds.t() @ qb)
     return dk, dv
+
+
+# ------------------------------------------------------------------------------------------------------------ [B, L, H, D]
+def block_mask(lut, nblk):
+    """[B,H,Mblk,topk] LUT -> bool [B,H,Mblk,Nblk].  Every LUT here lists a key block at most once per row."""
+    b, h, m, _ = lut.shape
+    return torch.zeros(b, h, m, nblk, dtype=torch.bool, device=lut.device).scatter_(-1, lut.long(), True)
+
+
+def ref_dq(q, k, v, d_o, bm, blkq, ref, b, hi, mi, sm_scale=SM):
+    """Closed-form float64 dQ of query block mi (its valid rows), given ref["lse"] and ref["delta"] [B,H,L]."""
+    l = q.shape[1]
+    r0, r1 = mi * blkq, min(l, (mi + 1) * blkq)
+    cols = bm[b, hi, mi][torch.arange(k.shape[1], device=q.device) // BK].nonzero().squeeze(-1)
+    kc, vc = k[b, cols, hi].to(F64), v[b, cols, hi].to(F64)
+    s = (q[b, r0:r1, hi].to(F64) @ kc.t()) * (sm_scale * LOG2E)
+    p = torch.exp2(s - ref["lse"][b, hi, r0:r1, None].to(F64))
+    ds = p * (d_o[b, r0:r1, hi].to(F64) @ vc.t() - ref["delta"][b, hi, r0:r1, None].to(F64))
+    return sm_scale * ds @ kc
+
+
+def ref_dkdv(q, k, v, d_o, bm, blkq, ref, b, hi, ni, sm_scale=SM):
+    """Closed-form float64 (dK, dV) of key block ni (its valid rows): the sum over every query row whose block selects it."""
+    l = q.shape[1]
+    c0, c1 = ni * BK, min(k.shape[1], (ni + 1) * BK)
+    rows = bm[b, hi, :, ni][torch.arange(l, device=q.device) // blkq].nonzero().squeeze(-1)
+    qr, gr = q[b, rows, hi].to(F64), d_o[b, rows, hi].to(F64)
+    kc, vc = k[b, c0:c1, hi].to(F64), v[b, c0:c1, hi].to(F64)
+    p = torch.exp2((qr @ kc.t()) * (sm_scale * LOG2E) - ref["lse"][b, hi, rows, None].to(F64))
+    ds = p * (gr @ vc.t() - ref["delta"][b, hi, rows, None].to(F64))
+    return sm_scale * ds.t() @ qr, p.t() @ gr
+
+
+# Large-score patterns.  The q-scaling ones are the INT8 lazy-rescale tests' (test_gpu_sla.py): pattern, q scale, L, ratio.
+#   all          every row scaled: log2-domain scores spread over tens of units, running maxima jump by more than 8
+#   half_warp    rows r with r % 16 < 8: one of the two rows each thread of a 16-row warp slice holds
+#   one_warp     the first 16 rows of every query block: one warp (of warpgroup 0 on 128-row blocks)
+#   ragged_last  the maximum of many rows sits in the ragged last key block
+# Entry-split patterns (hand-made LUTs; on 64-row blocks warpgroup g takes the entries j = g mod 2).  Every LUT row lists
+# pairs (2i, 2i + 1) of key blocks in ascending order, so odd LUT positions always hold odd key blocks, and a magnitude ramp
+# on K per key block places the scores:
+#   split_dominant  odd blocks 140 + 12 i above the even ones: the row maximum lies in warpgroup 1's entries, more than 128
+#                   log2 units above all warpgroup 0 sees (exp2 of the difference taken the wrong way round overflows fp32)
+#   split_merge     even blocks at 10 i, odd ones at 10 i + 14, times a per-row factor in [1, 4]: both warpgroups rescale,
+#                   and warpgroup 1 ends about 14 to 56 units above warpgroup 0, so both states enter the merge
+SCALED = {"all_x8": ("all", 8.0, 1280, 0.5), "all_x16": ("all", 16.0, 700, 1.0), "half_warp": ("half_warp", 16.0, 640, 1.0),
+          "one_warp": ("one_warp", 16.0, 640, 1.0), "ragged_last": ("ragged_last", 12.0, 1000, 1.0)}
+SPLIT = ("split_dominant", "split_merge")
+
+
+def randn_qkv(l, h, seed):
+    g = torch.Generator().manual_seed(seed)
+    return [torch.randn(1, l, h, D, generator=g) for _ in range(3)]
+
+
+def scaled_case(name, blkq, h=2, seed=0):
+    """(q, k, v [1, L, H, D] float32 on the CPU, the module's top-k ratio) of a SCALED pattern."""
+    pattern, qscale, l, ratio = SCALED[name]
+    q, k, v = randn_qkv(l, h, 4000 + l + seed)
+    rows = torch.arange(l)
+    if pattern in ("all", "ragged_last"):
+        q = q * qscale
+    elif pattern == "half_warp":
+        q[:, (rows % 16) < 8] *= qscale
+    elif pattern == "one_warp":
+        q[:, (rows % blkq) < 16] *= qscale
+    if pattern == "ragged_last":
+        q = q + 2.0 * qscale * U
+        k[:, -(l % BK):] += 6.0 * U
+    return q, k, v, ratio
+
+
+def pair_lut(h, mblk, npairs, keep, seed):
+    """[1,h,mblk,2*keep] int32: per row `keep` of the `npairs` pairs (2i, 2i+1), ascending."""
+    g = torch.Generator().manual_seed(seed)
+    lut = torch.empty(1, h, mblk, 2 * keep, dtype=torch.int32)
+    for hi in range(h):
+        for mi in range(mblk):
+            pairs = torch.randperm(npairs, generator=g)[:keep].sort().values
+            lut[0, hi, mi] = torch.stack([2 * pairs, 2 * pairs + 1], -1).flatten()
+    return lut
+
+
+def split_case(name, blkq, h=2, seed=0):
+    """(q, k, v [1, L, H, D] float32 on the CPU, lut) of a SPLIT pattern.  L = 1240: 20 key blocks (the last one 24 keys, odd:
+    in warpgroup 1's entries), ragged last query block."""
+    l, a = 1240, 4.0
+    q, k, v = randn_qkv(l, h, 7000 + seed)
+    q = q - (q @ U)[..., None] * U                           # q orthogonal to U, then a chosen component along it
+    g = torch.Generator().manual_seed(8000 + seed)
+    alpha = torch.ones(1, l, h, 1) if name == "split_dominant" else 1.0 + 3.0 * torch.rand(1, l, h, 1, generator=g)
+    q = q + a * alpha * U
+    n = torch.arange(cdiv(l, BK))
+    if name == "split_dominant":
+        offset = torch.where(n % 2 == 1, 140.0 + 12.0 * (n // 2), torch.zeros(()))
+    else:
+        offset = 10.0 * (n // 2) + 14.0 * (n % 2)
+    c = (offset / (a * SM * LOG2E)).repeat_interleave(BK)[:l]    # score offset of key block n = alpha * offset[n]
+    k = k + c[None, :, None, None] * U
+    return q, k, v, pair_lut(h, cdiv(l, blkq), 10, 7, 9000 + seed + blkq)
+
+
+def long_inputs(l, h, dtype, seed):
+    """randn q, k, v on the GPU plus a ramp of 6 log2 units over the key blocks (later blocks weigh up to 64x more), so that
+    every part of a long LUT row, its last entries included, carries a visible share of each row's softmax mass."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    q, k, v = (torch.randn(1, l, h, D, generator=g, device="cuda") for _ in range(3))
+    a, u = 4.0, U.cuda()
+    q = q - (q @ u)[..., None] * u + a * u
+    ramp = 6.0 * (torch.arange(l, device="cuda") // BK) / (cdiv(l, BK) - 1)
+    k = k + (ramp / (a * SM * LOG2E))[None, :, None, None] * u
+    return [t.to(dtype) for t in (q, k, v)]

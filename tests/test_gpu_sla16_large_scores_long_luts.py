@@ -22,12 +22,13 @@ import torch.nn.functional as F
 
 from oracle import td_oracle as O
 
+import sla_backward_oracle as B
+
 pytestmark = pytest.mark.gpu
 D, BK = 128, 64
 LOG2E, LN2 = 1.0 / math.log(2.0), math.log(2.0)
 F64 = torch.float64
 SM = D ** -0.5
-U = torch.ones(D) / D ** 0.5                      # the direction the magnitude ramps below live on
 BF16, FP16 = torch.bfloat16, torch.float16
 DTYPES = [pytest.param(BF16, id="bf16"), pytest.param(FP16, id="fp16")]
 
@@ -49,12 +50,6 @@ def _bars(got, want, cos, rel, what):
     return s
 
 
-def _block_mask(lut, nblk):
-    """[B,H,Mblk,topk] LUT -> bool [B,H,Mblk,Nblk].  Every LUT here lists a key block at most once per row."""
-    b, h, m, _ = lut.shape
-    return torch.zeros(b, h, m, nblk, dtype=torch.bool, device=lut.device).scatter_(-1, lut.long(), True)
-
-
 def _ref_forward(q, k, v, lut, blkq, sm_scale=SM, d_o=None, entry_max=False):
     """Float64 block-sparse attention of q, k, v [B,L,H,D] (on the GPU) over `lut`, in query chunks.  Returns a dict:
     o [B,L,H,D]; lse and smax [B,H,L] in log2 units (smax = max |s| over the row's selected scores); delta [B,H,L] =
@@ -62,7 +57,7 @@ def _ref_forward(q, k, v, lut, blkq, sm_scale=SM, d_o=None, entry_max=False):
     block, in LUT order."""
     b, l, h, d = q.shape
     nblk = _cdiv(l, BK)
-    bm = _block_mask(lut, nblk)
+    bm = B.block_mask(lut, nblk)
     dev = q.device
     colblk = torch.arange(l, device=dev) // BK
     out = {"o": torch.empty(b, l, h, d, dtype=F64, device=dev)}
@@ -96,7 +91,7 @@ def _sparse_attention(q, k, v, lut, blkq, sm_scale=SM, p_dtype=None):
     """Differentiable block-sparse attention of [B,L,H,D] tensors over `lut` (one masked dense softmax; short sequences
     only).  p_dtype: P rounded to that type before P.V, the row sum taken from the unrounded P."""
     l = q.shape[1]
-    sel = _block_mask(lut, _cdiv(l, BK))[:, :, torch.arange(l, device=q.device) // blkq][..., torch.arange(l, device=q.device) // BK]
+    sel = B.block_mask(lut, _cdiv(l, BK))[:, :, torch.arange(l, device=q.device) // blkq][..., torch.arange(l, device=q.device) // BK]
     qh, kh, vh = (t.transpose(1, 2) for t in (q, k, v))
     s = ((qh @ kh.transpose(-1, -2)) * sm_scale).masked_fill(~sel, -math.inf)
     e = torch.exp(s - s.amax(-1, keepdim=True).detach())
@@ -130,30 +125,6 @@ def _ref_grads(q, k, v, d_o, lut, blkq, sm_scale=SM, w=None, bias=None, rdtype=N
         o = o + _linear_branch(*leaves, rdtype=rdtype)
     (o * d_o.to(ct)).sum().backward()
     return [t.grad for t in leaves]
-
-
-def _ref_dq(q, k, v, d_o, bm, blkq, ref, b, hi, mi, sm_scale=SM):
-    """Closed-form float64 dQ of query block mi (its valid rows), given float64 lse and delta."""
-    l = q.shape[1]
-    r0, r1 = mi * blkq, min(l, (mi + 1) * blkq)
-    cols = bm[b, hi, mi][torch.arange(l, device=q.device) // BK].nonzero().squeeze(-1)
-    kc, vc = k[b, cols, hi].to(F64), v[b, cols, hi].to(F64)
-    s = (q[b, r0:r1, hi].to(F64) @ kc.t()) * (sm_scale * LOG2E)
-    p = torch.exp2(s - ref["lse"][b, hi, r0:r1, None])
-    ds = p * (d_o[b, r0:r1, hi].to(F64) @ vc.t() - ref["delta"][b, hi, r0:r1, None])
-    return sm_scale * ds @ kc
-
-
-def _ref_dkdv(q, k, v, d_o, bm, blkq, ref, b, hi, ni, sm_scale=SM):
-    """Closed-form float64 (dK, dV) of key block ni (its valid rows): the sum over every query row whose block selects it."""
-    l = q.shape[1]
-    c0, c1 = ni * BK, min(l, (ni + 1) * BK)
-    rows = bm[b, hi, :, ni][torch.arange(l, device=q.device) // blkq].nonzero().squeeze(-1)
-    qr, gr = q[b, rows, hi].to(F64), d_o[b, rows, hi].to(F64)
-    kc, vc = k[b, c0:c1, hi].to(F64), v[b, c0:c1, hi].to(F64)
-    p = torch.exp2((qr @ kc.t()) * (sm_scale * LOG2E) - ref["lse"][b, hi, rows, None])
-    ds = p * (gr @ vc.t() - ref["delta"][b, hi, rows, None])
-    return sm_scale * ds.t() @ qr, p.t() @ gr
 
 
 def _check_lse(lse, ref, what):
@@ -191,72 +162,9 @@ def _rescale_fraction(emax, blkq):
 
 
 # ------------------------------------------------------------------------------------------------------------ inputs
-# Large-score patterns.  The q-scaling ones are the INT8 lazy-rescale tests' (test_gpu_sla.py): pattern, q scale, L, ratio.
-#   all          every row scaled: log2-domain scores spread over tens of units, running maxima jump by more than 8
-#   half_warp    rows r with r % 16 < 8: one of the two rows each thread of a 16-row warp slice holds
-#   one_warp     the first 16 rows of every query block: one warp (of warpgroup 0 on 128-row blocks)
-#   ragged_last  the maximum of many rows sits in the ragged last key block
-# Entry-split patterns (hand-made LUTs; on 64-row blocks warpgroup g takes the entries j = g mod 2).  Every LUT row lists
-# pairs (2i, 2i + 1) of key blocks in ascending order, so odd LUT positions always hold odd key blocks, and a magnitude ramp
-# on K per key block places the scores:
-#   split_dominant  odd blocks 140 + 12 i above the even ones: the row maximum lies in warpgroup 1's entries, more than 128
-#                   log2 units above all warpgroup 0 sees (exp2 of the difference taken the wrong way round overflows fp32)
-#   split_merge     even blocks at 10 i, odd ones at 10 i + 14, times a per-row factor in [1, 4]: both warpgroups rescale,
-#                   and warpgroup 1 ends about 14 to 56 units above warpgroup 0, so both states enter the merge
-SCALED = {"all_x8": ("all", 8.0, 1280, 0.5), "all_x16": ("all", 16.0, 700, 1.0), "half_warp": ("half_warp", 16.0, 640, 1.0),
-          "one_warp": ("one_warp", 16.0, 640, 1.0), "ragged_last": ("ragged_last", 12.0, 1000, 1.0)}
-SPLIT = ("split_dominant", "split_merge")
+# The input builders (large-score and entry-split patterns, long lists) are sla_backward_oracle's.
+SCALED, SPLIT = B.SCALED, B.SPLIT
 MIN_FRACTION = {"all": 0.2, "ragged_last": 0.3, "half_warp": 0.08, "one_warp": 0.04, "split_dominant": 0.9, "split_merge": 0.9}
-
-
-def _randn(l, h, seed):
-    g = torch.Generator().manual_seed(seed)
-    return [torch.randn(1, l, h, D, generator=g) for _ in range(3)]
-
-
-def _scaled_case(name, blkq, h=2, seed=0):
-    pattern, qscale, l, ratio = SCALED[name]
-    q, k, v = _randn(l, h, 4000 + l + seed)
-    rows = torch.arange(l)
-    if pattern in ("all", "ragged_last"):
-        q = q * qscale
-    elif pattern == "half_warp":
-        q[:, (rows % 16) < 8] *= qscale
-    elif pattern == "one_warp":
-        q[:, (rows % blkq) < 16] *= qscale
-    if pattern == "ragged_last":
-        q = q + 2.0 * qscale * U
-        k[:, -(l % BK):] += 6.0 * U
-    return q, k, v, ratio
-
-
-def _pair_lut(h, mblk, npairs, keep, seed):
-    """[1,h,mblk,2*keep] int32: per row `keep` of the `npairs` pairs (2i, 2i+1), ascending."""
-    g = torch.Generator().manual_seed(seed)
-    lut = torch.empty(1, h, mblk, 2 * keep, dtype=torch.int32)
-    for hi in range(h):
-        for mi in range(mblk):
-            pairs = torch.randperm(npairs, generator=g)[:keep].sort().values
-            lut[0, hi, mi] = torch.stack([2 * pairs, 2 * pairs + 1], -1).flatten()
-    return lut
-
-
-def _split_case(name, blkq, h=2, seed=0):
-    """L = 1240: 20 key blocks (the last one 24 keys, odd: in warpgroup 1's entries), ragged last query block."""
-    l, a = 1240, 4.0
-    q, k, v = _randn(l, h, 7000 + seed)
-    q = q - (q @ U)[..., None] * U                           # q orthogonal to U, then a chosen component along it
-    g = torch.Generator().manual_seed(8000 + seed)
-    alpha = torch.ones(1, l, h, 1) if name == "split_dominant" else 1.0 + 3.0 * torch.rand(1, l, h, 1, generator=g)
-    q = q + a * alpha * U
-    n = torch.arange(_cdiv(l, BK))
-    if name == "split_dominant":
-        offset = torch.where(n % 2 == 1, 140.0 + 12.0 * (n // 2), torch.zeros(()))
-    else:
-        offset = 10.0 * (n // 2) + 14.0 * (n % 2)
-    c = (offset / (a * SM * LOG2E)).repeat_interleave(BK)[:l]    # score offset of key block n = alpha * offset[n]
-    k = k + c[None, :, None, None] * U
-    return q, k, v, _pair_lut(h, _cdiv(l, blkq), 10, 7, 9000 + seed + blkq)
 
 
 def _module(blkq, ratio, dtype, seed=5, **kw):
@@ -273,10 +181,10 @@ def _module(blkq, ratio, dtype, seed=5, **kw):
 def _case(name, blkq, dtype):
     """(q, k, v on the GPU in dtype, lut or None (the module selects), ratio)."""
     if name in SPLIT:
-        q, k, v, lut = _split_case(name, blkq)
+        q, k, v, lut = B.split_case(name, blkq)
         ratio, lut = 1.0, lut.cuda()
     else:
-        q, k, v, ratio = _scaled_case(name, blkq)
+        q, k, v, ratio = B.scaled_case(name, blkq)
         lut = None
     return [t.to(dtype).cuda() for t in (q, k, v)], lut, ratio
 
@@ -419,18 +327,6 @@ def test_sm_scale_other_than_head_dim(cuda, blkq):
 
 
 # ------------------------------------------------------------------------------------------------------------ 3. long lists
-def _long_inputs(l, h, dtype, seed):
-    """randn q, k, v on the GPU plus a ramp of 6 log2 units over the key blocks (later blocks weigh up to 64x more), so that
-    every part of a long LUT row, its last entries included, carries a visible share of each row's softmax mass."""
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    q, k, v = (torch.randn(1, l, h, D, generator=g, device="cuda") for _ in range(3))
-    a, u = 4.0, U.cuda()
-    q = q - (q @ u)[..., None] * u + a * u
-    ramp = 6.0 * (torch.arange(l, device="cuda") // BK) / (_cdiv(l, BK) - 1)
-    k = k + (ramp / (a * SM * LOG2E))[None, :, None, None] * u
-    return [t.to(dtype) for t in (q, k, v)]
-
-
 def _check_long(q, k, v, lut, blkq, q_blocks, k_blocks, what):
     """Forward with lse and backward on `lut`: o_s and lse of every row against float64 attention, dQ of q_blocks and dK /
     dV of k_blocks against the closed-form float64 backward (float64 lse and delta), on every head."""
@@ -441,16 +337,16 @@ def _check_long(q, k, v, lut, blkq, q_blocks, k_blocks, what):
     row_err = (o_s.to(F64) - ref["o"]).norm(dim=-1) / ref["o"].norm(dim=-1)
     assert row_err.max() <= 2e-2, (what, "o_s row", row_err.max().item())
     worst = _check_lse(lse, ref, what)
-    bm = _block_mask(lut, _cdiv(l, BK))
+    bm = B.block_mask(lut, _cdiv(l, BK))
     lines = [f"{what}: o_s rel-L2 {s_os['rel_l2']:.2e} (worst row {row_err.max().item():.2e}), lse max |err| {worst:.2e}"]
     for hi in range(h):
         for mi in q_blocks:
             r0, r1 = mi * blkq, min(l, (mi + 1) * blkq)
-            s = _bars(dq[0, r0:r1, hi], _ref_dq(q, k, v, d_o, bm, blkq, ref, 0, hi, mi), 0.999, 2e-2, (what, "dq", hi, mi))
+            s = _bars(dq[0, r0:r1, hi], B.ref_dq(q, k, v, d_o, bm, blkq, ref, 0, hi, mi), 0.999, 2e-2, (what, "dq", hi, mi))
             lines.append(f"  dq h{hi} qblk {mi}: rel-L2 {s['rel_l2']:.2e}")
         for ni in k_blocks:
             c0, c1 = ni * BK, min(l, (ni + 1) * BK)
-            wk, wv = _ref_dkdv(q, k, v, d_o, bm, blkq, ref, 0, hi, ni)
+            wk, wv = B.ref_dkdv(q, k, v, d_o, bm, blkq, ref, 0, hi, ni)
             sk = _bars(dk[0, c0:c1, hi], wk, 0.999, 2e-2, (what, "dk", hi, ni))
             sv = _bars(dv[0, c0:c1, hi], wv, 0.999, 2e-2, (what, "dv", hi, ni))
             lines.append(f"  dk / dv h{hi} kblk {ni} (list {int(bm[0, hi, :, ni].sum())}): rel-L2 {sk['rel_l2']:.2e} / "
@@ -474,7 +370,7 @@ def test_long_dense_block_lists(cuda, blkq, l, dtype):
     h = 2
     mblk, nblk = _cdiv(l, blkq), _cdiv(l, BK)
     assert nblk > (288 if blkq == 128 else 384) and nblk > 256
-    q, k, v = _long_inputs(l, h, dtype, seed=l)
+    q, k, v = B.long_inputs(l, h, dtype, seed=l)
     lut = torch.arange(nblk, dtype=torch.int32, device="cuda").expand(1, h, mblk, nblk).contiguous()
     _check_long(q, k, v, lut, blkq, (0, mblk // 2, mblk - 1), (0, nblk // 2, nblk - 1), f"dense q{blkq} L{l} {dtype}")
 
@@ -485,7 +381,7 @@ def test_long_sparse_hand_made_lut(cuda, blkq):
     every row holding key block 0 and the last one, whose dK / dV lists are therefore mblk long."""
     l, h, topk = 32760, 2, 400
     mblk, nblk = _cdiv(l, blkq), _cdiv(l, BK)
-    q, k, v = _long_inputs(l, h, BF16, seed=blkq)
+    q, k, v = B.long_inputs(l, h, BF16, seed=blkq)
     g = torch.Generator().manual_seed(31 + blkq)
     lut = torch.empty(1, h, mblk, topk, dtype=torch.int32)
     for hi in range(h):
@@ -519,7 +415,7 @@ def test_long_dense_lists_fused_forward(cuda, family, l):
             mod.proj_l.weight.copy_(torch.randn(D, D, generator=g) * 0.05)
             mod.proj_l.bias.copy_(torch.randn(D, generator=g) * 0.05)
         bars = (0.999, 2e-2)                    # the INT8 families' bars against the exact oracle (test_gpu_sla.py)
-    q, k, v = _long_inputs(l, h, BF16, seed=l + 1)
+    q, k, v = B.long_inputs(l, h, BF16, seed=l + 1)
     prev = set_served_arch("sm90" if (blkq, blkk) == (64, 128) else "sm100")
     try:
         assert mod.block_sizes(0) == (blkq, blkk)

@@ -36,9 +36,31 @@ def _fwd_lse(lib, q=True, topk=4, d=128, dtype=0, l=256, blkq=BQ, blkk=BK, b=1):
                                          None)
 
 
-def _bwd(lib, ws=_p(), ws_bytes=1 << 30, topk=4, d=128, dtype=0, l=256, lse=True, blkq=BQ, blkk=BK, b=1):
+def _bwd(lib, ws=_p(), ws_bytes=1 << 30, topk=4, d=128, dtype=0, l=256, lse=True, blkq=BQ, blkk=BK, b=1, h=2):
     return lib.tdb200_sla_attn16_bwd(_p(), _p(), _p(), _p(), _p(), _p() if lse else None, dtype, _p(), topk, _p(), _p(), _p(), ws,
-                                     ws_bytes, b, l, 2, d, 0.088, blkq, blkk, None)
+                                     ws_bytes, b, l, h, d, 0.088, blkq, blkk, None)
+
+
+# The backward's own limits (tdb200_sla_attn16_bwd; the dQ kernels stage a LUT row on chip as uint16 ids):
+#   nblk <= 65535 (grid.x of the dK / dV kernel; the uint16 ids), and b * h * mblk * topk <= 2^31 - 1 (the key-major index);
+#   1024 (alignment) + kOffLut + round16(2 topk) <= 227 KB, kOffLut the dQ kernel's shared memory before its LUT:
+#     (128, 64)  sla_bwd_dq_kernel      Q 32768 | dO 32768 | 3 K + 3 V stages of 16384 | 256 barriers = 164096
+#                232448 - 1024 - 164096 = 67328 = 2 * 33664: topk 33664 fits, 33665 is refused for its LUT.  topk <= nblk
+#                puts L >= 64 topk and mblk = L / 128 ~ topk / 2, so at b = h = 1 the index bound (topk^2 / 2) is far away.
+#     (64, 64)   sla_bwd_dq_q64_kernel  Q 16384 | dO 16384 | 3 K + 3 V stages of 16384 | 256 barriers = 131328
+#                the LUT would allow topk <= (232448 - 1024 - 131328) / 2 = 50048, but mblk = L / 64 >= nblk >= topk, so
+#                b * h * mblk * topk >= topk^2 and the index bound refuses first: 46340^2 <= 2^31 - 1 < 46341^2.  The LUT
+#                refusal cannot be reached on 64-row blocks.
+BWD_TOPK_LIMIT = {128: 33664, 64: 46340}
+BWD_MAX_NBLK = 65535
+
+
+def _bwd_at(lib, blkq, topk, nblk=None, ws_bytes=None):
+    """A backward call at b = h = 1 with L = 64 * nblk (default: topk key blocks, every one selected)."""
+    l = 64 * (topk if nblk is None else nblk)
+    if ws_bytes is None:
+        ws_bytes = lib.tdb200_sla_attn16_bwd_workspace_bytes(1, 1, l, topk, blkq)
+    return _bwd(lib, ws_bytes=ws_bytes, topk=topk, l=l, blkq=blkq, b=1, h=1)
 
 
 def test_argument_validation(lib):
@@ -70,6 +92,12 @@ def test_argument_validation(lib):
                   (f"lse blocks {blkq}x{blkk}", lambda q=blkq, k=blkk: _fwd_lse(lib, blkq=q, blkk=k), UNSUPPORTED, b"block"),
                   (f"bwd blocks {blkq}x{blkk}", lambda q=blkq, k=blkk: _bwd(lib, blkq=q, blkk=k), UNSUPPORTED, b"block")]
     cases.append(("workspace blkq 32", lambda: lib.tdb200_sla_attn16_bwd_workspace_bytes(1, 2, 256, 4, 32), UNSUPPORTED, b"block"))
+    cases += [("bwd q128 topk limit + 1", lambda: _bwd_at(lib, 128, BWD_TOPK_LIMIT[128] + 1), UNSUPPORTED, b"LUT"),
+              ("bwd q64 topk limit + 1", lambda: _bwd_at(lib, 64, BWD_TOPK_LIMIT[64] + 1), UNSUPPORTED, b"dimension too large"),
+              ("bwd q64 LUT bound + 1", lambda: _bwd_at(lib, 64, 50049), UNSUPPORTED, b"dimension too large")]
+    for blkq in (128, 64):
+        cases.append((f"bwd q{blkq} nblk 65536", lambda q=blkq: _bwd_at(lib, q, 4, nblk=BWD_MAX_NBLK + 1, ws_bytes=1 << 40),
+                      UNSUPPORTED, b"dimension too large"))
     for name, call, code, needle in cases:
         rc = call()
         msg = lib.tdb200_last_error() or b""
@@ -85,6 +113,20 @@ def test_valid_calls_pass_validation(lib):
     for call in (lambda: _fwd(lib, feature=2), lambda: _fwd_lse(lib),
                  lambda: _bwd(lib, ws_bytes=lib.tdb200_sla_attn16_bwd_workspace_bytes(1, 2, 256, 4, BQ))):
         assert call() in (-3, -4) and lib.tdb200_last_error()
+
+
+def test_backward_limits_pass_validation(lib):
+    """Each of the backward's limits is accepted by validation (one more is refused, test_argument_validation): the largest
+    top-k of both block heights with every key block selected, and 65,535 key blocks at both heights.  On a host without a
+    GPU the calls stop at the device check."""
+    if torch.cuda.is_available():
+        pytest.skip("this check is for hosts without a GPU")
+    for blkq in (128, 64):
+        for name, call in ((f"q{blkq} topk {BWD_TOPK_LIMIT[blkq]}", lambda: _bwd_at(lib, blkq, BWD_TOPK_LIMIT[blkq])),
+                           (f"q{blkq} nblk {BWD_MAX_NBLK}", lambda: _bwd_at(lib, blkq, 4, nblk=BWD_MAX_NBLK))):
+            rc = call()
+            msg = lib.tdb200_last_error() or b""
+            assert rc in (-3, -4) and msg, (name, rc, msg)
 
 
 @pytest.mark.parametrize("b,h,l,topk", [(1, 2, 256, 4), (2, 3, 1000, 7), (1, 40, 75600, 118), (1, 12, 32760, 51)])

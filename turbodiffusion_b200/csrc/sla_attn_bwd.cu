@@ -24,6 +24,13 @@
 // in fp32 registers and are rounded to T once.  No floating-point atomics: every output element is written by one thread in a
 // fixed order, so the gradients are bit-for-bit reproducible.  Key columns >= lk are masked to -inf; query rows >= lq get
 // lse = +inf (P = 0) and delta = 0 explicitly, because TMA zero-fill gives their scores, not their statistics.
+//
+// fp16 only: dS = P o (dP - delta) is small where P is (peaked softmax) or dO is (loss-scaled training), and below fp16's
+// normal range (2^-14) rounding it keeps only a few bits although dq and dk themselves are normal fp16 values.  So the dS
+// operand is rounded as dS * 2^e, e per accumulator row (a query row of dQ, a key row of dK) and chosen from the largest |dS|
+// that row has seen (its top bit at 2^14); when a later tile needs a smaller e the row's fp32 accumulator is rescaled by the
+// power of two, and it is divided by 2^e before the store.  Every rescale is exact.  bf16 has fp32's exponent range and takes
+// none of this: its instructions are unchanged.
 #include <type_traits>
 
 #include "sla_attn.cuh"
@@ -114,6 +121,68 @@ __global__ void __launch_bounds__(kIndexThreads) sla_bwd_kmajor_index_kernel(con
       idx[off[k] + atomicAdd(&cur[k], 1)] = i;
     }
     __syncthreads();
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ fp16 dS operand scale
+// e[hf] is the exponent of rows hf = 0, 1 (r0, r0 + 8) of this thread's accumulator fragment; kDsUnset until the row has seen a
+// nonzero |dS|.  Clamped to [-60, 60], so 2^e, 2^-e and every rescale ratio are normal fp32 powers of two.
+constexpr int kDsUnset = 1 << 30, kDsMaxExp = 60;
+
+__device__ __forceinline__ float pow2f(int e) { return __int_as_float((e + 127) << 23); }
+
+// The fragment's four lanes of a row share the row maximum m[hf] of |dS| in this tile (butterfly over lanes ^1, ^2); e[hf]
+// drops to 14 - floor(log2 m) when that is below it, and acc's row is rescaled to the new exponent.
+__device__ __forceinline__ void ds_exponent(int (&e)[2], float (&m)[2], float (&acc)[HD / 2]) {
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    float mm = fmaxf(m[hf], __shfl_xor_sync(0xffffffffu, m[hf], 1));
+    mm = fmaxf(mm, __shfl_xor_sync(0xffffffffu, mm, 2));
+    if (mm > 0.f) {
+      const int want = min(max(14 - (((__float_as_int(mm) >> 23) & 0xff) - 127), -kDsMaxExp), kDsMaxExp);
+      if (want < e[hf]) {
+        if (e[hf] != kDsUnset) {
+          const float r = pow2f(want - e[hf]);
+#pragma unroll
+          for (int c = 0; c < HD / 8; ++c) {
+            acc[4 * c + 2 * hf] *= r;
+            acc[4 * c + 2 * hf + 1] *= r;
+          }
+        }
+        e[hf] = want;
+      }
+    }
+  }
+}
+
+// the accumulator rows back to the unscaled sum: acc row hf *= 2^-e[hf]
+__device__ __forceinline__ void ds_unscale(const int (&e)[2], float (&acc)[HD / 2]) {
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    const float r = pow2f(-min(e[hf], kDsMaxExp));
+#pragma unroll
+    for (int c = 0; c < HD / 8; ++c) {
+      acc[4 * c + 2 * hf] *= r;
+      acc[4 * c + 2 * hf + 1] *= r;
+    }
+  }
+}
+
+// dS of a 64 x 64 tile (fp32, fragment layout: element i in row (i >> 1) & 1) -> the T operand fragments.  fp16: scaled by
+// 2^e of its row after ds_exponent has settled e (and rescaled acc) for this tile.
+template <typename T>
+__device__ __forceinline__ void pack_ds(float (&ds)[32], uint32_t (&da)[4][4], int (&e)[2], float (&acc)[HD / 2]) {
+  if constexpr (std::is_same<T, __half>::value) {
+    float m[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < 32; ++i) m[(i >> 1) & 1] = fmaxf(m[(i >> 1) & 1], fabsf(ds[i]));
+    ds_exponent(e, m, acc);
+    const float sc[2] = {pow2f(min(e[0], kDsMaxExp)), pow2f(min(e[1], kDsMaxExp))};
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) da[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(ds[i] * sc[(i >> 1) & 1], ds[i + 1] * sc[(i >> 1) & 1]);
+  } else {
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) da[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(ds[i], ds[i + 1]);
   }
 }
 
@@ -222,6 +291,7 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
   float acc[HD / 2];
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) acc[i] = 0.f;
+  int ds_e[2] = {kDsUnset, kDsUnset};   // per query row (fp16)
 
   mbar_wait(&bars[kQFull], 0);
   for (int j = 0; j < p.topk; ++j) {
@@ -260,12 +330,24 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
 
     // ---- P = exp2(S sc - lse) (columns past l masked), dS = P o (dP - delta), rounded to T into the A fragments
     uint32_t da[BLKK / 16][4];
+    if constexpr (kBF16) {
 #pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const int hf = (i >> 1) & 1, col = 8 * (i >> 2) + cq;
-      const float p0 = col < valid ? fast_exp2(fmaf(s[i], sc, -lse[hf])) : 0.f;
-      const float p1 = col + 1 < valid ? fast_exp2(fmaf(s[i + 1], sc, -lse[hf])) : 0.f;
-      da[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0 * (dp[i] - dlt[hf]), p1 * (dp[i + 1] - dlt[hf]));
+      for (int i = 0; i < 32; i += 2) {
+        const int hf = (i >> 1) & 1, col = 8 * (i >> 2) + cq;
+        const float p0 = col < valid ? fast_exp2(fmaf(s[i], sc, -lse[hf])) : 0.f;
+        const float p1 = col + 1 < valid ? fast_exp2(fmaf(s[i + 1], sc, -lse[hf])) : 0.f;
+        da[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0 * (dp[i] - dlt[hf]), p1 * (dp[i + 1] - dlt[hf]));
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int hf = (i >> 1) & 1, col = 8 * (i >> 2) + cq;
+        const float p0 = col < valid ? fast_exp2(fmaf(s[i], sc, -lse[hf])) : 0.f;
+        const float p1 = col + 1 < valid ? fast_exp2(fmaf(s[i + 1], sc, -lse[hf])) : 0.f;
+        s[i] = p0 * (dp[i] - dlt[hf]);
+        s[i + 1] = p1 * (dp[i + 1] - dlt[hf]);
+      }
+      pack_ds<T>(s, da, ds_e, acc);
     }
     // ---- dQ += dS.K  (K: [64 keys x HD], the MN-major operand; +16 keys = +2048 B per K step)
     const uint64_t kmn = make_desc_mnmajor_sw128(sk, BLKK * 128);
@@ -280,6 +362,7 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
     __syncwarp();
     if (lane == 0) mbar_arrive(&bars[kKEmpty + st]);
   }
+  if constexpr (!kBF16) ds_unscale(ds_e, acc);
   store_rows<T>(acc, p.sm_scale, p.dq, int64_t(m_blk) * BLKQ + r_lo, p.lq, p.h, hh, b, cq);
 }
 
@@ -391,6 +474,7 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   float dk[HD / 2], dv[HD / 2];
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) dk[i] = dv[i] = 0.f;
+  int ds_e[2] = {kDsUnset, kDsUnset};   // per key row of dk (fp16)
 
   mbar_wait(&bars[L::kKVFull], 0);
   for (int j = L::kSplit ? wg : 0, it = 0; j < n_list; j += L::kSplit ? 2 : 1, ++it) {
@@ -448,8 +532,10 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
       const float2 dl = *reinterpret_cast<const float2*>(sb + 64 + 8 * (i >> 2) + cq);
-      da[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(s[i] * (dp[i] - dl.x), s[i + 1] * (dp[i + 1] - dl.y));
+      dp[i] = s[i] * (dp[i] - dl.x);
+      dp[i + 1] = s[i + 1] * (dp[i + 1] - dl.y);
     }
+    pack_ds<T>(dp, da, ds_e, dk);
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) wgmma_f16_rs<HD, kBF16, 1>(dk, da[kk], make_desc_mnmajor_sw128(sq, kBQ * 128) + uint64_t(kk * 128));
@@ -465,7 +551,8 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     warp_release(&bars[L::kEmpty + st], lane);
   }
 
-  // ---- warpgroup 1's partials -> warpgroup 0 through the Q / dO ring, which both warpgroups have drained
+  // ---- warpgroup 1's partials -> warpgroup 0 through the Q / dO ring, which both warpgroups have drained (dk unscaled first)
+  if constexpr (!kBF16) ds_unscale(ds_e, dk);
   const Handoff x = handoff_wg1_to_wg0(smem + L::kOffQ, wg, 3, [&](const Handoff& x) {
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) {
@@ -571,6 +658,7 @@ sla_bwd_dq_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   float acc[HD / 2];
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) acc[i] = 0.f;
+  int ds_e[2] = {kDsUnset, kDsUnset};   // per query row (fp16)
 
   mbar_wait(&bars[kQFull], 0);
   for (int j = wg; j < p.topk; j += 2) {
@@ -609,12 +697,24 @@ sla_bwd_dq_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
 
     // ---- P = exp2(S sc - lse) (columns past l masked), dS = P o (dP - delta), rounded to T into the A fragments
     uint32_t da[BLKK / 16][4];
+    if constexpr (kBF16) {
 #pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const int hf = (i >> 1) & 1, col = 8 * (i >> 2) + cq;
-      const float p0 = col < valid ? fast_exp2(fmaf(s[i], sc, -lse[hf])) : 0.f;
-      const float p1 = col + 1 < valid ? fast_exp2(fmaf(s[i + 1], sc, -lse[hf])) : 0.f;
-      da[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0 * (dp[i] - dlt[hf]), p1 * (dp[i + 1] - dlt[hf]));
+      for (int i = 0; i < 32; i += 2) {
+        const int hf = (i >> 1) & 1, col = 8 * (i >> 2) + cq;
+        const float p0 = col < valid ? fast_exp2(fmaf(s[i], sc, -lse[hf])) : 0.f;
+        const float p1 = col + 1 < valid ? fast_exp2(fmaf(s[i + 1], sc, -lse[hf])) : 0.f;
+        da[i >> 3][(i >> 1) & 3] = F16Traits<T>::pack(p0 * (dp[i] - dlt[hf]), p1 * (dp[i + 1] - dlt[hf]));
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int hf = (i >> 1) & 1, col = 8 * (i >> 2) + cq;
+        const float p0 = col < valid ? fast_exp2(fmaf(s[i], sc, -lse[hf])) : 0.f;
+        const float p1 = col + 1 < valid ? fast_exp2(fmaf(s[i + 1], sc, -lse[hf])) : 0.f;
+        s[i] = p0 * (dp[i] - dlt[hf]);
+        s[i + 1] = p1 * (dp[i + 1] - dlt[hf]);
+      }
+      pack_ds<T>(s, da, ds_e, acc);
     }
     // ---- dQ += dS.K  (K as the MN-major operand; +16 keys = +2048 B per K step)
     const uint64_t kmn = make_desc_mnmajor_sw128(sk, BLKK * 128);
@@ -630,7 +730,8 @@ sla_bwd_dq_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     if (lane == 0) mbar_arrive(&bars[kKEmpty + st]);
   }
 
-  // ---- dQ = partial of warpgroup 0 + partial of warpgroup 1, through the drained K ring
+  // ---- dQ = partial of warpgroup 0 + partial of warpgroup 1, through the drained K ring (each unscaled first)
+  if constexpr (!kBF16) ds_unscale(ds_e, acc);
   const Handoff x = handoff_wg1_to_wg0(smem + kOffK, wg, 1, [&](const Handoff& x) {
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) x[i] = acc[i];

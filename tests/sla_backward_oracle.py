@@ -3,9 +3,11 @@ reference for the SparseLinearAttention backward kernels (csrc/sla_attn_bwd.cu).
 row statistics of the forward: lse (log2 units) and delta = rowsum(dO * O).  Test infrastructure only.  Tensors are
 [B, H, L, D] like td_oracle.sparse_attention; lut [B, H, Mblk, topk] key-block ids.
 
-The second half holds what the 16-bit GPU tests share, on the module layout [B, L, H, D] and on whatever device the tensors
-live: the large-score and entry-split input builders, the long-list inputs, and the closed-form dQ / dK / dV of one block
-given float64 (or any) lse and delta."""
+The second half holds what the GPU float64 tests of the attention kernels share, on the module layout [B, L, H, D] and on
+whatever device the tensors live: the large-score and entry-split input builders, the long-list inputs, the closed-form
+dQ / dK / dV of one block given float64 (or any) lse and delta, the module's block selection, sentinel-filled output
+buffers, seeded GPU inputs, the linear branch's feature maps, the library's last error, and two rounding points of the
+forward kernels' restatements (the lazily rescaled running maximum and the fp16 linear-branch operand)."""
 from __future__ import annotations
 
 import math
@@ -198,3 +200,68 @@ def long_inputs(l, h, dtype, seed):
     ramp = 6.0 * (torch.arange(l, device="cuda") // BK) / (cdiv(l, BK) - 1)
     k = k + (ramp / (a * SM * LOG2E))[None, :, None, None] * u
     return [t.to(dtype) for t in (q, k, v)]
+
+
+def block_map_lut(q, k, blkq, topk, blkk=BK):
+    """The module's block selection (mean pooling over blocks, top-k of the pooled scores), ascending [B,H,Mblk,topk], of
+    16-bit q, k [B, L, H, D] on the GPU."""
+    from turbodiffusion_b200.SLA.utils import block_map_from_pools, mean_pool
+    qh, kh = (t.transpose(1, 2).contiguous() for t in (q, k))
+    return block_map_from_pools(mean_pool(qh, blkq), mean_pool(kh, blkk), topk)[1].contiguous()
+
+
+def sentinel_buffers(dtype, dev, pad_rows, sentinel, *shapes):
+    """Flat buffers filled with `sentinel`, pad_rows rows longer than each [..., l, h, d] shape (a row: h * d values):
+    (views of the shapes, the pads after them)."""
+    views, pads = [], []
+    for shape in shapes:
+        n = math.prod(shape)
+        buf = torch.full((n + pad_rows * shape[-2] * shape[-1],), sentinel, dtype=dtype, device=dev)
+        views.append(buf[:n].view(*shape))
+        pads.append(buf[n:])
+    return views, pads
+
+
+def running_max(ent_max, two_warpgroups):
+    """The row maximum each entry's P is formed against in the SLA forward kernels ([R, entries] float32, in list order):
+    the first entry of a warpgroup sets it, and it moves only when an entry's maximum exceeds it by more than 2^8 (the lazy
+    rescale).  The 64-row kernels run one such sequence per warpgroup, over alternate entries."""
+    m = ent_max.clone()
+    for j in range(2 if two_warpgroups else 1, ent_max.shape[1]):
+        prev = m[:, j - 2] if two_warpgroups else m[:, j - 1]
+        m[:, j] = torch.where(ent_max[:, j] > prev + 8.0, ent_max[:, j], prev)
+    return m
+
+
+def round_operand(a, dtype):
+    """T(a) as the fused forwards form the linear branch's MMA operand: in fp16 a row whose max lies outside [2^-6, 2^15) is
+    rounded as a * 2^sc with sc = clamp(14 - floor(log2 max), -64, 64), and the power of two divided out again (sla_attn.cu)."""
+    if dtype == torch.bfloat16:
+        return a.to(dtype).double()
+    amax = a.amax(-1, keepdim=True)
+    e = torch.frexp(amax.clamp_min(1e-300)).exponent - 1          # floor(log2 amax)
+    sc = (14 - e).clamp(-64, 64).double()
+    sc = torch.where(((amax > 0) & (amax < 2.0 ** -6)) | (amax >= 2.0 ** 15), sc, torch.zeros_like(sc))
+    return (a * torch.exp2(sc)).to(dtype).double() * torch.exp2(-sc)
+
+
+def randn(shape, dtype, seed, scale=1.0):
+    """randn * scale in `dtype` on the GPU, from its own seeded generator."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    return (torch.randn(shape, generator=g, device="cuda") * scale).to(dtype)
+
+
+def phi(x, feature):
+    """The linear branch's feature map (SLA/core.py:57-73): 0 softmax over the channels, 1 elu + 1, 2 relu."""
+    if feature == 0:
+        return torch.softmax(x, -1)
+    if feature == 1:
+        return torch.nn.functional.elu(x) + 1
+    return torch.relu(x)
+
+
+def last_error():
+    """The library's message for its last failed call."""
+    from turbodiffusion_b200._lib import lib
+    msg = lib().tdb200_last_error()
+    return msg.decode() if msg else ""

@@ -84,6 +84,15 @@ def test_argument_checks_return_codes(lib, entry, fn, prefix, name, kw, code, ne
     assert msg.startswith(prefix) and needle in msg, (entry, name, msg)
 
 
+def test_the_largest_staged_lut_passes_validation(lib):
+    """The sparse tangent at topk = 8640 ids (the LUT row fills the shared memory the kernel may use, jvp::kMaxLutIds) gets
+    past validation; 8641 is refused (SLA_SHAPES)."""
+    if torch.cuda.is_available():
+        pytest.skip("this check is for hosts without a GPU")
+    rc = _sla(lib, l=8640 * 64, topk=8640)
+    assert rc in (-3, -4) and lib.tdb200_last_error()
+
+
 def test_valid_calls_without_a_gpu_report_an_error_code(lib):
     if torch.cuda.is_available():
         pytest.skip("this check is for hosts without a GPU")

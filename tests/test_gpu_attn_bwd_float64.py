@@ -69,20 +69,12 @@ def _lib():
     return _lib
 
 
-def _last_error():
-    msg = _lib().lib().tdb200_last_error()
-    return msg.decode() if msg else ""
+_last_error = B.last_error
 
 
 def _buffers(dtype, dev, *shapes):
     """Sentinel-filled flat buffers PAD_ROWS rows longer than each [b, l, h, d] shape: (views, pads)."""
-    views, pads = [], []
-    for b, l, h, d in shapes:
-        n = b * l * h * d
-        buf = torch.full((n + PAD_ROWS * h * d,), SENTINEL, dtype=dtype, device=dev)
-        views.append(buf[:n].view(b, l, h, d))
-        pads.append(buf[n:])
-    return views, pads
+    return B.sentinel_buffers(dtype, dev, PAD_ROWS, SENTINEL, *shapes)
 
 
 def _sla_forward(q, k, v, lut, blkq):
@@ -154,9 +146,7 @@ def _run(x):
     return _finish(_sla_bwd(x) if x.lut is not None else _dense_bwd(x))
 
 
-def _randn(shape, dtype, seed, scale=1.0):
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    return (torch.randn(shape, generator=g, device="cuda") * scale).to(dtype)
+_randn = B.randn
 
 
 # ------------------------------------------------------------------------------------------------------------ references
@@ -340,11 +330,7 @@ def _check(x, what, q_blocks=None, k_blocks=None, bh=None):
 
 
 # ------------------------------------------------------------------------------------------------------------ inputs
-def _block_map_lut(q, k, blkq, topk):
-    """The module's block selection (mean pooling over blocks, top-k of the pooled scores), ascending [B,H,Mblk,topk]."""
-    from turbodiffusion_b200.SLA.utils import block_map_from_pools, mean_pool
-    qh, kh = (t.transpose(1, 2).contiguous() for t in (q, k))
-    return block_map_from_pools(mean_pool(qh, blkq), mean_pool(kh, BK), topk)[1].contiguous()
+_block_map_lut = B.block_map_lut
 
 
 def _inputs(b, l, h, dtype, seed, lk=None):

@@ -28,6 +28,8 @@ import math
 import pytest
 import torch
 
+import sla_backward_oracle as B
+
 pytestmark = pytest.mark.gpu
 
 FAMILIES = {"sm100": (128, 64), "sm90": (64, 128)}   # (BLKQ, BLKK): sla_attn_fwd_kernel, sla_attn_fwd_q64_kernel
@@ -181,42 +183,11 @@ def _run(x, lut, k_seq_major=False, lk=None, topk=None):
     return rc, buf[:n].view(x.b, x.lq, x.h, x.d), buf[n:]
 
 
-def _last_error():
-    from turbodiffusion_b200._lib import lib
-    msg = lib().tdb200_last_error()
-    return msg.decode() if msg else ""
+_last_error = B.last_error
 
 
 # ------------------------------------------------------------------------------------------------------------ references
-def _phi(x, feature):
-    if feature == 0:
-        return torch.softmax(x, -1)
-    if feature == 1:
-        return torch.nn.functional.elu(x) + 1
-    return torch.relu(x)
-
-
-def _round_operand(a, dtype):
-    """T(a) as the kernel forms the linear branch's MMA operand: in fp16 a row whose max lies outside [2^-6, 2^15) is rounded
-    as a * 2^sc with sc = clamp(14 - floor(log2 max), -64, 64), and the power of two divided out again (sla_attn.cu)."""
-    if dtype == torch.bfloat16:
-        return a.to(dtype).double()
-    amax = a.amax(-1, keepdim=True)
-    e = torch.frexp(amax.clamp_min(1e-300)).exponent - 1          # floor(log2 amax)
-    sc = (14 - e).clamp(-64, 64).double()
-    sc = torch.where(((amax > 0) & (amax < 2.0 ** -6)) | (amax >= 2.0 ** 15), sc, torch.zeros_like(sc))
-    return (a * torch.exp2(sc)).to(dtype).double() * torch.exp2(-sc)
-
-
-def _running_max(ent_max, two_warpgroups):
-    """The row maximum each entry's P is formed against in the kernel ([R, entries] float32, in LUT order): the first entry
-    of a warpgroup sets it, and it moves only when an entry's maximum exceeds it by more than 2^8 (the lazy rescale).  The
-    64-row kernel runs one such sequence per warpgroup, over alternate entries."""
-    m = ent_max.clone()
-    for j in range(2 if two_warpgroups else 1, ent_max.shape[1]):
-        prev = m[:, j - 2] if two_warpgroups else m[:, j - 1]
-        m[:, j] = torch.where(ent_max[:, j] > prev + 8.0, ent_max[:, j], prev)
-    return m
+_phi = B.phi
 
 
 def _flip_step(p):
@@ -268,7 +239,7 @@ def _references(x, bi, hi, rows, entries, q_scale=None, entry_k_scale=None, key_
     for _, _, s64, s32 in tiles():
         m64 = torch.maximum(m64, s64.amax(-1, keepdim=True))
         ent_max.append(s32.view(len(rows), -1, bk).amax(-1))
-    m_ent = _running_max(torch.cat(ent_max, 1).cpu(), x.blkq == 64).to(dev)
+    m_ent = B.running_max(torch.cat(ent_max, 1).cpu(), x.blkq == 64).to(dev)
     m_top = m_ent[:, -2:].amax(-1, keepdim=True).double()   # the maximum after the last entry (and the warpgroups' merge)
     w_ent = torch.exp2(m_ent.double() - m_top)               # exact rescale factor of each entry's P into that maximum
     # pass 2: float64 softmax . V; P against the running maximum, rounded to T, weighted into the final maximum
@@ -303,7 +274,7 @@ def _references(x, bi, hi, rows, entries, q_scale=None, entry_k_scale=None, key_
     kvw = x.kvw[bi, hi].double()
     pb = x.proj_b.double()
     ref = o64 / l64 + (phi @ kvw.t()) / den[:, None] + pb
-    a = _round_operand(phi * (l32 / den[:, None]), x.dtype)
+    a = B.round_operand(phi * (l32 / den[:, None]), x.dtype)
     r32 = (o32 + a @ kvw.t()) / l32 + pb
     rest = r32.to(x.dtype).double()
     if fp8 is None:

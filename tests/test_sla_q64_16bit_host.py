@@ -53,6 +53,19 @@ def _bwd(lib, ws=_p(), ws_bytes=1 << 30, topk=4, d=128, dtype=0, l=256, lse=True
 #                refusal cannot be reached on 64-row blocks.
 BWD_TOPK_LIMIT = {128: 33664, 64: 46340}
 BWD_MAX_NBLK = 65535
+# The 16-bit forwards' limit (tdb200_sla_attn16_fwd and _fwd_lse, sla_attn.cu launch()): 1024 (alignment) + Lay::kOffLut +
+# round16(2 topk) (uint16 ids) + 4 topk (a k_scale copy the 16-bit kernels do not read) <= 227 KB = 232448.
+# Lay<128, true, BQ, 64>: Q BQ*256 | 3 K + 3 V stages of 16384 | KVW 32768 | 256 B of barriers (the lse forward reserves KVW too).
+#   (128, 64)  32768 + 98304 + 32768 + 256 = 164096;  232448 - 1024 - 164096 = 67328 = round16(22440) + 44880
+#              = 22448 + 44880: topk 11220 fits exactly; 11221 needs round16(22442) + 44884 = 67332 > 67328.
+#   (64, 64)   16384 + 98304 + 32768 + 256 = 147712;  232448 - 1024 - 147712 = 83712 = round16(27904) + 55808
+#              = 27904 + 55808: topk 13952 fits exactly; 13953 needs round16(27906) + 55812 = 83732 > 83712.
+FWD_TOPK_LIMIT = {128: 11220, 64: 13952}
+
+
+def _fwd_at(lib, fn, blkq, topk):
+    """A forward call (fn: _fwd or _fwd_lse) at b = 1, L = 64 topk: every key block selected."""
+    return fn(lib, topk=topk, l=64 * topk, blkq=blkq)
 
 
 def _bwd_at(lib, blkq, topk, nblk=None, ws_bytes=None):
@@ -96,6 +109,10 @@ def test_argument_validation(lib):
               ("bwd q64 topk limit + 1", lambda: _bwd_at(lib, 64, BWD_TOPK_LIMIT[64] + 1), UNSUPPORTED, b"dimension too large"),
               ("bwd q64 LUT bound + 1", lambda: _bwd_at(lib, 64, 50049), UNSUPPORTED, b"dimension too large")]
     for blkq in (128, 64):
+        cases += [(f"fwd q{blkq} topk limit + 1", lambda q=blkq: _fwd_at(lib, _fwd, q, FWD_TOPK_LIMIT[q] + 1), UNSUPPORTED,
+                   b"on-chip LUT"),
+                  (f"lse q{blkq} topk limit + 1", lambda q=blkq: _fwd_at(lib, _fwd_lse, q, FWD_TOPK_LIMIT[q] + 1), UNSUPPORTED,
+                   b"on-chip LUT")]
         cases.append((f"bwd q{blkq} nblk 65536", lambda q=blkq: _bwd_at(lib, q, 4, nblk=BWD_MAX_NBLK + 1, ws_bytes=1 << 40),
                       UNSUPPORTED, b"dimension too large"))
     for name, call, code, needle in cases:
@@ -106,12 +123,15 @@ def test_argument_validation(lib):
 
 
 def test_valid_calls_pass_validation(lib):
-    """Well-formed (64, 64) calls, with exactly the queried workspace, get past validation: on a host without a GPU they stop
-    at the device check."""
+    """Well-formed (64, 64) calls, with exactly the queried workspace, and the forwards at their largest top-k on both block
+    heights, get past validation: on a host without a GPU they stop at the device check."""
     if torch.cuda.is_available():
         pytest.skip("this check is for hosts without a GPU")
-    for call in (lambda: _fwd(lib, feature=2), lambda: _fwd_lse(lib),
-                 lambda: _bwd(lib, ws_bytes=lib.tdb200_sla_attn16_bwd_workspace_bytes(1, 2, 256, 4, BQ))):
+    calls = [lambda: _fwd(lib, feature=2), lambda: _fwd_lse(lib),
+             lambda: _bwd(lib, ws_bytes=lib.tdb200_sla_attn16_bwd_workspace_bytes(1, 2, 256, 4, BQ))]
+    for blkq, topk in FWD_TOPK_LIMIT.items():     # the forwards' largest top-k (one more is refused, test_argument_validation)
+        calls += [lambda q=blkq, t=topk: _fwd_at(lib, _fwd, q, t), lambda q=blkq, t=topk: _fwd_at(lib, _fwd_lse, q, t)]
+    for call in calls:
         assert call() in (-3, -4) and lib.tdb200_last_error()
 
 

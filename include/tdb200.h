@@ -350,6 +350,39 @@ int tdb200_attn_dense_fwd(const void* q, const void* k, const void* v, int dtype
                           int64_t h, int64_t d, float sm_scale, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * f1 key lengths. Key-padding masks as per-sample key lengths (a batched text cross-attention whose prompts tokenise to different
+ * lengths): each entry point of the f1 family has a twin, suffixed _kl, that takes k_lens right after lk and is otherwise the
+ * same call.
+ *   k_lens [b] int32, device memory, 4-byte aligned: batch entry i attends to keys 0 .. lk_i - 1 of its own [lk, h, d] slab,
+ *   lk_i = min(max(k_lens[i], 0), lk).  The values are device data and are clamped by the kernels, never read by the host.
+ * Batch entry i computes the bits the entry point without _kl computes on entry i alone with k and v (and k_t, v_t) cut to
+ * their first lk_i rows: its key tiles past lk_i are neither loaded nor visited, columns >= lk_i are masked, and in the tile
+ * that straddles lk_i the rows >= lk_i of k, v (and k_t, v_t) are zeroed in shared memory after the load, as the load's zero
+ * fill past lk would be.  So what those rows hold in memory, inf and NaN included, never reaches a result.  An entry with lk_i = 0 has no keys: out = 0, out_t = 0 and lse = +inf (the
+ * convention of rows >= lq), so its dq is 0.  The backward stores dk = dv = 0 in rows lk_i .. lk - 1.
+ *   tdb200_attn_dense_fwd_kl, tdb200_attn_dense_fwd_lse_kl, tdb200_attn_dense_jvp_kl, tdb200_attn_dense_jvp_lse_kl,
+ *   tdb200_attn_dense_tangent_kl, tdb200_attn_dense_bwd_kl (its workspace: tdb200_attn_dense_bwd_workspace_bytes).
+ * Errors: those of the twin without _kl, plus k_lens null or not 4-byte aligned -> TDB200_ERR_INVALID_ARG, all before any CUDA
+ * call.  Launches, synchronisation and graph capture as the twin without _kl.
+ * ------------------------------------------------------------------------------------------- */
+int tdb200_attn_dense_fwd_kl(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq, int64_t lk,
+                             const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream);
+int tdb200_attn_dense_fwd_lse_kl(const void* q, const void* k, const void* v, int dtype, void* out, float* lse, int64_t b,
+                                 int64_t lq, int64_t lk, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream);
+int tdb200_attn_dense_jvp_kl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                             int dtype, void* out, void* out_t, int64_t b, int64_t lq, int64_t lk, const int32_t* k_lens, int64_t h,
+                             int64_t d, float sm_scale, void* stream);
+int tdb200_attn_dense_jvp_lse_kl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                                 int dtype, void* out, void* out_t, float* lse, int64_t b, int64_t lq, int64_t lk,
+                                 const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream);
+int tdb200_attn_dense_tangent_kl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                                 const void* out, const float* lse, int dtype, void* out_t, int64_t b, int64_t lq, int64_t lk,
+                                 const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream);
+int tdb200_attn_dense_bwd_kl(const void* q, const void* k, const void* v, const void* out, const void* d_out, const float* lse,
+                             int dtype, void* dq, void* dk, void* dv, void* workspace, int64_t workspace_bytes, int64_t b, int64_t lq,
+                             int64_t lk, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * f1 JVP. Forward-mode derivative of the dense attention above (rCM distillation's tangent pass, reference
  * turbodiffusion/rcm/networks/wan2pt1_jvp.py): the attention output and its tangent for tangents q_t, k_t, v_t, in one kernel.
  *   S = sm_scale q.k^T,  S_t = sm_scale (q_t.k^T + q.k_t^T),  P = softmax(S),  out = T(P.v)

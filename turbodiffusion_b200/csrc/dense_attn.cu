@@ -46,11 +46,15 @@ struct DenseParams {
   float* lse;   // [b, h, lq] fp32, log2 domain (kLse only)
   int lq, lk, h;
   float sm_scale;
+  const int32_t* k_lens = nullptr;   // [b] int32 (kKeyLens only)
 };
 
 // kLse: also lse[b, h, row] = m_used + log2(l), the row log-sum-exp of the scores in the log2 domain with m_used the maximum the
 // lazy rescale last used (tdb200_sla_attn16_fwd_lse's convention), for the backward (sla_attn_bwd.cu) to recompute P from.
-template <typename T, bool kLse>
+// kKeyLens: batch entry b attends to its first lk_b = keys_of(k_lens, lk, b) keys only; tiles past them are neither loaded nor
+// visited, the last tile's rows past them are zeroed (zero_key_rows), and a row with no keys (lk_b = 0) stores out = 0 and
+// lse = +inf, the convention of rows past lq.
+template <typename T, bool kLse, bool kKeyLens = false>
 __global__ void __launch_bounds__(split::kThreads, 1)
 dense_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                       const __grid_constant__ CUtensorMap tmap_v, DenseParams p) {
@@ -61,7 +65,8 @@ dense_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
-  const int n_tiles = (p.lk + BK - 1) / BK;
+  const int lk = keys_of<kKeyLens>(p.k_lens, p.lk, b);
+  const int n_tiles = (lk + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
     mbar_init(&bars[kQFull], 1);
@@ -124,10 +129,18 @@ dense_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
 
     float s[BK / 2];
     mbar_wait(&bars[kKFull + st], ph);
+    if constexpr (kKeyLens)
+      if (lk - j * BK < BK && lk < p.lk) {   // the last tile, with rows past the entry's keys inside the buffer
+        mbar_wait(&bars[kVFull + st], ph);
+        zero_key_rows(smem + kOffK + st * kTileBytes, BK, HD / 64, lk - j * BK, threadIdx.x);
+        zero_key_rows(smem + kOffV + st * kTileBytes, BK, HD / 64, lk - j * BK, threadIdx.x);
+        fence_proxy_async_smem();
+        named_bar_sync(1, kConsumerWarps * 32);
+      }
     score_tile<true, HD, BK, kBF16>(s, sbase + kOffQ + wg * (64 * 128), BQ * 128, sbase + kOffK + st * kTileBytes, sc);
     warp_release(&bars[kKEmpty + st], lane);
     uint32_t pa[BK / 16][4];
-    softmax_step<T, HD, BK>(s, o, m_used, l_part, pa, p.lk - j * BK, cq, j == 0);   // valid < BK only in the ragged last tile
+    softmax_step<T, HD, BK>(s, o, m_used, l_part, pa, lk - j * BK, cq, j == 0);   // valid < BK only in the ragged last tile
     mbar_wait(&bars[kVFull + st], ph);
     pv_step<HD, BK, kBF16>(o, pa, sbase + kOffV + st * kTileBytes);
     warp_release(&bars[kVEmpty + st], lane);
@@ -138,16 +151,17 @@ dense_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     const float l_tot = quad_sum(l_part[h]);   // all four lanes of a row take part, stored or not
     const int64_t qr = int64_t(m_blk) * BQ + r_lo + 8 * h;
     if (qr >= p.lq) continue;
+    const bool empty = kKeyLens && lk == 0;   // o = 0 and l = 0: store 0 * 0 and lse = +inf
     if constexpr (kLse)
-      if (cq == 0) p.lse[(int64_t(b) * p.h + hh) * p.lq + qr] = m_used[h] + __log2f(l_tot);
-    store_o_row<T, HD>(static_cast<T*>(p.out) + ((int64_t(b) * p.lq + qr) * p.h + hh) * HD, o, h, 1.0f / l_tot, cq);
+      if (cq == 0) p.lse[(int64_t(b) * p.h + hh) * p.lq + qr] = empty ? INFINITY : m_used[h] + __log2f(l_tot);
+    store_o_row<T, HD>(static_cast<T*>(p.out) + ((int64_t(b) * p.lq + qr) * p.h + hh) * HD, o, h, empty ? 0.f : 1.0f / l_tot, cq);
   }
 }
 
-template <typename T, bool kLse>
+template <typename T, bool kLse, bool kKeyLens>
 int launch(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const DenseParams& p, dim3 grid, cudaStream_t st) {
   static bool smem_set[64];
-  const auto kern = dense_attn_fwd_kernel<T, kLse>;
+  const auto kern = dense_attn_fwd_kernel<T, kLse, kKeyLens>;
   if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), kSmemBytes, smem_set, "cudaFuncSetAttribute(dense_attn)"))
     return rc;
   kern<<<grid, split::kThreads, kSmemBytes, st>>>(tq, tk, tv, p);
@@ -199,6 +213,7 @@ struct Params {
   float sm_scale;
   const int32_t* lut;   // [b, h, mblk, topk] key-block ids (kSparse only)
   int topk, mblk;
+  const int32_t* k_lens = nullptr;   // [b] int32 (kKeyLens only)
 };
 
 // d (+)= Q.K^T over one 64-key tile: Q rows at sq (HD/64 chunks kQBytes/2 apart), K at sk (chunks BK * 128 bytes apart)
@@ -255,8 +270,9 @@ __device__ __forceinline__ void softmax_step_jvp(float (&s)[BK / 2], float (&o)[
   }
 }
 
-// kLse: also the row lse of the primal, as dense_attn_fwd_kernel<T, true> stores it
-template <typename T, bool kLse, bool kSparse = false>
+// kLse: also the row lse of the primal, as dense_attn_fwd_kernel<T, true> stores it.  kKeyLens (dense only): the forward's, so
+// a row with no keys also stores out_t = 0, and the ragged last tile's rows past the entry's keys (K, K_t, V and V_t) are zeroed.
+template <typename T, bool kLse, bool kSparse = false, bool kKeyLens = false>
 __global__ void __launch_bounds__(split::kThreads, 1)
 dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                       const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_qt,
@@ -269,7 +285,8 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
-  const int n_tiles = kSparse ? p.topk : (p.lk + BK - 1) / BK;
+  const int lk = keys_of<kKeyLens>(p.k_lens, p.lk, b);
+  const int n_tiles = kSparse ? p.topk : (lk + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
     mbar_init(&bars[kQFull], 1);
@@ -350,8 +367,18 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
 
     float s[BK / 2], sd[BK / 2];
     mbar_wait(&bars[kKFull + st], ph);
+    if constexpr (kKeyLens)
+      if (lk - j * BK < BK && lk < p.lk) {   // the last tile, with rows past the entry's keys inside the buffer
+        mbar_wait(&bars[kVFull + st], ph);
+        uint8_t* const tiles[4] = {smem + kOffK + st * kStageBytes, smem + kOffK + st * kStageBytes + kHalfBytes,
+                                   smem + kOffV + st * kStageBytes, smem + kOffV + st * kStageBytes + kHalfBytes};
+#pragma unroll
+        for (uint8_t* t : tiles) zero_key_rows(t, BK, HD / 64, lk - j * BK, threadIdx.x);
+        fence_proxy_async_smem();
+        named_bar_sync(1, kConsumerWarps * 32);
+      }
     score_tile<true, HD, BK, kBF16>(s, sq, BQ * 128, sk, sc);
-    softmax_step_jvp<!kBF16>(s, o, a, m_used, m_run, l_part, mu_part, p.lk - (kSparse ? s_lut[j] : j) * BK, cq,
+    softmax_step_jvp<!kBF16>(s, o, a, m_used, m_run, l_part, mu_part, lk - (kSparse ? s_lut[j] : j) * BK, cq,
                              j == 0);   // s := p
 #pragma unroll
     for (int i = 0; i < BK / 2; ++i) sd[i] = 0.f;
@@ -434,9 +461,10 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     const int64_t qr = int64_t(m_blk) * BQ + r_lo + 8 * h;
     if (qr >= p.lq) continue;
     const int64_t row = ((int64_t(b) * p.lq + qr) * p.h + hh) * HD;
+    const bool empty = kKeyLens && lk == 0;   // o = a = 0 and l = mu = 0: store zeros and lse = +inf
     if constexpr (kLse)
-      if (cq == 0) p.lse[(int64_t(b) * p.h + hh) * p.lq + qr] = m_used[h] + __log2f(l_tot);
-    const float inv_l = 1.0f / l_tot, mu_l = mu_tot * inv_l;
+      if (cq == 0) p.lse[(int64_t(b) * p.h + hh) * p.lq + qr] = empty ? INFINITY : m_used[h] + __log2f(l_tot);
+    const float inv_l = empty ? 0.f : 1.0f / l_tot, mu_l = mu_tot * inv_l;
     store_o_row<T, HD>(static_cast<T*>(p.out) + row, o, h, inv_l, cq);
     T* trow = static_cast<T*>(p.out_t) + row;
 #pragma unroll
@@ -448,10 +476,10 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   }
 }
 
-template <typename T, bool kLse>
+template <typename T, bool kLse, bool kKeyLens>
 int launch(const CUtensorMap (&tm)[6], const Params& p, dim3 grid, cudaStream_t st) {
   static bool smem_set[64];
-  const auto kern = dense_attn_jvp_kernel<T, kLse>;
+  const auto kern = dense_attn_jvp_kernel<T, kLse, false, kKeyLens>;
   if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), kSmemBytes, smem_set, "cudaFuncSetAttribute(dense_attn_jvp)"))
     return rc;
   kern<<<grid, split::kThreads, kSmemBytes, st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p);
@@ -480,8 +508,10 @@ int launch_sparse(const CUtensorMap (&tm)[6], const Params& p, dim3 grid, cudaSt
 // term, which saves the product O = P.V.  Five products per tile against the JVP kernel's six; warp roles, shared memory,
 // the rings and kSparse as dense_attn_jvp_kernel's.  Query rows >= lq read no lse and store nothing (their P is 0).
 // p.out and p.lse are inputs here.  The set-up and the producer are dense_attn_jvp_kernel's, written out again: moved into a
-// shared function they changed that kernel's register allocation.
-template <typename T, bool kSparse>
+// shared function they changed that kernel's register allocation.  kKeyLens (dense only): tiles past k_lens[b] are neither
+// loaded nor visited, the last tile's rows past them are zeroed as in dense_attn_jvp_kernel, and a row with no keys has A = 0
+// and mu = 0, so it stores out_t = 0.
+template <typename T, bool kSparse, bool kKeyLens = false>
 __global__ void __launch_bounds__(split::kThreads, 1)
 attn_tangent_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                     const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_qt,
@@ -494,7 +524,8 @@ attn_tangent_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
-  const int n_tiles = kSparse ? p.topk : (p.lk + BK - 1) / BK;
+  const int lk = keys_of<kKeyLens>(p.k_lens, p.lk, b);
+  const int n_tiles = kSparse ? p.topk : (lk + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
     mbar_init(&bars[kQFull], 1);
@@ -580,8 +611,18 @@ attn_tangent_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 
     float s[BK / 2], sd[BK / 2];
     mbar_wait(&bars[kKFull + st], ph);
+    if constexpr (kKeyLens)
+      if (lk - j * BK < BK && lk < p.lk) {   // the last tile, with rows past the entry's keys inside the buffer
+        mbar_wait(&bars[kVFull + st], ph);
+        uint8_t* const tiles[4] = {smem + kOffK + st * kStageBytes, smem + kOffK + st * kStageBytes + kHalfBytes,
+                                   smem + kOffV + st * kStageBytes, smem + kOffV + st * kStageBytes + kHalfBytes};
+#pragma unroll
+        for (uint8_t* t : tiles) zero_key_rows(t, BK, HD / 64, lk - j * BK, threadIdx.x);
+        fence_proxy_async_smem();
+        named_bar_sync(1, kConsumerWarps * 32);
+      }
     score_tile<true, HD, BK, kBF16>(s, sq, BQ * 128, sk, sc);
-    const int valid = p.lk - (kSparse ? s_lut[j] : j) * BK;
+    const int valid = lk - (kSparse ? s_lut[j] : j) * BK;
 #pragma unroll
     for (int i = 0; i < BK / 2; ++i) {
       const float x = s[i] - lse[(i >> 1) & 1];
@@ -644,10 +685,10 @@ attn_tangent_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 }
 
 // kSparse: the dynamic shared memory grows by the LUT row, as for launch_sparse
-template <typename T, bool kSparse>
+template <typename T, bool kSparse, bool kKeyLens = false>
 int launch_tangent(const CUtensorMap (&tm)[6], const Params& p, dim3 grid, cudaStream_t st) {
   static bool smem_set[64];
-  const auto kern = attn_tangent_kernel<T, kSparse>;
+  const auto kern = attn_tangent_kernel<T, kSparse, kKeyLens>;
   const size_t smem_max = kSparse ? kSparseSmemMax : kSmemBytes;
   if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), smem_max, smem_set,
                                          kSparse ? "cudaFuncSetAttribute(sla_attn16_tangent)" : "cudaFuncSetAttribute(attn_dense_tangent)"))
@@ -668,14 +709,18 @@ int tmap16(CUtensorMap* m, const void* base, int dtype, int64_t b, int64_t l, in
 
 bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
 
-// tdb200_attn_dense_fwd (lse null) and tdb200_attn_dense_fwd_lse; `what` prefixes the messages
+// tdb200_attn_dense_fwd (lse null) and tdb200_attn_dense_fwd_lse; `what` prefixes the messages.  key_lens: their _kl twins,
+// which take k_lens [b] and launch the kKeyLens kernels.
 int dense_fwd(const char* what, const void* q, const void* k, const void* v, int dtype, void* out, float* lse, bool with_lse,
-              int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  if (!q || !k || !v || !out || (with_lse && !lse)) return fail(TDB200_ERR_INVALID_ARG, "%s: null pointer", what);
+              int64_t b, int64_t lq, int64_t lk, const int32_t* k_lens, bool key_lens, int64_t h, int64_t d, float sm_scale,
+              void* stream) {
+  if (!q || !k || !v || !out || (with_lse && !lse) || (key_lens && !k_lens))
+    return fail(TDB200_ERR_INVALID_ARG, "%s: null pointer", what);
   if (int rc = dense_attn_shape(what, b, lq, lk, h, d)) return rc;
   if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out))
     return fail(TDB200_ERR_INVALID_ARG, "%s: q, k, v and out must be 16-byte aligned", what);
   if (with_lse && !aligned4(lse)) return fail(TDB200_ERR_INVALID_ARG, "%s: lse must be 4-byte aligned", what);
+  if (key_lens && !aligned4(k_lens)) return fail(TDB200_ERR_INVALID_ARG, "%s: k_lens must be 4-byte aligned", what);
   if (int rc = dense_attn_limits(what, dtype, b, lq, lk, h, d)) return rc;
   if (int rc = require_sm90()) return rc;
 
@@ -690,24 +735,33 @@ int dense_fwd(const char* what, const void* q, const void* k, const void* v, int
   p.lk = int(lk);
   p.h = int(h);
   p.sm_scale = sm_scale;
+  p.k_lens = k_lens;
   const dim3 grid(static_cast<unsigned>(cdiv64(lq, BQ)), static_cast<unsigned>(h), static_cast<unsigned>(b));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool bf16 = dtype == TDB200_DTYPE_BF16;
-  if (!with_lse) return bf16 ? launch<__nv_bfloat16, false>(tq, tk, tv, p, grid, st) : launch<__half, false>(tq, tk, tv, p, grid, st);
-  return bf16 ? launch<__nv_bfloat16, true>(tq, tk, tv, p, grid, st) : launch<__half, true>(tq, tk, tv, p, grid, st);
+  if (!key_lens) {
+    if (!with_lse)
+      return bf16 ? launch<__nv_bfloat16, false, false>(tq, tk, tv, p, grid, st) : launch<__half, false, false>(tq, tk, tv, p, grid, st);
+    return bf16 ? launch<__nv_bfloat16, true, false>(tq, tk, tv, p, grid, st) : launch<__half, true, false>(tq, tk, tv, p, grid, st);
+  }
+  if (!with_lse)
+    return bf16 ? launch<__nv_bfloat16, false, true>(tq, tk, tv, p, grid, st) : launch<__half, false, true>(tq, tk, tv, p, grid, st);
+  return bf16 ? launch<__nv_bfloat16, true, true>(tq, tk, tv, p, grid, st) : launch<__half, true, true>(tq, tk, tv, p, grid, st);
 }
 
-// tdb200_attn_dense_jvp (lse null), tdb200_attn_dense_jvp_lse and, `tangent`, tdb200_attn_dense_tangent (out and lse inputs)
+// tdb200_attn_dense_jvp (lse null), tdb200_attn_dense_jvp_lse and, `tangent`, tdb200_attn_dense_tangent (out and lse inputs);
+// key_lens: their _kl twins, as for dense_fwd
 int dense_jvp(const char* what, const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
-              int dtype, void* out, void* out_t, float* lse, bool with_lse, int64_t b, int64_t lq, int64_t lk, int64_t h, int64_t d,
-              float sm_scale, void* stream, bool tangent = false) {
-  if (!q || !k || !v || !q_t || !k_t || !v_t || !out || !out_t || (with_lse && !lse))
+              int dtype, void* out, void* out_t, float* lse, bool with_lse, int64_t b, int64_t lq, int64_t lk, const int32_t* k_lens,
+              bool key_lens, int64_t h, int64_t d, float sm_scale, void* stream, bool tangent = false) {
+  if (!q || !k || !v || !q_t || !k_t || !v_t || !out || !out_t || (with_lse && !lse) || (key_lens && !k_lens))
     return fail(TDB200_ERR_INVALID_ARG, "%s: null pointer", what);
   if (int rc = dense_attn_shape(what, b, lq, lk, h, d)) return rc;
   if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(q_t) || !aligned16(k_t) || !aligned16(v_t) ||
       !aligned16(out) || !aligned16(out_t))
     return fail(TDB200_ERR_INVALID_ARG, "%s: q, k, v, their tangents, out and out_t must be 16-byte aligned", what);
   if (with_lse && !aligned4(lse)) return fail(TDB200_ERR_INVALID_ARG, "%s: lse must be 4-byte aligned", what);
+  if (key_lens && !aligned4(k_lens)) return fail(TDB200_ERR_INVALID_ARG, "%s: k_lens must be 4-byte aligned", what);
   if (int rc = dense_attn_limits(what, dtype, b, lq, lk, h, d)) return rc;
   if (int rc = require_sm90()) return rc;
 
@@ -726,13 +780,23 @@ int dense_jvp(const char* what, const void* q, const void* k, const void* v, con
   p.lk = int(lk);
   p.h = int(h);
   p.sm_scale = sm_scale;
+  p.k_lens = k_lens;
   const dim3 grid(static_cast<unsigned>(cdiv64(lq, BQ)), static_cast<unsigned>(h), static_cast<unsigned>(b));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool bf16 = dtype == TDB200_DTYPE_BF16;
+  if (!key_lens) {
+    if (tangent)
+      return bf16 ? jvp::launch_tangent<__nv_bfloat16, false>(tm, p, grid, st) : jvp::launch_tangent<__half, false>(tm, p, grid, st);
+    if (!with_lse)
+      return bf16 ? jvp::launch<__nv_bfloat16, false, false>(tm, p, grid, st) : jvp::launch<__half, false, false>(tm, p, grid, st);
+    return bf16 ? jvp::launch<__nv_bfloat16, true, false>(tm, p, grid, st) : jvp::launch<__half, true, false>(tm, p, grid, st);
+  }
   if (tangent)
-    return bf16 ? jvp::launch_tangent<__nv_bfloat16, false>(tm, p, grid, st) : jvp::launch_tangent<__half, false>(tm, p, grid, st);
-  if (!with_lse) return bf16 ? jvp::launch<__nv_bfloat16, false>(tm, p, grid, st) : jvp::launch<__half, false>(tm, p, grid, st);
-  return bf16 ? jvp::launch<__nv_bfloat16, true>(tm, p, grid, st) : jvp::launch<__half, true>(tm, p, grid, st);
+    return bf16 ? jvp::launch_tangent<__nv_bfloat16, false, true>(tm, p, grid, st)
+                : jvp::launch_tangent<__half, false, true>(tm, p, grid, st);
+  if (!with_lse)
+    return bf16 ? jvp::launch<__nv_bfloat16, false, true>(tm, p, grid, st) : jvp::launch<__half, false, true>(tm, p, grid, st);
+  return bf16 ? jvp::launch<__nv_bfloat16, true, true>(tm, p, grid, st) : jvp::launch<__half, true, true>(tm, p, grid, st);
 }
 
 // tdb200_sla_attn16_jvp (lse null) and tdb200_sla_attn16_jvp_lse: the JVP kernel over the LUT's key blocks, lq = lk = l;
@@ -791,24 +855,26 @@ int sla_jvp(const char* what, const void* q, const void* k, const void* v, const
 
 extern "C" int tdb200_attn_dense_fwd(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq,
                                      int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  return dense_fwd("attn_dense_fwd", q, k, v, dtype, out, nullptr, false, b, lq, lk, h, d, sm_scale, stream);
+  return dense_fwd("attn_dense_fwd", q, k, v, dtype, out, nullptr, false, b, lq, lk, nullptr, false, h, d, sm_scale, stream);
 }
 
 extern "C" int tdb200_attn_dense_fwd_lse(const void* q, const void* k, const void* v, int dtype, void* out, float* lse, int64_t b,
                                          int64_t lq, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  return dense_fwd("attn_dense_fwd_lse", q, k, v, dtype, out, lse, true, b, lq, lk, h, d, sm_scale, stream);
+  return dense_fwd("attn_dense_fwd_lse", q, k, v, dtype, out, lse, true, b, lq, lk, nullptr, false, h, d, sm_scale, stream);
 }
 
 extern "C" int tdb200_attn_dense_jvp(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
                                      const void* v_t, int dtype, void* out, void* out_t, int64_t b, int64_t lq, int64_t lk,
                                      int64_t h, int64_t d, float sm_scale, void* stream) {
-  return dense_jvp("attn_dense_jvp", q, k, v, q_t, k_t, v_t, dtype, out, out_t, nullptr, false, b, lq, lk, h, d, sm_scale, stream);
+  return dense_jvp("attn_dense_jvp", q, k, v, q_t, k_t, v_t, dtype, out, out_t, nullptr, false, b, lq, lk, nullptr, false, h, d,
+                   sm_scale, stream);
 }
 
 extern "C" int tdb200_attn_dense_jvp_lse(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
                                          const void* v_t, int dtype, void* out, void* out_t, float* lse, int64_t b, int64_t lq,
                                          int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  return dense_jvp("attn_dense_jvp_lse", q, k, v, q_t, k_t, v_t, dtype, out, out_t, lse, true, b, lq, lk, h, d, sm_scale, stream);
+  return dense_jvp("attn_dense_jvp_lse", q, k, v, q_t, k_t, v_t, dtype, out, out_t, lse, true, b, lq, lk, nullptr, false, h, d,
+                   sm_scale, stream);
 }
 
 extern "C" int tdb200_sla_attn16_jvp(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
@@ -830,7 +896,7 @@ extern "C" int tdb200_attn_dense_tangent(const void* q, const void* k, const voi
                                          const void* v_t, const void* out, const float* lse, int dtype, void* out_t, int64_t b,
                                          int64_t lq, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
   return dense_jvp("attn_dense_tangent", q, k, v, q_t, k_t, v_t, dtype, const_cast<void*>(out), out_t, const_cast<float*>(lse), true,
-                   b, lq, lk, h, d, sm_scale, stream, true);
+                   b, lq, lk, nullptr, false, h, d, sm_scale, stream, true);
 }
 
 extern "C" int tdb200_sla_attn16_tangent(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
@@ -839,4 +905,39 @@ extern "C" int tdb200_sla_attn16_tangent(const void* q, const void* k, const voi
                                          int64_t blkq, int64_t blkk, void* stream) {
   return sla_jvp("sla_attn16_tangent", q, k, v, q_t, k_t, v_t, dtype, lut, topk, const_cast<void*>(o_s), o_s_t, const_cast<float*>(lse),
                  true, b, l, h, d, sm_scale, blkq, blkk, stream, true);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// The _kl twins: the entry points above with per-sample key lengths k_lens [b] (the kKeyLens kernels)
+extern "C" int tdb200_attn_dense_fwd_kl(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq,
+                                        int64_t lk, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream) {
+  return dense_fwd("attn_dense_fwd_kl", q, k, v, dtype, out, nullptr, false, b, lq, lk, k_lens, true, h, d, sm_scale, stream);
+}
+
+extern "C" int tdb200_attn_dense_fwd_lse_kl(const void* q, const void* k, const void* v, int dtype, void* out, float* lse, int64_t b,
+                                            int64_t lq, int64_t lk, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale,
+                                            void* stream) {
+  return dense_fwd("attn_dense_fwd_lse_kl", q, k, v, dtype, out, lse, true, b, lq, lk, k_lens, true, h, d, sm_scale, stream);
+}
+
+extern "C" int tdb200_attn_dense_jvp_kl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
+                                        const void* v_t, int dtype, void* out, void* out_t, int64_t b, int64_t lq, int64_t lk,
+                                        const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream) {
+  return dense_jvp("attn_dense_jvp_kl", q, k, v, q_t, k_t, v_t, dtype, out, out_t, nullptr, false, b, lq, lk, k_lens, true, h, d,
+                   sm_scale, stream);
+}
+
+extern "C" int tdb200_attn_dense_jvp_lse_kl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
+                                            const void* v_t, int dtype, void* out, void* out_t, float* lse, int64_t b, int64_t lq,
+                                            int64_t lk, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream) {
+  return dense_jvp("attn_dense_jvp_lse_kl", q, k, v, q_t, k_t, v_t, dtype, out, out_t, lse, true, b, lq, lk, k_lens, true, h, d,
+                   sm_scale, stream);
+}
+
+extern "C" int tdb200_attn_dense_tangent_kl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
+                                            const void* v_t, const void* out, const float* lse, int dtype, void* out_t, int64_t b,
+                                            int64_t lq, int64_t lk, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale,
+                                            void* stream) {
+  return dense_jvp("attn_dense_tangent_kl", q, k, v, q_t, k_t, v_t, dtype, const_cast<void*>(out), out_t, const_cast<float*>(lse),
+                   true, b, lq, lk, k_lens, true, h, d, sm_scale, stream, true);
 }

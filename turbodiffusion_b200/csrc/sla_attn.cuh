@@ -22,6 +22,28 @@ __device__ __forceinline__ void warp_release(uint64_t* empty, int lane) {
   if (lane == 0) mbar_arrive(empty);
 }
 
+// The keys batch entry b of a dense attention kernel attends to: lk, or (kKeyLens, the _kl entry points) k_lens[b] clamped to
+// [0, lk].  Read once per CTA before its first barrier, so that the producer and the consumers derive the same tile count.
+template <bool kKeyLens>
+__device__ __forceinline__ int keys_of(const int32_t* k_lens, int lk, int b) {
+  if constexpr (kKeyLens) return min(max(__ldg(k_lens + b), 0), lk);
+  return lk;
+}
+
+// kKeyLens: key rows [valid, rows) of a streamed tile lie past the entry's keys but inside the buffer, so TMA loaded whatever
+// memory holds there rather than zero fill.  Their score columns are masked, but an MMA multiplies the masked zeros by the
+// rows themselves (P.V, the tangent's S_t = q_t.k^T + q.k_t^T, dP = dO.V^T, dS.K), and 0 * inf is NaN: so the consumers zero
+// those rows, as TMA's zero fill would.  Whole 128-byte rows: the 128-byte swizzle permutes 16-byte units within a row.  A
+// tile of `chunks` column chunks of rows x 128 B at `tile`; the 256 consumer threads share the work (tid = threadIdx.x).
+// The caller then runs fence_proxy_async_smem() and a barrier over the consumers, before any MMA reads the tile.
+__device__ __forceinline__ void zero_key_rows(uint8_t* tile, int rows, int chunks, int valid, int tid) {
+  const int per_chunk = (rows - valid) * 8;   // 16-byte units
+  for (int e = tid; e < chunks * per_chunk; e += 256) {
+    const int c = e / per_chunk, u = e - c * per_chunk;
+    *reinterpret_cast<uint4*>(tile + c * rows * 128 + valid * 128 + u * 16) = make_uint4(0u, 0u, 0u, 0u);
+  }
+}
+
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kRescaleThreshold = 8.0f;  // log2 domain
 

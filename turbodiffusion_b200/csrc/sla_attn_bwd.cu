@@ -18,7 +18,10 @@
 // Dense attention (tdb200_attn_dense_bwd, the backward of dense_attn.cu's kLse forwards, lq != lk allowed) runs the delta
 // kernel and the 128-row dQ and dK/dV kernels with kDense: the dQ CTA visits every 64-key tile and the dK/dV CTA every 128-row
 // query block, in ascending order, with no LUT staging, no index read and no index kernel.  kDense is a compile-time choice
-// that only replaces where a block id comes from; the per-tile arithmetic is the same instructions.
+// that only replaces where a block id comes from; the per-tile arithmetic is the same instructions.  kKeyLens (with kDense,
+// tdb200_attn_dense_bwd_kl): batch entry b has lk_b = k_lens[b] keys; the dQ CTA visits tiles 0 .. ceil(lk_b / 64) - 1 with
+// columns >= lk_b masked and the last tile's K and V rows >= lk_b zeroed (zero_key_rows), a dK/dV CTA whose key block starts
+// at or past lk_b stores zeros, and rows >= lk_b of a block that straddles lk_b are stored as zeros.
 //
 // Rounding points (FlashAttention-2's): P and dS are formed in fp32 and rounded to T only as MMA operands; dQ, dK, dV accumulate
 // in fp32 registers and are rounded to T once.  No floating-point atomics: every output element is written by one thread in a
@@ -54,6 +57,7 @@ struct BwdParams {
   int h, mblk, nblk;       // mblk / nblk: query / key blocks
   int topk;                // key blocks per query block (dense: nblk)
   float sm_scale;
+  const int32_t* k_lens = nullptr;   // [b] int32 (kKeyLens only)
 };
 
 // ------------------------------------------------------------------------------------------------ preprocessing
@@ -213,7 +217,7 @@ constexpr uint32_t kOffBars = kOffV + kStages * kTileK, kOffLut = kOffBars + 256
 enum Bar { kQFull = 0, kKFull = 1, kKEmpty = 4, kVFull = 7, kVEmpty = 10 };
 }  // namespace dq
 
-template <typename T, bool kDense = false>
+template <typename T, bool kDense = false, bool kKeyLens = false>
 __global__ void __launch_bounds__(dq::kThreads, 1)
 sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
                   const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v, BwdParams p) {
@@ -226,6 +230,8 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
   const int bh = b * p.h + hh;
+  const int lk = keys_of<kKeyLens>(p.k_lens, p.lk, b);
+  const int n_tiles = kKeyLens ? (lk + BLKK - 1) / BLKK : p.topk;
 
   if (threadIdx.x == 0) {
     mbar_init(&bars[kQFull], 1);
@@ -256,7 +262,7 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
         tma_load_4d(smem + kOffQ + c * (BLKQ * 128), &tmap_q, &bars[kQFull], c * 64, hh, m_blk * BLKQ, b);
         tma_load_4d(smem + kOffDO + c * (BLKQ * 128), &tmap_do, &bars[kQFull], c * 64, hh, m_blk * BLKQ, b);
       }
-      for (int j = 0; j < p.topk; ++j) {
+      for (int j = 0; j < n_tiles; ++j) {
         const int st = j % kStages;
         const uint32_t ph = ((j / kStages) & 1) ^ 1;
         const int blk = kDense ? j : s_lut[j];
@@ -294,10 +300,10 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
   int ds_e[2] = {kDsUnset, kDsUnset};   // per query row (fp16)
 
   mbar_wait(&bars[kQFull], 0);
-  for (int j = 0; j < p.topk; ++j) {
+  for (int j = 0; j < n_tiles; ++j) {
     const int st = j % kStages;
     const uint32_t ph = (j / kStages) & 1;
-    const int valid = p.lk - (kDense ? j : s_lut[j]) * BLKK;
+    const int valid = lk - (kDense ? j : s_lut[j]) * BLKK;
     const uint32_t sk = sbase + kOffK + st * kTileK, sv = sbase + kOffV + st * kTileK;
 
     // ---- S = Q.K^T and dP = dO.V^T for this warpgroup's 64 rows (all operands K-major over d)
@@ -305,6 +311,14 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
 #pragma unroll
     for (int i = 0; i < 32; ++i) s[i] = dp[i] = 0.f;
     mbar_wait(&bars[kKFull + st], ph);
+    if constexpr (kKeyLens)
+      if (valid < BLKK && lk < p.lk) {   // the last tile, with rows past the entry's keys inside the buffer
+        mbar_wait(&bars[kVFull + st], ph);
+        zero_key_rows(smem + kOffK + st * kTileK, BLKK, HD / 64, valid, threadIdx.x);
+        zero_key_rows(smem + kOffV + st * kTileK, BLKK, HD / 64, valid, threadIdx.x);
+        fence_proxy_async_smem();
+        named_bar_sync(1, kConsumerWarps * 32);
+      }
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < HD / 16; ++ks) {
@@ -391,7 +405,7 @@ struct Dkv {
   static_assert(HD * 128 * 4 <= 2 * kStages * kTileQ, "partial dK / dV do not fit in the ring");
 };
 
-template <typename T, int kBQ, bool kDense = false>
+template <typename T, int kBQ, bool kDense = false, bool kKeyLens = false>
 __global__ void __launch_bounds__(split::kThreads, 1)
 sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
                     const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v, BwdParams p) {
@@ -411,6 +425,8 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     list = p.kv_idx + int64_t(bh) * p.mblk * p.topk + __ldg(kv_off + n_blk);
     n_list = __ldg(kv_off + n_blk + 1) - __ldg(kv_off + n_blk);
   }
+  const int lk = keys_of<kKeyLens>(p.k_lens, p.lk, b);
+  if (kKeyLens && n_blk * BLKK >= lk) n_list = 0;   // a key block past this entry's keys
 
   if (n_list == 0) {  // no query block selected this key block: its gradients are zero (the outputs are not pre-zeroed)
     for (int e = threadIdx.x; e < BLKK * HD / 8; e += split::kThreads) {
@@ -567,6 +583,16 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     dv[i] += x[HD / 2 + i];
   }
   const int64_t row0 = int64_t(n_blk) * BLKK + kr_lo;
+  if constexpr (kKeyLens) {
+    // key rows >= lk of the block that straddles lk saw keys the entry does not have: their rows are zero (assigned, not
+    // scaled, since such a row may hold inf or NaN from whatever its keys' memory holds)
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf)
+      if (row0 + 8 * hf >= lk) {
+#pragma unroll
+        for (int c = 0; c < HD / 8; ++c) dk[4 * c + 2 * hf] = dk[4 * c + 2 * hf + 1] = dv[4 * c + 2 * hf] = dv[4 * c + 2 * hf + 1] = 0.f;
+      }
+  }
   store_rows<T>(dk, p.sm_scale, p.dk, row0, p.lk, p.h, hh, b, cq);
   store_rows<T>(dv, 1.0f, p.dv, row0, p.lk, p.h, hh, b, cq);
 }
@@ -898,11 +924,12 @@ constexpr int64_t kMaxDenseRows = int64_t(8) * 0x7FFFFFFF;
 
 bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
 
-// delta kernel, then dQ over every key tile and dK / dV over every 128-row query block (no index kernel)
-template <typename T>
+// delta kernel, then dQ over every key tile and dK / dV over every 128-row query block (no index kernel); kKeyLens: over the
+// tiles and key blocks below k_lens[b]
+template <typename T, bool kKeyLens>
 int launch_dense_bwd(const void* q, const void* k, const void* v, const void* out, const void* d_out, const float* lse, void* dq,
-                     void* dk, void* dv, float* delta, int64_t b, int64_t lq, int64_t lk, int64_t h, float sm_scale,
-                     cudaStream_t st) {
+                     void* dk, void* dv, float* delta, int64_t b, int64_t lq, int64_t lk, const int32_t* k_lens, int64_t h,
+                     float sm_scale, cudaStream_t st) {
   const CUtensorMapDataType t16 = std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                                                         : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUtensorMap tq, tdo, tk, tv;
@@ -929,10 +956,11 @@ int launch_dense_bwd(const void* q, const void* k, const void* v, const void* ou
   p.nblk = int(cdiv64(lk, BLKK));
   p.topk = p.nblk;
   p.sm_scale = sm_scale;
+  p.k_lens = k_lens;
 
   static bool smem_set_dq[64], smem_set_kv[64];
-  const auto dq_kern = sla_bwd_dq_kernel<T, true>;
-  const auto dkdv_kern = sla_bwd_dkdv_kernel<T, BLKQ, true>;
+  const auto dq_kern = sla_bwd_dq_kernel<T, true, kKeyLens>;
+  const auto dkdv_kern = sla_bwd_dkdv_kernel<T, BLKQ, true, kKeyLens>;
   const size_t smem_dq = 1024 + dq::kOffLut, smem_kv = 1024 + Dkv<BLKQ>::kSmem;
   if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(dq_kern), smem_dq, smem_set_dq, "cudaFuncSetAttribute(dense_bwd_dq)"))
     return rc;
@@ -955,17 +983,20 @@ extern "C" int64_t tdb200_attn_dense_bwd_workspace_bytes(int64_t b, int64_t h, i
   return b * h * lq * int64_t(sizeof(float));
 }
 
-extern "C" int tdb200_attn_dense_bwd(const void* q, const void* k, const void* v, const void* out, const void* d_out, const float* lse,
-                                     int dtype, void* dq, void* dk, void* dv, void* workspace, int64_t workspace_bytes, int64_t b,
-                                     int64_t lq, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  const char* what = "attn_dense_bwd";
-  if (!q || !k || !v || !out || !d_out || !lse || !dq || !dk || !dv || !workspace)
+namespace {
+
+// tdb200_attn_dense_bwd and, key_lens, its _kl twin
+int dense_bwd(const char* what, const void* q, const void* k, const void* v, const void* out, const void* d_out, const float* lse,
+              int dtype, void* dq, void* dk, void* dv, void* workspace, int64_t workspace_bytes, int64_t b, int64_t lq, int64_t lk,
+              const int32_t* k_lens, bool key_lens, int64_t h, int64_t d, float sm_scale, void* stream) {
+  if (!q || !k || !v || !out || !d_out || !lse || !dq || !dk || !dv || !workspace || (key_lens && !k_lens))
     return fail(TDB200_ERR_INVALID_ARG, "%s: null pointer", what);
   if (int rc = dense_attn_shape(what, b, lq, lk, h, d)) return rc;
   if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out) || !aligned16(d_out) || !aligned16(dq) || !aligned16(dk) ||
       !aligned16(dv))
     return fail(TDB200_ERR_INVALID_ARG, "%s: q, k, v, out, d_out, dq, dk and dv must be 16-byte aligned", what);
   if (!aligned4(lse) || !aligned4(workspace)) return fail(TDB200_ERR_INVALID_ARG, "%s: lse and workspace must be 4-byte aligned", what);
+  if (key_lens && !aligned4(k_lens)) return fail(TDB200_ERR_INVALID_ARG, "%s: k_lens must be 4-byte aligned", what);
   if (int rc = dense_attn_limits(what, dtype, b, lq, lk, h, d)) return rc;
   if (b * lq * h > kMaxDenseRows)
     return fail(TDB200_ERR_UNSUPPORTED, "%s: dimension too large (b * lq * h above 8 * (2^31 - 1), the delta kernel's grid)", what);
@@ -980,7 +1011,29 @@ extern "C" int tdb200_attn_dense_bwd(const void* q, const void* k, const void* v
   if (int rc = check_cuda(cudaSetDevice(dev), "cudaSetDevice")) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   float* delta = static_cast<float*>(workspace);
+  if (!key_lens) {
+    if (dtype == TDB200_DTYPE_BF16)
+      return launch_dense_bwd<__nv_bfloat16, false>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, nullptr, h, sm_scale, st);
+    return launch_dense_bwd<__half, false>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, nullptr, h, sm_scale, st);
+  }
   if (dtype == TDB200_DTYPE_BF16)
-    return launch_dense_bwd<__nv_bfloat16>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, h, sm_scale, st);
-  return launch_dense_bwd<__half>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, h, sm_scale, st);
+    return launch_dense_bwd<__nv_bfloat16, true>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, k_lens, h, sm_scale, st);
+  return launch_dense_bwd<__half, true>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, k_lens, h, sm_scale, st);
+}
+
+}  // namespace
+
+extern "C" int tdb200_attn_dense_bwd(const void* q, const void* k, const void* v, const void* out, const void* d_out, const float* lse,
+                                     int dtype, void* dq, void* dk, void* dv, void* workspace, int64_t workspace_bytes, int64_t b,
+                                     int64_t lq, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
+  return dense_bwd("attn_dense_bwd", q, k, v, out, d_out, lse, dtype, dq, dk, dv, workspace, workspace_bytes, b, lq, lk, nullptr, false,
+                   h, d, sm_scale, stream);
+}
+
+extern "C" int tdb200_attn_dense_bwd_kl(const void* q, const void* k, const void* v, const void* out, const void* d_out,
+                                        const float* lse, int dtype, void* dq, void* dk, void* dv, void* workspace,
+                                        int64_t workspace_bytes, int64_t b, int64_t lq, int64_t lk, const int32_t* k_lens, int64_t h,
+                                        int64_t d, float sm_scale, void* stream) {
+  return dense_bwd("attn_dense_bwd_kl", q, k, v, out, d_out, lse, dtype, dq, dk, dv, workspace, workspace_bytes, b, lq, lk, k_lens,
+                   true, h, d, sm_scale, stream);
 }

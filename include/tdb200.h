@@ -334,7 +334,8 @@ int64_t tdb200_sla_attn_bwd_workspace_bytes(int64_t b, int64_t h, int64_t l, int
 /* ---------------------------------------------------------------------------------------------
  * f1. Dense softmax attention, forward only: the block's cross-attention over the text tokens and `--attention_type original`
  * (reference: the `attention` wrapper over FlashAttention / F.scaled_dot_product_attention, turbodiffusion/rcm/utils/attention.py:120-167,
- * without its dropout, causal, window and variable-length arguments, which the denoise path leaves at their defaults).
+ * without its dropout, causal and window arguments, which the denoise path leaves at their defaults; its variable-length
+ * arguments are the _kl (key lengths) and _vl (query and key lengths) twins below).
  *   out = T( softmax(q . k^T * sm_scale) . v )   per (batch, head)
  * q, out [b, lq, h, d] and k, v [b, lk, h, d], contiguous 16-bit of type `dtype`, 16-byte aligned, read and written in place
  * (row stride h*d: the [l, h*d] output of a projection GEMM is consumed as it is, no transposed copies).  lq and lk are
@@ -381,6 +382,46 @@ int tdb200_attn_dense_tangent_kl(const void* q, const void* k, const void* v, co
 int tdb200_attn_dense_bwd_kl(const void* q, const void* k, const void* v, const void* out, const void* d_out, const float* lse,
                              int dtype, void* dq, void* dk, void* dv, void* workspace, int64_t workspace_bytes, int64_t b, int64_t lq,
                              int64_t lk, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * f1 query lengths. Self-attention over a padded batch (clips of different token counts packed to one lq, queries and keys both
+ * padded): each entry point of the f1 family has a twin, suffixed _vl (variable length), that takes q_lens and k_lens right after
+ * lk and is otherwise the same call.  Both are required: self-attention passes the same pointer twice, and a caller with query
+ * lengths only passes k_lens filled with lk.
+ *   q_lens [b] int32, device memory, 4-byte aligned: batch entry i owns query rows 0 .. lq_i - 1 of its own [lq, h, d] slab,
+ *   lq_i = min(max(q_lens[i], 0), lq).  k_lens as for the _kl twins.  The values are device data, clamped by the kernels and
+ *   never read by the host.
+ * Batch entry i's results in rows < lq_i are bit-identical to the entry point without lengths called on entry i alone with q (and
+ * q_t, out and d_out where the call reads them) cut to its first lq_i rows and k, v (and k_t, v_t) cut to their first lk_i rows;
+ * dk and dv of entry i are bit-identical to that trimmed call's.  Rows lq_i .. lq - 1 store out = 0, out_t = 0, dq = 0 and
+ * lse = +inf (the convention of rows >= lq), and contribute nothing to dk and dv; an entry with lq_i = 0 also gets dk = dv = 0.
+ * What the rows past lq_i of q, q_t, out and d_out hold, inf and NaN included, never reaches an output: query tiles wholly past
+ * lq_i are neither loaded nor visited (their CTAs store the zero rows and exit, in the forward, JVP, tangent and dQ kernels; the
+ * dK/dV kernel walks only the query blocks below lq_i), the dK/dV kernel zeroes the straddling block's Q and dO rows past lq_i on
+ * chip after the load and stages their lse / delta as +inf / 0, and the delta kernel writes delta = 0 for them without reading.
+ *   tdb200_attn_dense_fwd_vl, tdb200_attn_dense_fwd_lse_vl, tdb200_attn_dense_jvp_vl, tdb200_attn_dense_jvp_lse_vl,
+ *   tdb200_attn_dense_tangent_vl, tdb200_attn_dense_bwd_vl (its workspace: tdb200_attn_dense_bwd_workspace_bytes).
+ * Errors: those of the _kl twin, plus q_lens null or not 4-byte aligned -> TDB200_ERR_INVALID_ARG, all before any CUDA call.
+ * Launches, synchronisation and graph capture as the twin without _vl.
+ * ------------------------------------------------------------------------------------------- */
+int tdb200_attn_dense_fwd_vl(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq, int64_t lk,
+                             const int32_t* q_lens, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream);
+int tdb200_attn_dense_fwd_lse_vl(const void* q, const void* k, const void* v, int dtype, void* out, float* lse, int64_t b,
+                                 int64_t lq, int64_t lk, const int32_t* q_lens, const int32_t* k_lens, int64_t h, int64_t d,
+                                 float sm_scale, void* stream);
+int tdb200_attn_dense_jvp_vl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                             int dtype, void* out, void* out_t, int64_t b, int64_t lq, int64_t lk, const int32_t* q_lens,
+                             const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream);
+int tdb200_attn_dense_jvp_lse_vl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                                 int dtype, void* out, void* out_t, float* lse, int64_t b, int64_t lq, int64_t lk,
+                                 const int32_t* q_lens, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream);
+int tdb200_attn_dense_tangent_vl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
+                                 const void* out, const float* lse, int dtype, void* out_t, int64_t b, int64_t lq, int64_t lk,
+                                 const int32_t* q_lens, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream);
+int tdb200_attn_dense_bwd_vl(const void* q, const void* k, const void* v, const void* out, const void* d_out, const float* lse,
+                             int dtype, void* dq, void* dk, void* dv, void* workspace, int64_t workspace_bytes, int64_t b, int64_t lq,
+                             int64_t lk, const int32_t* q_lens, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale,
+                             void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * f1 JVP. Forward-mode derivative of the dense attention above (rCM distillation's tangent pass, reference

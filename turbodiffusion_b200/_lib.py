@@ -83,6 +83,12 @@ _PROTOS = {
     "tdb200_attn_dense_jvp_lse_kl": [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _I64, _I64, _I64, _P, _I64, _I64, _F, _P],
     "tdb200_attn_dense_tangent_kl": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I64, _I64, _I64, _P, _I64, _I64, _F, _P],
     "tdb200_attn_dense_bwd_kl": [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _P, _I64, _I64, _F, _P],
+    "tdb200_attn_dense_fwd_vl": [_P, _P, _P, _I, _P, _I64, _I64, _I64, _P, _P, _I64, _I64, _F, _P],
+    "tdb200_attn_dense_fwd_lse_vl": [_P, _P, _P, _I, _P, _P, _I64, _I64, _I64, _P, _P, _I64, _I64, _F, _P],
+    "tdb200_attn_dense_jvp_vl": [_P, _P, _P, _P, _P, _P, _I, _P, _P, _I64, _I64, _I64, _P, _P, _I64, _I64, _F, _P],
+    "tdb200_attn_dense_jvp_lse_vl": [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _I64, _I64, _I64, _P, _P, _I64, _I64, _F, _P],
+    "tdb200_attn_dense_tangent_vl": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I64, _I64, _I64, _P, _P, _I64, _I64, _F, _P],
+    "tdb200_attn_dense_bwd_vl": [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _P, _P, _I64, _I64, _F, _P],
     "tdb200_sla_attn16_tangent": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _I64, _I64, _I64, _I64, _F, _I64, _I64, _P],
     "tdb200_ltx_modulated_rms_norm_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_ltx_modulate_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
@@ -156,7 +162,7 @@ class _DeviceGuarded:
 
 
 LAUNCHES = 0  # kernels launched through the C ABI (each entry point documents how many it enqueues)
-_KERNELS_PER_CALL = {"sla_quant_qk": 4, "layernorm_modulate_quant": 2, "sla_attn16_bwd": 4, "attn_dense_bwd": 3, "attn_dense_bwd_kl": 3,
+_KERNELS_PER_CALL = {"sla_quant_qk": 4, "layernorm_modulate_quant": 2, "sla_attn16_bwd": 4, "attn_dense_bwd": 3, "attn_dense_bwd_kl": 3, "attn_dense_bwd_vl": 3,
                      "sla_linear_bwd": 8, "sla_linear_tangent": 5, "sla_quant_v_fp8": 4}  # upper bounds per entry point
 
 

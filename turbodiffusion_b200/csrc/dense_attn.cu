@@ -47,6 +47,7 @@ struct DenseParams {
   int lq, lk, h;
   float sm_scale;
   const int32_t* k_lens = nullptr;   // [b] int32 (kKeyLens only)
+  const int32_t* q_lens = nullptr;   // [b] int32 (kQueryLens only)
 };
 
 // kLse: also lse[b, h, row] = m_used + log2(l), the row log-sum-exp of the scores in the log2 domain with m_used the maximum the
@@ -54,7 +55,10 @@ struct DenseParams {
 // kKeyLens: batch entry b attends to its first lk_b = keys_of(k_lens, lk, b) keys only; tiles past them are neither loaded nor
 // visited, the last tile's rows past them are zeroed (zero_key_rows), and a row with no keys (lk_b = 0) stores out = 0 and
 // lse = +inf, the convention of rows past lq.
-template <typename T, bool kLse, bool kKeyLens = false>
+// kQueryLens: batch entry b owns its first lq_b = queries_of(q_lens, lq, b) query rows only; rows past them store out = 0 and
+// lse = +inf (assigned, not scaled: their q rows may hold inf or NaN), and a CTA whose block lies wholly past lq_b loads
+// nothing and only stores those rows.  Rows do not mix in the forward, so the straddling block needs nothing more.
+template <typename T, bool kLse, bool kKeyLens = false, bool kQueryLens = false>
 __global__ void __launch_bounds__(split::kThreads, 1)
 dense_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                       const __grid_constant__ CUtensorMap tmap_v, DenseParams p) {
@@ -66,7 +70,9 @@ dense_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
   const int lk = keys_of<kKeyLens>(p.k_lens, p.lk, b);
-  const int n_tiles = (lk + BK - 1) / BK;
+  const int lq = queries_of<kQueryLens>(p.q_lens, p.lq, b);
+  const bool idle = kQueryLens && m_blk * BQ >= lq;   // the block lies wholly past the entry's queries
+  const int n_tiles = idle ? 0 : (lk + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
     mbar_init(&bars[kQFull], 1);
@@ -83,7 +89,7 @@ dense_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   if (warp >= kConsumerWarps) {
     // =============================================================== TMA producer
     reg_dealloc<split::kProducerRegs>();
-    if (warp == kConsumerWarps && lane == 0) {
+    if (warp == kConsumerWarps && lane == 0 && !idle) {
       tma_prefetch_desc(&tmap_q);
       tma_prefetch_desc(&tmap_k);
       tma_prefetch_desc(&tmap_v);
@@ -122,7 +128,7 @@ dense_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
   float m_used[2] = {-INFINITY, -INFINITY}, l_part[2] = {0.f, 0.f};  // l_part: this thread's columns of the row sum
 
-  mbar_wait(&bars[kQFull], 0);
+  if (!idle) mbar_wait(&bars[kQFull], 0);
   for (int j = 0; j < n_tiles; ++j) {
     const int st = j % kStages;
     const uint32_t ph = (j / kStages) & 1;
@@ -151,17 +157,19 @@ dense_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     const float l_tot = quad_sum(l_part[h]);   // all four lanes of a row take part, stored or not
     const int64_t qr = int64_t(m_blk) * BQ + r_lo + 8 * h;
     if (qr >= p.lq) continue;
-    const bool empty = kKeyLens && lk == 0;   // o = 0 and l = 0: store 0 * 0 and lse = +inf
+    const bool pad = kQueryLens && qr >= lq;   // a row past the entry's queries
+    if (pad) zero_o_row(o, h);
+    const bool empty = (kKeyLens && lk == 0) || pad;   // o = 0 and l = 0: store 0 * 0 and lse = +inf
     if constexpr (kLse)
       if (cq == 0) p.lse[(int64_t(b) * p.h + hh) * p.lq + qr] = empty ? INFINITY : m_used[h] + __log2f(l_tot);
     store_o_row<T, HD>(static_cast<T*>(p.out) + ((int64_t(b) * p.lq + qr) * p.h + hh) * HD, o, h, empty ? 0.f : 1.0f / l_tot, cq);
   }
 }
 
-template <typename T, bool kLse, bool kKeyLens>
+template <typename T, bool kLse, bool kKeyLens, bool kQueryLens = false>
 int launch(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const DenseParams& p, dim3 grid, cudaStream_t st) {
   static bool smem_set[64];
-  const auto kern = dense_attn_fwd_kernel<T, kLse, kKeyLens>;
+  const auto kern = dense_attn_fwd_kernel<T, kLse, kKeyLens, kQueryLens>;
   if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), kSmemBytes, smem_set, "cudaFuncSetAttribute(dense_attn)"))
     return rc;
   kern<<<grid, split::kThreads, kSmemBytes, st>>>(tq, tk, tv, p);
@@ -214,6 +222,7 @@ struct Params {
   const int32_t* lut;   // [b, h, mblk, topk] key-block ids (kSparse only)
   int topk, mblk;
   const int32_t* k_lens = nullptr;   // [b] int32 (kKeyLens only)
+  const int32_t* q_lens = nullptr;   // [b] int32 (kQueryLens only)
 };
 
 // d (+)= Q.K^T over one 64-key tile: Q rows at sq (HD/64 chunks kQBytes/2 apart), K at sk (chunks BK * 128 bytes apart)
@@ -272,7 +281,8 @@ __device__ __forceinline__ void softmax_step_jvp(float (&s)[BK / 2], float (&o)[
 
 // kLse: also the row lse of the primal, as dense_attn_fwd_kernel<T, true> stores it.  kKeyLens (dense only): the forward's, so
 // a row with no keys also stores out_t = 0, and the ragged last tile's rows past the entry's keys (K, K_t, V and V_t) are zeroed.
-template <typename T, bool kLse, bool kSparse = false, bool kKeyLens = false>
+// kQueryLens (dense only): the forward's, so a row past the entry's queries also stores out_t = 0.
+template <typename T, bool kLse, bool kSparse = false, bool kKeyLens = false, bool kQueryLens = false>
 __global__ void __launch_bounds__(split::kThreads, 1)
 dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                       const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_qt,
@@ -286,7 +296,9 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
   const int lk = keys_of<kKeyLens>(p.k_lens, p.lk, b);
-  const int n_tiles = kSparse ? p.topk : (lk + BK - 1) / BK;
+  // the block lies wholly past the entry's queries (the epilogue reads the length again rather than hold it in a register)
+  const bool idle = kQueryLens && m_blk * BQ >= queries_of<kQueryLens>(p.q_lens, p.lq, b);
+  const int n_tiles = idle ? 0 : kSparse ? p.topk : (lk + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
     mbar_init(&bars[kQFull], 1);
@@ -307,7 +319,7 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   if (warp >= kConsumerWarps) {
     // =============================================================== TMA producer
     reg_dealloc<split::kProducerRegs>();
-    if (warp == kConsumerWarps && lane == 0) {
+    if (warp == kConsumerWarps && lane == 0 && !idle) {
       tma_prefetch_desc(&tmap_q);
       tma_prefetch_desc(&tmap_qt);
       tma_prefetch_desc(&tmap_k);
@@ -359,7 +371,7 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   for (int i = 0; i < HD / 2; ++i) o[i] = a[i] = 0.f;
   float m_used[2] = {-INFINITY, -INFINITY}, m_run[2], l_part[2] = {0.f, 0.f}, mu_part[2] = {0.f, 0.f};
 
-  mbar_wait(&bars[kQFull], 0);
+  if (!idle) mbar_wait(&bars[kQFull], 0);
   for (int j = 0; j < n_tiles; ++j) {
     const int st = j % kStages;
     const uint32_t ph = (j / kStages) & 1;
@@ -455,16 +467,22 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     warp_release(&bars[kVEmpty + st], lane);
   }
 
+  const int lq = queries_of<kQueryLens>(p.q_lens, p.lq, b);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const float l_tot = quad_sum(l_part[h]), mu_tot = quad_sum(mu_part[h]);   // all four lanes of a row take part
     const int64_t qr = int64_t(m_blk) * BQ + r_lo + 8 * h;
     if (qr >= p.lq) continue;
     const int64_t row = ((int64_t(b) * p.lq + qr) * p.h + hh) * HD;
-    const bool empty = kKeyLens && lk == 0;   // o = a = 0 and l = mu = 0: store zeros and lse = +inf
+    const bool pad = kQueryLens && qr >= lq;   // a row past the entry's queries: o = a = mu = 0, assigned
+    if (pad) {
+      zero_o_row(o, h);
+      zero_o_row(a, h);
+    }
+    const bool empty = (kKeyLens && lk == 0) || pad;   // o = a = 0 and l = mu = 0: store zeros and lse = +inf
     if constexpr (kLse)
       if (cq == 0) p.lse[(int64_t(b) * p.h + hh) * p.lq + qr] = empty ? INFINITY : m_used[h] + __log2f(l_tot);
-    const float inv_l = empty ? 0.f : 1.0f / l_tot, mu_l = mu_tot * inv_l;
+    const float inv_l = empty ? 0.f : 1.0f / l_tot, mu_l = pad ? 0.f : mu_tot * inv_l;
     store_o_row<T, HD>(static_cast<T*>(p.out) + row, o, h, inv_l, cq);
     T* trow = static_cast<T*>(p.out_t) + row;
 #pragma unroll
@@ -476,10 +494,10 @@ dense_attn_jvp_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   }
 }
 
-template <typename T, bool kLse, bool kKeyLens>
+template <typename T, bool kLse, bool kKeyLens, bool kQueryLens = false>
 int launch(const CUtensorMap (&tm)[6], const Params& p, dim3 grid, cudaStream_t st) {
   static bool smem_set[64];
-  const auto kern = dense_attn_jvp_kernel<T, kLse, false, kKeyLens>;
+  const auto kern = dense_attn_jvp_kernel<T, kLse, false, kKeyLens, kQueryLens>;
   if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), kSmemBytes, smem_set, "cudaFuncSetAttribute(dense_attn_jvp)"))
     return rc;
   kern<<<grid, split::kThreads, kSmemBytes, st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p);
@@ -510,8 +528,9 @@ int launch_sparse(const CUtensorMap (&tm)[6], const Params& p, dim3 grid, cudaSt
 // p.out and p.lse are inputs here.  The set-up and the producer are dense_attn_jvp_kernel's, written out again: moved into a
 // shared function they changed that kernel's register allocation.  kKeyLens (dense only): tiles past k_lens[b] are neither
 // loaded nor visited, the last tile's rows past them are zeroed as in dense_attn_jvp_kernel, and a row with no keys has A = 0
-// and mu = 0, so it stores out_t = 0.
-template <typename T, bool kSparse, bool kKeyLens = false>
+// and mu = 0, so it stores out_t = 0.  kQueryLens (dense only): a row past the entry's queries reads no lse and no out and
+// stores out_t = 0, and a CTA whose block lies wholly past them loads nothing.
+template <typename T, bool kSparse, bool kKeyLens = false, bool kQueryLens = false>
 __global__ void __launch_bounds__(split::kThreads, 1)
 attn_tangent_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                     const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_qt,
@@ -525,7 +544,9 @@ attn_tangent_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
   const int lk = keys_of<kKeyLens>(p.k_lens, p.lk, b);
-  const int n_tiles = kSparse ? p.topk : (lk + BK - 1) / BK;
+  const int lq = queries_of<kQueryLens>(p.q_lens, p.lq, b);
+  const bool idle = kQueryLens && m_blk * BQ >= lq;   // the block lies wholly past the entry's queries
+  const int n_tiles = idle ? 0 : kSparse ? p.topk : (lk + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
     mbar_init(&bars[kQFull], 1);
@@ -546,7 +567,7 @@ attn_tangent_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   if (warp >= kConsumerWarps) {
     // =============================================================== TMA producer (dense_attn_jvp_kernel's)
     reg_dealloc<split::kProducerRegs>();
-    if (warp == kConsumerWarps && lane == 0) {
+    if (warp == kConsumerWarps && lane == 0 && !idle) {
       tma_prefetch_desc(&tmap_q);
       tma_prefetch_desc(&tmap_qt);
       tma_prefetch_desc(&tmap_k);
@@ -596,14 +617,14 @@ attn_tangent_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int64_t qr = int64_t(m_blk) * BQ + r_lo + 8 * h;
-    lse[h] = qr < p.lq ? p.lse[(int64_t(b) * p.h + hh) * p.lq + qr] : INFINITY;
+    lse[h] = qr < lq ? p.lse[(int64_t(b) * p.h + hh) * p.lq + qr] : INFINITY;
   }
   float a[HD / 2];
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) a[i] = 0.f;
   float mu_part[2] = {0.f, 0.f};
 
-  mbar_wait(&bars[kQFull], 0);
+  if (!idle) mbar_wait(&bars[kQFull], 0);
   for (int j = 0; j < n_tiles; ++j) {
     const int st = j % kStages;
     const uint32_t ph = (j / kStages) & 1;
@@ -674,6 +695,11 @@ attn_tangent_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     const int64_t row = ((int64_t(b) * p.lq + qr) * p.h + hh) * HD;
     const T* orow = static_cast<const T*>(p.out) + row;
     T* trow = static_cast<T*>(p.out_t) + row;
+    if (kQueryLens && qr >= lq) {   // a row past the entry's queries
+#pragma unroll
+      for (int c = 0; c < HD / 8; ++c) *reinterpret_cast<uint32_t*>(trow + 8 * c + cq) = 0u;
+      continue;
+    }
 #pragma unroll
     for (int c = 0; c < HD / 8; ++c) {
       const int i = 4 * c + 2 * h;
@@ -685,10 +711,10 @@ attn_tangent_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 }
 
 // kSparse: the dynamic shared memory grows by the LUT row, as for launch_sparse
-template <typename T, bool kSparse, bool kKeyLens = false>
+template <typename T, bool kSparse, bool kKeyLens = false, bool kQueryLens = false>
 int launch_tangent(const CUtensorMap (&tm)[6], const Params& p, dim3 grid, cudaStream_t st) {
   static bool smem_set[64];
-  const auto kern = attn_tangent_kernel<T, kSparse, kKeyLens>;
+  const auto kern = attn_tangent_kernel<T, kSparse, kKeyLens, kQueryLens>;
   const size_t smem_max = kSparse ? kSparseSmemMax : kSmemBytes;
   if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(kern), smem_max, smem_set,
                                          kSparse ? "cudaFuncSetAttribute(sla_attn16_tangent)" : "cudaFuncSetAttribute(attn_dense_tangent)"))
@@ -710,17 +736,19 @@ int tmap16(CUtensorMap* m, const void* base, int dtype, int64_t b, int64_t l, in
 bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
 
 // tdb200_attn_dense_fwd (lse null) and tdb200_attn_dense_fwd_lse; `what` prefixes the messages.  key_lens: their _kl twins,
-// which take k_lens [b] and launch the kKeyLens kernels.
+// which take k_lens [b] and launch the kKeyLens kernels; query_lens (with key_lens): their _vl twins, which also take q_lens [b]
+// and launch the kernels with both flags set.
 int dense_fwd(const char* what, const void* q, const void* k, const void* v, int dtype, void* out, float* lse, bool with_lse,
-              int64_t b, int64_t lq, int64_t lk, const int32_t* k_lens, bool key_lens, int64_t h, int64_t d, float sm_scale,
-              void* stream) {
-  if (!q || !k || !v || !out || (with_lse && !lse) || (key_lens && !k_lens))
+              int64_t b, int64_t lq, int64_t lk, const int32_t* q_lens, bool query_lens, const int32_t* k_lens, bool key_lens,
+              int64_t h, int64_t d, float sm_scale, void* stream) {
+  if (!q || !k || !v || !out || (with_lse && !lse) || (key_lens && !k_lens) || (query_lens && !q_lens))
     return fail(TDB200_ERR_INVALID_ARG, "%s: null pointer", what);
   if (int rc = dense_attn_shape(what, b, lq, lk, h, d)) return rc;
   if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out))
     return fail(TDB200_ERR_INVALID_ARG, "%s: q, k, v and out must be 16-byte aligned", what);
   if (with_lse && !aligned4(lse)) return fail(TDB200_ERR_INVALID_ARG, "%s: lse must be 4-byte aligned", what);
   if (key_lens && !aligned4(k_lens)) return fail(TDB200_ERR_INVALID_ARG, "%s: k_lens must be 4-byte aligned", what);
+  if (query_lens && !aligned4(q_lens)) return fail(TDB200_ERR_INVALID_ARG, "%s: q_lens must be 4-byte aligned", what);
   if (int rc = dense_attn_limits(what, dtype, b, lq, lk, h, d)) return rc;
   if (int rc = require_sm90()) return rc;
 
@@ -736,9 +764,16 @@ int dense_fwd(const char* what, const void* q, const void* k, const void* v, int
   p.h = int(h);
   p.sm_scale = sm_scale;
   p.k_lens = k_lens;
+  p.q_lens = q_lens;
   const dim3 grid(static_cast<unsigned>(cdiv64(lq, BQ)), static_cast<unsigned>(h), static_cast<unsigned>(b));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool bf16 = dtype == TDB200_DTYPE_BF16;
+  if (query_lens) {
+    if (!with_lse)
+      return bf16 ? launch<__nv_bfloat16, false, true, true>(tq, tk, tv, p, grid, st)
+                  : launch<__half, false, true, true>(tq, tk, tv, p, grid, st);
+    return bf16 ? launch<__nv_bfloat16, true, true, true>(tq, tk, tv, p, grid, st) : launch<__half, true, true, true>(tq, tk, tv, p, grid, st);
+  }
   if (!key_lens) {
     if (!with_lse)
       return bf16 ? launch<__nv_bfloat16, false, false>(tq, tk, tv, p, grid, st) : launch<__half, false, false>(tq, tk, tv, p, grid, st);
@@ -750,11 +785,13 @@ int dense_fwd(const char* what, const void* q, const void* k, const void* v, int
 }
 
 // tdb200_attn_dense_jvp (lse null), tdb200_attn_dense_jvp_lse and, `tangent`, tdb200_attn_dense_tangent (out and lse inputs);
-// key_lens: their _kl twins, as for dense_fwd
+// key_lens: their _kl twins, query_lens: their _vl twins, as for dense_fwd
 int dense_jvp(const char* what, const void* q, const void* k, const void* v, const void* q_t, const void* k_t, const void* v_t,
-              int dtype, void* out, void* out_t, float* lse, bool with_lse, int64_t b, int64_t lq, int64_t lk, const int32_t* k_lens,
-              bool key_lens, int64_t h, int64_t d, float sm_scale, void* stream, bool tangent = false) {
-  if (!q || !k || !v || !q_t || !k_t || !v_t || !out || !out_t || (with_lse && !lse) || (key_lens && !k_lens))
+              int dtype, void* out, void* out_t, float* lse, bool with_lse, int64_t b, int64_t lq, int64_t lk, const int32_t* q_lens,
+              bool query_lens, const int32_t* k_lens, bool key_lens, int64_t h, int64_t d, float sm_scale, void* stream,
+              bool tangent = false) {
+  if (!q || !k || !v || !q_t || !k_t || !v_t || !out || !out_t || (with_lse && !lse) || (key_lens && !k_lens) ||
+      (query_lens && !q_lens))
     return fail(TDB200_ERR_INVALID_ARG, "%s: null pointer", what);
   if (int rc = dense_attn_shape(what, b, lq, lk, h, d)) return rc;
   if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(q_t) || !aligned16(k_t) || !aligned16(v_t) ||
@@ -762,6 +799,7 @@ int dense_jvp(const char* what, const void* q, const void* k, const void* v, con
     return fail(TDB200_ERR_INVALID_ARG, "%s: q, k, v, their tangents, out and out_t must be 16-byte aligned", what);
   if (with_lse && !aligned4(lse)) return fail(TDB200_ERR_INVALID_ARG, "%s: lse must be 4-byte aligned", what);
   if (key_lens && !aligned4(k_lens)) return fail(TDB200_ERR_INVALID_ARG, "%s: k_lens must be 4-byte aligned", what);
+  if (query_lens && !aligned4(q_lens)) return fail(TDB200_ERR_INVALID_ARG, "%s: q_lens must be 4-byte aligned", what);
   if (int rc = dense_attn_limits(what, dtype, b, lq, lk, h, d)) return rc;
   if (int rc = require_sm90()) return rc;
 
@@ -781,9 +819,18 @@ int dense_jvp(const char* what, const void* q, const void* k, const void* v, con
   p.h = int(h);
   p.sm_scale = sm_scale;
   p.k_lens = k_lens;
+  p.q_lens = q_lens;
   const dim3 grid(static_cast<unsigned>(cdiv64(lq, BQ)), static_cast<unsigned>(h), static_cast<unsigned>(b));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool bf16 = dtype == TDB200_DTYPE_BF16;
+  if (query_lens) {
+    if (tangent)
+      return bf16 ? jvp::launch_tangent<__nv_bfloat16, false, true, true>(tm, p, grid, st)
+                  : jvp::launch_tangent<__half, false, true, true>(tm, p, grid, st);
+    if (!with_lse)
+      return bf16 ? jvp::launch<__nv_bfloat16, false, true, true>(tm, p, grid, st) : jvp::launch<__half, false, true, true>(tm, p, grid, st);
+    return bf16 ? jvp::launch<__nv_bfloat16, true, true, true>(tm, p, grid, st) : jvp::launch<__half, true, true, true>(tm, p, grid, st);
+  }
   if (!key_lens) {
     if (tangent)
       return bf16 ? jvp::launch_tangent<__nv_bfloat16, false>(tm, p, grid, st) : jvp::launch_tangent<__half, false>(tm, p, grid, st);
@@ -855,25 +902,25 @@ int sla_jvp(const char* what, const void* q, const void* k, const void* v, const
 
 extern "C" int tdb200_attn_dense_fwd(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq,
                                      int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  return dense_fwd("attn_dense_fwd", q, k, v, dtype, out, nullptr, false, b, lq, lk, nullptr, false, h, d, sm_scale, stream);
+  return dense_fwd("attn_dense_fwd", q, k, v, dtype, out, nullptr, false, b, lq, lk, nullptr, false, nullptr, false, h, d, sm_scale, stream);
 }
 
 extern "C" int tdb200_attn_dense_fwd_lse(const void* q, const void* k, const void* v, int dtype, void* out, float* lse, int64_t b,
                                          int64_t lq, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  return dense_fwd("attn_dense_fwd_lse", q, k, v, dtype, out, lse, true, b, lq, lk, nullptr, false, h, d, sm_scale, stream);
+  return dense_fwd("attn_dense_fwd_lse", q, k, v, dtype, out, lse, true, b, lq, lk, nullptr, false, nullptr, false, h, d, sm_scale, stream);
 }
 
 extern "C" int tdb200_attn_dense_jvp(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
                                      const void* v_t, int dtype, void* out, void* out_t, int64_t b, int64_t lq, int64_t lk,
                                      int64_t h, int64_t d, float sm_scale, void* stream) {
-  return dense_jvp("attn_dense_jvp", q, k, v, q_t, k_t, v_t, dtype, out, out_t, nullptr, false, b, lq, lk, nullptr, false, h, d,
+  return dense_jvp("attn_dense_jvp", q, k, v, q_t, k_t, v_t, dtype, out, out_t, nullptr, false, b, lq, lk, nullptr, false, nullptr, false, h, d,
                    sm_scale, stream);
 }
 
 extern "C" int tdb200_attn_dense_jvp_lse(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
                                          const void* v_t, int dtype, void* out, void* out_t, float* lse, int64_t b, int64_t lq,
                                          int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
-  return dense_jvp("attn_dense_jvp_lse", q, k, v, q_t, k_t, v_t, dtype, out, out_t, lse, true, b, lq, lk, nullptr, false, h, d,
+  return dense_jvp("attn_dense_jvp_lse", q, k, v, q_t, k_t, v_t, dtype, out, out_t, lse, true, b, lq, lk, nullptr, false, nullptr, false, h, d,
                    sm_scale, stream);
 }
 
@@ -896,7 +943,7 @@ extern "C" int tdb200_attn_dense_tangent(const void* q, const void* k, const voi
                                          const void* v_t, const void* out, const float* lse, int dtype, void* out_t, int64_t b,
                                          int64_t lq, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
   return dense_jvp("attn_dense_tangent", q, k, v, q_t, k_t, v_t, dtype, const_cast<void*>(out), out_t, const_cast<float*>(lse), true,
-                   b, lq, lk, nullptr, false, h, d, sm_scale, stream, true);
+                   b, lq, lk, nullptr, false, nullptr, false, h, d, sm_scale, stream, true);
 }
 
 extern "C" int tdb200_sla_attn16_tangent(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
@@ -911,26 +958,26 @@ extern "C" int tdb200_sla_attn16_tangent(const void* q, const void* k, const voi
 // The _kl twins: the entry points above with per-sample key lengths k_lens [b] (the kKeyLens kernels)
 extern "C" int tdb200_attn_dense_fwd_kl(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq,
                                         int64_t lk, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream) {
-  return dense_fwd("attn_dense_fwd_kl", q, k, v, dtype, out, nullptr, false, b, lq, lk, k_lens, true, h, d, sm_scale, stream);
+  return dense_fwd("attn_dense_fwd_kl", q, k, v, dtype, out, nullptr, false, b, lq, lk, nullptr, false, k_lens, true, h, d, sm_scale, stream);
 }
 
 extern "C" int tdb200_attn_dense_fwd_lse_kl(const void* q, const void* k, const void* v, int dtype, void* out, float* lse, int64_t b,
                                             int64_t lq, int64_t lk, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale,
                                             void* stream) {
-  return dense_fwd("attn_dense_fwd_lse_kl", q, k, v, dtype, out, lse, true, b, lq, lk, k_lens, true, h, d, sm_scale, stream);
+  return dense_fwd("attn_dense_fwd_lse_kl", q, k, v, dtype, out, lse, true, b, lq, lk, nullptr, false, k_lens, true, h, d, sm_scale, stream);
 }
 
 extern "C" int tdb200_attn_dense_jvp_kl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
                                         const void* v_t, int dtype, void* out, void* out_t, int64_t b, int64_t lq, int64_t lk,
                                         const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream) {
-  return dense_jvp("attn_dense_jvp_kl", q, k, v, q_t, k_t, v_t, dtype, out, out_t, nullptr, false, b, lq, lk, k_lens, true, h, d,
+  return dense_jvp("attn_dense_jvp_kl", q, k, v, q_t, k_t, v_t, dtype, out, out_t, nullptr, false, b, lq, lk, nullptr, false, k_lens, true, h, d,
                    sm_scale, stream);
 }
 
 extern "C" int tdb200_attn_dense_jvp_lse_kl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
                                             const void* v_t, int dtype, void* out, void* out_t, float* lse, int64_t b, int64_t lq,
                                             int64_t lk, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream) {
-  return dense_jvp("attn_dense_jvp_lse_kl", q, k, v, q_t, k_t, v_t, dtype, out, out_t, lse, true, b, lq, lk, k_lens, true, h, d,
+  return dense_jvp("attn_dense_jvp_lse_kl", q, k, v, q_t, k_t, v_t, dtype, out, out_t, lse, true, b, lq, lk, nullptr, false, k_lens, true, h, d,
                    sm_scale, stream);
 }
 
@@ -939,5 +986,45 @@ extern "C" int tdb200_attn_dense_tangent_kl(const void* q, const void* k, const 
                                             int64_t lq, int64_t lk, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale,
                                             void* stream) {
   return dense_jvp("attn_dense_tangent_kl", q, k, v, q_t, k_t, v_t, dtype, const_cast<void*>(out), out_t, const_cast<float*>(lse),
-                   true, b, lq, lk, k_lens, true, h, d, sm_scale, stream, true);
+                   true, b, lq, lk, nullptr, false, k_lens, true, h, d, sm_scale, stream, true);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// The _vl twins: per-sample query lengths q_lens [b] and key lengths k_lens [b] (the kernels with kQueryLens and kKeyLens)
+extern "C" int tdb200_attn_dense_fwd_vl(const void* q, const void* k, const void* v, int dtype, void* out, int64_t b, int64_t lq,
+                                        int64_t lk, const int32_t* q_lens, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale,
+                                        void* stream) {
+  return dense_fwd("attn_dense_fwd_vl", q, k, v, dtype, out, nullptr, false, b, lq, lk, q_lens, true, k_lens, true, h, d, sm_scale,
+                   stream);
+}
+
+extern "C" int tdb200_attn_dense_fwd_lse_vl(const void* q, const void* k, const void* v, int dtype, void* out, float* lse, int64_t b,
+                                            int64_t lq, int64_t lk, const int32_t* q_lens, const int32_t* k_lens, int64_t h, int64_t d,
+                                            float sm_scale, void* stream) {
+  return dense_fwd("attn_dense_fwd_lse_vl", q, k, v, dtype, out, lse, true, b, lq, lk, q_lens, true, k_lens, true, h, d, sm_scale,
+                   stream);
+}
+
+extern "C" int tdb200_attn_dense_jvp_vl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
+                                        const void* v_t, int dtype, void* out, void* out_t, int64_t b, int64_t lq, int64_t lk,
+                                        const int32_t* q_lens, const int32_t* k_lens, int64_t h, int64_t d, float sm_scale,
+                                        void* stream) {
+  return dense_jvp("attn_dense_jvp_vl", q, k, v, q_t, k_t, v_t, dtype, out, out_t, nullptr, false, b, lq, lk, q_lens, true, k_lens,
+                   true, h, d, sm_scale, stream);
+}
+
+extern "C" int tdb200_attn_dense_jvp_lse_vl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
+                                            const void* v_t, int dtype, void* out, void* out_t, float* lse, int64_t b, int64_t lq,
+                                            int64_t lk, const int32_t* q_lens, const int32_t* k_lens, int64_t h, int64_t d,
+                                            float sm_scale, void* stream) {
+  return dense_jvp("attn_dense_jvp_lse_vl", q, k, v, q_t, k_t, v_t, dtype, out, out_t, lse, true, b, lq, lk, q_lens, true, k_lens,
+                   true, h, d, sm_scale, stream);
+}
+
+extern "C" int tdb200_attn_dense_tangent_vl(const void* q, const void* k, const void* v, const void* q_t, const void* k_t,
+                                            const void* v_t, const void* out, const float* lse, int dtype, void* out_t, int64_t b,
+                                            int64_t lq, int64_t lk, const int32_t* q_lens, const int32_t* k_lens, int64_t h,
+                                            int64_t d, float sm_scale, void* stream) {
+  return dense_jvp("attn_dense_tangent_vl", q, k, v, q_t, k_t, v_t, dtype, const_cast<void*>(out), out_t, const_cast<float*>(lse),
+                   true, b, lq, lk, q_lens, true, k_lens, true, h, d, sm_scale, stream, true);
 }

@@ -44,6 +44,26 @@ __device__ __forceinline__ void zero_key_rows(uint8_t* tile, int rows, int chunk
   }
 }
 
+// The query rows batch entry b of a dense attention kernel owns: lq, or (kQueryLens, the _vl entry points) q_lens[b] clamped
+// to [0, lq].  Read once per CTA before its first barrier, as keys_of.
+template <bool kQueryLens>
+__device__ __forceinline__ int queries_of(const int32_t* q_lens, int lq, int b) {
+  return keys_of<kQueryLens>(q_lens, lq, b);
+}
+
+// kQueryLens: query rows [lo, hi) of a streamed Q or dO tile (`chunks` column chunks of rows x 128 B at `tile`) lie past the
+// entry's queries but inside the buffer.  Where one query row's values reach a sum over query rows (the dK / dV kernel's
+// P^T.dO and dS^T.Q), 0 * inf would be NaN: so the warpgroup that reads those rows zeroes them, as TMA's zero fill would.
+// The 128 threads of that warpgroup share the work (t = threadIdx.x & 127); whole 128-byte rows, as zero_key_rows.  The caller
+// then runs fence_proxy_async_smem() and a barrier over the warpgroup, before any MMA reads the tile.
+__device__ __forceinline__ void zero_query_rows(uint8_t* tile, int rows, int chunks, int lo, int hi, int t) {
+  const int per_chunk = (hi - lo) * 8;   // 16-byte units
+  for (int e = t; e < chunks * per_chunk; e += 128) {
+    const int c = e / per_chunk, u = e - c * per_chunk;
+    *reinterpret_cast<uint4*>(tile + c * rows * 128 + lo * 128 + u * 16) = make_uint4(0u, 0u, 0u, 0u);
+  }
+}
+
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kRescaleThreshold = 8.0f;  // log2 domain
 
@@ -351,6 +371,14 @@ __device__ __forceinline__ void store_o_row(T* orow, const float (&o)[HD / 2], i
 #pragma unroll
   for (int c = 0; c < HD / 8; ++c)
     *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) = F16Traits<T>::pack(o[4 * c + 2 * h] * inv_l, o[4 * c + 2 * h + 1] * inv_l);
+}
+
+// Row h (0: r_lo, 1: r_lo + 8) of this thread's m64 accumulator fragment set to zero: a query row past its entry's queries
+// (kQueryLens) stores zeros whatever its q held, where scaling by zero would keep inf or NaN
+template <int N>
+__device__ __forceinline__ void zero_o_row(float (&o)[N], int h) {
+#pragma unroll
+  for (int c = 0; c < N / 4; ++c) o[4 * c + 2 * h] = o[4 * c + 2 * h + 1] = 0.f;
 }
 
 namespace split {

@@ -21,7 +21,11 @@
 // that only replaces where a block id comes from; the per-tile arithmetic is the same instructions.  kKeyLens (with kDense,
 // tdb200_attn_dense_bwd_kl): batch entry b has lk_b = k_lens[b] keys; the dQ CTA visits tiles 0 .. ceil(lk_b / 64) - 1 with
 // columns >= lk_b masked and the last tile's K and V rows >= lk_b zeroed (zero_key_rows), a dK/dV CTA whose key block starts
-// at or past lk_b stores zeros, and rows >= lk_b of a block that straddles lk_b are stored as zeros.
+// at or past lk_b stores zeros, and rows >= lk_b of a block that straddles lk_b are stored as zeros.  kQueryLens (with kDense
+// and kKeyLens, tdb200_attn_dense_bwd_vl): batch entry b has lq_b = q_lens[b] query rows; the delta kernel writes delta = 0 for
+// rows >= lq_b without reading them, a dQ CTA whose block starts at or past lq_b loads nothing and stores zeros, rows >= lq_b
+// of the dQ block that straddles lq_b are stored as zeros, and the dK/dV CTA visits query blocks 0 .. ceil(lq_b / 128) - 1 with
+// the straddling block's Q and dO rows >= lq_b zeroed on chip (zero_query_rows) and their lse / delta staged as +inf / 0.
 //
 // Rounding points (FlashAttention-2's): P and dS are formed in fp32 and rounded to T only as MMA operands; dQ, dK, dV accumulate
 // in fp32 registers and are rounded to T once.  No floating-point atomics: every output element is written by one thread in a
@@ -58,15 +62,27 @@ struct BwdParams {
   int topk;                // key blocks per query block (dense: nblk)
   float sm_scale;
   const int32_t* k_lens = nullptr;   // [b] int32 (kKeyLens only)
+  const int32_t* q_lens = nullptr;   // [b] int32 (kQueryLens only)
 };
 
 // ------------------------------------------------------------------------------------------------ preprocessing
-// One warp per (b, row, head); lanes take 4 consecutive columns, then a butterfly sum (fixed order).
-template <typename T>
-__global__ void __launch_bounds__(256) sla_bwd_delta_kernel(const T* o, const T* d_o, float* delta, int64_t rows, int l, int h) {
+// One warp per (b, row, head); lanes take 4 consecutive columns, then a butterfly sum (fixed order).  kQueryLens: a row past its
+// entry's q_lens[b] gets delta = 0 and reads neither o nor d_o.
+template <typename T, bool kQueryLens = false>
+__global__ void __launch_bounds__(256) sla_bwd_delta_kernel(const T* o, const T* d_o, float* delta, int64_t rows, int l, int h,
+                                                            const int32_t* q_lens) {
   const int64_t r = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (r >= rows) return;
+  if constexpr (kQueryLens) {
+    const int64_t bl = r / h;           // b * l + row
+    const int hh = int(r - bl * h);
+    const int64_t b = bl / l, row = bl - b * l;
+    if (row >= queries_of<true>(q_lens, l, int(b))) {
+      if (lane == 0) delta[(b * h + hh) * l + row] = 0.f;
+      return;
+    }
+  }
   const uint2 ov = *reinterpret_cast<const uint2*>(o + r * HD + lane * 4);
   const uint2 gv = *reinterpret_cast<const uint2*>(d_o + r * HD + lane * 4);
   float acc = F16Traits<T>::lo(ov.x) * F16Traits<T>::lo(gv.x);
@@ -217,7 +233,7 @@ constexpr uint32_t kOffBars = kOffV + kStages * kTileK, kOffLut = kOffBars + 256
 enum Bar { kQFull = 0, kKFull = 1, kKEmpty = 4, kVFull = 7, kVEmpty = 10 };
 }  // namespace dq
 
-template <typename T, bool kDense = false, bool kKeyLens = false>
+template <typename T, bool kDense = false, bool kKeyLens = false, bool kQueryLens = false>
 __global__ void __launch_bounds__(dq::kThreads, 1)
 sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
                   const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v, BwdParams p) {
@@ -231,7 +247,9 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
   const int bh = b * p.h + hh;
   const int lk = keys_of<kKeyLens>(p.k_lens, p.lk, b);
-  const int n_tiles = kKeyLens ? (lk + BLKK - 1) / BLKK : p.topk;
+  const int lq = queries_of<kQueryLens>(p.q_lens, p.lq, b);
+  const bool idle = kQueryLens && m_blk * BLKQ >= lq;   // the block lies wholly past the entry's queries
+  const int n_tiles = idle ? 0 : kKeyLens ? (lk + BLKK - 1) / BLKK : p.topk;
 
   if (threadIdx.x == 0) {
     mbar_init(&bars[kQFull], 1);
@@ -251,7 +269,7 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
 
   if (warp == kConsumerWarps) {
     // =============================================================== TMA producer
-    if (lane == 0) {
+    if (lane == 0 && !idle) {
       tma_prefetch_desc(&tmap_q);
       tma_prefetch_desc(&tmap_do);
       tma_prefetch_desc(&tmap_k);
@@ -291,15 +309,15 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     const int64_t r = int64_t(m_blk) * BLKQ + r_lo + 8 * hf;
-    lse[hf] = r < p.lq ? __ldg(p.lse + int64_t(bh) * p.lq + r) : INFINITY;
-    dlt[hf] = r < p.lq ? __ldg(p.delta + int64_t(bh) * p.lq + r) : 0.f;
+    lse[hf] = r < lq ? __ldg(p.lse + int64_t(bh) * p.lq + r) : INFINITY;
+    dlt[hf] = r < lq ? __ldg(p.delta + int64_t(bh) * p.lq + r) : 0.f;
   }
   float acc[HD / 2];
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) acc[i] = 0.f;
   int ds_e[2] = {kDsUnset, kDsUnset};   // per query row (fp16)
 
-  mbar_wait(&bars[kQFull], 0);
+  if (!idle) mbar_wait(&bars[kQFull], 0);
   for (int j = 0; j < n_tiles; ++j) {
     const int st = j % kStages;
     const uint32_t ph = (j / kStages) & 1;
@@ -377,6 +395,12 @@ sla_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
     if (lane == 0) mbar_arrive(&bars[kKEmpty + st]);
   }
   if constexpr (!kBF16) ds_unscale(ds_e, acc);
+  if constexpr (kQueryLens) {
+    // rows past the entry's queries are zero (assigned, not scaled: their q and d_out rows may hold inf or NaN)
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf)
+      if (int64_t(m_blk) * BLKQ + r_lo + 8 * hf >= lq) zero_o_row(acc, hf);
+  }
   store_rows<T>(acc, p.sm_scale, p.dq, int64_t(m_blk) * BLKQ + r_lo, p.lq, p.h, hh, b, cq);
 }
 
@@ -405,7 +429,7 @@ struct Dkv {
   static_assert(HD * 128 * 4 <= 2 * kStages * kTileQ, "partial dK / dV do not fit in the ring");
 };
 
-template <typename T, int kBQ, bool kDense = false, bool kKeyLens = false>
+template <typename T, int kBQ, bool kDense = false, bool kKeyLens = false, bool kQueryLens = false>
 __global__ void __launch_bounds__(split::kThreads, 1)
 sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
                     const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v, BwdParams p) {
@@ -426,6 +450,8 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     n_list = __ldg(kv_off + n_blk + 1) - __ldg(kv_off + n_blk);
   }
   const int lk = keys_of<kKeyLens>(p.k_lens, p.lk, b);
+  const int lq = queries_of<kQueryLens>(p.q_lens, p.lq, b);
+  if (kQueryLens) n_list = (lq + kBQ - 1) / kBQ;     // (kDense) only the query blocks below this entry's queries
   if (kKeyLens && n_blk * BLKK >= lk) n_list = 0;   // a key block past this entry's keys
 
   if (n_list == 0) {  // no query block selected this key block: its gradients are zero (the outputs are not pre-zeroed)
@@ -501,7 +527,7 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     float* sb = stats + ((L::kSplit ? it : j) & 1) * 128;
     {
       const int64_t r = int64_t(qb) * kBQ + q0 + (t & 63);
-      const bool in = r < p.lq;
+      const bool in = r < lq;
       sb[t] = t < 64 ? (in ? __ldg(p.lse + int64_t(bh) * p.lq + r) : INFINITY) : (in ? __ldg(p.delta + int64_t(bh) * p.lq + r) : 0.f);
     }
     named_bar_sync(1 + wg, 128);
@@ -512,6 +538,18 @@ sla_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 #pragma unroll
     for (int i = 0; i < 32; ++i) s[i] = dp[i] = 0.f;
     mbar_wait(&bars[L::kFull + st], ph);
+    if constexpr (kQueryLens) {
+      // this warpgroup's rows of the block that straddles lq lie past the entry's queries but inside the buffer: zeroed (and
+      // their lse / delta staged as +inf / 0 above), as a trimmed call's TMA zero fill leaves them, so that no inf or NaN
+      // there reaches dK or dV through P^T = 0.  Only this warpgroup reads its 64 rows of the slot.
+      const int lo = lq - qb * kBQ - q0;
+      if (lo < 64 && lq < p.lq) {
+        zero_query_rows(smem + L::kOffQ + st * L::kTileQ + q0 * 128, kBQ, HD / 64, max(lo, 0), 64, t);
+        zero_query_rows(smem + L::kOffDO + st * L::kTileQ + q0 * 128, kBQ, HD / 64, max(lo, 0), 64, t);
+        fence_proxy_async_smem();
+        named_bar_sync(1 + wg, 128);
+      }
+    }
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < HD / 16; ++ks) {
@@ -812,7 +850,7 @@ int launch_bwd(const void* q, const void* k, const void* v, const void* o_s, con
 
   const int64_t rows = b * l * h;
   sla_bwd_delta_kernel<T><<<unsigned(cdiv64(rows, 8)), 256, 0, st>>>(static_cast<const T*>(o_s), static_cast<const T*>(d_o), delta,
-                                                                       rows, int(l), int(h));
+                                                                       rows, int(l), int(h), nullptr);
   if (int rc = check_launch("sla_bwd_delta_kernel")) return rc;
   sla_bwd_kmajor_index_kernel<<<unsigned(b * h), kIndexThreads, 0, st>>>(lut, int(mblk), int(nblk), int(topk), kv_off, cursor, kv_idx);
   if (int rc = check_launch("sla_bwd_kmajor_index_kernel")) return rc;
@@ -925,11 +963,11 @@ constexpr int64_t kMaxDenseRows = int64_t(8) * 0x7FFFFFFF;
 bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
 
 // delta kernel, then dQ over every key tile and dK / dV over every 128-row query block (no index kernel); kKeyLens: over the
-// tiles and key blocks below k_lens[b]
-template <typename T, bool kKeyLens>
+// tiles and key blocks below k_lens[b]; kQueryLens: also over the query rows and blocks below q_lens[b]
+template <typename T, bool kKeyLens, bool kQueryLens = false>
 int launch_dense_bwd(const void* q, const void* k, const void* v, const void* out, const void* d_out, const float* lse, void* dq,
-                     void* dk, void* dv, float* delta, int64_t b, int64_t lq, int64_t lk, const int32_t* k_lens, int64_t h,
-                     float sm_scale, cudaStream_t st) {
+                     void* dk, void* dv, float* delta, int64_t b, int64_t lq, int64_t lk, const int32_t* q_lens,
+                     const int32_t* k_lens, int64_t h, float sm_scale, cudaStream_t st) {
   const CUtensorMapDataType t16 = std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                                                         : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUtensorMap tq, tdo, tk, tv;
@@ -939,8 +977,8 @@ int launch_dense_bwd(const void* q, const void* k, const void* v, const void* ou
   if (int rc = tmap_rows(&tv, v, t16, b, lk, h, BLKK)) return rc;
 
   const int64_t rows = b * lq * h;
-  sla_bwd_delta_kernel<T><<<unsigned(cdiv64(rows, 8)), 256, 0, st>>>(static_cast<const T*>(out), static_cast<const T*>(d_out), delta,
-                                                                       rows, int(lq), int(h));
+  sla_bwd_delta_kernel<T, kQueryLens><<<unsigned(cdiv64(rows, 8)), 256, 0, st>>>(
+      static_cast<const T*>(out), static_cast<const T*>(d_out), delta, rows, int(lq), int(h), q_lens);
   if (int rc = check_launch("sla_bwd_delta_kernel")) return rc;
 
   BwdParams p = {};
@@ -957,10 +995,11 @@ int launch_dense_bwd(const void* q, const void* k, const void* v, const void* ou
   p.topk = p.nblk;
   p.sm_scale = sm_scale;
   p.k_lens = k_lens;
+  p.q_lens = q_lens;
 
   static bool smem_set_dq[64], smem_set_kv[64];
-  const auto dq_kern = sla_bwd_dq_kernel<T, true, kKeyLens>;
-  const auto dkdv_kern = sla_bwd_dkdv_kernel<T, BLKQ, true, kKeyLens>;
+  const auto dq_kern = sla_bwd_dq_kernel<T, true, kKeyLens, kQueryLens>;
+  const auto dkdv_kern = sla_bwd_dkdv_kernel<T, BLKQ, true, kKeyLens, kQueryLens>;
   const size_t smem_dq = 1024 + dq::kOffLut, smem_kv = 1024 + Dkv<BLKQ>::kSmem;
   if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(dq_kern), smem_dq, smem_set_dq, "cudaFuncSetAttribute(dense_bwd_dq)"))
     return rc;
@@ -985,11 +1024,12 @@ extern "C" int64_t tdb200_attn_dense_bwd_workspace_bytes(int64_t b, int64_t h, i
 
 namespace {
 
-// tdb200_attn_dense_bwd and, key_lens, its _kl twin
+// tdb200_attn_dense_bwd and, key_lens, its _kl twin, and, query_lens (with key_lens), its _vl twin
 int dense_bwd(const char* what, const void* q, const void* k, const void* v, const void* out, const void* d_out, const float* lse,
               int dtype, void* dq, void* dk, void* dv, void* workspace, int64_t workspace_bytes, int64_t b, int64_t lq, int64_t lk,
-              const int32_t* k_lens, bool key_lens, int64_t h, int64_t d, float sm_scale, void* stream) {
-  if (!q || !k || !v || !out || !d_out || !lse || !dq || !dk || !dv || !workspace || (key_lens && !k_lens))
+              const int32_t* q_lens, bool query_lens, const int32_t* k_lens, bool key_lens, int64_t h, int64_t d, float sm_scale,
+              void* stream) {
+  if (!q || !k || !v || !out || !d_out || !lse || !dq || !dk || !dv || !workspace || (key_lens && !k_lens) || (query_lens && !q_lens))
     return fail(TDB200_ERR_INVALID_ARG, "%s: null pointer", what);
   if (int rc = dense_attn_shape(what, b, lq, lk, h, d)) return rc;
   if (!aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out) || !aligned16(d_out) || !aligned16(dq) || !aligned16(dk) ||
@@ -997,6 +1037,7 @@ int dense_bwd(const char* what, const void* q, const void* k, const void* v, con
     return fail(TDB200_ERR_INVALID_ARG, "%s: q, k, v, out, d_out, dq, dk and dv must be 16-byte aligned", what);
   if (!aligned4(lse) || !aligned4(workspace)) return fail(TDB200_ERR_INVALID_ARG, "%s: lse and workspace must be 4-byte aligned", what);
   if (key_lens && !aligned4(k_lens)) return fail(TDB200_ERR_INVALID_ARG, "%s: k_lens must be 4-byte aligned", what);
+  if (query_lens && !aligned4(q_lens)) return fail(TDB200_ERR_INVALID_ARG, "%s: q_lens must be 4-byte aligned", what);
   if (int rc = dense_attn_limits(what, dtype, b, lq, lk, h, d)) return rc;
   if (b * lq * h > kMaxDenseRows)
     return fail(TDB200_ERR_UNSUPPORTED, "%s: dimension too large (b * lq * h above 8 * (2^31 - 1), the delta kernel's grid)", what);
@@ -1011,14 +1052,23 @@ int dense_bwd(const char* what, const void* q, const void* k, const void* v, con
   if (int rc = check_cuda(cudaSetDevice(dev), "cudaSetDevice")) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   float* delta = static_cast<float*>(workspace);
+  if (query_lens) {
+    if (dtype == TDB200_DTYPE_BF16)
+      return launch_dense_bwd<__nv_bfloat16, true, true>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, q_lens, k_lens, h,
+                                                         sm_scale, st);
+    return launch_dense_bwd<__half, true, true>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, q_lens, k_lens, h, sm_scale,
+                                                st);
+  }
   if (!key_lens) {
     if (dtype == TDB200_DTYPE_BF16)
-      return launch_dense_bwd<__nv_bfloat16, false>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, nullptr, h, sm_scale, st);
-    return launch_dense_bwd<__half, false>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, nullptr, h, sm_scale, st);
+      return launch_dense_bwd<__nv_bfloat16, false>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, nullptr, nullptr, h,
+                                                    sm_scale, st);
+    return launch_dense_bwd<__half, false>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, nullptr, nullptr, h, sm_scale, st);
   }
   if (dtype == TDB200_DTYPE_BF16)
-    return launch_dense_bwd<__nv_bfloat16, true>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, k_lens, h, sm_scale, st);
-  return launch_dense_bwd<__half, true>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, k_lens, h, sm_scale, st);
+    return launch_dense_bwd<__nv_bfloat16, true>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, nullptr, k_lens, h, sm_scale,
+                                                 st);
+  return launch_dense_bwd<__half, true>(q, k, v, out, d_out, lse, dq, dk, dv, delta, b, lq, lk, nullptr, k_lens, h, sm_scale, st);
 }
 
 }  // namespace
@@ -1027,13 +1077,21 @@ extern "C" int tdb200_attn_dense_bwd(const void* q, const void* k, const void* v
                                      int dtype, void* dq, void* dk, void* dv, void* workspace, int64_t workspace_bytes, int64_t b,
                                      int64_t lq, int64_t lk, int64_t h, int64_t d, float sm_scale, void* stream) {
   return dense_bwd("attn_dense_bwd", q, k, v, out, d_out, lse, dtype, dq, dk, dv, workspace, workspace_bytes, b, lq, lk, nullptr, false,
-                   h, d, sm_scale, stream);
+                   nullptr, false, h, d, sm_scale, stream);
 }
 
 extern "C" int tdb200_attn_dense_bwd_kl(const void* q, const void* k, const void* v, const void* out, const void* d_out,
                                         const float* lse, int dtype, void* dq, void* dk, void* dv, void* workspace,
                                         int64_t workspace_bytes, int64_t b, int64_t lq, int64_t lk, const int32_t* k_lens, int64_t h,
                                         int64_t d, float sm_scale, void* stream) {
-  return dense_bwd("attn_dense_bwd_kl", q, k, v, out, d_out, lse, dtype, dq, dk, dv, workspace, workspace_bytes, b, lq, lk, k_lens,
-                   true, h, d, sm_scale, stream);
+  return dense_bwd("attn_dense_bwd_kl", q, k, v, out, d_out, lse, dtype, dq, dk, dv, workspace, workspace_bytes, b, lq, lk, nullptr,
+                   false, k_lens, true, h, d, sm_scale, stream);
+}
+
+extern "C" int tdb200_attn_dense_bwd_vl(const void* q, const void* k, const void* v, const void* out, const void* d_out,
+                                        const float* lse, int dtype, void* dq, void* dk, void* dv, void* workspace,
+                                        int64_t workspace_bytes, int64_t b, int64_t lq, int64_t lk, const int32_t* q_lens,
+                                        const int32_t* k_lens, int64_t h, int64_t d, float sm_scale, void* stream) {
+  return dense_bwd("attn_dense_bwd_vl", q, k, v, out, d_out, lse, dtype, dq, dk, dv, workspace, workspace_bytes, b, lq, lk, q_lens,
+                   true, k_lens, true, h, d, sm_scale, stream);
 }

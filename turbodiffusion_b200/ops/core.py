@@ -342,32 +342,52 @@ def _dense_args(what, q, k, v):
     return q.dtype if q.dtype in DTYPE_TAG else torch.bfloat16
 
 
-def _key_lens(what, k_lens, b: int, lk: int, device) -> Optional[torch.Tensor]:
-    """The k_lens argument of dense_attention / dense_attention_jvp as the int32 [b] device tensor the _kl entry points read, or
-    None.  An integer [b] tensor holds the key lengths; a boolean [b, lk] key-padding mask (True = keep) is turned into them and
-    refused unless each row is a run of Trues followed by Falses (for a CUDA mask that check synchronises once).  Lengths the
-    caller hands in on the CPU are checked against [0, lk]; CUDA lengths are not read on the host (no synchronisation): wider
-    integer types are clamped to [0, lk] on their device before they are narrowed to int32, and the kernels clamp int32
-    lengths to [0, lk]."""
-    if k_lens is None:
+def _lengths(what, lens, b: int, l: int, device, name: str, side: str, dim: str) -> Optional[torch.Tensor]:
+    """A per-sample length argument of dense_attention / dense_attention_jvp (`name`: k_lens or q_lens, over the `side` rows,
+    key or query, of length `dim` = l) as the int32 [b] device tensor the _kl / _vl entry points read, or None.  An integer [b]
+    tensor holds the lengths; a boolean [b, l] padding mask (True = keep) is turned into them and refused unless each row is a
+    run of Trues followed by Falses (for a CUDA mask that check synchronises once).  Lengths the caller hands in on the CPU are
+    checked against [0, l]; CUDA lengths are not read on the host (no synchronisation): wider integer types are clamped to
+    [0, l] on their device before they are narrowed to int32, and the kernels clamp int32 lengths to [0, l]."""
+    if lens is None:
         return None
-    if not isinstance(k_lens, torch.Tensor):
-        raise TypeError(f"{what}: k_lens must be a tensor, got {type(k_lens).__name__}")
-    if k_lens.dtype == torch.bool:
-        if tuple(k_lens.shape) != (b, lk):
-            raise ValueError(f"{what}: a boolean k_lens is a key-padding mask [B, Lk] = {(b, lk)}, got {tuple(k_lens.shape)}")
-        lens = k_lens.sum(dim=1)
-        if not torch.equal(torch.arange(lk, device=k_lens.device) < lens[:, None], k_lens):
-            raise ValueError(f"{what}: the key-padding mask must keep a prefix of every row (Trues, then Falses)")
-        k_lens = lens
-    elif k_lens.is_floating_point() or k_lens.is_complex() or tuple(k_lens.shape) != (b,):
-        raise ValueError(f"{what}: k_lens must be an integer tensor [B] = [{b}] or a boolean mask [B, Lk], got "
-                         f"{k_lens.dtype} {tuple(k_lens.shape)}")
-    elif not k_lens.is_cuda and b and (int(k_lens.min()) < 0 or int(k_lens.max()) > lk):
-        raise ValueError(f"{what}: k_lens {k_lens.tolist()} outside [0, Lk = {lk}]")
-    if k_lens.dtype != torch.int32:   # widen, then clamp, then narrow: no length wraps around into [0, lk]
-        k_lens = k_lens.to(torch.int64).clamp(0, lk)
-    return k_lens.to(device=device, dtype=torch.int32).contiguous()
+    if not isinstance(lens, torch.Tensor):
+        raise TypeError(f"{what}: {name} must be a tensor, got {type(lens).__name__}")
+    if lens.dtype == torch.bool:
+        if tuple(lens.shape) != (b, l):
+            raise ValueError(f"{what}: a boolean {name} is a {side}-padding mask [B, {dim}] = {(b, l)}, got {tuple(lens.shape)}")
+        n = lens.sum(dim=1)
+        if not torch.equal(torch.arange(l, device=lens.device) < n[:, None], lens):
+            raise ValueError(f"{what}: the {side}-padding mask must keep a prefix of every row (Trues, then Falses)")
+        lens = n
+    elif lens.is_floating_point() or lens.is_complex() or tuple(lens.shape) != (b,):
+        raise ValueError(f"{what}: {name} must be an integer tensor [B] = [{b}] or a boolean mask [B, {dim}], got "
+                         f"{lens.dtype} {tuple(lens.shape)}")
+    elif not lens.is_cuda and b and (int(lens.min()) < 0 or int(lens.max()) > l):
+        raise ValueError(f"{what}: {name} {lens.tolist()} outside [0, {dim} = {l}]")
+    if lens.dtype != torch.int32:   # widen, then clamp, then narrow: no length wraps around into [0, l]
+        lens = lens.to(torch.int64).clamp(0, l)
+    return lens.to(device=device, dtype=torch.int32).contiguous()
+
+
+def _key_lens(what, k_lens, b: int, lk: int, device) -> Optional[torch.Tensor]:
+    """The k_lens argument (key lengths, or a [b, lk] key-padding mask) as _lengths returns it."""
+    return _lengths(what, k_lens, b, lk, device, "k_lens", "key", "Lk")
+
+
+def _query_lens(what, q_lens, b: int, lq: int, device) -> Optional[torch.Tensor]:
+    """The q_lens argument (query lengths, or a [b, lq] query-padding mask) as _lengths returns it."""
+    return _lengths(what, q_lens, b, lq, device, "q_lens", "query", "Lq")
+
+
+def _seq_lens(what, q_lens, k_lens, b: int, lq: int, lk: int, device):
+    """(q_lens, k_lens) as the entry points take them: (None, None) or (None, k) for the plain and _kl entry points, and with
+    query lengths (q, k) for the _vl ones, k filled with lk when the caller gave query lengths only."""
+    kl = _key_lens(what, k_lens, b, lk, device)
+    ql = _query_lens(what, q_lens, b, lq, device)
+    if ql is not None and kl is None:
+        kl = torch.full((b,), lk, dtype=torch.int32, device=device)
+    return ql, kl
 
 
 def _needs_grad(*tensors) -> bool:
@@ -375,12 +395,17 @@ def _needs_grad(*tensors) -> bool:
     return torch.is_grad_enabled() and any(t.requires_grad for t in tensors)
 
 
-def _dense_fwd_lse(q, k, v, sm_scale, k_lens):
-    """(out, lse) of tdb200_attn_dense_fwd_lse, or with k_lens of tdb200_attn_dense_fwd_lse_kl."""
+def _dense_fwd_lse(q, k, v, sm_scale, k_lens, q_lens):
+    """(out, lse) of tdb200_attn_dense_fwd_lse, or with k_lens of tdb200_attn_dense_fwd_lse_kl, or with q_lens (and k_lens) of
+    tdb200_attn_dense_fwd_lse_vl."""
     b, lq, h, d = q.shape
     out = torch.empty_like(q)
     lse = torch.empty(b, h, lq, dtype=torch.float32, device=q.device)
-    if k_lens is None:
+    if q_lens is not None:
+        check(lib().tdb200_attn_dense_fwd_lse_vl(ptr(q), ptr(k), ptr(v), DTYPE_TAG[q.dtype], ptr(out), ptr(lse), b, lq, k.shape[1],
+                                                 ptr(q_lens), ptr(k_lens), h, d, sm_scale, stream_ptr(q.device)),
+              "attn_dense_fwd_lse_vl")
+    elif k_lens is None:
         check(lib().tdb200_attn_dense_fwd_lse(ptr(q), ptr(k), ptr(v), DTYPE_TAG[q.dtype], ptr(out), ptr(lse), b, lq, k.shape[1], h, d,
                                               sm_scale, stream_ptr(q.device)), "attn_dense_fwd_lse")
     else:
@@ -390,9 +415,9 @@ def _dense_fwd_lse(q, k, v, sm_scale, k_lens):
 
 
 def _dense_bwd(ctx, d_out):
-    """(dq, dk, dv) from tdb200_attn_dense_bwd (or, with the k_lens the forward saved, tdb200_attn_dense_bwd_kl), for the
-    tensors the lse forward saved."""
-    q, k, v, out, lse, k_lens = ctx.saved_tensors
+    """(dq, dk, dv) from tdb200_attn_dense_bwd (or, with the k_lens the forward saved, tdb200_attn_dense_bwd_kl, and with its
+    q_lens tdb200_attn_dense_bwd_vl), for the tensors the lse forward saved."""
+    q, k, v, out, lse, k_lens, q_lens = ctx.saved_tensors
     b, lq, h, d = q.shape
     lk = k.shape[1]
     d_out = d_out.to(q.dtype).contiguous()
@@ -400,7 +425,12 @@ def _dense_bwd(ctx, d_out):
     nbytes = lib().tdb200_attn_dense_bwd_workspace_bytes(b, h, lq)
     check(0 if nbytes >= 0 else nbytes, "attn_dense_bwd_workspace_bytes", launches=0)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
-    if k_lens is None:
+    if q_lens is not None:
+        check(lib().tdb200_attn_dense_bwd_vl(ptr(q), ptr(k), ptr(v), ptr(out), ptr(d_out), ptr(lse), DTYPE_TAG[q.dtype], ptr(dq),
+                                             ptr(dk), ptr(dv), ptr(ws), nbytes, b, lq, lk, ptr(q_lens), ptr(k_lens), h, d, ctx.sm_scale,
+                                             stream_ptr(q.device)),
+              "attn_dense_bwd_vl")
+    elif k_lens is None:
         check(lib().tdb200_attn_dense_bwd(ptr(q), ptr(k), ptr(v), ptr(out), ptr(d_out), ptr(lse), DTYPE_TAG[q.dtype], ptr(dq), ptr(dk),
                                           ptr(dv), ptr(ws), nbytes, b, lq, lk, h, d, ctx.sm_scale, stream_ptr(q.device)),
               "attn_dense_bwd")
@@ -413,30 +443,36 @@ def _dense_bwd(ctx, d_out):
 
 
 class _DenseAttention(torch.autograd.Function):
-    """dense_attention's training path on 16-bit contiguous q, k, v: the lse forward, and the dense backward.  k_lens (int32 [b]
-    on the device, or None) is not differentiable; when set, both run their _kl twins."""
+    """dense_attention's training path on 16-bit contiguous q, k, v: the lse forward, and the dense backward.  k_lens and q_lens
+    (int32 [b] on the device, or None) are not differentiable; with k_lens alone both run their _kl twins, with q_lens (and
+    k_lens) their _vl twins."""
 
     @staticmethod
-    def forward(ctx, q, k, v, sm_scale, k_lens):
-        out, lse = _dense_fwd_lse(q, k, v, sm_scale, k_lens)
-        ctx.save_for_backward(q, k, v, out, lse, k_lens)
+    def forward(ctx, q, k, v, sm_scale, k_lens, q_lens):
+        out, lse = _dense_fwd_lse(q, k, v, sm_scale, k_lens, q_lens)
+        ctx.save_for_backward(q, k, v, out, lse, k_lens, q_lens)
         ctx.sm_scale = sm_scale
         return out
 
     @staticmethod
     def backward(ctx, d_out):
-        return (*_dense_bwd(ctx, d_out), None, None)
+        return (*_dense_bwd(ctx, d_out), None, None, None)
 
 
 class _DenseAttentionJvp(torch.autograd.Function):
     """dense_attention_jvp's training path: out differentiable in q, k and v; out_t, and the tangents, carry no gradient."""
 
     @staticmethod
-    def forward(ctx, q, k, v, q_t, k_t, v_t, sm_scale, k_lens):
+    def forward(ctx, q, k, v, q_t, k_t, v_t, sm_scale, k_lens, q_lens):
         b, lq, h, d = q.shape
         out, out_t = torch.empty_like(q), torch.empty_like(q)
         lse = torch.empty(b, h, lq, dtype=torch.float32, device=q.device)
-        if k_lens is None:
+        if q_lens is not None:
+            check(lib().tdb200_attn_dense_jvp_lse_vl(ptr(q), ptr(k), ptr(v), ptr(q_t), ptr(k_t), ptr(v_t), DTYPE_TAG[q.dtype],
+                                                     ptr(out), ptr(out_t), ptr(lse), b, lq, k.shape[1], ptr(q_lens), ptr(k_lens), h,
+                                                     d, sm_scale, stream_ptr(q.device)),
+                  "attn_dense_jvp_lse_vl")
+        elif k_lens is None:
             check(lib().tdb200_attn_dense_jvp_lse(ptr(q), ptr(k), ptr(v), ptr(q_t), ptr(k_t), ptr(v_t), DTYPE_TAG[q.dtype], ptr(out),
                                                   ptr(out_t), ptr(lse), b, lq, k.shape[1], h, d, sm_scale, stream_ptr(q.device)),
                   "attn_dense_jvp_lse")
@@ -447,15 +483,15 @@ class _DenseAttentionJvp(torch.autograd.Function):
                   "attn_dense_jvp_lse_kl")
         ctx.mark_non_differentiable(out_t)
         ctx.set_materialize_grads(False)    # out_t's gradient is never used: no zero tensor for it
-        ctx.save_for_backward(q, k, v, out, lse, k_lens)
+        ctx.save_for_backward(q, k, v, out, lse, k_lens, q_lens)
         ctx.sm_scale = sm_scale
         return out, out_t
 
     @staticmethod
     def backward(ctx, d_out, d_out_t):
         if d_out is None:
-            return (None,) * 8
-        return (*_dense_bwd(ctx, d_out), None, None, None, None, None)
+            return (None,) * 9
+        return (*_dense_bwd(ctx, d_out), None, None, None, None, None, None)
 
 
 class _DenseAttentionAD(torch.autograd.Function):
@@ -464,28 +500,33 @@ class _DenseAttentionAD(torch.autograd.Function):
     backward.  lse is an output only so that setup_context can save it.  The tangent carries no gradient."""
 
     @staticmethod
-    def forward(q, k, v, sm_scale, k_lens):
-        return _dense_fwd_lse(q, k, v, sm_scale, k_lens)
+    def forward(q, k, v, sm_scale, k_lens, q_lens):
+        return _dense_fwd_lse(q, k, v, sm_scale, k_lens, q_lens)
 
     @staticmethod
     def setup_context(ctx, inputs, output):
-        q, k, v, sm_scale, k_lens = inputs
+        q, k, v, sm_scale, k_lens, q_lens = inputs
         out, lse = output
         ctx.mark_non_differentiable(lse)
         ctx.set_materialize_grads(False)
-        ctx.save_for_backward(q, k, v, out, lse, k_lens)
-        ctx.save_for_forward(q, k, v, out, lse, k_lens)
+        ctx.save_for_backward(q, k, v, out, lse, k_lens, q_lens)
+        ctx.save_for_forward(q, k, v, out, lse, k_lens, q_lens)
         ctx.sm_scale = sm_scale
 
     @staticmethod
     def jvp(ctx, q_t, k_t, v_t, *_):
         with torch._C._DisableFuncTorch():
-            q, k, v, out, lse, k_lens = (plain(t) for t in ctx.saved_tensors)
+            q, k, v, out, lse, k_lens, q_lens = (plain(t) for t in ctx.saved_tensors)
             q_t, k_t, v_t = (torch.zeros_like(p) if t is None else plain(t).detach().to(p.dtype).contiguous()
                              for t, p in ((q_t, q), (k_t, k), (v_t, v)))
             b, lq, h, d = q.shape
             out_t = torch.empty_like(q)
-            if k_lens is None:
+            if q_lens is not None:
+                check(lib().tdb200_attn_dense_tangent_vl(ptr(q), ptr(k), ptr(v), ptr(q_t), ptr(k_t), ptr(v_t), ptr(out), ptr(lse),
+                                                         DTYPE_TAG[q.dtype], ptr(out_t), b, lq, k.shape[1], ptr(q_lens),
+                                                         ptr(k_lens), h, d, ctx.sm_scale, stream_ptr(q.device)),
+                      "attn_dense_tangent_vl")
+            elif k_lens is None:
                 check(lib().tdb200_attn_dense_tangent(ptr(q), ptr(k), ptr(v), ptr(q_t), ptr(k_t), ptr(v_t), ptr(out), ptr(lse),
                                                       DTYPE_TAG[q.dtype], ptr(out_t), b, lq, k.shape[1], h, d, ctx.sm_scale,
                                                       stream_ptr(q.device)), "attn_dense_tangent")
@@ -498,12 +539,12 @@ class _DenseAttentionAD(torch.autograd.Function):
     @staticmethod
     def backward(ctx, d_out, d_lse):
         if d_out is None:
-            return None, None, None, None, None
-        return (*_dense_bwd(ctx, d_out), None, None)
+            return None, None, None, None, None, None
+        return (*_dense_bwd(ctx, d_out), None, None, None)
 
 
 def dense_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, sm_scale: Optional[float] = None,
-                    k_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
+                    k_lens: Optional[torch.Tensor] = None, q_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
     """softmax(q.k^T * sm_scale).v per (batch, head), the reference's dense attention (rcm/utils/attention.py:120-167):
     q [B, Lq, H, D], k and v [B, Lk, H, D], D = 128, any Lq and Lk; returns [B, Lq, H, D] in q's dtype.  bf16 / fp16 inputs run
     in their own type, any other float type in bf16.  sm_scale defaults to D ** -0.5.  One kernel on the current stream
@@ -521,19 +562,33 @@ def dense_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, sm_scale:
     tangent alike; the gradients of keys and values past k_lens[i] are zero, and an entry with no keys gets out = 0.  What the
     rows of k and v (and of their tangents) past k_lens[i] hold, inf and NaN included, does not reach any output: the kernels
     do not load whole key tiles past it, and zero the rows past it in the tile they do load.  Lengths on the CPU are checked
-    against [0, Lk]; lengths on a CUDA device are used without a synchronisation, clamped to [0, Lk]."""
+    against [0, Lk]; lengths on a CUDA device are used without a synchronisation, clamped to [0, Lk].
+
+    q_lens: a query-padding mask, for self-attention over a padded batch (clips of different token counts packed to one Lq):
+    an integer tensor [B] on any device, batch entry i owning query rows 0 .. q_lens[i] - 1 of its own Lq, or a boolean mask
+    [B, Lq] (True = keep) whose rows keep a prefix; lengths are checked or clamped to [0, Lq] as k_lens are.  Entry i's rows
+    below q_lens[i] get the bits of this operator called on entry i alone with q cut to those rows (and k, v cut by k_lens when
+    given), in the forward, the backward and the tangent alike, and so do its key and value gradients; rows past q_lens[i] get
+    out = 0 (and out_t = 0, and a zero gradient), and add nothing to the key and value gradients.  What the rows of q, of its
+    tangent and of the output gradient past q_lens[i] hold, inf and NaN included, does not reach any output: query blocks wholly
+    past it are not computed, and the backward zeroes the rows past it on chip in the block it loads.  With q_lens the calls
+    run the _vl entry points (tdb200_attn_dense_fwd_vl and its twins), given k_lens filled with Lk when k_lens is None."""
     require_cuda(q, k, v)
     dtype = _dense_args("dense_attention", q, k, v)
     qc, kc, vc = (t.to(dtype).contiguous() for t in (q, k, v))
     b, lq, h, d = qc.shape
     sm_scale = float(d ** -0.5 if sm_scale is None else sm_scale)
-    kl = _key_lens("dense_attention", k_lens, b, kc.shape[1], qc.device)
+    ql, kl = _seq_lens("dense_attention", q_lens, k_lens, b, lq, kc.shape[1], qc.device)
     if has_tangent(q, k, v):
-        return _DenseAttentionAD.apply(qc, kc, vc, sm_scale, kl)[0].to(q.dtype)
+        return _DenseAttentionAD.apply(qc, kc, vc, sm_scale, kl, ql)[0].to(q.dtype)
     if _needs_grad(q, k, v):
-        return _DenseAttention.apply(qc, kc, vc, sm_scale, kl).to(q.dtype)
+        return _DenseAttention.apply(qc, kc, vc, sm_scale, kl, ql).to(q.dtype)
     out = torch.empty_like(qc)
-    if kl is None:
+    if ql is not None:
+        check(lib().tdb200_attn_dense_fwd_vl(ptr(qc), ptr(kc), ptr(vc), DTYPE_TAG[dtype], ptr(out), b, lq, kc.shape[1], ptr(ql),
+                                             ptr(kl), h, d, sm_scale, stream_ptr(qc.device)),
+              "attn_dense_fwd_vl")
+    elif kl is None:
         check(lib().tdb200_attn_dense_fwd(ptr(qc), ptr(kc), ptr(vc), DTYPE_TAG[dtype], ptr(out), b, lq, kc.shape[1], h, d, sm_scale,
                                           stream_ptr(qc.device)),
               "attn_dense_fwd")
@@ -546,15 +601,17 @@ def dense_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, sm_scale:
 
 def dense_attention_jvp(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, q_t: torch.Tensor, k_t: torch.Tensor,
                         v_t: torch.Tensor, sm_scale: Optional[float] = None,
-                        k_lens: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+                        k_lens: Optional[torch.Tensor] = None,
+                        q_lens: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """dense_attention(q, k, v) and its forward-mode derivative along the tangents (q_t, k_t, v_t), from one kernel
     (tdb200_attn_dense_jvp): (out, out_t) with out_t = sum_j P_j S_t,j v_j - (sum_j P_j S_t,j) out + P.v_t, S_t =
     sm_scale (q_t.k^T + q.k_t^T).  Shapes and dtype rules as dense_attention; each tangent has its primal's shape and runs in
     the primal's 16-bit type.  Both outputs are [B, Lq, H, D] in q's dtype.  With grad enabled and any of q, k, v requiring
     grad, out is differentiable in q, k and v (tdb200_attn_dense_jvp_lse, the same bits, then tdb200_attn_dense_bwd), as a
     consistency-distillation loss needs; out_t never carries a gradient (a stop-gradient target) and the tangents get none.
-    k_lens: per-sample key lengths or a prefix key-padding mask, as for dense_attention (tdb200_attn_dense_jvp_kl).  Not a
-    `tdb200::` operator: eager use."""
+    k_lens: per-sample key lengths or a prefix key-padding mask, as for dense_attention (tdb200_attn_dense_jvp_kl).  q_lens:
+    per-sample query lengths or a prefix query-padding mask, as for dense_attention (tdb200_attn_dense_jvp_vl); rows past
+    q_lens[i] get out = out_t = 0.  Not a `tdb200::` operator: eager use."""
     require_cuda(q, k, v, q_t, k_t, v_t)
     dtype = _dense_args("dense_attention_jvp", q, k, v)
     for name, t, primal in (("q_t", q_t, q), ("k_t", k_t, k), ("v_t", v_t, v)):
@@ -563,12 +620,16 @@ def dense_attention_jvp(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, q_t: 
     qc, kc, vc, qtc, ktc, vtc = (t.to(dtype).contiguous() for t in (q, k, v, q_t, k_t, v_t))
     b, lq, h, d = qc.shape
     sm_scale = float(d ** -0.5 if sm_scale is None else sm_scale)
-    kl = _key_lens("dense_attention_jvp", k_lens, b, kc.shape[1], qc.device)
+    ql, kl = _seq_lens("dense_attention_jvp", q_lens, k_lens, b, lq, kc.shape[1], qc.device)
     if _needs_grad(q, k, v):
-        out, out_t = _DenseAttentionJvp.apply(qc, kc, vc, qtc, ktc, vtc, sm_scale, kl)
+        out, out_t = _DenseAttentionJvp.apply(qc, kc, vc, qtc, ktc, vtc, sm_scale, kl, ql)
         return out.to(q.dtype), out_t.to(q.dtype)
     out, out_t = torch.empty_like(qc), torch.empty_like(qc)
-    if kl is None:
+    if ql is not None:
+        check(lib().tdb200_attn_dense_jvp_vl(ptr(qc), ptr(kc), ptr(vc), ptr(qtc), ptr(ktc), ptr(vtc), DTYPE_TAG[dtype], ptr(out),
+                                             ptr(out_t), b, lq, kc.shape[1], ptr(ql), ptr(kl), h, d, sm_scale, stream_ptr(qc.device)),
+              "attn_dense_jvp_vl")
+    elif kl is None:
         check(lib().tdb200_attn_dense_jvp(ptr(qc), ptr(kc), ptr(vc), ptr(qtc), ptr(ktc), ptr(vtc), DTYPE_TAG[dtype], ptr(out),
                                           ptr(out_t), b, lq, kc.shape[1], h, d, sm_scale, stream_ptr(qc.device)),
               "attn_dense_jvp")

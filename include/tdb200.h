@@ -207,6 +207,34 @@ int tdb200_sla_attn_fwd(const int8_t* q_i8, const float* q_scale, const int8_t* 
                         const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
                         int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq, int64_t blkk,
                         int k_seq_major, void* stream);
+/* Per-entry lengths (the _vl twins; inference only, d = 128, lq = lk = l): a padded batch whose entry i owns its first
+ * seq_lens[i] rows of q, k and v (seq_lens [b] device int32, clamped to [0, l] on the device).  Entry i's results over those
+ * rows are the bits of the entry point without `_vl` called on entry i alone, cut to those rows: its own key mean, pooled means
+ * and scales, its own mblk_i = ceil(n_i / blkq), nblk_i = ceil(n_i / blkk) and topks[i] blocks per row (device int32, clamped to
+ * [1, min(nblk_i, topk)]), its own moments (the split count and summation order tdb200_sla_linear_moments picks for n_i rows),
+ * and keys masked at n_i.  Output rows past n_i are 0; what q, k and v hold past n_i, inf and NaN included, reaches no result.
+ * tdb200_sla_quant_qk_vl       one length for both halves; either half may be NULL as for tdb200_sla_quant_qk.  Rows past n_i
+ *                              of the INT8 codes are not written; blocks wholly past n_i pool to 0.
+ * tdb200_sla_block_map_vl      blkq, blkk: the block sizes of the pools.  LUT [b,h,mblk,topk] keeps the row stride `topk`, the
+ *                              largest topks[i]; LUT entries past topks[i] and rows past mblk_i are -1, sparse_map is 0 there.
+ * tdb200_sla_linear_moments_vl accumulated like tdb200_sla_linear_moments (the caller zeroes kv and ksum).
+ * tdb200_sla_attn_fwd_vl       INT8 Q/K with head-major K, (blkq, blkk) = (128, 64) or (64, 128), 16-bit P.V.
+ * tdb200_sla_attn16_fwd_vl     (blkq, blkk) = (128, 64) or (64, 64).
+ * Errors as their twins; a null or misaligned seq_lens or topks is TDB200_ERR_INVALID_ARG, d != 128 TDB200_ERR_UNSUPPORTED,
+ * l != lk (attention) TDB200_ERR_INVALID_ARG, all before any CUDA call. */
+int tdb200_sla_quant_qk_vl(const void* q, const void* k, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
+                           const int32_t* seq_lens, float* kmean, int8_t* q_i8, float* q_scale, int8_t* k_i8, float* k_scale,
+                           void* q_pool, void* k_pool, int64_t blkq, int64_t blkk, void* stream);
+int tdb200_sla_block_map_vl(const void* q_pool, const void* k_pool, int dtype, int64_t b, int64_t h, int64_t mblk, int64_t nblk,
+                            int64_t d, int64_t topk, const int32_t* seq_lens, const int32_t* topks, int64_t blkq, int64_t blkk,
+                            int8_t* sparse_map, int32_t* lut, void* stream);
+int tdb200_sla_linear_moments_vl(const void* k, const void* v, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
+                                 const int32_t* seq_lens, int feature, float* kv, float* ksum, void* stream);
+int tdb200_sla_attn_fwd_vl(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
+                           const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk, const void* kvw,
+                           const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk, int64_t h,
+                           int64_t d, const int32_t* seq_lens, const int32_t* topks, float sm_scale, int feature, int64_t blkq,
+                           int64_t blkk, void* stream);
 /* SageSLA with FP8 P.V (SageAttention2's arithmetic: e4m3 P and V, per-channel V scales), an option beside the 16-bit P.V of
  * tdb200_sla_attn_fwd; d = 128 only.
  * tdb200_sla_quant_v_fp8  v [b,l,h,d] 16-bit (`dtype`) -> v_scale [b,h,d] fp32 and v_fp8 [b,h,d,l_pad] e4m3 codes, l_pad =
@@ -313,6 +341,11 @@ int tdb200_sla_quant_k_seq(const void* k, const float* kmean, int dtype, int64_t
 int tdb200_sla_attn16_fwd(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
                           const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
                           int64_t h, int64_t d, float sm_scale, int feature, int64_t blkq, int64_t blkk, void* stream);
+/* tdb200_sla_attn16_fwd with per-entry lengths: see tdb200_sla_attn_fwd_vl above. */
+int tdb200_sla_attn16_fwd_vl(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
+                             const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
+                             int64_t h, int64_t d, const int32_t* seq_lens, const int32_t* topks, float sm_scale, int feature,
+                             int64_t blkq, int64_t blkk, void* stream);
 int tdb200_sla_attn16_fwd_lse(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk, void* o_s,
                               float* lse, int64_t b, int64_t l, int64_t h, int64_t d, float sm_scale, int64_t blkq, int64_t blkk,
                               void* stream);

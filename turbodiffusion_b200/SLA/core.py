@@ -36,6 +36,16 @@ def linear_moments(k: torch.Tensor, v: torch.Tensor, feature: int = 0):
     return buf[: b * h * d * d].view(b, h, d, d), buf[b * h * d * d:].view(b, h, d)
 
 
+def linear_moments_vl(k: torch.Tensor, v: torch.Tensor, seq_lens: torch.Tensor, feature: int = 0):
+    """linear_moments per entry of a padded batch (tdb200_sla_linear_moments_vl): entry i's kv [H,D,D] and ksum [H,D] over its
+    first seq_lens[i] rows, the bits of linear_moments on entry i alone cut to those rows.  D = 128."""
+    b, l, h, d = k.shape
+    buf = torch.zeros(b * h * d * (d + 1), dtype=torch.float32, device=k.device)
+    check(lib().tdb200_sla_linear_moments_vl(ptr(k), ptr(v), DTYPE_TAG[k.dtype], b, l, h, d, ptr(seq_lens), feature, ptr(buf),
+                                             ptr(buf) + 4 * b * h * d * d, stream_ptr(k.device)), "sla_linear_moments_vl")
+    return buf[: b * h * d * d].view(b, h, d, d), buf[b * h * d * d:].view(b, h, d)
+
+
 def project_moments(proj_w: torch.Tensor, kv: torch.Tensor, dtype) -> torch.Tensor:
     """kvw [B,H,D_out,D_k] = T(proj_w . kv): proj_l's weight folded into the moment matrix (the fused kernel's last MMA)."""
     b, h, d, _ = kv.shape
@@ -325,11 +335,24 @@ class _SLABase(nn.Module):
             nn.init.zeros_(self.proj_l.weight)
             nn.init.zeros_(self.proj_l.bias)
 
-    def forward(self, q, k, v, return_sparsity=False):
+    def forward(self, q, k, v, return_sparsity=False, seq_lens=None):
         """q,k,v [B, L, H, D] (any float dtype), D in {64, 128} (SLA/core.py:207) -> [B, L, H, D] in q.dtype.
         SparseLinearAttention with grad enabled and any of q, k, v requiring grad takes the differentiable training path
         (_forward_train); every other call runs the fused forward-only kernels.  When any of q, k, v carries a forward-mode
-        tangent (torch.func.jvp, torch.autograd.forward_ad), the call takes _forward_ad, whose output carries the tangent."""
+        tangent (torch.func.jvp, torch.autograd.forward_ad), the call takes _forward_ad, whose output carries the tangent.
+
+        seq_lens: per-entry lengths of a padded batch (clips of different token counts packed to one L), an integer tensor [B]
+        or a boolean prefix mask [B, L], as dense_attention's q_lens (ops.core._lengths: CPU lengths are checked, GPU lengths
+        clamped to [0, L] on the device, without a synchronisation).  Entry i's rows below n_i = seq_lens[i] are bit-identical
+        to this module on entry i alone with q, k and v cut to n_i rows: its own key mean, block selection (topk_i = max(1,
+        min(nblk_i, int(topk * nblk_i))) of its own nblk_i key blocks), moments and key mask.  Rows past n_i are 0, and what q, k
+        and v hold there, NaN and inf included, reaches no output.  return_sparsity then gives a float64 [B] tensor of
+        topk_i / nblk_i (0 for an empty entry).  The _keep_selection record (forward_with_lut) keeps "topk" an int, the LUT's
+        row stride, and adds "topks", the int32 [B] topk_i on the device; LUT entries past topk_i are -1.  Inference only, eager only (the _vl entry points are called through ctypes,
+        not `tdb200::` operators), d = 128, 16-bit P.V: grad-requiring inputs, forward-mode tangents, head dim 64 and
+        set_sage_pv("fp8") raise NotImplementedError before any CUDA work."""
+        if seq_lens is not None:
+            return self._forward_vl(q, k, v, return_sparsity, seq_lens)
         if has_tangent(q, k, v):
             return self._forward_ad(q, k, v, return_sparsity)
         if not self.quantised_qk and torch.is_grad_enabled() and any(t.requires_grad for t in (q, k, v)):
@@ -366,6 +389,56 @@ class _SLABase(nn.Module):
                          fp8_v=fp8_v)
         o = o if o.dtype == dtype else o.to(dtype)
         return (o, real_topk / nblk) if return_sparsity else o
+
+    def _forward_vl(self, q, k, v, return_sparsity, seq_lens):
+        """forward() with per-entry lengths: tdb200_sla_quant_qk_vl, _block_map_vl, _linear_moments_vl, then
+        tdb200_sla_attn16_fwd_vl or tdb200_sla_attn_fwd_vl, in the branch forward() takes without lengths."""
+        what = f"{type(self).__name__}.forward with seq_lens"
+        if has_tangent(q, k, v):
+            raise NotImplementedError(f"{what}: inputs carry a forward-mode tangent; per-entry lengths serve inference only")
+        if torch.is_grad_enabled() and any(t.requires_grad for t in (q, k, v)):
+            raise NotImplementedError(f"{what}: inputs require grad; per-entry lengths serve inference only (use torch.no_grad())")
+        if q.shape[-1] != 128:
+            raise NotImplementedError(f"{what}: head dim {q.shape[-1]}; per-entry lengths serve d = 128")
+        if self.quantised_qk and _utils.SAGE_PV == "fp8":
+            raise NotImplementedError(f"{what}: FP8 P.V (SLA.utils.set_sage_pv('fp8')); per-entry lengths serve 16-bit P.V")
+        if not (q.dim() == 4 and q.shape == k.shape == v.shape):
+            raise ValueError(f"{what}: q, k, v [B, L, H, D] of one shape, got {tuple(q.shape)}, {tuple(k.shape)}, {tuple(v.shape)}")
+        require_cuda(q, k, v)
+        from ..ops.core import _lengths
+        dtype = q.dtype
+        q, k, v = (t if (t.dtype == self.dtype and t.is_contiguous()) else t.to(self.dtype).contiguous() for t in (q, k, v))
+        b, l, h, d = q.shape
+        # clamped here too (int32 device lengths reach the kernels unclamped): topk_i and the sparsity then count the n_i the
+        # kernels use, on the device, without a synchronisation
+        lens = _lengths(what, seq_lens, b, l, q.device, "seq_lens", "sequence", "L").clamp(0, l)
+        blkq, blkk = self.block_sizes(q.device.index)
+        nblk = _utils.cdiv(l, blkk)
+        topk = max(1, min(nblk, int(self.topk * nblk)))   # the LUT's row stride: no entry keeps more
+        prep = _utils.quant_qk_vl(q, k, lens, blkq, blkk)
+        topks = _utils.seq_topks(lens, self.topk, blkk)   # after the prep launches: its small ops then run under them
+        sparse_map, lut = _utils.block_map_vl(prep.q_pool, prep.k_pool, topk, lens, topks, blkq, blkk)
+        if getattr(self, "_keep_selection", None) is not None:
+            self._keep_selection.update(lut=lut, sparse_map=sparse_map, topk=topk, topks=topks)
+        kv, ksum = linear_moments_vl(k, v, lens, self.feature)
+        kvw = project_moments(self.proj_l.weight.detach(), kv, self.dtype)
+        proj_b = self.proj_l.bias.detach().float().contiguous()
+        out = torch.empty_like(q)
+        sm_scale = d ** -0.5
+        if not self.quantised_qk and (self.feature == 0 or blkq == 64):
+            check(lib().tdb200_sla_attn16_fwd_vl(ptr(q), ptr(k), ptr(v), DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum),
+                                                 ptr(proj_b), ptr(out), b, l, l, h, d, ptr(lens), ptr(topks), sm_scale,
+                                                 self.feature, blkq, blkk, stream_ptr(q.device)), "sla_attn16_fwd_vl")
+        else:
+            check(lib().tdb200_sla_attn_fwd_vl(ptr(prep.q_i8), ptr(prep.q_scale), ptr(prep.k_i8), ptr(prep.k_scale), ptr(v), ptr(q),
+                                               DTYPE_TAG[q.dtype], ptr(lut), topk, ptr(kvw), ptr(ksum), ptr(proj_b), ptr(out), b, l, l,
+                                               h, d, ptr(lens), ptr(topks), sm_scale, self.feature, blkq, blkk,
+                                               stream_ptr(q.device)), "sla_attn_fwd_vl")
+        o = out if out.dtype == dtype else out.to(dtype)
+        if not return_sparsity:
+            return o
+        nblk_i = (lens.to(torch.int64) + blkk - 1) // blkk
+        return o, torch.where(nblk_i > 0, topks.to(torch.float64) / nblk_i.clamp(min=1).to(torch.float64), 0.0)
 
     def _forward_train(self, q, k, v, return_sparsity):
         """The reference's SparseLinearAttention.forward (SLA/core.py:81-119) with autograd: the same block selection as the

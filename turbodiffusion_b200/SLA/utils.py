@@ -159,6 +159,57 @@ def quant_k_seq(k: torch.Tensor, kmean: torch.Tensor, k_i8=None, blkk: int = 64)
     return k_i8, k_scale, k_pool
 
 
+def seq_topks(seq_lens: torch.Tensor, ratio, blkk: int) -> torch.Tensor:
+    """Per-entry blocks per row for lengths seq_lens (int32 [B]): topk_i = max(1, min(nblk_i, int(ratio * nblk_i))) with
+    nblk_i = ceil(n_i / blkk), the modules' rule on each entry's own key-block count, evaluated on the lengths' device in float64
+    (Python's int(ratio * nblk) truncates the same float64 product), so device lengths are never read on the host."""
+    nblk = torch.div(seq_lens + (blkk - 1), blkk, rounding_mode="floor")    # lengths are in [0, L]: no int32 overflow
+    nb = nblk.to(torch.float64)
+    # min(nblk, int(x)) == int(min(nblk, x)) for an integer nblk; the conversion truncates toward zero, as int() does
+    return torch.clamp(torch.minimum(nb * float(ratio), nb).to(torch.int32), min=1)
+
+
+def quant_qk_vl(q: torch.Tensor, k: torch.Tensor, seq_lens: torch.Tensor, blkq: int, blkk: int) -> QKPrep:
+    """quant_qk (or, at (64, 64), quant_q_only + quant_k_into) of a padded batch q, k [B, L, H, 128] whose entry i owns its
+    first seq_lens[i] rows (int32 [B] on q's device): tdb200_sla_quant_qk_vl, one call per half where the pair is not a SageSLA
+    family.  Entry i's codes, scales and pools over its rows are those of the call on entry i alone."""
+    require_cuda(q, k, seq_lens)
+    b, l, h, d = q.shape
+    o = QKPrep()
+    o.mblk, o.nblk, o.k_seq_major = cdiv(l, blkq), cdiv(l, blkk), False
+    o.q_i8, o.q_scale, o.q_pool = _ops._q_half(q, blkq)
+    o.kmean, o.k_i8, o.k_scale, o.k_pool = _ops._k_half(k, l, blkk)
+    other = {128: 64, 64: 128}
+    if (blkq, blkk) in SAGE_BLOCKS.values():
+        halves = ((q, k, blkq, blkk),)
+    else:   # the key block size only matters to the key half and the query block size to the query half
+        halves = ((q, None, blkq, other[blkq]), (None, k, other[blkk], blkk))
+    for qq, kk, bq, bk in halves:
+        qh, kh = qq is not None, kk is not None
+        check(lib().tdb200_sla_quant_qk_vl(ptr(qq) if qh else None, ptr(kk) if kh else None, DTYPE_TAG[q.dtype], b, l, h, d,
+                                           ptr(seq_lens), ptr(o.kmean) if kh else None, ptr(o.q_i8) if qh else None,
+                                           ptr(o.q_scale) if qh else None, ptr(o.k_i8) if kh else None,
+                                           ptr(o.k_scale) if kh else None, ptr(o.q_pool) if qh else None,
+                                           ptr(o.k_pool) if kh else None, bq, bk, stream_ptr(q.device)),
+              "sla_quant_qk_vl", launches=(1 if qh else 0) + (3 if kh else 0))
+    return o
+
+
+def block_map_vl(q_pool: torch.Tensor, k_pool: torch.Tensor, topk: int, seq_lens: torch.Tensor, topks: torch.Tensor,
+                 blkq: int, blkk: int):
+    """block_map_from_pools per entry (tdb200_sla_block_map_vl): entry i selects topks[i] of its own ceil(n_i / blkk) key blocks
+    for each of its ceil(n_i / blkq) query blocks.  Returns (sparse_map int8 [B,H,Mblk,Nblk], lut int32 [B,H,Mblk,topk]); LUT
+    entries past topks[i] and rows past entry i's query blocks are -1, the map 0 there."""
+    b, h, mblk, d = q_pool.shape
+    nblk = k_pool.shape[2]
+    sparse_map = torch.empty(b, h, mblk, nblk, dtype=torch.int8, device=q_pool.device)
+    lut = torch.empty(b, h, mblk, topk, dtype=torch.int32, device=q_pool.device)
+    check(lib().tdb200_sla_block_map_vl(ptr(q_pool), ptr(k_pool), DTYPE_TAG[q_pool.dtype], b, h, mblk, nblk, d, topk,
+                                        ptr(seq_lens), ptr(topks), blkq, blkk, ptr(sparse_map), ptr(lut),
+                                        stream_ptr(q_pool.device)), "sla_block_map_vl")
+    return sparse_map, lut
+
+
 def block_map_from_pools(q_pool: torch.Tensor, k_pool: torch.Tensor, topk: int):
     """Pooled score + top-k (SLA/utils.py:59-66).  Returns (sparse_map int8 [B,H,Mblk,Nblk], lut int32 ascending)."""
     return _ops.sla_block_map(q_pool, k_pool, topk)

@@ -89,6 +89,13 @@ _PROTOS = {
     "tdb200_attn_dense_jvp_lse_vl": [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _I64, _I64, _I64, _P, _P, _I64, _I64, _F, _P],
     "tdb200_attn_dense_tangent_vl": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I64, _I64, _I64, _P, _P, _I64, _I64, _F, _P],
     "tdb200_attn_dense_bwd_vl": [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _P, _P, _I64, _I64, _F, _P],
+    "tdb200_sla_quant_qk_vl": [_P, _P, _I, _I64, _I64, _I64, _I64, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _P],
+    "tdb200_sla_block_map_vl": [_P, _P, _I, _I64, _I64, _I64, _I64, _I64, _I64, _P, _P, _I64, _I64, _P, _P, _P],
+    "tdb200_sla_linear_moments_vl": [_P, _P, _I, _I64, _I64, _I64, _I64, _P, _I, _P, _P, _P],
+    "tdb200_sla_attn_fwd_vl": [_P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _P, _P, _F, _I,
+                               _I64, _I64, _P],
+    "tdb200_sla_attn16_fwd_vl": [_P, _P, _P, _I, _P, _I64, _P, _P, _P, _P, _I64, _I64, _I64, _I64, _I64, _P, _P, _F, _I, _I64,
+                                 _I64, _P],
     "tdb200_sla_attn16_tangent": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I64, _P, _I64, _I64, _I64, _I64, _F, _I64, _I64, _P],
     "tdb200_ltx_modulated_rms_norm_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _F, _P],
     "tdb200_ltx_modulate_ada": [_P, _I, _P, _P, _I, _I, _I, _P, _I64, _I64, _I64, _I64, _P],
@@ -163,7 +170,8 @@ class _DeviceGuarded:
 
 LAUNCHES = 0  # kernels launched through the C ABI (each entry point documents how many it enqueues)
 _KERNELS_PER_CALL = {"sla_quant_qk": 4, "layernorm_modulate_quant": 2, "sla_attn16_bwd": 4, "attn_dense_bwd": 3, "attn_dense_bwd_kl": 3, "attn_dense_bwd_vl": 3,
-                     "sla_linear_bwd": 8, "sla_linear_tangent": 5, "sla_quant_v_fp8": 4}  # upper bounds per entry point
+                     "sla_linear_bwd": 8, "sla_linear_tangent": 5, "sla_quant_v_fp8": 4,
+                     "sla_quant_qk_vl": 4}  # upper bounds per entry point
 
 
 def check(rc: int, what: str, launches: int = None) -> None:

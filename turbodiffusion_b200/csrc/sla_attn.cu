@@ -68,7 +68,44 @@ struct AttnParams {
   float sm_scale;
   float* lse;             // [b,h,l] fp32, log2 domain (kLse kernels only)
   const float* v_scale;   // [b,h,d] fp32 (kF8V kernels only)
+  const int32_t* seq_lens;   // [b] int32 (kVL kernels only): entry b's rows, lq = lk
+  const int32_t* topks;      // [b] int32 (kVL kernels only): the LUT entries each of entry b's rows walks
+  const void* v;             // [b,l,h,d] T (kVL 128-row kernels only: the producer's straddling V block)
 };
+
+// kVL (the _vl entry points): entry b owns its first n = seq_lens[b] query and key rows (clamped to [0, l], read once before the
+// first barrier) and walks topks[b] LUT entries, clamped to [1, min(ceil(n / BK), topk)] as the block map clamps them.  Rows past
+// n are stored as zeros; a query block wholly past n stores its zero rows and exits (vl_store_zero_block).  Keys past n are masked
+// as keys past lk are, and the V rows past n of the straddling key block are zero in shared memory before the P.V reads them (TMA
+// would load the padding there, where a call on the entry alone gets zero fill, and 0 * NaN is NaN): in the 128-row kernel the
+// producer warp loads that block itself (vl_load_v_block), in the 64-row kernel its warpgroup zeroes the rows.
+__device__ __forceinline__ int vl_topk(const AttnParams& p, int b, int n, int bk) {
+  return min(max(__ldg(p.topks + b), 1), min((n + bk - 1) / bk, p.topk));
+}
+
+// The 128-row kVL kernel's straddling V block: rows [0, valid) of key block blk of head hh of entry b, the rest zero, written by
+// the producer warp in the layout TMA gives (HD/64 chunks of [BK rows x 128 B], 16-byte units swizzled by row & 7).  The caller
+// then fences the async proxy and arrives on the V-full barrier.
+template <typename T, int HD, int BK>
+__device__ __forceinline__ void vl_load_v_block(uint8_t* sv, const AttnParams& p, int b, int hh, int blk, int valid, int lane) {
+  for (int e = lane; e < BK * (HD / 8); e += 32) {
+    const int r = e / (HD / 8), cu = e % (HD / 8);
+    uint4 x = make_uint4(0u, 0u, 0u, 0u);
+    if (r < valid) x = ldg_nc_v4(static_cast<const T*>(p.v) + ((int64_t(b) * p.l + int64_t(blk) * BK + r) * p.h + hh) * HD + cu * 8);
+    *reinterpret_cast<uint4*>(sv + (cu >> 3) * (BK * 128) + r * 128 + (((cu & 7) ^ (r & 7)) << 4)) = x;
+  }
+}
+
+// rows [row0, min(row0 + rows, l)) of head hh of entry b of the output are zero; every thread of the CTA takes part
+template <int HD>
+__device__ __forceinline__ void vl_store_zero_block(const AttnParams& p, int row0, int rows, int b, int hh) {
+  const int n_rows = min(rows, p.l - row0);
+  uint8_t* base = static_cast<uint8_t*>(p.out);
+  for (int e = threadIdx.x; e < n_rows * (HD / 8); e += blockDim.x) {
+    const int r = e / (HD / 8), c = e % (HD / 8);
+    *reinterpret_cast<uint4*>(base + (((int64_t(b) * p.l + row0 + r) * p.h + hh) * HD + c * 8) * 2) = make_uint4(0u, 0u, 0u, 0u);
+  }
+}
 
 enum Bar { kQFull = 0, kKFull = 1 /*3*/, kKEmpty = 4 /*3*/, kVFull = 7 /*3*/, kVEmpty = 10 /*3*/, kNumBars = 13 };
 
@@ -111,15 +148,22 @@ __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
 __device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
+// volatile: read where it is used, so that the value does not hold a register across the loop that uses it
+__device__ __forceinline__ int lds_s32(uint32_t addr) {
+  int v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
 
 // After the last key block, for the 64 query rows of one warpgroup (rows qrow0 + {0, 8} for this thread): the linear branch
 // adds A.KVW^T to O, then out = T( O / l + proj_b ).  kvw_smem: the KVW tile (K-major, swizzled like Q).
 // kTile (the INT8 kernels): the query rows are read from and the output rows written through the warp's RowTile, and rows
 // >= l are clipped by the tensor map; otherwise the query rows are read from and the output rows stored to global memory.
-template <typename T, int HD, bool kTile = false>
+// kVL: rows >= n (the entry's length) are stored as zeros.
+template <typename T, int HD, bool kTile = false, bool kVL = false>
 __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const float (&l_part)[2], const AttnParams& p,
                                                     uint32_t kvw_smem, int64_t qrow0, int cq, int b, int hh, int bh,
-                                                    const RowTile& tile = RowTile{}) {
+                                                    const RowTile& tile = RowTile{}, int n = 0) {
   constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
   const float l_tot[2] = {quad_sum(l_part[0]), quad_sum(l_part[1])};
   const int lane = threadIdx.x & 31;
@@ -226,8 +270,13 @@ __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const fl
 #pragma unroll
       for (int c = 0; c < HD / 8; ++c) {
         const float2 pb = __ldg(reinterpret_cast<const float2*>(p.proj_b + 8 * c + cq));
-        sts_u32(row_s + (c >> 3) * tile.chunk + (((c & 7) ^ (lane >> 2)) << 4),
-                F16Traits<T>::pack(fmaf(o[4 * c + 2 * h], inv_l, pb.x), fmaf(o[4 * c + 2 * h + 1], inv_l, pb.y)));
+        if constexpr (kVL)
+          sts_u32(row_s + (c >> 3) * tile.chunk + (((c & 7) ^ (lane >> 2)) << 4),
+                  qrow0 + 8 * h < n ? F16Traits<T>::pack(fmaf(o[4 * c + 2 * h], inv_l, pb.x), fmaf(o[4 * c + 2 * h + 1], inv_l, pb.y))
+                                    : 0u);
+        else
+          sts_u32(row_s + (c >> 3) * tile.chunk + (((c & 7) ^ (lane >> 2)) << 4),
+                  F16Traits<T>::pack(fmaf(o[4 * c + 2 * h], inv_l, pb.x), fmaf(o[4 * c + 2 * h + 1], inv_l, pb.y)));
       }
     }
     fence_proxy_async_smem();
@@ -248,8 +297,9 @@ __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const fl
 #pragma unroll
       for (int c = 0; c < HD / 8; ++c) {
         const float2 pb = __ldg(reinterpret_cast<const float2*>(p.proj_b + 8 * c + cq));
-        *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) =
-            F16Traits<T>::pack(fmaf(o[4 * c + 2 * h], inv_l, pb.x), fmaf(o[4 * c + 2 * h + 1], inv_l, pb.y));
+        uint32_t packed = F16Traits<T>::pack(fmaf(o[4 * c + 2 * h], inv_l, pb.x), fmaf(o[4 * c + 2 * h + 1], inv_l, pb.y));
+        if constexpr (kVL) packed = qr < n ? packed : 0u;
+        *reinterpret_cast<uint32_t*>(orow + 8 * c + cq) = packed;
       }
     }
   }
@@ -258,11 +308,12 @@ __device__ __forceinline__ void linear_branch_store(float (&o)[HD / 2], const fl
 // 128-row query blocks.  CTA = 2 consumer warpgroups + 1 TMA warp; warpgroup g owns query rows [64g, 64g+64) of the block.
 // kLse: the sparse branch alone for the training path (sla_attn_bwd.cu): store_o_lse instead of the KVW load and the linear branch.
 // kF8V (INT8 Q/K, HD = 128): e4m3 P.V on the [b, h, d, lk_pad] codes of tdb200_sla_quant_v_fp8 (PvOps), unscaled by v_scale.
-template <typename T, int HD, bool kQK16, bool kLse = false, bool kF8V = false>
+template <typename T, int HD, bool kQK16, bool kLse = false, bool kF8V = false, bool kVL = false>
 __global__ void __launch_bounds__(kThreads, 1)
 sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                     const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw, AttnParams p,
                     const __grid_constant__ CUtensorMap tmap_q16, const __grid_constant__ CUtensorMap tmap_out) {
+  static_assert(!(kVL && (kLse || kF8V)), "per-entry lengths serve the inference kernels with 16-bit P.V");
   using L = Lay<HD, kQK16, BLKQ, BLKK, kF8V>;
   using PV = PvOps<T, HD, BLKK, kF8V>;
   constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
@@ -275,9 +326,24 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
   const int bh = b * p.h + hh;
-  const int T_blocks = p.topk;
+  const int n = kVL ? keys_of<true>(p.seq_lens, p.l, b) : p.l;   // kVL: the entry's rows, queries and keys alike
+  if constexpr (kVL)
+    if (m_blk * BLKQ >= n) {   // the block lies wholly past the entry's rows
+      vl_store_zero_block<HD>(p, m_blk * BLKQ, BLKQ, b, hh);
+      return;
+    }
+  const int T_blocks = kVL ? vl_topk(p, b, n, BLKK) : p.topk;
+  // kVL: the consumers read the entry's length and LUT entry count from shared memory where they use them (beside the
+  // barriers, 13 of the slot's 32), so that neither holds a register across the LUT walk: at 168 registers that spills.
+  const uint32_t s_vl = smem_u32(smem + L::kOffBars + 128);
+  auto keys_n = [&]() { return kVL ? lds_s32(s_vl) : p.lk; };
+  auto n_blocks = [&]() { return kVL ? lds_s32(s_vl + 4) : p.topk; };
 
   if (threadIdx.x == 0) {
+    if constexpr (kVL) {
+      sts_u32(s_vl, uint32_t(n));
+      sts_u32(s_vl + 4, uint32_t(T_blocks));
+    }
     mbar_init(&bars[kQFull], 1);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&bars[kKFull + i], 1);
@@ -300,6 +366,66 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 
   if (warp == kConsumerWarps) {
     // =============================================================== TMA producer
+    if constexpr (kVL) {   // the loads of the code below, but the straddling V block from vl_load_v_block, by the whole warp
+      if (lane == 0) {
+        tma_prefetch_desc(&tmap_q);
+        tma_prefetch_desc(&tmap_k);
+        tma_prefetch_desc(&tmap_v);
+        tma_prefetch_desc(&tmap_kvw);
+        mbar_expect_tx(&bars[kQFull], L::kQBytes + L::kWBytes + L::kQ16Bytes);
+        if constexpr (kQK16) {
+#pragma unroll
+          for (int c = 0; c < HD / 64; ++c)
+            tma_load_4d(smem + L::kOffQ + c * (BLKQ * 128), &tmap_q, &bars[kQFull], c * 64, hh, m_blk * BLKQ, b);
+        } else {
+          tma_prefetch_desc(&tmap_q16);
+          tma_prefetch_desc(&tmap_out);
+          tma_load_4d(smem + L::kOffQ, &tmap_q, &bars[kQFull], 0, m_blk * BLKQ, bh, 0);
+#pragma unroll
+          for (int c = 0; c < HD / 64; ++c)
+            tma_load_4d(smem + L::kOffQ16 + c * (BLKQ * 128), &tmap_q16, &bars[kQFull], c * 64, hh, m_blk * BLKQ, b);
+        }
+#pragma unroll
+        for (int c = 0; c < HD / 64; ++c)
+          tma_load_4d(smem + L::kOffW + c * (HD * 128), &tmap_kvw, &bars[kQFull], c * 64, 0, bh, 0);
+      }
+      for (int j = 0; j < T_blocks; ++j) {
+        const int st = j % kStages;
+        const uint32_t ph = ((j / kStages) & 1) ^ 1;
+        const int blk = s_lut[j];
+        uint8_t* sk = smem + L::kOffK + st * L::kKBytes;
+        uint8_t* sv = smem + L::kOffV + st * L::kVBytes;
+        const int valid = n - blk * BLKK;
+        if (lane == 0) {
+          mbar_wait(&bars[kKEmpty + st], ph);
+          mbar_expect_tx(&bars[kKFull + st], L::kKBytes);
+          if constexpr (kQK16) {
+#pragma unroll
+            for (int c = 0; c < HD / 64; ++c)
+              tma_load_4d(sk + c * (BLKK * 128), &tmap_k, &bars[kKFull + st], c * 64, hh, blk * BLKK, b);
+          } else {
+            tma_load_4d(sk, &tmap_k, &bars[kKFull + st], 0, blk * BLKK, hh, b);
+          }
+          mbar_wait(&bars[kVEmpty + st], ph);
+          if (valid >= BLKK) {
+            mbar_expect_tx(&bars[kVFull + st], L::kVBytes);
+#pragma unroll
+            for (int c = 0; c < HD / 64; ++c)
+              tma_load_4d(sv + c * (BLKK * 128), &tmap_v, &bars[kVFull + st], c * 64, hh, blk * BLKK, b);
+          }
+        }
+        if (valid < BLKK) {
+          __syncwarp();   // lane 0 saw the stage empty
+          vl_load_v_block<T, HD, BLKK>(sv, p, b, hh, blk, valid, lane);
+          fence_proxy_async_smem();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&bars[kVFull + st]);
+        }
+      }
+      return;
+    }
+    // The producer of the kernels without kVL.  The kVL branch above is a copy of its load schedule (it differs only in the
+    // straddling V block): a change to one belongs in both.  The copy keeps these instantiations' code as it was.
     if (lane == 0) {
       tma_prefetch_desc(&tmap_q);
       tma_prefetch_desc(&tmap_k);
@@ -381,13 +507,13 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   if constexpr (kF8V) {
     // e4m3 P.V gives each block's P.V an accumulator of its own (PvOps), and that beside O, S_{j+1} and P_j does not fit in
     // this kernel's 168 registers: the steps of an entry run one after the other, as in the 64-row kernel.
-    for (int j = 0; j < T_blocks; ++j) {
+    for (int j = 0; j < n_blocks(); ++j) {
       const int st = j % kStages;
       mbar_wait(&bars[kKFull + st], (j / kStages) & 1);
       score_issue<kQK16, HD, BLKK, kBF16>(sacc, sq, BLKQ * 128, sbase + L::kOffK + st * L::kKBytes);
       wgmma_wait<0>();
       warp_release(&bars[kKEmpty + st], lane);
-      softmax_p_i8<BLKK>(sacc, s, qsc * s_ksc[j], m_used, l_part, rescale, alpha, p.lk - int(s_lut[j]) * BLKK, cq, j == 0);
+      softmax_p_i8<BLKK>(sacc, s, qsc * s_ksc[j], m_used, l_part, rescale, alpha, keys_n() - int(s_lut[j]) * BLKK, cq, j == 0);
       rescale_o<HD>(o, rescale, alpha);
       PV::pack(s, pa);
       mbar_wait(&bars[kVFull + st], (j / kStages) & 1);
@@ -402,14 +528,14 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     if constexpr (kQK16) {
       score_finish<kQK16, BLKK>(sacc, s, qsc * s_ksc[0]);
       warp_release(&bars[kKEmpty], lane);
-      softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, p.lk - int(s_lut[0]) * BLKK, cq, true);
+      softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, keys_n() - int(s_lut[0]) * BLKK, cq, true);
     } else {
       warp_release(&bars[kKEmpty], lane);
-      softmax_p_i8<BLKK>(sacc, s, qsc * s_ksc[0], m_used, l_part, rescale, alpha, p.lk - int(s_lut[0]) * BLKK, cq, true);
+      softmax_p_i8<BLKK>(sacc, s, qsc * s_ksc[0], m_used, l_part, rescale, alpha, keys_n() - int(s_lut[0]) * BLKK, cq, true);
     }
-    for (int j = 0; j < T_blocks; ++j) {
+    for (int j = 0; j < n_blocks(); ++j) {
       const int st = j % kStages, st1 = (j + 1) % kStages;
-      const bool next = j + 1 < T_blocks;
+      const bool next = j + 1 < n_blocks();
       if (next) {
         mbar_wait(&bars[kKFull + st1], ((j + 1) / kStages) & 1);
         score_issue<kQK16, HD, BLKK, kBF16>(sacc, sq, BLKQ * 128, sbase + L::kOffK + st1 * L::kKBytes);
@@ -423,10 +549,10 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
         if constexpr (kQK16) {
           score_finish<kQK16, BLKK>(sacc, s, qsc * s_ksc[j + 1]);
           warp_release(&bars[kKEmpty + st1], lane);
-          softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, p.lk - int(s_lut[j + 1]) * BLKK, cq, false);
+          softmax_p<BLKK>(s, m_used, l_part, rescale, alpha, keys_n() - int(s_lut[j + 1]) * BLKK, cq, false);
         } else {
           warp_release(&bars[kKEmpty + st1], lane);
-          softmax_p_i8<BLKK>(sacc, s, qsc * s_ksc[j + 1], m_used, l_part, rescale, alpha, p.lk - int(s_lut[j + 1]) * BLKK, cq,
+          softmax_p_i8<BLKK>(sacc, s, qsc * s_ksc[j + 1], m_used, l_part, rescale, alpha, keys_n() - int(s_lut[j + 1]) * BLKK, cq,
                              false);
         }
       }
@@ -439,11 +565,11 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   if constexpr (kLse) {
     store_o_lse<T, HD>(o, m_used, l_part, p, int64_t(m_blk) * BLKQ + r_lo, cq, b, hh, bh);
   } else if constexpr (kQK16) {
-    linear_branch_store<T, HD>(o, l_part, p, sbase + L::kOffW, int64_t(m_blk) * BLKQ + r_lo, cq, b, hh, bh);
+    linear_branch_store<T, HD, false, kVL>(o, l_part, p, sbase + L::kOffW, int64_t(m_blk) * BLKQ + r_lo, cq, b, hh, bh, RowTile{}, keys_n());
   } else {
     const int row16 = wg * 64 + w4 * 16;   // this warp's 16 rows of the block
     const RowTile tile{smem + L::kOffQ16 + row16 * 128, BLKQ * 128, &tmap_out, m_blk * BLKQ + row16};
-    linear_branch_store<T, HD, true>(o, l_part, p, sbase + L::kOffW, int64_t(m_blk) * BLKQ + r_lo, cq, b, hh, bh, tile);
+    linear_branch_store<T, HD, true, kVL>(o, l_part, p, sbase + L::kOffW, int64_t(m_blk) * BLKQ + r_lo, cq, b, hh, bh, tile, keys_n());
   }
 }
 
@@ -456,7 +582,7 @@ sla_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 //   of SLA/kernel.py:21-82); wgmma m64n64k16 into fp32.
 // After both loops warpgroup 1 hands its (m, l, O) to warpgroup 0, which merges the two states and then runs the linear
 // branch and the output (linear_branch_store), or with kLse stores o_s and the row lse.
-template <typename T, int HD, bool kQK16, int BK, bool kLse, bool kF8V = false>
+template <typename T, int HD, bool kQK16, int BK, bool kLse, bool kF8V = false, bool kVL = false>
 __global__ void __launch_bounds__(split::kThreads, 1)
 sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                         const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_kvw, AttnParams p,
@@ -472,11 +598,18 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kOffBars);
   uint16_t* s_lut = reinterpret_cast<uint16_t*>(smem + L::kOffLut);
   float* s_ksc = reinterpret_cast<float*>(smem + L::kOffLut + ((p.topk * 2 + 15) & ~15));  // INT8 only
+  static_assert(!(kVL && (kLse || kF8V)), "per-entry lengths serve the inference kernels with 16-bit P.V");
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
   const int bh = b * p.h + hh;
-  const int T_blocks = p.topk;
+  const int n = kVL ? keys_of<true>(p.seq_lens, p.l, b) : p.l;   // kVL: the entry's rows, queries and keys alike
+  if constexpr (kVL)
+    if (m_blk * BQ >= n) {   // the block lies wholly past the entry's rows
+      vl_store_zero_block<HD>(p, m_blk * BQ, BQ, b, hh);
+      return;
+    }
+  const int T_blocks = kVL ? vl_topk(p, b, n, BK) : p.topk;
 
   if (threadIdx.x == 0) split::init_barriers(bars);
   {
@@ -564,7 +697,7 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
     const uint32_t ph = split::full_phase(j);
     const int blk = s_lut[j];
     const float sc = kQK16 ? qsc : qsc * s_ksc[j];
-    const int valid = p.lk - blk * BK;                  // < BK only in the ragged last key block
+    const int valid = (kVL ? n : p.lk) - blk * BK;      // < BK only in the ragged last key block
 
     float s[BK / 2];
     typename PV::Frag pa;
@@ -586,6 +719,12 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
       PV::pack(s, pa);
     }
     mbar_wait(&bars[split::full(split::kVFull, j)], ph);
+    if constexpr (kVL)
+      if (valid < BK) {   // the straddling key block, this warpgroup's alone: V rows past the entry's keys are padding
+        zero_query_rows(smem + L::kOffV + st * L::kVBytes, BK, HD / 64, valid, BK, threadIdx.x & 127);
+        fence_proxy_async_smem();
+        named_bar_sync(2 + wg, 128);
+      }
     PV::step(o, pacc, pa, sbase + L::kOffV + st * L::kVBytes);
     warp_release(&bars[split::kVEmpty + st], lane);
   }
@@ -620,16 +759,19 @@ sla_attn_fwd_q64_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid
   if constexpr (kLse) {
     store_o_lse<T, HD>(o, m_used, l_part, p, qrow0, cq, b, hh, bh);
   } else if constexpr (kQK16) {
-    linear_branch_store<T, HD>(o, l_part, p, sbase + L::kOffW, qrow0, cq, b, hh, bh);
+    linear_branch_store<T, HD, false, kVL>(o, l_part, p, sbase + L::kOffW, qrow0, cq, b, hh, bh, RowTile{}, n);
   } else {
     const RowTile tile{smem + L::kOffQ16 + w4 * 16 * 128, BQ * 128, &tmap_out, m_blk * BQ + w4 * 16};
-    linear_branch_store<T, HD, true>(o, l_part, p, sbase + L::kOffW, qrow0, cq, b, hh, bh, tile);
+    linear_branch_store<T, HD, true, kVL>(o, l_part, p, sbase + L::kOffW, qrow0, cq, b, hh, bh, tile, n);
   }
 }
 
-template <typename T, int HD, bool kQK16, int kBQ, int kBK, bool kLse, bool kF8V>
+template <typename T, int HD, bool kQK16, int kBQ, int kBK, bool kLse, bool kF8V, bool kVL = false>
 constexpr auto attn_kernel() {
-  if constexpr (kF8V) {
+  if constexpr (kVL) {
+    if constexpr (kBQ == kBlkQ64) return sla_attn_fwd_q64_kernel<T, HD, kQK16, kBK, false, false, true>;
+    else return sla_attn_fwd_kernel<T, HD, kQK16, false, false, true>;
+  } else if constexpr (kF8V) {
     if constexpr (kBQ == kBlkQ64) return sla_attn_fwd_q64_kernel<T, HD, kQK16, kBK, kLse, true>;
     else return sla_attn_fwd_kernel<T, HD, kQK16, kLse, true>;
   } else {
@@ -644,11 +786,11 @@ constexpr auto attn_kernel() {
 // kLse (16-bit only): sparse branch and row log-sum-exp into `lse`; kvw, ksum and proj_b are not read.
 // kF8V (INT8 only, HD = 128): v is tdb200_sla_quant_v_fp8's e4m3 [b, h, d, lk_pad] with lk_pad = ceil(lk / kBK) * kBK, and
 // v_scale its [b, h, d] channel scales.
-template <int HD, bool kQK16, int kBQ = BLKQ, int kBK = BLKK, bool kLse = false, bool kF8V = false>
+template <int HD, bool kQK16, int kBQ = BLKQ, int kBK = BLKK, bool kLse = false, bool kF8V = false, bool kVL = false>
 int launch(const void* q_op, const float* q_scale, const void* k_op, const float* k_scale, const void* v, const void* q, int dtype,
            const int32_t* lut, int64_t topk, const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b,
            int64_t l, int64_t lk, int64_t h, float sm_scale, int feature, bool k_seq_major, void* stream, float* lse = nullptr,
-           const float* v_scale = nullptr) {
+           const float* v_scale = nullptr, const int32_t* seq_lens = nullptr, const int32_t* topks = nullptr) {
   using L = Lay<HD, kQK16, kBQ, kBK, kF8V>;
   const int64_t d = HD;
   const int64_t mblk = cdiv64(l, kBQ), nblk = cdiv64(lk, kBK);
@@ -734,12 +876,15 @@ int launch(const void* q_op, const float* q_scale, const void* k_op, const float
   p.sm_scale = sm_scale;
   p.lse = lse;
   p.v_scale = v_scale;
+  p.seq_lens = seq_lens;
+  p.topks = topks;
+  p.v = v;
   dim3 grid(static_cast<unsigned>(mblk), static_cast<unsigned>(h), static_cast<unsigned>(b));
   const int threads = kBQ == kBlkQ64 ? split::kThreads : kThreads;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define TDB_ATTN(T)                                                                                                   \
   do {                                                                                                                \
-    const auto kern = attn_kernel<T, HD, kQK16, kBQ, kBK, kLse, kF8V>();                                                        \
+    const auto kern = attn_kernel<T, HD, kQK16, kBQ, kBK, kLse, kF8V, kVL>();                                                    \
     if (int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), \
                             "cudaFuncSetAttribute(sla_attn)"))                                                        \
       return rc;                                                                                                      \
@@ -886,4 +1031,58 @@ extern "C" int tdb200_sla_attn_fwd_fp8v(const int8_t* q_i8, const float* q_scale
   return launch<128, false, kBlkQ64, kHopperBlkK, false, true>(q_i8, q_scale, k_i8, k_scale, v_fp8, q, dtype, lut, topk, kvw, ksum,
                                                                proj_b, out, b, l, lk, h, sm_scale, feature, k_seq_major != 0, stream,
                                                                nullptr, v_scale);
+}
+
+// ---- per-entry lengths: the _vl twins of tdb200_sla_attn_fwd (INT8 Q/K, K head-major) and tdb200_sla_attn16_fwd, d = 128, l = lk.
+// seq_lens [b] and topks [b] are device int32: entry b's rows below seq_lens[b] get the bits of the entry point without lengths
+// called on entry b alone, cut to those rows, with its own LUT, topk, moments and scales; its rows past the length are zero.
+// Their kernels are instantiated here, after every other kernel of this file.
+namespace {
+int check_vl(const char* what, const int32_t* seq_lens, const int32_t* topks, int64_t l, int64_t lk, int64_t d) {
+  if (!seq_lens || !topks || (reinterpret_cast<uintptr_t>(seq_lens) & 3u) || (reinterpret_cast<uintptr_t>(topks) & 3u))
+    return fail(TDB200_ERR_INVALID_ARG, "%s: seq_lens and topks must be non-null, 4-byte aligned int32 [b]", what);
+  if (l != lk) return fail(TDB200_ERR_INVALID_ARG, "%s: l = %lld and lk = %lld (one length per entry: self-attention)", what,
+                           (long long)l, (long long)lk);
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "%s: head dim %lld (per-entry lengths serve d = 128)", what, (long long)d);
+  return 0;
+}
+}  // namespace
+
+extern "C" int tdb200_sla_attn_fwd_vl(const int8_t* q_i8, const float* q_scale, const int8_t* k_i8, const float* k_scale,
+                                      const void* v, const void* q, int dtype, const int32_t* lut, int64_t topk, const void* kvw,
+                                      const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l, int64_t lk,
+                                      int64_t h, int64_t d, const int32_t* seq_lens, const int32_t* topks, float sm_scale,
+                                      int feature, int64_t blkq, int64_t blkk, void* stream) {
+  const bool hopper = blkq == kBlkQ64 && blkk == kHopperBlkK;
+  if (!hopper && !(blkq == BLKQ && blkk == BLKK))
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_attn_fwd_vl: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 128)",
+                (long long)blkq, (long long)blkk);
+  if (int rc = check_common(q_i8, k_i8, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
+  if (!q_scale || !k_scale) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd_vl: null pointer");
+  if (int rc = check_vl("sla_attn_fwd_vl", seq_lens, topks, l, lk, d)) return rc;
+  if (feature < 0 || feature > 2) return fail(TDB200_ERR_INVALID_ARG, "sla_attn_fwd_vl: feature map tag %d", feature);
+  if (!hopper)
+    return launch<128, false, BLKQ, BLKK, false, false, true>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw, ksum,
+                                                              proj_b, out, b, l, lk, h, sm_scale, feature, false, stream, nullptr,
+                                                              nullptr, seq_lens, topks);
+  return launch<128, false, kBlkQ64, kHopperBlkK, false, false, true>(q_i8, q_scale, k_i8, k_scale, v, q, dtype, lut, topk, kvw,
+                                                                      ksum, proj_b, out, b, l, lk, h, sm_scale, feature, false,
+                                                                      stream, nullptr, nullptr, seq_lens, topks);
+}
+
+extern "C" int tdb200_sla_attn16_fwd_vl(const void* q, const void* k, const void* v, int dtype, const int32_t* lut, int64_t topk,
+                                        const void* kvw, const float* ksum, const float* proj_b, void* out, int64_t b, int64_t l,
+                                        int64_t lk, int64_t h, int64_t d, const int32_t* seq_lens, const int32_t* topks,
+                                        float sm_scale, int feature, int64_t blkq, int64_t blkk, void* stream) {
+  if (int rc = check_blocks16("sla_attn16_fwd_vl", blkq, blkk)) return rc;
+  if (int rc = check_common(q, k, v, q, lut, kvw, ksum, proj_b, out, b, l, lk, h)) return rc;
+  if (int rc = check_vl("sla_attn16_fwd_vl", seq_lens, topks, l, lk, d)) return rc;
+  if (feature < 0 || feature > 2) return fail(TDB200_ERR_INVALID_ARG, "sla_attn16_fwd_vl: feature map tag %d", feature);
+  if (blkq == BLKQ)
+    return launch<128, true, BLKQ, BLKK, false, false, true>(q, nullptr, k, nullptr, v, q, dtype, lut, topk, kvw, ksum, proj_b, out,
+                                                             b, l, lk, h, sm_scale, feature, false, stream, nullptr, nullptr,
+                                                             seq_lens, topks);
+  return launch<128, true, kBlkQ64, BLKK, false, false, true>(q, nullptr, k, nullptr, v, q, dtype, lut, topk, kvw, ksum, proj_b, out,
+                                                              b, l, lk, h, sm_scale, feature, false, stream, nullptr, nullptr,
+                                                              seq_lens, topks);
 }

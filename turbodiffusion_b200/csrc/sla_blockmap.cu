@@ -24,16 +24,29 @@ __device__ __forceinline__ uint32_t order_key(float score) {
   return (u & 0x8000u) ? (~u & 0xFFFFu) : (u | 0x8000u);
 }
 
-template <typename T, int D>
+// kVL (tdb200_sla_block_map_vl): batch entry b = bh / h has seq_lens[b] rows (clamped to [0, mblk * blkq], which holds l), so mb = its query
+// blocks, nb = its key blocks and tk = topks[b] (clamped to [1, min(nb, topk)], 0 when nb = 0) blocks per row; the score, selection and
+// compaction run over those alone, as on the entry by itself.  LUT entries past tk and LUT rows past mb are -1, the map is 0
+// past nb and on rows past mb.
+template <typename T, int D, bool kVL = false>
 __global__ void __launch_bounds__(kThreads) block_map_kernel(const T* __restrict__ q_pool, const T* __restrict__ k_pool,
                                                              int mblk, int nblk, int topk,
-                                                             int8_t* __restrict__ sparse_map, int32_t* __restrict__ lut) {
+                                                             int8_t* __restrict__ sparse_map, int32_t* __restrict__ lut,
+                                                             const int32_t* seq_lens = nullptr, const int32_t* topks = nullptr,
+                                                             int h = 1, int blkq = 1, int blkk = 1) {
   extern __shared__ uint8_t smem_raw[];
   float* sq = reinterpret_cast<float*>(smem_raw);                          // [kRows][D]
   uint16_t* keys = reinterpret_cast<uint16_t*>(smem_raw + kRows * D * 4);  // [kRows][nblk]
   const int bh = blockIdx.y;
   const int m0 = blockIdx.x * kRows;
-  const int rows = min(kRows, mblk - m0);
+  int mb = mblk, nb = nblk, tk = topk;
+  if constexpr (kVL) {
+    const int len = min(max(__ldg(seq_lens + bh / h), 0), mblk * blkq);
+    mb = min(mblk, (len + blkq - 1) / blkq);
+    nb = min(nblk, (len + blkk - 1) / blkk);
+    tk = min(max(__ldg(topks + bh / h), 1), min(nb, topk));
+  }
+  const int rows = min(kRows, mb - m0);
 
   for (int i = threadIdx.x; i < kRows * D; i += kThreads) {
     const int r = i / D, c = i % D;
@@ -42,7 +55,7 @@ __global__ void __launch_bounds__(kThreads) block_map_kernel(const T* __restrict
   __syncthreads();
 
   // ---- scores: thread n handles key blocks n, n+256, ...
-  for (int n = threadIdx.x; n < nblk; n += kThreads) {
+  for (int n = threadIdx.x; n < nb; n += kThreads) {
     const T* kr = k_pool + (int64_t(bh) * nblk + n) * D;
     float acc[kRows];
 #pragma unroll
@@ -70,6 +83,12 @@ __global__ void __launch_bounds__(kThreads) block_map_kernel(const T* __restrict
 
   // ---- selection: warp w owns row w
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if constexpr (kVL)
+    if (w >= rows && w < mblk - m0) {   // a row past the entry's query blocks: an empty selection
+      for (int i = lane; i < topk; i += 32) lut[(int64_t(bh) * mblk + m0 + w) * topk + i] = -1;
+      for (int n = lane; n < nblk; n += 32) sparse_map[(int64_t(bh) * mblk + m0 + w) * nblk + n] = 0;
+      return;
+    }
   if (w >= rows) return;
   const uint16_t* kk = keys + w * nblk;
   // largest threshold t such that count(key >= t) >= topk  == the topk-th largest key
@@ -77,32 +96,36 @@ __global__ void __launch_bounds__(kThreads) block_map_kernel(const T* __restrict
   for (int bit = 15; bit >= 0; --bit) {
     const uint32_t cand = thr | (1u << bit);
     int cnt = 0;
-    for (int n = lane; n < nblk; n += 32) cnt += (kk[n] >= cand) ? 1 : 0;
+    for (int n = lane; n < nb; n += 32) cnt += (kk[n] >= cand) ? 1 : 0;
     cnt = __reduce_add_sync(0xffffffffu, cnt);
-    if (cnt >= topk) thr = cand;
+    if (cnt >= tk) thr = cand;
   }
   int cnt_gt = 0;
-  for (int n = lane; n < nblk; n += 32) cnt_gt += (kk[n] > thr) ? 1 : 0;
+  for (int n = lane; n < nb; n += 32) cnt_gt += (kk[n] > thr) ? 1 : 0;
   cnt_gt = __reduce_add_sync(0xffffffffu, cnt_gt);
-  const int need_eq = topk - cnt_gt;  // how many of the threshold-valued blocks to take, lowest index first
+  const int need_eq = tk - cnt_gt;  // how many of the threshold-valued blocks to take, lowest index first
 
   int8_t* map_row = sparse_map + (int64_t(bh) * mblk + m0 + w) * nblk;
   int32_t* lut_row = lut + (int64_t(bh) * mblk + m0 + w) * topk;
   int run_sel = 0, run_eq = 0;
   const uint32_t lt_mask = (1u << lane) - 1u;
-  for (int base = 0; base < nblk; base += 32) {
+  for (int base = 0; base < nb; base += 32) {
     const int n = base + lane;
-    const uint32_t key = (n < nblk) ? kk[n] : 0u;
-    const bool gt = (n < nblk) && key > thr;
-    const bool eq = (n < nblk) && key == thr;
+    const uint32_t key = (n < nb) ? kk[n] : 0u;
+    const bool gt = (n < nb) && key > thr;
+    const bool eq = (n < nb) && key == thr;
     const uint32_t eq_ballot = __ballot_sync(0xffffffffu, eq);
     const int eq_rank = run_eq + __popc(eq_ballot & lt_mask);
     const bool sel = gt || (eq && eq_rank < need_eq);
     const uint32_t sel_ballot = __ballot_sync(0xffffffffu, sel);
     if (sel) lut_row[run_sel + __popc(sel_ballot & lt_mask)] = n;
-    if (n < nblk) map_row[n] = sel ? 1 : 0;
+    if (n < nb) map_row[n] = sel ? 1 : 0;
     run_sel += __popc(sel_ballot);
     run_eq += __popc(eq_ballot);
+  }
+  if constexpr (kVL) {
+    for (int i = tk + lane; i < topk; i += 32) lut_row[i] = -1;
+    for (int n = nb + lane; n < nblk; n += 32) map_row[n] = 0;
   }
 }
 
@@ -143,4 +166,45 @@ extern "C" int tdb200_sla_block_map(const void* q_pool, const void* k_pool, int 
   }
 #undef TDB_BM
   return fail(TDB200_ERR_UNSUPPORTED, "sla_block_map: dtype tag %d", dtype);
+}
+
+// tdb200_sla_block_map for a padded batch: q_pool [b, h, mblk, d] and k_pool [b, h, nblk, d] of tdb200_sla_quant_qk_vl with the
+// same blkq, blkk and seq_lens [b]; topks [b] (device int32) the blocks each of entry b's rows keeps.  Entry b's rows get the
+// map and LUT tdb200_sla_block_map gives on that entry alone; the LUT keeps its row stride `topk` (the largest topks[b]).
+extern "C" int tdb200_sla_block_map_vl(const void* q_pool, const void* k_pool, int dtype, int64_t b, int64_t h, int64_t mblk,
+                                       int64_t nblk, int64_t d, int64_t topk, const int32_t* seq_lens, const int32_t* topks,
+                                       int64_t blkq, int64_t blkk, int8_t* sparse_map, int32_t* lut, void* stream) {
+  using namespace tdb;
+  if (!q_pool || !k_pool || !sparse_map || !lut) return fail(TDB200_ERR_INVALID_ARG, "sla_block_map_vl: null pointer");
+  if (!seq_lens || !topks || (reinterpret_cast<uintptr_t>(seq_lens) & 3u) || (reinterpret_cast<uintptr_t>(topks) & 3u))
+    return fail(TDB200_ERR_INVALID_ARG, "sla_block_map_vl: seq_lens and topks must be non-null, 4-byte aligned int32 [b]");
+  if (b <= 0 || h <= 0 || mblk <= 0 || nblk <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_block_map_vl: bad shape");
+  if (!((blkq == 128 && blkk == 64) || (blkq == 64 && (blkk == 64 || blkk == 128))))
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_block_map_vl: block sizes (%lld, %lld)", (long long)blkq, (long long)blkk);
+  if (topk <= 0 || topk > nblk) return fail(TDB200_ERR_INVALID_ARG, "sla_block_map_vl: topk=%lld outside [1, nblk=%lld]", (long long)topk, (long long)nblk);
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_block_map_vl: head dim %lld (per-entry lengths serve d = 128)", (long long)d);
+  if (b * h > 65535) return fail(TDB200_ERR_UNSUPPORTED, "sla_block_map_vl: b*h too large");
+  const size_t smem = size_t(kRows) * d * 4 + size_t(kRows) * nblk * 2;
+  if (smem > 200 * 1024) return fail(TDB200_ERR_UNSUPPORTED, "sla_block_map_vl: nblk=%lld too large for the on-chip score rows", (long long)nblk);
+  if (!aligned16(k_pool)) return fail(TDB200_ERR_INVALID_ARG, "sla_block_map_vl: k_pool must be 16-byte aligned");
+  if (dtype != TDB200_DTYPE_BF16 && dtype != TDB200_DTYPE_FP16) return fail(TDB200_ERR_UNSUPPORTED, "sla_block_map_vl: dtype tag %d", dtype);
+  if (int rc = require_sm90()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  dim3 grid(static_cast<unsigned>(cdiv64(mblk, kRows)), static_cast<unsigned>(b * h));
+#define TDB_BM(T)                                                                                                  \
+  do {                                                                                                             \
+    if (smem > 48 * 1024)                                                                                          \
+      if (int rc = check_cuda(cudaFuncSetAttribute(block_map_kernel<T, 128, true>,                                 \
+                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)), \
+                              "cudaFuncSetAttribute(block_map_vl)"))                                               \
+        return rc;                                                                                                 \
+    block_map_kernel<T, 128, true><<<grid, kThreads, smem, st>>>(                                                 \
+        static_cast<const T*>(q_pool), static_cast<const T*>(k_pool), static_cast<int>(mblk), static_cast<int>(nblk), \
+        static_cast<int>(topk), sparse_map, lut, seq_lens, topks, static_cast<int>(h), static_cast<int>(blkq),     \
+        static_cast<int>(blkk));                                                                                   \
+    return check_launch("block_map_kernel<vl>");                                                                   \
+  } while (0)
+  if (dtype == TDB200_DTYPE_BF16) TDB_BM(__nv_bfloat16);
+  TDB_BM(__half);
+#undef TDB_BM
 }

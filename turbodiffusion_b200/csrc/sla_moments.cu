@@ -57,9 +57,15 @@ struct MomParams {
   int l, h, tiles, splits;
   int hd;        // 128, or 64 (two heads per 128-wide row; `h` is then the number of REAL heads, grid.x = ceil(h/2) pairs)
   int feature;   // 0 softmax, 1 elu+1, 2 relu
+  const int32_t* seq_lens;   // [b] int32 (kVL only)
 };
 
-template <typename T, bool kPair>
+// kVL (tdb200_sla_linear_moments_vl): batch entry b has n = seq_lens[b] rows (clamped to [0, l]; l stays the row stride), so
+// ceil(n / 128) tiles over S_b = min(tiles, kMaxSplits) splits: the tiles, splits and summation order of a call on the entry
+// alone.  The launch's cluster is sized for l; its CTAs past S_b load nothing, and the reduction sums splits 0 .. S_b - 1 only.
+// V rows past n in the straddling tile are zeroed in shared memory before the MMAs read them (TMA loads the padding there,
+// where a call on the entry alone gets zero fill, and 0 * NaN is NaN).
+template <typename T, bool kPair, bool kVL = false>
 __global__ void __launch_bounds__(kThreads, 1)
 sla_moments_kernel(const __grid_constant__ CUtensorMap tmap_v, MomParams p) {
   constexpr int N = kPair ? 64 : 128;          // key channels of this warpgroup's accumulator
@@ -72,7 +78,11 @@ sla_moments_kernel(const __grid_constant__ CUtensorMap tmap_v, MomParams p) {
   const int head0 = kPair ? 2 * hh : hh;                           // first real head of this CTA
   const bool second_ok = !kPair || head0 + 1 < p.h;                // odd head count: the last pair has one real head
   const int64_t row_elems = int64_t(p.h) * p.hd;                   // elements per token row of k / v
-  const int my_tiles = (p.tiles - split + p.splits - 1) / p.splits;  // tiles split, split+splits, ...; >= 1 (splits <= tiles)
+  const int n = kVL ? min(max(__ldg(p.seq_lens + b), 0), p.l) : p.l;   // rows of this entry
+  const int tiles = kVL ? (n + kRowsPerTile - 1) / kRowsPerTile : p.tiles;
+  const int splits = kVL ? min(tiles, kMaxSplits) : p.splits;
+  // tiles split, split+splits, ...; >= 1 (splits <= tiles), or with kVL 0 on the CTAs past the entry's splits
+  const int my_tiles = kVL ? (split < splits ? (tiles - split + splits - 1) / splits : 0) : (p.tiles - split + p.splits - 1) / p.splits;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kVStages; ++i) mbar_init(&vfull[i], 1);
@@ -80,7 +90,7 @@ sla_moments_kernel(const __grid_constant__ CUtensorMap tmap_v, MomParams p) {
   }
   __syncthreads();
   auto load_v = [&](int i) {   // thread 0: V tile i -> stage i % kVStages
-    const int st = i % kVStages, tile = split + i * p.splits;
+    const int st = i % kVStages, tile = split + i * splits;
     uint8_t* sv = smem + kOffV + st * kOperandBytes;
     mbar_expect_tx(&vfull[st], kOperandBytes);
     // 128-wide head: columns [0,64) and [64,128) of head hh; 64-wide heads: heads 2hh and 2hh+1 (a missing second
@@ -105,8 +115,8 @@ sla_moments_kernel(const __grid_constant__ CUtensorMap tmap_v, MomParams p) {
   // flight under the exponentials), and phi needs ONE exponential per element: e_j is kept in fp32 registers until the
   // row sum is known.
   auto load_row = [&](int i, uint4 (&dst)[8]) {
-    const int64_t row = int64_t(split + i * p.splits) * kRowsPerTile + r;
-    const bool ok = i < my_tiles && row < p.l && (half == 0 || second_ok);   // missing second head: zeros
+    const int64_t row = int64_t(split + i * splits) * kRowsPerTile + r;
+    const bool ok = i < my_tiles && row < n && (half == 0 || second_ok);   // missing second head: zeros
     const uint4* src = reinterpret_cast<const uint4*>(static_cast<const T*>(p.k) + (int64_t(b) * p.l + (ok ? row : 0)) * row_elems +
                                                       int64_t(head0) * p.hd + half * 64);
 #pragma unroll
@@ -115,14 +125,14 @@ sla_moments_kernel(const __grid_constant__ CUtensorMap tmap_v, MomParams p) {
   uint4 cur[8];
   load_row(0, cur);
   for (int i = 0; i < my_tiles; ++i) {
-    const int tile = split + i * p.splits;
+    const int tile = split + i * splits;
     const int64_t row = int64_t(tile) * kRowsPerTile + r;
     uint4 nxt[8];
     load_row(i + 1, nxt);
     uint32_t w[32];
 #pragma unroll
     for (int c = 0; c < 8; ++c) { w[4 * c] = cur[c].x; w[4 * c + 1] = cur[c].y; w[4 * c + 2] = cur[c].z; w[4 * c + 3] = cur[c].w; }
-    const bool live = row < p.l && (half == 0 || second_ok);
+    const bool live = row < n && (half == 0 || second_ok);
     if (p.feature == 0) {
       // softmax over the head: my 64 channels, combined with the partner thread's for a 128-wide head
       float m = -INFINITY;
@@ -172,6 +182,17 @@ sla_moments_kernel(const __grid_constant__ CUtensorMap tmap_v, MomParams p) {
     {
       const int st = i % kVStages;
       mbar_wait(&vfull[st], (i / kVStages) & 1);
+      if constexpr (kVL)
+        if ((tile + 1) * kRowsPerTile > n) {   // whole 128-byte rows of both 64-channel blocks (the swizzle stays in a row)
+          const int valid = n - tile * kRowsPerTile, per_block = (kRowsPerTile - valid) * 8;
+          uint8_t* sv = smem + kOffV + st * kOperandBytes;
+          for (int e = threadIdx.x; e < 2 * per_block; e += kThreads) {
+            const int c = e / per_block, u = e - c * per_block;
+            *reinterpret_cast<uint4*>(sv + c * kBlockBytes + valid * 128 + u * 16) = make_uint4(0u, 0u, 0u, 0u);
+          }
+          fence_proxy_async_smem();
+          __syncthreads();
+        }
       // A = V^T (dv rows of block wg), B = phi (key channels; a pair's warpgroup takes its own 64-channel block): both MN-major,
       // K = 16 key rows per MMA: +2048 B in both operands
       const uint64_t adesc = make_desc_mnmajor_sw128(sbase + kOffV + st * kOperandBytes + wg * kBlockBytes, kBlockBytes);
@@ -223,36 +244,37 @@ sla_moments_kernel(const __grid_constant__ CUtensorMap tmap_v, MomParams p) {
   // ---- reduce: CTA `rank` owns every S-th run of kThreads float4 chunks; each element is summed over splits 0..S-1
   {
     const uint32_t rank = cluster_ctarank(), S = p.splits;
+    const uint32_t SS = kVL ? uint32_t(splits) : S;   // the splits summed (kVL: the entry's; 0 for an entry with no rows)
     const uint32_t spart = smem_u32(part);
     const int64_t bh0 = int64_t(b) * p.h + head0;
     constexpr int kChunks = (kPair ? 2 * 64 * 64 : D * D) / 4;
     const int live_chunks = second_ok ? kChunks : kChunks / 2;   // odd head count: the last pair's second head is absent
     float4* const dst = reinterpret_cast<float4*>(p.kv + bh0 * (kPair ? 64 * 64 : D * D));
     // all S loads of an element are issued before the first add, so the remote reads overlap
-    for (int c = int(rank) * kThreads + threadIdx.x; c < live_chunks; c += S * kThreads) {
+    for (int c = int(rank) * kThreads + threadIdx.x; (!kVL || SS > 0) && c < live_chunks; c += S * kThreads) {
       float4 g = dst[c];
       float4 u[kMaxSplits];
 #pragma unroll
       for (uint32_t s = 0; s < kMaxSplits; ++s)
-        if (s < S) u[s] = ld_dsmem_v4(spart + c * 16, s);
+        if (s < SS) u[s] = ld_dsmem_v4(spart + c * 16, s);
       float4 t = u[0];
 #pragma unroll
       for (uint32_t s = 1; s < kMaxSplits; ++s)
-        if (s < S) { t.x += u[s].x; t.y += u[s].y; t.z += u[s].z; t.w += u[s].w; }
+        if (s < SS) { t.x += u[s].x; t.y += u[s].y; t.z += u[s].z; t.w += u[s].w; }
       g.x += t.x; g.y += t.y; g.z += t.z; g.w += t.w;
       dst[c] = g;
     }
     const int live_cols = second_ok ? 128 : 64;
-    for (int c = int(rank) * kThreads + threadIdx.x; c < live_cols; c += S * kThreads) {
+    for (int c = int(rank) * kThreads + threadIdx.x; (!kVL || SS > 0) && c < live_cols; c += S * kThreads) {
       const uint32_t a = spart + kOffPartKsum + c * 4;
       float u[kMaxSplits][2];
 #pragma unroll
       for (uint32_t s = 0; s < kMaxSplits; ++s)
-        if (s < S) { u[s][0] = ld_dsmem_f32(a, s); u[s][1] = ld_dsmem_f32(a + 128 * 4, s); }
+        if (s < SS) { u[s][0] = ld_dsmem_f32(a, s); u[s][1] = ld_dsmem_f32(a + 128 * 4, s); }
       float t = u[0][0] + u[0][1];
 #pragma unroll
       for (uint32_t s = 1; s < kMaxSplits; ++s)
-        if (s < S) t += u[s][0] + u[s][1];
+        if (s < SS) t += u[s][0] + u[s][1];
       p.ksum[bh0 * p.hd + c] += t;   // a pair's channels 64.. are head0+1's, which follow head0's 64 in ksum
     }
   }
@@ -288,6 +310,7 @@ extern "C" int tdb200_sla_linear_moments(const void* k, const void* v, int dtype
   p.h = int(h);
   p.hd = int(d);
   p.feature = feature;
+  p.seq_lens = nullptr;
   p.tiles = int(cdiv64(l, kRowsPerTile));
   p.splits = p.tiles < kMaxSplits ? p.tiles : kMaxSplits;   // the tile count alone decides the summation order
   cudaLaunchConfig_t cfg = {};
@@ -366,4 +389,64 @@ extern "C" int tdb200_sla_project_moments(const float* proj_w, const float* kv, 
   }
 #undef TDB_PM
   return fail(TDB200_ERR_UNSUPPORTED, "sla_project_moments: dtype tag %d", dtype);
+}
+
+// tdb200_sla_linear_moments for a padded batch: k and v [b, l, h, 128], seq_lens [b] (device int32, clamped to [0, l]).  Entry b's
+// kv and ksum get the bits tdb200_sla_linear_moments gives on that entry alone cut to its first seq_lens[b] rows; what the rows
+// past it hold, inf and NaN included, does not reach them.  Accumulated like tdb200_sla_linear_moments (the caller zeroes).
+extern "C" int tdb200_sla_linear_moments_vl(const void* k, const void* v, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
+                                            const int32_t* seq_lens, int feature, float* kv, float* ksum, void* stream) {
+  using namespace tdb;
+  if (!k || !v || !kv || !ksum) return fail(TDB200_ERR_INVALID_ARG, "sla_linear_moments_vl: null pointer");
+  if (!seq_lens || (reinterpret_cast<uintptr_t>(seq_lens) & 3u))
+    return fail(TDB200_ERR_INVALID_ARG, "sla_linear_moments_vl: seq_lens must be a non-null, 4-byte aligned int32 [b]");
+  if (b <= 0 || l <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_linear_moments_vl: bad shape");
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_linear_moments_vl: head dim %lld (per-entry lengths serve d = 128)", (long long)d);
+  if (feature < 0 || feature > 2) return fail(TDB200_ERR_INVALID_ARG, "sla_linear_moments_vl: feature map tag %d", feature);
+  if (h > 65535 || b > 65535 || l > 0x7FFFFFFF) return fail(TDB200_ERR_UNSUPPORTED, "sla_linear_moments_vl: dimension too large");
+  if (!aligned16(k) || !aligned16(kv)) return fail(TDB200_ERR_INVALID_ARG, "sla_linear_moments_vl: buffers must be 16-byte aligned");
+  if (dtype != TDB200_DTYPE_BF16 && dtype != TDB200_DTYPE_FP16) return fail(TDB200_ERR_UNSUPPORTED, "sla_linear_moments_vl: dtype tag %d", dtype);
+  if (int rc = require_sm90()) return rc;
+  const CUtensorMapDataType t16 = dtype == TDB200_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUtensorMap tv;
+  {
+    const uint64_t dims[4] = {uint64_t(d), uint64_t(h), uint64_t(l), uint64_t(b)};
+    const uint64_t str[3] = {uint64_t(d * 2), uint64_t(h * d * 2), uint64_t(l * h * d * 2)};
+    const uint32_t box[4] = {64, 1, kRowsPerTile, 1};
+    if (int rc = make_tmap_4d(&tv, v, t16, 2, dims, str, box)) return rc;
+  }
+  MomParams p;
+  p.k = k;
+  p.kv = kv;
+  p.ksum = ksum;
+  p.l = int(l);
+  p.h = int(h);
+  p.hd = int(d);
+  p.feature = feature;
+  p.seq_lens = seq_lens;
+  p.tiles = int(cdiv64(l, kRowsPerTile));
+  p.splits = p.tiles < kMaxSplits ? p.tiles : kMaxSplits;   // the cluster size; each entry sums its own splits
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(static_cast<unsigned>(h), static_cast<unsigned>(p.splits), static_cast<unsigned>(b));
+  cfg.blockDim = dim3(kThreads);
+  cfg.dynamicSmemBytes = kSmemBytes;
+  cfg.stream = static_cast<cudaStream_t>(stream);
+  cudaLaunchAttribute cluster;
+  cluster.id = cudaLaunchAttributeClusterDimension;
+  cluster.val.clusterDim.x = 1;
+  cluster.val.clusterDim.y = static_cast<unsigned>(p.splits);
+  cluster.val.clusterDim.z = 1;
+  cfg.attrs = &cluster;
+  cfg.numAttrs = 1;
+#define TDB_MOM(T)                                                                                                  \
+  do {                                                                                                              \
+    static bool attr_done[64] = {false};                                                                            \
+    if (int rc = set_max_dynamic_smem_once(reinterpret_cast<const void*>(sla_moments_kernel<T, false, true>), kSmemBytes, \
+                                           attr_done, "cudaFuncSetAttribute(sla_moments_vl)"))                      \
+      return rc;                                                                                                    \
+    return check_cuda(cudaLaunchKernelEx(&cfg, sla_moments_kernel<T, false, true>, tv, p), "sla_moments_kernel<vl>"); \
+  } while (0)
+  if (dtype == TDB200_DTYPE_BF16) TDB_MOM(__nv_bfloat16);
+  TDB_MOM(__half);
+#undef TDB_MOM
 }

@@ -19,10 +19,18 @@ using namespace tdb;
 constexpr int kMeanRows = 128;  // rows per partial in the key-mean pass (= the sequence-parallel shard alignment, so a rank's
                                 // partials are exactly the single-GPU partials of its rows)
 
+// kVL (tdb200_sla_quant_qk_vl): batch entry b owns its first seq_lens[b] rows, clamped to [0, l] on the device; l stays the row
+// stride of the padded buffers.  Every row test below then masks at that length, as a call on the entry alone masks at its l.
+template <bool kVL>
+__device__ __forceinline__ int64_t rows_of(const int32_t* seq_lens, int64_t l, int b) {
+  if constexpr (kVL) return min(max(int64_t(__ldg(seq_lens + b)), int64_t(0)), l);
+  return l;
+}
+
 // ---- stage 1 of the key mean: partial column sums over kMeanRows rows ---------------------------------------
-template <typename T, int D>
+template <typename T, int D, bool kVL = false>
 __global__ void __launch_bounds__(256) kmean_partial_kernel(const T* __restrict__ k, float* __restrict__ partial,
-                                                            int64_t l, int h, int chunks) {
+                                                            int64_t l, int h, int chunks, const int32_t* seq_lens = nullptr) {
   constexpr int CPR = D / 8;          // 16-byte chunks per row
   constexpr int RPP = 256 / CPR;      // rows per pass
   __shared__ float red[RPP][D];
@@ -30,10 +38,11 @@ __global__ void __launch_bounds__(256) kmean_partial_kernel(const T* __restrict_
   const int c = threadIdx.x % CPR, r = threadIdx.x / CPR;
   float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   const int64_t row_begin = int64_t(chunk) * kMeanRows;
+  const int64_t n = rows_of<kVL>(seq_lens, l, b);
 #pragma unroll 4
   for (int p = 0; p < kMeanRows / RPP; ++p) {
     const int64_t row = row_begin + p * RPP + r;
-    if (row < l) {
+    if (row < n) {
       const uint4 raw = ldg_nc_v4(k + ((int64_t(b) * l + row) * h + hh) * D + c * 8);
       const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
 #pragma unroll
@@ -57,31 +66,37 @@ __global__ void __launch_bounds__(256) kmean_partial_kernel(const T* __restrict_
 // ---- stage 2: fixed-order reduction of the partials -> kmean [b,h,d] fp32 -------------------------------------
 // 1024 threads per (b,h): thread = (group g, column); group g adds chunks g, g+G, g+2G, ... in order, the G group sums are
 // combined in index order through shared memory (deterministic).  One CTA per head used to walk all chunks serially: 14 us of
-// pure load latency per call.
+// pure load latency per call.  kVL: entry b reduces its own ceil(n / 128) chunks (the partials a call on the entry alone forms,
+// in the same order) and divides by its n; an entry with no rows gets a zero mean.
+template <bool kVL = false>
 __global__ void __launch_bounds__(1024) kmean_final_kernel(const float* __restrict__ partial, float* __restrict__ kmean, int64_t l,
-                                                           int chunks, int d) {
+                                                           int chunks, int d, const int32_t* seq_lens = nullptr, int h = 1) {
   __shared__ float red[1024];
   const int bh = blockIdx.x;
   const int groups = 1024 / d;                 // 8 for d = 128, 16 for d = 64
   const int col = threadIdx.x % d, g = threadIdx.x / d;
+  const int64_t n = rows_of<kVL>(seq_lens, l, kVL ? bh / h : 0);
+  const int my_chunks = kVL ? static_cast<int>(cdiv64(n, kMeanRows)) : chunks;
   float s = 0.f;
-  for (int ch = g; ch < chunks; ch += groups) s += partial[(int64_t(bh) * chunks + ch) * d + col];
+  for (int ch = g; ch < my_chunks; ch += groups) s += partial[(int64_t(bh) * chunks + ch) * d + col];
   red[threadIdx.x] = s;
   __syncthreads();
   if (threadIdx.x < d) {
     float t = 0.f;
     for (int gg = 0; gg < groups; ++gg) t += red[gg * d + threadIdx.x];
-    kmean[int64_t(bh) * d + threadIdx.x] = t / static_cast<float>(l);
+    kmean[int64_t(bh) * d + threadIdx.x] = (kVL && n == 0) ? 0.f : t / static_cast<float>(n);
   }
 }
 
 // ---- block pass: pooled mean + Sage int8 quant of one ROWS x D tile ---------------------------------------------
-template <typename T, int D, int ROWS, bool kSubMean>
+// kVL: rows past the entry's length are masked as rows past l are; a block wholly past it pools to zero.
+template <typename T, int D, int ROWS, bool kSubMean, bool kVL = false>
 __global__ void __launch_bounds__(ROWS* D / 64) pool_quant_kernel(const T* __restrict__ x,
                                                                    const float* __restrict__ kmean,
                                                                    int8_t* __restrict__ x_i8, float* __restrict__ scale,
                                                                    T* __restrict__ pool, int64_t l, int h, int nblk,
-                                                                   int64_t out_row_stride, int64_t out_head_stride) {
+                                                                   int64_t out_row_stride, int64_t out_head_stride,
+                                                                   const int32_t* seq_lens = nullptr) {
   constexpr int THREADS = ROWS * D / 64;
   constexpr int CPR = D / 8;
   constexpr int RPP = THREADS / CPR;
@@ -91,6 +106,7 @@ __global__ void __launch_bounds__(ROWS* D / 64) pool_quant_kernel(const T* __res
   const int hh = blockIdx.x, blk = blockIdx.y, b = blockIdx.z;  // heads fastest: concurrent CTAs read whole [row, H*D] lines
   const int c = threadIdx.x % CPR, r = threadIdx.x / CPR;
   const int64_t bh = int64_t(b) * h + hh;
+  const int64_t n = rows_of<kVL>(seq_lens, l, b);
 
   float km[8];
 #pragma unroll
@@ -101,7 +117,7 @@ __global__ void __launch_bounds__(ROWS* D / 64) pool_quant_kernel(const T* __res
   for (int p = 0; p < 8; ++p) {
     const int64_t row = int64_t(blk) * ROWS + p * RPP + r;
     raw[p] = make_uint4(0u, 0u, 0u, 0u);
-    if (row < l) raw[p] = ldg_nc_v4(x + ((int64_t(b) * l + row) * h + hh) * D + c * 8);
+    if (row < n) raw[p] = ldg_nc_v4(x + ((int64_t(b) * l + row) * h + hh) * D + c * 8);
   }
   float v[8][8];
   float colsum[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -109,7 +125,7 @@ __global__ void __launch_bounds__(ROWS* D / 64) pool_quant_kernel(const T* __res
 #pragma unroll
   for (int p = 0; p < 8; ++p) {
     const int64_t row = int64_t(blk) * ROWS + p * RPP + r;
-    const bool ok = row < l;
+    const bool ok = row < n;
     const uint32_t w[4] = {raw[p].x, raw[p].y, raw[p].z, raw[p].w};
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -131,9 +147,9 @@ __global__ void __launch_bounds__(ROWS* D / 64) pool_quant_kernel(const T* __res
     float s = 0.f;
 #pragma unroll 4
     for (int rr = 0; rr < RPP; ++rr) s += red[rr][threadIdx.x];
-    const int64_t rem = l - int64_t(blk) * ROWS;
+    const int64_t rem = n - int64_t(blk) * ROWS;
     const float cnt = static_cast<float>(rem < ROWS ? rem : ROWS);
-    pool[(bh * nblk + blk) * D + threadIdx.x] = static_cast<T>(s / cnt);
+    pool[(bh * nblk + blk) * D + threadIdx.x] = (kVL && rem <= 0) ? static_cast<T>(0.f) : static_cast<T>(s / cnt);
   }
 #pragma unroll
   for (int w = 0; w < THREADS / 32; ++w) amax = fmaxf(amax, warp_amax[w]);
@@ -159,7 +175,7 @@ __global__ void __launch_bounds__(ROWS* D / 64) pool_quant_kernel(const T* __res
       else
         hi |= (static_cast<uint32_t>(qi) & 0xFFu) << (8 * (j - 4));
     }
-    if (row < l)
+    if (row < n)
       *reinterpret_cast<uint2*>(x_i8 + int64_t(b) * h * l * D + hh * out_head_stride + row * out_row_stride + c * 8) = make_uint2(lo, hi);
   }
 }
@@ -202,7 +218,7 @@ int run_k(const void* k, int64_t b, int64_t l, int64_t h, float* kmean, int8_t* 
   // per head) whenever 4*chunks <= l, i.e. l >= 4; a single chunk (l <= 128) reduces in place in the kmean output itself.
   float* partial = chunks == 1 ? kmean : reinterpret_cast<float*>(k_i8);
   if (int rc = run_kmean_partial<T, D>(k, b, l, h, partial, st)) return rc;
-  kmean_final_kernel<<<static_cast<unsigned>(b * h), 1024, 0, st>>>(partial, kmean, l, chunks, D);
+  kmean_final_kernel<><<<static_cast<unsigned>(b * h), 1024, 0, st>>>(partial, kmean, l, chunks, D);
   if (int rc = check_launch("kmean_final_kernel")) return rc;
   return run_k_quant<T, D, BK>(k, b, l, h, kmean, k_i8, k_scale, k_pool, false, st);
 }
@@ -277,7 +293,7 @@ extern "C" int tdb200_sla_kmean_final(const float* partial, int64_t b, int64_t h
   if (b <= 0 || h <= 0 || chunks <= 0 || l_total <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_kmean_final: bad shape");
   if (d != 64 && d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_kmean_final: head dim %lld (64 or 128)", (long long)d);
   if (int rc = require_sm90()) return rc;
-  kmean_final_kernel<<<static_cast<unsigned>(b * h), 1024, 0, static_cast<cudaStream_t>(stream)>>>(partial, kmean, l_total,
+  kmean_final_kernel<><<<static_cast<unsigned>(b * h), 1024, 0, static_cast<cudaStream_t>(stream)>>>(partial, kmean, l_total,
                                                                                                   static_cast<int>(chunks), static_cast<int>(d));
   return check_launch("kmean_final_kernel");
 }
@@ -422,4 +438,65 @@ extern "C" int tdb200_sla_quant_v_fp8(const void* v, int dtype, int64_t b, int64
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (dtype == TDB200_DTYPE_BF16) return run_quant_v_fp8<__nv_bfloat16>(v, b, l, h, blkk, v_fp8, v_scale, st);
   return run_quant_v_fp8<__half>(v, b, l, h, blkk, v_fp8, v_scale, st);
+}
+
+// ---- per-entry lengths (tdb200_sla_quant_qk_vl): the kVL instantiations, after every existing one -------------------------
+namespace {
+template <typename T, int BQ, int BK>
+int run_vl(const void* q, const void* k, int64_t b, int64_t l, int64_t h, const int32_t* seq_lens, float* kmean, int8_t* q_i8,
+           float* q_scale, int8_t* k_i8, float* k_scale, void* q_pool, void* k_pool, cudaStream_t st) {
+  constexpr int D = 128;
+  if (q != nullptr) {
+    const int mblk = static_cast<int>(cdiv64(l, BQ));
+    pool_quant_kernel<T, D, BQ, false, true><<<dim3(static_cast<unsigned>(h), mblk, static_cast<unsigned>(b)), BQ * D / 64, 0, st>>>(
+        static_cast<const T*>(q), nullptr, q_i8, q_scale, static_cast<T*>(q_pool), l, static_cast<int>(h), mblk, D, l * D, seq_lens);
+    if (int rc = check_launch("pool_quant_kernel<q, vl>")) return rc;
+  }
+  if (k != nullptr) {
+    const int chunks = static_cast<int>(cdiv64(l, kMeanRows));
+    float* partial = chunks == 1 ? kmean : reinterpret_cast<float*>(k_i8);   // as run_k
+    kmean_partial_kernel<T, D, true><<<dim3(static_cast<unsigned>(h), chunks, static_cast<unsigned>(b)), 256, 0, st>>>(
+        static_cast<const T*>(k), partial, l, static_cast<int>(h), chunks, seq_lens);
+    if (int rc = check_launch("kmean_partial_kernel<vl>")) return rc;
+    kmean_final_kernel<true><<<static_cast<unsigned>(b * h), 1024, 0, st>>>(partial, kmean, l, chunks, D, seq_lens,
+                                                                             static_cast<int>(h));
+    if (int rc = check_launch("kmean_final_kernel<vl>")) return rc;
+    const int nblk = static_cast<int>(cdiv64(l, BK));
+    pool_quant_kernel<T, D, BK, true, true><<<dim3(static_cast<unsigned>(h), nblk, static_cast<unsigned>(b)), BK * D / 64, 0, st>>>(
+        static_cast<const T*>(k), kmean, k_i8, k_scale, static_cast<T*>(k_pool), l, static_cast<int>(h), nblk, D, l * D, seq_lens);
+    if (int rc = check_launch("pool_quant_kernel<k, vl>")) return rc;
+  }
+  return TDB200_OK;
+}
+}  // namespace
+
+// tdb200_sla_quant_qk for a padded batch: q and k [b, l, h, 128] share one length per entry, seq_lens [b] (device int32, clamped
+// to [0, l]).  Entry b's rows below its length get the bits tdb200_sla_quant_qk gives on that entry alone cut to those rows: its
+// own key mean, pooled means and scales.  Rows past it are not written; blocks wholly past it pool to zero.  Either half may be
+// NULL, as for tdb200_sla_quant_qk.
+extern "C" int tdb200_sla_quant_qk_vl(const void* q, const void* k, int dtype, int64_t b, int64_t l, int64_t h, int64_t d,
+                                      const int32_t* seq_lens, float* kmean, int8_t* q_i8, float* q_scale, int8_t* k_i8,
+                                      float* k_scale, void* q_pool, void* k_pool, int64_t blkq, int64_t blkk, void* stream) {
+  using namespace tdb;
+  if (!((blkq == 128 && blkk == 64) || (blkq == 64 && blkk == 128)))
+    return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_qk_vl: block sizes (%lld, %lld) (BLKQ x BLKK = 128 x 64 or 64 x 128)",
+                (long long)blkq, (long long)blkk);
+  if ((!q && !k) || (q && (!q_i8 || !q_scale || !q_pool)) || (k && (!kmean || !k_i8 || !k_scale || !k_pool)))
+    return fail(TDB200_ERR_INVALID_ARG, "sla_quant_qk_vl: null pointer");
+  if (!seq_lens || (reinterpret_cast<uintptr_t>(seq_lens) & 3u))
+    return fail(TDB200_ERR_INVALID_ARG, "sla_quant_qk_vl: seq_lens must be a non-null, 4-byte aligned int32 [b]");
+  if (b <= 0 || l <= 0 || h <= 0) return fail(TDB200_ERR_INVALID_ARG, "sla_quant_qk_vl: bad shape");
+  if (d != 128) return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_qk_vl: head dim %lld (per-entry lengths serve d = 128)", (long long)d);
+  if (h > 65535 || b > 65535 || cdiv64(l, 64) > 65535) return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_qk_vl: h, b or sequence length too large");
+  if ((q && (!aligned16(q) || !aligned16(q_i8))) || (k && (!aligned16(k) || !aligned16(k_i8))))
+    return fail(TDB200_ERR_INVALID_ARG, "sla_quant_qk_vl: buffers must be 16-byte aligned");
+  if (dtype != TDB200_DTYPE_BF16 && dtype != TDB200_DTYPE_FP16) return fail(TDB200_ERR_UNSUPPORTED, "sla_quant_qk_vl: dtype tag %d", dtype);
+  if (int rc = require_sm90()) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+#define TDB_RUN(T)                                                                                                         \
+  return blkq == 128 ? run_vl<T, 128, 64>(q, k, b, l, h, seq_lens, kmean, q_i8, q_scale, k_i8, k_scale, q_pool, k_pool, st) \
+                     : run_vl<T, 64, 128>(q, k, b, l, h, seq_lens, kmean, q_i8, q_scale, k_i8, k_scale, q_pool, k_pool, st)
+  if (dtype == TDB200_DTYPE_BF16) TDB_RUN(__nv_bfloat16);
+  TDB_RUN(__half);
+#undef TDB_RUN
 }
